@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — requests/s of the GoFr request hot path on B200 (BASELINE.json metric).
+"""bench.py — requests/s of the GoFr request hot path on H100 (BASELINE.json metric).
 
   python bench.py --gpus N --steps K --warmup W            # this repo's CUDA path
   python bench.py --impl reference --gpus N --steps K ...  # the CPU restatement of the reference path, host cores
@@ -10,7 +10,10 @@ contiguous shard of the request stream; no data-path collective, the sealed rout
   value  : whole-job requests/s with the batch already resident in HBM (CUDA events, max over ranks)
   e2e    : the same through the host-buffer call a user makes (gofr_batch_submit/_wait): pinned host buffers,
            H2D and D2H inside the timed region
-  roofline: algorithmic bytes of one launch / its mean CUDA-event duration, against the measured HBM copy peak
+  roofline: algorithmic bytes of one launch / its mean CUDA-event duration, against the H100 SXM data-sheet HBM3 bandwidth
+
+  --dump-outputs DIR writes what the last timed step computed (response lengths and statuses of every request, the bytes of a
+  fixed, seeded sample of responses) as .npy files, so that two builds can be compared output for output.
 """
 from __future__ import annotations
 
@@ -34,50 +37,24 @@ from gofr_b200 import synth  # noqa: E402
 METRIC = "requests_per_sec_256B_json_body"
 UNIT = "req/s"
 DATE_UNIX = 1789974595
-HBM_FALLBACK_GBS = 6650.0  # /opt/skills/guides/B200_PROFILING.md fallback
+HBM_PEAK_GBS = 3350.0  # H100 SXM data sheet: 3.35 TB/s of HBM3 (a bound, not a measured rate)
+DUMP_SAMPLE = 16384   # responses whose bytes --dump-outputs writes: 16384 x 528 bytes as float32 = 34.6 MB
 
 
 def hbm_peak():
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    try:
-        with open(p) as f:
-            return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    except Exception:
-        return HBM_FALLBACK_GBS, "fallback (B200_PROFILING.md)"
+    return HBM_PEAK_GBS, "H100 SXM data sheet (3.35 TB/s HBM3)"
 
 
-KERNEL_SOURCES = ["gofr_b200/csrc/serve_body.cuh", "gofr_b200/csrc/serve_device.cuh", "gofr_b200/csrc/bind_device.cuh",
-                  "gofr_b200/csrc/serve_slots_kernel.cu", "gofr_b200/csrc/serve_slots_wide_kernel.cu", "gofr_b200/csrc/serve_values_kernel.cu", "gofr_b200/csrc/serve_slots_values_kernel.cu", "gofr_b200/csrc/value_device.cuh", "gofr_b200/csrc/float_device.cuh", "gofr_b200/csrc/serve_kernel.cu", "gofr_b200/csrc/tile_common.cuh",
-                  "gofr_b200/csrc/table_format.h"]
-
-
-def kernel_source_hash():
-    """SHA-256 over what decides the serve kernels' binaries: their sources and headers, the compiler flags and the list of
-    translation units built with the 256-bit sector store (not the whole build script: adding an unrelated kernel to the
-    build must not invalidate a capture of this one)."""
-    import hashlib
-    from gofr_b200 import _build
-    h = hashlib.sha256()
-    for f in KERNEL_SOURCES:
-        with open(os.path.join(ROOT, f), "rb") as fh:
-            h.update(fh.read())
-    h.update(repr((_build.NVCC_FLAGS, sorted(x for x in _build.SECTOR256 if x.startswith("serve")))).encode())
-    return h.hexdigest()
-
-
-def profiled_traffic(layout="slots"):
-    """dram__bytes_read.sum + dram__bytes_write.sum of ONE launch of the headline kernel on this exact workload, from an
-    `ncu --set full` capture — reported only when the capture was taken from the kernel sources that are being run now
-    (profiles/r02/traffic.json records their SHA-256; a stale capture yields null, never an old number)."""
-    try:
-        with open(os.path.join(ROOT, "profiles", "r02", "traffic.json")) as f:
-            t = json.load(f)
-        ent = t.get(layout)
-        if not ent or ent.get("source_sha256") != kernel_source_hash():
-            return None
-        return float(ent["dram_bytes_read"]) + float(ent["dram_bytes_write"])
-    except Exception:
-        return None
+def dump_outputs(dirname, n, slot, rows, lengths, meta):
+    """The caller-visible results of the last timed step as float32 / float64 .npy files (64 MB at most): every request's
+    response length and meta word, and the bytes of DUMP_SAMPLE responses picked by a fixed seed, each in a row of `slot`
+    bytes (zero past its length).  rows(idx) returns those responses as a uint8 array [len(idx), slot]."""
+    os.makedirs(dirname, exist_ok=True)
+    idx = np.sort(np.random.default_rng(0).choice(n, size=min(n, DUMP_SAMPLE), replace=False))
+    np.save(os.path.join(dirname, "response_len.npy"), lengths.astype(np.float64))
+    np.save(os.path.join(dirname, "response_meta.npy"), meta.astype(np.float64))
+    np.save(os.path.join(dirname, "sample_index.npy"), idx.astype(np.float64))
+    np.save(os.path.join(dirname, "sample_responses.npy"), rows(idx).astype(np.float32))
 
 
 class ClockSampler:
@@ -315,7 +292,7 @@ def workload_config(n, gpus, args):
                         "framing), %d requests per step per worker (GPU rank / CPU arm)" % n,
             "requests_per_step_per_worker": n, "frame_mode": "wire", "routes": 16,
             "parallelism": f"dp{gpus} (requests sharded, no data-path collective)",
-            "l2": "inputs+outputs per step (~%.2f GB) %s the 126 MB L2" % (n * 793 / 1e9, "exceed" if n * 793 > 126e6 else "DO NOT exceed"),
+            "l2": "inputs+outputs per step (~%.2f GB) %s the 50 MB L2" % (n * 793 / 1e9, "exceed" if n * 793 > 50e6 else "DO NOT exceed"),
             "resident_layout": ("slots: response i in its own 528-byte slot (gofr_serve_device_slots)" if args.layout == "slots" else "packed offsets (gofr_serve_device)"),
             "e2e_layout": ("slots (gofr_batch_submit_slots)" if args.e2e_layout == "slots" else "packed offsets (gofr_batch_submit)")}
 
@@ -536,7 +513,7 @@ def run_secondary(args):
 
 
 def sharded_config4(eng_factory, rank, world, dev, barrier, reduce_max, steps, per_gpu=1 << 18):
-    """BASELINE config 4 ("mixed 64-route GET/POST with the 3-deep middleware chain, 4xB200 shard"): the 64-route table is
+    """BASELINE config 4 ("mixed 64-route GET/POST with the 3-deep middleware chain, 4-GPU shard"): the 64-route table is
     sealed on rank 0 and broadcast (NCCL), every rank serves its contiguous shard of ONE request stream, resident and
     through host buffers; parity of a sample of the rank's shard against the oracle run on exactly those requests."""
     import torch
@@ -607,7 +584,7 @@ def sharded_config4(eng_factory, rank, world, dev, barrier, reduce_max, steps, p
 
 
 def sharded_config5(eng, rank, world, dev, barrier, reduce_max, steps, per_gpu=1 << 20):
-    """BASELINE config 5 ("gRPC unary protobuf encode path, 1M req, 8xB200 with NCCL route-table broadcast"): every rank
+    """BASELINE config 5 ("gRPC unary protobuf encode path, 1M req, 8 GPUs with NCCL route-table broadcast"): every rank
     decodes / answers / encodes its contiguous shard of one HelloRequest frame stream (the engine's table came from the
     NCCL broadcast at start-up); parity of a sample against the oracle."""
     import torch
@@ -672,6 +649,7 @@ def main():
     ap.add_argument("--layout", default="slots", choices=["packed", "slots"],
                     help="resident measurement: packed offsets (gofr_serve_device) or one 528-byte slot per response "
                          "(gofr_serve_device_slots)")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write what the last timed step computed to DIR/<name>.npy (config2)")
     ap.add_argument("--workload", default="config2", choices=["config2", "config3", "config4", "config5", "proto", "reqlog", "http"],
                     help="config2 is the BASELINE metric line; the others are secondary measurements (resident only)")
     args = ap.parse_args()
@@ -760,6 +738,21 @@ def main():
     barrier()
     ms = reduce_max(ev0.elapsed_time(ev1))
     clocks = sampler.stop()
+    if args.dump_outputs and rank == 0:
+        if args.layout == "slots":
+            dump_outputs(args.dump_outputs, n, slot, lambda idx: s_out.view(n, slot)[torch.from_numpy(idx).to(dev)].cpu().numpy(),
+                         s_len.cpu().numpy().view(np.uint32), s_meta.cpu().numpy().view(np.uint32))
+        else:
+            p_off = resp.out_off.cpu().numpy().view(np.uint32).astype(np.int64)
+            p_out = resp.out.cpu().numpy()
+
+            def packed_rows(idx):
+                r = np.zeros((len(idx), slot), dtype=np.uint8)
+                for k, i in enumerate(idx):
+                    b = p_out[p_off[i]:p_off[i] + min(p_off[i + 1] - p_off[i], slot)]
+                    r[k, :len(b)] = b
+                return r
+            dump_outputs(args.dump_outputs, n, slot, packed_rows, np.diff(p_off), resp.meta[:n].cpu().numpy().view(np.uint32))
     kernel_ms, kernel_launches = eng.kernel_time_ms(reset=True)
     launches = eng.launch_count() - launches0
     value = n * world * args.steps / (ms / 1e3)
@@ -894,7 +887,7 @@ def main():
                 "ms_per_step": ms / args.steps, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
                 "dtype": "u8", "data": "synthetic", "config": workload_config(n, world, args),
                 "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                             "traffic": profiled_traffic(args.layout) if n == (1 << 20) else None, "peak_source": peak_src, "algorithmic_bytes_per_launch": algo_bytes,
+                             "peak_source": peak_src, "algorithmic_bytes_per_launch": algo_bytes,
                              "algorithmic_bytes_per_request": algo_bytes / n, "kernel_ms_per_launch": per_launch_ms,
                              "kernel": ("gofr::serve_slots_kernel_wide (4 CTAs/SM, 128 registers)" if eng.slot_ctas() == 4 else
                                         "gofr::serve_slots_kernel (5 CTAs/SM)") if args.layout == "slots" else "gofr::serve_kernel"},

@@ -1,6 +1,6 @@
 """Quickstart: the examples/http-server routes of the reference (examples/http-server/main.go:21-25) served by the GPU.
 
-    python examples/quickstart.py            # needs a B200 (there is no CPU path)
+    python examples/quickstart.py            # needs an H100 (there is no CPU path)
 
 Prints the wire bytes of three responses, then the RequestLog lines middleware.Logging would have written for them."""
 import os

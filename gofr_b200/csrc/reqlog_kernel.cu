@@ -1,4 +1,4 @@
-// reqlog_kernel.cu — the RequestLog JSON line of middleware.Logging for a whole batch (sm_100a).
+// reqlog_kernel.cu — the RequestLog JSON line of middleware.Logging for a whole batch (sm_90a).
 //
 // Same execution model as serve_kernel.cu / grpc_kernel.cu: persistent co-resident CTAs, one thread per record, the
 // tile's contiguous arena byte range pulled into shared memory with one TMA bulk copy, exact line lengths scanned in

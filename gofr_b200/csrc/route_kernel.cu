@@ -1,4 +1,4 @@
-// route_kernel.cu — stage 1 of the split API for routes whose closure runs on the host (GOFR_H_HOST), sm_100a.
+// route_kernel.cu — stage 1 of the split API for routes whose closure runs on the host (GOFR_H_HOST), sm_90a.
 //
 // What mux.Router.ServeHTTP and the middleware chain decide before handler.ServeHTTP is reached
 // (pkg/gofr/http/router.go:14,30-33; middleware/cors.go:10-13; pkg/gofr/handler.go:32-36): cleanPath redirect, the

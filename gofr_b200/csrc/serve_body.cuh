@@ -1,6 +1,5 @@
-// serve_body.cuh — the fused, persistent serve kernel for sm_100a (body shared by the two kernels: serve_kernel.cu
-// instantiates the packed layout, serve_slots_kernel.cu the slot layout; separate translation units so that each can be
-// built with the store shape that compiles correctly for it, see gofr_b200/_build.py).
+// serve_body.cuh — the fused, persistent serve kernel for sm_90a (body shared by the two kernels: serve_kernel.cu
+// instantiates the packed layout, serve_slots_kernel.cu the slot layout).
 //
 // One launch replaces, for a whole batch, what the reference does per request on a goroutine:
 // mux.Router.ServeHTTP → Tracer/Logging/CORS → handler.ServeHTTP → Responder.Respond → net/http framing

@@ -85,10 +85,9 @@ GOFR_HD bool warp_any(bool p) {
 
 // ---------------------------------------------------------------------------------------------------------------
 // output writer: appends bytes at an arbitrary byte address of the output; HBM only ever sees whole, aligned 32-byte
-// SECTORS written by one 256-bit st.global.cs.v8 (STG.E.256, new with sm_100) per lane — plus the few edge bytes a
-// response shares with its neighbours.  Measured on B200 (scratch/experiments/bulk_store/v8_bench.cu): one lane per
-// response writing its 528-byte slot with 16-byte stores takes 0.39 ms per 1 Mi responses (every store is a partial
-// sector for L2), with aligned 32-byte stores 0.14 ms — the same as fully coalesced warp-wide stores.
+// SECTORS, each written by two back-to-back 16-byte st.global.cs.v4 of one lane — plus the few edge bytes a response
+// shares with its neighbours.  One lane per response storing at arbitrary 16-byte offsets makes every store a partial
+// sector for L2; aligned whole sectors cost what fully coalesced warp-wide stores cost.
 //
 // Each thread owns a 16-word staging buffer in shared memory, laid out word-major (word k of thread t at
 // [k * CTA + t]): whatever word index a lane is at, its bank is its lane id, so accesses never conflict.  The buffer is
@@ -99,7 +98,7 @@ GOFR_HD bool warp_any(bool p) {
 //            bytes treated as a prefix of the source ("virtual source"): one aligned load + one funnel shift per
 //            output word regardless of source and destination alignment.
 //   flush:   decoupled from producing — between ops, when at least 8 words wait, whole sectors leave as
-//            8 conflict-free LDS + one st.global.cs.v8; no shifting is needed because the buffer is already aligned.
+//            8 conflict-free LDS + two st.global.cs.v4; no shifting is needed because the buffer is already aligned.
 //   edges:   the first sector's leading `lead` bytes and the last sector's tail belong to neighbouring responses
 //            written by other threads; only this response's bytes are stored there.
 // ---------------------------------------------------------------------------------------------------------------
@@ -208,24 +207,14 @@ struct Writer {
 #if defined(GOFR_EXP_NO_STORE)  /* experiment: the kernel without its global stores (what is left is issue/latency bound) */
         if (v0 == 0x12345678u && v1 == 0x9ABCDEF0u && v2 == 0x0F1E2D3Cu)
 #endif
-#if defined(GOFR_STORE256)
-        // not .cs: in a 256-bit build the ONLY evict-first stores are the sector stores, which is what the build-time SASS
-        // check relies on (gofr_b200/_build.py, check_sector_stores)
-        *(uint4*)addr = make_uint4(v0, v1, v2, v3);
-#else
         __stcs((uint4*)addr, make_uint4(v0, v1, v2, v3));
-#endif
 #else
         uint32_t v[4] = {v0, v1, v2, v3};
         memcpy(addr, v, 16);
 #endif
     }
-    // One whole sector: addr is 32-byte aligned.  Two back-to-back 16-byte stores by default.  A single 256-bit store
-    // (st.global.v8.b32 -> STG.E.256, new with sm_100; -DGOFR_STORE256) is 7 % faster on the 1 Mi config-2 batch (0.318
-    // against 0.340 ms) but is NOT shipped: with it, and only with it — two `st.global.v4` in the same asm pass every
-    // test — responses of divergent warps in the packed layout come out with sectors whose first word is right and whose
-    // other seven are stale (DESIGN.md section 6b: memcheck / racecheck clean, deterministic, worse from a noinline
-    // wrapper; the store itself is correct in isolation, scratch/experiments/bulk_store/v8_check.cu).  Unexplained, so off.
+    // One whole sector: addr is 32-byte aligned.  sm_90 has no 256-bit global store, so it is two back-to-back 16-byte
+    // stores; L2 merges the two halves, so HBM still sees a full-sector write.
     template <int SITE = 0>
     GOFR_HD static void store32(uint8_t* addr, uint32_t v0, uint32_t v1, uint32_t v2, uint32_t v3, uint32_t v4, uint32_t v5,
                                 uint32_t v6, uint32_t v7) {
@@ -233,22 +222,7 @@ struct Writer {
 #if defined(GOFR_EXP_NO_STORE)
         if (v0 == 0x12345678u && v1 == 0x9ABCDEF0u && v2 == 0x0F1E2D3Cu)
 #endif
-#if defined(GOFR_STORE256) && defined(GOFR_EXP_V8_PLAIN)
-        asm volatile("st.global.v8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(addr), "r"(v0), "r"(v1), "r"(v2), "r"(v3),
-                     "r"(v4), "r"(v5), "r"(v6), "r"(v7)
-                     : "memory");
-#elif defined(GOFR_STORE256) && defined(GOFR_EXP_V4B64)
-        asm volatile("{\n\t.reg .b64 q0, q1, q2, q3;\n\tmov.b64 q0, {%1,%2};\n\tmov.b64 q1, {%3,%4};\n\tmov.b64 q2, {%5,%6};\n\tmov.b64 q3, {%7,%8};\n\t"
-                     "st.global.cs.v4.b64 [%0], {q0,q1,q2,q3};\n\t}" ::"l"(addr), "r"(v0), "r"(v1), "r"(v2), "r"(v3),
-                     "r"(v4), "r"(v5), "r"(v6), "r"(v7)
-                     : "memory");
-#elif defined(GOFR_STORE256)
-        asm volatile("st.global.cs.v8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(addr), "r"(v0), "r"(v1), "r"(v2), "r"(v3),
-                     "r"(v4), "r"(v5), "r"(v6), "r"(v7)
-                     : "memory");
-#else
         { __stcs((uint4*)addr, make_uint4(v0, v1, v2, v3)); __stcs((uint4*)(addr + 16), make_uint4(v4, v5, v6, v7)); }
-#endif
 #else
         uint32_t v[8] = {v0, v1, v2, v3, v4, v5, v6, v7};
         memcpy(addr, v, 32);

@@ -1,11 +1,9 @@
 // serve_slots_kernel.cu — slot-layout instance of the serve kernel (serve_body.cuh): the resident headline kernel.
 //
-// Two register budgets of the same body exist: this one (5 CTAs/SM, 96 registers: the default) and
-// serve_slots_wide_kernel.cu (4 CTAs/SM, 128 registers: opt-in).  The kernel is issue/latency bound; with five CTAs really
-// resident (the staging budget comes from the occupancy calculator, engine.cu) this instance is 7.5 % faster than the wide
-// one on config 2 (0.2737 against 0.2959 ms per 1 Mi requests) and 11 % faster on config 4 than it was with four.  They
-// are separate translation units because whether CUDA 12.9's ptxas scalarises the 256-bit sector store
-// (serve_device.cuh Writer::store32, _build.py) changes with what else is in the unit.
+// Two register budgets of the same body exist: this one (5 CTAs/SM, 96 registers) and serve_slots_wide_kernel.cu (4 CTAs/SM,
+// 128 registers, for tables that answer with one fast-path program shape: engine.cu choose_slot_residency).  The kernel is
+// issue/latency bound; the staging budget keeps each instance's CTAs really resident (occupancy calculator, engine.cu).
+// Each register budget is its own translation unit, as __launch_bounds__ applies to a whole kernel.
 // Like the packed instance of serve_kernel.cu, this one and the wide one are compiled without the programs of the wider
 // data model (GOFR_TU_VALUES 0); tables that have such programs run serve_slots_values_kernel.cu.
 #define GOFR_TU_VALUES 0

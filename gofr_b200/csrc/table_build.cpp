@@ -693,8 +693,7 @@ namespace gofr {
 
 // The tables the wide slot-layout instance (serve_slots_wide_kernel.cu: 4 CTAs/SM, 128 registers) was meant for: every live
 // route answers through the template fast path with ONE program shape and no Bind — warps never diverge between programs
-// and the general pass after the tile loop only sees the odd escaped string.  Informational since the end of round 2: the
-// 5-CTA instance is the faster one even there (engine.cu choose_slot_residency).
+// and the general pass after the tile loop only sees the odd escaped string (engine.cu choose_slot_residency).
 bool image_wants_wide_slots(const uint8_t* img) {
     const ImageHeader& H = *reinterpret_cast<const ImageHeader*>(img);
     const RouteRec* routes = reinterpret_cast<const RouteRec*>(img + H.routes_off);
@@ -1517,7 +1516,7 @@ int gofr_table_add_route(gofr_table* t, uint32_t method, const char* pattern, ui
 int gofr_table_slot_ctas(const gofr_table* t, int* ctas_per_sm) {
     if (!t || !ctas_per_sm) return GOFR_ERR_INVALID;
     if (!t->sealed) return GOFR_ERR_NOT_SEALED;
-    *ctas_per_sm = gofr::kServeCtas;  // the wide instance is opt-in (engine.cu choose_slot_residency)
+    *ctas_per_sm = gofr::image_wants_wide_slots(t->image.data()) ? gofr::kServeCtasWide : gofr::kServeCtas;  // engine.cu choose_slot_residency
     return GOFR_OK;
 }
 

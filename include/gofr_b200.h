@@ -1,5 +1,5 @@
 /*
- * gofr_b200.h — C ABI of the B200-native GoFr request hot path.
+ * gofr_b200.h — C ABI of the H100-native GoFr request hot path.
  *
  * This is the drop-in boundary (SURVEY.md §8b).  The reference (JigarJoshi04/gofr) has no FFI of its own: its seams
  * are in-process Go interfaces.  Each entry point below names the reference interface it stands in for, so a Go shim
@@ -330,11 +330,12 @@ int gofr_engine_set_chunk(gofr_engine*, uint32_t requests_per_chunk);
 int gofr_engine_set_tile(gofr_engine*, uint32_t in_bytes_per_req);
 int gofr_engine_geometry(const gofr_engine*, uint32_t* grid, uint32_t* blocks_per_sm, uint32_t* smem_bytes,
                          uint32_t* sm_count);
-/* Slot layout: which instance of the serve kernel answers — 5 CTAs/SM with 96 registers (the default, the faster one on every
- * table measured) or 4 CTAs/SM with 128 registers.  ctas_per_sm 0 = query, 4 or 5 = force; *in_effect (may be NULL)
+/* Slot layout: which instance of the serve kernel answers — 4 CTAs/SM with 128 registers (the default for tables whose live
+ * routes answer with one fast-path program shape) or 5 CTAs/SM with 96 registers (every other table).  ctas_per_sm 0 = query,
+ * 4 or 5 = force; *in_effect (may be NULL)
  * receives the value in effect.  Tuning knob, no effect on results. */
 int gofr_engine_slot_ctas(gofr_engine*, int ctas_per_sm, int* in_effect);
-/* the engine's default for a sealed table (5), computable without a GPU */
+/* the engine's default for a sealed table (4 or 5), computable without a GPU */
 int gofr_table_slot_ctas(const gofr_table*, int* ctas_per_sm);
 /* gofr_serve_device reports an undersized d_out through this flag (the launch itself is asynchronous). */
 int gofr_engine_overflowed(gofr_engine*, int* flag_out, int reset);

@@ -2,7 +2,7 @@
  * gofr_oracle.c — TEST INFRASTRUCTURE ONLY (see gofr_oracle.h: "parity unpinned" status and who may call this).
  *
  * Scalar C restatement of one GoFr HTTP request, in the order the reference executes it
- * (SURVEY.md §3.4; all file:line below are relative to /root/reference):
+ * (SURVEY.md §3.4; all file:line below are relative to the reference, JigarJoshi04/gofr @ 17218229):
  *
  *   mux.Router.ServeHTTP            (gorilla/mux v1.8.1 via pkg/gofr/http/router.go:14)   → serve_one()
  *     cleanPath → 301               (mux, before any middleware)                           → mux_clean_path()

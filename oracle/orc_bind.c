@@ -2,7 +2,7 @@
  * orc_bind.c — TEST INFRASTRUCTURE ONLY (see gofr_oracle.h).
  *
  * Restatement of Request.Bind (pkg/gofr/http/request.go:40-47): io.ReadAll + json.Unmarshal(body, &i) where i holds
- * a *struct.  The arithmetic is Go 1.21 encoding/json, which is not in /root/reference (stdlib):
+ * a *struct.  The arithmetic is Go 1.21 encoding/json, which is not in the reference checkout (stdlib):
  *   - checkValid: the byte-at-a-time scanner state machine and its SyntaxError texts        → scan_*()
  *   - decodeState.object/array/literalStore into a struct of string/int/bool fields          → dec_*()
  *   - UnmarshalTypeError texts with errorContext (Struct.Field path)                         → type_error()

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
-"""Opcode histogram per kernel of the built library (cuobjdump -sass): instruction count, the Blackwell / bulk-copy
-mnemonics the profiling guide asks for (UBLKCP = cp.async.bulk, SYNCS = mbarrier, STG.*.256 = 256-bit stores), stores by
+"""Opcode histogram per kernel of the built library (cuobjdump -sass): instruction count, the Hopper bulk-copy
+mnemonics (UBLKCP = cp.async.bulk, SYNCS = mbarrier), stores by
 width, and the 25 most frequent opcodes.  usage: sass_histogram.py [lib.so] > profiles/rNN/sass_histogram.txt"""
 import collections, re, subprocess, sys
 lib = sys.argv[1] if len(sys.argv) > 1 else "gofr_b200/libgofr_b200.so"

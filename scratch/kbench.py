@@ -54,7 +54,7 @@ per = ms / k
 line = {"tag": a.tag or os.environ.get("GOFR_LIB_PATH", "in-tree"), "workload": a.workload, "layout": a.layout, "n": n, "kernel_ms": round(per, 5), "Greq_s": round(n / per / 1e6, 3)}
 if a.workload == "config2":
     algo = batch.input_bytes() + n * synth.C2_WIRE_BYTES + 8 * n + 4
-    line["frac"] = round(algo / (per / 1e3) / 1e9 / 6576.1, 4)
+    line["frac"] = round(algo / (per / 1e3) / 1e9 / 3350.0, 4)  # H100 SXM data-sheet HBM3 bandwidth
 if a.check:
     from tests import oracle as O
     m = min(n, 1 << 16)

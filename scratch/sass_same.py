@@ -3,8 +3,7 @@
 
 "This feature must not touch that kernel" as a check that needs no GPU: the named translation units are compiled from the
 working tree and from REF (default HEAD) with the build's flags, and their `cuobjdump -sass` instruction streams (opcodes,
-registers, immediates — addresses and encodings stripped) are compared.  Used before re-stamping profiles/r02/traffic.json
-(bench.py reports the ncu DRAM traffic of the headline kernel only while the capture still describes the binary that runs).
+registers, immediates — addresses and encodings stripped) are compared.
 """
 import os
 import re
@@ -19,9 +18,7 @@ from gofr_b200 import _build  # noqa: E402
 
 def sass(src_root: str, tu: str, out: str):
     obj = out + ".o"
-    want256 = tu in _build.SECTOR256
-    subprocess.check_call(["nvcc"] + _build.NVCC_FLAGS + (["-DGOFR_STORE256"] if want256 else []) +
-                          ["-c", "-o", obj, os.path.join(src_root, "gofr_b200", "csrc", tu)], stderr=subprocess.DEVNULL)
+    subprocess.check_call(["nvcc"] + _build.NVCC_FLAGS + ["-c", "-o", obj, os.path.join(src_root, "gofr_b200", "csrc", tu)], stderr=subprocess.DEVNULL)
     text = subprocess.run(["cuobjdump", "-sass", obj], capture_output=True, text=True, check=True).stdout
     ins = []
     for ln in text.splitlines():

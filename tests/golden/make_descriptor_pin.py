@@ -2,14 +2,15 @@
 (examples/grpc-server/grpc/hello.pb.go: file_hello_proto_rawDesc) into tests/golden/hello_proto_rawdesc.hex.
 
 It is the one byte string in the reference that a real protobuf encoder produced: tests/test_proto.py pins the proto3
-encoder and decoder to it.  Run in the build container only (the reference is not present on the GPU box):
+encoder and decoder to it.  Needs a checkout of the reference (JigarJoshi04/gofr @ 17218229):
 
-    python tests/golden/make_descriptor_pin.py
+    python tests/golden/make_descriptor_pin.py <reference checkout>
 """
 import os
 import re
+import sys
 
-REF = "/root/reference/examples/grpc-server/grpc/hello.pb.go"
+REF = os.path.join(sys.argv[1], "examples", "grpc-server", "grpc", "hello.pb.go")
 HERE = os.path.dirname(os.path.abspath(__file__))
 
 src = open(REF).read()

@@ -1,4 +1,4 @@
-"""GPU parity (run with -m gpu on the B200 box): the CUDA path, called through the C ABI, vs the CPU oracle."""
+"""GPU parity (run with -m gpu on an H100): the CUDA path, called through the C ABI, vs the CPU oracle."""
 import os
 
 import numpy as np

@@ -115,18 +115,19 @@ def test_mixed_traffic_and_short_slots(torch_cuda):
 
 
 def test_slot_residency_choice():
-    """the 5-CTA instance is the default for every table (the 128-register one is opt-in: it measured slower once the
-    fifth CTA really was resident)"""
-    for spec in (synth.config2_spec(), synth.config4_spec(), synth.config3_spec(), synth.config1_spec()):
+    """the 128-register (4-CTA) instance serves tables that answer with one fast-path program shape (config 2), the 5-CTA
+    instance every other table"""
+    assert Table(synth.config2_spec()).slot_ctas() == 4
+    for spec in (synth.config4_spec(), synth.config3_spec(), synth.config1_spec()):
         assert Table(spec).slot_ctas() == 5
 
 
 @pytest.mark.gpu
 def test_both_slot_residencies(torch_cuda):
-    """The engine runs the 5-CTA instance unless the 4-CTA (128-register) one is asked for; either instance forced on any
-    table gives the same bytes."""
+    """The engine runs the instance the table asks for (Table.slot_ctas); either instance forced on any table gives the
+    same bytes."""
     from gofr_b200.engine import Engine
-    for spec, batch, slot, auto in ((synth.config2_spec(), synth.config2_batch(40000, escape_every=11), 544, 5),
+    for spec, batch, slot, auto in ((synth.config2_spec(), synth.config2_batch(40000, escape_every=11), 544, 4),
                                     (synth.config4_spec(), synth.config4_batch(20000), 1024, 5),
                                     (synth.config3_spec(), synth.config3_batch(4096), 1024, 5)):
         eng = Engine(Table(spec), 0)
