@@ -13,7 +13,7 @@
 
 namespace gofr {
 
-constexpr int BT = 128;
+constexpr int BT = kBindThreads;
 
 __global__ void __launch_bounds__(BT) bind_kernel(const BindParams p) {
     extern __shared__ __align__(128) uint8_t smem[];
@@ -46,15 +46,6 @@ __global__ void __launch_bounds__(BT) bind_kernel(const BindParams p) {
         p.len[i] = len;
         p.status[i] = st;
     }
-}
-
-int launch_bind(const BindParams& p, int sm_count, void* stream) {
-    const uint32_t smem = (p.hot_bytes + 127u) & ~127u;
-    if (cudaFuncSetAttribute(bind_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return (int)cudaGetLastError();
-    int grid = (int)((p.n + BT - 1) / BT);
-    if (grid > sm_count * 8) grid = sm_count * 8;
-    bind_kernel<<<grid, BT, smem, (cudaStream_t)stream>>>(p);
-    return (int)cudaGetLastError();
 }
 
 }  // namespace gofr

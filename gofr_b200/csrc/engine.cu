@@ -47,9 +47,59 @@ void set_last_error(const char* fmt, ...) {
 
 using namespace gofr;
 
+namespace gofr {
+// The kernels (defined in the *_kernel.cu translation units; launched from here through launch()).
+__global__ void serve_kernel(const ServeParams p);               // serve_kernel.cu: packed layout
+__global__ void serve_kernel_values(const ServeParams p);        // serve_values_kernel.cu: packed, PF_VALUES programs
+__global__ void serve_slots_kernel(const ServeParams p);         // serve_slots_kernel.cu: slot layout, 5 CTAs/SM
+__global__ void serve_slots_kernel_wide(const ServeParams p);    // serve_slots_wide_kernel.cu: slot layout, 4 CTAs/SM
+__global__ void serve_slots_kernel_values(const ServeParams p);  // serve_slots_values_kernel.cu: slot layout, PF_VALUES
+__global__ void grpc_hello_kernel(const GrpcParams p);           // grpc_kernel.cu
+__global__ void proto_encode_kernel(const GrpcParams p, const ProtoSchema S);
+__global__ void proto_decode_kernel(const GrpcParams p, const ProtoSchema S);
+__global__ void proto_encode_nested_kernel(const GrpcParams p, const PbnDesc D);  // proto_nested_kernel.cu
+__global__ void proto_decode_nested_kernel(const GrpcParams p, const PbnDesc D);  // proto_nested_decode_kernel.cu
+__global__ void reqlog_kernel(const LogParams p);                // reqlog_kernel.cu
+__global__ void http_parse_kernel(const HttpParams p);           // http_kernel.cu
+__global__ void route_kernel(const RouteParams p);               // route_kernel.cu
+__global__ void bind_kernel(const BindParams p);                 // bind_kernel.cu
+}  // namespace gofr
+
 namespace {
 
+enum Kern {
+    K_SERVE, K_SERVE_VALUES, K_SLOTS, K_SLOTS_WIDE, K_SLOTS_VALUES, K_HELLO, K_PROTO_ENC, K_PROTO_DEC, K_PBN_ENC, K_PBN_DEC,
+    K_REQLOG, K_HTTP, K_ROUTE, K_BIND, K_COUNT
+};
+struct KernelRec {
+    const void* fn;
+    const char* what;  // in error messages: "<what> kernel launch failed"
+    int threads;
+};
+const KernelRec kKernels[K_COUNT] = {
+    {(const void*)serve_kernel, "serve", kServeT},
+    {(const void*)serve_kernel_values, "serve", kServeT},
+    {(const void*)serve_slots_kernel, "serve", kServeT},
+    {(const void*)serve_slots_kernel_wide, "serve", kServeT},
+    {(const void*)serve_slots_kernel_values, "serve", kServeT},
+    {(const void*)grpc_hello_kernel, "grpc", kServeThreads},
+    {(const void*)proto_encode_kernel, "proto", kServeThreads},
+    {(const void*)proto_decode_kernel, "proto", kServeThreads},
+    {(const void*)proto_encode_nested_kernel, "proto", kServeThreads},
+    {(const void*)proto_decode_nested_kernel, "proto", kServeThreads},
+    {(const void*)reqlog_kernel, "request-log", kServeThreads},
+    {(const void*)http_parse_kernel, "http", kServeThreads},
+    {(const void*)route_kernel, "route", kRouteThreads},
+    {(const void*)bind_kernel, "bind", kBindThreads},
+};
+
 constexpr int kSlots = 3;  // pipeline depth of the host-batch path
+
+// Look-back scratch of the kernels that pack their output: one state word per tile of a launch (tile_common.cuh).
+struct TileState {
+    unsigned long long* words = nullptr;
+    size_t tiles = 0;
+};
 
 struct Slot {
     cudaStream_t stream = nullptr;
@@ -59,10 +109,13 @@ struct Slot {
     // device buffers (grown on demand)
     void* d_desc = nullptr; void* d_ids = nullptr; uint8_t* d_arena = nullptr; uint8_t* d_out = nullptr;
     uint32_t* d_off = nullptr; uint32_t* d_meta = nullptr;
-    unsigned long long* d_state = nullptr; uint32_t* d_flag = nullptr; uint32_t* d_bind = nullptr;
-    size_t cap_n = 0, cap_arena = 0, cap_out = 0, cap_tiles = 0;
+    uint32_t* d_flag = nullptr; uint32_t* d_bind = nullptr;
+    TileState state;  // packed layout only
+    size_t cap_n = 0, cap_arena = 0, cap_out = 0;
     // pinned staging for the tiny per-chunk read-backs
     uint32_t* h_tail = nullptr;  // [0] = chunk total bytes, [1] = overflow flag
+
+    int reserve(gofr_engine* e, uint32_t requests, size_t arena_bytes, size_t out_bytes);
 };
 
 }  // namespace
@@ -81,11 +134,11 @@ struct gofr_engine {
     int wide_grid = 0, wide_blocks_per_sm = 0;
     bool slots_wide = false;  // choose_slot_residency
     bool has_values = false;  // some program has PF_VALUES: the packed layout runs serve_kernel_values (serve_values_kernel.cu)
-    int grid = 0, blocks_per_sm = 0, grpc_grid = 0, reqlog_grid = 0, http_grid = 0, proto_grid = 0, proto_decode_grid = 0, proto_nested_grid = 0, proto_nested_decode_grid = 0;
+    int grid = 0, blocks_per_sm = 0;
+    int resident[K_COUNT] = {};  // resident grid of each kernel without dynamic shared memory, asked once (resident_grid)
     uint32_t epoch = 0;
     // resident path scratch
-    unsigned long long* d_state = nullptr;
-    size_t state_tiles = 0;
+    TileState state;
     uint32_t* d_flag = nullptr;
     uint32_t* d_bind = nullptr;  // Bind scratch of the resident path
     size_t bind_cap = 0;
@@ -135,6 +188,62 @@ static void register_engine(int device, int delta) {
     if (device >= 0 && device < 64) g_live_engines[device] += delta;
 }
 
+// cudaFuncAttributeMaxDynamicSharedMemorySize belongs to a kernel on a device, so it is shared by every engine there.  It
+// is only ever raised: once a launch or an occupancy query has made sure it covers some size, it keeps covering it.
+static std::mutex g_attr_mu;
+static uint32_t g_smem_attr[K_COUNT][64];
+static cudaError_t cover_smem(Kern k, int device, uint32_t smem) {
+    std::lock_guard<std::mutex> g(g_attr_mu);
+    const bool cached = device >= 0 && device < 64;
+    if (cached && smem <= g_smem_attr[k][device]) return cudaSuccess;
+    const cudaError_t er = cudaFuncSetAttribute(kKernels[k].fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (er == cudaSuccess && cached) g_smem_attr[k][device] = smem;
+    return er;
+}
+
+// CTAs of kernel k resident per SM with `smem` bytes of dynamic shared memory, asked from the runtime; -1 if it cannot say.
+static int blocks_per_sm(Kern k, int device, uint32_t smem) {
+    int nb = 0;
+    if (cover_smem(k, device, smem) != cudaSuccess ||
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, kKernels[k].fn, kKernels[k].threads, smem) != cudaSuccess) return -1;
+    return nb;
+}
+
+// The serve kernel's five instances: the layout (packed or slots), the programs the table has (PF_VALUES or not) and, for
+// the slot layout, the register budget (the wide 4-CTA instance or the 5-CTA one) pick one.
+static Kern serve_instance(bool slots, bool values, bool wide) {
+    if (!slots) return values ? K_SERVE_VALUES : K_SERVE;
+    return values ? K_SLOTS_VALUES : wide ? K_SLOTS_WIDE : K_SLOTS;
+}
+
+static uint32_t serve_smem_bytes(uint32_t hot_bytes, uint32_t in_cap) { return ((hot_bytes + 127u) & ~127u) + in_cap + 64; }
+
+// CTAs per SM with which every instance of a residency group is resident for `smem` bytes of dynamic shared memory: the wide
+// slot-layout instance alone, or all the others (packed / slots, with and without the wider data model).  Asked from the
+// runtime (static shared memory, registers and the per-CTA reservation included) — a hand-kept formula fell behind the
+// kernel once and the "5-CTA" instances silently ran 4 per SM.
+static int serve_blocks_per_sm(int device, uint32_t smem, bool wide) {
+    if (wide) return blocks_per_sm(K_SLOTS_WIDE, device, smem);
+    int nb = 1 << 30;
+    for (Kern k : {K_SERVE, K_SLOTS, K_SLOTS_VALUES, K_SERVE_VALUES}) {
+        const int b = blocks_per_sm(k, device, smem);
+        if (b < 0) return -1;
+        nb = std::min(nb, b);
+    }
+    return nb;
+}
+
+// The largest request staging budget (bytes per request: a multiple of 16 from 16 to 256) with which `ctas` CTAs of the
+// group stay resident per SM next to a table of hot_bytes; 0 when not even the smallest one fits.
+static uint32_t serve_fit_in_per(int device, uint32_t hot_bytes, int ctas, bool wide) {
+    for (uint32_t in_per = 256; in_per >= 16; in_per -= 16) {
+        const uint32_t smem = serve_smem_bytes(hot_bytes, ((uint32_t)kServeT * in_per + 127u) & ~127u);
+        if (smem > 227u * 1024u) continue;
+        if (serve_blocks_per_sm(device, smem, wide) >= ctas) return in_per;
+    }
+    return 0;
+}
+
 // Which slot-layout instance serves this table (serve_slots_kernel.cu): the wide one (4 CTAs/SM, 128 registers) for tables
 // whose live routes all answer through the template fast path with one program shape (image_wants_wide_slots,
 // table_build.cpp), the 5-CTA one otherwise; GOFR_SLOT_CTAS=4 / 5 (or gofr_engine_slot_ctas) forces one.  On an H100 SXM
@@ -154,11 +263,11 @@ static int configure_geometry(gofr_engine* e, uint32_t in_per_req, uint32_t w_in
     e->w_in_cap = (kServeT * w_in_per_req + 127u) & ~127u;
     e->w_smem_bytes = serve_smem_bytes(e->hdr.hot_bytes, e->w_in_cap);
     if (e->smem_bytes > 227 * 1024 || e->w_smem_bytes > 227 * 1024) { set_last_error("tile geometry needs %u bytes of shared memory", std::max(e->smem_bytes, e->w_smem_bytes)); return GOFR_ERR_CAPACITY; }
-    int g = serve_max_grid(e->smem_bytes, e->device, &e->blocks_per_sm, false);
-    if (g <= 0) { set_last_error("serve kernel cannot be resident with %u bytes of shared memory", e->smem_bytes); return GOFR_ERR_CUDA; }
-    e->grid = g;
-    e->wide_grid = serve_max_grid(e->w_smem_bytes, e->device, &e->wide_blocks_per_sm, true);
-    if (e->wide_grid < 0) e->wide_grid = 0;  // the wide instance is optional: the engine falls back to the others
+    e->blocks_per_sm = serve_blocks_per_sm(e->device, e->smem_bytes, false);
+    if (e->blocks_per_sm <= 0) { set_last_error("serve kernel cannot be resident with %u bytes of shared memory", e->smem_bytes); return GOFR_ERR_CUDA; }
+    e->grid = e->blocks_per_sm * e->sm_count;
+    e->wide_blocks_per_sm = serve_blocks_per_sm(e->device, e->w_smem_bytes, true);
+    e->wide_grid = std::max(0, e->wide_blocks_per_sm * e->sm_count);  // the wide instance is optional: the engine falls back to the others
     return GOFR_OK;
 }
 
@@ -206,8 +315,8 @@ static int engine_init(gofr_engine* e, const std::vector<uint8_t>& img, int devi
     // its CTAs per SM (5, or 4 for the wide slot-layout instance — the kernel is latency bound: residency matters more than
     // staging every tile; larger tiles are read from HBM directly).  The budget is found by asking the runtime's occupancy
     // calculator, not by a formula.
-    uint32_t in_per = serve_fit_in_per(e->hdr.hot_bytes, kServeCtas, false);
-    uint32_t w_in_per = serve_fit_in_per(e->hdr.hot_bytes, kServeCtasWide, true);
+    uint32_t in_per = serve_fit_in_per(device, e->hdr.hot_bytes, kServeCtas, false);
+    uint32_t w_in_per = serve_fit_in_per(device, e->hdr.hot_bytes, kServeCtasWide, true);
     if (in_per < 64u) in_per = 64u;    // a table this large: stage at least short requests, whatever residency is left
     if (w_in_per < in_per) w_in_per = in_per;
     int rc = configure_geometry(e, in_per, w_in_per);
@@ -249,7 +358,7 @@ void gofr_engine_destroy(gofr_engine* e) {
         if (s.ev_served) cudaEventDestroy(s.ev_served);
         if (s.ev_egress) cudaEventDestroy(s.ev_egress);
         cudaFree(s.d_desc); cudaFree(s.d_ids); cudaFree(s.d_arena); cudaFree(s.d_out); cudaFree(s.d_off); cudaFree(s.d_meta);
-        cudaFree(s.d_state); cudaFree(s.d_flag); cudaFree(s.d_bind);
+        cudaFree(s.state.words); cudaFree(s.d_flag); cudaFree(s.d_bind);
         if (s.h_tail) cudaFreeHost(s.h_tail);
     }
     for (auto& ev : e->timing) { cudaEventDestroy(ev.first); cudaEventDestroy(ev.second); }
@@ -259,7 +368,7 @@ void gofr_engine_destroy(gofr_engine* e) {
     if (e->ev_batch_done) cudaEventDestroy(e->ev_batch_done);
     cudaFree(e->d_chain); cudaFree(e->d_info);
     if (e->h_status) cudaFreeHost(e->h_status);
-    cudaFree(e->d_image); cudaFree(e->d_state); cudaFree(e->d_flag); cudaFree(e->d_bind);
+    cudaFree(e->d_image); cudaFree(e->state.words); cudaFree(e->d_flag); cudaFree(e->d_bind);
     cudaFree(e->d_rt_desc); cudaFree(e->d_rt_arena); cudaFree(e->d_rt_meta); cudaFree(e->d_rt_vars); cudaFree(e->d_rt_rows);
     delete e;
 }
@@ -305,9 +414,9 @@ static int next_epoch(gofr_engine* e, uint32_t* out) {
     uint32_t ep = (e->epoch + 1) & gofr::kEpochMask;
     if (ep == 0) {  // wrapped (epoch 0 is what zero-initialised words carry: never handed out)
         if (cudaDeviceSynchronize() != cudaSuccess) { set_last_error("device synchronisation failed at the look-back epoch wrap"); return GOFR_ERR_CUDA; }
-        if (e->d_state && cudaMemset(e->d_state, 0, e->state_tiles * 8) != cudaSuccess) return GOFR_ERR_CUDA;
+        if (e->state.words && cudaMemset(e->state.words, 0, e->state.tiles * 8) != cudaSuccess) return GOFR_ERR_CUDA;
         for (auto& s : e->slots)
-            if (s.d_state && cudaMemset(s.d_state, 0, ((s.cap_n + 63) / 64) * 8) != cudaSuccess) return GOFR_ERR_CUDA;
+            if (s.state.words && cudaMemset(s.state.words, 0, s.state.tiles * 8) != cudaSuccess) return GOFR_ERR_CUDA;
         ep = 1;
     }
     e->epoch = ep;
@@ -315,19 +424,71 @@ static int next_epoch(gofr_engine* e, uint32_t* out) {
     return GOFR_OK;
 }
 
-// one fused launch; `state`/`flag` are scratch owned by the caller of this helper
-static int launch_one(gofr_engine* e, const void* d_desc, const void* d_ids, const uint8_t* d_arena, uint32_t n,
-                      const char* date29, uint8_t* d_out, uint64_t out_cap, uint32_t* d_off, uint32_t* d_meta,
-                      unsigned long long* d_state, uint32_t* d_flag, uint32_t* d_bind, cudaStream_t stream,
-                      const unsigned long long* chain_pos = nullptr, uint32_t slot_bytes = 0) {
+// Grows look-back scratch to the tile count of a launch; new words are zero ("not ready" in every epoch).  A buffer in use
+// by earlier launches is safe to replace: cudaFree synchronises the device.
+static int grow_state(TileState& s, size_t tiles) {
+    if (tiles <= s.tiles) return GOFR_OK;
+    cudaFree(s.words);
+    s.words = nullptr;
+    s.tiles = 0;
+    CUDA_TRY(cudaMalloc(&s.words, tiles * 8));
+    CUDA_TRY(cudaMemset(s.words, 0, tiles * 8));
+    s.tiles = tiles;
+    return GOFR_OK;
+}
+
+// Every kernel launch goes through here, with the engine lock held: the dynamic shared memory the kernel may use on this
+// device covers `smem`, the launch is timed with CUDA events on its stream when timing is on, and it is counted.
+template <class... Args>
+static int launch(gofr_engine* e, Kern k, int grid, uint32_t smem, cudaStream_t st, const Args&... args) {
+    const KernelRec& K = kKernels[k];
+    cudaError_t er = cover_smem(k, e->device, smem);
+    if (er != cudaSuccess) { set_last_error("%s kernel cannot use %u bytes of shared memory: %s", K.what, smem, cudaGetErrorString(er)); return GOFR_ERR_CUDA; }
+    cudaEvent_t ev0 = nullptr, ev1 = nullptr;
+    if (e->timing_on) {
+        fold_timing(e);
+        CUDA_TRY(cudaEventCreate(&ev0));
+        CUDA_TRY(cudaEventCreate(&ev1));
+        CUDA_TRY(cudaEventRecord(ev0, st));
+    }
+    void* argv[] = {const_cast<void*>(static_cast<const void*>(&args))...};
+    cudaLaunchKernel(K.fn, dim3((unsigned)grid), dim3((unsigned)K.threads), argv, smem, st);
+    er = cudaGetLastError();
+    if (er != cudaSuccess) { set_last_error("%s kernel launch failed: %s", K.what, cudaGetErrorString(er)); return GOFR_ERR_CUDA; }
+    if (e->timing_on) {
+        CUDA_TRY(cudaEventRecord(ev1, st));
+        e->timing.emplace_back(ev0, ev1);
+    }
+    e->launches++;
+    return GOFR_OK;
+}
+
+// Resident grid (CTAs per SM x SMs) of a kernel without dynamic shared memory, asked once per engine; 0 with the error set.
+static int resident_grid(gofr_engine* e, Kern k) {
+    if (e->resident[k] <= 0) e->resident[k] = std::max(0, blocks_per_sm(k, e->device, 0)) * e->sm_count;
+    if (e->resident[k] <= 0) set_last_error("%s kernel cannot be resident", kKernels[k].what);
+    return e->resident[k];
+}
+
+// One fused serve launch.  The packed layout (slot_bytes == 0) chains its tiles through the look-back scratch `state`; the
+// slot layout makes the tiles independent of each other and takes none.
+static int launch_serve(gofr_engine* e, const void* d_desc, const void* d_ids, const uint8_t* d_arena, uint32_t n,
+                        const char* date29, uint8_t* d_out, uint64_t out_cap, uint32_t* d_off, uint32_t* d_meta,
+                        TileState* state, uint32_t* d_flag, uint32_t* d_bind, cudaStream_t stream,
+                        const unsigned long long* chain_pos = nullptr, uint32_t slot_bytes = 0) {
     ServeParams p;
     memset(&p, 0, sizeof p);
     p.desc = d_desc; p.ids = d_ids; p.arena = d_arena; p.n = n;
     p.n_tiles = (n + kServeT - 1) / kServeT;
+    if (!slot_bytes) {
+        int rc = grow_state(*state, p.n_tiles);
+        if (rc) return rc;
+        p.tile_state = state->words;
+    }
     p.image = e->d_image; p.hot_bytes = e->hdr.hot_bytes;
     { int erc = next_epoch(e, &p.epoch); if (erc) return erc; }
     p.out = d_out; p.out_cap = out_cap; p.out_off = d_off; p.meta = d_meta;
-    p.tile_state = d_state; p.overflow = d_flag;
+    p.overflow = d_flag;
     const bool wide = slot_bytes && e->slots_wide && !e->has_values && e->wide_grid > 0;
     p.in_cap = wide ? e->w_in_cap : e->in_cap;
     p.bind_scratch = d_bind; p.bind_row_words = e->hdr.bind_row_words;
@@ -337,21 +498,76 @@ static int launch_one(gofr_engine* e, const void* d_desc, const void* d_ids, con
     memcpy(p.date, date29, 29);
     int grid = (int)std::min<uint32_t>((uint32_t)(wide ? e->wide_grid : e->grid), p.n_tiles);
     if (!slot_bytes) grid = std::max(1, std::min(grid, e->grid / engines_on_device(e->device)));  // look-back: see engines_on_device
-    cudaEvent_t ev0 = nullptr, ev1 = nullptr;
-    if (e->timing_on) {
-        fold_timing(e);
-        CUDA_TRY(cudaEventCreate(&ev0));
-        CUDA_TRY(cudaEventCreate(&ev1));
-        CUDA_TRY(cudaEventRecord(ev0, stream));
-    }
-    int rc = launch_serve(p, grid, wide ? e->w_smem_bytes : e->smem_bytes, stream, wide, e->has_values);
-    if (rc != 0) { set_last_error("serve kernel launch failed: %s", cudaGetErrorString((cudaError_t)rc)); return GOFR_ERR_CUDA; }
-    if (e->timing_on) {
-        CUDA_TRY(cudaEventRecord(ev1, stream));
-        e->timing.emplace_back(ev0, ev1);
-    }
-    e->launches++;
+    return launch(e, serve_instance(slot_bytes != 0, e->has_values, wide), grid, wide ? e->w_smem_bytes : e->smem_bytes, stream, p);
+}
+
+// Bind scratch of the resident serve path (tables with GOFR_H_BIND_ECHO routes)
+static int grow_bind_scratch(gofr_engine* e, uint32_t n) {
+    if (!e->hdr.bind_row_words) return GOFR_OK;
+    const size_t need = (size_t)n * e->hdr.bind_row_words * 4;
+    if (need <= e->bind_cap) return GOFR_OK;
+    cudaFree(e->d_bind);
+    e->d_bind = nullptr;
+    e->bind_cap = 0;
+    CUDA_TRY(cudaMalloc(&e->d_bind, need + need / 4 + 256));
+    e->bind_cap = need + need / 4;
     return GOFR_OK;
+}
+
+// The launch of the frame kernels (Hello, proto3 encode / decode, flat and nested, the request log): one thread per record,
+// tiles of kServeThreads chained by the look-back over the engine's resident scratch.  The caller has validated its own
+// arguments and filled the input fields of `p`; `extra` are the kernel's parameters after it (schema or descriptor).
+template <class Params, class... Extra>
+static int launch_frames(gofr_engine* e, Kern k, Params p, uint32_t n, uint8_t* d_out, uint64_t out_cap, uint32_t* d_out_off,
+                         void* stream, const Extra&... extra) {
+    std::lock_guard<std::mutex> g(e->mu);
+    CUDA_TRY(cudaSetDevice(e->device));
+    cudaStream_t st = (cudaStream_t)stream;
+    if (n == 0) { if (d_out_off) CUDA_TRY(cudaMemsetAsync(d_out_off, 0, 4, st)); return GOFR_OK; }
+    const uint32_t tiles = (n + kServeThreads - 1) / kServeThreads;
+    { int rc = grow_state(e->state, tiles); if (rc) return rc; }
+    const int resident = resident_grid(e, k);
+    if (!resident) return GOFR_ERR_CUDA;
+    p.n = n; p.n_tiles = tiles;
+    { int rc = next_epoch(e, &p.epoch); if (rc) return rc; }
+    p.out = d_out; p.out_cap = out_cap; p.out_off = d_out_off;
+    p.tile_state = e->state.words; p.overflow = e->d_flag;
+    const int grid = (int)std::min<uint32_t>((uint32_t)std::max(1, resident / engines_on_device(e->device)), tiles);
+    return launch(e, k, grid, 0, st, p, extra...);
+}
+
+// The schema index of a Bind target, or an error: not part of the engine's table, or not a struct Bind takes.
+static int bind_schema(const gofr_engine* e, uint32_t schema_id, uint32_t* idx) {
+    for (size_t k = 0; k < e->schema_ids.size(); k++) {
+        if (e->schema_ids[k] != schema_id) continue;
+        if (!(e->schema_flags[k] & SF_BINDABLE)) { set_last_error("schema %u: Bind takes flat structs of int / float64 / bool / string fields only", schema_id); return GOFR_ERR_UNSUPPORTED; }
+        *idx = (uint32_t)k;
+        return GOFR_OK;
+    }
+    set_last_error("schema %u is not part of the engine's table", schema_id);
+    return GOFR_ERR_INVALID;
+}
+
+// The stages of the split API: one thread per request over the table's hot part in shared memory, no dependence between
+// requests, so the grid is capped at a few CTAs per SM rather than sized for residency.
+static int launch_route_kernel(gofr_engine* e, const void* d_desc, const uint8_t* d_arena, uint32_t n, uint32_t* d_meta,
+                               uint32_t* d_vars, cudaStream_t st) {
+    RouteParams p;
+    memset(&p, 0, sizeof p);
+    p.desc = d_desc; p.arena = d_arena; p.n = n; p.image = e->d_image; p.hot_bytes = e->hdr.hot_bytes;
+    p.meta = d_meta; p.vars = d_vars;
+    const uint32_t grid = std::min<uint32_t>((n + kRouteThreads - 1) / kRouteThreads, (uint32_t)e->sm_count * 4);
+    return launch(e, K_ROUTE, (int)grid, (e->hdr.hot_bytes + 127u) & ~127u, st, p);
+}
+
+static int launch_bind_kernel(gofr_engine* e, uint32_t schema_idx, const void* d_desc, const uint8_t* d_arena, uint32_t n,
+                              uint8_t* d_rows, uint32_t slot_bytes, uint32_t* d_len, uint32_t* d_status, cudaStream_t st) {
+    BindParams p;
+    memset(&p, 0, sizeof p);
+    p.desc = d_desc; p.arena = d_arena; p.n = n; p.image = e->d_image; p.hot_bytes = e->hdr.hot_bytes; p.schema_idx = schema_idx;
+    p.out = d_rows; p.slot_bytes = slot_bytes; p.len = d_len; p.status = d_status;
+    const uint32_t grid = std::min<uint32_t>((n + kBindThreads - 1) / kBindThreads, (uint32_t)e->sm_count * 8);
+    return launch(e, K_BIND, (int)grid, (e->hdr.hot_bytes + 127u) & ~127u, st, p);
 }
 
 extern "C" {
@@ -367,26 +583,9 @@ int gofr_serve_device(gofr_engine* e, const gofr_req_desc* d_desc, const uint8_t
         if (d_out_off) CUDA_TRY(cudaMemsetAsync(d_out_off, 0, 4, st));
         return GOFR_OK;
     }
-    size_t tiles = (n + 63) / 64;  // enough for any tile size in use (serve: kServeT, gRPC / log: 128)
-    if (tiles > e->state_tiles) {
-        // grow the look-back scratch; stream-ordered w.r.t. earlier launches because cudaFree synchronises
-        cudaFree(e->d_state);
-        e->d_state = nullptr;
-        CUDA_TRY(cudaMalloc(&e->d_state, tiles * 8));
-        CUDA_TRY(cudaMemset(e->d_state, 0, tiles * 8));
-        e->state_tiles = tiles;
-    }
-    if (e->hdr.bind_row_words) {
-        size_t need = (size_t)n * e->hdr.bind_row_words * 4;
-        if (need > e->bind_cap) {
-            cudaFree(e->d_bind);
-            e->d_bind = nullptr;
-            CUDA_TRY(cudaMalloc(&e->d_bind, need + need / 4 + 256));
-            e->bind_cap = need + need / 4;
-        }
-    }
-    return launch_one(e, d_desc, d_trace_ids, d_arena, n, date29, d_out, out_cap, d_out_off, d_meta, e->d_state, e->d_flag,
-                      e->d_bind, st);
+    { int rc = grow_bind_scratch(e, n); if (rc) return rc; }
+    return launch_serve(e, d_desc, d_trace_ids, d_arena, n, date29, d_out, out_cap, d_out_off, d_meta, &e->state, e->d_flag,
+                        e->d_bind, st);
 }
 
 int gofr_serve_device_slots(gofr_engine* e, const gofr_req_desc* d_desc, const uint8_t* d_trace_ids, const uint8_t* d_arena,
@@ -400,18 +599,9 @@ int gofr_serve_device_slots(gofr_engine* e, const gofr_req_desc* d_desc, const u
     if (n == 0) return GOFR_OK;
     std::lock_guard<std::mutex> g(e->mu);
     CUDA_TRY(cudaSetDevice(e->device));
-    if (e->hdr.bind_row_words) {
-        size_t need = (size_t)n * e->hdr.bind_row_words * 4;
-        if (need > e->bind_cap) {
-            cudaFree(e->d_bind);
-            e->d_bind = nullptr;
-            CUDA_TRY(cudaMalloc(&e->d_bind, need + need / 4 + 256));
-            e->bind_cap = need + need / 4;
-        }
-    }
-    // no look-back scratch: slots make the tiles independent of each other
-    return launch_one(e, d_desc, d_trace_ids, d_arena, n, date29, d_out, (uint64_t)n * slot_bytes, d_out_len, d_meta, nullptr,
-                      e->d_flag, e->d_bind, (cudaStream_t)stream, nullptr, slot_bytes);
+    { int rc = grow_bind_scratch(e, n); if (rc) return rc; }
+    return launch_serve(e, d_desc, d_trace_ids, d_arena, n, date29, d_out, (uint64_t)n * slot_bytes, d_out_len, d_meta, nullptr,
+                        e->d_flag, e->d_bind, (cudaStream_t)stream, nullptr, slot_bytes);
 }
 
 int gofr_engine_overflowed(gofr_engine* e, int* flag_out, int reset) {
@@ -495,15 +685,15 @@ static constexpr size_t kArenaSlack = 16;
 // A chunk = contiguous request range [lo, hi) and the arena byte range it covers.
 struct ChunkPlan { uint32_t lo, hi; uint32_t arena_lo, arena_hi; };
 
-// The arena byte range [*alo, *ahi) (16-byte granular) that requests [lo, hi) reference.  All arithmetic in 64 bits: a
-// descriptor with a huge arena_off or data_len (say a data_len taken from a Content-Length header) must be refused, not
-// wrap around and pass.
-static int chunk_arena_range(const gofr_req_batch* in, uint32_t lo, uint32_t hi, uint32_t* alo_out, uint32_t* ahi_out) {
+// The arena byte range [*alo, *ahi) (16-byte granular) that requests [lo, hi) reference: their whole requests, or their paths
+// only (what routing reads).  All arithmetic in 64 bits: a descriptor with a huge arena_off or data_len (say a data_len taken
+// from a Content-Length header) must be refused, not wrap around and pass.
+static int chunk_arena_range(const gofr_req_batch* in, uint32_t lo, uint32_t hi, bool path_only, uint32_t* alo_out, uint32_t* ahi_out) {
     uint64_t alo = ~0ull, ahi = 0;
     const gofr_req_desc* dd = in->desc;
     for (uint32_t i = lo; i < hi; i++) {
         const uint64_t a = dd[i].arena_off;
-        const uint64_t dend = ((a + dd[i].path_len + dd[i].query_len + 3u) & ~3ull) + dd[i].data_len;
+        const uint64_t dend = path_only ? a + dd[i].path_len : ((a + dd[i].path_len + dd[i].query_len + 3u) & ~3ull) + dd[i].data_len;
         alo = a < alo ? a : alo;
         ahi = dend > ahi ? dend : ahi;
     }
@@ -518,6 +708,53 @@ static int chunk_arena_range(const gofr_req_batch* in, uint32_t lo, uint32_t hi,
     *alo_out = (uint32_t)alo;
     *ahi_out = (uint32_t)(ahi > alo ? ahi : alo);
     return GOFR_OK;
+}
+
+// Enqueues the H2D copies of a chunk on `st`: descriptors and trace ids of requests [lo, lo + n) (no ids: d_ids null) and
+// the arena bytes [alo, ahi) they reference, as far as the caller's arena has them.
+static int upload_chunk(const gofr_req_batch* in, uint32_t lo, uint32_t n, uint32_t alo, uint32_t ahi, void* d_desc, void* d_ids,
+                        uint8_t* d_arena, cudaStream_t st) {
+    CUDA_TRY(cudaMemcpyAsync(d_desc, in->desc + lo, (size_t)n * 16, cudaMemcpyHostToDevice, st));
+    if (d_ids) CUDA_TRY(cudaMemcpyAsync(d_ids, in->trace_ids + (size_t)lo * 16, (size_t)n * 16, cudaMemcpyHostToDevice, st));
+    if (ahi > alo) {
+        const size_t avail = in->arena_bytes > alo ? (size_t)in->arena_bytes - alo : 0;
+        CUDA_TRY(cudaMemcpyAsync(d_arena, in->arena + alo, std::min<size_t>(ahi - alo, avail), cudaMemcpyHostToDevice, st));
+    }
+    return GOFR_OK;
+}
+
+// The slot's previous chunk must have left (egress) before its buffers are overwritten: a wait on the H2D stream, unless
+// the buffers have to grow (cudaFree needs the host to be sure).
+static int wait_egress(gofr_engine* e, Slot& s, bool grows) {
+    if (!s.egress_pending) return GOFR_OK;
+    if (grows) CUDA_TRY(cudaEventSynchronize(s.ev_egress));
+    else CUDA_TRY(cudaStreamWaitEvent(e->st_h2d, s.ev_egress, 0));
+    s.egress_pending = false;
+    return GOFR_OK;
+}
+
+// Makes the slot's buffers ready for a chunk of `requests` requests, `arena_bytes` arena bytes and `out_bytes` of output.
+int Slot::reserve(gofr_engine* e, uint32_t requests, size_t arena_bytes, size_t out_bytes) {
+    { int rc = wait_egress(e, *this, requests > cap_n || arena_bytes + kArenaSlack > cap_arena || out_bytes > cap_out); if (rc) return rc; }
+    if (requests > cap_n) {
+        cudaFree(d_desc); cudaFree(d_ids); cudaFree(d_off); cudaFree(d_meta); cudaFree(d_bind);
+        d_desc = d_ids = nullptr; d_off = d_meta = nullptr; d_bind = nullptr;
+        cap_n = 0;
+        const size_t c = (size_t)requests + requests / 4 + 256;
+        if (cudaMalloc(&d_desc, c * 16) != cudaSuccess || cudaMalloc(&d_ids, c * 16) != cudaSuccess ||
+            cudaMalloc(&d_off, (c + 1) * 4) != cudaSuccess || cudaMalloc(&d_meta, c * 4) != cudaSuccess ||
+            (e->hdr.bind_row_words && cudaMalloc(&d_bind, c * e->hdr.bind_row_words * 4 + 256) != cudaSuccess)) {
+            set_last_error("cudaMalloc failed for a %zu-request chunk", c);
+            return GOFR_ERR_NOMEM;
+        }
+        cap_n = c;
+    }
+    if (!d_flag && (cudaMalloc(&d_flag, 64) != cudaSuccess || cudaMemset(d_flag, 0, 64) != cudaSuccess)) {
+        set_last_error("cudaMalloc failed for a chunk's overflow flag");
+        return GOFR_ERR_NOMEM;
+    }
+    int rc = grow((void**)&d_arena, &cap_arena, arena_bytes + kArenaSlack, 256);
+    return rc ? rc : grow((void**)&d_out, &cap_out, out_bytes, 256);
 }
 
 // Waits for everything enqueued on the egress stream.  A large batch takes milliseconds: the thread sleeps on a
@@ -576,7 +813,7 @@ static int batch_submit_locked(gofr_engine* e, const gofr_req_batch* in, gofr_re
         if (planned[ci]) return GOFR_OK;
         uint32_t lo = (uint32_t)(ci * e->chunk), hi = std::min<uint32_t>(n, lo + e->chunk);
         uint32_t alo = 0, ahi = 0;
-        int prc = chunk_arena_range(in, lo, hi, &alo, &ahi);
+        int prc = chunk_arena_range(in, lo, hi, false, &alo, &ahi);
         if (prc) return prc;
         plan[ci] = {lo, hi, alo, ahi};
         planned[ci] = 1;
@@ -588,26 +825,7 @@ static int batch_submit_locked(gofr_engine* e, const gofr_req_batch* in, gofr_re
         if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); return false; }
         return a.type == cudaMemoryTypeHost || a.type == cudaMemoryTypeManaged;
     };
-    if (n && !getenv("GOFR_LEGACY_EGRESS") && device_visible(out->out) && device_visible(out->out_off) && device_visible(out->meta)) {
-        auto ensure_s = [&](Slot& s, uint32_t cn, size_t abytes, size_t ocap) -> int {
-            if (cn > s.cap_n) {
-                cudaFree(s.d_desc); cudaFree(s.d_ids); cudaFree(s.d_off); cudaFree(s.d_meta); cudaFree(s.d_state); cudaFree(s.d_bind);
-                s.d_desc = s.d_ids = nullptr; s.d_off = s.d_meta = nullptr; s.d_state = nullptr; s.d_bind = nullptr;
-                size_t c = (size_t)cn + cn / 4 + 256;
-                size_t tiles = (c + 63) / 64;
-                if (cudaMalloc(&s.d_desc, c * 16) != cudaSuccess || cudaMalloc(&s.d_ids, c * 16) != cudaSuccess ||
-                    cudaMalloc(&s.d_off, (c + 1) * 4) != cudaSuccess || cudaMalloc(&s.d_meta, c * 4) != cudaSuccess ||
-                    cudaMalloc(&s.d_state, tiles * 8) != cudaSuccess) { set_last_error("cudaMalloc failed for a %zu-request chunk", c); s.cap_n = 0; return GOFR_ERR_NOMEM; }
-                if (cudaMemset(s.d_state, 0, tiles * 8) != cudaSuccess) return GOFR_ERR_CUDA;
-                if (e->hdr.bind_row_words && cudaMalloc(&s.d_bind, c * e->hdr.bind_row_words * 4 + 256) != cudaSuccess) { s.cap_n = 0; return GOFR_ERR_NOMEM; }
-                s.cap_n = c;
-            }
-            if (!s.d_flag) { if (cudaMalloc(&s.d_flag, 64) != cudaSuccess || cudaMemset(s.d_flag, 0, 64) != cudaSuccess) return GOFR_ERR_NOMEM; }
-            int rc;
-            if ((rc = grow((void**)&s.d_arena, &s.cap_arena, abytes + kArenaSlack, 256))) return rc;
-            if ((rc = grow((void**)&s.d_out, &s.cap_out, ocap, 256))) return rc;
-            return GOFR_OK;
-        };
+    if (n && device_visible(out->out) && device_visible(out->out_off) && device_visible(out->meta)) {
         // growing buffers frees memory: make sure nothing from an earlier batch is still using them
         CUDA_TRY(cudaMemsetAsync(e->d_chain, 0, 8, e->st_compute));
         e->h_status[0] = 0; e->h_status[1] = 0;
@@ -618,26 +836,13 @@ static int batch_submit_locked(gofr_engine* e, const gofr_req_batch* in, gofr_re
             uint32_t cn = c.hi - c.lo;
             size_t abytes = (size_t)c.arena_hi - c.arena_lo;
             size_t ocap = std::min<size_t>((size_t)cn * (e->hdr.max_fixed_len + 64) + (size_t)image_data_expand(e->hdr) * abytes + 4096, 0xFFFFFFF0ull);
-            if (s.egress_pending) {
-                // the slot's previous chunk must have left before its buffers are overwritten: a stream-side wait,
-                // unless the buffers have to grow (cudaFree needs the host to be sure)
-                const bool grows = cn > s.cap_n || abytes + kArenaSlack > s.cap_arena || ocap > s.cap_out;
-                if (grows) CUDA_TRY(cudaEventSynchronize(s.ev_egress));
-                else CUDA_TRY(cudaStreamWaitEvent(e->st_h2d, s.ev_egress, 0));
-                s.egress_pending = false;
-            }
-            int rc = ensure_s(s, cn, abytes, ocap);
+            int rc = s.reserve(e, cn, abytes, ocap);
+            if (!rc) rc = upload_chunk(in, c.lo, cn, c.arena_lo, c.arena_hi, s.d_desc, s.d_ids, s.d_arena, e->st_h2d);
             if (rc) return rc;
-            CUDA_TRY(cudaMemcpyAsync(s.d_desc, in->desc + c.lo, (size_t)cn * 16, cudaMemcpyHostToDevice, e->st_h2d));
-            CUDA_TRY(cudaMemcpyAsync(s.d_ids, in->trace_ids + (size_t)c.lo * 16, (size_t)cn * 16, cudaMemcpyHostToDevice, e->st_h2d));
-            if (abytes) {
-                size_t avail = in->arena_bytes > c.arena_lo ? (size_t)in->arena_bytes - c.arena_lo : 0;
-                CUDA_TRY(cudaMemcpyAsync(s.d_arena, in->arena + c.arena_lo, std::min(abytes, avail), cudaMemcpyHostToDevice, e->st_h2d));
-            }
             CUDA_TRY(cudaEventRecord(s.ev_h2d, e->st_h2d));
             CUDA_TRY(cudaStreamWaitEvent(e->st_compute, s.ev_h2d, 0));
-            rc = launch_one(e, s.d_desc, s.d_ids, s.d_arena - c.arena_lo, cn, in->date, s.d_out, s.cap_out, s.d_off, s.d_meta,
-                            s.d_state, s.d_flag, s.d_bind, e->st_compute, e->d_chain);
+            rc = launch_serve(e, s.d_desc, s.d_ids, s.d_arena - c.arena_lo, cn, in->date, s.d_out, s.cap_out, s.d_off, s.d_meta,
+                              &s.state, s.d_flag, s.d_bind, e->st_compute, e->d_chain);
             if (rc) return rc;
             if (launch_advance(e->d_chain, s.d_off, cn, s.d_flag, e->d_info + (ci % kSlots), out->out_cap, e->st_compute) != 0) {
                 set_last_error("advance kernel launch failed"); return GOFR_ERR_CUDA;
@@ -664,27 +869,7 @@ static int batch_submit_locked(gofr_engine* e, const gofr_req_batch* in, gofr_re
         return GOFR_OK;
     }
 
-    // ---- straightforward 3-slot software pipeline ----
-    auto ensure = [&](Slot& s, uint32_t cn, size_t abytes, size_t ocap) -> int {
-        int rc;
-        if (cn > s.cap_n) {
-            cudaFree(s.d_desc); cudaFree(s.d_ids); cudaFree(s.d_off); cudaFree(s.d_meta); cudaFree(s.d_state); cudaFree(s.d_bind);
-            s.d_desc = s.d_ids = nullptr; s.d_off = s.d_meta = nullptr; s.d_state = nullptr; s.d_bind = nullptr;
-            size_t c = (size_t)cn + cn / 4 + 256;
-            size_t tiles = (c + 63) / 64;
-            if (cudaMalloc(&s.d_desc, c * 16) != cudaSuccess || cudaMalloc(&s.d_ids, c * 16) != cudaSuccess ||
-                cudaMalloc(&s.d_off, (c + 1) * 4) != cudaSuccess || cudaMalloc(&s.d_meta, c * 4) != cudaSuccess ||
-                cudaMalloc(&s.d_state, tiles * 8) != cudaSuccess) { set_last_error("cudaMalloc failed for a %zu-request chunk", c); s.cap_n = 0; return GOFR_ERR_NOMEM; }
-            if (cudaMemset(s.d_state, 0, tiles * 8) != cudaSuccess) return GOFR_ERR_CUDA;
-            if (e->hdr.bind_row_words && cudaMalloc(&s.d_bind, c * e->hdr.bind_row_words * 4 + 256) != cudaSuccess) { set_last_error("cudaMalloc failed for Bind scratch"); s.cap_n = 0; return GOFR_ERR_NOMEM; }
-            s.cap_n = c;
-        }
-        if (!s.d_flag) { if (cudaMalloc(&s.d_flag, 64) != cudaSuccess || cudaMemset(s.d_flag, 0, 64) != cudaSuccess) return GOFR_ERR_NOMEM; }
-        if ((rc = grow((void**)&s.d_arena, &s.cap_arena, abytes + kArenaSlack, 256))) return rc;
-        if ((rc = grow((void**)&s.d_out, &s.cap_out, ocap, 256))) return rc;
-        return GOFR_OK;
-    };
-
+    // ---- pageable caller buffers: 3-slot software pipeline, each chunk's exact size copied back once it is known ----
     size_t issued = 0, finished = 0;
     uint64_t write_pos = 0;
     const size_t nchunks = plan.size();
@@ -699,17 +884,12 @@ static int batch_submit_locked(gofr_engine* e, const gofr_req_batch* in, gofr_re
             uint32_t cn = c.hi - c.lo;
             size_t abytes = (size_t)c.arena_hi - c.arena_lo;
             size_t ocap = std::min<size_t>((size_t)cn * (e->hdr.max_fixed_len + 64) + (size_t)image_data_expand(e->hdr) * abytes + 4096, 0xFFFFFFF0ull);
-            int rc = ensure(s, cn, abytes, ocap);
+            int rc = s.reserve(e, cn, abytes, ocap);
+            if (!rc) rc = upload_chunk(in, c.lo, cn, c.arena_lo, c.arena_hi, s.d_desc, s.d_ids, s.d_arena, s.stream);
             if (rc) return rc;
-            CUDA_TRY(cudaMemcpyAsync(s.d_desc, in->desc + c.lo, (size_t)cn * 16, cudaMemcpyHostToDevice, s.stream));
-            CUDA_TRY(cudaMemcpyAsync(s.d_ids, in->trace_ids + (size_t)c.lo * 16, (size_t)cn * 16, cudaMemcpyHostToDevice, s.stream));
-            if (abytes) {
-                size_t avail = in->arena_bytes > c.arena_lo ? (size_t)in->arena_bytes - c.arena_lo : 0;
-                CUDA_TRY(cudaMemcpyAsync(s.d_arena, in->arena + c.arena_lo, std::min(abytes, avail), cudaMemcpyHostToDevice, s.stream));
-            }
             // descriptors keep absolute arena offsets: pass a rebased arena pointer
-            rc = launch_one(e, s.d_desc, s.d_ids, s.d_arena - c.arena_lo, cn, in->date, s.d_out, s.cap_out, s.d_off, s.d_meta,
-                            s.d_state, s.d_flag, s.d_bind, s.stream);
+            rc = launch_serve(e, s.d_desc, s.d_ids, s.d_arena - c.arena_lo, cn, in->date, s.d_out, s.cap_out, s.d_off, s.d_meta,
+                              &s.state, s.d_flag, s.d_bind, s.stream);
             if (rc) return rc;
             CUDA_TRY(cudaMemcpyAsync(out->out_off + c.lo, s.d_off, (size_t)cn * 4, cudaMemcpyDeviceToHost, s.stream));
             CUDA_TRY(cudaMemcpyAsync(out->meta + c.lo, s.d_meta, (size_t)cn * 4, cudaMemcpyDeviceToHost, s.stream));
@@ -760,39 +940,15 @@ static int batch_submit_slots_locked(gofr_engine* e, const gofr_req_batch* in, g
         // the chunk's request range and the arena bytes it covers (scanned right before the chunk is enqueued)
         const uint32_t lo = (uint32_t)(ci * e->chunk), hi = std::min<uint32_t>(n, lo + e->chunk), cn = hi - lo;
         uint32_t alo = 0, ahi = 0;
-        { int prc = chunk_arena_range(in, lo, hi, &alo, &ahi); if (prc) return prc; }
-        const size_t abytes = (size_t)ahi - alo, obytes = (size_t)cn * slot;
-        if (s.egress_pending) {  // the slot's previous chunk must have left before its buffers are reused
-            const bool grows = cn > s.cap_n || abytes + kArenaSlack > s.cap_arena || obytes > s.cap_out;
-            if (grows) CUDA_TRY(cudaEventSynchronize(s.ev_egress));
-            else CUDA_TRY(cudaStreamWaitEvent(e->st_h2d, s.ev_egress, 0));
-            s.egress_pending = false;
-        }
-        if (cn > s.cap_n) {
-            cudaFree(s.d_desc); cudaFree(s.d_ids); cudaFree(s.d_off); cudaFree(s.d_meta); cudaFree(s.d_state); cudaFree(s.d_bind);
-            s.d_desc = s.d_ids = nullptr; s.d_off = s.d_meta = nullptr; s.d_state = nullptr; s.d_bind = nullptr;
-            const size_t c = (size_t)cn + cn / 4 + 256, tiles = (c + 63) / 64;
-            if (cudaMalloc(&s.d_desc, c * 16) != cudaSuccess || cudaMalloc(&s.d_ids, c * 16) != cudaSuccess ||
-                cudaMalloc(&s.d_off, (c + 1) * 4) != cudaSuccess || cudaMalloc(&s.d_meta, c * 4) != cudaSuccess ||
-                cudaMalloc(&s.d_state, tiles * 8) != cudaSuccess) { set_last_error("cudaMalloc failed for a %zu-request chunk", c); s.cap_n = 0; return GOFR_ERR_NOMEM; }
-            if (cudaMemset(s.d_state, 0, tiles * 8) != cudaSuccess) return GOFR_ERR_CUDA;
-            if (e->hdr.bind_row_words && cudaMalloc(&s.d_bind, c * e->hdr.bind_row_words * 4 + 256) != cudaSuccess) { s.cap_n = 0; return GOFR_ERR_NOMEM; }
-            s.cap_n = c;
-        }
-        if (!s.d_flag) { if (cudaMalloc(&s.d_flag, 64) != cudaSuccess || cudaMemset(s.d_flag, 0, 64) != cudaSuccess) return GOFR_ERR_NOMEM; }
-        int rc;
-        if ((rc = grow((void**)&s.d_arena, &s.cap_arena, abytes + kArenaSlack, 256))) return rc;
-        if ((rc = grow((void**)&s.d_out, &s.cap_out, obytes, 256))) return rc;
-        CUDA_TRY(cudaMemcpyAsync(s.d_desc, in->desc + lo, (size_t)cn * 16, cudaMemcpyHostToDevice, e->st_h2d));
-        CUDA_TRY(cudaMemcpyAsync(s.d_ids, in->trace_ids + (size_t)lo * 16, (size_t)cn * 16, cudaMemcpyHostToDevice, e->st_h2d));
-        if (abytes) {
-            const size_t avail = in->arena_bytes > alo ? (size_t)in->arena_bytes - alo : 0;
-            CUDA_TRY(cudaMemcpyAsync(s.d_arena, in->arena + alo, std::min(abytes, avail), cudaMemcpyHostToDevice, e->st_h2d));
-        }
+        int rc = chunk_arena_range(in, lo, hi, false, &alo, &ahi);
+        const size_t obytes = (size_t)cn * slot;
+        if (!rc) rc = s.reserve(e, cn, (size_t)ahi - alo, obytes);
+        if (!rc) rc = upload_chunk(in, lo, cn, alo, ahi, s.d_desc, s.d_ids, s.d_arena, e->st_h2d);
+        if (rc) return rc;
         CUDA_TRY(cudaEventRecord(s.ev_h2d, e->st_h2d));
         CUDA_TRY(cudaStreamWaitEvent(e->st_compute, s.ev_h2d, 0));
-        rc = launch_one(e, s.d_desc, s.d_ids, s.d_arena - alo, cn, in->date, s.d_out, obytes, s.d_off, s.d_meta, s.d_state, s.d_flag,
-                        s.d_bind, e->st_compute, nullptr, slot);
+        rc = launch_serve(e, s.d_desc, s.d_ids, s.d_arena - alo, cn, in->date, s.d_out, obytes, s.d_off, s.d_meta, nullptr, s.d_flag,
+                          s.d_bind, e->st_compute, nullptr, slot);
         if (rc) return rc;
         CUDA_TRY(cudaEventRecord(s.ev_served, e->st_compute));
         CUDA_TRY(cudaStreamWaitEvent(e->st_egress, s.ev_served, 0));
@@ -904,40 +1060,10 @@ void gofr_format_http_date(int64_t unix_seconds, char out29[29]) {
 int gofr_grpc_hello_device(gofr_engine* e, const uint8_t* d_in, const uint32_t* d_in_off, uint32_t n, uint8_t* d_out,
                            uint64_t out_cap, uint32_t* d_out_off, uint32_t* d_meta, void* stream) {
     if (!e || (n && (!d_in || !d_in_off || !d_out || !d_out_off || !d_meta))) return GOFR_ERR_INVALID;
-    std::lock_guard<std::mutex> g(e->mu);
-    CUDA_TRY(cudaSetDevice(e->device));
-    cudaStream_t st = (cudaStream_t)stream;
-    if (n == 0) { if (d_out_off) CUDA_TRY(cudaMemsetAsync(d_out_off, 0, 4, st)); return GOFR_OK; }
-    size_t tiles = (n + kServeThreads - 1) / kServeThreads;
-    if (tiles > e->state_tiles) {
-        cudaFree(e->d_state);
-        e->d_state = nullptr;
-        CUDA_TRY(cudaMalloc(&e->d_state, tiles * 8));
-        CUDA_TRY(cudaMemset(e->d_state, 0, tiles * 8));
-        e->state_tiles = tiles;
-    }
-    if (e->grpc_grid <= 0) {
-        e->grpc_grid = grpc_max_grid(e->device);
-        if (e->grpc_grid <= 0) { set_last_error("grpc kernel cannot be resident"); return GOFR_ERR_CUDA; }
-    }
     GrpcParams p;
     memset(&p, 0, sizeof p);
-    p.in = d_in; p.in_off = d_in_off; p.n = n; p.n_tiles = (uint32_t)tiles;
-    { int erc = next_epoch(e, &p.epoch); if (erc) return erc; }
-    p.out = d_out; p.out_cap = out_cap; p.out_off = d_out_off; p.meta = d_meta;
-    p.tile_state = e->d_state; p.overflow = e->d_flag;
-    cudaEvent_t ev0 = nullptr, ev1 = nullptr;
-    if (e->timing_on) {
-        fold_timing(e);
-        CUDA_TRY(cudaEventCreate(&ev0));
-        CUDA_TRY(cudaEventCreate(&ev1));
-        CUDA_TRY(cudaEventRecord(ev0, st));
-    }
-    int rc = launch_grpc_hello(p, (int)std::min<size_t>((size_t)std::max(1, e->grpc_grid / engines_on_device(e->device)), tiles), st);
-    if (rc != 0) { set_last_error("grpc kernel launch failed: %s", cudaGetErrorString((cudaError_t)rc)); return GOFR_ERR_CUDA; }
-    if (e->timing_on) { CUDA_TRY(cudaEventRecord(ev1, st)); e->timing.emplace_back(ev0, ev1); }
-    e->launches++;
-    return GOFR_OK;
+    p.in = d_in; p.in_off = d_in_off; p.meta = d_meta;
+    return launch_frames(e, K_HELLO, p, n, d_out, out_cap, d_out_off, stream);
 }
 
 // rows → frames (decode == false) or frames → rows (decode == true): the same launch plumbing, two codecs
@@ -962,42 +1088,10 @@ static int proto_run(gofr_engine* e, const gofr_proto_field* fields, uint32_t n_
         S.cls[k] = (uint8_t)proto_class(t);
         S.fixed_bytes += is64 ? 8u : 4u;
     }
-    std::lock_guard<std::mutex> g(e->mu);
-    CUDA_TRY(cudaSetDevice(e->device));
-    cudaStream_t st = (cudaStream_t)stream;
-    if (n == 0) { if (d_out_off) CUDA_TRY(cudaMemsetAsync(d_out_off, 0, 4, st)); return GOFR_OK; }
-    size_t tiles = (n + kServeThreads - 1) / kServeThreads;
-    if (tiles > e->state_tiles) {
-        cudaFree(e->d_state);
-        e->d_state = nullptr;
-        CUDA_TRY(cudaMalloc(&e->d_state, tiles * 8));
-        CUDA_TRY(cudaMemset(e->d_state, 0, tiles * 8));
-        e->state_tiles = tiles;
-    }
-    int& grid = decode ? e->proto_decode_grid : e->proto_grid;
-    if (grid <= 0) {
-        grid = decode ? proto_decode_max_grid(e->device) : proto_max_grid(e->device);
-        if (grid <= 0) { set_last_error("proto kernel cannot be resident"); return GOFR_ERR_CUDA; }
-    }
     GrpcParams p;
     memset(&p, 0, sizeof p);
-    p.in = d_rows; p.in_off = d_row_off; p.n = n; p.n_tiles = (uint32_t)tiles;
-    { int erc = next_epoch(e, &p.epoch); if (erc) return erc; }
-    p.out = d_out; p.out_cap = out_cap; p.out_off = d_out_off; p.meta = d_meta;
-    p.tile_state = e->d_state; p.overflow = e->d_flag;
-    cudaEvent_t ev0 = nullptr, ev1 = nullptr;
-    if (e->timing_on) {
-        fold_timing(e);
-        CUDA_TRY(cudaEventCreate(&ev0));
-        CUDA_TRY(cudaEventCreate(&ev1));
-        CUDA_TRY(cudaEventRecord(ev0, st));
-    }
-    const int g_ = (int)std::min<size_t>((size_t)std::max(1, grid / engines_on_device(e->device)), tiles);
-    int rc = decode ? launch_proto_decode(p, S, g_, st) : launch_proto_encode(p, S, g_, st);
-    if (rc != 0) { set_last_error("proto kernel launch failed: %s", cudaGetErrorString((cudaError_t)rc)); return GOFR_ERR_CUDA; }
-    if (e->timing_on) { CUDA_TRY(cudaEventRecord(ev1, st)); e->timing.emplace_back(ev0, ev1); }
-    e->launches++;
-    return GOFR_OK;
+    p.in = d_rows; p.in_off = d_row_off; p.meta = d_meta;
+    return launch_frames(e, decode ? K_PROTO_DEC : K_PROTO_ENC, p, n, d_out, out_cap, d_out_off, stream, S);
 }
 
 // message types with nested / repeated fields -> the kernel's descriptor: validation, words of every fixed part, nesting depth
@@ -1069,34 +1163,10 @@ static int proto_nested_run(gofr_engine* e, const gofr_proto_nmsg* msgs, uint32_
     if (!e || (n && (!d_in || !d_in_off || !d_out || !d_out_off || !d_meta))) return GOFR_ERR_INVALID;
     PbnDesc D;
     { int rc = pbn_build(msgs, n_msgs, fields, n_fields, root, &D); if (rc) return rc; }
-    std::lock_guard<std::mutex> g(e->mu);
-    CUDA_TRY(cudaSetDevice(e->device));
-    cudaStream_t st = (cudaStream_t)stream;
-    if (n == 0) { if (d_out_off) CUDA_TRY(cudaMemsetAsync(d_out_off, 0, 4, st)); return GOFR_OK; }
-    size_t tiles = (n + kServeThreads - 1) / kServeThreads;
-    if (tiles > e->state_tiles) {
-        cudaFree(e->d_state);
-        e->d_state = nullptr;
-        CUDA_TRY(cudaMalloc(&e->d_state, tiles * 8));
-        CUDA_TRY(cudaMemset(e->d_state, 0, tiles * 8));
-        e->state_tiles = tiles;
-    }
-    int& grid = decode ? e->proto_nested_decode_grid : e->proto_nested_grid;
-    if (grid <= 0) {
-        grid = decode ? proto_nested_decode_max_grid(e->device) : proto_nested_max_grid(e->device);
-        if (grid <= 0) { set_last_error("proto kernel cannot be resident"); return GOFR_ERR_CUDA; }
-    }
     GrpcParams p;
     memset(&p, 0, sizeof p);
-    p.in = d_in; p.in_off = d_in_off; p.n = n; p.n_tiles = (uint32_t)tiles;
-    { int erc = next_epoch(e, &p.epoch); if (erc) return erc; }
-    p.out = d_out; p.out_cap = out_cap; p.out_off = d_out_off; p.meta = d_meta;
-    p.tile_state = e->d_state; p.overflow = e->d_flag;
-    const int g_ = (int)std::min<size_t>((size_t)std::max(1, grid / engines_on_device(e->device)), tiles);
-    int rc = decode ? launch_proto_decode_nested(p, D, g_, st) : launch_proto_encode_nested(p, D, g_, st);
-    if (rc != 0) { set_last_error("proto kernel launch failed: %s", cudaGetErrorString((cudaError_t)rc)); return GOFR_ERR_CUDA; }
-    e->launches++;
-    return GOFR_OK;
+    p.in = d_in; p.in_off = d_in_off; p.meta = d_meta;
+    return launch_frames(e, decode ? K_PBN_DEC : K_PBN_ENC, p, n, d_out, out_cap, d_out_off, stream, D);
 }
 
 int gofr_proto_encode_nested_device(gofr_engine* e, const gofr_proto_nmsg* msgs, uint32_t n_msgs, const gofr_proto_nfield* fields,
@@ -1140,34 +1210,40 @@ int gofr_route_device(gofr_engine* e, const gofr_req_desc* d_desc, const uint8_t
     if (n == 0) return GOFR_OK;
     std::lock_guard<std::mutex> g(e->mu);
     CUDA_TRY(cudaSetDevice(e->device));
-    RouteParams p;
-    memset(&p, 0, sizeof p);
-    p.desc = d_desc; p.arena = d_arena; p.n = n; p.image = e->d_image; p.hot_bytes = e->hdr.hot_bytes;
-    p.meta = d_meta; p.vars = d_vars;
-    int rc = launch_route(p, e->sm_count, stream);
-    if (rc != 0) { set_last_error("route kernel launch failed: %s", cudaGetErrorString((cudaError_t)rc)); return GOFR_ERR_CUDA; }
-    e->launches++;
-    return GOFR_OK;
+    return launch_route_kernel(e, d_desc, d_arena, n, d_meta, d_vars, (cudaStream_t)stream);
 }
 
 int gofr_bind_device(gofr_engine* e, uint32_t schema_id, const gofr_req_desc* d_desc, const uint8_t* d_arena, uint32_t n,
                      uint8_t* d_rows, uint32_t slot_bytes, uint32_t* d_len, uint32_t* d_status, void* stream) {
     if (!e || (n && (!d_desc || !d_arena || !d_rows || !d_len || !d_status))) return GOFR_ERR_INVALID;
     if (slot_bytes == 0 || (slot_bytes & 15u) || ((uintptr_t)d_rows & 15u)) { set_last_error("slot_bytes must be a positive multiple of 16 and d_rows 16-byte aligned"); return GOFR_ERR_INVALID; }
-    uint32_t sidx = 0xFFFFFFFFu;
-    for (size_t k = 0; k < e->schema_ids.size(); k++) if (e->schema_ids[k] == schema_id) sidx = (uint32_t)k;
-    if (sidx == 0xFFFFFFFFu) { set_last_error("schema %u is not part of the engine's table", schema_id); return GOFR_ERR_INVALID; }
-    if (!(e->schema_flags[sidx] & SF_BINDABLE)) { set_last_error("schema %u: Bind takes flat structs of int / float64 / bool / string fields only", schema_id); return GOFR_ERR_UNSUPPORTED; }
+    uint32_t sidx = 0;
+    { int rc = bind_schema(e, schema_id, &sidx); if (rc) return rc; }
     if (n == 0) return GOFR_OK;
     std::lock_guard<std::mutex> g(e->mu);
     CUDA_TRY(cudaSetDevice(e->device));
-    BindParams p;
-    memset(&p, 0, sizeof p);
-    p.desc = d_desc; p.arena = d_arena; p.n = n; p.image = e->d_image; p.hot_bytes = e->hdr.hot_bytes; p.schema_idx = sidx;
-    p.out = d_rows; p.slot_bytes = slot_bytes; p.len = d_len; p.status = d_status;
-    int rc = launch_bind(p, e->sm_count, stream);
-    if (rc != 0) { set_last_error("bind kernel launch failed: %s", cudaGetErrorString((cudaError_t)rc)); return GOFR_ERR_CUDA; }
-    e->launches++;
+    return launch_bind_kernel(e, sidx, d_desc, d_arena, n, d_rows, slot_bytes, d_len, d_status, (cudaStream_t)stream);
+}
+
+// The chunk loop of the split API's host stages (gofr_batch_route, gofr_batch_bind): a chunk's descriptors and the arena
+// bytes it reads go up, `stage(lo, n, arena, stream)` launches its kernel on them and enqueues the copies of its result
+// columns, and they are back before the next chunk goes up.
+static int host_stage(gofr_engine* e, const gofr_req_batch* in, bool path_only,
+                      const std::function<int(uint32_t, uint32_t, const uint8_t*, cudaStream_t)>& stage) {
+    std::lock_guard<std::mutex> g(e->mu);
+    CUDA_TRY(cudaSetDevice(e->device));
+    const cudaStream_t st = e->st_compute;
+    for (uint32_t lo = 0; lo < in->n; lo += e->chunk) {
+        const uint32_t hi = std::min<uint32_t>(in->n, lo + e->chunk), cn = hi - lo;
+        uint32_t alo = 0, ahi = 0;
+        int rc = chunk_arena_range(in, lo, hi, path_only, &alo, &ahi);
+        if (!rc) rc = grow((void**)&e->d_rt_desc, &e->rt_desc_cap, (size_t)cn * 16, 256);
+        if (!rc) rc = grow((void**)&e->d_rt_arena, &e->rt_arena_cap, (size_t)ahi - alo + kArenaSlack, 256);
+        if (!rc) rc = upload_chunk(in, lo, cn, alo, ahi, e->d_rt_desc, nullptr, e->d_rt_arena, st);
+        if (!rc) rc = stage(lo, cn, e->d_rt_arena - alo, st);  // descriptors keep absolute arena offsets
+        if (rc) return rc;
+        CUDA_TRY(cudaStreamSynchronize(st));
+    }
     return GOFR_OK;
 }
 
@@ -1175,88 +1251,33 @@ int gofr_batch_bind(gofr_engine* e, uint32_t schema_id, const gofr_req_batch* in
                     uint32_t* len, uint32_t* status) {
     if (!e || !in || (in->n && (!in->desc || !rows || !len || !status))) return GOFR_ERR_INVALID;
     if (slot_bytes == 0 || (slot_bytes & 15u)) { set_last_error("slot_bytes must be a positive multiple of 16"); return GOFR_ERR_INVALID; }
-    uint32_t sidx = 0xFFFFFFFFu;
-    for (size_t k = 0; k < e->schema_ids.size(); k++) if (e->schema_ids[k] == schema_id) sidx = (uint32_t)k;
-    if (sidx == 0xFFFFFFFFu) { set_last_error("schema %u is not part of the engine's table", schema_id); return GOFR_ERR_INVALID; }
-    if (!(e->schema_flags[sidx] & SF_BINDABLE)) { set_last_error("schema %u: Bind takes flat structs of int / float64 / bool / string fields only", schema_id); return GOFR_ERR_UNSUPPORTED; }
-    std::lock_guard<std::mutex> g(e->mu);
-    CUDA_TRY(cudaSetDevice(e->device));
-    const uint32_t n = in->n;
-    for (uint32_t lo = 0; lo < n; lo += e->chunk) {
-        const uint32_t hi = std::min<uint32_t>(n, lo + e->chunk), cn = hi - lo;
-        uint32_t alo = 0, ahi = 0;
-        { int prc = chunk_arena_range(in, lo, hi, &alo, &ahi); if (prc) return prc; }
-        const size_t abytes = (size_t)ahi - alo;
-        int rc;
-        if ((rc = grow((void**)&e->d_rt_desc, &e->rt_desc_cap, (size_t)cn * 16, 256))) return rc;
-        if ((rc = grow((void**)&e->d_rt_arena, &e->rt_arena_cap, abytes + 16, 256))) return rc;
-        if ((rc = grow((void**)&e->d_rt_meta, &e->rt_meta_cap, (size_t)cn * 8, 256))) return rc;
-        if ((rc = grow((void**)&e->d_rt_rows, &e->rt_rows_cap, (size_t)cn * slot_bytes, 256))) return rc;
-        cudaStream_t st = e->st_compute;
-        CUDA_TRY(cudaMemcpyAsync(e->d_rt_desc, in->desc + lo, (size_t)cn * 16, cudaMemcpyHostToDevice, st));
-        if (abytes) {
-            const size_t avail = in->arena_bytes > alo ? (size_t)in->arena_bytes - alo : 0;
-            CUDA_TRY(cudaMemcpyAsync(e->d_rt_arena, in->arena + alo, std::min(abytes, avail), cudaMemcpyHostToDevice, st));
-        }
-        BindParams p;
-        memset(&p, 0, sizeof p);
-        p.desc = e->d_rt_desc; p.arena = e->d_rt_arena - alo; p.n = cn; p.image = e->d_image; p.hot_bytes = e->hdr.hot_bytes;
-        p.schema_idx = sidx; p.out = e->d_rt_rows; p.slot_bytes = slot_bytes;
-        p.len = (uint32_t*)e->d_rt_meta; p.status = (uint32_t*)e->d_rt_meta + cn;
-        rc = launch_bind(p, e->sm_count, st);
-        if (rc != 0) { set_last_error("bind kernel launch failed: %s", cudaGetErrorString((cudaError_t)rc)); return GOFR_ERR_CUDA; }
-        e->launches++;
+    uint32_t sidx = 0;
+    { int rc = bind_schema(e, schema_id, &sidx); if (rc) return rc; }
+    return host_stage(e, in, false, [&](uint32_t lo, uint32_t cn, const uint8_t* d_arena, cudaStream_t st) -> int {
+        int rc = grow((void**)&e->d_rt_meta, &e->rt_meta_cap, (size_t)cn * 8, 256);
+        if (!rc) rc = grow((void**)&e->d_rt_rows, &e->rt_rows_cap, (size_t)cn * slot_bytes, 256);
+        uint32_t* d_len = (uint32_t*)e->d_rt_meta;
+        if (!rc) rc = launch_bind_kernel(e, sidx, e->d_rt_desc, d_arena, cn, e->d_rt_rows, slot_bytes, d_len, d_len + cn, st);
+        if (rc) return rc;
         CUDA_TRY(cudaMemcpyAsync(rows + (size_t)lo * slot_bytes, e->d_rt_rows, (size_t)cn * slot_bytes, cudaMemcpyDeviceToHost, st));
-        CUDA_TRY(cudaMemcpyAsync(len + lo, p.len, (size_t)cn * 4, cudaMemcpyDeviceToHost, st));
-        CUDA_TRY(cudaMemcpyAsync(status + lo, p.status, (size_t)cn * 4, cudaMemcpyDeviceToHost, st));
-        CUDA_TRY(cudaStreamSynchronize(st));
-    }
-    return GOFR_OK;
+        CUDA_TRY(cudaMemcpyAsync(len + lo, d_len, (size_t)cn * 4, cudaMemcpyDeviceToHost, st));
+        CUDA_TRY(cudaMemcpyAsync(status + lo, d_len + cn, (size_t)cn * 4, cudaMemcpyDeviceToHost, st));
+        return GOFR_OK;
+    });
 }
 
 int gofr_batch_route(gofr_engine* e, const gofr_req_batch* in, uint32_t* meta, uint32_t* vars) {
     if (!e || !in || (in->n && (!in->desc || !meta || !vars))) return GOFR_ERR_INVALID;
-    std::lock_guard<std::mutex> g(e->mu);
-    CUDA_TRY(cudaSetDevice(e->device));
-    const uint32_t n = in->n;
-    for (uint32_t lo = 0; lo < n; lo += e->chunk) {
-        const uint32_t hi = std::min<uint32_t>(n, lo + e->chunk), cn = hi - lo;
-        uint64_t alo64 = ~0ull, ahi64 = 0;
-        for (uint32_t i = lo; i < hi; i++) {  // routing reads the path only
-            const gofr_req_desc& d = in->desc[i];
-            const uint64_t a = d.arena_off, b = a + d.path_len;
-            alo64 = a < alo64 ? a : alo64;
-            ahi64 = b > ahi64 ? b : ahi64;
-        }
-        alo64 &= ~15ull;
-        ahi64 = (ahi64 + 15ull) & ~15ull;
-        if (ahi64 > (((uint64_t)in->arena_bytes + 15ull) & ~15ull) || ahi64 > 0xFFFFFFF0ull) { set_last_error("a descriptor of requests %u..%u points outside the arena", lo, hi); return GOFR_ERR_INVALID; }
-        if (ahi64 > alo64 && !in->arena) { set_last_error("requests reference arena bytes but the batch has no arena"); return GOFR_ERR_INVALID; }
-        const uint32_t alo = (uint32_t)alo64, ahi = (uint32_t)(ahi64 > alo64 ? ahi64 : alo64);
-        const size_t abytes = (size_t)ahi - alo;
-        int rc;
-        if ((rc = grow((void**)&e->d_rt_desc, &e->rt_desc_cap, (size_t)cn * 16, 256))) return rc;
-        if ((rc = grow((void**)&e->d_rt_arena, &e->rt_arena_cap, abytes + 16, 256))) return rc;
-        if ((rc = grow((void**)&e->d_rt_meta, &e->rt_meta_cap, (size_t)cn * 4, 256))) return rc;
-        if ((rc = grow((void**)&e->d_rt_vars, &e->rt_vars_cap, (size_t)cn * 4 * GOFR_MAX_PATH_VARS, 256))) return rc;
-        cudaStream_t st = e->st_compute;
-        CUDA_TRY(cudaMemcpyAsync(e->d_rt_desc, in->desc + lo, (size_t)cn * 16, cudaMemcpyHostToDevice, st));
-        if (abytes) {
-            const size_t avail = in->arena_bytes > alo ? (size_t)in->arena_bytes - alo : 0;
-            CUDA_TRY(cudaMemcpyAsync(e->d_rt_arena, in->arena + alo, std::min(abytes, avail), cudaMemcpyHostToDevice, st));
-        }
-        RouteParams p;
-        memset(&p, 0, sizeof p);
-        p.desc = (const gofr_req_desc*)e->d_rt_desc; p.arena = e->d_rt_arena - alo; p.n = cn; p.image = e->d_image;
-        p.hot_bytes = e->hdr.hot_bytes; p.meta = (uint32_t*)e->d_rt_meta; p.vars = (uint32_t*)e->d_rt_vars;
-        rc = launch_route(p, e->sm_count, st);
-        if (rc != 0) { set_last_error("route kernel launch failed: %s", cudaGetErrorString((cudaError_t)rc)); return GOFR_ERR_CUDA; }
-        e->launches++;
+    return host_stage(e, in, true, [&](uint32_t lo, uint32_t cn, const uint8_t* d_arena, cudaStream_t st) -> int {
+        const size_t vbytes = (size_t)cn * 4 * GOFR_MAX_PATH_VARS;
+        int rc = grow((void**)&e->d_rt_meta, &e->rt_meta_cap, (size_t)cn * 4, 256);
+        if (!rc) rc = grow((void**)&e->d_rt_vars, &e->rt_vars_cap, vbytes, 256);
+        if (!rc) rc = launch_route_kernel(e, e->d_rt_desc, d_arena, cn, (uint32_t*)e->d_rt_meta, (uint32_t*)e->d_rt_vars, st);
+        if (rc) return rc;
         CUDA_TRY(cudaMemcpyAsync(meta + lo, e->d_rt_meta, (size_t)cn * 4, cudaMemcpyDeviceToHost, st));
-        CUDA_TRY(cudaMemcpyAsync(vars + (size_t)lo * GOFR_MAX_PATH_VARS, e->d_rt_vars, (size_t)cn * 4 * GOFR_MAX_PATH_VARS, cudaMemcpyDeviceToHost, st));
-        CUDA_TRY(cudaStreamSynchronize(st));
-    }
-    return GOFR_OK;
+        CUDA_TRY(cudaMemcpyAsync(vars + (size_t)lo * GOFR_MAX_PATH_VARS, e->d_rt_vars, vbytes, cudaMemcpyDeviceToHost, st));
+        return GOFR_OK;
+    });
 }
 
 int gofr_http_parse_device(gofr_engine* e, const uint8_t* d_raw, const uint32_t* d_raw_off, uint32_t n, gofr_req_desc* d_desc,
@@ -1265,66 +1286,23 @@ int gofr_http_parse_device(gofr_engine* e, const uint8_t* d_raw, const uint32_t*
     if (n == 0) return GOFR_OK;
     std::lock_guard<std::mutex> g(e->mu);
     CUDA_TRY(cudaSetDevice(e->device));
-    if (e->http_grid <= 0) {
-        e->http_grid = http_max_grid(e->device);
-        if (e->http_grid <= 0) { set_last_error("http kernel cannot be resident"); return GOFR_ERR_CUDA; }
-    }
+    const int resident = resident_grid(e, K_HTTP);
+    if (!resident) return GOFR_ERR_CUDA;
     HttpParams p;
     memset(&p, 0, sizeof p);
     p.raw = d_raw; p.raw_off = d_raw_off; p.n = n; p.n_tiles = (n + kServeThreads - 1) / kServeThreads;
     p.desc = d_desc; p.arena = d_arena; p.status = d_status; p.spans = (unsigned long long*)d_spans;
-    cudaStream_t st = (cudaStream_t)stream;
-    cudaEvent_t ev0 = nullptr, ev1 = nullptr;
-    if (e->timing_on) {
-        fold_timing(e);
-        CUDA_TRY(cudaEventCreate(&ev0));
-        CUDA_TRY(cudaEventCreate(&ev1));
-        CUDA_TRY(cudaEventRecord(ev0, st));
-    }
-    int rc = launch_http_parse(p, (int)std::min<uint32_t>((uint32_t)e->http_grid, p.n_tiles), st);
-    if (rc != 0) { set_last_error("http kernel launch failed: %s", cudaGetErrorString((cudaError_t)rc)); return GOFR_ERR_CUDA; }
-    if (e->timing_on) { CUDA_TRY(cudaEventRecord(ev1, st)); e->timing.emplace_back(ev0, ev1); }
-    e->launches++;
-    return GOFR_OK;
+    // no look-back: every message's result lands in the bytes it occupies, so the whole resident grid runs
+    return launch(e, K_HTTP, (int)std::min<uint32_t>((uint32_t)resident, p.n_tiles), 0, (cudaStream_t)stream, p);
 }
 
 int gofr_requestlog_device(gofr_engine* e, const gofr_log_desc* d_desc, const uint8_t* d_trace_ids, const uint8_t* d_arena,
                            uint32_t n, uint8_t* d_out, uint64_t out_cap, uint32_t* d_out_off, void* stream) {
     if (!e || (n && (!d_desc || !d_trace_ids || !d_arena || !d_out || !d_out_off))) return GOFR_ERR_INVALID;
-    std::lock_guard<std::mutex> g(e->mu);
-    CUDA_TRY(cudaSetDevice(e->device));
-    cudaStream_t st = (cudaStream_t)stream;
-    if (n == 0) { if (d_out_off) CUDA_TRY(cudaMemsetAsync(d_out_off, 0, 4, st)); return GOFR_OK; }
-    size_t tiles = (n + kServeThreads - 1) / kServeThreads;
-    if (tiles > e->state_tiles) {
-        cudaFree(e->d_state);
-        e->d_state = nullptr;
-        CUDA_TRY(cudaMalloc(&e->d_state, tiles * 8));
-        CUDA_TRY(cudaMemset(e->d_state, 0, tiles * 8));
-        e->state_tiles = tiles;
-    }
-    if (e->reqlog_grid <= 0) {
-        e->reqlog_grid = reqlog_max_grid(e->device);
-        if (e->reqlog_grid <= 0) { set_last_error("request-log kernel cannot be resident"); return GOFR_ERR_CUDA; }
-    }
     LogParams p;
     memset(&p, 0, sizeof p);
-    p.desc = d_desc; p.ids = d_trace_ids; p.arena = d_arena; p.n = n; p.n_tiles = (uint32_t)tiles;
-    { int erc = next_epoch(e, &p.epoch); if (erc) return erc; }
-    p.out = d_out; p.out_cap = out_cap; p.out_off = d_out_off;
-    p.tile_state = e->d_state; p.overflow = e->d_flag;
-    cudaEvent_t ev0 = nullptr, ev1 = nullptr;
-    if (e->timing_on) {
-        fold_timing(e);
-        CUDA_TRY(cudaEventCreate(&ev0));
-        CUDA_TRY(cudaEventCreate(&ev1));
-        CUDA_TRY(cudaEventRecord(ev0, st));
-    }
-    int rc = launch_reqlog(p, (int)std::min<size_t>((size_t)std::max(1, e->reqlog_grid / engines_on_device(e->device)), tiles), st);
-    if (rc != 0) { set_last_error("request-log kernel launch failed: %s", cudaGetErrorString((cudaError_t)rc)); return GOFR_ERR_CUDA; }
-    if (e->timing_on) { CUDA_TRY(cudaEventRecord(ev1, st)); e->timing.emplace_back(ev0, ev1); }
-    e->launches++;
-    return GOFR_OK;
+    p.desc = d_desc; p.ids = d_trace_ids; p.arena = d_arena;
+    return launch_frames(e, K_REQLOG, p, n, d_out, out_cap, d_out_off, stream);
 }
 
 }  // extern "C"

@@ -63,15 +63,6 @@ inline uint32_t image_data_expand(const Header& H) { return H.reserved3[0] > 6u 
 // table_build.cpp: which slot-layout instance suits the sealed table (engine.cu choose_slot_residency)
 bool image_wants_wide_slots(const uint8_t* image);
 
-// Returns dynamic shared memory bytes needed for the table's hot part plus the request-byte staging area.
-uint32_t serve_smem_bytes(uint32_t hot_bytes, uint32_t in_cap);
-// cudaError_t as int
-int launch_serve(const ServeParams& p, int grid, uint32_t smem_bytes, void* stream, bool wide_slots = false, bool values = false);
-// grid of the persistent kernels of a group (wide: the 4-CTA slot-layout instance; else all the others) for that much
-// dynamic shared memory, and the largest per-request staging budget that keeps `ctas` CTAs of the group resident
-int serve_max_grid(uint32_t smem_bytes, int device, int* blocks_per_sm, bool wide);
-uint32_t serve_fit_in_per(uint32_t hot_bytes, int ctas, bool wide);
-
 // egress of the host-batch path (egress_kernel.cu)
 struct ChunkInfo {
     unsigned long long host_base;  // where this chunk starts in the caller's output buffer
@@ -98,7 +89,6 @@ struct GrpcParams {
     unsigned long long* tile_state;
     uint32_t* overflow;
 };
-int launch_grpc_hello(const GrpcParams& p, int grid, void* stream);
 // message types of gofr_proto_encode_nested_device (kernel parameter, by value): up to 8 message types with 48 fields in
 // all; fields of a type are consecutive, in ascending field-number order.  Rows use the layout of the wider data model
 // (include/gofr_b200.h "Row format"): a singular message field is a presence word + the message's fixed part inline, a
@@ -116,10 +106,6 @@ struct PbnDesc {
     uint16_t first[kPbnMaxMsgs], count[kPbnMaxMsgs], fixed_words[kPbnMaxMsgs];
     PbnField f[kPbnMaxFields];
 };
-int launch_proto_encode_nested(const GrpcParams& p, const PbnDesc& D, int grid, void* stream);
-int proto_nested_max_grid(int device);
-int launch_proto_decode_nested(const GrpcParams& p, const PbnDesc& D, int grid, void* stream);
-int proto_nested_decode_max_grid(int device);
 
 // message type of gofr_proto_encode_device (kernel parameter, by value); 32 = GOFR_PROTO_MAX_FIELDS
 struct ProtoSchema {
@@ -161,11 +147,8 @@ GOFR_INTERNAL_HD uint32_t proto_class(uint32_t t) {
     if (t == 8) c |= PC_BOOL;                 // BOOL
     return c;
 }
-int launch_proto_encode(const GrpcParams& p, const ProtoSchema& S, int grid, void* stream);
-int proto_max_grid(int device);
-int launch_proto_decode(const GrpcParams& p, const ProtoSchema& S, int grid, void* stream);
-int proto_decode_max_grid(int device);
 
+constexpr int kRouteThreads = 256;  // route_kernel.cu: requests per CTA, one per thread
 struct RouteParams {
     const void* desc;
     const uint8_t* arena;
@@ -175,8 +158,8 @@ struct RouteParams {
     uint32_t* meta;   // n: status | route << 16
     uint32_t* vars;   // n * kMaxVars: off | len << 16
 };
-int launch_route(const RouteParams& p, int sm_count, void* stream);
 
+constexpr int kBindThreads = 128;   // bind_kernel.cu
 struct BindParams {
     const void* desc;
     const uint8_t* arena;
@@ -189,7 +172,6 @@ struct BindParams {
     uint32_t* len;         // n
     uint32_t* status;      // n
 };
-int launch_bind(const BindParams& p, int sm_count, void* stream);
 
 struct HttpParams {
     const uint8_t* raw;
@@ -201,8 +183,6 @@ struct HttpParams {
     uint32_t* status;         // n
     unsigned long long* spans;  // n * GOFR_HTTP_SPANS
 };
-int launch_http_parse(const HttpParams& p, int grid, void* stream);
-int http_max_grid(int device);
 
 struct LogParams {
     const void* desc;   // gofr_log_desc[n]
@@ -217,8 +197,5 @@ struct LogParams {
     unsigned long long* tile_state;
     uint32_t* overflow;
 };
-int launch_reqlog(const LogParams& p, int grid, void* stream);
-int reqlog_max_grid(int device);
-int grpc_max_grid(int device);
 
 }  // namespace gofr

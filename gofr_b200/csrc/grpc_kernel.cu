@@ -43,49 +43,10 @@ __global__ void __launch_bounds__(GT, 8) proto_encode_kernel(const GrpcParams p,
     frame_tiles(p, ProtoCodec{S}, sh);
 }
 
-int launch_grpc_hello(const GrpcParams& p, int grid, void* stream) {
-    grpc_hello_kernel<<<grid, GT, 0, (cudaStream_t)stream>>>(p);
-    return (int)cudaGetLastError();
-}
-
 // frames → rows (gofr_proto_decode_device)
 __global__ void __launch_bounds__(GT, 8) proto_decode_kernel(const GrpcParams p, const __grid_constant__ ProtoSchema S) {
     __shared__ __align__(16) GrpcShared sh;
     frame_tiles(p, ProtoDecodeCodec{S}, sh);
-}
-
-int launch_proto_decode(const GrpcParams& p, const ProtoSchema& S, int grid, void* stream) {
-    proto_decode_kernel<<<grid, GT, 0, (cudaStream_t)stream>>>(p, S);
-    return (int)cudaGetLastError();
-}
-
-int proto_decode_max_grid(int device) {
-    cudaDeviceProp prop;
-    if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) return -1;
-    int nb = 0;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, proto_decode_kernel, GT, 0) != cudaSuccess) return -1;
-    return nb * prop.multiProcessorCount;
-}
-
-int launch_proto_encode(const GrpcParams& p, const ProtoSchema& S, int grid, void* stream) {
-    proto_encode_kernel<<<grid, GT, 0, (cudaStream_t)stream>>>(p, S);
-    return (int)cudaGetLastError();
-}
-
-int proto_max_grid(int device) {
-    cudaDeviceProp prop;
-    if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) return -1;
-    int nb = 0;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, proto_encode_kernel, GT, 0) != cudaSuccess) return -1;
-    return nb * prop.multiProcessorCount;
-}
-
-int grpc_max_grid(int device) {
-    cudaDeviceProp prop;
-    if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) return -1;
-    int nb = 0;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, grpc_hello_kernel, GT, 0) != cudaSuccess) return -1;
-    return nb * prop.multiProcessorCount;
 }
 
 }  // namespace gofr

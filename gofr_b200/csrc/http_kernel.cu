@@ -65,17 +65,4 @@ __global__ void __launch_bounds__(HT, 8) http_parse_kernel(const HttpParams p) {
     }
 }
 
-int launch_http_parse(const HttpParams& p, int grid, void* stream) {
-    http_parse_kernel<<<grid, HT, 0, (cudaStream_t)stream>>>(p);
-    return (int)cudaGetLastError();
-}
-
-int http_max_grid(int device) {
-    cudaDeviceProp prop;
-    if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) return -1;
-    int nb = 0;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, http_parse_kernel, HT, 0) != cudaSuccess) return -1;
-    return nb * prop.multiProcessorCount;
-}
-
 }  // namespace gofr

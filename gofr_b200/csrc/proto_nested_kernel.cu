@@ -20,17 +20,4 @@ __global__ void __launch_bounds__(GT, 6) proto_encode_nested_kernel(const GrpcPa
     frame_tiles(p, PbnCodec{D}, sh);
 }
 
-int launch_proto_encode_nested(const GrpcParams& p, const PbnDesc& D, int grid, void* stream) {
-    proto_encode_nested_kernel<<<grid, GT, 0, (cudaStream_t)stream>>>(p, D);
-    return (int)cudaGetLastError();
-}
-
-int proto_nested_max_grid(int device) {
-    cudaDeviceProp prop;
-    if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) return -1;
-    int nb = 0;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, proto_encode_nested_kernel, GT, 0) != cudaSuccess) return -1;
-    return nb * prop.multiProcessorCount;
-}
-
 }  // namespace gofr

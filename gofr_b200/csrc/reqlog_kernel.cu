@@ -122,17 +122,4 @@ __global__ void __launch_bounds__(LT, 5) reqlog_kernel(const LogParams p) {
     }
 }
 
-int launch_reqlog(const LogParams& p, int grid, void* stream) {
-    reqlog_kernel<<<grid, LT, 0, (cudaStream_t)stream>>>(p);
-    return (int)cudaGetLastError();
-}
-
-int reqlog_max_grid(int device) {
-    cudaDeviceProp prop;
-    if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) return -1;
-    int nb = 0;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, reqlog_kernel, LT, 0) != cudaSuccess) return -1;
-    return nb * prop.multiProcessorCount;
-}
-
 }  // namespace gofr

@@ -13,7 +13,7 @@
 
 namespace gofr {
 
-constexpr int RT = 256;
+constexpr int RT = kRouteThreads;
 
 __global__ void __launch_bounds__(RT) route_kernel(const RouteParams p) {
     extern __shared__ __align__(128) uint8_t smem[];
@@ -37,18 +37,5 @@ __global__ void __launch_bounds__(RT) route_kernel(const RouteParams p) {
     }
 }
 static_assert(kMaxVars == 8, "two 16-byte stores per request");
-
-int launch_route(const RouteParams& p, int sm_count, void* stream) {
-    const uint32_t smem = (p.hot_bytes + 127u) & ~127u;
-    static bool attr_set = false;
-    if (!attr_set) {
-        if (cudaFuncSetAttribute(route_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024) != cudaSuccess) return (int)cudaGetLastError();
-        attr_set = true;
-    }
-    int grid = (int)((p.n + RT - 1) / RT);
-    if (grid > sm_count * 4) grid = sm_count * 4;
-    route_kernel<<<grid, RT, smem, (cudaStream_t)stream>>>(p);
-    return (int)cudaGetLastError();
-}
 
 }  // namespace gofr

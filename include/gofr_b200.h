@@ -554,7 +554,9 @@ int gofr_http_parse_device(gofr_engine*, const uint8_t* d_raw, const uint32_t* d
 
 /* number of kernels launched by this engine so far (bench.py reports it as gpu_launches) */
 uint64_t gofr_engine_launch_count(const gofr_engine*);
-/* duration in ms of the kernels launched since the last reset, measured with CUDA events on the launch stream.
+/* duration in ms of the kernels launched since the last reset, measured with CUDA events on the launch stream.  Every
+ * kernel is timed except the two copy kernels of gofr_batch_submit's pinned-buffer path (chunk bookkeeping and egress
+ * into the caller's buffers, on the engine's own streams).
  * Timing is OFF by default (each timed launch costs two event objects): gofr_engine_set_timing(e, 1) first. */
 int gofr_engine_kernel_time_ms(gofr_engine*, double* total_ms, uint64_t* launches, int reset);
 

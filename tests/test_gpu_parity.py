@@ -204,6 +204,59 @@ def test_shards_concatenate_to_the_unsharded_result(torch_cuda):
     assert np.array_equal(np.concatenate(parts), o1[:int(f1[-1])])
 
 
+def test_lookback_epoch_wrap(torch_cuda, monkeypatch):
+    """An engine created three look-back epochs before the 24-bit epoch wraps (GOFR_DEBUG_EPOCH_START): the wrap falls in
+    the middle of a streamed host-path batch.  The packed serve, the host path, Hello, the flat proto encoder and the request
+    log run across it, twice over, and each matches the oracle."""
+    from tests.test_grpc import _gpu_hello
+    from tests.test_proto import _bulk
+    monkeypatch.setenv("GOFR_DEBUG_EPOCH_START", str((1 << 24) - 4))
+    spec = synth.config2_spec()
+    eng = _engine(spec)
+    frames, foff = synth.config5_frames(3000)
+    fields, msgs = _bulk(2000)
+    rows, roff = S.pack_proto_rows(fields, msgs)
+    lb = synth.reqlog_batch(3000, hostile_every=5, rpc_every=7)
+    for _ in range(2):
+        _check(spec, synth.config2_batch(3000), eng=eng)
+        _check(spec, synth.config2_batch(5000, start=7), eng=eng, host=True, chunk=1000)
+        o1, f1, m1 = O.grpc_hello(frames, foff)
+        o2, f2, m2 = _gpu_hello(frames, foff, eng)
+        assert np.array_equal(m1, m2) and np.array_equal(f1, f2) and np.array_equal(o1[:int(f1[-1])], o2[:int(f1[-1])])
+        out, o, meta = O.proto_encode(fields, rows, roff)
+        d_out, d_off, d_meta = eng.proto_encode_device(fields, rows, roff)
+        assert np.array_equal(d_off.cpu().numpy().view(np.uint32), o)
+        assert np.array_equal(d_meta.cpu().numpy().view(np.uint32), meta)
+        assert d_out[:int(o[-1])].cpu().numpy().tobytes() == out[:int(o[-1])].tobytes()
+        o1, f1 = O.request_log(lb)
+        d_out, d_off = eng.request_log_device(lb)
+        assert np.array_equal(d_off.cpu().numpy().view(np.uint32), f1)
+        assert d_out[:int(f1[-1])].cpu().numpy().tobytes() == o1[:f1[-1]].tobytes()
+        assert not eng.overflowed()
+    eng.close()
+
+
+def test_two_live_engines(torch_cuda):
+    """Two engines alive at once on tables with hot parts of different size.  The one created first stages 256 request
+    bytes per request, so its kernels need more dynamic shared memory than the 48 KB default and than the second engine's.
+    Once the second exists it still serves a slot batch with each slot-layout instance and a packed batch (whose grid the
+    two engines now share)."""
+    from tests import test_slots
+    big, small = synth.config4_spec(), synth.config2_spec()
+    eng = _engine(big)
+    eng.set_tile(256)
+    other = _engine(small)
+    assert eng.geometry()["smem_bytes"] > max(48 * 1024, other.geometry()["smem_bytes"])
+    batch = synth.config4_batch(20000)
+    for force in (4, 5):
+        assert eng.slot_ctas(force) == force
+        test_slots._check(eng, big, batch, 1024)
+    _check(big, batch, eng=eng)
+    _check(small, synth.config2_batch(5000), eng=other)
+    other.close()
+    eng.close()
+
+
 def test_path_params(torch_cuda):
     spec = S.TableSpec(routes=[
         S.Route(S.M_GET, "/users/{id}", S.H_PATHPARAM_FORMAT, s0=b"id", s2=b"user ", s3=b"!"),

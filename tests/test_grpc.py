@@ -107,13 +107,13 @@ def test_emu_random_messages(msgs, mis):
     _cmp(frames, off, emu.grpc_hello, mis)
 
 
-def _gpu_hello(frames, off):
+def _gpu_hello(frames, off, eng=None):
     import ctypes as C
     import torch
     from gofr_b200 import _abi
     from gofr_b200.engine import Engine
     from gofr_b200.table import Table
-    eng = Engine(Table(synth.config1_spec()), 0)
+    eng = eng or Engine(Table(synth.config1_spec()), 0)
     n = len(off) - 1
     cap = int(frames.size) + 40 * n + 64
     d_in = torch.from_numpy(np.concatenate([frames, np.zeros(64, np.uint8)])).cuda()
