@@ -54,11 +54,11 @@ constexpr int kServeCtas = GOFR_SERVE_CTAS;  // serve kernel: CTAs per SM the re
 #endif
 constexpr int kServeCtasWide = GOFR_SERVE_CTAS_WIDE;  // slot layout, "wide" instance: 128 registers per thread (serve_slots_kernel.cu)
 
-// How many response bytes one byte of a request's data section can turn into, at most (ImageHeader::reserved3[0], set at
+// How many response bytes one byte of a request's data section can turn into, at most (ImageHeader::data_expand, set at
 // seal): 6 for flat rows (a control character becomes \u00XX); more when the table has programs of the wider data model,
 // where a 4-byte element of a slice of structs drags its key literals along (`{"a_long_key":true},`).
 template <typename Header>
-inline uint32_t image_data_expand(const Header& H) { return H.reserved3[0] > 6u ? H.reserved3[0] : 6u; }
+inline uint32_t image_data_expand(const Header& H) { return H.data_expand > 6u ? H.data_expand : 6u; }
 
 // table_build.cpp: which slot-layout instance suits the sealed table (engine.cu choose_slot_residency)
 bool image_wants_wide_slots(const uint8_t* image);

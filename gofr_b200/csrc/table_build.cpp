@@ -249,6 +249,8 @@ static uint32_t field_words(const std::vector<SchemaDef>& all, const FieldDef& f
     const uint32_t w = f.kind == GOFR_F_STRUCT ? all[(size_t)f.elem].fixed_words : kind_words(f.kind);
     return w + (f.container == GOFR_C_PTR ? 1u : 0u);
 }
+// words a field of a bindable schema owns in a Bind span row (bind_device.cuh): strings are (offset, length) pairs
+static uint32_t bind_field_words(uint8_t kind) { return (kind == GOFR_F_INT32 || kind == GOFR_F_BOOL) ? 1u : 2u; }
 
 // symbolic op before literal-pool assignment
 struct SOp {
@@ -556,12 +558,12 @@ static SOp value_op(int schema_idx, size_t field_idx, uint16_t word) {
     v.code = OP_VALUE; v.body = true; v.off = word; v.aux = (uint32_t)schema_idx; v.arg = (uint8_t)field_idx;
     return v;
 }
-static void struct_level_ops(Prog& p, const std::vector<SchemaDef>& all, int sidx, bool bind_layout, uint16_t& word,
+static void struct_level_ops(std::vector<SOp>& ops, const std::vector<SchemaDef>& all, int sidx, bool bind_layout, uint16_t& word,
                              uint16_t& str_ord, std::string& acc) {
     const SchemaDef& sc = all[(size_t)sidx];
     if (sc.bare()) {  // the schema IS its one field's type: no braces, no key
-        if (!acc.empty()) { p.ops.push_back(lit(acc, true)); acc.clear(); }
-        p.ops.push_back(value_op(sidx, 0, word));
+        if (!acc.empty()) { ops.push_back(lit(acc, true)); acc.clear(); }
+        ops.push_back(value_op(sidx, 0, word));
         word = (uint16_t)(word + field_words(all, sc.fields[0]));
         return;
     }
@@ -573,9 +575,9 @@ static void struct_level_ops(Prog& p, const std::vector<SchemaDef>& all, int sid
         const FieldDef& f = sc.fields[fi];
         std::string key = "\"" + json_escape_go(f.json_name) + "\":";
         uint16_t w = word;
-        if (bind_layout) {  // span row (bind_device.cuh): 8 header words, strings are (offset, length) pairs
+        if (bind_layout) {  // span row (bind_device.cuh): 8 header words, then the fields
             w = (uint16_t)(8 + word);
-            word += (f.kind == GOFR_F_INT32 || f.kind == GOFR_F_BOOL) ? 1 : 2;
+            word = (uint16_t)(word + bind_field_words(f.kind));
         } else word = (uint16_t)(word + field_words(all, f));
         const bool plain = f.container == GOFR_C_VALUE;
         const bool is_str = plain && f.kind == GOFR_F_STRING;
@@ -596,53 +598,56 @@ static void struct_level_ops(Prog& p, const std::vector<SchemaDef>& all, int sid
             acc += key;
             if (plain && f.kind == GOFR_F_STRUCT && flattenable(all, all[(size_t)f.elem])) {
                 uint16_t sub_word = w;
-                struct_level_ops(p, all, f.elem, false, sub_word, str_ord, acc);
+                struct_level_ops(ops, all, f.elem, false, sub_word, str_ord, acc);
             } else {
                 if (is_str) acc += "\"";
-                p.ops.push_back(lit(acc, true));
-                p.ops.push_back(generic ? value_op(sidx, fi, w) : v);
+                ops.push_back(lit(acc, true));
+                ops.push_back(generic ? value_op(sidx, fi, w) : v);
                 acc = is_str ? "\"" : "";
             }
         } else {
-            if (!acc.empty()) { p.ops.push_back(lit(acc, true)); acc.clear(); }
+            if (!acc.empty()) { ops.push_back(lit(acc, true)); acc.clear(); }
             SOp k;
             k.code = OP_KEY; k.body = true; k.kind = (uint8_t)(f.kind | f.container << 4); k.off = w; k.lit = key;
             k.flags = f.omitempty ? OPF_OMITEMPTY : 0;
             if (is_str) k.lit += "\"";
-            p.ops.push_back(k);
+            ops.push_back(k);
             if (generic) v = value_op(sidx, fi, w);
             v.flags |= OPF_VALUE_OF_KEY;
-            p.ops.push_back(v);
-            if (is_str) { SOp q = lit("\"", true); q.flags |= OPF_VALUE_OF_KEY; p.ops.push_back(q); }
+            ops.push_back(v);
+            if (is_str) { SOp q = lit("\"", true); q.flags |= OPF_VALUE_OF_KEY; ops.push_back(q); }
         }
         first = false;
     }
     acc += "}";
 }
-static void build_struct_ops(Prog& p, const std::vector<SchemaDef>& all, const SchemaDef& sc, bool bind_layout = false,
-                             uint16_t word_base = 0) {
-    uint16_t word = word_base, str_ord = word_base ? 1 : 0;
-    std::string acc;
-    struct_level_ops(p, all, (int)(&sc - all.data()), bind_layout, word, str_ord, acc);
-    p.ops.push_back(lit(acc, true));
+
+// The body of one Write of `len` bytes; `chunked` (see build_header): one chunk, then chunkWriter.close's terminator
+static void add_body(Prog& p, const std::vector<SOp>& body_ops, bool chunked, size_t len) {
+    if (chunked) {
+        char hx[32];
+        snprintf(hx, sizeof hx, "%zx\r\n", len);
+        p.ops.push_back(lit(hx, true));
+    }
+    for (auto o : body_ops) { o.body = true; p.ops.push_back(o); }
+    if (chunked) p.ops.push_back(lit("\r\n0\r\n\r\n", true));
 }
 
 struct Builder {
-    gofr_table* t;
+    const gofr_table& t;
     std::vector<Prog> progs;
-    std::string err;
-
     std::map<std::string, int> prog_ids;
-    // identical programs (e.g. sixteen routes returning the same struct type) are stored once
+    // identical programs (e.g. sixteen routes returning the same struct type) are stored once.  Program indices follow the
+    // order of add calls.
     int add(Prog p) {
         // a program that can meet a NaN / Inf float gets a companion for "json.Encoder.Encode failed": same status and
-        // headers, no body bytes (ProgRec::encfail)
+        // headers, no body bytes (ProgRec::encfail).  The companion is added first, so its index is the lower one.
         bool may_fail = false;
         for (auto& o : p.ops) may_fail |= o.code == OP_F64 || o.code == OP_VALUE;
         if (may_fail && p.encfail < 0) {
             Prog q;
             q.status = p.status;
-            build_header(q, t->frame_mode, p.status, true, BODY_JSON_FAILED, false, "", "", false);
+            build_header(q, t.frame_mode, p.status, true, BODY_JSON_FAILED, false, "", "", false);
             p.encfail = add(std::move(q));
         }
         std::string sig = std::to_string(p.status) + (p.bind ? "B" : "R") + std::to_string(p.row_words);
@@ -660,26 +665,38 @@ struct Builder {
     }
 
     // Responder.Respond envelope: {"error":{"message":...},"data":...}\n  (error first; both omitempty)
-    int json_prog(int status, const std::vector<SOp>& body_ops, bool bind = false) {
+    int json_prog(int status, const std::vector<SOp>& body_ops, bool bind = false, int row_words = 0) {
         Prog p;
         p.status = status;
         p.bind = bind;
+        p.row_words = row_words;
         // a body that is all literals has its length now: beyond net/http's 2 KiB buffer the one Write of Encoder.Encode makes the
         // response chunked (see build_header) — decided here for static bodies; bodies whose length depends on the request keep
         // Content-Length whatever their size (DESIGN.md §8, a stated deviation)
         size_t static_len = 0;
         bool all_static = true;
         for (auto& o : body_ops) { all_static &= o.code == OP_LIT && !(o.flags & OPF_VALUE_OF_KEY); static_len += o.lit.size(); }
-        const bool chunked = all_static && t->frame_mode == GOFR_FRAME_WIRE && static_len > 2048;
-        build_header(p, t->frame_mode, status, true, BODY_JSON, false, "", "", false, chunked);
-        if (chunked) {
-            char hx[32];
-            snprintf(hx, sizeof hx, "%zx\r\n", static_len);
-            p.ops.push_back(lit(hx, true));
-        }
-        for (auto o : body_ops) { o.body = true; p.ops.push_back(o); }
-        if (chunked) p.ops.push_back(lit("\r\n0\r\n\r\n", true));
+        const bool chunked = all_static && t.frame_mode == GOFR_FRAME_WIRE && static_len > 2048;
+        build_header(p, t.frame_mode, status, true, BODY_JSON, false, "", "", false, chunked);
+        add_body(p, body_ops, chunked, static_len);
         return add(std::move(p));
+    }
+
+    // a string the host closure produced, between two literals: row word 0 is its length, the bytes follow
+    int str_prog(int status, const std::string& open, const std::string& close) {
+        return json_prog(status, {lit(open, true), op(OP_STR, true), lit(close, true)}, false, 1);
+    }
+
+    // a struct of schema `sc` after the ops `open`, then `close`.  word_base: row words before the struct's own (they then
+    // fix the row's size, whatever the route's schema)
+    int struct_prog(int status, std::vector<SOp> open, const SchemaDef& sc, const std::string& close, bool bind = false,
+                    uint16_t word_base = 0) {
+        uint16_t word = word_base, str_ord = word_base ? 1 : 0;
+        std::string acc;
+        struct_level_ops(open, t.schemas, (int)(&sc - t.schemas.data()), bind, word, str_ord, acc);
+        open.push_back(lit(acc, true));
+        open.push_back(lit(close, true));
+        return json_prog(status, open, bind, word_base ? (int)(word_base + sc.fixed_words) : 0);
     }
 };
 
@@ -714,7 +731,7 @@ bool image_wants_wide_slots(const uint8_t* img) {
     return shape >= 0;
 }
 
-
+// The literal pool: offsets follow the order of put / put16 calls, and equal literals are stored once.
 struct Pool {
     std::vector<uint8_t>& img;
     std::map<std::string, uint32_t> seen;
@@ -793,7 +810,7 @@ static const char* go_kind_name(uint8_t k) {
         case GOFR_F_INT32: return "int32";
         case GOFR_F_BOOL: return "bool";
         case GOFR_F_STRING: return "string";
-        case 5: return "int";
+        case GOFR_F_INT: return "int";
         case GOFR_F_FLOAT64: return "float64";
         case GOFR_F_STRUCT: return "struct";
         case GOFR_F_UINT64: return "uint64";
@@ -810,230 +827,153 @@ static std::string fold_lower(const std::string& s) {
     return r;
 }
 
-int seal_table(gofr_table* t) {
-    Builder b{t, {}, {}};
-    uint32_t fm = t->frame_mode;
+// the schema of a GOFR_H_ROW / BIND_ECHO / RESULT route; nullptr for other kinds and unknown ids
+static const SchemaDef* route_schema(const gofr_table& t, const RouteDef& r) {
+    if (r.hkind != GOFR_H_ROW && r.hkind != GOFR_H_BIND_ECHO && r.hkind != GOFR_H_RESULT) return nullptr;
+    for (auto& s : t.schemas) if (s.id == r.schema_id) return &s;
+    return nullptr;
+}
 
-    // ---- fixed programs (mux / middleware outcomes that exist for every table) ----
-    auto simple = [&](int status, bool with_mw, BodyKind bk, bool head_no_body, bool location, const std::string& body) {
+// What seal refuses in a route; every route is checked before any program is built.
+static int check_route(const gofr_table& t, const RouteDef& r) {
+    if (r.hkind > GOFR_H_RESULT) {
+        set_last_error("route %s: unknown handler kind %u", r.pattern.c_str(), r.hkind);
+        return GOFR_ERR_INVALID;
+    }
+    const SchemaDef* sc = route_schema(t, r);
+    // a closure that only ever returns strings / errors / nil needs no struct schema
+    if (!sc && (r.hkind == GOFR_H_ROW || r.hkind == GOFR_H_BIND_ECHO || (r.hkind == GOFR_H_RESULT && r.schema_id != 0))) {
+        set_last_error("route %s: unknown schema %u", r.pattern.c_str(), r.schema_id);
+        return GOFR_ERR_INVALID;
+    }
+    if (sc && r.hkind == GOFR_H_BIND_ECHO && !sc->bindable) {
+        set_last_error("route %s: Bind takes flat structs of int / float64 / bool / string fields only (schema %u)", r.pattern.c_str(), r.schema_id);
+        return GOFR_ERR_UNSUPPORTED;
+    }
+    if ((r.hkind == GOFR_H_PARAM_FORMAT || r.hkind == GOFR_H_PATHPARAM_FORMAT) && (!valid_utf8(r.s[2]) || !valid_utf8(r.s[3]))) {
+        set_last_error("route %s: format prefix/suffix must be valid UTF-8", r.pattern.c_str());
+        return GOFR_ERR_UNSUPPORTED;
+    }
+    return GOFR_OK;
+}
+
+// The programs every table has: what mux and the middleware answer before a handler runs.
+static void add_fixed_progs(Builder& b, ImageHeader& H) {
+    auto fixed = [&](int status, bool with_mw, BodyKind bk, bool head_no_body, bool location, const std::string& body) {
         Prog p;
         p.status = status;
-        build_header(p, fm, status, with_mw, bk, head_no_body, "", "", location);
+        build_header(p, b.t.frame_mode, status, with_mw, bk, head_no_body, "", "", location);
         if (!body.empty()) p.ops.push_back(lit(body, true));
-        return b.add(std::move(p));
+        return (uint16_t)b.add(std::move(p));
     };
-    int p301 = simple(301, false, BODY_NONE, false, true, "");
-    int p301h = simple(301, false, BODY_NONE, true, true, "");
-    int p404 = simple(404, false, BODY_PLAIN404, false, false, "404 page not found\n");  // http.NotFoundHandler
-    int p405 = simple(405, false, BODY_NONE, false, false, "");                           // mux methodNotAllowedHandler
-    int p405h = simple(405, false, BODY_NONE, true, false, "");
-    int popt = simple(200, true, BODY_NONE, false, false, "");                            // CORS short-circuit
-    int ppanic = simple(500, true, BODY_PANIC, false, false,
-                        "{\"code\":500,\"message\":\"Some unexpected error has occurred\",\"status\":\"ERROR\"}\n");
+    H.prog_301 = fixed(301, false, BODY_NONE, false, true, "");
+    H.prog_301_head = fixed(301, false, BODY_NONE, true, true, "");
+    H.prog_404 = fixed(404, false, BODY_PLAIN404, false, false, "404 page not found\n");  // http.NotFoundHandler
+    H.prog_405 = fixed(405, false, BODY_NONE, false, false, "");                           // mux methodNotAllowedHandler
+    H.prog_405_head = fixed(405, false, BODY_NONE, true, false, "");
+    H.prog_options = fixed(200, true, BODY_NONE, false, false, "");                        // CORS short-circuit
+    H.prog_panic = fixed(500, true, BODY_PANIC, false, false,
+                         "{\"code\":500,\"message\":\"Some unexpected error has occurred\",\"status\":\"ERROR\"}\n");
+}
 
-    // ---- per-route programs ----
-    std::vector<int> prog_ok(t->routes.size(), 0xFFFF), prog_err(t->routes.size(), 0xFFFF);
-    std::vector<int> prog_err404(t->routes.size(), 0xFFFF), prog_nil(t->routes.size(), 0xFFFF), prog_both(t->routes.size(), 0xFFFF),
-        prog_str(t->routes.size(), 0xFFFF);
-    std::vector<uint16_t> rawprogs(t->routes.size() * 9, 0xFFFF);  // response.Raw outcomes of GOFR_H_RESULT routes
-    for (size_t ri = 0; ri < t->routes.size(); ri++) {
-        RouteDef& r = t->routes[ri];
-        const SchemaDef* sc = nullptr;
-        if (r.hkind == GOFR_H_ROW || r.hkind == GOFR_H_BIND_ECHO || r.hkind == GOFR_H_RESULT) {
-            for (auto& s : t->schemas) if (s.id == r.schema_id) sc = &s;
-            // a closure that only ever returns strings / errors / nil needs no struct schema
-            if (!sc && !(r.hkind == GOFR_H_RESULT && r.schema_id == 0)) { set_last_error("route %s: unknown schema %u", r.pattern.c_str(), r.schema_id); return GOFR_ERR_INVALID; }
-            if (sc && r.hkind == GOFR_H_BIND_ECHO && !sc->bindable) {
-                set_last_error("route %s: Bind takes flat structs of int / float64 / bool / string fields only (schema %u)", r.pattern.c_str(), r.schema_id);
-                return GOFR_ERR_UNSUPPORTED;
-            }
+struct RouteProgs {  // the programs of a route's outcomes, 0xFFFF: none
+    uint16_t ok = 0xFFFF, err = 0xFFFF;                                   // RouteRec::prog_ok, prog_err
+    uint16_t nil = 0xFFFF, err404 = 0xFFFF, both = 0xFFFF, str = 0xFFFF;  // GOFR_H_RESULT: the other outcomes
+    uint16_t raw[9] = {0xFFFF, 0xFFFF, 0xFFFF, 0xFFFF, 0xFFFF, 0xFFFF, 0xFFFF, 0xFFFF, 0xFFFF};  // GOFR_H_RESULT: response.Raw (rawprog_off)
+};
+
+// A route's programs (the route passed check_route), added in the order the image numbers them.
+static RouteProgs add_route_progs(Builder& b, const RouteDef& r, uint16_t panic) {
+    const std::string data = "{\"data\":", error = "{\"error\":{\"message\":\"";
+    const SchemaDef* sc = route_schema(b.t, r);
+    RouteProgs rp;
+    switch (r.hkind) {
+        case GOFR_H_HOST: break;
+        case GOFR_H_STATIC_STRING: rp.ok = b.json_prog(200, {lit("{\"data\":\"" + json_escape_go(r.s[0]) + "\"}\n", true)}); break;
+        case GOFR_H_STATIC_ERROR: rp.ok = b.json_prog(500, {lit(error + json_escape_go(r.s[0]) + "\"}}\n", true)}); break;
+        case GOFR_H_NIL: rp.ok = b.json_prog(200, {lit("{}\n", true)}); break;
+        case GOFR_H_HEALTH: rp.ok = b.json_prog(200, {lit("{\"data\":{}}\n", true)}); break;
+        case GOFR_H_MISSING_FILE: rp.ok = b.json_prog(404, {lit(error + "http: no such file\"}}\n", true)}); break;
+        case GOFR_H_PANIC: rp.ok = panic; break;
+        case GOFR_H_PATHPARAM_FORMAT:
+        case GOFR_H_PARAM_FORMAT:
+            rp.ok = b.json_prog(200, {lit("{\"data\":\"" + json_escape_go(r.s[2]), true), op(OP_PARAM, true),
+                                      lit(json_escape_go(r.s[3]) + "\"}\n", true)});
+            break;
+        case GOFR_H_ROW:
+        case GOFR_H_BIND_ECHO: {
+            const bool bind = r.hkind == GOFR_H_BIND_ECHO;
+            rp.ok = b.struct_prog(200, {lit(data, true)}, *sc, "}\n", bind);
+            if (bind) rp.err = b.json_prog(500, {lit(error, true), op(OP_ERRMSG, true), lit("\"}}\n", true)}, true);
+            break;
         }
-        switch (r.hkind) {
-            case GOFR_H_HOST: break;
-            case GOFR_H_STATIC_STRING:
-                prog_ok[ri] = b.json_prog(200, {lit("{\"data\":\"" + json_escape_go(r.s[0]) + "\"}\n", true)});
-                break;
-            case GOFR_H_STATIC_ERROR:
-                prog_ok[ri] = b.json_prog(500, {lit("{\"error\":{\"message\":\"" + json_escape_go(r.s[0]) + "\"}}\n", true)});
-                break;
-            case GOFR_H_NIL: prog_ok[ri] = b.json_prog(200, {lit("{}\n", true)}); break;
-            case GOFR_H_HEALTH: prog_ok[ri] = b.json_prog(200, {lit("{\"data\":{}}\n", true)}); break;
-            case GOFR_H_MISSING_FILE:
-                prog_ok[ri] = b.json_prog(404, {lit("{\"error\":{\"message\":\"http: no such file\"}}\n", true)});
-                break;
-            case GOFR_H_PANIC: prog_ok[ri] = ppanic; break;
-            case GOFR_H_PATHPARAM_FORMAT:
-            case GOFR_H_PARAM_FORMAT: {
-                if (!valid_utf8(r.s[2]) || !valid_utf8(r.s[3])) {
-                    set_last_error("route %s: format prefix/suffix must be valid UTF-8", r.pattern.c_str());
-                    return GOFR_ERR_UNSUPPORTED;
-                }
-                prog_ok[ri] = b.json_prog(200, {lit("{\"data\":\"" + json_escape_go(r.s[2]), true), op(OP_PARAM, true),
-                                                lit(json_escape_go(r.s[3]) + "\"}\n", true)});
-                break;
+        case GOFR_H_RESULT:
+            // Responder.Respond on a (data, err) the host closure produced (responder.go:19-62)
+            if (sc) rp.ok = b.struct_prog(200, {lit(data, true)}, *sc, "}\n");
+            rp.str = b.str_prog(200, "{\"data\":\"", "\"}\n");  // data is a string (encoding/json string escaping)
+            rp.err = b.str_prog(500, error, "\"}}\n");
+            rp.err404 = b.str_prog(404, error, "\"}}\n");      // errors.Is(err, http.ErrMissingFile)
+            rp.nil = b.json_prog(200, {lit("{}\n", true)});
+            // response.Raw{Data: …}: the data encoded bare (responder.go:24-26); the error only picks the status
+            for (int es = 0; es < 3; es++) {
+                const int status = es == 0 ? 200 : es == 1 ? 500 : 404;
+                if (sc) rp.raw[es] = b.struct_prog(status, {}, *sc, "\n");
+                rp.raw[3 + es] = b.str_prog(status, "\"", "\"\n");
+                rp.raw[6 + es] = b.json_prog(status, {lit("null\n", true)});
             }
-            case GOFR_H_ROW:
-            case GOFR_H_BIND_ECHO: {
-                Prog p;
-                p.status = 200;
-                build_header(p, fm, 200, true, BODY_JSON, false, "", "", false);
-                p.ops.push_back(lit("{\"data\":", true));
-                build_struct_ops(p, t->schemas, *sc, r.hkind == GOFR_H_BIND_ECHO);
-                p.ops.push_back(lit("}\n", true));
-                p.bind = r.hkind == GOFR_H_BIND_ECHO;
-                prog_ok[ri] = b.add(std::move(p));
-                if (r.hkind == GOFR_H_BIND_ECHO)
-                    prog_err[ri] = b.json_prog(500, {lit("{\"error\":{\"message\":\"", true), op(OP_ERRMSG, true),
-                                                     lit("\"}}\n", true)}, true);
-                break;
+            // (data, err) both non-nil: response{Error, Data} with both members (responder.go:59-62)
+            if (sc) rp.both = b.struct_prog(500, {lit(error, true), op(OP_STR, true), lit("\"},\"data\":", true)}, *sc, "}\n", false, 1);
+            break;
+        case GOFR_H_FILE: {
+            const uint32_t fm = b.t.frame_mode;
+            Prog p;
+            p.status = 200;
+            if (r.blob.empty()) {
+                // Write(nil) after WriteHeader: empty body → "Content-Length: 0" and nothing to sniff; the
+                // recorder's live map (INTENDED) still shows the type the handler set.
+                build_header(p, fm, 200, true, fm == GOFR_FRAME_INTENDED ? BODY_FILE : BODY_NONE, false, r.s[0], "", false);
+            } else {
+                // w.Write(v.Content) is one Write: beyond net/http's 2 KiB buffer the response is chunked on the wire
+                // (the reference's own favicon, 13 149 bytes, is) — one chunk, then chunkWriter.close's terminator.
+                // (A HEAD request would get neither Content-Length nor Transfer-Encoding there; GoFr registers
+                // GET / PUT / POST / DELETE only, so no File route ever sees one.)
+                const bool chunked = fm == GOFR_FRAME_WIRE && r.blob.size() > 2048;
+                build_header(p, fm, 200, true, BODY_FILE, false, r.s[0], sniff_content_type(r.blob), false, chunked);
+                SOp bo = op(OP_BLOB, true);
+                bo.lit = r.blob;
+                add_body(p, {bo}, chunked, r.blob.size());
             }
-            case GOFR_H_RESULT: {
-                // Responder.Respond on a (data, err) the host closure produced (responder.go:19-62)
-                if (sc) {
-                    Prog p;
-                    p.status = 200;
-                    build_header(p, fm, 200, true, BODY_JSON, false, "", "", false);
-                    p.ops.push_back(lit("{\"data\":", true));
-                    build_struct_ops(p, t->schemas, *sc, false);
-                    p.ops.push_back(lit("}\n", true));
-                    prog_ok[ri] = b.add(std::move(p));
-                }
-                {   // data is a string: {"data":"…"} (encoding/json string escaping, as for struct fields)
-                    Prog p;
-                    p.status = 200;
-                    build_header(p, fm, 200, true, BODY_JSON, false, "", "", false);
-                    p.ops.push_back(lit("{\"data\":\"", true));
-                    SOp m = op(OP_STR, true);
-                    m.off = 0;  // row word 0 = len, the bytes follow
-                    p.ops.push_back(m);
-                    p.ops.push_back(lit("\"}\n", true));
-                    p.row_words = 1;
-                    prog_str[ri] = b.add(std::move(p));
-                }
-                for (int which = 0; which < 2; which++) {  // 500, and 404 for errors.Is(err, http.ErrMissingFile)
-                    Prog e;
-                    e.status = which ? 404 : 500;
-                    build_header(e, fm, e.status, true, BODY_JSON, false, "", "", false);
-                    e.ops.push_back(lit("{\"error\":{\"message\":\"", true));
-                    SOp m = op(OP_STR, true);
-                    m.off = 0;  // row word 0 = len(err.Error()), the bytes follow
-                    e.ops.push_back(m);
-                    e.ops.push_back(lit("\"}}\n", true));
-                    e.row_words = 1;
-                    (which ? prog_err404 : prog_err)[ri] = b.add(std::move(e));
-                }
-                prog_nil[ri] = b.json_prog(200, {lit("{}\n", true)});
-                // response.Raw{Data: …}: the data encoded bare (responder.go:24-26); the error only picks the status
-                for (int es = 0; es < 3; es++) {
-                    const int status = es == 0 ? 200 : es == 1 ? 500 : 404;
-                    if (sc) {
-                        Prog p;
-                        p.status = status;
-                        build_header(p, fm, status, true, BODY_JSON, false, "", "", false);
-                        build_struct_ops(p, t->schemas, *sc, false);
-                        p.ops.push_back(lit("\n", true));
-                        rawprogs[ri * 9 + 0 + es] = (uint16_t)b.add(std::move(p));
-                    }
-                    {
-                        Prog p;
-                        p.status = status;
-                        build_header(p, fm, status, true, BODY_JSON, false, "", "", false);
-                        p.ops.push_back(lit("\"", true));
-                        SOp m = op(OP_STR, true);
-                        m.off = 0;
-                        p.ops.push_back(m);
-                        p.ops.push_back(lit("\"\n", true));
-                        p.row_words = 1;
-                        rawprogs[ri * 9 + 3 + es] = (uint16_t)b.add(std::move(p));
-                    }
-                    rawprogs[ri * 9 + 6 + es] = (uint16_t)b.json_prog(status, {lit("null\n", true)});
-                }
-                if (sc) {  // (data, err) both non-nil: response{Error, Data} with both members (responder.go:59-62)
-                    Prog e;
-                    e.status = 500;
-                    build_header(e, fm, 500, true, BODY_JSON, false, "", "", false);
-                    e.ops.push_back(lit("{\"error\":{\"message\":\"", true));
-                    SOp m = op(OP_STR, true);
-                    m.off = 0;
-                    e.ops.push_back(m);
-                    e.ops.push_back(lit("\"},\"data\":", true));
-                    build_struct_ops(e, t->schemas, *sc, false, 1);
-                    e.ops.push_back(lit("}\n", true));
-                    e.row_words = (int)(1 + sc->fixed_words);
-                    prog_both[ri] = b.add(std::move(e));
-                }
-                break;
-            }
-            case GOFR_H_FILE: {
-                Prog p;
-                p.status = 200;
-                if (r.blob.empty()) {
-                    // Write(nil) after WriteHeader: empty body → "Content-Length: 0" and nothing to sniff; the
-                    // recorder's live map (INTENDED) still shows the type the handler set.
-                    build_header(p, fm, 200, true, fm == GOFR_FRAME_INTENDED ? BODY_FILE : BODY_NONE, false, r.s[0], "", false);
-                } else {
-                    // w.Write(v.Content) is one Write: beyond net/http's 2 KiB buffer the response is chunked on the wire
-                    // (the reference's own favicon, 13 149 bytes, is) — one chunk, then chunkWriter.close's terminator.
-                    // (A HEAD request would get neither Content-Length nor Transfer-Encoding there; GoFr registers
-                    // GET / PUT / POST / DELETE only, so no File route ever sees one.)
-                    const bool chunked = fm == GOFR_FRAME_WIRE && r.blob.size() > 2048;
-                    build_header(p, fm, 200, true, BODY_FILE, false, r.s[0], sniff_content_type(r.blob), false, chunked);
-                    if (chunked) {
-                        char hx[32];
-                        snprintf(hx, sizeof hx, "%zx\r\n", r.blob.size());
-                        p.ops.push_back(lit(hx, true));
-                    }
-                    SOp bo = op(OP_BLOB, true);
-                    bo.lit = r.blob;
-                    p.ops.push_back(bo);
-                    if (chunked) p.ops.push_back(lit("\r\n0\r\n\r\n", true));
-                }
-                prog_ok[ri] = b.add(std::move(p));
-                break;
-            }
-            default: set_last_error("route %s: unknown handler kind %u", r.pattern.c_str(), r.hkind); return GOFR_ERR_INVALID;
+            rp.ok = b.add(std::move(p));
+            break;
         }
     }
+    return rp;
+}
 
-    // ---- lay out the image ----
-    std::vector<uint8_t>& img = t->image;
-    img.clear();
-    img.resize(sizeof(ImageHeader), 0);
-    ImageHeader H;
-    memset(&H, 0, sizeof H);
-    H.magic = kMagic; H.version = kImageVersion; H.frame_mode = fm;
-    H.n_routes = (uint32_t)t->routes.size();
-    H.prog_301 = (uint16_t)p301; H.prog_301_head = (uint16_t)p301h; H.prog_404 = (uint16_t)p404; H.prog_405 = (uint16_t)p405;
-    H.prog_405_head = (uint16_t)p405h; H.prog_options = (uint16_t)popt; H.prog_panic = (uint16_t)ppanic;
-    H.has_catchall = t->has_catchall;
+struct RouteRecords { std::vector<RouteRec> routes; std::vector<PieceRec> pieces; };
 
-    auto align16 = [&]() { while (img.size() % 16) img.push_back(0); };
-    std::vector<RouteRec> routes(t->routes.size());
-    std::vector<PieceRec> pieces;
-    // We build sections into separate byte vectors, then concatenate.
-    std::vector<uint8_t> lits;
-    Pool pool(lits);
-    std::vector<uint8_t> cold;
-
-    for (size_t ri = 0; ri < t->routes.size(); ri++) {
-        RouteDef& r = t->routes[ri];
-        RouteRec& R = routes[ri];
-        memset(&R, 0, sizeof R);
+// RouteRec and PieceRec of every route.  Route by route, the pattern, piece and key / default literals go to the pool.
+static RouteRecords route_records(const gofr_table& t, const std::vector<RouteProgs>& route_progs, Pool& pool) {
+    RouteRecords rr;
+    rr.routes.resize(t.routes.size());
+    for (size_t ri = 0; ri < t.routes.size(); ri++) {
+        const RouteDef& r = t.routes[ri];
+        const RouteProgs& rp = route_progs[ri];
+        RouteRec& R = rr.routes[ri];
         R.method = (uint8_t)r.method;
         R.flags = (r.prefix ? RF_PREFIX : 0) | (r.dead ? RF_DEAD : 0) | (r.is_default ? RF_DEFAULT : 0);
         R.hkind = (uint8_t)r.hkind;
-        R.first_piece = (uint16_t)pieces.size();
+        R.first_piece = (uint16_t)rr.pieces.size();
         R.n_pieces = (uint8_t)r.pieces.size();
-        R.prog_ok = (uint16_t)prog_ok[ri];
-        R.prog_err = (uint16_t)prog_err[ri];
+        R.prog_ok = rp.ok;
+        R.prog_err = rp.err;
         if (!r.dead && !r.prefix && r.pieces.size() == 1 && !r.pieces[0].has_var) {
             R.flags |= RF_LITERAL;
             R.lit_off = pool.put(r.pattern);
             R.lit_len = (uint16_t)r.pattern.size();
         }
         for (auto& pc : r.pieces) {
-            PieceRec P;
-            memset(&P, 0, sizeof P);
+            PieceRec P{};
             P.lit_off = pool.put(pc.lit);
             P.lit_len = (uint16_t)pc.lit.size();
             P.has_var = pc.has_var;
@@ -1042,7 +982,7 @@ int seal_table(gofr_table* t) {
             P.var_idx = (uint8_t)pc.var_idx;
             P.var_flags = (uint8_t)((pc.var_first ? PV_FIRST : 0) | (pc.var_last ? PV_LAST : 0));
             memcpy(P.cls, pc.cls, sizeof P.cls);
-            pieces.push_back(P);
+            rr.pieces.push_back(P);
         }
         if (r.hkind == GOFR_H_PATHPARAM_FORMAT) {
             // mux.Vars(r)[s0]: resolved to the index of the variable; an unknown name always yields ""
@@ -1060,78 +1000,97 @@ int seal_table(gofr_table* t) {
             R.def_len = (uint16_t)d.size();
         }
         if (r.hkind == GOFR_H_RESULT) {  // the two spare 16-bit fields carry the other outcomes' programs
-            R.key_len = (uint16_t)prog_nil[ri];
-            R.def_len = (uint16_t)prog_err404[ri];
-            R.key_off = (uint32_t)prog_both[ri] | (uint32_t)prog_str[ri] << 16;
+            R.key_len = rp.nil;
+            R.def_len = rp.err404;
+            R.key_off = (uint32_t)rp.both | (uint32_t)rp.str << 16;
         }
-        if (r.hkind == GOFR_H_ROW || r.hkind == GOFR_H_BIND_ECHO || r.hkind == GOFR_H_RESULT)
-            for (size_t si = 0; si < t->schemas.size(); si++)
-                if (t->schemas[si].id == r.schema_id) R.schema = (uint16_t)si;
+        if (const SchemaDef* sc = route_schema(t, r)) R.schema = (uint16_t)(sc - t.schemas.data());
     }
+    return rr;
+}
 
-    // ---- literal-route dispatch structures ----
+struct Dispatch {  // how the kernels find the route of a path (ImageHeader hash_off .. last_method_off)
+    uint32_t hash_bits = 4, thash_bits = 4;
+    std::vector<uint16_t> hash, thash, tmpl, last_method;
+    std::vector<uint32_t> tmpl_keys;
+};
+
+// The literal-route hash, the keyed-template hash, the list of the other templates with their keys and the last route of
+// each method.  The routes of a hash bucket are chained through RouteRec::next_lit in registration order.
+static Dispatch dispatch_tables(const gofr_table& t, std::vector<RouteRec>& routes) {
+    Dispatch d;
     uint32_t n_lit = 0;
     for (auto& R : routes) n_lit += (R.flags & RF_LITERAL) ? 1 : 0;
-    uint32_t hash_bits = 4;
-    while ((1u << hash_bits) < 4 * n_lit && hash_bits < 11) hash_bits++;
-    std::vector<uint16_t> hash_tab(1u << hash_bits, 0xFFFF), tmpl_list, last_method(16, 0);
+    while ((1u << d.hash_bits) < 4 * n_lit && d.hash_bits < 11) d.hash_bits++;
+    d.hash.assign(1u << d.hash_bits, 0xFFFF);
+    d.last_method.assign(16, 0);
     // templates whose leading literal has at least 8 bytes are keyed by those bytes
     uint32_t n_keyed = 0;
     for (size_t ri = 0; ri < routes.size(); ri++)
-        if (!(routes[ri].flags & (RF_DEAD | RF_LITERAL)) && !t->routes[ri].pieces.empty() && t->routes[ri].pieces[0].lit.size() >= 8) n_keyed++;
-    uint32_t thash_bits = 4;
-    while ((1u << thash_bits) < 4 * n_keyed && thash_bits < 11) thash_bits++;
-    std::vector<uint16_t> thash_tab(1u << thash_bits, 0xFFFF);
-    {
-        std::vector<uint16_t> tail(1u << hash_bits, 0xFFFF), ttail(1u << thash_bits, 0xFFFF);
-        for (size_t ri = 0; ri < routes.size(); ri++) {
-            RouteRec& R = routes[ri];
-            R.next_lit = 0xFFFF;
-            if (R.flags & RF_DEAD) continue;
-            if (R.method < 16) last_method[R.method] = (uint16_t)(ri + 1);
-            if (!(R.flags & RF_LITERAL)) {
-                const std::string& l0 = t->routes[ri].pieces.empty() ? std::string() : t->routes[ri].pieces[0].lit;
-                if (l0.size() < 8) { tmpl_list.push_back((uint16_t)ri); continue; }
-                uint32_t w0 = 0, w1 = 0;
-                for (int k = 0; k < 4; k++) { w0 |= (uint32_t)(uint8_t)l0[k] << (8 * k); w1 |= (uint32_t)(uint8_t)l0[4 + k] << (8 * k); }
-                uint32_t slot = path_hash_step(path_hash_step(8u, w0), w1) >> (32 - thash_bits);
-                if (ttail[slot] == 0xFFFF) thash_tab[slot] = (uint16_t)ri; else routes[ttail[slot]].next_lit = (uint16_t)ri;
-                ttail[slot] = (uint16_t)ri;
-                continue;
-            }
-            const std::string& pat = t->routes[ri].pattern;
-            uint32_t h = (uint32_t)pat.size();
-            for (size_t i = 0; i < pat.size(); i += 4) {
-                uint32_t w = 0;
-                for (size_t k = 0; k < 4 && i + k < pat.size(); k++) w |= (uint32_t)(uint8_t)pat[i + k] << (8 * k);
-                h = path_hash_step(h, w);
-            }
-            uint32_t slot = h >> (32 - hash_bits);
-            if (tail[slot] == 0xFFFF) hash_tab[slot] = (uint16_t)ri; else routes[tail[slot]].next_lit = (uint16_t)ri;
-            tail[slot] = (uint16_t)ri;
+        if (!(routes[ri].flags & (RF_DEAD | RF_LITERAL)) && !t.routes[ri].pieces.empty() && t.routes[ri].pieces[0].lit.size() >= 8) n_keyed++;
+    while ((1u << d.thash_bits) < 4 * n_keyed && d.thash_bits < 11) d.thash_bits++;
+    d.thash.assign(1u << d.thash_bits, 0xFFFF);
+    std::vector<uint16_t> tail(1u << d.hash_bits, 0xFFFF), ttail(1u << d.thash_bits, 0xFFFF);
+    for (size_t ri = 0; ri < routes.size(); ri++) {
+        RouteRec& R = routes[ri];
+        R.next_lit = 0xFFFF;
+        if (R.flags & RF_DEAD) continue;
+        if (R.method < 16) d.last_method[R.method] = (uint16_t)(ri + 1);
+        if (!(R.flags & RF_LITERAL)) {
+            const std::string& l0 = t.routes[ri].pieces.empty() ? std::string() : t.routes[ri].pieces[0].lit;
+            if (l0.size() < 8) { d.tmpl.push_back((uint16_t)ri); continue; }
+            uint32_t w0 = 0, w1 = 0;
+            for (int k = 0; k < 4; k++) { w0 |= (uint32_t)(uint8_t)l0[k] << (8 * k); w1 |= (uint32_t)(uint8_t)l0[4 + k] << (8 * k); }
+            uint32_t slot = path_hash_step(path_hash_step(8u, w0), w1) >> (32 - d.thash_bits);
+            if (ttail[slot] == 0xFFFF) d.thash[slot] = (uint16_t)ri; else routes[ttail[slot]].next_lit = (uint16_t)ri;
+            ttail[slot] = (uint16_t)ri;
+            continue;
         }
+        const std::string& pat = t.routes[ri].pattern;
+        uint32_t h = (uint32_t)pat.size();
+        for (size_t i = 0; i < pat.size(); i += 4) {
+            uint32_t w = 0;
+            for (size_t k = 0; k < 4 && i + k < pat.size(); k++) w |= (uint32_t)(uint8_t)pat[i + k] << (8 * k);
+            h = path_hash_step(h, w);
+        }
+        uint32_t slot = h >> (32 - d.hash_bits);
+        if (tail[slot] == 0xFFFF) d.hash[slot] = (uint16_t)ri; else routes[tail[slot]].next_lit = (uint16_t)ri;
+        tail[slot] = (uint16_t)ri;
     }
+    d.tmpl_keys.assign(std::max<size_t>(d.tmpl.size(), 1) * 4, 0u);
+    for (size_t ti = 0; ti < d.tmpl.size(); ti++) {
+        const RouteDef& r = t.routes[d.tmpl[ti]];
+        const std::string& l0 = r.pieces.empty() ? std::string() : r.pieces[0].lit;
+        uint8_t kb[8] = {0}, mb[8] = {0};
+        for (size_t k = 0; k < l0.size() && k < 8; k++) { kb[k] = (uint8_t)l0[k]; mb[k] = 0xFF; }
+        memcpy(&d.tmpl_keys[ti * 4], kb, 8);
+        memcpy(&d.tmpl_keys[ti * 4 + 2], mb, 8);
+    }
+    return d;
+}
 
-    std::vector<ProgRec> progs(b.progs.size());
-    std::vector<Op> ops;
-    std::vector<uint32_t> fixups;
-    uint32_t max_fixed = 0;
-    for (size_t pi = 0; pi < b.progs.size(); pi++) {
-        Prog& p = b.progs[pi];
+// Lowers every program's symbolic ops to Op records at the end of `ops` and numbers the shape classes, program by program.
+// The literals and folded prefixes go to the pool, the offsets of their Date placeholders to `fixups`, and file blobs to
+// the cold section, all in program order.
+static std::vector<ProgRec> lower_progs(std::vector<Prog>& sprogs, Pool& pool, std::vector<uint8_t>& cold,
+                                        std::vector<uint32_t>& fixups, std::vector<Op>& ops) {
+    std::vector<ProgRec> progs(sprogs.size());
+    std::map<std::string, int> classes;  // shape class numbers follow program order
+    for (size_t pi = 0; pi < sprogs.size(); pi++) {
+        Prog& p = sprogs[pi];
         fold_static_clen(p.ops);
         merge_literals(p.ops);
         fold_prefixes(p.ops);
         ProgRec& P = progs[pi];
-        memset(&P, 0, sizeof P);
         P.first_op = (uint16_t)ops.size();
         P.n_ops = (uint16_t)p.ops.size();
         P.status = (uint16_t)p.status;
         P.row_words = (uint16_t)p.row_words;
         P.encfail = p.encfail >= 0 ? (uint16_t)p.encfail : (uint16_t)0xFFFF;
         if (p.bind) P.flags |= PF_BIND;
+        std::string shape;
         for (auto& so : p.ops) {
-            Op o;
-            memset(&o, 0, sizeof o);
+            Op o{};
             o.code = so.code; o.arg = so.arg; o.kind = so.kind;
             o.flags = so.flags | (so.body ? OPF_BODY : 0);
             o.off = so.off; o.aux = so.aux;
@@ -1173,30 +1132,22 @@ int seal_table(gofr_table* t) {
             }
             if (so.body) P.body_fixed += fixed; else P.hdr_fixed += fixed;
             ops.push_back(o);
+            shape += "|" + std::to_string(o.code) + "," + std::to_string(o.flags) + "," + std::to_string(o.kind) + (o.len ? "p" : "");
         }
-        max_fixed = std::max(max_fixed, P.hdr_fixed + P.body_fixed);
+        // shape class: the same op-code / flag sequence means the same control flow in the interpreter
+        shape = std::to_string(P.flags & (PF_BIND | PF_NEEDS_ROW)) + shape;
+        auto it = classes.find(shape);
+        int id = it != classes.end() ? it->second : (int)classes.size() + 1;
+        if (it == classes.end()) classes[shape] = id;
+        P.shape_class = (uint8_t)(id > 30 ? 30 : id);
     }
+    return progs;
+}
 
-    // shape classes: same op-code / flag sequence → same control flow in the interpreter
-    {
-        std::map<std::string, int> classes;
-        for (size_t pi = 0; pi < progs.size(); pi++) {
-            ProgRec& P = progs[pi];
-            std::string sig = std::to_string(P.flags & (PF_BIND | PF_NEEDS_ROW));
-            for (uint32_t k = 0; k < P.n_ops; k++) {
-                const Op& o = ops[P.first_op + k];
-                sig += "|" + std::to_string(o.code) + "," + std::to_string(o.flags) + "," + std::to_string(o.kind) + (o.len ? "p" : "");
-            }
-            auto it = classes.find(sig);
-            int id = it != classes.end() ? it->second : (int)classes.size() + 1;
-            if (it == classes.end()) classes[sig] = id;
-            P.shape_class = (uint8_t)(id > 30 ? 30 : id);
-        }
-    }
-
-    // the size pass only needs the ops whose length depends on the request (everything else is pre-summed)
-    for (size_t pi = 0; pi < progs.size(); pi++) {
-        ProgRec& P = progs[pi];
+// The size pass only needs the ops whose length depends on the request (everything else is pre-summed): each program's
+// list of them is appended to `ops`, program by program.
+static void append_dynamic_ops(std::vector<ProgRec>& progs, std::vector<Op>& ops) {
+    for (ProgRec& P : progs) {
         P.first_dyn = (uint16_t)ops.size();
         std::vector<Op> dyn;
         for (uint32_t k = 0; k < P.n_ops; k++) {
@@ -1210,13 +1161,15 @@ int seal_table(gofr_table* t) {
         P.n_hdr_ops = nh;
         ops.insert(ops.end(), dyn.begin(), dyn.end());
     }
+}
 
-    // ---- slot-layout fast path: templates and tail ops (table_format.h FastRec) ----
+// The slot-layout fast path (table_format.h FastRec) of every program that takes it (PF_FAST), in program order: a template
+// in the pool (put16), its Date placeholders in `fixups`, and a private copy of its tail ops at the end of `ops`.
+static std::vector<FastRec> fast_path(std::vector<ProgRec>& progs, std::vector<Op>& ops, Pool& pool, std::vector<uint32_t>& fixups) {
     std::vector<FastRec> fast(progs.size());
     for (size_t pi = 0; pi < progs.size(); pi++) {
         ProgRec& P = progs[pi];
         FastRec& F = fast[pi];
-        memset(&F, 0, sizeof F);
         F.hex_pos = 0xFFFF;
         F.tail_op = P.first_op;
         F.n_tail_ops = P.n_ops;
@@ -1247,7 +1200,7 @@ int seal_table(gofr_table* t) {
             spans.push_back({k, (uint32_t)tmpl.size(), o.len});
             for (uint32_t fx : fixups)
                 if (o.len >= 29 && fx >= loff && fx + 29 <= loff + o.len) date_at.push_back((uint32_t)tmpl.size() + (fx - loff));
-            tmpl.append((const char*)lits.data() + loff, o.len);
+            tmpl.append((const char*)pool.img.data() + loff, o.len);
             if (o.code == OP_LIT) continue;
             if (o.code == OP_HEXID && F.hex_pos == 0xFFFF) { F.hex_pos = (uint16_t)tmpl.size(); tmpl.append(32, '0'); continue; }
             stop_op = k;
@@ -1302,23 +1255,27 @@ int seal_table(gofr_table* t) {
             ops.push_back(o);
         }
     }
+    return fast;
+}
 
-    std::vector<uint8_t> schema_bytes;
-    std::vector<SchemaRec> srecs(t->schemas.size());
-    std::vector<std::vector<FieldRec>> frecs(t->schemas.size());
-    for (size_t si = 0; si < t->schemas.size(); si++) {
-        SchemaDef& s = t->schemas[si];
-        SchemaRec& S = srecs[si];
-        memset(&S, 0, sizeof S);
+struct SchemaRecords { std::vector<SchemaRec> recs; std::vector<std::vector<FieldRec>> fields; };
+
+// SchemaRec and FieldRec of every schema.  Schema by schema, the type name and each field's strings go to the pool.
+static SchemaRecords schema_records(const gofr_table& t, Pool& pool) {
+    SchemaRecords sr;
+    sr.recs.resize(t.schemas.size());
+    sr.fields.resize(t.schemas.size());
+    for (size_t si = 0; si < t.schemas.size(); si++) {
+        const SchemaDef& s = t.schemas[si];
+        SchemaRec& S = sr.recs[si];
         S.n_fields = (uint16_t)s.fields.size();
         S.type_off = pool.put(s.go_type + std::string(1, '\0'));
         uint16_t word = 0, so = 0;
         for (auto& f : s.fields) {
-            FieldRec F;
-            memset(&F, 0, sizeof F);
+            FieldRec F{};
             F.kind = f.kind; F.omitempty = f.omitempty; F.word = word;
             F.container = f.container;
-            F.n_words = (uint8_t)field_words(t->schemas, f);
+            F.n_words = (uint8_t)field_words(t.schemas, f);
             F.elem = f.elem >= 0 ? (uint16_t)f.elem : (uint16_t)0xFFFF;
             word = (uint16_t)(word + F.n_words);
             F.name_len = (uint16_t)f.json_name.size();
@@ -1331,101 +1288,137 @@ int seal_table(gofr_table* t) {
             std::string tn = go_kind_name(f.kind);
             F.type_off = pool.put(tn);
             F.type_len = (uint16_t)tn.size();
-            frecs[si].push_back(F);
+            sr.fields[si].push_back(F);
         }
         S.flags = (uint16_t)((s.flat ? SF_FLAT : 0) | (s.bare() ? SF_BARE : 0) | (s.bindable ? SF_BINDABLE : 0));
         S.fixed_words = word;
         S.n_strings = so;
     }
+    return sr;
+}
 
-    H.n_pieces = (uint32_t)pieces.size();
-    H.n_progs = (uint32_t)progs.size();
-    H.n_ops = (uint32_t)ops.size();
-    H.n_schemas = (uint32_t)srecs.size();
-    for (size_t ri = 0; ri < t->routes.size(); ri++) {
-        if (t->routes[ri].hkind != GOFR_H_BIND_ECHO) continue;
-        uint32_t words = 8;
-        for (auto& f : t->schemas[routes[ri].schema].fields) words += (f.kind == GOFR_F_INT32 || f.kind == GOFR_F_BOOL) ? 1 : 2;  // bindable: checked at seal
+struct ImageParts {  // what the stages build, the sections of the image
+    std::vector<RouteProgs> route_progs;
+    RouteRecords records;
+    Dispatch dispatch;
+    std::vector<ProgRec> progs;
+    std::vector<Op> ops;
+    std::vector<uint32_t> fixups;
+    std::vector<FastRec> fast;
+    SchemaRecords schemas;
+    std::vector<uint8_t> lits, cold;
+};
+
+static uint32_t align16(std::vector<uint8_t>& img) {
+    while (img.size() % 16) img.push_back(0);
+    return (uint32_t)img.size();
+}
+template <typename T>
+static uint32_t append16(std::vector<uint8_t>& img, const std::vector<T>& v) {
+    const uint32_t off = align16(img);
+    img.insert(img.end(), (const uint8_t*)v.data(), (const uint8_t*)(v.data() + v.size()));
+    return off;
+}
+
+// The header's numbers, then the sections in the order table_format.h lays them out, each 16-byte aligned: the hot part
+// ends with the literal pool, the cold section follows.  The checksum covers the whole image.  Returns the hot part's size.
+static uint32_t write_image(const gofr_table& t, ImageHeader H, const ImageParts& s, std::vector<uint8_t>& img) {
+    H.n_pieces = (uint32_t)s.records.pieces.size();
+    H.n_progs = (uint32_t)s.progs.size();
+    H.n_ops = (uint32_t)s.ops.size();
+    H.n_schemas = (uint32_t)s.schemas.recs.size();
+    for (const RouteDef& r : t.routes) {
+        if (r.hkind != GOFR_H_BIND_ECHO) continue;
+        uint32_t words = 8;  // the span row's header
+        for (auto& f : route_schema(t, r)->fields) words += bind_field_words(f.kind);
         H.bind_row_words = std::max(H.bind_row_words, words);
     }
-    H.max_fixed_len = max_fixed;
+    for (const ProgRec& P : s.progs) H.max_fixed_len = std::max(H.max_fixed_len, P.hdr_fixed + P.body_fixed);
     {   // image_data_expand (engine_internal.h): the smallest thing that owns data bytes is a 4-byte word; it can drag along
         // one key literal, a comma and a pair of braces per nesting level, and the longest scalar text (a float64: 25 bytes)
         bool any_values = false;
-        for (auto& P : progs) any_values |= (P.flags & PF_VALUES) != 0;
+        for (auto& P : s.progs) any_values |= (P.flags & PF_VALUES) != 0;
         size_t max_key = 0, depth = 1;
-        for (auto& sc : t->schemas) {
+        for (auto& sc : t.schemas) {
             depth = std::max(depth, (size_t)sc.depth);
             for (auto& f : sc.fields) max_key = std::max(max_key, json_escape_go(f.json_name).size() + 3);
         }
-        H.reserved3[0] = any_values ? (uint32_t)std::max<size_t>(6, (depth * (max_key + 3) + 28 + 3) / 4) : 6u;
+        H.data_expand = any_values ? (uint32_t)std::max<size_t>(6, (depth * (max_key + 3) + 28 + 3) / 4) : 6u;
     }
+    H.hash_bits = s.dispatch.hash_bits;
+    H.thash_bits = s.dispatch.thash_bits;
+    H.n_tmpl = (uint32_t)s.dispatch.tmpl.size();
+    H.n_fixups = (uint32_t)s.fixups.size();
 
-    auto append = [&](const void* p, size_t n) {
-        align16();
-        uint32_t off = (uint32_t)img.size();
-        img.insert(img.end(), (const uint8_t*)p, (const uint8_t*)p + n);
-        return off;
-    };
-    H.routes_off = append(routes.data(), routes.size() * sizeof(RouteRec));
-    H.pieces_off = append(pieces.data(), pieces.size() * sizeof(PieceRec));
-    H.progs_off = append(progs.data(), progs.size() * sizeof(ProgRec));
-    H.ops_off = append(ops.data(), ops.size() * sizeof(Op));
-    H.hash_off = append(hash_tab.data(), hash_tab.size() * 2);
-    H.hash_bits = hash_bits;
-    H.thash_off = append(thash_tab.data(), thash_tab.size() * 2);
-    H.thash_bits = thash_bits;
-    H.tmpl_off = append(tmpl_list.data(), tmpl_list.size() * 2);
-    H.n_tmpl = (uint32_t)tmpl_list.size();
-    {
-        std::vector<uint32_t> keys(tmpl_list.size() * 4, 0u);
-        for (size_t ti = 0; ti < tmpl_list.size(); ti++) {
-            const RouteDef& r = t->routes[tmpl_list[ti]];
-            const std::string& l0 = r.pieces.empty() ? std::string() : r.pieces[0].lit;
-            uint8_t kb[8] = {0}, mb[8] = {0};
-            for (size_t k = 0; k < l0.size() && k < 8; k++) { kb[k] = (uint8_t)l0[k]; mb[k] = 0xFF; }
-            memcpy(&keys[ti * 4], kb, 8);
-            memcpy(&keys[ti * 4 + 2], mb, 8);
-        }
-        if (keys.empty()) keys.resize(4, 0u);
-        H.tmplkey_off = append(keys.data(), keys.size() * 4);
-    }
-    H.last_method_off = append(last_method.data(), last_method.size() * 2);
-    {
-        std::vector<uint32_t> ids;
-        for (auto& sdef : t->schemas) ids.push_back(sdef.id);
-        if (ids.empty()) ids.push_back(0xFFFFFFFFu);
-        H.schema_ids_off = append(ids.data(), ids.size() * 4);
-    }
-    H.fast_off = append(fast.data(), fast.size() * sizeof(FastRec));
+    std::vector<uint32_t> schema_ids;
+    for (auto& sdef : t.schemas) schema_ids.push_back(sdef.id);
+    if (schema_ids.empty()) schema_ids.push_back(0xFFFFFFFFu);
+    std::vector<uint16_t> rawprogs;
+    for (const RouteProgs& rp : s.route_progs) rawprogs.insert(rawprogs.end(), rp.raw, rp.raw + 9);
     if (rawprogs.empty()) rawprogs.resize(9, 0xFFFF);
-    H.rawprog_off = append(rawprogs.data(), rawprogs.size() * 2);
-    H.fixups_off = append(fixups.data(), fixups.size() * 4);
-    H.n_fixups = (uint32_t)fixups.size();
+
+    img.assign(sizeof(ImageHeader), 0);
+    H.routes_off = append16(img, s.records.routes);
+    H.pieces_off = append16(img, s.records.pieces);
+    H.progs_off = append16(img, s.progs);
+    H.ops_off = append16(img, s.ops);
+    H.hash_off = append16(img, s.dispatch.hash);
+    H.thash_off = append16(img, s.dispatch.thash);
+    H.tmpl_off = append16(img, s.dispatch.tmpl);
+    H.tmplkey_off = append16(img, s.dispatch.tmpl_keys);
+    H.last_method_off = append16(img, s.dispatch.last_method);
+    H.schema_ids_off = append16(img, schema_ids);
+    H.fast_off = append16(img, s.fast);
+    H.rawprog_off = append16(img, rawprogs);
+    H.fixups_off = append16(img, s.fixups);
     // schemas: SchemaRec[n] then each field table
-    align16();
-    H.schemas_off = (uint32_t)img.size();
-    size_t srec_pos = img.size();
-    img.resize(img.size() + srecs.size() * sizeof(SchemaRec));
-    for (size_t si = 0; si < srecs.size(); si++) {
-        srecs[si].fields_off = append(frecs[si].data(), frecs[si].size() * sizeof(FieldRec));
-        memcpy(img.data() + srec_pos + si * sizeof(SchemaRec), &srecs[si], sizeof(SchemaRec));
+    H.schemas_off = append16(img, s.schemas.recs);
+    for (size_t si = 0; si < s.schemas.recs.size(); si++) {
+        SchemaRec S = s.schemas.recs[si];
+        S.fields_off = append16(img, s.schemas.fields[si]);
+        memcpy(img.data() + H.schemas_off + si * sizeof(SchemaRec), &S, sizeof S);
     }
-    H.lits_off = append(lits.data(), lits.size());
-    align16();
-    H.hot_bytes = (uint32_t)img.size();
-    H.cold_off = append(cold.data(), cold.size());
-    align16();
-    H.total_bytes = (uint32_t)img.size();
-    H.checksum = 0;
+    H.lits_off = append16(img, s.lits);
+    H.hot_bytes = align16(img);
+    H.cold_off = append16(img, s.cold);
+    H.total_bytes = align16(img);
     memcpy(img.data(), &H, sizeof H);
     H.checksum = image_checksum(img.data(), img.size());
     memcpy(img.data(), &H, sizeof H);
-    if (H.hot_bytes > kMaxHotBytes) {
-        set_last_error("sealed table needs %u bytes of shared memory (limit %u)", H.hot_bytes, kMaxHotBytes);
+    return H.hot_bytes;
+}
+
+// Compiles the table's registrations into a sealed image (table_format.h).  The table itself is not changed.
+static int seal_table(const gofr_table& t, std::vector<uint8_t>& image) {
+    for (const RouteDef& r : t.routes)
+        if (const int rc = check_route(t, r)) return rc;
+    ImageHeader H{};
+    H.magic = kMagic; H.version = kImageVersion; H.frame_mode = t.frame_mode;
+    H.n_routes = (uint32_t)t.routes.size();
+    H.has_catchall = t.has_catchall;
+
+    // program indices follow the order of Builder::add calls: the fixed programs, then every route's, route by route
+    Builder b{t, {}, {}};
+    add_fixed_progs(b, H);
+    ImageParts s;
+    for (const RouteDef& r : t.routes) s.route_progs.push_back(add_route_progs(b, r, H.prog_panic));
+
+    // literal-pool offsets follow the order of Pool::put calls: route records, program ops, fast-path templates, schemas.
+    // The op array is built in three parts, in this order: every program's ops, the dynamic-op lists, the fast-path tail
+    // copies.
+    Pool pool(s.lits);
+    s.records = route_records(t, s.route_progs, pool);
+    s.dispatch = dispatch_tables(t, s.records.routes);
+    s.progs = lower_progs(b.progs, pool, s.cold, s.fixups, s.ops);
+    append_dynamic_ops(s.progs, s.ops);
+    s.fast = fast_path(s.progs, s.ops, pool, s.fixups);
+    s.schemas = schema_records(t, pool);
+
+    const uint32_t hot_bytes = write_image(t, H, s, image);
+    if (hot_bytes > kMaxHotBytes) {
+        set_last_error("sealed table needs %u bytes of shared memory (limit %u)", hot_bytes, kMaxHotBytes);
         return GOFR_ERR_CAPACITY;
     }
-    t->sealed = true;
     return GOFR_OK;
 }
 
@@ -1543,7 +1536,13 @@ int gofr_table_add_default_routes(gofr_table* t, const uint8_t* favicon, uint32_
 int gofr_table_seal(gofr_table* t) {
     if (!t) return GOFR_ERR_INVALID;
     if (t->sealed) return GOFR_ERR_SEALED;
-    return seal_table(t);
+    std::vector<uint8_t> image;
+    const int rc = gofr::seal_table(*t, image);
+    if (rc == GOFR_OK) {  // a failed seal leaves the table as it was
+        t->image = std::move(image);
+        t->sealed = true;
+    }
+    return rc;
 }
 
 int gofr_table_serialize(const gofr_table* t, uint8_t* buf, uint64_t* len_inout) {

@@ -51,7 +51,9 @@ struct ImageHeader {  // 160 B
     uint32_t rawprog_off;    // uint16[n_routes][9]: GOFR_H_RESULT routes, programs of the response.Raw outcomes
                              // [(RAW_DATA, RAW_STRING, RAW_NIL) x (200, 500, 404)], 0xFFFF = none
     uint32_t schema_ids_off; // uint32[n_schemas]: the caller's schema ids in table order (gofr_bind_device looks one up)
-    uint32_t reserved3[2];
+    uint32_t data_expand;    // response bytes one byte of a request's data section can become, at most (engine_internal.h
+                             // image_data_expand)
+    uint32_t pad3;
 };
 static_assert(sizeof(ImageHeader) == 160, "ImageHeader layout");
 
@@ -101,7 +103,6 @@ static_assert(sizeof(PieceRec) == 48, "PieceRec layout");
 enum OpCode : uint8_t {
     OP_LIT = 0,     // literal bytes lits[off .. off+len)
     OP_HEXID = 1,   // 32 lower-case hex chars of the request's trace id   (middleware/logger.go:46-47)
-    OP_DATE = 2,    // (builder only) the batch's 29-byte IMF-fixdate: sealed as a literal placeholder + fixup
     OP_CLEN = 3,    // decimal length of the body                           (net/http Content-Length)
     OP_I64 = 4,     // strconv.AppendInt of a row field; off = word index in the row
     OP_I32 = 5,

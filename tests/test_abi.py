@@ -54,6 +54,29 @@ def test_table_errors_are_codes():
     assert L.gofr_table_add_route(t.handle, 0, b"/late", 5, C.byref(h), None) == 5  # GOFR_ERR_SEALED
     with pytest.raises(_abi.GofrError):
         Table(image=b"\x00" * 200)
+    # seal-time rejections: the code and the text gofr_last_error() gives
+    not_bindable = S.Schema(4, "main.Tags", [S.Field("Tags", S.F_STRING, "tags", container=S.C_SLICE)])
+    for routes, schemas, code, text in (
+            ([S.Route(S.M_POST, "/echo", S.H_BIND_ECHO, schema_id=4)], [not_bindable], 2, "Bind takes flat structs"),
+            ([S.Route(S.M_GET, "/q", S.H_PARAM_FORMAT, s0=b"k", s2=b"\xff")], [], 2, "must be valid UTF-8"),
+            ([S.Route(S.M_GET, "/x", 13)], [], 1, "unknown handler kind 13")):
+        with pytest.raises(_abi.GofrError) as e:
+            Table(S.TableSpec(schemas=schemas, routes=routes))
+        assert e.value.code == code and text in L.gofr_last_error().decode(), (code, text)
+    # a table whose hot part exceeds the 40 KB shared-memory budget is refused, and the failed seal leaves it unsealed
+    big = C.c_void_p()
+    assert L.gofr_table_create(C.byref(big), S.FRAME_WIRE) == 0
+    for i in range(200):
+        p = ("/" + ("r%03d" % i) * 60).encode()
+        assert L.gofr_table_add_route(big, S.M_GET, p, len(p), C.byref(h), None) == 0
+    favicon = S.TableSpec().favicon
+    assert L.gofr_table_add_default_routes(big, favicon, len(favicon)) == 0
+    assert L.gofr_table_seal(big) == 7  # GOFR_ERR_CAPACITY
+    assert b"needs 76400 bytes of shared memory" in L.gofr_last_error()
+    assert L.gofr_table_max_response_bytes(big, 100) == 0 and L.gofr_table_response_bound(big, 10, 0, 10) == 0
+    n = C.c_uint64(0)
+    assert L.gofr_table_serialize(big, None, C.byref(n)) == 6  # GOFR_ERR_NOT_SEALED
+    L.gofr_table_destroy(big)
 
 
 def test_http_date_helper():
