@@ -203,6 +203,32 @@ GOFR_HD uint32_t bd_skip_ws(const uint8_t* s, uint32_t n, uint32_t i) {
     while (i < n && js_space(s[i])) i++;
     return i;
 }
+#if GOFR_TU_VALUES
+// end (exclusive) of the string starting at the quote s[i]
+GOFR_HD uint32_t bd_skip_string(const uint8_t* s, uint32_t i) {
+    i++;
+    while (s[i] != '"') { if (s[i] == '\\') i++; i++; }
+    return i + 1;
+}
+// end (exclusive) of the value starting at i.  Not recursive here: a recursive device function grows its stack at run
+// time, beyond the per-thread size ptxas records for the kernel, and the VALUES instances' frames (1008 bytes packed,
+// 1104 slot layout) leave less than one call's 48 bytes under the 1 KB default limit — an H100 reported an illegal
+// memory access on the first Bind-echo request of a table with float64 members.  The default instances (frames of 480
+// bytes) keep the recursive form below: the loop changed their register allocation and cost the packed kernel 2.4 %.
+GOFR_HD_NOINLINE uint32_t bd_skip_value(const uint8_t* s, uint32_t n, uint32_t i) {
+    uint32_t c = s[i];
+    if (c == '"') return bd_skip_string(s, i);
+    if (c == '{' || c == '[') {
+        uint32_t depth = 0;
+        for (;;) {
+            uint32_t x = s[i];
+            if (x == '"') { i = bd_skip_string(s, i); continue; }
+            if (x == '{' || x == '[') depth++;
+            if (x == '}' || x == ']') { depth--; if (depth == 0) return i + 1; }
+            i++;
+        }
+    }
+#else
 // end (exclusive) of the value starting at i
 GOFR_HD uint32_t bd_skip_value(const uint8_t* s, uint32_t n, uint32_t i) {
     uint32_t c = s[i];
@@ -221,6 +247,7 @@ GOFR_HD uint32_t bd_skip_value(const uint8_t* s, uint32_t n, uint32_t i) {
             i++;
         }
     }
+#endif
     while (i < n) {
         uint32_t x = s[i];
         if (x == ',' || x == '}' || x == ']' || js_space(x)) break;

@@ -403,9 +403,6 @@ def _gpu_float_check():
 
 
 @pytest.mark.gpu
-@pytest.mark.xfail(strict=False, reason="float64 Bind targets were added after this round's GPU minutes were spent: the device code is "
-                   "checked on the CPU against the oracle and Python's float() (above); its first launch on a GPU is this test — "
-                   "XPASS means it matched")
 def test_gpu_bind_float_fields():
     """the serve kernels (VALUES instance, PF_BIND program with OP_F64) and gofr_bind_device on 20 000 bodies with float64
     members — in a child process, so that a fault cannot leave a sticky CUDA error behind for the other GPU tests"""
