@@ -683,20 +683,25 @@ static int grow(void** p, size_t* cap, size_t need, size_t slack) {
 static constexpr size_t kArenaSlack = 16;
 
 // A chunk = contiguous request range [lo, hi) and the arena byte range it covers.
-struct ChunkPlan { uint32_t lo, hi; uint32_t arena_lo, arena_hi; };
+struct ChunkPlan { uint32_t lo, hi; uint32_t arena_lo, arena_hi; uint64_t out_bound; };
 
 // The arena byte range [*alo, *ahi) (16-byte granular) that requests [lo, hi) reference: their whole requests, or their paths
 // only (what routing reads).  All arithmetic in 64 bits: a descriptor with a huge arena_off or data_len (say a data_len taken
-// from a Content-Length header) must be refused, not wrap around and pass.
-static int chunk_arena_range(const gofr_req_batch* in, uint32_t lo, uint32_t hi, bool path_only, uint32_t* alo_out, uint32_t* ahi_out) {
-    uint64_t alo = ~0ull, ahi = 0;
+// from a Content-Length header) must be refused, not wrap around and pass.  sizes (optional) receives the requests' total
+// path + query bytes and total data bytes: what their responses are bounded by (chunk_out_bound).
+static int chunk_arena_range(const gofr_req_batch* in, uint32_t lo, uint32_t hi, bool path_only, uint32_t* alo_out, uint32_t* ahi_out,
+                             uint64_t* sizes = nullptr) {
+    uint64_t alo = ~0ull, ahi = 0, pq = 0, data = 0;
     const gofr_req_desc* dd = in->desc;
     for (uint32_t i = lo; i < hi; i++) {
         const uint64_t a = dd[i].arena_off;
         const uint64_t dend = path_only ? a + dd[i].path_len : ((a + dd[i].path_len + dd[i].query_len + 3u) & ~3ull) + dd[i].data_len;
         alo = a < alo ? a : alo;
         ahi = dend > ahi ? dend : ahi;
+        pq += (uint64_t)dd[i].path_len + dd[i].query_len;
+        data += dd[i].data_len;
     }
+    if (sizes) { sizes[0] = pq; sizes[1] = data; }
     if (hi <= lo) alo = 0;
     alo &= ~15ull;
     ahi = (ahi + 15ull) & ~15ull;
@@ -708,6 +713,16 @@ static int chunk_arena_range(const gofr_req_batch* in, uint32_t lo, uint32_t hi,
     *alo_out = (uint32_t)alo;
     *ahi_out = (uint32_t)(ahi > alo ? ahi : alo);
     return GOFR_OK;
+}
+
+// Device output bytes a packed chunk can need: the sum of gofr_table_response_bound over its requests (fixed part,
+// Content-Length digits, six bytes per path and query byte, image_data_expand per data byte).  The arena span is no measure
+// of it: requests may share arena bytes (many descriptors pointing at one cached row), and each of them answers in full.
+static uint64_t chunk_out_bound(const gofr_engine* e, uint32_t cn, const uint64_t sizes[2]) {
+    // (the sums are clamped to 2^32 first: the products cannot wrap, and the result is capped below that anyway)
+    const uint64_t pq = std::min<uint64_t>(sizes[0], 1ull << 32), data = std::min<uint64_t>(sizes[1], 1ull << 32);
+    const uint64_t b = (uint64_t)cn * (e->hdr.max_fixed_len + 16 + 2) + 6 * pq + (uint64_t)image_data_expand(e->hdr) * data;
+    return std::min<uint64_t>(b, 0xFFFFFFF0ull);
 }
 
 // Enqueues the H2D copies of a chunk on `st`: descriptors and trace ids of requests [lo, lo + n) (no ids: d_ids null) and
@@ -813,9 +828,10 @@ static int batch_submit_locked(gofr_engine* e, const gofr_req_batch* in, gofr_re
         if (planned[ci]) return GOFR_OK;
         uint32_t lo = (uint32_t)(ci * e->chunk), hi = std::min<uint32_t>(n, lo + e->chunk);
         uint32_t alo = 0, ahi = 0;
-        int prc = chunk_arena_range(in, lo, hi, false, &alo, &ahi);
+        uint64_t sizes[2];
+        int prc = chunk_arena_range(in, lo, hi, false, &alo, &ahi, sizes);
         if (prc) return prc;
-        plan[ci] = {lo, hi, alo, ahi};
+        plan[ci] = {lo, hi, alo, ahi, chunk_out_bound(e, hi - lo, sizes)};
         planned[ci] = 1;
         return GOFR_OK;
     };
@@ -834,9 +850,7 @@ static int batch_submit_locked(gofr_engine* e, const gofr_req_batch* in, gofr_re
             { int prc = plan_chunk(ci); if (prc) return prc; }
             const ChunkPlan& c = plan[ci];
             uint32_t cn = c.hi - c.lo;
-            size_t abytes = (size_t)c.arena_hi - c.arena_lo;
-            size_t ocap = std::min<size_t>((size_t)cn * (e->hdr.max_fixed_len + 64) + (size_t)image_data_expand(e->hdr) * abytes + 4096, 0xFFFFFFF0ull);
-            int rc = s.reserve(e, cn, abytes, ocap);
+            int rc = s.reserve(e, cn, (size_t)c.arena_hi - c.arena_lo, c.out_bound);
             if (!rc) rc = upload_chunk(in, c.lo, cn, c.arena_lo, c.arena_hi, s.d_desc, s.d_ids, s.d_arena, e->st_h2d);
             if (rc) return rc;
             CUDA_TRY(cudaEventRecord(s.ev_h2d, e->st_h2d));
@@ -882,9 +896,7 @@ static int batch_submit_locked(gofr_engine* e, const gofr_req_batch* in, gofr_re
             { int prc = plan_chunk(issued); if (prc) return prc; }
             const ChunkPlan& c = plan[issued];
             uint32_t cn = c.hi - c.lo;
-            size_t abytes = (size_t)c.arena_hi - c.arena_lo;
-            size_t ocap = std::min<size_t>((size_t)cn * (e->hdr.max_fixed_len + 64) + (size_t)image_data_expand(e->hdr) * abytes + 4096, 0xFFFFFFF0ull);
-            int rc = s.reserve(e, cn, abytes, ocap);
+            int rc = s.reserve(e, cn, (size_t)c.arena_hi - c.arena_lo, c.out_bound);
             if (!rc) rc = upload_chunk(in, c.lo, cn, c.arena_lo, c.arena_hi, s.d_desc, s.d_ids, s.d_arena, s.stream);
             if (rc) return rc;
             // descriptors keep absolute arena offsets: pass a rebased arena pointer

@@ -441,11 +441,9 @@ def _gpu_decode_check():
 
 
 @pytest.mark.gpu
-@pytest.mark.xfail(strict=False, reason="the nested decoder's kernel was finished after this round's GPU minutes were spent: its device "
-                   "code is checked on the CPU three ways (above), its first launch on a GPU is this test — XPASS means it matched")
 def test_gpu_decode_matches_oracle():
     """gofr_proto_decode_nested_device on the GPU == oracle (statuses, offsets, rows) — in a child process, so that a fault
-    in a kernel that has never run cannot leave a sticky CUDA error in the process the other GPU tests run in"""
+    in the kernel cannot leave a sticky CUDA error in the process the other GPU tests run in"""
     import os
     import subprocess
     import sys

@@ -145,14 +145,20 @@ def test_gpu_matches_oracle(which, n):
 # oracle's literal restatement of mux (recursive leftmost-first), including variable spans ----
 from hypothesis import given, settings, strategies as st  # noqa: E402
 
-_seg = st.sampled_from(["a", "b", "ab", "users", "v1", "x.y", "1", "22", "a-b", "_", "apiservice", "apiserver", "api"])  # the long ones
-# give templates a leading literal of >= 8 bytes (keyed dispatch), two of them with the same first 8 bytes
-_var = st.sampled_from(["{id}", "{n:[0-9]+}", "{w:[a-z]+}", "{s:[a-z0-9.]*}", "{id}.{ext}", "{a}{b:[0-9]+}", "p{q}", "{d:\\d+}x",
-                        "{y:[0-9]{2}}", "{v:v[0-9]+}", "{f:[a-z]+\\.[a-z]{1,3}}", "{o:[a-z]?[0-9]{1,2}}", "{r:\\d{1,}-?\\w*}", "{m:a{2,}b?}",
-                        "{h:[a-z]+-[a-z0-9]+}", "{t:.*x}"])
+# the long segments give templates a leading literal of >= 8 bytes (keyed dispatch), two of them with the same first 8 bytes
+SEGMENTS = ["a", "b", "ab", "users", "v1", "x.y", "1", "22", "a-b", "_", "apiservice", "apiserver", "api"]
+VARIABLES = ["{id}", "{n:[0-9]+}", "{w:[a-z]+}", "{s:[a-z0-9.]*}", "{id}.{ext}", "{a}{b:[0-9]+}", "p{q}", "{d:\\d+}x",
+             "{y:[0-9]{2}}", "{v:v[0-9]+}", "{f:[a-z]+\\.[a-z]{1,3}}", "{o:[a-z]?[0-9]{1,2}}", "{r:\\d{1,}-?\\w*}", "{m:a{2,}b?}",
+             "{h:[a-z]+-[a-z0-9]+}", "{t:.*x}"]
+ROUTE_METHODS = [S.M_GET, S.M_GET, S.M_POST, S.M_DELETE, S.M_ANY]
+REQ_METHODS = [S.M_GET, S.M_POST, S.M_DELETE, S.M_OPTIONS, S.M_HEAD, S.M_OTHER]
+PATH_SEGMENTS = ["a", "b", "ab", "users", "v1", "x.y", "1", "22", "a-b", "_", "42", "abc9", "apiservice", "apiserver", "api", "apiserv",
+                 "p7", "3x", "q.tar.gz", "", ".", ".."]
+_seg = st.sampled_from(SEGMENTS)
+_var = st.sampled_from(VARIABLES)
 _piece = st.one_of(_seg, _var)
 _pattern = st.lists(_piece, min_size=0, max_size=4).map(lambda ps: "/" + "/".join(ps))
-_method = st.sampled_from([S.M_GET, S.M_GET, S.M_POST, S.M_DELETE, S.M_ANY])
+_method = st.sampled_from(ROUTE_METHODS)
 
 
 def _rename_vars(pattern: str, k: int) -> str:
@@ -174,9 +180,7 @@ def _rename_vars(pattern: str, k: int) -> str:
 
 @settings(max_examples=250, deadline=None)
 @given(st.lists(st.tuples(_method, _pattern), min_size=1, max_size=10), st.booleans(),
-       st.lists(st.tuples(st.sampled_from([S.M_GET, S.M_POST, S.M_DELETE, S.M_OPTIONS, S.M_HEAD, S.M_OTHER]),
-                          st.lists(st.sampled_from(["a", "b", "ab", "users", "v1", "x.y", "1", "22", "a-b", "_", "42", "abc9", "apiservice", "apiserver", "api", "apiserv",
-                                                    "p7", "3x", "q.tar.gz", "", ".", ".."]), min_size=0, max_size=4)),
+       st.lists(st.tuples(st.sampled_from(REQ_METHODS), st.lists(st.sampled_from(PATH_SEGMENTS), min_size=0, max_size=4)),
                 min_size=1, max_size=24))
 def test_random_tables_property(routes, defaults, reqs):
     spec = S.TableSpec(default_routes=defaults,

@@ -653,8 +653,6 @@ def _gpu_late_kinds_check():
 
 
 @pytest.mark.gpu
-@pytest.mark.xfail(strict=False, reason="uint64 / []byte / float32 members were added after this round's GPU minutes were spent: oracle, device "
-                   "code on the CPU and the Python model agree (above); the first launch on a GPU is this test — XPASS means it matched")
 def test_gpu_late_kinds():
     """6 000 rows of the kinds added late (uint64, []byte as base64, float32; by value, behind pointers, in slices and maps),
     packed and slot layouts, GOFR_H_ROW and GOFR_H_RESULT — in a child process (a fault cannot reach the other GPU tests)"""
@@ -760,20 +758,17 @@ def _rand_schemas(rnd, n_types, late=False):
     return schemas, bare
 
 
-@pytest.mark.parametrize("seed", range(24))
-def test_random_schemas_three_ways(seed):
+def _random_schema_case(seed, n=400):
+    """A table of random schemas and n requests of random values for them: (spec, routed schemas, batch, want) where
+    want[i] is the body the Python model writes (None: encoding/json cannot encode the value)."""
     rnd = random.Random(1000 + seed)
     structs, bare = _rand_schemas(rnd, rnd.randint(2, 5), late=seed >= 12)
     routed = structs + bare
     mode = [S.FRAME_WIRE, S.FRAME_BODY, S.FRAME_INTENDED][seed % 3]
     spec = S.TableSpec(frame_mode=mode, schemas=structs + bare,
                        routes=[S.Route(S.M_GET, "/t/%d" % sc.id, S.H_RESULT if seed % 2 else S.H_ROW, schema_id=sc.id) for sc in routed])
-    try:
-        table = Table(spec)
-    except Exception as e:      # deeper than 8 levels cannot happen with <= 5 types; anything else is a bug
-        raise AssertionError((e, structs, bare))
     reqs, want = [], []
-    for i in range(400):
+    for i in range(n):
         sc = routed[rnd.randrange(len(routed))]
         vals = _rand_value(rnd, spec, sc, nan_rate=0.005)
         row = sc.encode_row(vals, spec.schema)
@@ -790,7 +785,17 @@ def test_random_schemas_three_ways(seed):
             body = None if body is None else '{"data":%s}\n' % body
         reqs.append(S.Req(S.M_GET, b"/t/%d" % sc.id, b"", data))
         want.append(body)
-    batch = S.RequestBatch.pack(reqs, seed=seed)
+    return spec, routed, S.RequestBatch.pack(reqs, seed=seed), want
+
+
+@pytest.mark.parametrize("seed", range(24))
+def test_random_schemas_three_ways(seed):
+    spec, routed, batch, want = _random_schema_case(seed)
+    mode = spec.frame_mode
+    try:
+        table = Table(spec)
+    except Exception as e:      # deeper than 8 levels cannot happen with <= 5 types; anything else is a bug
+        raise AssertionError((e, routed))
     o1, f1, m1 = O.OracleTable(spec).serve(batch, DATE, out_cap=1 << 22)
     image = table.serialize()
     E.set_flush_mode(seed % 3)
@@ -814,6 +819,30 @@ def test_random_schemas_three_ways(seed):
             assert out[i, :L].tobytes() == ob[int(f1[i]):int(f1[i]) + L], i
 
 
+def _mutated_rows(rnd, spec, routed, kind, n):
+    """n requests for the /t/<id> routes of `routed` whose rows (or result records) have bytes flipped, count words
+    overwritten, tails cut off or garbage appended"""
+    reqs = []
+    for i in range(n):
+        sc = routed[rnd.randrange(len(routed))]
+        row = sc.encode_row(_rand_value(rnd, spec, sc), spec.schema)
+        data = bytearray(S.result_record(rnd.choice([S.RESULT_DATA, S.RESULT_RAW_DATA]), row) if kind == S.H_RESULT else row)
+        for _k in range(rnd.randint(0, 3)):
+            if not data:
+                break
+            r, p = rnd.random(), rnd.randrange(len(data))
+            if r < 0.4:
+                data[p] ^= 1 << rnd.randrange(8)
+            elif r < 0.6:
+                data[p & ~3:(p & ~3) + 4] = rnd.choice([0xFFFFFFFF, 0xFFFFFFFE, 0x7FFFFFFF, 1 << 20, 3]).to_bytes(4, "little")
+            elif r < 0.8:
+                del data[p:]
+            else:
+                data += bytes(rnd.randrange(256) for _ in range(rnd.randint(1, 9)))
+        reqs.append(S.Req(S.M_GET, b"/t/%d" % sc.id, b"", bytes(data)))
+    return reqs
+
+
 @pytest.mark.parametrize("seed", list(range(6)) + list(range(10, 18)))
 def test_mutated_rows_device_code_equals_oracle(seed):
     """rows of random schemas with bytes flipped, count words overwritten, tails cut off or garbage appended: whatever the
@@ -824,25 +853,7 @@ def test_mutated_rows_device_code_equals_oracle(seed):
         routed = structs + bare
         kind = S.H_RESULT if seed % 2 else S.H_ROW
         spec = S.TableSpec(schemas=routed, routes=[S.Route(S.M_GET, "/t/%d" % sc.id, kind, schema_id=sc.id) for sc in routed])
-        reqs = []
-        for i in range(250):
-            sc = routed[rnd.randrange(len(routed))]
-            row = sc.encode_row(_rand_value(rnd, spec, sc), spec.schema)
-            data = bytearray(S.result_record(rnd.choice([S.RESULT_DATA, S.RESULT_RAW_DATA]), row) if kind == S.H_RESULT else row)
-            for _k in range(rnd.randint(0, 3)):
-                if not data:
-                    break
-                r, p = rnd.random(), rnd.randrange(len(data))
-                if r < 0.4:
-                    data[p] ^= 1 << rnd.randrange(8)
-                elif r < 0.6:
-                    data[p & ~3:(p & ~3) + 4] = rnd.choice([0xFFFFFFFF, 0xFFFFFFFE, 0x7FFFFFFF, 1 << 20, 3]).to_bytes(4, "little")
-                elif r < 0.8:
-                    del data[p:]
-                else:
-                    data += bytes(rnd.randrange(256) for _ in range(rnd.randint(1, 9)))
-            reqs.append(S.Req(S.M_GET, b"/t/%d" % sc.id, b"", bytes(data)))
-        b = S.RequestBatch.pack(reqs, seed=seed)
+        b = S.RequestBatch.pack(_mutated_rows(rnd, spec, routed, kind, 250), seed=seed)
         o1, f1, m1 = O.OracleTable(spec).serve(b, DATE, out_cap=1 << 24)
         o2, f2, m2 = E.serve(Table(spec).serialize(), b, DATE, out_cap=1 << 24)
         assert np.array_equal(m1, m2) and np.array_equal(f1, f2)
