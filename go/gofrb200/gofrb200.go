@@ -301,7 +301,9 @@ func (e *Engine) ProtoDecodeDevice(fields []ProtoField, dIn, dInOff unsafe.Point
 // ProtoNField / ProtoNMsg describe message types with nested and repeated fields (gofr_proto_nfield / gofr_proto_nmsg):
 // Msgs[m] owns Fields[FirstField : FirstField+NFields] in ascending field-number order; a field of Type 11
 // (TYPE_MESSAGE) names its message type in Msg.  protoreflect gives all of it: for a generated message,
-// walk md.Fields() (fd.Number(), fd.Kind(), fd.IsList(), fd.Message()).
+// walk md.Fields() (fd.Number(), fd.Kind(), fd.IsList(), fd.Message()).  A map field (fd.IsMap()) has Type ProtoMap,
+// Repeated 0 and its entry type (fd.Message(): fields 1 key, 2 value) in Msg; rows carry its entries in ascending key
+// order, which makes the output protobuf-go's Deterministic bytes.  (This file is not compiled in the repository's tests.)
 type ProtoNField struct {
 	Number   uint32
 	Type     uint8
@@ -309,6 +311,9 @@ type ProtoNField struct {
 	Msg      uint16
 }
 type ProtoNMsg struct{ FirstField, NFields uint16 }
+
+// ProtoMap is the ProtoNField.Type of a map field (GOFR_PB_MAP).
+const ProtoMap = C.GOFR_PB_MAP
 
 // ProtoEncodeNestedDevice marshals n rows as messages of type msgs[root] and frames them for gRPC
 // (gofr_proto_encode_nested_device): proto.Marshal for responses that are not flat — nested messages (a presence word

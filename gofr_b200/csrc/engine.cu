@@ -59,6 +59,8 @@ __global__ void proto_encode_kernel(const GrpcParams p, const ProtoSchema S);
 __global__ void proto_decode_kernel(const GrpcParams p, const ProtoSchema S);
 __global__ void proto_encode_nested_kernel(const GrpcParams p, const PbnDesc D);  // proto_nested_kernel.cu
 __global__ void proto_decode_nested_kernel(const GrpcParams p, const PbnDesc D);  // proto_nested_decode_kernel.cu
+__global__ void proto_encode_nested_maps_kernel(const GrpcParams p, const PbnDesc D);  // proto_nested_maps_kernel.cu: the
+__global__ void proto_decode_nested_maps_kernel(const GrpcParams p, const PbnDesc D);  // same for descriptions with maps
 __global__ void reqlog_kernel(const LogParams p);                // reqlog_kernel.cu
 __global__ void http_parse_kernel(const HttpParams p);           // http_kernel.cu
 __global__ void route_kernel(const RouteParams p);               // route_kernel.cu
@@ -69,7 +71,7 @@ namespace {
 
 enum Kern {
     K_SERVE, K_SERVE_VALUES, K_SLOTS, K_SLOTS_WIDE, K_SLOTS_VALUES, K_HELLO, K_PROTO_ENC, K_PROTO_DEC, K_PBN_ENC, K_PBN_DEC,
-    K_REQLOG, K_HTTP, K_ROUTE, K_BIND, K_COUNT
+    K_PBN_ENC_MAPS, K_PBN_DEC_MAPS, K_REQLOG, K_HTTP, K_ROUTE, K_BIND, K_COUNT
 };
 struct KernelRec {
     const void* fn;
@@ -87,6 +89,8 @@ const KernelRec kKernels[K_COUNT] = {
     {(const void*)proto_decode_kernel, "proto", kServeThreads},
     {(const void*)proto_encode_nested_kernel, "proto", kServeThreads},
     {(const void*)proto_decode_nested_kernel, "proto", kServeThreads},
+    {(const void*)proto_encode_nested_maps_kernel, "proto", kServeThreads},
+    {(const void*)proto_decode_nested_maps_kernel, "proto", kServeThreads},
     {(const void*)reqlog_kernel, "request-log", kServeThreads},
     {(const void*)http_parse_kernel, "http", kServeThreads},
     {(const void*)route_kernel, "route", kRouteThreads},
@@ -1114,7 +1118,7 @@ static int pbn_build(const gofr_proto_nmsg* msgs, uint32_t n_msgs, const gofr_pr
         return GOFR_ERR_CAPACITY;
     }
     memset(D, 0, sizeof *D);
-    D->n_msgs = n_msgs;
+    D->n_msgs = (uint16_t)n_msgs;
     D->root = root;
     for (uint32_t m = 0; m < n_msgs; m++) {
         if (msgs[m].n_fields == 0 || (uint32_t)msgs[m].first_field + msgs[m].n_fields > n_fields) { set_last_error("message type %u: bad field range", m); return GOFR_ERR_INVALID; }
@@ -1124,18 +1128,55 @@ static int pbn_build(const gofr_proto_nmsg* msgs, uint32_t n_msgs, const gofr_pr
             const gofr_proto_nfield& f = fields[msgs[m].first_field + k];
             const uint32_t num = f.number, t = f.type;
             const bool scalar = (t >= GOFR_PB_DOUBLE && t <= GOFR_PB_STRING) || (t >= GOFR_PB_BYTES && t <= GOFR_PB_SINT64);
-            if (!scalar && t != GOFR_PB_MESSAGE) { set_last_error("message type %u field %u: type %u is not taken", m, num, t); return GOFR_ERR_UNSUPPORTED; }
-            if (t == GOFR_PB_MESSAGE && f.msg >= n_msgs) { set_last_error("message type %u field %u: unknown message type %u", m, num, f.msg); return GOFR_ERR_INVALID; }
+            const bool sub = t == GOFR_PB_MESSAGE || t == GOFR_PB_MAP;
+            if (!scalar && !sub) { set_last_error("message type %u field %u: type %u is not taken", m, num, t); return GOFR_ERR_UNSUPPORTED; }
+            if (sub && f.msg >= n_msgs) { set_last_error("message type %u field %u: unknown message type %u", m, num, f.msg); return GOFR_ERR_INVALID; }
+            if (t == GOFR_PB_MAP && f.repeated) { set_last_error("message type %u field %u: a map field is not repeated", m, num); return GOFR_ERR_INVALID; }
             if (num == 0 || num > 0x1FFFFFFFu || (num >= 19000 && num <= 19999)) { set_last_error("field number %u is not valid", num); return GOFR_ERR_INVALID; }
             if (k && num <= fields[msgs[m].first_field + k - 1].number) { set_last_error("message type %u: fields must be in ascending field-number order", m); return GOFR_ERR_INVALID; }
             PbnField& F = D->f[msgs[m].first_field + k];
-            F.repeated = f.repeated ? 1 : 0;
-            F.msg = t == GOFR_PB_MESSAGE ? (uint8_t)f.msg : (uint8_t)0xFF;
-            F.cls = t == GOFR_PB_MESSAGE ? 0 : (uint8_t)proto_class(t);
-            // messages, strings, bytes and PACKED repeated scalars are length-delimited
-            const uint32_t wire = (t == GOFR_PB_MESSAGE || (f.repeated && proto_wire(t) != 2)) ? 2u : proto_wire(t);
+            F.flags = t == GOFR_PB_MAP ? (uint8_t)(PBN_REPEATED | PBN_MAP) : f.repeated ? (uint8_t)PBN_REPEATED : (uint8_t)0;
+            F.msg = sub ? (uint8_t)f.msg : (uint8_t)0xFF;
+            F.cls = sub ? 0 : (uint8_t)proto_class(t);
+            // messages, map entries, strings, bytes and PACKED repeated scalars are length-delimited
+            const uint32_t wire = (sub || (f.repeated && proto_wire(t) != 2)) ? 2u : proto_wire(t);
             F.tag = num << 3 | wire;
         }
+    }
+    // map entry types: exactly (1 key, 2 value), singular; keys of integer, bool or string type; values anything but a map.
+    // An entry type is neither the root nor the type of a message field.
+    bool entry[kPbnMaxMsgs] = {false};
+    for (uint32_t m = 0; m < n_msgs; m++)
+        for (uint32_t k = 0; k < msgs[m].n_fields; k++)
+            if (fields[msgs[m].first_field + k].type == GOFR_PB_MAP) entry[fields[msgs[m].first_field + k].msg] = true;
+    for (uint32_t m = 0; m < n_msgs; m++) {
+        for (uint32_t k = 0; k < msgs[m].n_fields; k++) {
+            const gofr_proto_nfield& f = fields[msgs[m].first_field + k];
+            if (f.type == GOFR_PB_MESSAGE && entry[f.msg]) { set_last_error("message type %u field %u: map entry type %u used as a message", m, f.number, f.msg); return GOFR_ERR_INVALID; }
+        }
+        if (!entry[m]) continue;
+        D->maps = 1;
+        if (m == root) { set_last_error("the root type %u is a map entry type", m); return GOFR_ERR_INVALID; }
+        // the entry's key and value are marked in the shared field table: no other type may name them
+        for (uint32_t o = 0; o < n_msgs; o++) {
+            const uint32_t a0 = msgs[m].first_field, a1 = a0 + msgs[m].n_fields, b0 = msgs[o].first_field, b1 = b0 + msgs[o].n_fields;
+            if (o != m && a0 < b1 && b0 < a1) { set_last_error("map entry type %u shares fields with message type %u", m, o); return GOFR_ERR_INVALID; }
+        }
+        const gofr_proto_nfield* kv = fields + msgs[m].first_field;
+        if (msgs[m].n_fields != 2 || kv[0].number != 1 || kv[1].number != 2 || kv[0].repeated || kv[1].repeated) {
+            set_last_error("map entry type %u: exactly the singular fields 1 (key) and 2 (value)", m);
+            return GOFR_ERR_INVALID;
+        }
+        const uint32_t kt = kv[0].type;
+        const bool key_ok = kt == GOFR_PB_INT32 || kt == GOFR_PB_INT64 || kt == GOFR_PB_UINT32 || kt == GOFR_PB_UINT64 || kt == GOFR_PB_SINT32 ||
+                            kt == GOFR_PB_SINT64 || kt == GOFR_PB_FIXED32 || kt == GOFR_PB_FIXED64 || kt == GOFR_PB_SFIXED32 ||
+                            kt == GOFR_PB_SFIXED64 || kt == GOFR_PB_BOOL || kt == GOFR_PB_STRING;
+        if (!key_ok) { set_last_error("map entry type %u: a key of type %u", m, kt); return GOFR_ERR_INVALID; }
+        if (kv[1].type == GOFR_PB_MAP) { set_last_error("map entry type %u: a map-valued map", m); return GOFR_ERR_INVALID; }
+        const bool signed_key = kt == GOFR_PB_INT32 || kt == GOFR_PB_INT64 || kt == GOFR_PB_SINT32 || kt == GOFR_PB_SINT64 ||
+                                kt == GOFR_PB_SFIXED32 || kt == GOFR_PB_SFIXED64;
+        D->f[D->first[m]].flags |= (uint8_t)(PBN_ENTRY | (signed_key ? PBN_SIGNED : 0));
+        D->f[D->first[m] + 1].flags |= (uint8_t)PBN_ENTRY;
     }
     // fixed words and depth, depth first; a message type that reaches itself has no bound on its nesting
     int state[kPbnMaxMsgs] = {0}, depth[kPbnMaxMsgs] = {0};
@@ -1147,12 +1188,12 @@ static int pbn_build(const gofr_proto_nmsg* msgs, uint32_t n_msgs, const gofr_pr
         int d = 1;
         for (uint32_t k = 0; k < D->count[m]; k++) {
             PbnField& F = D->f[D->first[m] + k];
-            uint32_t w = F.repeated ? 1u : (F.cls & PC_64) ? 2u : 1u;
+            uint32_t w = (F.flags & PBN_REPEATED) ? 1u : (F.cls & PC_64) ? 2u : 1u;
             if (F.msg != 0xFF) {
                 int rc = visit(F.msg);
                 if (rc) return rc;
                 d = std::max(d, 1 + depth[F.msg]);
-                if (!F.repeated) w = 1u + D->fixed_words[F.msg];
+                if (!(F.flags & PBN_REPEATED)) w = 1u + D->fixed_words[F.msg];
             }
             if (w > 255u) { set_last_error("message type %u: fixed part too wide", m); return GOFR_ERR_UNSUPPORTED; }
             F.fixed_words = (uint8_t)w;
@@ -1178,7 +1219,8 @@ static int proto_nested_run(gofr_engine* e, const gofr_proto_nmsg* msgs, uint32_
     GrpcParams p;
     memset(&p, 0, sizeof p);
     p.in = d_in; p.in_off = d_in_off; p.meta = d_meta;
-    return launch_frames(e, decode ? K_PBN_DEC : K_PBN_ENC, p, n, d_out, out_cap, d_out_off, stream, D);
+    const Kern k = D.maps ? (decode ? K_PBN_DEC_MAPS : K_PBN_ENC_MAPS) : (decode ? K_PBN_DEC : K_PBN_ENC);  // map-free: no map code
+    return launch_frames(e, k, p, n, d_out, out_cap, d_out_off, stream, D);
 }
 
 int gofr_proto_encode_nested_device(gofr_engine* e, const gofr_proto_nmsg* msgs, uint32_t n_msgs, const gofr_proto_nfield* fields,

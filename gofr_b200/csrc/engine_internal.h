@@ -92,17 +92,27 @@ struct GrpcParams {
 // message types of gofr_proto_encode_nested_device (kernel parameter, by value): up to 8 message types with 48 fields in
 // all; fields of a type are consecutive, in ascending field-number order.  Rows use the layout of the wider data model
 // (include/gofr_b200.h "Row format"): a singular message field is a presence word + the message's fixed part inline, a
-// repeated field a count word with its elements in the variable part.
-constexpr int kPbnMaxMsgs = 8, kPbnMaxFields = 48, kPbnMaxDepth = 4;
+// repeated field a count word with its elements in the variable part.  A map field is laid out (and written) as a repeated
+// message field of its entry type; the decoder takes at most kPbnMaxMapEntries entries of one map field in one message
+// (selection of the canonical order is quadratic) and answers GOFR_GRPC_DEFER beyond that.
+constexpr int kPbnMaxMsgs = 8, kPbnMaxFields = 48, kPbnMaxDepth = 4, kPbnMaxMapEntries = 64;
+enum : uint8_t {
+    PBN_REPEATED = 1u,  // a count word in the fixed part, the elements in the variable part (map fields too)
+    PBN_MAP = 2u,       // a map field (GOFR_PB_MAP; always with PBN_REPEATED): entries in ascending key order
+    PBN_ENTRY = 4u,     // the key or value of a map entry type: written even at its zero value, a value message always
+    PBN_SIGNED = 8u,    // an entry's key of a signed integer type (key order)
+};
 struct PbnField {
     uint32_t tag;        // number << 3 | wire type (2 for messages and for packed repeated scalars)
     uint8_t cls;         // PC_* bits of the scalar type; 0 for a message
-    uint8_t repeated;
-    uint8_t msg;         // message type index (type GOFR_PB_MESSAGE), else 0xFF
+    uint8_t flags;       // PBN_* bits
+    uint8_t msg;         // message type index (type GOFR_PB_MESSAGE), the entry type of a map field, else 0xFF
     uint8_t fixed_words; // words the field owns in the fixed part of its message
 };
 struct PbnDesc {
-    uint32_t n_msgs, root;
+    uint16_t n_msgs;
+    uint16_t maps;  // the description has map fields: the *_maps kernels run it (map-free types keep the plain kernels)
+    uint32_t root;
     uint16_t first[kPbnMaxMsgs], count[kPbnMaxMsgs], fixed_words[kPbnMaxMsgs];
     PbnField f[kPbnMaxFields];
 };

@@ -10,7 +10,12 @@
 //   * a singular message field occurring more than once is MERGED by protobuf-go; that is not done here: the frame comes
 //     back with GOFR_GRPC_DEFER ("valid, but decode it on the host") — canonical encoders write the field once;
 //   * repeated strings / bytes / messages: one element per occurrence, in wire order; unknown fields and balanced groups
-//     are skipped at every level; nested messages are only parsed where the schema knows them.
+//     are skipped at every level; nested messages are only parsed where the schema knows them;
+//   * map fields (codec_map.go): each occurrence is an entry message, decoded like any message (last key and value win, a
+//     value message sent twice is merged -> DEFER as above); across entries a later equal key replaces the earlier entry.
+//     The row holds the map in the encoder's canonical form: keys ascending, each once.  The walks find it by SELECTION —
+//     per output slot, the smallest key above the previous one among all entries, the last entry carrying it — no scratch,
+//     quadratic, so more than kPbnMaxMapEntries entries of one map field in one message (duplicates counted) are DEFER.
 // Three walks per frame, none recursive (explicit stacks, at most kPbnMaxDepth message levels):
 //   validate   wire order: framing of every level that the schema knows, UTF-8, packed payloads, repeated singular messages
 //   size       field order: the row's byte count
@@ -79,17 +84,85 @@ GOFR_HD bool pdn_next(const uint8_t* f, uint32_t* ip, uint32_t hi, PdnItem* it) 
 }
 
 // the field of message type mt that a (number, wire type) addresses, or -1: same number, and the field's own wire type or —
-// for a repeated numeric scalar — either its element wire type or 2 (packed)
+// for a repeated numeric scalar — either its element wire type or 2 (packed).  (MAPS == false: a map-free description,
+// whose flag bytes hold PBN_REPEATED alone)
+template <bool MAPS = true>
 GOFR_HD int pdn_field_of(const PbnDesc& D, uint32_t mt, uint32_t num, uint32_t wt) {
     const PbnField* F = D.f + D.first[mt];
     for (uint32_t q = 0; q < D.count[mt]; q++) {
         if ((F[q].tag >> 3) != num) continue;
         const uint32_t own = F[q].msg != 0xFF ? 2u : (uint32_t)(F[q].cls & PC_WIRE);
         if (wt == own) return (int)q;
-        if (F[q].repeated && F[q].msg == 0xFF && own != 2u && wt == 2u) return (int)q;  // packed
+        if ((MAPS ? (F[q].flags & PBN_REPEATED) : F[q].flags) && F[q].msg == 0xFF && own != 2u && wt == 2u) return (int)q;  // packed
         return -1;
     }
     return -1;
+}
+
+// top-level items of [i, hi) (a message of type mt; unknown groups skipped whole) that address field q: how many — stops
+// early at malformed bytes, which the validating walk reports anyway
+GOFR_HD uint32_t pdn_count_after(const PbnDesc& D, const uint8_t* f, uint32_t i, uint32_t hi, uint32_t mt, uint32_t q) {
+    uint32_t n = 0, g = 0;
+    while (i < hi) {
+        PdnItem it;
+        if (!pdn_next(f, &i, hi, &it)) break;
+        if (it.wt == 3) { g++; continue; }
+        if (it.wt == 4) { if (!g) break; g--; continue; }
+        if (!g && pdn_field_of(D, mt, it.num, it.wt) == (int)q) n++;
+    }
+    return n;
+}
+
+// A map's key in [lo, hi), the content of one entry (type E; its key is field index 0): the last occurrence, else the zero
+// value.  Integer and bool keys as pbn_key_order numbers; string keys as (offset << 32 | length) of their bytes in f.
+GOFR_HD uint64_t pdn_entry_key(const PbnDesc& D, const uint8_t* f, uint32_t lo, uint32_t hi, uint32_t E) {
+    const PbnField& K = D.f[D.first[E]];
+    const bool str = (K.cls & PC_WIRE) == 2;
+    uint64_t key = str ? 0u : pbn_key_order(K.flags, K.cls, 0u, 0u);
+    uint32_t i = lo, g = 0;
+    while (i < hi) {
+        PdnItem it;
+        pdn_next(f, &i, hi, &it);
+        if (it.wt == 3) { g++; continue; }
+        if (it.wt == 4) { g--; continue; }
+        if (g || pdn_field_of(D, E, it.num, it.wt) != 0) continue;
+        if (str) key = (uint64_t)it.poff << 32 | it.plen;
+        else {
+            uint32_t w0, w1;
+            pdn_scalar_words(K.cls, it.wt, it.v, &w0, &w1);
+            key = pbn_key_order(K.flags, K.cls, w0, w1);
+        }
+    }
+    return key;
+}
+GOFR_HD bool pdn_key_less(const uint8_t* f, bool str, uint64_t a, uint64_t b) {
+    if (!str) return a < b;
+    return pbn_bytes_cmp(f + (a >> 32), (uint32_t)a, f + (b >> 32), (uint32_t)b) < 0;
+}
+
+// The next entry of map field q (entry type E) of the message [lo, hi) of type mt in canonical order, by selection: the
+// smallest key above *key (any key when !have_key), the last entry on the wire that carries it.  False when there is none.
+GOFR_HD bool pdn_map_next(const PbnDesc& D, const uint8_t* f, uint32_t lo, uint32_t hi, uint32_t mt, uint32_t q, uint32_t E,
+                          bool have_key, uint64_t* key, PdnItem* out) {
+    const bool str = (D.f[D.first[E]].cls & PC_WIRE) == 2;
+    bool found = false;
+    uint64_t best = 0;
+    uint32_t i = lo, g = 0;
+    while (i < hi) {
+        PdnItem it;
+        pdn_next(f, &i, hi, &it);
+        if (it.wt == 3) { g++; continue; }
+        if (it.wt == 4) { g--; continue; }
+        if (g || pdn_field_of(D, mt, it.num, it.wt) != (int)q) continue;
+        const uint64_t k = pdn_entry_key(D, f, it.poff, it.poff + it.plen, E);
+        if (have_key && !pdn_key_less(f, str, *key, k)) continue;  // not above the previous key
+        if (found && pdn_key_less(f, str, best, k)) continue;      // above the best so far
+        best = k;                                                  // smaller, or equal and later on the wire: this one
+        *out = it;
+        found = true;
+    }
+    if (found) *key = best;
+    return found;
 }
 
 // elements of a packed payload [lo, hi) of class cls: count them, or fail when the payload is not a whole number of elements
@@ -110,6 +183,8 @@ GOFR_HD bool pdn_packed_count(const uint8_t* f, uint32_t lo, uint32_t hi, uint32
 }
 
 // ---- walk 1: validate, in wire order ----
+// (MAPS == false: the instance for descriptions without map fields, as for the walks below)
+template <bool MAPS>
 GOFR_HD_NOINLINE uint32_t pdn_validate(const PbnDesc& D, const uint8_t* f, uint32_t lo, uint32_t hi) {
     struct Lv { uint32_t end; uint64_t seen; uint8_t mt; uint8_t gbase; } lv[kPbnMaxDepth + 1];
     uint32_t groups[kMaxGroupDepth];
@@ -137,13 +212,16 @@ GOFR_HD_NOINLINE uint32_t pdn_validate(const PbnDesc& D, const uint8_t* f, uint3
             continue;
         }
         if (gdepth != L.gbase) continue;  // inside an unknown group: nothing is known
-        const int q = pdn_field_of(D, L.mt, it.num, it.wt);
+        const int q = pdn_field_of<MAPS>(D, L.mt, it.num, it.wt);
         if (q < 0) continue;
         const PbnField& F = D.f[D.first[L.mt] + (uint32_t)q];
         if (F.msg != 0xFF) {
-            if (!F.repeated) {
+            if (!(MAPS ? (F.flags & PBN_REPEATED) : F.flags)) {
                 if (L.seen >> q & 1u) defer = true;
                 L.seen |= 1ull << q;
+            } else if (MAPS && (F.flags & PBN_MAP) && !(L.seen >> q & 1u)) {  // first entry of a map field: count them all once
+                L.seen |= 1ull << q;
+                if (1u + pdn_count_after(D, f, i, L.end, L.mt, (uint32_t)q) > (uint32_t)kPbnMaxMapEntries) defer = true;
             }
             if (depth > kPbnMaxDepth) return GOFR_GRPC_BAD_PROTO;  // cannot happen: the schema's depth was checked
             i = it.poff;  // descend: the payload is parsed as a message of type F.msg
@@ -162,9 +240,12 @@ GOFR_HD void pdn_st32(uint8_t* p, uint32_t v) { p[0] = (uint8_t)v; p[1] = (uint8
 
 // ---- walks 2 and 3: field order; EMIT stores into row[] ----
 // Returns the row's byte count before padding.  The frame has been validated: no check can fail here.
-template <bool EMIT>
+template <bool EMIT, bool MAPS>
 GOFR_HD_NOINLINE uint32_t pdn_walk(const PbnDesc& D, const uint8_t* f, uint32_t lo, uint32_t hi, uint8_t* row) {
+    // in_rep: 1 elements of a repeated message field in wire order (scan: where to look on), 2 / 3 entries of a map field in
+    // key order (3: keys[frame] = the key of the entry taken last)
     struct Fr { uint32_t lo, hi, fx, scan; uint8_t mt, fi, in_rep; } st[kPbnMaxDepth + 1];
+    uint64_t keys[kPbnMaxDepth + 1];
     int depth = 0;
     uint32_t vc = (uint32_t)D.fixed_words[D.root] * 4u;  // append position of the variable part
     st[0].lo = lo; st[0].hi = hi; st[0].fx = 0; st[0].scan = 0; st[0].mt = (uint8_t)D.root; st[0].fi = 0; st[0].in_rep = 0;
@@ -178,7 +259,7 @@ GOFR_HD_NOINLINE uint32_t pdn_walk(const PbnDesc& D, const uint8_t* f, uint32_t 
             if (it.wt == 3) { g++; continue; }
             if (it.wt == 4) { g--; continue; }
             if (g) continue;
-            if (pdn_field_of(D, mt, it.num, it.wt) == (int)q) { *out = it; *ip = i; return true; }
+            if (pdn_field_of<MAPS>(D, mt, it.num, it.wt) == (int)q) { *out = it; *ip = i; return true; }
         }
         *ip = i;
         return false;
@@ -186,10 +267,16 @@ GOFR_HD_NOINLINE uint32_t pdn_walk(const PbnDesc& D, const uint8_t* f, uint32_t 
     while (depth > 0) {
         Fr& fr = st[depth - 1];
         const PbnField* fields = D.f + D.first[fr.mt];
-        if (fr.in_rep) {  // repeated message field fr.fi - 1: the next occurrence becomes the next element
+        if (fr.in_rep) {  // repeated message field fr.fi - 1: the next occurrence (the next entry of a map) is the next element
             const PbnField& F = fields[fr.fi - 1];
             PdnItem it;
-            if (find(fr.mt, fr.fi - 1u, &fr.scan, fr.hi, &it)) {
+            bool more;
+            if (!MAPS || fr.in_rep == 1) more = find(fr.mt, fr.fi - 1u, &fr.scan, fr.hi, &it);
+            else {
+                more = pdn_map_next(D, f, fr.lo, fr.hi, fr.mt, fr.fi - 1u, F.msg, fr.in_rep == 3, &keys[depth - 1], &it);
+                fr.in_rep = 3;
+            }
+            if (more) {
                 const uint32_t efx = vc;
                 vc += (uint32_t)D.fixed_words[F.msg] * 4u;
                 Fr& ch = st[depth++];
@@ -207,11 +294,12 @@ GOFR_HD_NOINLINE uint32_t pdn_walk(const PbnDesc& D, const uint8_t* f, uint32_t 
         const uint32_t cls = F.cls;
         PdnItem it;
         uint32_t i = fr.lo;
-        if (!F.repeated) {
+        if (!(MAPS ? (F.flags & PBN_REPEATED) : F.flags)) {
             if (F.msg != 0xFF) {  // singular message: presence word + its fixed part inline (zeros when absent)
+                // (a map value is always present: a missing one is an empty message)
                 const bool present = find(fr.mt, q, &i, fr.hi, &it);
                 if (EMIT) {
-                    pdn_st32(row + fxo, present ? 1u : 0u);
+                    pdn_st32(row + fxo, present || (MAPS && (F.flags & PBN_ENTRY)) ? 1u : 0u);
                     if (!present) for (uint32_t k = 0; k < (uint32_t)D.fixed_words[F.msg] * 4u; k++) row[fxo + 4u + k] = 0;
                 }
                 if (present) {
@@ -234,7 +322,13 @@ GOFR_HD_NOINLINE uint32_t pdn_walk(const PbnDesc& D, const uint8_t* f, uint32_t 
             continue;
         }
         // repeated: the count word, the elements appended
-        if (F.msg != 0xFF) {
+        if (MAPS && (F.flags & PBN_MAP)) {  // the distinct keys
+            uint32_t n = 0;
+            uint64_t key = 0;
+            while (pdn_map_next(D, f, fr.lo, fr.hi, fr.mt, q, F.msg, n != 0, &key, &it)) n++;
+            if (EMIT) pdn_st32(row + fxo, n);
+            if (n) fr.in_rep = 2;
+        } else if (F.msg != 0xFF) {
             uint32_t n = 0;
             while (find(fr.mt, q, &i, fr.hi, &it)) n++;
             if (EMIT) pdn_st32(row + fxo, n);
@@ -287,25 +381,36 @@ GOFR_HD_NOINLINE uint32_t pdn_walk(const PbnDesc& D, const uint8_t* f, uint32_t 
     return vc;
 }
 
-// size pass of one frame
-GOFR_HD PdnRow pdn_decode_size(const PbnDesc& D, const uint8_t* f, uint32_t fn) {
+// size pass of one frame.  The kernels instantiate it for MAPS == D.maps (one kernel per choice, picked on the host: the
+// map-free kernel contains no map code); pdn_decode_size dispatches at run time.
+template <bool MAPS>
+GOFR_HD PdnRow pdn_decode_size_as(const PbnDesc& D, const uint8_t* f, uint32_t fn) {
     PdnRow r = {GOFR_GRPC_OK, 0};
     if (fn < 5) { r.status = GOFR_GRPC_BAD_LENGTH; return r; }
     if (f[0] == 1) { r.status = GOFR_GRPC_COMPRESSED; return r; }
     if (f[0] != 0) { r.status = GOFR_GRPC_BAD_LENGTH; return r; }
     const uint32_t L = (uint32_t)f[1] << 24 | (uint32_t)f[2] << 16 | (uint32_t)f[3] << 8 | f[4];
     if (L != fn - 5) { r.status = GOFR_GRPC_BAD_LENGTH; return r; }
-    r.status = pdn_validate(D, f, 5, 5 + L);
+    r.status = pdn_validate<MAPS>(D, f, 5, 5 + L);
     if (r.status != GOFR_GRPC_OK) return r;
-    r.out_len = (pdn_walk<false>(D, f, 5, 5 + L, nullptr) + 3u) & ~3u;
+    r.out_len = (pdn_walk<false, MAPS>(D, f, 5, 5 + L, nullptr) + 3u) & ~3u;
     return r;
 }
 
 // emit pass: the row at dst (4-byte aligned: every row is a multiple of 4 bytes long)
-GOFR_HD void pdn_decode_emit(const PbnDesc& D, const uint8_t* f, uint32_t fn, const PdnRow r, uint8_t* dst) {
+template <bool MAPS>
+GOFR_HD void pdn_decode_emit_as(const PbnDesc& D, const uint8_t* f, uint32_t fn, const PdnRow r, uint8_t* dst) {
     if (!r.out_len) return;
-    uint32_t end = pdn_walk<true>(D, f, 5, fn, dst);
+    uint32_t end = pdn_walk<true, MAPS>(D, f, 5, fn, dst);
     for (; end < r.out_len; end++) dst[end] = 0;
+}
+
+GOFR_HD PdnRow pdn_decode_size(const PbnDesc& D, const uint8_t* f, uint32_t fn) {
+    return D.maps ? pdn_decode_size_as<true>(D, f, fn) : pdn_decode_size_as<false>(D, f, fn);
+}
+GOFR_HD void pdn_decode_emit(const PbnDesc& D, const uint8_t* f, uint32_t fn, const PdnRow r, uint8_t* dst) {
+    if (D.maps) pdn_decode_emit_as<true>(D, f, fn, r, dst);
+    else pdn_decode_emit_as<false>(D, f, fn, r, dst);
 }
 
 }  // namespace gofr

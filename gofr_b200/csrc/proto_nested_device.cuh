@@ -9,8 +9,10 @@
 //   * repeated scalars of numeric type are PACKED: one tag (wire type 2), the payload length, the elements back to back —
 //     nothing at all for zero elements; repeated strings / bytes / messages: one tag + length + payload PER ELEMENT,
 //     empty elements included;
-//   * map fields are not modelled: protobuf-go writes them in Go's random map order unless Deterministic is set, so there
-//     is no byte sequence to be identical to.
+//   * map fields (codec_map.go) are repeated entry messages (1 key, 2 value) whose key and value are written even at their
+//     zero value, a message value always (tag + length 0 when it is nil).  protobuf-go writes entries in Go's random map
+//     order unless Deterministic is set, which sorts the keys; the row carries the entries in that order (checked: strictly
+//     ascending keys, else BAD_ROW), so the bytes are the Deterministic ones.
 // Rows use the layout of the wider data model (include/gofr_b200.h "Row format"): fixed words of a message in field order
 // (64-bit kinds two words, string / bytes their length, a singular message a presence word + its own fixed part inline, a
 // repeated field its element count), then the variable part in field order (string bytes; a set message's variable part;
@@ -30,14 +32,39 @@ struct PbnFrame {
     uint8_t mt, fi;        // message type, next field (index inside the type)
     uint8_t pend_tl;       // SIZE walk: tag length of the message field whose content the child frame is sizing
 };
+// SIZE walk, per frame with a map field in progress: the key of the entry seen last (kept apart from PbnFrame: the
+// emitting walk, and message types without maps, never touch it)
+struct PbnKey {
+    uint64_t key;          // its order key (pbn_key_order), or for a string key:
+    const uint8_t* s;      //     its bytes in the row
+    uint32_t n;
+    uint32_t have;         // an entry has been seen
+};
 
 GOFR_HD uint32_t pbn_ld32(const uint8_t* p) { return (uint32_t)p[0] | (uint32_t)p[1] << 8 | (uint32_t)p[2] << 16 | (uint32_t)p[3] << 24; }
+
+// map keys: the row words of an integer or bool key as a number whose unsigned order is the key order (bool false < true,
+// signed kinds signed, unsigned kinds unsigned) — encoder and decoder compare through it
+GOFR_HD uint64_t pbn_key_order(uint32_t flags, uint32_t cls, uint32_t w0, uint32_t w1) {
+    if (cls & PC_BOOL) return w0 ? 1u : 0u;
+    if (!(flags & PBN_SIGNED)) return (uint64_t)w0 | (uint64_t)((cls & PC_64) ? w1 : 0u) << 32;
+    const uint64_t v = (cls & PC_64) ? ((uint64_t)w0 | (uint64_t)w1 << 32) : (uint64_t)(int64_t)(int32_t)w0;
+    return v ^ 0x8000000000000000ull;
+}
+// string keys: Go's <, byte order with a shorter prefix first.  <0, 0, >0
+GOFR_HD int pbn_bytes_cmp(const uint8_t* a, uint32_t an, const uint8_t* b, uint32_t bn) {
+    const uint32_t n = an < bn ? an : bn;
+    for (uint32_t i = 0; i < n; i++)
+        if (a[i] != b[i]) return a[i] < b[i] ? -1 : 1;
+    return an < bn ? -1 : an > bn ? 1 : 0;
+}
 
 // One walk over message type `mt` whose fixed part is at `fixed` and whose variable part starts at *var (end = end of the
 // row).  EMIT == false: returns the size of the message's content, validates the row (*status: GOFR_GRPC_BAD_ROW /
 // GOFR_GRPC_BAD_UTF8) and advances *var past the message's variable part.  EMIT == true: writes the content through w
-// (the row has been validated by the sizing walk of the whole row).
-template <bool EMIT>
+// (the row has been validated by the sizing walk of the whole row).  MAPS == false: the instance for descriptions without
+// map fields, with no map code in it.
+template <bool EMIT, bool MAPS>
 GOFR_HD_NOINLINE uint32_t pbn_walk(const PbnDesc& D, uint32_t mt, const uint8_t* fixed, const uint8_t** var_io, const uint8_t* end,
                                    Writer* w, uint32_t* status) {
     PbnFrame st[kPbnMaxDepth + 1];
@@ -54,6 +81,23 @@ GOFR_HD_NOINLINE uint32_t pbn_walk(const PbnDesc& D, uint32_t mt, const uint8_t*
         if (depth > kPbnMaxDepth) { err = GOFR_GRPC_BAD_ROW; return; }
         PbnFrame& f = st[depth++];
         f.fixed = fx; f.size = 0; f.rep_left = 0; f.mt = (uint8_t)m; f.fi = 0; f.pend_tl = 0;
+    };
+    PbnKey keys[kPbnMaxDepth + 1];
+    // SIZE walk, the key of a map entry (frame fi; the map's frame is fi - 1): strictly above the previous entry's key
+    auto key_in_order = [&](int fi, const PbnField& K, const uint8_t* p, const uint8_t* s) -> bool {
+        PbnKey& M = keys[fi - 1];
+        bool ok;
+        if ((K.cls & PC_WIRE) == 2) {
+            const uint32_t n = pbn_ld32(p);
+            ok = !M.have || pbn_bytes_cmp(M.s, M.n, s, n) < 0;
+            M.s = s; M.n = n;
+        } else {
+            const uint64_t k = pbn_key_order(K.flags, K.cls, pbn_ld32(p), (K.cls & PC_64) ? pbn_ld32(p + 4) : 0u);
+            ok = !M.have || M.key < k;
+            M.key = k;
+        }
+        M.have = 1;
+        return ok;
     };
     auto put_varint = [&](uint64_t v) { w->reserve(3); proto_put_varint(*w, v); };
     // a scalar payload (what follows the tag) of class cls whose words are at p: its encoded length, written when EMIT
@@ -72,7 +116,7 @@ GOFR_HD_NOINLINE uint32_t pbn_walk(const PbnDesc& D, uint32_t mt, const uint8_t*
         if constexpr (EMIT) {  // (constexpr: the sizing instance must not contain a call to itself)
             const uint8_t* v2 = var;
             uint32_t st2 = GOFR_GRPC_OK;
-            const uint32_t sub = pbn_walk<false>(D, F.msg, fx, &v2, end, nullptr, &st2);
+            const uint32_t sub = pbn_walk<false, MAPS>(D, F.msg, fx, &v2, end, nullptr, &st2);
             put_varint(F.tag);
             put_varint(sub);
         } else st[parent].pend_tl = (uint8_t)varint_len(F.tag);
@@ -104,21 +148,31 @@ GOFR_HD_NOINLINE uint32_t pbn_walk(const PbnDesc& D, uint32_t mt, const uint8_t*
         const uint8_t* p = st[fi].fixed + (size_t)wo * 4;
         st[fi].fi++;
         const uint32_t tl = varint_len(F.tag), cls = F.cls, wire = cls & PC_WIRE;
-        if (!F.repeated) {
+        // (a map-free description has no flag bits but PBN_REPEATED: its instance tests the byte, as before maps)
+        if (!(MAPS ? (F.flags & PBN_REPEATED) : F.flags)) {
+            // the key or value of a map entry: written at its zero value too; the key (field index 0) in order (SIZE walk of
+            // the whole row: the entry's frame has its map's frame below it)
+            const bool entry = MAPS && (F.flags & PBN_ENTRY), is_key = !EMIT && entry && st[fi].fi == 1 && fi > 0;
             if (F.msg != 0xFF) {  // singular message: presence word, then the fixed part inline
                 if (pbn_ld32(p)) enter_message(F, p + 4, fi);
+                else if (entry) {  // a nil map value is written as an empty message
+                    if (EMIT) { put_varint(F.tag); put_varint(0); }
+                    st[fi].size += tl + 1;
+                }
             } else if (wire == 2) {  // string / bytes
                 const uint32_t len = pbn_ld32(p);
                 const uint8_t* s = take(len);
                 if (!s) break;
                 if (!EMIT && (cls & PC_UTF8) && !proto_utf8_ok(s, len)) { err = GOFR_GRPC_BAD_UTF8; break; }
-                if (len) {
-                    if (EMIT) { put_varint(F.tag); put_varint(len); w->copy<false>(s, len); }
+                if (is_key && !key_in_order(fi, F, p, s)) { err = GOFR_GRPC_BAD_ROW; break; }
+                if (len || entry) {
+                    if (EMIT) { put_varint(F.tag); put_varint(len); if (len) w->copy<false>(s, len); }
                     st[fi].size += tl + varint_len(len) + len;
                 }
             } else {
                 const uint32_t w0 = pbn_ld32(p), w1 = (cls & PC_64) ? pbn_ld32(p + 4) : 0u;
-                if (w0 | w1) {
+                if (is_key && !key_in_order(fi, F, p, nullptr)) { err = GOFR_GRPC_BAD_ROW; break; }
+                if ((w0 | w1) || entry) {
                     if (EMIT) put_varint(F.tag);
                     st[fi].size += tl + scalar(cls, p);
                 }
@@ -126,10 +180,11 @@ GOFR_HD_NOINLINE uint32_t pbn_walk(const PbnDesc& D, uint32_t mt, const uint8_t*
             continue;
         }
         const uint32_t n = pbn_ld32(p);
-        if (F.msg != 0xFF) {  // repeated messages: one after the other through the frame's rep_left
+        if (F.msg != 0xFF) {  // repeated messages and map entries: one after the other through the frame's rep_left
             if ((uint32_t)(end - var) / 4u < n && D.fixed_words[F.msg]) { err = GOFR_GRPC_BAD_ROW; break; }
             if (n > 0x00FFFFFFu) { err = GOFR_GRPC_BAD_ROW; break; }
             st[fi].rep_left = n;
+            if (!EMIT && MAPS && (F.flags & PBN_MAP)) keys[fi].have = 0;
         } else if (wire == 2) {  // repeated string / bytes: tag + length + payload per element
             if ((uint32_t)(end - var) / 4u < n) { err = GOFR_GRPC_BAD_ROW; break; }
             for (uint32_t i = 0; i < n; i++) {
@@ -171,21 +226,24 @@ struct PbnMsg {
     uint32_t out_len;  // 5 + message bytes (0 on error)
 };
 
-// size pass of one row: validates it and returns the exact frame length
-GOFR_HD PbnMsg pbn_size(const PbnDesc& D, const uint8_t* row, uint32_t rn) {
+// size pass of one row: validates it and returns the exact frame length.  The kernels instantiate it for MAPS == D.maps
+// (one kernel per choice, picked on the host: the map-free kernel contains no map code); pbn_size dispatches at run time.
+template <bool MAPS>
+GOFR_HD PbnMsg pbn_size_as(const PbnDesc& D, const uint8_t* row, uint32_t rn) {
     PbnMsg m = {GOFR_GRPC_OK, 0};
     const uint32_t fb = (uint32_t)D.fixed_words[D.root] * 4u;
     if (rn < fb) { m.status = GOFR_GRPC_BAD_ROW; return m; }
     const uint8_t* var = row + fb;
     uint32_t st = GOFR_GRPC_OK;
-    const uint32_t len = pbn_walk<false>(D, D.root, row, &var, row + rn, nullptr, &st);
+    const uint32_t len = pbn_walk<false, MAPS>(D, D.root, row, &var, row + rn, nullptr, &st);
     m.status = st;
     m.out_len = st == GOFR_GRPC_OK ? 5u + len : 0u;
     return m;
 }
 
 // emit pass: the frame at dst (arbitrary alignment inside the packed output)
-GOFR_HD void pbn_emit(const PbnDesc& D, const uint8_t* row, uint32_t rn, const PbnMsg m, uint8_t* dst, uint32_t* stage_col) {
+template <bool MAPS>
+GOFR_HD void pbn_emit_as(const PbnDesc& D, const uint8_t* row, uint32_t rn, const PbnMsg m, uint8_t* dst, uint32_t* stage_col) {
     if (!m.out_len) return;
     Writer w;
     w.init(dst, stage_col);
@@ -194,8 +252,16 @@ GOFR_HD void pbn_emit(const PbnDesc& D, const uint8_t* row, uint32_t rn, const P
     w.putc(plen & 0xFF);
     const uint8_t* var = row + (size_t)D.fixed_words[D.root] * 4;
     uint32_t st = GOFR_GRPC_OK;
-    pbn_walk<true>(D, D.root, row, &var, row + rn, &w, &st);
+    pbn_walk<true, MAPS>(D, D.root, row, &var, row + rn, &w, &st);
     w.finish();
+}
+
+GOFR_HD PbnMsg pbn_size(const PbnDesc& D, const uint8_t* row, uint32_t rn) {
+    return D.maps ? pbn_size_as<true>(D, row, rn) : pbn_size_as<false>(D, row, rn);
+}
+GOFR_HD void pbn_emit(const PbnDesc& D, const uint8_t* row, uint32_t rn, const PbnMsg m, uint8_t* dst, uint32_t* stage_col) {
+    if (D.maps) pbn_emit_as<true>(D, row, rn, m, dst, stage_col);
+    else pbn_emit_as<false>(D, row, rn, m, dst, stage_col);
 }
 
 }  // namespace gofr

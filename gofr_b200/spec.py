@@ -388,15 +388,16 @@ def pack_proto_rows(fields: Sequence[ProtoField], messages: Sequence[Sequence]) 
 
 
 PB_MESSAGE = 11
+PB_MAP = 32          # a map field: msg is its entry type (fields 1 key, 2 value); not repeated
 
 
 @dataclass
 class ProtoNField:
     """one field of a message type with nested / repeated fields (gofr_proto_nfield)"""
     number: int
-    type: int            # PB_* or PB_MESSAGE
+    type: int            # PB_*, PB_MESSAGE or PB_MAP
     repeated: bool = False
-    msg: int = 0         # PB_MESSAGE: index of the message type
+    msg: int = 0         # PB_MESSAGE: index of the message type; PB_MAP: index of the entry type
 
 
 def proto_nested_tables(msgs: Sequence[Sequence[ProtoNField]]):
@@ -425,10 +426,24 @@ def _pb_scalar_words(t: int, v) -> bytes:
     return (int(v) & 0xFFFFFFFF).to_bytes(4, "little")
 
 
+def map_key_order(key_type: int, k):
+    """a sort key giving protobuf-go's Deterministic map order: bool false < true, signed kinds signed, unsigned kinds
+    unsigned (both as the row words hold them), strings by their UTF-8 bytes with a shorter prefix first"""
+    if key_type == PB_STRING:
+        return k.encode("utf-8", "surrogateescape") if isinstance(k, str) else bytes(k)
+    if key_type == PB_BOOL:
+        return 1 if k else 0
+    bits = 64 if key_type in PB_64BIT else 32
+    v = int(k) & ((1 << bits) - 1)
+    if key_type in (PB_INT32, PB_INT64, PB_SINT32, PB_SINT64, PB_SFIXED32, PB_SFIXED64) and v >> (bits - 1):
+        v -= 1 << bits
+    return v
+
+
 def _pb_fixed_bytes(msgs, m: int) -> int:
     n = 0
     for f in msgs[m]:
-        if f.repeated:
+        if f.repeated or f.type == PB_MAP:
             n += 4
         elif f.type == PB_MESSAGE:
             n += 4 + _pb_fixed_bytes(msgs, f.msg)
@@ -439,18 +454,25 @@ def _pb_fixed_bytes(msgs, m: int) -> int:
 
 def pack_proto_nested_message(msgs, m: int, value) -> "tuple[bytes, bytes]":
     """(fixed part, variable part) of one message of type m.  value: one entry per field — scalars as for pack_proto_rows, a
-    singular message None (not set) or its own value list, a repeated field a list."""
+    singular message None (not set) or its own value list, a repeated field a list.  A map field takes a dict, whose
+    entries are laid out in protobuf-go's Deterministic key order (map_key_order), or a list of (key, value) pairs laid
+    out as given (unsorted or duplicate keys make a row the encoder refuses); a message value None is a nil message."""
     def element(f, v) -> bytes:
         if f.type in (PB_STRING, PB_BYTES):
             b = v.encode("utf-8", "surrogateescape") if isinstance(v, str) else bytes(v)
             return len(b).to_bytes(4, "little") + b
-        if f.type == PB_MESSAGE:
+        if f.type in (PB_MESSAGE, PB_MAP):
             fx, vr = pack_proto_nested_message(msgs, f.msg, v)
             return fx + vr
         return _pb_scalar_words(f.type, v)
     fixed, var = bytearray(), bytearray()
     for f, v in zip(msgs[m], value):
-        if f.repeated:
+        if f.type == PB_MAP:
+            if isinstance(v, dict):
+                kt = msgs[f.msg][0].type
+                v = sorted(v.items(), key=lambda kv: map_key_order(kt, kv[0]))
+            v = [list(kv) for kv in v]
+        if f.repeated or f.type == PB_MAP:
             fixed += len(v).to_bytes(4, "little")
             for e in v:
                 var += element(f, e)

@@ -402,19 +402,27 @@ int gofr_proto_decode_device(gofr_engine*, const gofr_proto_field* fields, uint3
  * in field-number order, singular zero values skipped, a set message field written even when empty, repeated numeric
  * scalars packed, repeated strings / bytes / messages one tag per element).  msgs[m] names fields[first_field ..
  * first_field + n_fields) (ascending numbers); a field of type GOFR_PB_MESSAGE names its message type in `msg`; `root` is the
- * type of the rows.  At most 8 message types with 48 fields in all, nested at most 4 levels deep, no recursive types;
- * map fields are not taken (protobuf-go writes them in random order: there is no byte sequence to match).
- * Rows: the layout of "Row format" above — fixed words of a message in field order (64-bit kinds two words, string /
- * bytes their length, a singular message a presence word 0 / 1 followed by its own fixed part, a repeated field its
- * element count), then the variable part in field order (string bytes; a set message's variable part; the elements of a
- * repeated field: scalars as their words, strings as u32 length + bytes, messages as fixed part + variable part).
- * Output and d_meta as for gofr_proto_encode_device. */
+ * type of the rows.  At most 8 message types with 48 fields in all, nested at most 4 levels deep, no recursive types.
+ * MAP FIELDS: a field of type GOFR_PB_MAP (repeated = 0) names its ENTRY TYPE in `msg`: a message type with exactly two
+ * singular fields, number 1 the key (an integer kind, bool or string) and number 2 the value (any type but GOFR_PB_MAP).
+ * An entry type may serve several map fields; it is not the root, not the type of a GOFR_PB_MESSAGE field, and its field
+ * range is shared with no other message type (GOFR_ERR_INVALID otherwise); it counts
+ * toward the limits (map<string, M> is two levels).  Every entry is written with its key and value, zero values included,
+ * a message value always (tag, length 0 when its presence word is 0) — protobuf-go's Deterministic bytes: entries must be
+ * in strictly ascending key order (bool false < true; signed kinds signed, unsigned kinds unsigned, strings by bytes with a
+ * shorter prefix first, keys compared as the row words hold them), else the row is GOFR_GRPC_BAD_ROW (a Go map cannot hold
+ * it).  Rows: the layout of "Row format" above — fixed words of a message in field order (64-bit kinds two words, string /
+ * bytes their length, a singular message a presence word 0 / 1 followed by its own fixed part, a repeated field or a map
+ * its element count), then the variable part in field order (string bytes; a set message's variable part; the elements of
+ * a repeated field: scalars as their words, strings as u32 length + bytes, messages — and map entries — as fixed part +
+ * variable part).  Output and d_meta as for gofr_proto_encode_device. */
 #define GOFR_PB_MESSAGE 11u
+#define GOFR_PB_MAP 32u
 typedef struct gofr_proto_nfield {
     uint32_t number;
-    uint8_t type;     /* GOFR_PB_* or GOFR_PB_MESSAGE */
-    uint8_t repeated; /* 0 / 1 */
-    uint16_t msg;     /* GOFR_PB_MESSAGE: index into msgs */
+    uint8_t type;     /* GOFR_PB_*, GOFR_PB_MESSAGE or GOFR_PB_MAP */
+    uint8_t repeated; /* 0 / 1 (0 for a map) */
+    uint16_t msg;     /* GOFR_PB_MESSAGE: index into msgs; GOFR_PB_MAP: the entry type */
 } gofr_proto_nfield;
 typedef struct gofr_proto_nmsg {
     uint16_t first_field, n_fields;
@@ -425,14 +433,20 @@ int gofr_proto_encode_nested_device(gofr_engine*, const gofr_proto_nmsg* msgs, u
 /* The other direction for the same message types: length-prefixed frames -> rows (proto.Unmarshal as protobuf-go does it:
  * unknown fields and balanced groups skipped at every level; a known number with a foreign wire type is unknown, except that
  * repeated numeric scalars are accepted packed and unpacked; singular scalars and strings: the last occurrence wins;
- * repeated strings / bytes / messages: one element per occurrence in wire order; strings must be valid UTF-8).  d_meta[i]:
+ * repeated strings / bytes / messages: one element per occurrence in wire order; strings must be valid UTF-8).  A map
+ * field's row holds the resulting map in the encoder's canonical form: distinct keys in ascending order, the last entry on
+ * the wire for each key winning (message values replaced, not merged); inside an entry the last key and value win, a
+ * missing key or value is its zero value, a missing message value an empty message (presence 1: message values are always
+ * present).  A value message sent twice inside one entry (merged by protobuf-go), and a map field with more than 64 entries
+ * on the wire in one message (duplicates counted), give DEFER.  d_meta[i]:
  * GOFR_GRPC_OK or COMPRESSED / BAD_LENGTH / BAD_PROTO / BAD_UTF8 / DEFER (a failed frame gives an empty row); rows are
  * packed, 4-byte aligned, zero padded to a multiple of 4, d_row_off[n + 1]. */
 int gofr_proto_decode_nested_device(gofr_engine*, const gofr_proto_nmsg* msgs, uint32_t n_msgs, const gofr_proto_nfield* fields,
                                     uint32_t n_fields, uint32_t root, const uint8_t* d_in, const uint32_t* d_in_off, uint32_t n,
                                     uint8_t* d_rows, uint64_t rows_cap, uint32_t* d_row_off, uint32_t* d_meta, void* stream);
-/* validation of such a description without a GPU; desc_out (>= 512 bytes, may be NULL with desc_cap 0 to validate only...
- * then GOFR_ERR_CAPACITY means "valid") receives the kernel's internal descriptor (test infrastructure reads it) */
+/* validation of such a description without a GPU (map rules included: a description that breaks them is GOFR_ERR_INVALID);
+ * desc_out (>= 512 bytes, may be NULL with desc_cap 0 to validate only... then GOFR_ERR_CAPACITY means "valid") receives
+ * the kernel's internal descriptor (test infrastructure reads it) */
 int gofr_proto_nested_describe(const gofr_proto_nmsg* msgs, uint32_t n_msgs, const gofr_proto_nfield* fields, uint32_t n_fields,
                                uint32_t root, void* desc_out, uint32_t desc_cap);
 

@@ -1,0 +1,132 @@
+#!/usr/bin/env python
+"""pbn_bench.py — kernel time of the nested proto3 codec (gofr_proto_encode_nested_device / gofr_proto_decode_nested_device):
+   [GOFR_LIB_PATH=scratch/variants/libgofr_X.so] python scratch/pbn_bench.py [--n 1048576] [--steps 20] [--only a,b,c]
+Workloads (1 Mi messages each; 1024 distinct rows repeated):
+   a  the PAGE / ITEM type of tests/test_proto_nested.py (no maps)
+   b  M { map<string, string> labels = 1; map<int64, Item> items = 2; } with 8 labels and 8 items
+   c  the same type with 64 labels and 64 items (short strings, no tags): the decoder's worst case (selection over 64
+      entries per map)
+The decoder runs on the encoder's output.  CUDA events around `steps` launches after 3 warm-up launches; one JSON line per
+workload and direction, after the card's name, power limit and max SM clock (nvidia-smi, read-only query)."""
+import argparse
+import json
+import os
+import random
+import subprocess
+import sys
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+import numpy as np  # noqa: E402
+import torch  # noqa: E402
+
+from gofr_b200 import _abi, synth  # noqa: E402
+from gofr_b200 import spec as S  # noqa: E402
+from gofr_b200.engine import Engine  # noqa: E402
+from gofr_b200.table import Table  # noqa: E402
+from tests.test_proto_nested import MSGS, _rand_value  # noqa: E402
+
+F = S.ProtoNField
+ITEM = [F(1, S.PB_INT64), F(2, S.PB_STRING), F(3, S.PB_STRING, True), F(4, S.PB_DOUBLE)]
+MAP_MSGS = [[F(1, S.PB_MAP, False, 1), F(2, S.PB_MAP, False, 2)],
+            [F(1, S.PB_STRING), F(2, S.PB_STRING)],
+            [F(1, S.PB_INT64), F(2, S.PB_MESSAGE, False, 3)],
+            ITEM]
+
+
+def map_value(rnd, n, compact=False):
+    """compact: short strings and no tags, so that 1 Mi rows of 64 + 64 entries stay within 32-bit offsets"""
+    if compact:
+        labels = {"l%02d" % k: "v%d" % rnd.randint(0, 9) for k in range(n)}
+    else:
+        labels = {"label-%02d-%d" % (k, rnd.randint(0, 999)): "value-%d" % rnd.randint(0, 10 ** 6) for k in range(n)}
+    items = {}
+    while len(items) < n:
+        items[rnd.randint(-10 ** 12, 10 ** 12)] = ([rnd.randint(0, 10 ** 9), "i", [], rnd.random()] if compact else
+                                                   [rnd.randint(0, 10 ** 9), "item-%d" % rnd.randint(0, 999), ["t1", "t2"], rnd.random()])
+    return [labels, items]
+
+
+def tiled_rows(msgs, values, n):
+    """rows of `values` repeated to n messages"""
+    rows, off = S.pack_proto_nested_rows(msgs, 0, values)
+    k, blen = len(values), int(off[-1])
+    reps = (n + k - 1) // k
+    all_rows = np.concatenate([np.tile(rows[:blen], reps), np.zeros(16, np.uint8)])
+    j = np.arange(n + 1, dtype=np.int64)
+    all_off = off.astype(np.int64)[j % k] + (j // k) * blen
+    assert all_off[-1] < 1 << 32, "rows beyond 32-bit offsets"
+    return all_rows, all_off.astype(np.uint32)
+
+
+def timed(fn, steps):
+    for _ in range(3):
+        fn()
+    torch.cuda.synchronize()
+    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    a.record()
+    for _ in range(steps):
+        fn()
+    b.record()
+    torch.cuda.synchronize()
+    return a.elapsed_time(b) / steps
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--n", type=int, default=1 << 20)
+    ap.add_argument("--steps", type=int, default=20)
+    ap.add_argument("--only", default="a,b,c")
+    ap.add_argument("--tag", default=os.environ.get("GOFR_LIB_PATH", "tree"))
+    a = ap.parse_args()
+    smi = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"], capture_output=True, text=True)
+    print(json.dumps({"gpu": smi.stdout.strip().splitlines()[0] if smi.returncode == 0 else "nvidia-smi failed", "lib": a.tag}), flush=True)
+    rnd = random.Random(5)
+    work = {"a": (MSGS, lambda: [_rand_value(rnd, MSGS, 0) for _ in range(1024)]),
+            "b": (MAP_MSGS, lambda: [map_value(rnd, 8) for _ in range(1024)]),
+            "c": (MAP_MSGS, lambda: [map_value(rnd, 64, compact=True) for _ in range(1024)])}
+    eng = Engine(Table(synth.config1_spec()), 0)
+    L = _abi.lib()
+    st = torch.cuda.current_stream().cuda_stream
+    for w in a.only.split(","):
+        msgs, gen = work[w]
+        rows, off = tiled_rows(msgs, gen(), a.n)
+        n = a.n
+        nm, nf, k = S.proto_nested_tables(msgs)
+        d_rows = torch.from_numpy(rows).cuda()
+        d_off = torch.from_numpy(off.view(np.int32)).cuda()
+        cap = int(off[-1]) * 2 + 64 * n
+        d_out = torch.empty(cap + 16, dtype=torch.uint8, device="cuda")
+        d_out_off = torch.zeros(n + 1, dtype=torch.int32, device="cuda")
+        d_meta = torch.zeros(n, dtype=torch.int32, device="cuda")
+
+        def enc():
+            _abi.check(L.gofr_proto_encode_nested_device(eng._e, nm.ctypes.data, len(msgs), nf.ctypes.data, k, 0, d_rows.data_ptr(),
+                                                         d_off.data_ptr(), n, d_out.data_ptr(), cap, d_out_off.data_ptr(),
+                                                         d_meta.data_ptr(), st), "encode")
+        t_enc = timed(enc, a.steps)
+        assert not d_meta.any().item()
+        out_bytes = int(d_out_off[-1].item()) & 0xFFFFFFFF   # a u32 offset in an int32 tensor
+        rows_cap = int(off[-1]) + 64 * n
+        d_back = torch.empty(rows_cap, dtype=torch.uint8, device="cuda")
+        d_back_off = torch.zeros(n + 1, dtype=torch.int32, device="cuda")
+        d_meta2 = torch.zeros(n, dtype=torch.int32, device="cuda")
+
+        def dec():
+            _abi.check(L.gofr_proto_decode_nested_device(eng._e, nm.ctypes.data, len(msgs), nf.ctypes.data, k, 0, d_out.data_ptr(),
+                                                         d_out_off.data_ptr(), n, d_back.data_ptr(), rows_cap, d_back_off.data_ptr(),
+                                                         d_meta2.data_ptr(), st), "decode")
+        t_dec = timed(dec, a.steps)
+        assert not d_meta2.any().item()
+        same = bool(torch.equal(d_back[:int(off[-1])], d_rows[:int(off[-1])]))   # decode(encode(rows)) == rows
+        for direction, t in (("encode", t_enc), ("decode", t_dec)):
+            print(json.dumps({"workload": w, "dir": direction, "n": n, "ms": round(t, 4), "Mmsg_per_s": round(n / t / 1e3, 1),
+                              "frame_GBps": round(out_bytes / t / 1e6, 1), "row_bytes": int(off[-1]), "frame_bytes": out_bytes,
+                              "round_trip_equal": same, "lib": a.tag}), flush=True)
+        del d_rows, d_out, d_back
+        torch.cuda.empty_cache()
+    eng.close()
+
+
+if __name__ == "__main__":
+    main()
