@@ -337,7 +337,12 @@ int gofr_engine_geometry(const gofr_engine*, uint32_t* grid, uint32_t* blocks_pe
 int gofr_engine_slot_ctas(gofr_engine*, int ctas_per_sm, int* in_effect);
 /* the engine's default for a sealed table (4 or 5), computable without a GPU */
 int gofr_table_slot_ctas(const gofr_table*, int* ctas_per_sm);
-/* gofr_serve_device reports an undersized d_out through this flag (the launch itself is asynchronous). */
+/* The device calls with a packed output — gofr_serve_device, the frame codecs (gofr_grpc_hello_device, gofr_proto_encode_device,
+ * gofr_proto_decode_device, gofr_proto_encode_nested_device, gofr_proto_decode_nested_device) and gofr_requestlog_device —
+ * report an undersized d_out through this flag (the launch itself is asynchronous).  Output is written a tile of 128
+ * records at a time: the first tile that does not fit and every tile after it are dropped whole, and nothing is written at
+ * or past out_cap.  d_out_off and d_meta (where the call has one) are still written in full: the offsets every record would
+ * have had with room enough (d_out_off[n] = the capacity needed) and every status. */
 int gofr_engine_overflowed(gofr_engine*, int* flag_out, int reset);
 int gofr_engine_set_timing(gofr_engine*, int on);
 
@@ -367,8 +372,8 @@ int gofr_grpc_hello_device(gofr_engine*, const uint8_t* d_in, const uint32_t* d_
  *              emits them; at most GOFR_PROTO_MAX_FIELDS
  *   d_rows     row i = d_rows[d_row_off[i] .. d_row_off[i+1]), offsets multiples of 4, GOFR_H_ROW layout: per field
  *              (same order) 64-bit types two LE words (lo, hi), the others one (float / double: IEEE bits; string /
- *              bytes: byte length), then the string bytes in field order.  The buffer must stay readable for 8 bytes
- *              past the last row.
+ *              bytes: byte length), then the string bytes in field order.  The buffer follows the rule for
+ *              device input buffers at the top of this file: 16-byte aligned, 16 readable bytes past the last row.
  *   output     packed frames in row order, d_out_off[n+1]; d_meta[i] = GOFR_GRPC_OK, GOFR_GRPC_BAD_UTF8 (a string
  *              field is not valid UTF-8: proto.Marshal fails, the RPC fails — no frame), GOFR_GRPC_BAD_ROW (malformed
  *              row from the host shim — no frame).
@@ -392,8 +397,8 @@ int gofr_proto_encode_device(gofr_engine*, const gofr_proto_field* fields, uint3
  * the layout above (row sizes are multiples of 4; absent fields hold their zero value), packed, d_row_off[n+1].
  * d_meta[i]: GOFR_GRPC_OK or COMPRESSED / BAD_LENGTH / BAD_PROTO / BAD_UTF8 as for the Hello call (a failed frame gives an
  * empty row).  Unknown fields — and known fields arriving with a foreign wire type — are skipped; the last occurrence of
- * a field wins; int32 / uint32 / enum keep the low 32 bits of the varint, bool is v != 0.  d_in must stay readable for 8
- * bytes past the last frame. */
+ * a field wins; int32 / uint32 / enum keep the low 32 bits of the varint, bool is v != 0.  d_in follows the rule for
+ * device input buffers at the top of this file: 16-byte aligned, 16 readable bytes past the last frame. */
 int gofr_proto_decode_device(gofr_engine*, const gofr_proto_field* fields, uint32_t n_fields, const uint8_t* d_in,
                              const uint32_t* d_in_off, uint32_t n, uint8_t* d_rows, uint64_t rows_cap, uint32_t* d_row_off,
                              uint32_t* d_meta, void* stream);

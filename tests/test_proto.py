@@ -280,45 +280,54 @@ def test_decode_round_trip_and_python_protobuf():
         assert e_rows[mis:int(e_off[-1])].tobytes() == r2[:int(o2[-1])].tobytes()
 
 
+def T(num, wt):
+    """a tag: varint(number << 3 | wire type)"""
+    return _varint(num << 3 | wt)
+
+
+# hostile message bodies for HOSTILE_FIELDS; the last one nests groups deeper than 16 (BAD_PROTO by design, python accepts)
+HOSTILE_FIELDS = [S.ProtoField(1, S.PB_STRING), S.ProtoField(2, S.PB_INT32), S.ProtoField(3, S.PB_SINT32), S.ProtoField(4, S.PB_BOOL),
+                  S.ProtoField(5, S.PB_FIXED32), S.ProtoField(6, S.PB_UINT64), S.ProtoField(7, S.PB_BYTES), S.ProtoField(8, S.PB_SINT64),
+                  S.ProtoField(9, S.PB_DOUBLE)]
+HOSTILE_BODIES = [
+    b"",                                                                    # all defaults
+    T(1, 2) + b"\x02hi" + T(1, 2) + b"\x03bye",                              # last occurrence wins
+    T(2, 0) + _varint(2**64 - 1),                                           # int32 -1 as ten bytes
+    T(2, 0) + _varint(2**35 + 7),                                           # int32 keeps the low 32 bits
+    T(4, 0) + _varint(2**40),                                               # bool: any non-zero varint is true
+    T(3, 0) + _varint(2**33 + 3),                                           # sint32: zigzag of the low 32 bits
+    T(8, 0) + _varint(2**64 - 1) + T(6, 0) + _varint(2**64 - 1),
+    T(2, 2) + b"\x01\x07",                                                  # int32 with a length-delimited wire type: unknown, skipped
+    T(1, 0) + b"\x05",                                                      # string with a varint wire type: unknown, skipped
+    T(5, 5) + b"\x01\x02\x03\x04" + T(9, 1) + struct.pack("<d", -0.0),
+    T(99, 0) + b"\x01" + T(100, 2) + b"\x03abc" + T(101, 1) + b"\0" * 8 + T(102, 5) + b"\0" * 4 + T(1, 2) + b"\x01z",  # unknown fields
+    T(50, 3) + T(1, 2) + b"\x01q" + T(50, 4) + T(1, 2) + b"\x01r",           # field 1 inside an unknown group belongs to the group
+    T(50, 3) + T(51, 3) + T(51, 4) + T(50, 4),
+    T(50, 3),                                                               # unterminated group
+    T(50, 4),                                                               # end group without start
+    T(50, 3) + T(51, 4),                                                    # mismatched end group
+    T(1, 2) + b"\x05ab",                                                    # length runs past the message
+    T(1, 2) + b"\x01\xff",                                                  # invalid UTF-8 in a string
+    T(1, 2) + b"\x01\xff" + T(1, 2) + b"\x01a",                              # … even when overwritten later
+    T(7, 2) + b"\x02\xff\xfe",                                              # bytes may hold anything
+    b"\x00",                                                                # field number 0
+    _varint((2**29) << 3),                                                  # field number 2^29
+    T(1, 6), T(1, 7),                                                       # wire types 6 and 7
+    T(2, 0) + b"\x80" * 10 + b"\x01",                                       # varint longer than ten bytes
+    T(2, 0) + b"\xff" * 9 + b"\x02",                                        # tenth byte > 1
+    T(2, 0) + b"\x80",                                                      # truncated varint
+    T(5, 5) + b"\x01\x02",                                                  # truncated fixed32
+    T(9, 1) + b"\0" * 7,                                                    # truncated fixed64
+    b"".join(T(60 + d, 3) for d in range(17)),                              # groups nested deeper than 16
+]
+# frames whose 5-byte header is wrong: compressed flag, flag 2, shorter than a header, empty, length one too long / too short
+HOSTILE_HEADER_FRAMES = [_frame(T(2, 0) + b"\x01", flag=1), _frame(b"", flag=2), b"\x00\x00\x00", b"",
+                         b"\x00\x00\x00\x00\x05" + T(2, 0) + b"\x01", _frame(T(2, 0) + b"\x01") + b"\x00"]
+
+
 def test_decode_hostile_frames():
-    f = [S.ProtoField(1, S.PB_STRING), S.ProtoField(2, S.PB_INT32), S.ProtoField(3, S.PB_SINT32), S.ProtoField(4, S.PB_BOOL),
-         S.ProtoField(5, S.PB_FIXED32), S.ProtoField(6, S.PB_UINT64), S.ProtoField(7, S.PB_BYTES), S.ProtoField(8, S.PB_SINT64),
-         S.ProtoField(9, S.PB_DOUBLE)]
-    T = lambda num, wt: _varint(num << 3 | wt)
-    bodies = [
-        b"",                                                                    # all defaults
-        T(1, 2) + b"\x02hi" + T(1, 2) + b"\x03bye",                              # last occurrence wins
-        T(2, 0) + _varint(2**64 - 1),                                           # int32 -1 as ten bytes
-        T(2, 0) + _varint(2**35 + 7),                                           # int32 keeps the low 32 bits
-        T(4, 0) + _varint(2**40),                                               # bool: any non-zero varint is true
-        T(3, 0) + _varint(2**33 + 3),                                           # sint32: zigzag of the low 32 bits
-        T(8, 0) + _varint(2**64 - 1) + T(6, 0) + _varint(2**64 - 1),
-        T(2, 2) + b"\x01\x07",                                                  # int32 with a length-delimited wire type: unknown, skipped
-        T(1, 0) + b"\x05",                                                      # string with a varint wire type: unknown, skipped
-        T(5, 5) + b"\x01\x02\x03\x04" + T(9, 1) + struct.pack("<d", -0.0),
-        T(99, 0) + b"\x01" + T(100, 2) + b"\x03abc" + T(101, 1) + b"\0" * 8 + T(102, 5) + b"\0" * 4 + T(1, 2) + b"\x01z",  # unknown fields
-        T(50, 3) + T(1, 2) + b"\x01q" + T(50, 4) + T(1, 2) + b"\x01r",           # field 1 inside an unknown group belongs to the group
-        T(50, 3) + T(51, 3) + T(51, 4) + T(50, 4),
-        T(50, 3),                                                               # unterminated group
-        T(50, 4),                                                               # end group without start
-        T(50, 3) + T(51, 4),                                                    # mismatched end group
-        T(1, 2) + b"\x05ab",                                                    # length runs past the message
-        T(1, 2) + b"\x01\xff",                                                  # invalid UTF-8 in a string
-        T(1, 2) + b"\x01\xff" + T(1, 2) + b"\x01a",                              # … even when overwritten later
-        T(7, 2) + b"\x02\xff\xfe",                                              # bytes may hold anything
-        b"\x00",                                                                # field number 0
-        _varint((2**29) << 3),                                                  # field number 2^29
-        T(1, 6), T(1, 7),                                                       # wire types 6 and 7
-        T(2, 0) + b"\x80" * 10 + b"\x01",                                       # varint longer than ten bytes
-        T(2, 0) + b"\xff" * 9 + b"\x02",                                        # tenth byte > 1
-        T(2, 0) + b"\x80",                                                      # truncated varint
-        T(5, 5) + b"\x01\x02",                                                  # truncated fixed32
-        T(9, 1) + b"\0" * 7,                                                    # truncated fixed64
-        b"".join(T(60 + d, 3) for d in range(17)),                              # groups nested deeper than 16
-    ]
-    frames = [_frame(b) for b in bodies]
-    frames += [_frame(T(2, 0) + b"\x01", flag=1), _frame(b"", flag=2), b"\x00\x00\x00", b"", b"\x00\x00\x00\x00\x05" + T(2, 0) + b"\x01",
-               _frame(T(2, 0) + b"\x01") + b"\x00"]
+    f, bodies = HOSTILE_FIELDS, HOSTILE_BODIES
+    frames = [_frame(b) for b in bodies] + HOSTILE_HEADER_FRAMES
     raw, off = _pack_frames(frames)
     rows, roff, meta = O.proto_decode(f, raw, off)
     py = _py_parse_rows(f, frames[:len(bodies)])

@@ -413,47 +413,58 @@ def _s(num, b):
     return _varint(num << 3 | 2) + _varint(len(b)) + b
 
 
+# M { map<string, V> a = 1; map<int32, int64> b = 2; map<bool, string> c = 3; int32 d = 4; }  V { int32 x = 1; map<uint64, bytes> y = 2; }
+NONCANON_MSGS = [[F(1, S.PB_MAP, False, 1), F(2, S.PB_MAP, False, 2), F(3, S.PB_MAP, False, 3), F(4, S.PB_INT32)],
+                 [F(1, S.PB_STRING), F(2, S.PB_MESSAGE, False, 4)], [F(1, S.PB_INT32), F(2, S.PB_INT64)], [F(1, S.PB_BOOL), F(2, S.PB_STRING)],
+                 [F(1, S.PB_INT32), F(2, S.PB_MAP, False, 5)], [F(1, S.PB_UINT64), F(2, S.PB_BYTES)]]
+_V1, _V2 = b"\x08\x01", b"\x08\x02" + _entry(2, b"\x08\x05\x12\x01z")
+
+
+def _A(k, v):
+    return _entry(1, _s(1, k) + _s(2, v))
+
+
+def _B(k, v):
+    return _entry(2, b"\x08" + _varint(k & (2 ** 64 - 1)) + b"\x10" + _varint(v & (2 ** 64 - 1)))
+
+
+NONCANON_OK = [
+    _A(b"b", _V1) + _A(b"a", _V2) + _A(b"", b""),                            # shuffled
+    _A(b"a", _V1) + _A(b"a", _V2),                                         # duplicate key: the later value replaces
+    _A(b"a", _V2) + _B(3, 1) + _A(b"a", _V1) + _B(-3, 2) + _B(3, 9),          # duplicates interleaved with another map
+    _entry(1, _s(2, _V1) + _s(1, b"k")),                                # value before key
+    _entry(1, _s(1, b"k")) + _entry(1, _s(2, _V2)) + _entry(2, b"") + _entry(3, b"\x12\x00"),   # missing value / key / both
+    _entry(1, _s(1, b"x") + _s(1, b"k") + _s(2, _V1)),                  # key twice inside an entry: the last wins
+    _entry(2, b"\x08\x01\x10\x05\x10\x07\x08\x02"),                    # scalar key and value twice
+    _entry(1, _s(1, b"k") + b"\x18\x05" + b"\x2b\x08\x01\x2c" + _s(2, _V1) + b"\x25\x00\x00\x00\x00"),  # unknown fields and a group
+    _entry(2, b"\x0d\x01\x00\x00\x00\x08\x04\x11" + bytes(8) + b"\x10\x06"),  # foreign wire types for key and value: unknown
+    b"\x08\x03" + b"\x10\x05" + b"\x18\x01" + _entry(3, b"\x08\x02\x12\x01t") + b"\x20\x07",   # map fields with a foreign wire type
+    _entry(3, b"\x08\x01\x12\x01t") + _entry(3, b"\x12\x01f"),          # bool keys: true first on the wire
+    b"\x0b" + _A(b"g", _V1) + b"\x0c" + _A(b"h", _V1),                     # an entry inside an unknown group is skipped
+    _entry(1, _s(1, b"n") + _s(2, _entry(2, b"\x08\x02") + _entry(2, b"\x08\x01\x12\x01a") + _entry(2, b"\x08\x02\x12\x01b"))),
+    b"".join(_B(k, k) for k in range(63, -1, -1)),                      # exactly 64 entries
+    b"".join(_B(k % 8, k) for k in range(64)),                          # 64 on the wire, 8 keys
+]
+NONCANON_DEFER = [
+    b"".join(_B(k, k) for k in range(65)),                              # 65 entries
+    b"".join(_B(k % 2, k) for k in range(65)),                          # 65 on the wire, duplicates counted
+    _entry(1, _s(1, b"k") + _s(2, _V1) + _s(2, _V2)),                    # a value message twice in one entry (merged by Go)
+    _A(b"a", _entry(2, b"") * 65),                                      # too many entries one level down
+]
+NONCANON_BAD = [
+    _entry(1, _s(1, b"\xff") + _s(2, _V1)),                             # invalid UTF-8 key -> BAD_UTF8
+    _A(b"a", _V1) + _A(b"\xc3", _V1) + _A(b"a", _V2),                        # ... in an entry that a later one replaces
+    _entry(3, b"\x08\x01\x12\x01\xff"),                                # invalid UTF-8 value
+    _entry(1, b"\x0a\x05ab"),                                          # malformed inside an entry -> BAD_PROTO
+    _entry(1, b"\x0b"),                                                # open group inside an entry
+    _entry(1, _s(2, b"\x12\x03\x08")),                                 # malformed inside a value's map
+    b"".join(_B(k, k) for k in range(70)) + _entry(1, b"\x0a\x05ab"),   # malformed beats DEFER
+    b"".join(_B(k, k) for k in range(70)) + _entry(1, _s(1, b"\xff")),  # invalid UTF-8 beats DEFER
+]
+
+
 def test_decode_noncanonical_frames():
-    # M { map<string, V> a = 1; map<int32, int64> b = 2; map<bool, string> c = 3; int32 d = 4; }  V { int32 x = 1; map<uint64, bytes> y = 2; }
-    msgs = [[F(1, S.PB_MAP, False, 1), F(2, S.PB_MAP, False, 2), F(3, S.PB_MAP, False, 3), F(4, S.PB_INT32)],
-            [F(1, S.PB_STRING), F(2, S.PB_MESSAGE, False, 4)], [F(1, S.PB_INT32), F(2, S.PB_INT64)], [F(1, S.PB_BOOL), F(2, S.PB_STRING)],
-            [F(1, S.PB_INT32), F(2, S.PB_MAP, False, 5)], [F(1, S.PB_UINT64), F(2, S.PB_BYTES)]]
-    v1, v2 = b"\x08\x01", b"\x08\x02" + _entry(2, b"\x08\x05\x12\x01z")
-    A = lambda k, v: _entry(1, _s(1, k) + _s(2, v))  # noqa: E731
-    B = lambda k, v: _entry(2, b"\x08" + _varint(k & (2 ** 64 - 1)) + b"\x10" + _varint(v & (2 ** 64 - 1)))  # noqa: E731
-    ok = [
-        A(b"b", v1) + A(b"a", v2) + A(b"", b""),                            # shuffled
-        A(b"a", v1) + A(b"a", v2),                                         # duplicate key: the later value replaces
-        A(b"a", v2) + B(3, 1) + A(b"a", v1) + B(-3, 2) + B(3, 9),          # duplicates interleaved with another map
-        _entry(1, _s(2, v1) + _s(1, b"k")),                                # value before key
-        _entry(1, _s(1, b"k")) + _entry(1, _s(2, v2)) + _entry(2, b"") + _entry(3, b"\x12\x00"),   # missing value / key / both
-        _entry(1, _s(1, b"x") + _s(1, b"k") + _s(2, v1)),                  # key twice inside an entry: the last wins
-        _entry(2, b"\x08\x01\x10\x05\x10\x07\x08\x02"),                    # scalar key and value twice
-        _entry(1, _s(1, b"k") + b"\x18\x05" + b"\x2b\x08\x01\x2c" + _s(2, v1) + b"\x25\x00\x00\x00\x00"),  # unknown fields and a group
-        _entry(2, b"\x0d\x01\x00\x00\x00\x08\x04\x11" + bytes(8) + b"\x10\x06"),  # foreign wire types for key and value: unknown
-        b"\x08\x03" + b"\x10\x05" + b"\x18\x01" + _entry(3, b"\x08\x02\x12\x01t") + b"\x20\x07",   # map fields with a foreign wire type
-        _entry(3, b"\x08\x01\x12\x01t") + _entry(3, b"\x12\x01f"),          # bool keys: true first on the wire
-        b"\x0b" + A(b"g", v1) + b"\x0c" + A(b"h", v1),                     # an entry inside an unknown group is skipped
-        _entry(1, _s(1, b"n") + _s(2, _entry(2, b"\x08\x02") + _entry(2, b"\x08\x01\x12\x01a") + _entry(2, b"\x08\x02\x12\x01b"))),
-        b"".join(B(k, k) for k in range(63, -1, -1)),                      # exactly 64 entries
-        b"".join(B(k % 8, k) for k in range(64)),                          # 64 on the wire, 8 keys
-    ]
-    defer = [
-        b"".join(B(k, k) for k in range(65)),                              # 65 entries
-        b"".join(B(k % 2, k) for k in range(65)),                          # 65 on the wire, duplicates counted
-        _entry(1, _s(1, b"k") + _s(2, v1) + _s(2, v2)),                    # a value message twice in one entry (merged by Go)
-        A(b"a", _entry(2, b"") * 65),                                      # too many entries one level down
-    ]
-    bad = [
-        _entry(1, _s(1, b"\xff") + _s(2, v1)),                             # invalid UTF-8 key -> BAD_UTF8
-        A(b"a", v1) + A(b"\xc3", v1) + A(b"a", v2),                        # ... in an entry that a later one replaces
-        _entry(3, b"\x08\x01\x12\x01\xff"),                                # invalid UTF-8 value
-        _entry(1, b"\x0a\x05ab"),                                          # malformed inside an entry -> BAD_PROTO
-        _entry(1, b"\x0b"),                                                # open group inside an entry
-        _entry(1, _s(2, b"\x12\x03\x08")),                                 # malformed inside a value's map
-        b"".join(B(k, k) for k in range(70)) + _entry(1, b"\x0a\x05ab"),   # malformed beats DEFER
-        b"".join(B(k, k) for k in range(70)) + _entry(1, _s(1, b"\xff")),  # invalid UTF-8 beats DEFER
-    ]
+    msgs, ok, defer, bad = NONCANON_MSGS, NONCANON_OK, NONCANON_DEFER, NONCANON_BAD
     frames = [_frame(b) for b in ok + defer + bad]
     rows, meta = _decode_model_emu(msgs, 0, frames)
     D, P, U = S.GRPC_DEFER, S.GRPC_BAD_PROTO, S.GRPC_BAD_UTF8

@@ -341,34 +341,40 @@ def test_decode_canonical_frames_round_trip():
             assert a == b, (i, values[i])
 
 
+# message types and frames, well-formed but not canonical, or hostile: statuses as test_decode_noncanonical_and_hostile_frames
+# states them (the singular message sent twice is DEFER; the four header frames come last)
+HOSTILE_MSGS = [[F(1, S.PB_INT32), F(2, S.PB_STRING), F(3, S.PB_SINT64, True), F(4, S.PB_MESSAGE, False, 1), F(5, S.PB_MESSAGE, True, 1),
+                 F(6, S.PB_FIXED32, True), F(7, S.PB_STRING, True), F(8, S.PB_DOUBLE, True), F(9, S.PB_BOOL)],
+                [F(1, S.PB_STRING), F(2, S.PB_UINT64, True), F(3, S.PB_BYTES)]]
+_SUB = b"\x0a\x02hi" + b"\x10\x05" + b"\x12\x02\x01\x02" + b"\x1a\x01\xff"         # name, unpacked + packed uint64, bytes
+HOSTILE_BODIES = [
+    b"",                                                           # nothing
+    b"\x08\x01\x08\x02",                                           # singular scalar twice: last wins
+    b"\x12\x01a\x12\x02bc",                                        # string twice: last wins
+    b"\x18\x01\x18\x03" + b"\x1a\x02\x05\x07" + b"\x18\x09",       # repeated sint64: unpacked, packed, unpacked — wire order
+    b"\x22" + _varint(len(_SUB)) + _SUB,                             # singular message
+    b"\x2a\x00" + b"\x2a" + _varint(len(_SUB)) + _SUB + b"\x2a\x00",  # three elements, two empty
+    b"\x35\x01\x00\x00\x00" + b"\x32\x08\x02\x00\x00\x00\x03\x00\x00\x00",  # fixed32 unpacked then packed
+    b"\x3a\x00\x3a\x01x",                                          # repeated strings incl. an empty one
+    b"\x42\x10" + struct.pack("<dd", 1.5, -0.0) + b"\x41" + struct.pack("<d", 2.5),  # doubles packed + unpacked
+    b"\x48\x02",                                                   # bool from a varint that is not 0 / 1
+    b"\x0d\x01\x00\x00\x00" + b"\x10\x07" + b"\xf8\x07\x01" + b"\x92\x03\x03abc",    # foreign wire types and unknown numbers: skipped
+    b"\x0b\x08\x01\x13\x14\x0c" + b"\x08\x05",                      # unknown groups, nested, balanced
+    b"\x22\x02\x0a\x00" + b"\x08\x03",                             # message with an explicit empty string
+    b"\x22\x00\x22\x00",                                           # singular message twice: protobuf-go merges -> DEFER
+    b"\x2a\x04\x22\x02\x08\x01",                                   # element with fields the sub-message does not know
+    # malformed
+    b"\x08", b"\x12\x05ab", b"\x22\x03\x0a\x05a", b"\x0b\x08\x01", b"\x0c", b"\x32\x03\x01\x00\x00", b"\x1a\x02\x80\x80",
+    b"\x00\x01", b"\x0e\x01", b"\x42\x07" + b"\0" * 7, b"\x2a\x02\x12\x05",
+    # invalid UTF-8: top level, in an element, in an occurrence that is overwritten later
+    b"\x12\x01\xff", b"\x2a\x03\x0a\x01\xc3", b"\x12\x01\xff\x12\x01a", b"\x3a\x02\xed\xa0",
+]
+HOSTILE_HEADER_FRAMES = [b"\x01\x00\x00\x00\x00", b"\x00\x00\x00\x00\x05\x08", b"\x00\x00", b"\x02\x00\x00\x00\x00"]   # header problems
+
+
 def test_decode_noncanonical_and_hostile_frames():
-    msgs = [[F(1, S.PB_INT32), F(2, S.PB_STRING), F(3, S.PB_SINT64, True), F(4, S.PB_MESSAGE, False, 1), F(5, S.PB_MESSAGE, True, 1),
-             F(6, S.PB_FIXED32, True), F(7, S.PB_STRING, True), F(8, S.PB_DOUBLE, True), F(9, S.PB_BOOL)],
-            [F(1, S.PB_STRING), F(2, S.PB_UINT64, True), F(3, S.PB_BYTES)]]
-    sub = b"\x0a\x02hi" + b"\x10\x05" + b"\x12\x02\x01\x02" + b"\x1a\x01\xff"         # name, unpacked + packed uint64, bytes
-    frames = [_frame(b) for b in [
-        b"",                                                           # nothing
-        b"\x08\x01\x08\x02",                                           # singular scalar twice: last wins
-        b"\x12\x01a\x12\x02bc",                                        # string twice: last wins
-        b"\x18\x01\x18\x03" + b"\x1a\x02\x05\x07" + b"\x18\x09",       # repeated sint64: unpacked, packed, unpacked — wire order
-        b"\x22" + _varint(len(sub)) + sub,                             # singular message
-        b"\x2a\x00" + b"\x2a" + _varint(len(sub)) + sub + b"\x2a\x00",  # three elements, two empty
-        b"\x35\x01\x00\x00\x00" + b"\x32\x08\x02\x00\x00\x00\x03\x00\x00\x00",  # fixed32 unpacked then packed
-        b"\x3a\x00\x3a\x01x",                                          # repeated strings incl. an empty one
-        b"\x42\x10" + struct.pack("<dd", 1.5, -0.0) + b"\x41" + struct.pack("<d", 2.5),  # doubles packed + unpacked
-        b"\x48\x02",                                                   # bool from a varint that is not 0 / 1
-        b"\x0d\x01\x00\x00\x00" + b"\x10\x07" + b"\xf8\x07\x01" + b"\x92\x03\x03abc",    # foreign wire types and unknown numbers: skipped
-        b"\x0b\x08\x01\x13\x14\x0c" + b"\x08\x05",                      # unknown groups, nested, balanced
-        b"\x22\x02\x0a\x00" + b"\x08\x03",                             # message with an explicit empty string
-        b"\x22\x00\x22\x00",                                           # singular message twice: protobuf-go merges -> DEFER
-        b"\x2a\x04\x22\x02\x08\x01",                                   # element with fields the sub-message does not know
-        # malformed
-        b"\x08", b"\x12\x05ab", b"\x22\x03\x0a\x05a", b"\x0b\x08\x01", b"\x0c", b"\x32\x03\x01\x00\x00", b"\x1a\x02\x80\x80",
-        b"\x00\x01", b"\x0e\x01", b"\x42\x07" + b"\0" * 7, b"\x2a\x02\x12\x05",
-        # invalid UTF-8: top level, in an element, in an occurrence that is overwritten later
-        b"\x12\x01\xff", b"\x2a\x03\x0a\x01\xc3", b"\x12\x01\xff\x12\x01a", b"\x3a\x02\xed\xa0",
-    ]]
-    frames += [b"\x01\x00\x00\x00\x00", b"\x00\x00\x00\x00\x05\x08", b"\x00\x00", b"\x02\x00\x00\x00\x00"]   # header problems
+    msgs = HOSTILE_MSGS
+    frames = [_frame(b) for b in HOSTILE_BODIES] + HOSTILE_HEADER_FRAMES
     rows, off, meta = _decode_three_ways(msgs, 0, frames)
     assert list(meta[:15]) == [S.GRPC_OK] * 13 + [S.GRPC_DEFER, S.GRPC_OK]
     assert all(m == S.GRPC_BAD_PROTO for m in meta[15:26]) and all(m == S.GRPC_BAD_UTF8 for m in meta[26:30])
