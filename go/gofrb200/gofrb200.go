@@ -348,3 +348,77 @@ func (e *Engine) ProtoDecodeNestedDevice(msgs []ProtoNMsg, fields []ProtoNField,
 		(*C.uint32_t)(dInOff), C.uint32_t(n), (*C.uint8_t)(dRows), C.uint64_t(rowsCap), (*C.uint32_t)(dRowOff), (*C.uint32_t)(dMeta), stream),
 		"gofr_proto_decode_nested_device")
 }
+
+// ProtoOptional is the presence byte of a proto3 optional field (GOFR_PB_OPTIONAL).
+const ProtoOptional = C.GOFR_PB_OPTIONAL
+
+// presenceArg checks that presence has one byte per field and returns the C pointer (nil: no presence).
+func presenceArg(presence []uint8, fields []ProtoNField) (*C.uint8_t, error) {
+	if presence == nil {
+		return nil, nil
+	}
+	if len(presence) != len(fields) {
+		return nil, errors.New("gofrb200: one presence byte per field")
+	}
+	return (*C.uint8_t)(unsafe.Pointer(&presence[0])), nil
+}
+
+// ProtoEncodeNestedExDevice is ProtoEncodeNestedDevice for message types with field presence
+// (gofr_proto_encode_nested_ex_device): presence[i] describes fields[i].  From protoreflect:
+//   - fd.ContainingOneof() that is not synthetic (oneof.IsSynthetic() == false): the field is a member of that oneof; give
+//     the message type's oneofs the numbers 1..7 (md.Oneofs() in order, synthetic ones skipped) — at most 7 per type;
+//   - fd.HasOptionalKeyword(): ProtoOptional (its synthetic oneof is not a group);
+//   - anything else: 0.
+// A set explicit-presence field is written even at its zero value.  In the row, an optional or oneof scalar, string or
+// bytes field has a presence word 0 / 1 before its usual words; a oneof message member is laid out as any singular message
+// field.  A nil presence is ProtoEncodeNestedDevice.
+func (e *Engine) ProtoEncodeNestedExDevice(msgs []ProtoNMsg, fields []ProtoNField, root uint32, presence []uint8, dRows, dRowOff unsafe.Pointer,
+	n int, dOut unsafe.Pointer, outCap uint64, dOutOff, dMeta unsafe.Pointer, stream unsafe.Pointer) error {
+	if len(msgs) == 0 || len(fields) == 0 {
+		return errors.New("gofrb200: empty message description")
+	}
+	pp, err := presenceArg(presence, fields)
+	if err != nil {
+		return err
+	}
+	return check(C.gofr_proto_encode_nested_ex_device(e.e, (*C.gofr_proto_nmsg)(unsafe.Pointer(&msgs[0])), C.uint32_t(len(msgs)),
+		(*C.gofr_proto_nfield)(unsafe.Pointer(&fields[0])), C.uint32_t(len(fields)), C.uint32_t(root), pp, (*C.uint8_t)(dRows),
+		(*C.uint32_t)(dRowOff), C.uint32_t(n), (*C.uint8_t)(dOut), C.uint64_t(outCap), (*C.uint32_t)(dOutOff), (*C.uint32_t)(dMeta), stream),
+		"gofr_proto_encode_nested_ex_device")
+}
+
+// ProtoDecodeNestedExDevice is ProtoDecodeNestedDevice with the presence bytes of ProtoEncodeNestedExDevice
+// (gofr_proto_decode_nested_ex_device): an optional field is set iff it occurs; of a oneof, the member occurring last on
+// the wire is the set one; a oneof message member sent twice gives dMeta[i] == 6 (GOFR_GRPC_DEFER).
+func (e *Engine) ProtoDecodeNestedExDevice(msgs []ProtoNMsg, fields []ProtoNField, root uint32, presence []uint8, dIn, dInOff unsafe.Pointer,
+	n int, dRows unsafe.Pointer, rowsCap uint64, dRowOff, dMeta unsafe.Pointer, stream unsafe.Pointer) error {
+	if len(msgs) == 0 || len(fields) == 0 {
+		return errors.New("gofrb200: empty message description")
+	}
+	pp, err := presenceArg(presence, fields)
+	if err != nil {
+		return err
+	}
+	return check(C.gofr_proto_decode_nested_ex_device(e.e, (*C.gofr_proto_nmsg)(unsafe.Pointer(&msgs[0])), C.uint32_t(len(msgs)),
+		(*C.gofr_proto_nfield)(unsafe.Pointer(&fields[0])), C.uint32_t(len(fields)), C.uint32_t(root), pp, (*C.uint8_t)(dIn),
+		(*C.uint32_t)(dInOff), C.uint32_t(n), (*C.uint8_t)(dRows), C.uint64_t(rowsCap), (*C.uint32_t)(dRowOff), (*C.uint32_t)(dMeta), stream),
+		"gofr_proto_decode_nested_ex_device")
+}
+
+// ProtoNestedDescribeEx validates a description with presence bytes without a GPU (gofr_proto_nested_describe_ex): nil
+// when the encode and decode calls would accept it.
+func ProtoNestedDescribeEx(msgs []ProtoNMsg, fields []ProtoNField, root uint32, presence []uint8) error {
+	if len(msgs) == 0 || len(fields) == 0 {
+		return errors.New("gofrb200: empty message description")
+	}
+	pp, err := presenceArg(presence, fields)
+	if err != nil {
+		return err
+	}
+	rc := C.gofr_proto_nested_describe_ex((*C.gofr_proto_nmsg)(unsafe.Pointer(&msgs[0])), C.uint32_t(len(msgs)),
+		(*C.gofr_proto_nfield)(unsafe.Pointer(&fields[0])), C.uint32_t(len(fields)), C.uint32_t(root), pp, nil, 0)
+	if rc == C.GOFR_ERR_CAPACITY { // valid: no room asked for the descriptor
+		return nil
+	}
+	return check(rc, "gofr_proto_nested_describe_ex")
+}

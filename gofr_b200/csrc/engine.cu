@@ -61,6 +61,8 @@ __global__ void proto_encode_nested_kernel(const GrpcParams p, const PbnDesc D);
 __global__ void proto_decode_nested_kernel(const GrpcParams p, const PbnDesc D);  // proto_nested_decode_kernel.cu
 __global__ void proto_encode_nested_maps_kernel(const GrpcParams p, const PbnDesc D);  // proto_nested_maps_kernel.cu: the
 __global__ void proto_decode_nested_maps_kernel(const GrpcParams p, const PbnDesc D);  // same for descriptions with maps
+__global__ void proto_encode_nested_presence_kernel(const GrpcParams p, const PbnDesc D);  // proto_nested_presence_kernel.cu:
+__global__ void proto_decode_nested_presence_kernel(const GrpcParams p, const PbnDesc D);  // with explicit presence (and maps)
 __global__ void reqlog_kernel(const LogParams p);                // reqlog_kernel.cu
 __global__ void http_parse_kernel(const HttpParams p);           // http_kernel.cu
 __global__ void route_kernel(const RouteParams p);               // route_kernel.cu
@@ -71,7 +73,7 @@ namespace {
 
 enum Kern {
     K_SERVE, K_SERVE_VALUES, K_SLOTS, K_SLOTS_WIDE, K_SLOTS_VALUES, K_HELLO, K_PROTO_ENC, K_PROTO_DEC, K_PBN_ENC, K_PBN_DEC,
-    K_PBN_ENC_MAPS, K_PBN_DEC_MAPS, K_REQLOG, K_HTTP, K_ROUTE, K_BIND, K_COUNT
+    K_PBN_ENC_MAPS, K_PBN_DEC_MAPS, K_PBN_ENC_PRES, K_PBN_DEC_PRES, K_REQLOG, K_HTTP, K_ROUTE, K_BIND, K_COUNT
 };
 struct KernelRec {
     const void* fn;
@@ -91,6 +93,8 @@ const KernelRec kKernels[K_COUNT] = {
     {(const void*)proto_decode_nested_kernel, "proto", kServeThreads},
     {(const void*)proto_encode_nested_maps_kernel, "proto", kServeThreads},
     {(const void*)proto_decode_nested_maps_kernel, "proto", kServeThreads},
+    {(const void*)proto_encode_nested_presence_kernel, "proto", kServeThreads},
+    {(const void*)proto_decode_nested_presence_kernel, "proto", kServeThreads},
     {(const void*)reqlog_kernel, "request-log", kServeThreads},
     {(const void*)http_parse_kernel, "http", kServeThreads},
     {(const void*)route_kernel, "route", kRouteThreads},
@@ -1110,15 +1114,16 @@ static int proto_run(gofr_engine* e, const gofr_proto_field* fields, uint32_t n_
     return launch_frames(e, decode ? K_PROTO_DEC : K_PROTO_ENC, p, n, d_out, out_cap, d_out_off, stream, S);
 }
 
-// message types with nested / repeated fields -> the kernel's descriptor: validation, words of every fixed part, nesting depth
+// message types with nested / repeated fields -> the kernel's descriptor: validation, words of every fixed part, nesting depth.
+// presence: one byte per field (0, GOFR_PB_OPTIONAL or a oneof group 1..7), or null
 static int pbn_build(const gofr_proto_nmsg* msgs, uint32_t n_msgs, const gofr_proto_nfield* fields, uint32_t n_fields, uint32_t root,
-                     PbnDesc* D) {
+                     const uint8_t* presence, PbnDesc* D) {
     if (!msgs || !fields || n_msgs == 0 || n_msgs > (uint32_t)kPbnMaxMsgs || n_fields > (uint32_t)kPbnMaxFields || root >= n_msgs) {
         set_last_error("at most %d message types with %d fields in all", kPbnMaxMsgs, kPbnMaxFields);
         return GOFR_ERR_CAPACITY;
     }
     memset(D, 0, sizeof *D);
-    D->n_msgs = (uint16_t)n_msgs;
+    D->n_msgs = (uint8_t)n_msgs;
     D->root = root;
     for (uint32_t m = 0; m < n_msgs; m++) {
         if (msgs[m].n_fields == 0 || (uint32_t)msgs[m].first_field + msgs[m].n_fields > n_fields) { set_last_error("message type %u: bad field range", m); return GOFR_ERR_INVALID; }
@@ -1141,6 +1146,17 @@ static int pbn_build(const gofr_proto_nmsg* msgs, uint32_t n_msgs, const gofr_pr
             // messages, map entries, strings, bytes and PACKED repeated scalars are length-delimited
             const uint32_t wire = (sub || (f.repeated && proto_wire(t) != 2)) ? 2u : proto_wire(t);
             F.tag = num << 3 | wire;
+            // explicit presence: a oneof member is singular; optional on a message field is what a singular message field
+            // is anyway (its presence word), so it marks nothing
+            const uint32_t pr = presence ? presence[msgs[m].first_field + k] : 0u;
+            if (pr > 7u && pr != GOFR_PB_OPTIONAL) { set_last_error("message type %u field %u: presence byte %u", m, num, pr); return GOFR_ERR_INVALID; }
+            if (pr && (f.repeated || t == GOFR_PB_MAP)) {
+                set_last_error("message type %u field %u: a repeated or map field has no presence", m, num);
+                return GOFR_ERR_INVALID;
+            }
+            if (pr && pr != GOFR_PB_OPTIONAL) F.flags = (uint8_t)(pr << PBN_ONEOF_SHIFT | (sub ? 0u : (uint32_t)PBN_PRESENCE));
+            else if (pr && !sub) F.flags = (uint8_t)PBN_PRESENCE;
+            if (F.flags & (PBN_PRESENCE | PBN_ONEOF)) D->presence = 1;
         }
     }
     // map entry types: exactly (1 key, 2 value), singular; keys of integer, bool or string type; values anything but a map.
@@ -1167,6 +1183,10 @@ static int pbn_build(const gofr_proto_nmsg* msgs, uint32_t n_msgs, const gofr_pr
             set_last_error("map entry type %u: exactly the singular fields 1 (key) and 2 (value)", m);
             return GOFR_ERR_INVALID;
         }
+        if (presence && (presence[msgs[m].first_field] || presence[msgs[m].first_field + 1])) {
+            set_last_error("map entry type %u: its key and value carry no presence", m);
+            return GOFR_ERR_INVALID;
+        }
         const uint32_t kt = kv[0].type;
         const bool key_ok = kt == GOFR_PB_INT32 || kt == GOFR_PB_INT64 || kt == GOFR_PB_UINT32 || kt == GOFR_PB_UINT64 || kt == GOFR_PB_SINT32 ||
                             kt == GOFR_PB_SINT64 || kt == GOFR_PB_FIXED32 || kt == GOFR_PB_FIXED64 || kt == GOFR_PB_SFIXED32 ||
@@ -1189,6 +1209,7 @@ static int pbn_build(const gofr_proto_nmsg* msgs, uint32_t n_msgs, const gofr_pr
         for (uint32_t k = 0; k < D->count[m]; k++) {
             PbnField& F = D->f[D->first[m] + k];
             uint32_t w = (F.flags & PBN_REPEATED) ? 1u : (F.cls & PC_64) ? 2u : 1u;
+            if (F.flags & PBN_PRESENCE) w++;  // the presence word
             if (F.msg != 0xFF) {
                 int rc = visit(F.msg);
                 if (rc) return rc;
@@ -1211,39 +1232,64 @@ static int pbn_build(const gofr_proto_nmsg* msgs, uint32_t n_msgs, const gofr_pr
 }
 
 static int proto_nested_run(gofr_engine* e, const gofr_proto_nmsg* msgs, uint32_t n_msgs, const gofr_proto_nfield* fields, uint32_t n_fields,
-                            uint32_t root, const uint8_t* d_in, const uint32_t* d_in_off, uint32_t n, uint8_t* d_out, uint64_t out_cap,
-                            uint32_t* d_out_off, uint32_t* d_meta, void* stream, bool decode) {
+                            uint32_t root, const uint8_t* presence, const uint8_t* d_in, const uint32_t* d_in_off, uint32_t n,
+                            uint8_t* d_out, uint64_t out_cap, uint32_t* d_out_off, uint32_t* d_meta, void* stream, bool decode) {
     if (!e || (n && (!d_in || !d_in_off || !d_out || !d_out_off || !d_meta))) return GOFR_ERR_INVALID;
     PbnDesc D;
-    { int rc = pbn_build(msgs, n_msgs, fields, n_fields, root, &D); if (rc) return rc; }
+    { int rc = pbn_build(msgs, n_msgs, fields, n_fields, root, presence, &D); if (rc) return rc; }
     GrpcParams p;
     memset(&p, 0, sizeof p);
     p.in = d_in; p.in_off = d_in_off; p.meta = d_meta;
-    const Kern k = D.maps ? (decode ? K_PBN_DEC_MAPS : K_PBN_ENC_MAPS) : (decode ? K_PBN_DEC : K_PBN_ENC);  // map-free: no map code
+    // presence-free: no presence code; map-free too: no map code
+    const Kern k = D.presence ? (decode ? K_PBN_DEC_PRES : K_PBN_ENC_PRES)
+                 : D.maps     ? (decode ? K_PBN_DEC_MAPS : K_PBN_ENC_MAPS) : (decode ? K_PBN_DEC : K_PBN_ENC);
     return launch_frames(e, k, p, n, d_out, out_cap, d_out_off, stream, D);
 }
 
 int gofr_proto_encode_nested_device(gofr_engine* e, const gofr_proto_nmsg* msgs, uint32_t n_msgs, const gofr_proto_nfield* fields,
                                     uint32_t n_fields, uint32_t root, const uint8_t* d_rows, const uint32_t* d_row_off, uint32_t n,
                                     uint8_t* d_out, uint64_t out_cap, uint32_t* d_out_off, uint32_t* d_meta, void* stream) {
-    return proto_nested_run(e, msgs, n_msgs, fields, n_fields, root, d_rows, d_row_off, n, d_out, out_cap, d_out_off, d_meta, stream, false);
+    return proto_nested_run(e, msgs, n_msgs, fields, n_fields, root, nullptr, d_rows, d_row_off, n, d_out, out_cap, d_out_off, d_meta,
+                            stream, false);
 }
 
 int gofr_proto_decode_nested_device(gofr_engine* e, const gofr_proto_nmsg* msgs, uint32_t n_msgs, const gofr_proto_nfield* fields,
                                     uint32_t n_fields, uint32_t root, const uint8_t* d_in, const uint32_t* d_in_off, uint32_t n,
                                     uint8_t* d_rows, uint64_t rows_cap, uint32_t* d_row_off, uint32_t* d_meta, void* stream) {
-    return proto_nested_run(e, msgs, n_msgs, fields, n_fields, root, d_in, d_in_off, n, d_rows, rows_cap, d_row_off, d_meta, stream, true);
+    return proto_nested_run(e, msgs, n_msgs, fields, n_fields, root, nullptr, d_in, d_in_off, n, d_rows, rows_cap, d_row_off, d_meta,
+                            stream, true);
+}
+
+int gofr_proto_encode_nested_ex_device(gofr_engine* e, const gofr_proto_nmsg* msgs, uint32_t n_msgs, const gofr_proto_nfield* fields,
+                                       uint32_t n_fields, uint32_t root, const uint8_t* presence, const uint8_t* d_rows,
+                                       const uint32_t* d_row_off, uint32_t n, uint8_t* d_out, uint64_t out_cap, uint32_t* d_out_off,
+                                       uint32_t* d_meta, void* stream) {
+    return proto_nested_run(e, msgs, n_msgs, fields, n_fields, root, presence, d_rows, d_row_off, n, d_out, out_cap, d_out_off, d_meta,
+                            stream, false);
+}
+
+int gofr_proto_decode_nested_ex_device(gofr_engine* e, const gofr_proto_nmsg* msgs, uint32_t n_msgs, const gofr_proto_nfield* fields,
+                                       uint32_t n_fields, uint32_t root, const uint8_t* presence, const uint8_t* d_in,
+                                       const uint32_t* d_in_off, uint32_t n, uint8_t* d_rows, uint64_t rows_cap, uint32_t* d_row_off,
+                                       uint32_t* d_meta, void* stream) {
+    return proto_nested_run(e, msgs, n_msgs, fields, n_fields, root, presence, d_in, d_in_off, n, d_rows, rows_cap, d_row_off, d_meta,
+                            stream, true);
 }
 
 // the descriptor gofr_proto_encode_nested_device would hand to its kernel (tests/emu drives the device code with it)
-int gofr_proto_nested_describe(const gofr_proto_nmsg* msgs, uint32_t n_msgs, const gofr_proto_nfield* fields, uint32_t n_fields,
-                               uint32_t root, void* desc_out, uint32_t desc_cap) {
+int gofr_proto_nested_describe_ex(const gofr_proto_nmsg* msgs, uint32_t n_msgs, const gofr_proto_nfield* fields, uint32_t n_fields,
+                                  uint32_t root, const uint8_t* presence, void* desc_out, uint32_t desc_cap) {
     PbnDesc D;
-    int rc = pbn_build(msgs, n_msgs, fields, n_fields, root, &D);
+    int rc = pbn_build(msgs, n_msgs, fields, n_fields, root, presence, &D);
     if (rc) return rc;
     if (!desc_out || desc_cap < sizeof D) return GOFR_ERR_CAPACITY;
     memcpy(desc_out, &D, sizeof D);
     return GOFR_OK;
+}
+
+int gofr_proto_nested_describe(const gofr_proto_nmsg* msgs, uint32_t n_msgs, const gofr_proto_nfield* fields, uint32_t n_fields,
+                               uint32_t root, void* desc_out, uint32_t desc_cap) {
+    return gofr_proto_nested_describe_ex(msgs, n_msgs, fields, n_fields, root, nullptr, desc_out, desc_cap);
 }
 
 int gofr_proto_encode_device(gofr_engine* e, const gofr_proto_field* fields, uint32_t n_fields, const uint8_t* d_rows,

@@ -101,7 +101,11 @@ enum : uint8_t {
     PBN_MAP = 2u,       // a map field (GOFR_PB_MAP; always with PBN_REPEATED): entries in ascending key order
     PBN_ENTRY = 4u,     // the key or value of a map entry type: written even at its zero value, a value message always
     PBN_SIGNED = 8u,    // an entry's key of a signed integer type (key order)
+    PBN_PRESENCE = 16u, // a singular scalar / string / bytes with explicit presence (proto3 optional, a oneof member): a
+                        // presence word 0 / 1 before its value words; written when set, even at its zero value
+    PBN_ONEOF = 0xE0u,  // the oneof group (1..7) of a member, << PBN_ONEOF_SHIFT; members of type message have this alone
 };
+constexpr int PBN_ONEOF_SHIFT = 5;
 struct PbnField {
     uint32_t tag;        // number << 3 | wire type (2 for messages and for packed repeated scalars)
     uint8_t cls;         // PC_* bits of the scalar type; 0 for a message
@@ -110,7 +114,8 @@ struct PbnField {
     uint8_t fixed_words; // words the field owns in the fixed part of its message
 };
 struct PbnDesc {
-    uint16_t n_msgs;
+    uint8_t n_msgs;
+    uint8_t presence;  // some field has PBN_PRESENCE or PBN_ONEOF bits: the *_presence kernels run it (maps or not)
     uint16_t maps;  // the description has map fields: the *_maps kernels run it (map-free types keep the plain kernels)
     uint32_t root;
     uint16_t first[kPbnMaxMsgs], count[kPbnMaxMsgs], fixed_words[kPbnMaxMsgs];

@@ -15,7 +15,10 @@
 //     value message sent twice is merged -> DEFER as above); across entries a later equal key replaces the earlier entry.
 //     The row holds the map in the encoder's canonical form: keys ascending, each once.  The walks find it by SELECTION —
 //     per output slot, the smallest key above the previous one among all entries, the last entry carrying it — no scratch,
-//     quadratic, so more than kPbnMaxMapEntries entries of one map field in one message (duplicates counted) are DEFER.
+//     quadratic, so more than kPbnMaxMapEntries entries of one map field in one message (duplicates counted) are DEFER;
+//   * explicit presence: an optional field is set iff it occurs (with its own wire type), the last occurrence winning; of a
+//     oneof group the member occurring last among all the group's members is the set one, with its last value.  A message
+//     member sent twice (even with another member between) is DEFER, by the rule for singular message fields above.
 // Three walks per frame, none recursive (explicit stacks, at most kPbnMaxDepth message levels):
 //   validate   wire order: framing of every level that the schema knows, UTF-8, packed payloads, repeated singular messages
 //   size       field order: the row's byte count
@@ -239,8 +242,9 @@ GOFR_HD_NOINLINE uint32_t pdn_validate(const PbnDesc& D, const uint8_t* f, uint3
 GOFR_HD void pdn_st32(uint8_t* p, uint32_t v) { p[0] = (uint8_t)v; p[1] = (uint8_t)(v >> 8); p[2] = (uint8_t)(v >> 16); p[3] = (uint8_t)(v >> 24); }
 
 // ---- walks 2 and 3: field order; EMIT stores into row[] ----
-// Returns the row's byte count before padding.  The frame has been validated: no check can fail here.
-template <bool EMIT, bool MAPS>
+// Returns the row's byte count before padding.  The frame has been validated: no check can fail here.  PRES == true (with
+// MAPS): the instance for descriptions with explicit-presence fields.
+template <bool EMIT, bool MAPS, bool PRES = false>
 GOFR_HD_NOINLINE uint32_t pdn_walk(const PbnDesc& D, const uint8_t* f, uint32_t lo, uint32_t hi, uint8_t* row) {
     // in_rep: 1 elements of a repeated message field in wire order (scan: where to look on), 2 / 3 entries of a map field in
     // key order (3: keys[frame] = the key of the entry taken last)
@@ -294,6 +298,44 @@ GOFR_HD_NOINLINE uint32_t pdn_walk(const PbnDesc& D, const uint8_t* f, uint32_t 
         const uint32_t cls = F.cls;
         PdnItem it;
         uint32_t i = fr.lo;
+        if constexpr (PRES) {
+            if (F.flags & (PBN_PRESENCE | PBN_ONEOF)) {
+                // one pass over the message: the field's last occurrence, and whether a member of its oneof group came
+                // after it (then that member is the set one)
+                const uint32_t group = (uint32_t)F.flags >> PBN_ONEOF_SHIFT;
+                bool set = false;
+                uint32_t g = 0;
+                while (i < fr.hi) {
+                    PdnItem x;
+                    pdn_next(f, &i, fr.hi, &x);
+                    if (x.wt == 3) { g++; continue; }
+                    if (x.wt == 4) { g--; continue; }
+                    if (g) continue;
+                    const int o = pdn_field_of<MAPS>(D, fr.mt, x.num, x.wt);
+                    if (o == (int)q) { set = true; it = x; }
+                    else if (group && o >= 0 && ((uint32_t)fields[o].flags >> PBN_ONEOF_SHIFT) == group) set = false;
+                }
+                if (EMIT) pdn_st32(row + fxo, set ? 1u : 0u);
+                if (F.msg != 0xFF) {  // a oneof member of message type: its fixed part inline (zeros when unset)
+                    if (set) {
+                        Fr& ch = st[depth++];
+                        ch.lo = it.poff; ch.hi = it.poff + it.plen; ch.fx = fxo + 4u; ch.scan = 0; ch.mt = F.msg; ch.fi = 0; ch.in_rep = 0;
+                    } else if (EMIT) for (uint32_t k = 0; k < (uint32_t)D.fixed_words[F.msg] * 4u; k++) row[fxo + 4u + k] = 0;
+                } else if ((cls & PC_WIRE) == 2) {
+                    const uint32_t plen = set ? it.plen : 0u;
+                    if (EMIT) {
+                        pdn_st32(row + fxo + 4u, plen);
+                        for (uint32_t k = 0; k < plen; k++) row[vc + k] = f[it.poff + k];
+                    }
+                    vc += plen;
+                } else {
+                    uint32_t w0 = 0, w1 = 0;
+                    if (set) pdn_scalar_words(cls, it.wt, it.v, &w0, &w1);
+                    if (EMIT) { pdn_st32(row + fxo + 4u, w0); if (cls & PC_64) pdn_st32(row + fxo + 8u, w1); }
+                }
+                continue;
+            }
+        }
         if (!(MAPS ? (F.flags & PBN_REPEATED) : F.flags)) {
             if (F.msg != 0xFF) {  // singular message: presence word + its fixed part inline (zeros when absent)
                 // (a map value is always present: a missing one is an empty message)
@@ -381,9 +423,11 @@ GOFR_HD_NOINLINE uint32_t pdn_walk(const PbnDesc& D, const uint8_t* f, uint32_t 
     return vc;
 }
 
-// size pass of one frame.  The kernels instantiate it for MAPS == D.maps (one kernel per choice, picked on the host: the
-// map-free kernel contains no map code); pdn_decode_size dispatches at run time.
-template <bool MAPS>
+// size pass of one frame.  The kernels instantiate it for MAPS == D.maps and PRES == D.presence (one kernel per choice,
+// picked on the host: the map-free kernel contains no map code, only the presence kernels presence code); pdn_decode_size
+// dispatches at run time.  Validation is the same for both values of PRES: a oneof member of message type is a singular
+// message field (sent twice: DEFER), the other members and optional fields are checked like any singular field.
+template <bool MAPS, bool PRES = false>
 GOFR_HD PdnRow pdn_decode_size_as(const PbnDesc& D, const uint8_t* f, uint32_t fn) {
     PdnRow r = {GOFR_GRPC_OK, 0};
     if (fn < 5) { r.status = GOFR_GRPC_BAD_LENGTH; return r; }
@@ -393,23 +437,25 @@ GOFR_HD PdnRow pdn_decode_size_as(const PbnDesc& D, const uint8_t* f, uint32_t f
     if (L != fn - 5) { r.status = GOFR_GRPC_BAD_LENGTH; return r; }
     r.status = pdn_validate<MAPS>(D, f, 5, 5 + L);
     if (r.status != GOFR_GRPC_OK) return r;
-    r.out_len = (pdn_walk<false, MAPS>(D, f, 5, 5 + L, nullptr) + 3u) & ~3u;
+    r.out_len = (pdn_walk<false, MAPS, PRES>(D, f, 5, 5 + L, nullptr) + 3u) & ~3u;
     return r;
 }
 
 // emit pass: the row at dst (4-byte aligned: every row is a multiple of 4 bytes long)
-template <bool MAPS>
+template <bool MAPS, bool PRES = false>
 GOFR_HD void pdn_decode_emit_as(const PbnDesc& D, const uint8_t* f, uint32_t fn, const PdnRow r, uint8_t* dst) {
     if (!r.out_len) return;
-    uint32_t end = pdn_walk<true, MAPS>(D, f, 5, fn, dst);
+    uint32_t end = pdn_walk<true, MAPS, PRES>(D, f, 5, fn, dst);
     for (; end < r.out_len; end++) dst[end] = 0;
 }
 
 GOFR_HD PdnRow pdn_decode_size(const PbnDesc& D, const uint8_t* f, uint32_t fn) {
+    if (D.presence) return pdn_decode_size_as<true, true>(D, f, fn);
     return D.maps ? pdn_decode_size_as<true>(D, f, fn) : pdn_decode_size_as<false>(D, f, fn);
 }
 GOFR_HD void pdn_decode_emit(const PbnDesc& D, const uint8_t* f, uint32_t fn, const PdnRow r, uint8_t* dst) {
-    if (D.maps) pdn_decode_emit_as<true>(D, f, fn, r, dst);
+    if (D.presence) pdn_decode_emit_as<true, true>(D, f, fn, r, dst);
+    else if (D.maps) pdn_decode_emit_as<true>(D, f, fn, r, dst);
     else pdn_decode_emit_as<false>(D, f, fn, r, dst);
 }
 

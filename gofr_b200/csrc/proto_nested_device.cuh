@@ -12,11 +12,14 @@
 //   * map fields (codec_map.go) are repeated entry messages (1 key, 2 value) whose key and value are written even at their
 //     zero value, a message value always (tag + length 0 when it is nil).  protobuf-go writes entries in Go's random map
 //     order unless Deterministic is set, which sorts the keys; the row carries the entries in that order (checked: strictly
-//     ascending keys, else BAD_ROW), so the bytes are the Deterministic ones.
+//     ascending keys, else BAD_ROW), so the bytes are the Deterministic ones;
+//   * explicit presence (proto3 optional, oneof members; codec_field.go initOneofFieldCoders gives each member its own coder
+//     in the field-number order): a set field is written even at its zero value or empty, an unset one not at all.
 // Rows use the layout of the wider data model (include/gofr_b200.h "Row format"): fixed words of a message in field order
 // (64-bit kinds two words, string / bytes their length, a singular message a presence word + its own fixed part inline, a
-// repeated field its element count), then the variable part in field order (string bytes; a set message's variable part;
-// repeated elements: scalars as their words, strings as u32 length + bytes, messages as fixed part + variable part).
+// repeated field its element count; an explicit-presence scalar / string a presence word before its usual words), then the
+// variable part in field order (string bytes; a set message's variable part; repeated elements: scalars as their words,
+// strings as u32 length + bytes, messages as fixed part + variable part).
 // Device code does not recurse: the walk keeps an explicit stack of at most kPbnMaxDepth message levels (checked on the
 // host when the call is made); the length prefix of a nested message comes from a sizing walk of that message.
 // __host__ __device__ like the rest: tests/emu runs it on the CPU against the oracle and python google.protobuf.
@@ -63,8 +66,9 @@ GOFR_HD int pbn_bytes_cmp(const uint8_t* a, uint32_t an, const uint8_t* b, uint3
 // row).  EMIT == false: returns the size of the message's content, validates the row (*status: GOFR_GRPC_BAD_ROW /
 // GOFR_GRPC_BAD_UTF8) and advances *var past the message's variable part.  EMIT == true: writes the content through w
 // (the row has been validated by the sizing walk of the whole row).  MAPS == false: the instance for descriptions without
-// map fields, with no map code in it.
-template <bool EMIT, bool MAPS>
+// map fields, with no map code in it.  PRES == true (with MAPS): the instance for descriptions with explicit-presence
+// fields (PbnDesc::presence); the others contain no presence code.
+template <bool EMIT, bool MAPS, bool PRES = false>
 GOFR_HD_NOINLINE uint32_t pbn_walk(const PbnDesc& D, uint32_t mt, const uint8_t* fixed, const uint8_t** var_io, const uint8_t* end,
                                    Writer* w, uint32_t* status) {
     PbnFrame st[kPbnMaxDepth + 1];
@@ -77,8 +81,12 @@ GOFR_HD_NOINLINE uint32_t pbn_walk(const PbnDesc& D, uint32_t mt, const uint8_t*
         var += n;
         return p;
     };
+    // SIZE walk, per frame: the oneof groups (bit k: group k) that have a present member so far (kept apart from PbnFrame,
+    // like PbnKey: the instances without presence never touch it)
+    uint8_t groups_set[kPbnMaxDepth + 1];
     auto push = [&](uint32_t m, const uint8_t* fx) {
         if (depth > kPbnMaxDepth) { err = GOFR_GRPC_BAD_ROW; return; }
+        if constexpr (PRES) groups_set[depth] = 0;
         PbnFrame& f = st[depth++];
         f.fixed = fx; f.size = 0; f.rep_left = 0; f.mt = (uint8_t)m; f.fi = 0; f.pend_tl = 0;
     };
@@ -116,7 +124,7 @@ GOFR_HD_NOINLINE uint32_t pbn_walk(const PbnDesc& D, uint32_t mt, const uint8_t*
         if constexpr (EMIT) {  // (constexpr: the sizing instance must not contain a call to itself)
             const uint8_t* v2 = var;
             uint32_t st2 = GOFR_GRPC_OK;
-            const uint32_t sub = pbn_walk<false, MAPS>(D, F.msg, fx, &v2, end, nullptr, &st2);
+            const uint32_t sub = pbn_walk<false, MAPS, PRES>(D, F.msg, fx, &v2, end, nullptr, &st2);
             put_varint(F.tag);
             put_varint(sub);
         } else st[parent].pend_tl = (uint8_t)varint_len(F.tag);
@@ -148,6 +156,32 @@ GOFR_HD_NOINLINE uint32_t pbn_walk(const PbnDesc& D, uint32_t mt, const uint8_t*
         const uint8_t* p = st[fi].fixed + (size_t)wo * 4;
         st[fi].fi++;
         const uint32_t tl = varint_len(F.tag), cls = F.cls, wire = cls & PC_WIRE;
+        if constexpr (PRES) {
+            if (F.flags & (PBN_PRESENCE | PBN_ONEOF)) {  // explicit presence: the presence word, then the value words
+                const uint32_t set = pbn_ld32(p), group = (uint32_t)F.flags >> PBN_ONEOF_SHIFT;
+                if (!EMIT) {  // set is 0 / 1; an unset field's value words are zero; one set member per oneof group
+                    bool bad = set > 1u;
+                    if (!set) for (uint32_t k = 1; k < F.fixed_words; k++) bad |= pbn_ld32(p + 4u * k) != 0u;
+                    if (set && group) { bad |= (groups_set[fi] >> group & 1u) != 0u; groups_set[fi] |= (uint8_t)(1u << group); }
+                    if (bad) { err = GOFR_GRPC_BAD_ROW; break; }
+                }
+                if (!set) continue;
+                const uint8_t* v = p + 4;
+                if (F.msg != 0xFF) enter_message(F, v, fi);
+                else if (wire == 2) {  // written even when empty
+                    const uint32_t len = pbn_ld32(v);
+                    const uint8_t* s = take(len);
+                    if (!s) break;
+                    if (!EMIT && (cls & PC_UTF8) && !proto_utf8_ok(s, len)) { err = GOFR_GRPC_BAD_UTF8; break; }
+                    if (EMIT) { put_varint(F.tag); put_varint(len); if (len) w->copy<false>(s, len); }
+                    st[fi].size += tl + varint_len(len) + len;
+                } else {  // written even at its zero value
+                    if (EMIT) put_varint(F.tag);
+                    st[fi].size += tl + scalar(cls, v);
+                }
+                continue;
+            }
+        }
         // (a map-free description has no flag bits but PBN_REPEATED: its instance tests the byte, as before maps)
         if (!(MAPS ? (F.flags & PBN_REPEATED) : F.flags)) {
             // the key or value of a map entry: written at its zero value too; the key (field index 0) in order (SIZE walk of
@@ -227,22 +261,24 @@ struct PbnMsg {
 };
 
 // size pass of one row: validates it and returns the exact frame length.  The kernels instantiate it for MAPS == D.maps
-// (one kernel per choice, picked on the host: the map-free kernel contains no map code); pbn_size dispatches at run time.
-template <bool MAPS>
+// and PRES == D.presence (one kernel per choice, picked on the host: the map-free kernel contains no map code, only the
+// presence kernels contain presence code — with maps, whether the description has any or not); pbn_size dispatches at
+// run time.
+template <bool MAPS, bool PRES = false>
 GOFR_HD PbnMsg pbn_size_as(const PbnDesc& D, const uint8_t* row, uint32_t rn) {
     PbnMsg m = {GOFR_GRPC_OK, 0};
     const uint32_t fb = (uint32_t)D.fixed_words[D.root] * 4u;
     if (rn < fb) { m.status = GOFR_GRPC_BAD_ROW; return m; }
     const uint8_t* var = row + fb;
     uint32_t st = GOFR_GRPC_OK;
-    const uint32_t len = pbn_walk<false, MAPS>(D, D.root, row, &var, row + rn, nullptr, &st);
+    const uint32_t len = pbn_walk<false, MAPS, PRES>(D, D.root, row, &var, row + rn, nullptr, &st);
     m.status = st;
     m.out_len = st == GOFR_GRPC_OK ? 5u + len : 0u;
     return m;
 }
 
 // emit pass: the frame at dst (arbitrary alignment inside the packed output)
-template <bool MAPS>
+template <bool MAPS, bool PRES = false>
 GOFR_HD void pbn_emit_as(const PbnDesc& D, const uint8_t* row, uint32_t rn, const PbnMsg m, uint8_t* dst, uint32_t* stage_col) {
     if (!m.out_len) return;
     Writer w;
@@ -252,15 +288,17 @@ GOFR_HD void pbn_emit_as(const PbnDesc& D, const uint8_t* row, uint32_t rn, cons
     w.putc(plen & 0xFF);
     const uint8_t* var = row + (size_t)D.fixed_words[D.root] * 4;
     uint32_t st = GOFR_GRPC_OK;
-    pbn_walk<true, MAPS>(D, D.root, row, &var, row + rn, &w, &st);
+    pbn_walk<true, MAPS, PRES>(D, D.root, row, &var, row + rn, &w, &st);
     w.finish();
 }
 
 GOFR_HD PbnMsg pbn_size(const PbnDesc& D, const uint8_t* row, uint32_t rn) {
+    if (D.presence) return pbn_size_as<true, true>(D, row, rn);
     return D.maps ? pbn_size_as<true>(D, row, rn) : pbn_size_as<false>(D, row, rn);
 }
 GOFR_HD void pbn_emit(const PbnDesc& D, const uint8_t* row, uint32_t rn, const PbnMsg m, uint8_t* dst, uint32_t* stage_col) {
-    if (D.maps) pbn_emit_as<true>(D, row, rn, m, dst, stage_col);
+    if (D.presence) pbn_emit_as<true, true>(D, row, rn, m, dst, stage_col);
+    else if (D.maps) pbn_emit_as<true>(D, row, rn, m, dst, stage_col);
     else pbn_emit_as<false>(D, row, rn, m, dst, stage_col);
 }
 

@@ -389,6 +389,7 @@ def pack_proto_rows(fields: Sequence[ProtoField], messages: Sequence[Sequence]) 
 
 PB_MESSAGE = 11
 PB_MAP = 32          # a map field: msg is its entry type (fields 1 key, 2 value); not repeated
+PB_OPTIONAL = 0x80   # ProtoNField.presence: proto3 optional (1..7: a member of that oneof group)
 
 
 @dataclass
@@ -398,6 +399,19 @@ class ProtoNField:
     type: int            # PB_*, PB_MESSAGE or PB_MAP
     repeated: bool = False
     msg: int = 0         # PB_MESSAGE: index of the message type; PB_MAP: index of the entry type
+    presence: int = 0    # 0 implicit presence, PB_OPTIONAL, or 1..7: a member of that oneof group of its message type
+
+
+def _explicit(f: ProtoNField) -> bool:
+    """a scalar / string / bytes field with a presence word of its own in the row"""
+    return bool(f.presence) and f.type not in (PB_MESSAGE, PB_MAP) and not f.repeated
+
+
+def proto_nested_presence(msgs: Sequence[Sequence[ProtoNField]]):
+    """the presence bytes of the _ex calls (one per field, in the order of proto_nested_tables), or None when no field has
+    explicit presence (then the calls without presence are the same)"""
+    pr = [f.presence for fields in msgs for f in fields]
+    return np.array(pr, dtype=np.uint8) if any(pr) else None
 
 
 def proto_nested_tables(msgs: Sequence[Sequence[ProtoNField]]):
@@ -448,7 +462,7 @@ def _pb_fixed_bytes(msgs, m: int) -> int:
         elif f.type == PB_MESSAGE:
             n += 4 + _pb_fixed_bytes(msgs, f.msg)
         else:
-            n += 8 if f.type in PB_64BIT or f.type == PB_DOUBLE else 4
+            n += (8 if f.type in PB_64BIT or f.type == PB_DOUBLE else 4) + (4 if _explicit(f) else 0)
     return n
 
 
@@ -456,7 +470,8 @@ def pack_proto_nested_message(msgs, m: int, value) -> "tuple[bytes, bytes]":
     """(fixed part, variable part) of one message of type m.  value: one entry per field — scalars as for pack_proto_rows, a
     singular message None (not set) or its own value list, a repeated field a list.  A map field takes a dict, whose
     entries are laid out in protobuf-go's Deterministic key order (map_key_order), or a list of (key, value) pairs laid
-    out as given (unsorted or duplicate keys make a row the encoder refuses); a message value None is a nil message."""
+    out as given (unsorted or duplicate keys make a row the encoder refuses); a message value None is a nil message.  A
+    scalar, string or bytes field with explicit presence (optional, a oneof member) takes None for "not set"."""
     def element(f, v) -> bytes:
         if f.type in (PB_STRING, PB_BYTES):
             b = v.encode("utf-8", "surrogateescape") if isinstance(v, str) else bytes(v)
@@ -483,6 +498,16 @@ def pack_proto_nested_message(msgs, m: int, value) -> "tuple[bytes, bytes]":
                 fx, vr = pack_proto_nested_message(msgs, f.msg, v)
                 fixed += (1).to_bytes(4, "little") + fx
                 var += vr
+        elif _explicit(f) and v is None:
+            fixed += bytes(4 + (8 if f.type in PB_64BIT or f.type == PB_DOUBLE else 4))
+        elif _explicit(f):
+            fixed += (1).to_bytes(4, "little")
+            if f.type in (PB_STRING, PB_BYTES):
+                b = v.encode("utf-8", "surrogateescape") if isinstance(v, str) else bytes(v)
+                fixed += len(b).to_bytes(4, "little")
+                var += b
+            else:
+                fixed += _pb_scalar_words(f.type, v)
         elif f.type in (PB_STRING, PB_BYTES):
             b = v.encode("utf-8", "surrogateescape") if isinstance(v, str) else bytes(v)
             fixed += len(b).to_bytes(4, "little")

@@ -455,6 +455,40 @@ int gofr_proto_decode_nested_device(gofr_engine*, const gofr_proto_nmsg* msgs, u
 int gofr_proto_nested_describe(const gofr_proto_nmsg* msgs, uint32_t n_msgs, const gofr_proto_nfield* fields, uint32_t n_fields,
                                uint32_t root, void* desc_out, uint32_t desc_cap);
 
+/* FIELD PRESENCE: the three calls above with `presence`, one byte per entry of `fields` (NULL: exactly the call above).
+ *   0                  implicit presence, as above;
+ *   GOFR_PB_OPTIONAL   a proto3 `optional` field (explicit presence; protoreflect: fd.HasOptionalKeyword());
+ *   1 .. 7             a member of oneof group k of its message type (protoreflect: fd.ContainingOneof() when it is not
+ *                      synthetic; at most 7 groups per message type).
+ * A oneof member is singular (not repeated, not a map); the key and value of a map entry type carry no presence; optional
+ * on a message field means what a singular message field means anyway.  Anything else is GOFR_ERR_INVALID.
+ * Rows: an explicit-presence scalar, string or bytes field (optional, or a oneof member) owns a PRESENCE WORD 0 / 1
+ * followed by its usual words in the fixed part; its string bytes are in the variable part only when it is set.  A
+ * message-typed member keeps the layout of a singular message field (presence word + its fixed part inline).  Each oneof
+ * member has its own slot, in field order.  The encoder refuses (GOFR_GRPC_BAD_ROW) a presence word other than 0 / 1 on
+ * such a field, an unset one whose value words (a message member: its inline fixed part) are not all zero, and more than
+ * one set member in one oneof group — so decode(encode(row)) == row for every row it accepts.
+ * Encoder (proto.Marshal, protobuf-go v1.32.0): a set field is written even at its zero value or empty, an unset one not
+ * at all; members go out at their own field numbers, in field-number order.  Decoder (proto.Unmarshal): an optional field
+ * is set iff it occurs with its own wire type, the last occurrence winning; in a oneof group, the member whose occurrence is
+ * last among all the group's members is the set one, with its last value, and the others are unset.  A member arriving
+ * with a foreign wire type is an unknown field and does not change the case.  A message member that occurs twice at one
+ * message level is GOFR_GRPC_DEFER, even with another member in between (protobuf-go merges A, A and replaces in A, B, A:
+ * either way, decode it on the host).  UTF-8 is checked on every occurrence, the losing members' too; status precedence
+ * malformed > invalid UTF-8 > DEFER as above.  The flat codec (gofr_proto_encode_device / _decode_device) has no presence:
+ * a flat message type with it goes through these calls. */
+#define GOFR_PB_OPTIONAL 0x80u
+int gofr_proto_encode_nested_ex_device(gofr_engine*, const gofr_proto_nmsg* msgs, uint32_t n_msgs, const gofr_proto_nfield* fields,
+                                       uint32_t n_fields, uint32_t root, const uint8_t* presence, const uint8_t* d_rows,
+                                       const uint32_t* d_row_off, uint32_t n, uint8_t* d_out, uint64_t out_cap, uint32_t* d_out_off,
+                                       uint32_t* d_meta, void* stream);
+int gofr_proto_decode_nested_ex_device(gofr_engine*, const gofr_proto_nmsg* msgs, uint32_t n_msgs, const gofr_proto_nfield* fields,
+                                       uint32_t n_fields, uint32_t root, const uint8_t* presence, const uint8_t* d_in,
+                                       const uint32_t* d_in_off, uint32_t n, uint8_t* d_rows, uint64_t rows_cap, uint32_t* d_row_off,
+                                       uint32_t* d_meta, void* stream);
+int gofr_proto_nested_describe_ex(const gofr_proto_nmsg* msgs, uint32_t n_msgs, const gofr_proto_nfield* fields, uint32_t n_fields,
+                                  uint32_t root, const uint8_t* presence, void* desc_out, uint32_t desc_cap);
+
 /* Bind as a stage of the split API: Context.Bind(&v) for closures that stay on the host (pkg/gofr/context.go:52-54 ->
  * pkg/gofr/http/request.go:40-47 -> json.Unmarshal(body, &v), v a struct of a registered schema).  Body i is the data
  * section of request i (same descriptors / arena as the serve calls); result i lies in its own slot d_rows + i * slot_bytes

@@ -6,6 +6,11 @@ Workloads (1 Mi messages each; 1024 distinct rows repeated):
    b  M { map<string, string> labels = 1; map<int64, Item> items = 2; } with 8 labels and 8 items
    c  the same type with 64 labels and 64 items (short strings, no tags): the decoder's worst case (selection over 64
       entries per map)
+   d  Event { int64 id = 1; optional string note = 2; optional int64 parent = 3;
+              oneof payload { Click click = 4; string text = 5; int64 code = 6; } repeated Tag tags = 7; }
+      (field presence: the *_presence kernels through the _ex calls) with about half of the optional fields set and the
+      oneof cases (none, click, text, code) spread evenly
+A workload named twice in --only (a,d,a,d) runs again on the same rows: alternate two workloads to see the noise.
 The decoder runs on the encoder's output.  CUDA events around `steps` launches after 3 warm-up launches; one JSON line per
 workload and direction, after the card's name, power limit and max SM clock (nvidia-smi, read-only query)."""
 import argparse
@@ -32,6 +37,22 @@ MAP_MSGS = [[F(1, S.PB_MAP, False, 1), F(2, S.PB_MAP, False, 2)],
             [F(1, S.PB_STRING), F(2, S.PB_STRING)],
             [F(1, S.PB_INT64), F(2, S.PB_MESSAGE, False, 3)],
             ITEM]
+OPT = S.PB_OPTIONAL
+EVENT_MSGS = [[F(1, S.PB_INT64), F(2, S.PB_STRING, presence=OPT), F(3, S.PB_INT64, presence=OPT), F(4, S.PB_MESSAGE, False, 1, 1),
+               F(5, S.PB_STRING, presence=1), F(6, S.PB_INT64, presence=1), F(7, S.PB_MESSAGE, True, 2)],
+              [F(1, S.PB_INT32), F(2, S.PB_INT32)],        # Click { int32 x = 1; int32 y = 2; }
+              [F(1, S.PB_STRING)]]                          # Tag { string name = 1; }
+
+
+def event_value(rnd, i):
+    case = i % 4                                            # the oneof: unset, click, text, code
+    return [rnd.randint(1, 10 ** 12),
+            "note-%d" % rnd.randint(0, 999) if rnd.random() < 0.5 else None,
+            rnd.randint(0, 10 ** 9) if rnd.random() < 0.5 else None,
+            [rnd.randint(0, 1920), rnd.randint(0, 1080)] if case == 1 else None,
+            "text-%d" % rnd.randint(0, 10 ** 6) if case == 2 else None,
+            rnd.randint(-10 ** 6, 10 ** 6) if case == 3 else None,
+            [["tag-%d" % rnd.randint(0, 99)] for _ in range(rnd.randint(0, 3))]]
 
 
 def map_value(rnd, n, compact=False):
@@ -84,15 +105,20 @@ def main():
     rnd = random.Random(5)
     work = {"a": (MSGS, lambda: [_rand_value(rnd, MSGS, 0) for _ in range(1024)]),
             "b": (MAP_MSGS, lambda: [map_value(rnd, 8) for _ in range(1024)]),
-            "c": (MAP_MSGS, lambda: [map_value(rnd, 64, compact=True) for _ in range(1024)])}
+            "c": (MAP_MSGS, lambda: [map_value(rnd, 64, compact=True) for _ in range(1024)]),
+            "d": (EVENT_MSGS, lambda: [event_value(rnd, i) for i in range(1024)])}
+    cache = {}
     eng = Engine(Table(synth.config1_spec()), 0)
     L = _abi.lib()
     st = torch.cuda.current_stream().cuda_stream
     for w in a.only.split(","):
         msgs, gen = work[w]
-        rows, off = tiled_rows(msgs, gen(), a.n)
+        if w not in cache:
+            cache[w] = tiled_rows(msgs, gen(), a.n)
+        rows, off = cache[w]
         n = a.n
         nm, nf, k = S.proto_nested_tables(msgs)
+        pr = S.proto_nested_presence(msgs)
         d_rows = torch.from_numpy(rows).cuda()
         d_off = torch.from_numpy(off.view(np.int32)).cuda()
         cap = int(off[-1]) * 2 + 64 * n
@@ -101,6 +127,11 @@ def main():
         d_meta = torch.zeros(n, dtype=torch.int32, device="cuda")
 
         def enc():
+            if pr is not None:
+                _abi.check(L.gofr_proto_encode_nested_ex_device(eng._e, nm.ctypes.data, len(msgs), nf.ctypes.data, k, 0, pr.ctypes.data,
+                                                                d_rows.data_ptr(), d_off.data_ptr(), n, d_out.data_ptr(), cap,
+                                                                d_out_off.data_ptr(), d_meta.data_ptr(), st), "encode")
+                return
             _abi.check(L.gofr_proto_encode_nested_device(eng._e, nm.ctypes.data, len(msgs), nf.ctypes.data, k, 0, d_rows.data_ptr(),
                                                          d_off.data_ptr(), n, d_out.data_ptr(), cap, d_out_off.data_ptr(),
                                                          d_meta.data_ptr(), st), "encode")
@@ -113,6 +144,11 @@ def main():
         d_meta2 = torch.zeros(n, dtype=torch.int32, device="cuda")
 
         def dec():
+            if pr is not None:
+                _abi.check(L.gofr_proto_decode_nested_ex_device(eng._e, nm.ctypes.data, len(msgs), nf.ctypes.data, k, 0, pr.ctypes.data,
+                                                                d_out.data_ptr(), d_out_off.data_ptr(), n, d_back.data_ptr(), rows_cap,
+                                                                d_back_off.data_ptr(), d_meta2.data_ptr(), st), "decode")
+                return
             _abi.check(L.gofr_proto_decode_nested_device(eng._e, nm.ctypes.data, len(msgs), nf.ctypes.data, k, 0, d_out.data_ptr(),
                                                          d_out_off.data_ptr(), n, d_back.data_ptr(), rows_cap, d_back_off.data_ptr(),
                                                          d_meta2.data_ptr(), st), "decode")
