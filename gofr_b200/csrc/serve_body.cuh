@@ -16,7 +16,7 @@
 //   * each thread streams its response through a funnel-shift word writer (serve_device.cuh) whose completed words
 //     collect in a conflict-free shared-memory ring and leave for HBM as whole 32-byte sectors, two 16-byte
 //     st.global.cs.v4 each; in the slot layout's fast path lane pairs share those stores, so every warp store
-//     covers whole sectors (Writer::store32_paired).  No output tile lives in shared
+//     covers whole sectors (the PairStores store policy).  No output tile lives in shared
 //     memory, which keeps 5 CTAs (20 warps) resident per SM for this latency-bound byte work.
 #pragma once
 #include <cuda_runtime.h>
@@ -74,10 +74,10 @@ static __device__ __noinline__ void general_pass(const ServeParams* pp, const Ta
         emit_request_general<true>(tv, br, c, p.out + (size_t)r * p.slot_bytes, &sh->ring[tid]);
 }
 
-// PAIRS (slot layout): the fast path stores sectors in lane pairs (emit_fast_paired).  Its store rounds are warp-uniform, so a
-// warp whose lanes run different programs makes every lane take every other lane's rounds: on mixed traffic (config 4:
-// 0.31 -> 0.35 ms on an H100 SXM at 400 W) that costs more than whole-sector stores gain.  Only the wide instance, which the
-// engine runs for tables with one fast-path program shape, pairs.
+// PAIRS (slot layout): the fast path stores sectors in lane pairs (emit_fast with PairStores).  Its store rounds are
+// warp-uniform, so a warp whose lanes run different programs makes every lane take every other lane's rounds: on mixed
+// traffic (config 4: 0.31 -> 0.35 ms on an H100 SXM at 400 W) that costs more than whole-sector stores gain.  Only the
+// wide instance, which the engine runs for tables with one fast-path program shape, pairs.
 template <bool SLOTS, bool PAIRS = false>
 __device__ __forceinline__ void serve_body(const ServeParams& p) {
     // (p is a __grid_constant__ kernel parameter: its address can be handed to the out-of-line general pass)
@@ -247,7 +247,7 @@ __device__ __forceinline__ void serve_body(const ServeParams& p) {
                     p.meta[r] = request_status(tv, c) | (c.route << 16);
                     if (c.total_len <= p.slot_bytes && c.total_len) {
                         if (PAIRS) emit = true;
-                        else emit_fast(tv, br, c, p.out + (size_t)r * p.slot_bytes, &sh.ring[tid]);
+                        else emit_fast(tv, br, c, p.out + (size_t)r * p.slot_bytes, &sh.ring[tid], SoloStores{});
                     }
                 } else {
                     p.out_off[r] = kDeferred;  // left for the general pass after the tile loop
@@ -256,7 +256,7 @@ __device__ __forceinline__ void serve_body(const ServeParams& p) {
             if (PAIRS) {
                 // every thread of the CTA is here: the lanes that write a response form the pair mask
                 const uint32_t pm = __ballot_sync(0xFFFFFFFFu, emit);
-                if (emit) emit_fast_paired(tv, br, c, p.out + (size_t)r * p.slot_bytes, &sh.ring[tid], pm);
+                if (emit) emit_fast(tv, br, c, p.out + (size_t)r * p.slot_bytes, &sh.ring[tid], PairStores{pm});
             }
             continue;
         }

@@ -88,12 +88,12 @@ GOFR_HD bool warp_any(bool p) {
 // plus the few edge bytes a response shares with its neighbours.  sm_90 has no 256-bit store, so a sector is two 16-byte
 // st.global.cs.v4.  When one lane issues both, a warp store touches 32 sectors 528 bytes apart (the config-2 slots) and
 // fills half of each.  Storing 1 Mi such slots and nothing else, at full occupancy (scratch/experiments/sector_stores,
-// H100 SXM at 400 W; the times rank store patterns, they are not the serve kernel's store cost), took 1.82 ms.  So where the
-// caller names the lanes that run the Writer together (the pair mask: the fast path of the wide slot-layout instance,
-// serve_body.cuh PAIRS), lanes 2k and 2k+1 share
-// both stores: the first writes the even lane's sector, the second the odd lane's, each lane one half of each, and every
-// warp store covers 16 whole sectors (0.60 ms for the same slots; fully coalesced rows 0.17 ms).  A lane whose partner has
-// no sector in a round, and every path without a pair mask, stores its own sector as two back-to-back halves.
+// H100 SXM at 400 W; the times rank store patterns, they are not the serve kernel's store cost), took 1.82 ms.  How
+// sectors leave is the store policy the caller passes to flush, copy and finish_padded (below): SoloStores, the default,
+// stores each lane's sector as two back-to-back halves; with PairStores (the fast path of the wide slot-layout instance,
+// serve_body.cuh PAIRS) lanes 2k and 2k+1 share both stores: the first writes the even lane's sector, the second the
+// odd lane's, each lane one half of each, and every warp store covers 16 whole sectors (0.60 ms for the same slots;
+// fully coalesced rows 0.17 ms).
 //
 // Each thread owns a 16-word staging buffer in shared memory, laid out word-major (word k of thread t at
 // [k * CTA + t]): whatever word index a lane is at, its bank is its lane id, so accesses never conflict.  The buffer is
@@ -104,7 +104,7 @@ GOFR_HD bool warp_any(bool p) {
 //            bytes treated as a prefix of the source ("virtual source"): one aligned load + one funnel shift per
 //            output word regardless of source and destination alignment.
 //   flush:   decoupled from producing — between ops, when at least 8 words wait, whole sectors leave as
-//            8 conflict-free LDS + two st.global.cs.v4 (flush_paired: shared by a lane pair as above); no shifting
+//            8 conflict-free LDS + two st.global.cs.v4 (PairStores: shared by a lane pair as above); no shifting
 //            is needed because the buffer is already aligned.
 //   edges:   the first sector's leading `lead` bytes and the last sector's tail belong to neighbouring responses
 //            written by other threads; only this response's bytes are stored there.
@@ -189,17 +189,78 @@ GOFR_HD uint32_t load_bytes(const uint8_t* p, uint32_t k) {
     return fsr(w0, w1, o * 8);
 }
 
-// Pair mask `pm`: the lanes of the warp that make every call of a store routine below together (0: this lane alone, no
-// pairing).  A store round with a pair mask runs while any lane of it still has something to store; a lane with nothing
-// takes part with `have` false.
-GOFR_HD bool pair_round(uint32_t pm, bool have) {
+// 16 bytes at the 16-byte aligned addr: the one global store of a whole sector half
+GOFR_HD void store16(uint8_t* addr, uint32_t v0, uint32_t v1, uint32_t v2, uint32_t v3) {
 #if defined(__CUDA_ARCH__)
-    return pm ? __any_sync(pm, have) : have;
+#if defined(GOFR_EXP_NO_STORE)  /* experiment: the kernel without its global stores (what is left is issue/latency bound) */
+    if (v0 == 0x12345678u && v1 == 0x9ABCDEF0u && v2 == 0x0F1E2D3Cu)
+#endif
+    __stcs((uint4*)addr, make_uint4(v0, v1, v2, v3));
 #else
-    (void)pm;
-    return have;
+    uint32_t v[4] = {v0, v1, v2, v3};
+    memcpy(addr, v, 16);
 #endif
 }
+
+// Store policies of the Writer's flush, copy and finish_padded, and of emit_fast: how the lanes that run them take a flush
+// decision (vote), how long a store round runs (round: while the lane, or its group, has something to store), and how
+// a whole 32-byte sector leaves (store32: the sector v0..v7 at the 32-byte aligned addr, if `have`).  kLockstep: every
+// lane of the group makes every call of these routines together, also with nothing to store.
+//
+// SoloStores: each lane on its own, its sector as two back-to-back 16-byte stores; a flush decision is taken by all
+// active lanes of the warp.
+struct SoloStores {
+    static constexpr bool kLockstep = false;
+    GOFR_HD bool vote(bool p) const { return warp_any(p); }
+    GOFR_HD bool round(bool have) const { return have; }
+    GOFR_HD void store32(bool have, uint8_t* addr, uint32_t v0, uint32_t v1, uint32_t v2, uint32_t v3, uint32_t v4,
+                         uint32_t v5, uint32_t v6, uint32_t v7) const {
+        if (have) { store16(addr, v0, v1, v2, v3); store16(addr + 16, v4, v5, v6, v7); }
+    }
+};
+// PairStores: the lanes of the pair mask pm take every decision and run every round together, while any of them still
+// has something to store (a lane with nothing takes part with `have` false).  When lanes 2k and 2k+1 both have a
+// sector, they write them together: in each of the two 16-byte stores the even lane writes the lower and the odd lane
+// the upper half of one sector (first the even lane's, then the odd lane's), so each warp store covers whole sectors.  A
+// lane whose partner has no sector writes both halves of its own.  On the host (tests/emu) lanes run one at a time: pm
+// is ignored, and the vote is warp_any's so that the emulation replays extra flushes here too.
+struct PairStores {
+    uint32_t pm;
+    static constexpr bool kLockstep = true;
+    GOFR_HD bool vote(bool p) const {
+#if defined(__CUDA_ARCH__)
+        return __any_sync(pm, p);
+#else
+        return warp_any(p);
+#endif
+    }
+    GOFR_HD bool round(bool have) const {
+#if defined(__CUDA_ARCH__)
+        return __any_sync(pm, have);
+#else
+        return have;
+#endif
+    }
+    GOFR_HD void store32(bool have, uint8_t* addr, uint32_t v0, uint32_t v1, uint32_t v2, uint32_t v3, uint32_t v4,
+                         uint32_t v5, uint32_t v6, uint32_t v7) const {
+        uint8_t* a0 = addr;
+        uint8_t* a1 = addr + 16;
+#if defined(__CUDA_ARCH__)
+        {
+            const uint32_t lane = threadIdx.x & 31u, odd = lane & 1u;
+            const uint32_t haves = __ballot_sync(pm, have);  // by every lane of pm: not behind a short-circuit on `have`
+            const bool pair = have && ((haves >> (lane ^ 1u)) & 1u);
+            // the half the partner writes: the even lane's upper half, the odd lane's lower half
+            const uint32_t x0 = __shfl_xor_sync(pm, odd ? v0 : v4, 1), x1 = __shfl_xor_sync(pm, odd ? v1 : v5, 1);
+            const uint32_t x2 = __shfl_xor_sync(pm, odd ? v2 : v6, 1), x3 = __shfl_xor_sync(pm, odd ? v3 : v7, 1);
+            uint8_t* const pa = (uint8_t*)__shfl_xor_sync(pm, (unsigned long long)addr, 1);
+            if (pair && odd) { a0 = pa + 16; v0 = x0; v1 = x1; v2 = x2; v3 = x3; }
+            if (pair && !odd) { a1 = pa; v4 = x0; v5 = x1; v6 = x2; v7 = x3; }
+        }
+#endif
+        if (have) { store16(a0, v0, v1, v2, v3); store16(a1, v4, v5, v6, v7); }
+    }
+};
 
 struct Writer {
     uint8_t* chunk;  // 32-byte aligned global address that staging word 0 maps to
@@ -221,42 +282,11 @@ struct Writer {
     }
     GOFR_HD uint32_t word(uint32_t k) const { return stg_ld(base + k * GOFR_RING_STRIDE_BYTES); }
 
-    GOFR_HD static void store16(uint8_t* addr, uint32_t v0, uint32_t v1, uint32_t v2, uint32_t v3) {
-#if defined(__CUDA_ARCH__)
-#if defined(GOFR_EXP_NO_STORE)  /* experiment: the kernel without its global stores (what is left is issue/latency bound) */
-        if (v0 == 0x12345678u && v1 == 0x9ABCDEF0u && v2 == 0x0F1E2D3Cu)
-#endif
-        __stcs((uint4*)addr, make_uint4(v0, v1, v2, v3));
-#else
-        uint32_t v[4] = {v0, v1, v2, v3};
-        memcpy(addr, v, 16);
-#endif
-    }
-    // One whole sector from this lane alone: addr is 32-byte aligned.  sm_90 has no 256-bit global store, so it is two
-    // back-to-back 16-byte stores (store32_paired shares them between two lanes).
-    template <int SITE = 0>
-    GOFR_HD static void store32(uint8_t* addr, uint32_t v0, uint32_t v1, uint32_t v2, uint32_t v3, uint32_t v4, uint32_t v5,
-                                uint32_t v6, uint32_t v7) {
-#if defined(__CUDA_ARCH__)
-#if defined(GOFR_EXP_NO_STORE)
-        if (v0 == 0x12345678u && v1 == 0x9ABCDEF0u && v2 == 0x0F1E2D3Cu)
-#endif
-        { __stcs((uint4*)addr, make_uint4(v0, v1, v2, v3)); __stcs((uint4*)(addr + 16), make_uint4(v4, v5, v6, v7)); }
-#else
-        uint32_t v[8] = {v0, v1, v2, v3, v4, v5, v6, v7};
-        memcpy(addr, v, 32);
-#endif
-    }
     // Write bytes [lo, hi) of the 32-byte sector at addr from the eight staging words at rp: a 16-byte half where one is
     // whole, else words, else single bytes.  Runs twice per response at most (first and last sector), so it is a loop,
     // not unrolled code.
-#if defined(__CUDA_ARCH__) && defined(GOFR_EXP_STG_PARTIAL)
-    static __device__ __forceinline__ void st8(uint8_t* a, uint32_t v) { asm volatile("st.global.u8 [%0], %1;" ::"l"(a), "r"(v) : "memory"); }
-    static __device__ __forceinline__ void st32(uint8_t* a, uint32_t v) { asm volatile("st.global.u32 [%0], %1;" ::"l"(a), "r"(v) : "memory"); }
-#else
     GOFR_HD static void st8(uint8_t* a, uint32_t v) { *a = (uint8_t)v; }
     GOFR_HD static void st32(uint8_t* a, uint32_t v) { *(uint32_t*)a = v; }
-#endif
     GOFR_HD static void store_partial(uint8_t* addr, saddr_t rp, uint32_t lo, uint32_t hi) {
         uint32_t b = lo;
 #pragma unroll 1
@@ -274,14 +304,9 @@ struct Writer {
 #pragma unroll 1
         for (; b < hi; b++) st8(addr + b, stg_ld8(rp + (b >> 2) * GOFR_RING_STRIDE_BYTES + (b & 3u)));
     }
-    GOFR_HD void store_sector(saddr_t rp) {
-        store32(chunk, stg_ld(rp), stg_ld(rp + GOFR_RING_STRIDE_BYTES), stg_ld(rp + 2 * GOFR_RING_STRIDE_BYTES),
-                stg_ld(rp + 3 * GOFR_RING_STRIDE_BYTES), stg_ld(rp + 4 * GOFR_RING_STRIDE_BYTES),
-                stg_ld(rp + 5 * GOFR_RING_STRIDE_BYTES), stg_ld(rp + 6 * GOFR_RING_STRIDE_BYTES),
-                stg_ld(rp + 7 * GOFR_RING_STRIDE_BYTES));
-    }
     // store every complete sector, move the (< 8) left-over words to the front
-    GOFR_HD void flush() {
+    template <typename P = SoloStores>
+    GOFR_HD void flush(P p = P()) {
         uint32_t n = wl >> 3;
         saddr_t rp = base;
         if (n && lead) {  // first sector of the response: skip the neighbour's bytes
@@ -292,10 +317,20 @@ struct Writer {
             n--;
         }
 #pragma unroll 1
-        for (; n; n--) {
-            store_sector(rp);
-            chunk += 32;
-            rp += 8 * GOFR_RING_STRIDE_BYTES;
+        while (p.round(n != 0)) {
+            const bool have = n != 0;
+            uint8_t* const at = chunk;
+            uint32_t v[8] = {0u, 0u, 0u, 0u, 0u, 0u, 0u, 0u};
+            if (have) {  // a lane without a sector may be at the end of its column: it reads nothing
+#pragma unroll
+                for (uint32_t j = 0; j < 8; j++) v[j] = stg_ld(rp + j * GOFR_RING_STRIDE_BYTES);
+            }
+            p.store32(have, at, v[0], v[1], v[2], v[3], v[4], v[5], v[6], v[7]);
+            if (have) {
+                chunk += 32;
+                rp += 8 * GOFR_RING_STRIDE_BYTES;
+                n--;
+            }
         }
         const uint32_t r = wl & 7;
         if (wl >= 8 && r) {
@@ -361,168 +396,12 @@ struct Writer {
     // previous one is carried) and one funnel shift.  Only word 0 mixes in `pend`.
     // Sources must be readable up to the end of the aligned word following their last byte (literal pool, staged
     // arena and blobs are padded accordingly); no byte before the source is ever read.
-    template <bool SH>
-    GOFR_HD void copy(typename SrcMem<SH>::A src, uint32_t len) {
+    // With PairStores every lane of the pair mask makes the call, also with len 0, and takes the flush and long-copy
+    // rounds below.
+    template <bool SH, typename P = SoloStores>
+    GOFR_HD void copy(typename SrcMem<SH>::A src, uint32_t len, P p = P()) {
         typedef SrcMem<SH> M;
-        if (!len) return;
-        const uint32_t yo = (M::low2(src) - nb) & 3u, sh = yo * 8;
-        typename M::A Y = src - nb - yo;  // aligned word that holds stream byte 0
-        const uint32_t total = nb + len;
-        uint32_t nwords = total >> 2;
-        const uint32_t nn = total & 3;
-        // Y[0] holds source bytes iff the source starts inside it
-        uint32_t cur = (yo + nb < 4) ? M::ld(Y) : 0u;
-        uint32_t nxt = (yo + total > 4) ? M::ld(Y + 4) : 0u;  // second word needed only if the data reaches it
-        uint32_t w0 = fsr(cur, nxt, sh);
-        if (nb) w0 = (w0 & (0xFFFFFFFFu << (8 * nb))) | (pend >> (8 * (4 - nb)));
-        if (nwords == 0) {  // still inside the same word
-            pend = w0 << (8 * (4 - nn));
-            nb = nn;
-            return;
-        }
-        reserve(8);  // at most 8 words staged from here on: this word + (head <= 7 | a short copy <= 7)
-        store_word(w0);
-        cur = nxt;
-        Y += 8;  // Y now points at the NEXT word to load
-        nwords--;
-        if (nwords >= 8) {
-            // Long copy.  Head: complete the sector under construction (<= 7 more words), store it; from then on the
-            // staging buffer is empty and whole sectors go from registers straight to HBM.
-            const uint32_t h = (8u - (wl & 7u)) & 7u;
-            if (h & 4u) stream_words<M, 4>(Y, cur, sh);
-            if (h & 2u) stream_words<M, 2>(Y, cur, sh);
-            if (h & 1u) stream_words<M, 1>(Y, cur, sh);
-            nwords -= h;
-            flush();  // wl is a multiple of 8: nothing is left behind
-#pragma unroll 1
-            while (nwords >= 8) {
-                const uint32_t n0 = M::ld(Y), n1 = M::ld(Y + 4), n2 = M::ld(Y + 8), n3 = M::ld(Y + 12);
-                const uint32_t n4 = M::ld(Y + 16), n5 = M::ld(Y + 20), n6 = M::ld(Y + 24), n7 = M::ld(Y + 28);
-                store32<1>(chunk, fsr(cur, n0, sh), fsr(n0, n1, sh), fsr(n1, n2, sh), fsr(n2, n3, sh), fsr(n3, n4, sh),
-                           fsr(n4, n5, sh), fsr(n5, n6, sh), fsr(n6, n7, sh));
-                chunk += 32;
-                cur = n7;
-                Y += 32;
-                nwords -= 8;
-            }
-        }
-        // <= 7 words left: 4 + 2 + 1, each group with its loads issued together and immediate offsets (a word-at-a-time
-        // loop spends more on its counters than on the words)
-        if (nwords & 4u) stream_words<M, 4>(Y, cur, sh);
-        if (nwords & 2u) stream_words<M, 2>(Y, cur, sh);
-        if (nwords & 1u) stream_words<M, 1>(Y, cur, sh);
-        if (nn) {
-            // the partial last word: its bytes may or may not spill into the next aligned word
-            nxt = (yo + nn > 4) ? M::ld(Y) : 0u;
-            pend = fsr(cur, nxt, sh) << (8 * (4 - nn));
-        }
-        nb = nn;
-    }
-    // Slot layout (gofr_serve_device_slots): the response owns its 16-byte aligned slot, so the last 16-byte chunk is
-    // stored whole, zero padded — no byte stores, nothing of a neighbour to preserve.  A slot starts either on a sector
-    // boundary or in the middle of one (lead 0 or 16).
-    GOFR_HD void finish_padded() {
-        flush();
-        const uint32_t end = 4 * wl + nb;  // bytes of the last sector in use, phantom lead included
-        if (end > lead) {
-            const uint32_t tail = nb ? pend >> (8 * (4 - nb)) : 0u;
-            uint32_t v[8];
-#pragma unroll
-            for (uint32_t j = 0; j < 8; j++) v[j] = j < wl ? word(j) : (j == wl ? tail : 0u);
-            if (lead) store16(chunk + 16, v[4], v[5], v[6], v[7]);              // upper half only: the lower one is the neighbour's
-            else if (end > 16) store32<2>(chunk, v[0], v[1], v[2], v[3], v[4], v[5], v[6], v[7]);
-            else store16(chunk, v[0], v[1], v[2], v[3]);                          // the upper half may be the next slot's
-        }
-    }
-    GOFR_HD void finish() {
-        flush();
-        if (4 * wl + nb > lead) {  // the last, partial sector; wl <= 7 after the flush
-            if (nb) stg_st(wp, pend >> (8 * (4 - nb)));
-            store_partial(chunk, base, lead, 4 * wl + nb);
-        }
-    }
-
-    // ---- lane-paired stores (the fast path of the wide slot-layout instance, emit_fast_paired) ----
-    // pm, the pair mask (see pair_round), names the lanes of the warp that make every call of these routines together.
-    // a flush decision of the lanes of the pair mask pm
-    GOFR_HD static bool any(bool p, uint32_t pm) {
-#if defined(__CUDA_ARCH__)
-        return __any_sync(pm, p);
-#else
-        (void)pm;
-        return warp_any(p);
-#endif
-    }
-
-    // store32 for a lane of the pair mask pm: the sector v0..v7 at the 32-byte aligned addr, if `have`; every lane of pm
-    // makes the call.  When lanes 2k and 2k+1 both have a sector,
-    // they write them together: in each of the two stores the even lane writes the lower and the odd lane the upper half
-    // of one sector (first the even lane's, then the odd lane's), so each warp store covers whole sectors.  A lane whose
-    // partner has no sector writes both halves of its own.
-    GOFR_HD static void store32_paired(uint32_t pm, bool have, uint8_t* addr, uint32_t v0, uint32_t v1, uint32_t v2, uint32_t v3,
-                                uint32_t v4, uint32_t v5, uint32_t v6, uint32_t v7) {
-#if defined(__CUDA_ARCH__)
-        uint8_t* a0 = addr;
-        uint8_t* a1 = addr + 16;
-        {
-            const uint32_t lane = threadIdx.x & 31u, odd = lane & 1u;
-            const uint32_t haves = __ballot_sync(pm, have);  // by every lane of pm: not behind a short-circuit on `have`
-            const bool pair = have && ((haves >> (lane ^ 1u)) & 1u);
-            // the half the partner writes: the even lane's upper half, the odd lane's lower half
-            const uint32_t x0 = __shfl_xor_sync(pm, odd ? v0 : v4, 1), x1 = __shfl_xor_sync(pm, odd ? v1 : v5, 1);
-            const uint32_t x2 = __shfl_xor_sync(pm, odd ? v2 : v6, 1), x3 = __shfl_xor_sync(pm, odd ? v3 : v7, 1);
-            uint8_t* const pa = (uint8_t*)__shfl_xor_sync(pm, (unsigned long long)addr, 1);
-            if (pair && odd) { a0 = pa + 16; v0 = x0; v1 = x1; v2 = x2; v3 = x3; }
-            if (pair && !odd) { a1 = pa; v4 = x0; v5 = x1; v6 = x2; v7 = x3; }
-        }
-        if (have) { store16(a0, v0, v1, v2, v3); store16(a1, v4, v5, v6, v7); }
-#else
-        (void)pm;
-        if (!have) return;
-        uint32_t v[8] = {v0, v1, v2, v3, v4, v5, v6, v7};
-        memcpy(addr, v, 32);
-#endif
-    }
-    // flush for a lane of the pair mask pm: every lane of pm calls it together
-    GOFR_HD void flush_paired(uint32_t pm) {
-        uint32_t n = wl >> 3;
-        saddr_t rp = base;
-        if (n && lead) {  // first sector of the response: skip the neighbour's bytes
-            store_partial(chunk, rp, lead, 32);
-            lead = 0;
-            chunk += 32;
-            rp += 8 * GOFR_RING_STRIDE_BYTES;
-            n--;
-        }
-#pragma unroll 1
-        while (pair_round(pm, n != 0)) {
-            const bool have = n != 0;
-            uint32_t v[8] = {0u, 0u, 0u, 0u, 0u, 0u, 0u, 0u};
-            if (have) {  // a lane without a sector may be at the end of its column: it reads nothing
-#pragma unroll
-                for (uint32_t j = 0; j < 8; j++) v[j] = stg_ld(rp + j * GOFR_RING_STRIDE_BYTES);
-            }
-            store32_paired(pm, have, chunk, v[0], v[1], v[2], v[3], v[4], v[5], v[6], v[7]);
-            if (have) {
-                chunk += 32;
-                rp += 8 * GOFR_RING_STRIDE_BYTES;
-                n--;
-            }
-        }
-        const uint32_t r = wl & 7;
-        if (wl >= 8 && r) {
-#pragma unroll
-            for (uint32_t j = 0; j < 7; j++)
-                if (r > j) stg_st(base + j * GOFR_RING_STRIDE_BYTES, stg_ld(rp + j * GOFR_RING_STRIDE_BYTES));
-        }
-        wl = r;
-        wp = base + r * GOFR_RING_STRIDE_BYTES;
-    }
-    // copy for a lane of the pair mask pm: every lane of pm calls it together, also with len 0, and takes the flush and
-    // long-copy rounds below
-    template <bool SH>
-    GOFR_HD void copy_paired(typename SrcMem<SH>::A src, uint32_t len, uint32_t pm) {
-        typedef SrcMem<SH> M;
+        if (!P::kLockstep && !len) return;
         const uint32_t yo = (M::low2(src) - nb) & 3u, sh = yo * 8;
         typename M::A Y = src - nb - yo;  // aligned word that holds stream byte 0
         const uint32_t total = nb + len;
@@ -542,36 +421,37 @@ struct Writer {
                 pend = w0 << (8 * (4 - nn));
                 nb = nn;
             }
+            if (!P::kLockstep) return;
         }
-        if (any(wl + 8 > GOFR_STAGE_WORDS, pm)) flush_paired(pm);  // at most 8 words staged from here on: this word + (head <= 7 | a short copy <= 7)
+        // at most 8 words staged from here on: this word + (head <= 7 | a short copy <= 7)
+        if (p.vote(wl + 8 > GOFR_STAGE_WORDS)) flush(p);
         if (words) {
             store_word(w0);
             cur = nxt;
             Y += 8;  // Y now points at the NEXT word to load
             nwords--;
         }
-        const bool lng = nwords >= 8;
-        if (lng) {
-            // Long copy.  Head: complete the sector under construction (<= 7 more words), store it; from then on the
-            // staging buffer is empty and whole sectors go from registers straight to HBM.
-            const uint32_t h = (8u - (wl & 7u)) & 7u;
-            if (h & 4u) stream_words<M, 4>(Y, cur, sh);
-            if (h & 2u) stream_words<M, 2>(Y, cur, sh);
-            if (h & 1u) stream_words<M, 1>(Y, cur, sh);
-            nwords -= h;
-        }
-        if (any(lng, pm)) {
-            flush_paired(pm);  // a long copy's wl is a multiple of 8: nothing is left behind
+        if (p.round(nwords >= 8)) {
+            if (nwords >= 8) {
+                // Long copy.  Head: complete the sector under construction (<= 7 more words), store it; from then on
+                // the staging buffer is empty and whole sectors go from registers straight to HBM.
+                const uint32_t h = (8u - (wl & 7u)) & 7u;
+                if (h & 4u) stream_words<M, 4>(Y, cur, sh);
+                if (h & 2u) stream_words<M, 2>(Y, cur, sh);
+                if (h & 1u) stream_words<M, 1>(Y, cur, sh);
+                nwords -= h;
+            }
+            flush(p);  // a long copy's wl is a multiple of 8: nothing is left behind
 #pragma unroll 1
-            while (pair_round(pm, nwords >= 8)) {
+            while (p.round(nwords >= 8)) {
                 const bool have = nwords >= 8;
                 uint32_t n0 = 0u, n1 = 0u, n2 = 0u, n3 = 0u, n4 = 0u, n5 = 0u, n6 = 0u, n7 = 0u;
                 if (have) {
                     n0 = M::ld(Y); n1 = M::ld(Y + 4); n2 = M::ld(Y + 8); n3 = M::ld(Y + 12);
                     n4 = M::ld(Y + 16); n5 = M::ld(Y + 20); n6 = M::ld(Y + 24); n7 = M::ld(Y + 28);
                 }
-                store32_paired(pm, have, chunk, fsr(cur, n0, sh), fsr(n0, n1, sh), fsr(n1, n2, sh), fsr(n2, n3, sh),
-                           fsr(n3, n4, sh), fsr(n4, n5, sh), fsr(n5, n6, sh), fsr(n6, n7, sh));
+                p.store32(have, chunk, fsr(cur, n0, sh), fsr(n0, n1, sh), fsr(n1, n2, sh), fsr(n2, n3, sh),
+                          fsr(n3, n4, sh), fsr(n4, n5, sh), fsr(n5, n6, sh), fsr(n6, n7, sh));
                 if (have) {
                     chunk += 32;
                     cur = n7;
@@ -593,9 +473,12 @@ struct Writer {
         }
         nb = nn;
     }
-    // finish_padded for a lane of the pair mask pm: every lane of pm makes the call, the last whole sectors are paired
-    GOFR_HD void finish_padded_paired(uint32_t pm) {
-        flush_paired(pm);
+    // Slot layout (gofr_serve_device_slots): the response owns its 16-byte aligned slot, so the last 16-byte chunk is
+    // stored whole, zero padded — no byte stores, nothing of a neighbour to preserve.  A slot starts either on a sector
+    // boundary or in the middle of one (lead 0 or 16).
+    template <typename P = SoloStores>
+    GOFR_HD void finish_padded(P p = P()) {
+        flush(p);
         const uint32_t end = 4 * wl + nb;  // bytes of the last sector in use, phantom lead included
         const bool some = end > lead;
         uint32_t v[8] = {0u, 0u, 0u, 0u, 0u, 0u, 0u, 0u};
@@ -603,11 +486,21 @@ struct Writer {
             const uint32_t tail = nb ? pend >> (8 * (4 - nb)) : 0u;
 #pragma unroll
             for (uint32_t j = 0; j < 8; j++) v[j] = j < wl ? word(j) : (j == wl ? tail : 0u);
+            if (lead) store16(chunk + 16, v[4], v[5], v[6], v[7]);  // upper half only: the lower one is the neighbour's
+            else if (end > 16) { if (!P::kLockstep) p.store32(true, chunk, v[0], v[1], v[2], v[3], v[4], v[5], v[6], v[7]); }
+            else store16(chunk, v[0], v[1], v[2], v[3]);  // the upper half may be the next slot's
         }
-        const bool whole = some && !lead && end > 16;
-        store32_paired(pm, whole, chunk, v[0], v[1], v[2], v[3], v[4], v[5], v[6], v[7]);
-        if (some && lead) store16(chunk + 16, v[4], v[5], v[6], v[7]);  // upper half only: the lower one is the neighbour's
-        else if (some && !whole) store16(chunk, v[0], v[1], v[2], v[3]);  // the upper half may be the next slot's
+        // The whole last sector (the `end > 16` case above).  A lane on its own stores it in that branch; a lockstep
+        // group makes the call with every lane, outside the per-lane branches.  (One `whole` flag and one call after
+        // the branches would read better, but it changes the solo code: Bind's kernel grows by 8 to 16 instructions.)
+        if (P::kLockstep) p.store32(some && !lead && end > 16, chunk, v[0], v[1], v[2], v[3], v[4], v[5], v[6], v[7]);
+    }
+    GOFR_HD void finish() {
+        flush();
+        if (4 * wl + nb > lead) {  // the last, partial sector; wl <= 7 after the flush
+            if (nb) stg_st(wp, pend >> (8 * (4 - nb)));
+            store_partial(chunk, base, lead, 4 * wl + nb);
+        }
     }
 };
 
@@ -1570,6 +1463,19 @@ struct RowReader {
     GOFR_HD uint32_t operator[](uint32_t k) const { return gl ? gl[k] : stg_ld(sh + 4 * k); }
 };
 
+// OP_KEY `raw` (op flags `oflags`): true if it has omitempty and its field holds the zero value, so that the key and the
+// ops it governs are left out.  bind: the row is a Bind span row.
+GOFR_HD bool key_omitted(const uint4& raw, uint32_t oflags, const RowReader& row, bool bind) {
+    bool empty = false;
+    if (oflags & OPF_OMITEMPTY) {
+        const uint32_t okind = raw.x >> 24, wv = row[raw.w];
+        if (okind == GOFR_F_INT64 || okind == GOFR_F_INT) empty = (wv | row[raw.w + 1]) == 0;
+        else if (okind == GOFR_F_STRING && bind) empty = (row[raw.w + 1] & 0x7FFFFFFFu) == 0;
+        else empty = wv == 0;
+    }
+    return empty;
+}
+
 // Lean size pass of a PF_FAST program (every dynamic op is a plain value of the body).  Returns false when the request
 // needs something emit_fast does not do — a string encoding/json would escape, a query value that needs decoding, a
 // malformed row, a tile that is not staged, HEAD — and the caller runs the general size pass instead.
@@ -1592,13 +1498,7 @@ GOFR_HD bool size_fast(const TableView& tv, const BatchRefs& br, ReqCtx& c) {
         const uint4 raw = *(const uint4*)(ops + oi);
         const uint32_t code = raw.x & 0xFFu, oflags = (raw.x >> 16) & 0xFFu, ooff = raw.z;
         if (code == OP_KEY) {
-            bool empty = false;
-            if (oflags & OPF_OMITEMPTY) {
-                const uint32_t okind = raw.x >> 24, wv = row[raw.w];
-                if (okind == GOFR_F_INT64 || okind == GOFR_F_INT) empty = (wv | row[raw.w + 1]) == 0;
-                else if (okind == GOFR_F_STRING && (P.flags & PF_BIND)) empty = (row[raw.w + 1] & 0x7FFFFFFFu) == 0;
-                else empty = wv == 0;
-            }
+            const bool empty = key_omitted(raw, oflags, row, P.flags & PF_BIND);
             skip = empty;
             if (!empty) { dyn += (first ? 0u : 1u) + raw.y; first = false; }
             continue;
@@ -1642,145 +1542,6 @@ GOFR_HD bool size_fast(const TableView& tv, const BatchRefs& br, ReqCtx& c) {
     return true;
 }
 
-// Template windows [k0, k1) of a response into its slot: whole 32-byte sectors wherever the destination allows (a slot
-// starts on a sector boundary or in the middle of one), single 16-byte windows at the ends.
-GOFR_HD void copy_template_windows(uint8_t* dst, saddr_t tp, uint32_t k0, uint32_t k1) {
-    uint32_t k = k0;
-    if (k < k1 && (((uintptr_t)dst + 16 * k) & 16u)) {
-        const uint4 v = src_ld128(tp + 16 * k);
-        Writer::store16(dst + 16 * k, v.x, v.y, v.z, v.w);
-        k++;
-    }
-#pragma unroll 1
-    for (; k + 2 <= k1; k += 2) {
-        const uint4 a = src_ld128(tp + 16 * k), b = src_ld128(tp + 16 * k + 16);
-        Writer::store32<3>(dst + 16 * k, a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w);
-    }
-    if (k < k1) {
-        const uint4 v = src_ld128(tp + 16 * k);
-        Writer::store16(dst + 16 * k, v.x, v.y, v.z, v.w);
-    }
-}
-
-// Writes a response sized by size_fast into its 16-byte aligned slot: the template with aligned 16-byte loads and
-// stores, the trace id patched into the windows it touches, then the tail ops through the Writer.
-GOFR_HD void emit_fast(const TableView& tv, const BatchRefs& br, ReqCtx& c, uint8_t* dst, uint32_t* ring_col) {
-    const FastRec F = *(tv.fast() + c.prog);
-    const uint32_t nwin = F.tmpl_windows;
-    // the trace id is needed after the template copy: ask for it now
-    uint4 id = {0u, 0u, 0u, 0u};
-    if (F.hex_pos != 0xFFFFu) id = *(const uint4*)(br.ids + (size_t)c.index * 16);
-    if (nwin) {
-        const saddr_t tp = to_saddr(tv.lits() + F.tmpl_off);
-        uint32_t h0 = nwin, h1 = nwin;  // [h0, h1): windows the 32 hex characters touch
-        if (F.hex_pos != 0xFFFFu) { h0 = (uint32_t)F.hex_pos >> 4; h1 = (((uint32_t)F.hex_pos + 31u) >> 4) + 1u; }
-        copy_template_windows(dst, tp, 0, h0);
-        copy_template_windows(dst, tp, h1, nwin);
-        if (h0 < nwin) {
-            // the 2 or 3 windows around the trace id: template words into the (idle) staging column, the 8 hex words
-            // shifted to their byte offset on top, then whole windows out
-            const saddr_t col = to_saddr(ring_col);
-            const uint32_t nw = (h1 - h0) * 4;  // 8 or 12 words
-#pragma unroll 1
-            for (uint32_t k = 0; k < nw; k++) stg_st(col + k * GOFR_RING_STRIDE_BYTES, src_ld(tp + 16 * h0 + 4 * k));
-            uint32_t H[8];
-            hex8(id.x, H[0], H[1]); hex8(id.y, H[2], H[3]); hex8(id.z, H[4], H[5]); hex8(id.w, H[6], H[7]);
-            const uint32_t o = (uint32_t)F.hex_pos & 15u, q = o >> 2, sh = (o & 3u) * 8;
-            const saddr_t hp = col + q * GOFR_RING_STRIDE_BYTES;
-            if (sh == 0) {
-#pragma unroll
-                for (uint32_t j = 0; j < 8; j++) stg_st(hp + j * GOFR_RING_STRIDE_BYTES, H[j]);
-            } else {
-                const uint32_t lowmask = (1u << sh) - 1u;
-                stg_st(hp, (stg_ld(hp) & lowmask) | (H[0] << sh));
-#pragma unroll
-                for (uint32_t j = 1; j < 8; j++) stg_st(hp + j * GOFR_RING_STRIDE_BYTES, fsr(H[j - 1], H[j], 32 - sh));
-                stg_st(hp + 8 * GOFR_RING_STRIDE_BYTES, (H[7] >> (32 - sh)) | (stg_ld(hp + 8 * GOFR_RING_STRIDE_BYTES) & ~lowmask));
-            }
-#pragma unroll 1
-            for (uint32_t k = h0; k < h1; k++) {
-                const saddr_t rp = col + (k - h0) * 4 * GOFR_RING_STRIDE_BYTES;
-                Writer::store16(dst + 16 * k, stg_ld(rp), stg_ld(rp + GOFR_RING_STRIDE_BYTES), stg_ld(rp + 2 * GOFR_RING_STRIDE_BYTES),
-                                stg_ld(rp + 3 * GOFR_RING_STRIDE_BYTES));
-            }
-        }
-    }
-    if (F.flags & FR_COMPLETE) return;
-
-    Writer w;
-    w.init(dst + 16 * nwin, ring_col);
-    const Op* ops = tv.ops() + F.tail_op;
-    const uint8_t* const lits = tv.lits();
-    RowReader row;
-    row.sh = to_saddr(c.data());
-    row.gl = (F.flags & FR_BIND) ? c.brow(br) : nullptr;
-    uint32_t str_cursor = 0;
-    bool first = true, skip = false;
-#pragma unroll 1
-    for (uint32_t oi = 0; oi < F.n_tail_ops; oi++) {
-        const uint4 raw = *(const uint4*)(ops + oi);
-        const uint32_t code = raw.x & 0xFFu, oflags = (raw.x >> 16) & 0xFFu, ooff = raw.z;
-        if (code == OP_KEY) {
-            bool empty = false;
-            if (oflags & OPF_OMITEMPTY) {
-                const uint32_t okind = raw.x >> 24, wv = row[raw.w];
-                if (okind == GOFR_F_INT64 || okind == GOFR_F_INT) empty = (wv | row[raw.w + 1]) == 0;
-                else if (okind == GOFR_F_STRING && (F.flags & FR_BIND)) empty = (row[raw.w + 1] & 0x7FFFFFFFu) == 0;
-                else empty = wv == 0;
-            }
-            skip = empty;
-            if (empty) continue;
-            if (!first) {
-                if (warp_any(w.wl >= GOFR_STAGE_WORDS - 8)) w.flush();
-                w.putc(',');
-            }
-            first = false;
-        } else if ((oflags & OPF_VALUE_OF_KEY) && skip) {
-            if (code == OP_STR) str_cursor += row[ooff];
-            continue;
-        }
-        const bool lit_only = code == OP_LIT || code == OP_KEY;
-        // step 0: the op's literal bytes (OP_LIT / OP_KEY: the literal itself, else the folded prefix); step 1: its value
-        const uint8_t* csrc = lits + (lit_only ? raw.z : raw.w);
-        uint32_t clen = raw.y;
-#pragma unroll 1
-        for (uint32_t step = 0; step < 2; step++) {
-            if (step == 1) {
-                if (lit_only) break;
-                clen = 0;
-                if (warp_any(w.wl >= GOFR_STAGE_WORDS - 8)) w.flush();  // a generated value appends at most 8 words
-                if (code == OP_STR) {
-                    clen = row[ooff];
-                    csrc = c.data() + c.str_base + str_cursor;
-                    str_cursor += clen;
-                } else if (code == OP_I64) {
-                    emit_i64<true>(&w, (int64_t)((uint64_t)row[ooff] | (uint64_t)row[ooff + 1] << 32));
-                } else if (code == OP_I32) {
-                    emit_i64<true>(&w, (int64_t)(int32_t)row[ooff]);
-                } else if (code == OP_BOOL) {
-                    if (row[ooff]) w.put4('t' | 'r' << 8 | 'u' << 16 | 'e' << 24);
-                    else { w.put4('f' | 'a' << 8 | 'l' << 16 | 's' << 24); w.putc('e'); }
-                } else if (code == OP_CLEN) {
-                    emit_u32<true>(&w, c.body_len);
-                } else if (code == OP_HEXID) {
-                    const uint4 id = *(const uint4*)(br.ids + (size_t)c.index * 16);
-                    const uint32_t idw[4] = {id.x, id.y, id.z, id.w};
-#pragma unroll
-                    for (int k = 0; k < 4; k++) { uint32_t a, b; hex8(idw[k], a, b); w.put4(a); w.put4(b); }
-                } else if (code == OP_PARAM) {
-                    if (c.pv_flags & 1) { csrc = ((c.pv_flags & 4) ? c.path : c.query()) + c.pv_off; clen = c.pv_len; }
-                    else { csrc = lits + c.def_off; clen = c.def_len; }
-                } else {  // OP_BSTR
-                    csrc = c.data() + row[ooff];
-                    clen = row[ooff + 1];
-                }
-            }
-            if (clen) w.copy<true>(SrcMem<true>::from(csrc), clen);
-        }
-    }
-    w.finish_padded();
-}
-
 // Window i (16 bytes) of a source: TMPL, a template in the literal pool (16-byte aligned); else a staging column.
 template <bool TMPL>
 GOFR_HD uint4 window_ld(saddr_t src, uint32_t i) {
@@ -1792,48 +1553,50 @@ GOFR_HD uint4 window_ld(saddr_t src, uint32_t i) {
 }
 
 // Windows [k0, k1) of a response into its slot, window k0 + i from window i of src: whole 32-byte sectors wherever the
-// destination allows (a slot starts on a sector boundary or in the middle of one), paired over pm, single 16-byte windows
-// at the ends.  Every lane of pm makes the call (k0 == k1: nothing to store).
-template <bool TMPL>
-GOFR_HD void copy_windows(uint32_t pm, uint8_t* dst, saddr_t src, uint32_t k0, uint32_t k1) {
+// destination allows (a slot starts on a sector boundary or in the middle of one), single 16-byte windows at the ends.
+// With PairStores every lane of the pair mask makes the call (k0 == k1: nothing to store).
+template <bool TMPL, typename P>
+GOFR_HD void copy_windows(uint8_t* dst, saddr_t src, uint32_t k0, uint32_t k1, P p) {
     const uint32_t n = k1 - k0;
     uint8_t* const d = dst + 16 * k0;
     uint32_t i = 0;
     if (n && ((uintptr_t)d & 16u)) {
         const uint4 v = window_ld<TMPL>(src, 0);
-        Writer::store16(d, v.x, v.y, v.z, v.w);
+        store16(d, v.x, v.y, v.z, v.w);
         i = 1;
     }
 #pragma unroll 1
-    while (pair_round(pm, i + 2 <= n)) {
+    while (p.round(i + 2 <= n)) {
         const bool have = i + 2 <= n;
         uint4 a = {0u, 0u, 0u, 0u}, b = {0u, 0u, 0u, 0u};
         if (have) { a = window_ld<TMPL>(src, i); b = window_ld<TMPL>(src, i + 1); }
-        Writer::store32_paired(pm, have, d + 16 * i, a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w);
+        p.store32(have, d + 16 * i, a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w);
         if (have) i += 2;
     }
     if (i < n) {
         const uint4 v = window_ld<TMPL>(src, i);
-        Writer::store16(d + 16 * i, v.x, v.y, v.z, v.w);
+        store16(d + 16 * i, v.x, v.y, v.z, v.w);
     }
 }
 
-// emit_fast with its sectors stored in lane pairs (Writer::store32_paired).  pm: the lanes of the warp that call it together,
-// never 0.  Every lane of pm runs every store round below, also when its program has no template or no tail: a lane
-// past its last op, or on an op that writes nothing, copies 0 bytes.  Only the appending of words differs between lanes.
-GOFR_HD void emit_fast_paired(const TableView& tv, const BatchRefs& br, ReqCtx& c, uint8_t* dst, uint32_t* ring_col, uint32_t pm) {
+// Writes a response sized by size_fast into its 16-byte aligned slot: the template with aligned 16-byte loads and
+// stores, the trace id patched into the windows it touches, then the tail ops through the Writer.  With PairStores every
+// lane of the pair mask runs every store round below, also when its program has no template or no tail: a lane past its
+// last op, or on an op that writes nothing, copies 0 bytes.  Only the appending of words differs between lanes.
+template <typename P>
+GOFR_HD void emit_fast(const TableView& tv, const BatchRefs& br, ReqCtx& c, uint8_t* dst, uint32_t* ring_col, P p) {
     const FastRec F = *(tv.fast() + c.prog);
     const uint32_t nwin = F.tmpl_windows;
     // the trace id is needed after the template copy: ask for it now
     uint4 id = {0u, 0u, 0u, 0u};
     if (F.hex_pos != 0xFFFFu) id = *(const uint4*)(br.ids + (size_t)c.index * 16);
-    {
+    if (P::kLockstep || nwin) {
         const saddr_t tp = to_saddr(tv.lits() + F.tmpl_off);
         const saddr_t col = to_saddr(ring_col);
         uint32_t h0 = nwin, h1 = nwin;  // [h0, h1): windows the 32 hex characters touch
         if (nwin && F.hex_pos != 0xFFFFu) { h0 = (uint32_t)F.hex_pos >> 4; h1 = (((uint32_t)F.hex_pos + 31u) >> 4) + 1u; }
-        copy_windows<true>(pm, dst, tp, 0, h0);
-        copy_windows<true>(pm, dst, tp + 16 * h1, h1, nwin);
+        copy_windows<true>(dst, tp, 0, h0, p);
+        copy_windows<true>(dst, tp + 16 * h1, h1, nwin, p);
         if (h0 < nwin) {
             // the 2 or 3 windows around the trace id: template words into the (idle) staging column, the 8 hex words
             // shifted to their byte offset on top, then whole windows out
@@ -1855,9 +1618,22 @@ GOFR_HD void emit_fast_paired(const TableView& tv, const BatchRefs& br, ReqCtx& 
                 stg_st(hp + 8 * GOFR_RING_STRIDE_BYTES, (H[7] >> (32 - sh)) | (stg_ld(hp + 8 * GOFR_RING_STRIDE_BYTES) & ~lowmask));
             }
         }
-        copy_windows<false>(pm, dst, col, h0, h0 < nwin ? h1 : h0);
+        // a lane on its own stores the 2 or 3 trace-id windows one at a time: through copy_windows the 5-CTA slot
+        // instance took 4 % longer on config 4, well outside the run-to-run spread (DESIGN §6 has the A/B)
+        if (P::kLockstep) {
+            copy_windows<false>(dst, col, h0, h0 < nwin ? h1 : h0, p);
+        } else if (h0 < nwin) {
+#pragma unroll 1
+            for (uint32_t k = h0; k < h1; k++) {
+                const saddr_t rp = col + (k - h0) * 4 * GOFR_RING_STRIDE_BYTES;
+                store16(dst + 16 * k, stg_ld(rp), stg_ld(rp + GOFR_RING_STRIDE_BYTES), stg_ld(rp + 2 * GOFR_RING_STRIDE_BYTES),
+                        stg_ld(rp + 3 * GOFR_RING_STRIDE_BYTES));
+            }
+        }
     }
-    // a template-only program runs the tail with no ops: its Writer stores nothing, but takes part in the store rounds
+    // a template-only program: with PairStores its Writer runs the tail with no ops, storing nothing but taking part in
+    // the store rounds
+    if (!P::kLockstep && (F.flags & FR_COMPLETE)) return;
     const uint32_t n_ops = (F.flags & FR_COMPLETE) ? 0u : F.n_tail_ops;
 
     Writer w;
@@ -1870,22 +1646,15 @@ GOFR_HD void emit_fast_paired(const TableView& tv, const BatchRefs& br, ReqCtx& 
     uint32_t str_cursor = 0;
     bool first = true, skip = false;
 #pragma unroll 1
-    for (uint32_t oi = 0; pair_round(pm, oi < n_ops); oi++) {
-        bool live = oi < n_ops;
+    for (uint32_t oi = 0; p.round(oi < n_ops); oi++) {
+        bool live = oi < n_ops;  // false: this op writes nothing (a lane past its last op, an omitted key or value)
         uint4 raw = {0u, 0u, 0u, 0u};
         if (live) raw = *(const uint4*)(ops + oi);
         const uint32_t code = raw.x & 0xFFu, oflags = (raw.x >> 16) & 0xFFu, ooff = raw.z;
         bool comma = false;
         if (live && code == OP_KEY) {
-            bool empty = false;
-            if (oflags & OPF_OMITEMPTY) {
-                const uint32_t okind = raw.x >> 24, wv = row[raw.w];
-                if (okind == GOFR_F_INT64 || okind == GOFR_F_INT) empty = (wv | row[raw.w + 1]) == 0;
-                else if (okind == GOFR_F_STRING && (F.flags & FR_BIND)) empty = (row[raw.w + 1] & 0x7FFFFFFFu) == 0;
-                else empty = wv == 0;
-            }
-            skip = empty;
-            if (empty) live = false;
+            skip = key_omitted(raw, oflags, row, F.flags & FR_BIND);
+            if (skip) live = false;
             else {
                 comma = !first;
                 first = false;
@@ -1894,7 +1663,8 @@ GOFR_HD void emit_fast_paired(const TableView& tv, const BatchRefs& br, ReqCtx& 
             if (code == OP_STR) str_cursor += row[ooff];
             live = false;
         }
-        if (Writer::any(w.wl >= GOFR_STAGE_WORDS - 8, pm)) w.flush_paired(pm);  // room for the comma
+        if (!P::kLockstep && !live) continue;
+        if ((P::kLockstep || comma) && p.vote(w.wl >= GOFR_STAGE_WORDS - 8)) w.flush(p);  // room for the comma
         if (comma) w.putc(',');
         const bool lit_only = code == OP_LIT || code == OP_KEY;
         // step 0: the op's literal bytes (OP_LIT / OP_KEY: the literal itself, else the folded prefix); step 1: its value
@@ -1903,8 +1673,9 @@ GOFR_HD void emit_fast_paired(const TableView& tv, const BatchRefs& br, ReqCtx& 
 #pragma unroll 1
         for (uint32_t step = 0; step < 2; step++) {
             if (step == 1) {
+                if (!P::kLockstep && lit_only) break;
                 clen = 0;
-                if (Writer::any(w.wl >= GOFR_STAGE_WORDS - 8, pm)) w.flush_paired(pm);  // a generated value appends at most 8 words
+                if (p.vote(w.wl >= GOFR_STAGE_WORDS - 8)) w.flush(p);  // a generated value appends at most 8 words
                 if (!live || lit_only) {
                     // no value: the copy below stores nothing
                 } else if (code == OP_STR) {
@@ -1933,10 +1704,10 @@ GOFR_HD void emit_fast_paired(const TableView& tv, const BatchRefs& br, ReqCtx& 
                     clen = row[ooff + 1];
                 }
             }
-            w.copy_paired<true>(SrcMem<true>::from(csrc), clen, pm);
+            if (P::kLockstep || clen) w.copy<true>(SrcMem<true>::from(csrc), clen, p);
         }
     }
-    w.finish_padded_paired(pm);
+    w.finish_padded(p);
 }
 
 // Full size stage for one request: route, size; a malformed handler-result row is answered like a handler panic.
@@ -2045,7 +1816,7 @@ template <bool SLOTS = false, bool VO = (GOFR_TU_VALUES != 0)>
 GOFR_HD void emit_request(const TableView& tv, const BatchRefs& br, ReqCtx& c, uint8_t* dst, uint32_t* ring_col) {
     if (c.total_len == 0) return;
     if (SLOTS) {
-        if (c.fast()) emit_fast(tv, br, c, dst, ring_col);
+        if (c.fast()) emit_fast(tv, br, c, dst, ring_col, SoloStores{});
         else { ReqCtx t = c; emit_request_slots_call<VO>(tv, br, &t, dst, ring_col); }  // a copy: see size_routed
         return;
     }

@@ -109,6 +109,12 @@ def set_stage_mode(mode: int):
     lib().emu_set_stage_mode(mode)
 
 
+def set_pair_stores(on: bool):
+    """Slot emulation: write fast-path responses with the PairStores store policy of the wide instance (True) or with
+    SoloStores (False, the default)."""
+    lib().emu_set_pair_stores(1 if on else 0)
+
+
 def set_flush_mode(mode: int):
     """0: flush decisions per request; 1: flush at every decision point; 2: pseudo-random extra flushes (on the GPU the
     other lanes of a warp impose theirs)."""

@@ -191,6 +191,11 @@ extern "C" void emu_float_text_many(const uint64_t* bits, uint32_t n, uint8_t* o
 extern "C" void emu_set_stage_mode(int m) { g_stage_mode = m; }
 static uint64_t g_fast_taken = 0;  // requests sized by size_fast (and therefore written by emit_fast) since the last reset
 extern "C" uint64_t emu_fast_taken(int reset) { const uint64_t v = g_fast_taken; if (reset) g_fast_taken = 0; return v; }
+// store policy of the fast path: 0 SoloStores (serve_slots_kernel), 1 PairStores (the wide instance): its lockstep code
+// paths — zero-length copies through the flush votes, trace-id windows through copy_windows, an empty tail for a
+// template-only program, the last sector stored after the per-lane branches — run here one lane at a time
+static int g_pair_stores = 0;
+extern "C" void emu_set_pair_stores(int on) { g_pair_stores = on; }
 extern "C" int emu_serve_slots(const uint8_t* image, uint64_t image_len, const uint8_t* desc, const uint8_t* ids,
                                const uint8_t* arena, uint32_t n, const char* date29, uint8_t* out, uint32_t slot_bytes,
                                uint32_t* out_len, uint32_t* meta) {
@@ -218,7 +223,11 @@ extern "C" int emu_serve_slots(const uint8_t* image, uint64_t image_len, const u
         out_len[i] = c.total_len;
         meta[i] = request_status(tv, c) | (c.route << 16);
         if (c.fast()) g_fast_taken++;
-        if (c.total_len && c.total_len <= slot_bytes) emit_request<true>(tv, br, c, out + (size_t)i * slot_bytes, ring);
+        if (c.total_len && c.total_len <= slot_bytes) {
+            uint8_t* const dst = out + (size_t)i * slot_bytes;
+            if (g_pair_stores && c.fast()) emit_fast(tv, br, c, dst, ring, PairStores{~0u});
+            else emit_request<true>(tv, br, c, dst, ring);
+        }
     }
     return 0;
 }

@@ -1,6 +1,6 @@
 """The slot-layout fast path of the wide instance (4 CTAs/SM, the one config 2 runs) stores each whole 32-byte sector of a
 response with two 16-byte warp stores shared by a lane pair: lanes 2k and 2k+1 each write one half of the even lane's
-sector, then one half of the odd lane's (Writer::store32_paired in serve_device.cuh).  A lane whose partner has no sector
+sector, then one half of the odd lane's (the PairStores store policy in serve_device.cuh).  A lane whose partner has no sector
 in a round, every store outside the fast path and the 5-CTA instance write their own.  Mixed traffic (config 4) runs here
 on both instances: forced onto the wide one, its warps pair lanes of different programs, template-only programs next to
 tail ops, and lanes whose requests were deferred to the general pass.

@@ -51,21 +51,29 @@ def _check_slots(out, ln, meta, spec, batch, slot, untouched=True):
 
 @pytest.mark.parametrize("which,slot", [("config1", 320), ("config2", 528), ("config2", 544), ("config4", 352), ("config3", 1024)])
 def test_emu_slots_match_oracle(which, slot):
-    """the slot-layout emit path (emit_request<true>, Writer::finish_padded) on the CPU"""
+    """the slot-layout emit path (emit_request<true>, Writer::finish_padded) on the CPU, with the fast path's sectors
+    stored under both store policies (SoloStores as in serve_slots_kernel, PairStores as in the wide instance)"""
     from tests.emu import emu
     spec, batch = {"config1": (synth.config1_spec(), synth.config1_batch(200)),
                    "config2": (synth.config2_spec(), synth.config2_batch(300, escape_every=5)),
                    "config3": (synth.config3_spec(), synth.config3_batch(300)),
                    "config4": (synth.config4_spec(), synth.config4_batch(1500))}[which]
-    out, ln, meta = emu.serve_slots(Table(spec).serialize(), batch, DATE, slot)
-    _check_slots(out, ln, meta, spec, batch, slot)
+    image = Table(spec).serialize()
+    try:
+        for pair in (False, True):
+            emu.set_pair_stores(pair)
+            out, ln, meta = emu.serve_slots(image, batch, DATE, slot)
+            _check_slots(out, ln, meta, spec, batch, slot)
+    finally:
+        emu.set_pair_stores(False)
 
 
 @pytest.mark.parametrize("mode", [S.FRAME_WIRE, S.FRAME_INTENDED, S.FRAME_BODY])
 @pytest.mark.parametrize("flush_mode", [0, 1, 2])
 def test_emu_fast_path(mode, flush_mode):
     """emit_fast (seal-time response templates + tail ops) against the oracle: every framing mode, the flush decisions
-    other lanes impose on the GPU replayed (emu.set_flush_mode), and a check that the fast path really ran"""
+    other lanes impose on the GPU replayed (emu.set_flush_mode), both store policies (SoloStores; PairStores, whose
+    lockstep paths the wide instance runs), and a check that the fast path really ran"""
     from tests.emu import emu
     emu.set_flush_mode(flush_mode)
     emu.set_stage_mode(1)
@@ -76,14 +84,18 @@ def test_emu_fast_path(mode, flush_mode):
                 (synth.config2_spec(mode), synth.config2_batch(600, escape_every=4), 640, 0.7),
                 (synth.config4_spec(mode), synth.config4_batch(2500), 704, 0.5),
                 (synth.config3_spec(mode), synth.config3_batch(400), 1024, 0.5)):
-            emu.fast_taken()
-            out, ln, meta = emu.serve_slots(Table(spec).serialize(), batch, DATE, slot)
-            taken = emu.fast_taken()
-            _check_slots(out, ln, meta, spec, batch, slot)
-            assert taken >= min_fast * batch.n, (taken, batch.n)
+            image = Table(spec).serialize()
+            for pair in (False, True):
+                emu.set_pair_stores(pair)
+                emu.fast_taken()
+                out, ln, meta = emu.serve_slots(image, batch, DATE, slot)
+                taken = emu.fast_taken()
+                _check_slots(out, ln, meta, spec, batch, slot)
+                assert taken >= min_fast * batch.n, (taken, batch.n, pair)
     finally:
         emu.set_flush_mode(0)
         emu.set_stage_mode(0)
+        emu.set_pair_stores(False)
 
 
 @pytest.fixture(scope="module")
