@@ -169,15 +169,11 @@ class Engine:
         out = torch.empty(cap, dtype=torch.uint8, device=dev)
         off = torch.zeros(n + 1, dtype=torch.int32, device=dev)
         meta = torch.zeros(max(n, 1), dtype=torch.int32, device=dev)
-        pr = S.proto_nested_presence(msgs)
-        if pr is None:
-            _abi.check(_abi.lib().gofr_proto_encode_nested_device(self._e, nm.ctypes.data, len(msgs), nf.ctypes.data, k, root, d_rows.data_ptr(),
-                                                                  d_off.data_ptr(), n, out.data_ptr(), cap, off.data_ptr(), meta.data_ptr(),
-                                                                  st.cuda_stream), "gofr_proto_encode_nested_device")
-        else:   # a field with explicit presence (ProtoNField.presence)
-            _abi.check(_abi.lib().gofr_proto_encode_nested_ex_device(self._e, nm.ctypes.data, len(msgs), nf.ctypes.data, k, root, pr.ctypes.data,
-                                                                     d_rows.data_ptr(), d_off.data_ptr(), n, out.data_ptr(), cap, off.data_ptr(),
-                                                                     meta.data_ptr(), st.cuda_stream), "gofr_proto_encode_nested_ex_device")
+        pr = S.proto_nested_presence(msgs)   # None: no field has explicit presence, and the _ex call is the plain one
+        _abi.check(_abi.lib().gofr_proto_encode_nested_ex_device(self._e, nm.ctypes.data, len(msgs), nf.ctypes.data, k, root,
+                                                                 None if pr is None else pr.ctypes.data, d_rows.data_ptr(), d_off.data_ptr(), n,
+                                                                 out.data_ptr(), cap, off.data_ptr(), meta.data_ptr(), st.cuda_stream),
+                   "gofr_proto_encode_nested_ex_device")
         return out, off, meta[:n]
 
     def proto_decode_nested_device(self, msgs, root: int, frames: np.ndarray, in_off: np.ndarray, rows_cap: Optional[int] = None, stream=None):
@@ -194,15 +190,11 @@ class Engine:
         rows = torch.empty(cap, dtype=torch.uint8, device=dev)
         off = torch.zeros(n + 1, dtype=torch.int32, device=dev)
         meta = torch.zeros(max(n, 1), dtype=torch.int32, device=dev)
-        pr = S.proto_nested_presence(msgs)
-        if pr is None:
-            _abi.check(_abi.lib().gofr_proto_decode_nested_device(self._e, nm.ctypes.data, len(msgs), nf.ctypes.data, k, root, d_in.data_ptr(),
-                                                                  d_off.data_ptr(), n, rows.data_ptr(), cap, off.data_ptr(), meta.data_ptr(),
-                                                                  st.cuda_stream), "gofr_proto_decode_nested_device")
-        else:   # a field with explicit presence (ProtoNField.presence)
-            _abi.check(_abi.lib().gofr_proto_decode_nested_ex_device(self._e, nm.ctypes.data, len(msgs), nf.ctypes.data, k, root, pr.ctypes.data,
-                                                                     d_in.data_ptr(), d_off.data_ptr(), n, rows.data_ptr(), cap, off.data_ptr(),
-                                                                     meta.data_ptr(), st.cuda_stream), "gofr_proto_decode_nested_ex_device")
+        pr = S.proto_nested_presence(msgs)   # None: no field has explicit presence, and the _ex call is the plain one
+        _abi.check(_abi.lib().gofr_proto_decode_nested_ex_device(self._e, nm.ctypes.data, len(msgs), nf.ctypes.data, k, root,
+                                                                 None if pr is None else pr.ctypes.data, d_in.data_ptr(), d_off.data_ptr(), n,
+                                                                 rows.data_ptr(), cap, off.data_ptr(), meta.data_ptr(), st.cuda_stream),
+                   "gofr_proto_decode_nested_ex_device")
         return rows, off, meta[:n]
 
     def proto_decode_device(self, fields, frames: np.ndarray, in_off: np.ndarray, rows_cap: Optional[int] = None, stream=None):

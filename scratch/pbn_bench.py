@@ -2,7 +2,7 @@
 """pbn_bench.py — kernel time of the nested proto3 codec (gofr_proto_encode_nested_device / gofr_proto_decode_nested_device):
    [GOFR_LIB_PATH=scratch/variants/libgofr_X.so] python scratch/pbn_bench.py [--n 1048576] [--steps 20] [--only a,b,c]
 Workloads (1 Mi messages each; 1024 distinct rows repeated):
-   a  the PAGE / ITEM type of tests/test_proto_nested.py (no maps)
+   a  the PAGE / ITEM type of tests/proto_nested_harness.py (no maps)
    b  M { map<string, string> labels = 1; map<int64, Item> items = 2; } with 8 labels and 8 items
    c  the same type with 64 labels and 64 items (short strings, no tags): the decoder's worst case (selection over 64
       entries per map)
@@ -29,7 +29,7 @@ from gofr_b200 import _abi, synth  # noqa: E402
 from gofr_b200 import spec as S  # noqa: E402
 from gofr_b200.engine import Engine  # noqa: E402
 from gofr_b200.table import Table  # noqa: E402
-from tests.test_proto_nested import MSGS, _rand_value  # noqa: E402
+from tests.proto_nested_harness import MSGS, rand_value  # noqa: E402
 
 F = S.ProtoNField
 ITEM = [F(1, S.PB_INT64), F(2, S.PB_STRING), F(3, S.PB_STRING, True), F(4, S.PB_DOUBLE)]
@@ -103,7 +103,7 @@ def main():
     smi = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"], capture_output=True, text=True)
     print(json.dumps({"gpu": smi.stdout.strip().splitlines()[0] if smi.returncode == 0 else "nvidia-smi failed", "lib": a.tag}), flush=True)
     rnd = random.Random(5)
-    work = {"a": (MSGS, lambda: [_rand_value(rnd, MSGS, 0) for _ in range(1024)]),
+    work = {"a": (MSGS, lambda: [rand_value(rnd, MSGS, 0) for _ in range(1024)]),
             "b": (MAP_MSGS, lambda: [map_value(rnd, 8) for _ in range(1024)]),
             "c": (MAP_MSGS, lambda: [map_value(rnd, 64, compact=True) for _ in range(1024)]),
             "d": (EVENT_MSGS, lambda: [event_value(rnd, i) for i in range(1024)])}

@@ -205,16 +205,28 @@ def proto_encode(fields, rows, row_off, misalign: int = 0):
     return out, off, meta[:n]
 
 
-def proto_encode_nested(msgs, root, rows, row_off, misalign: int = 0):
-    """pbn_size + pbn_emit (proto_nested_device.cuh) on the CPU → (out, out_off, meta).  The descriptor comes from the
-    product's own validation (gofr_proto_nested_describe: host code, no GPU)."""
+def _pbn_desc(msgs, root, presence_instance):
+    """the descriptor the host hands to the nested kernels, from the product's own validation (gofr_proto_nested_describe_ex
+    with the description's presence bytes: host code, no GPU).  Its presence byte (byte 1) and maps half-word pick the
+    instance the emulation runs, as they pick the kernels on the host.  presence_instance: that byte set whatever the
+    description, so that the presence instance runs a presence-free description too."""
     from gofr_b200 import _abi
-    n = len(row_off) - 1
     nm, nf, n_fields = S.proto_nested_tables(msgs)
+    pr = S.proto_nested_presence(msgs)
     lib().emu_pbn_desc_bytes.restype = C.c_uint32
     desc = np.zeros(int(lib().emu_pbn_desc_bytes()), dtype=np.uint8)
-    _abi.check(_abi.lib().gofr_proto_nested_describe(nm.ctypes.data, len(msgs), nf.ctypes.data, n_fields, root, desc.ctypes.data, desc.size),
-               "gofr_proto_nested_describe")
+    _abi.check(_abi.lib().gofr_proto_nested_describe_ex(nm.ctypes.data, len(msgs), nf.ctypes.data, n_fields, root,
+                                                        None if pr is None else pr.ctypes.data, desc.ctypes.data, desc.size),
+               "gofr_proto_nested_describe_ex")
+    if presence_instance:
+        desc[1] = 1
+    return desc
+
+
+def proto_encode_nested(msgs, root, rows, row_off, misalign: int = 0, presence_instance: bool = False):
+    """pbn_size + pbn_emit (proto_nested_device.cuh) on the CPU → (out, out_off, meta)"""
+    n = len(row_off) - 1
+    desc = _pbn_desc(msgs, root, presence_instance)
     cap = int(rows.size) * 4 + 64 * n + 64 + misalign
     out = np.full(cap, 0xEE, dtype=np.uint8)
     off = np.zeros(n + 1, dtype=np.uint32)
@@ -228,20 +240,10 @@ def proto_encode_nested(msgs, root, rows, row_off, misalign: int = 0):
     return out, off, meta[:n]
 
 
-def _pbn_desc(msgs, root):
-    from gofr_b200 import _abi
-    nm, nf, n_fields = S.proto_nested_tables(msgs)
-    lib().emu_pbn_desc_bytes.restype = C.c_uint32
-    desc = np.zeros(int(lib().emu_pbn_desc_bytes()), dtype=np.uint8)
-    _abi.check(_abi.lib().gofr_proto_nested_describe(nm.ctypes.data, len(msgs), nf.ctypes.data, n_fields, root, desc.ctypes.data, desc.size),
-               "gofr_proto_nested_describe")
-    return desc
-
-
-def proto_decode_nested(msgs, root, frames, in_off):
+def proto_decode_nested(msgs, root, frames, in_off, presence_instance: bool = False):
     """pdn_decode_size + pdn_decode_emit (proto_nested_decode_device.cuh) on the CPU → (rows, row_off, meta)"""
     n = len(in_off) - 1
-    desc = _pbn_desc(msgs, root)
+    desc = _pbn_desc(msgs, root, presence_instance)
     cap = int(frames.size) * 10 + 4096 * max(n, 1)
     rows = np.full(cap, 0xEE, dtype=np.uint8)
     off = np.zeros(n + 1, dtype=np.uint32)

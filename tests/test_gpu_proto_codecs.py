@@ -7,7 +7,7 @@ is compared there with the oracle and python protobuf.  What exists only in the 
 the look-back that chain the packed offsets, the `fits` check that drops a whole tile when the output buffer is too small,
 and the staging Writer's partial 16-byte windows at frame edges.  Each campaign below feeds one kernel seeded inputs that
 reach those paths — all scalar types, tags of one to five bytes, hostile and mutated frames, lying headers, long strings —
-and requires the GPU result to equal the oracle (or, for map fields, the model tests/proto_maps_model.py) byte for byte,
+and requires the GPU result to equal the oracle (or, for map fields, the model tests/proto_nested_model.py) byte for byte,
 with 0xEE canaries behind every output.  The unmarked twin of each campaign checks on the CPU, on exactly the same inputs,
 that the oracle equals the emulated device code and agrees with python protobuf, so that a GPU mismatch is a kernel finding.
 
@@ -31,11 +31,10 @@ import pytest
 from gofr_b200 import _abi
 from gofr_b200 import spec as S
 from tests import oracle as O
-from tests import proto_maps_model as PM
+from tests import proto_nested_harness as H
+from tests import proto_nested_model as M
 from tests import test_grpc as TG
 from tests import test_proto as TP
-from tests import test_proto_maps as TM
-from tests import test_proto_nested as TN
 from tests.emu import emu
 
 ROOT_DIR = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -168,9 +167,9 @@ def reference(kind, spec, data, off):
     if kind in ("nenc", "ndec") and any(f.type == S.PB_MAP for fs in spec[0] for f in fs):
         msgs, root = spec
         if kind == "nenc":
-            items, meta = PM.encode(msgs, root, data, off)
+            items, meta = M.encode(msgs, root, data, off)
         else:
-            items, meta = PM.decode(msgs, root, [data[int(off[i]):int(off[i + 1])].tobytes() for i in range(n)])
+            items, meta = M.decode(msgs, root, [data[int(off[i]):int(off[i + 1])].tobytes() for i in range(n)])
         return b"".join(items), np.cumsum([0] + [len(x) for x in items]).astype(np.uint32), np.array(meta, dtype=np.uint32)
     if kind == "hello":
         out, o, meta = O.grpc_hello(data, off)
@@ -560,8 +559,8 @@ def _with_field(fields, f):
 
 
 def _nested_types(rnd):
-    msgs = TN._rand_types(rnd)
-    msgs[0] = _with_field(msgs[0], F(70000, rnd.choice(TN.SCALARS), rnd.random() < 0.5))
+    msgs = H.rand_types(rnd)
+    msgs[0] = _with_field(msgs[0], F(70000, rnd.choice(H.SCALARS), rnd.random() < 0.5))
     msgs[-1] = _with_field(msgs[-1], F(2 ** 29 - 1, rnd.choice([S.PB_STRING, S.PB_SINT64, S.PB_FIXED32]), rnd.random() < 0.5))
     return msgs
 
@@ -604,7 +603,7 @@ def nested_encoder_cases():
     cases = []
     for k in range(8):
         msgs = DEEP_STRINGS if k == 0 else _nested_types(rnd)
-        values = [TN._rand_value(rnd, msgs, 0) for _ in range(NESTED_ROWS)]
+        values = [H.rand_value(rnd, msgs, 0) for _ in range(NESTED_ROWS)]
         depths = set()
         py = list(values)
         for i in range(0, len(values), 9):           # one string made invalid UTF-8
@@ -642,8 +641,8 @@ def test_nested_encoder_cases_three_ways():
             assert np.array_equal(e_meta, meta) and np.array_equal(e_off, o + mis)
             assert e_out[mis:int(e_off[-1])].tobytes() == out[:int(o[-1])].tobytes()
         idx = [i for i, v in enumerate(values) if v is not None]
-        py = TN._py_frames(msgs, 0, [values[i] for i in idx])
-        fr = TN._frames(out, o)
+        py = H.py_frames(msgs, 0, [values[i] for i in idx])
+        fr = H.frames_of(out, o)
         for i, p in zip(idx, py):
             assert meta[i] == OK and fr[i] == p, i
         poisoned = np.array([v is None for v in values[:NESTED_ROWS]])
@@ -669,19 +668,19 @@ def _gpu_nested_encoder(eng):
 def nested_decoder_cases():
     """[(label, msgs, frames)] map-free (oracle) and with map fields (model)"""
     rnd = random.Random(0xD0D0)
-    cases = [("hostile", TN.HOSTILE_MSGS, [_frame(b) for b in TN.HOSTILE_BODIES] + TN.HOSTILE_HEADER_FRAMES)]
+    cases = [("hostile", H.HOSTILE_MSGS, [_frame(b) for b in H.HOSTILE_BODIES] + H.HOSTILE_HEADER_FRAMES)]
     for k in range(12):
         msgs = _nested_types(rnd)
-        rows, off = S.pack_proto_nested_rows(msgs, 0, [TN._rand_value(rnd, msgs, 0) for _ in range(400)])
+        rows, off = S.pack_proto_nested_rows(msgs, 0, [H.rand_value(rnd, msgs, 0) for _ in range(400)])
         out, o, _ = O.proto_encode_nested(msgs, 0, rows, off)
-        frames = [fr if i % 4 == 0 else _frame(_mutate(rnd, fr[5:])) for i, fr in enumerate(TN._frames(out, o))]
+        frames = [fr if i % 4 == 0 else _frame(_mutate(rnd, fr[5:])) for i, fr in enumerate(H.frames_of(out, o))]
         cases.append(("mutated %d" % k, msgs, frames))
-    entries = [b"".join(TM._A(b"k%03d" % k, TM._V1) for k in range(n)) for n in (64, 65)]
-    cases.append(("maps: non-canonical", TM.NONCANON_MSGS, [_frame(b) for b in TM.NONCANON_OK + TM.NONCANON_DEFER + TM.NONCANON_BAD + entries]))
+    entries = [b"".join(H._A(b"k%03d" % k, H._V1) for k in range(n)) for n in (64, 65)]
+    cases.append(("maps: non-canonical", H.NONCANON_MSGS, [_frame(b) for b in H.NONCANON_OK + H.NONCANON_DEFER + H.NONCANON_BAD + entries]))
     for k in range(6):
-        msgs = TM._rand_map_types(rnd)
-        rows, off = S.pack_proto_nested_rows(msgs, 0, [TM._rand_map_value(rnd, msgs, 0) for _ in range(300)])
-        frames, _ = PM.encode(msgs, 0, rows, off)
+        msgs = H.rand_map_types(rnd)
+        rows, off = S.pack_proto_nested_rows(msgs, 0, [H.rand_map_value(rnd, msgs, 0) for _ in range(300)])
+        frames, _ = M.encode(msgs, 0, rows, off)
         frames = [fr if i % 4 == 0 else _frame(_mutate(rnd, fr[5:])) for i, fr in enumerate(frames)]
         cases.append(("maps: mutated %d" % k, msgs, frames))
     return cases
@@ -692,12 +691,12 @@ def test_nested_decoder_cases_three_ways():
     fields: model == device code (CPU), pure-python protobuf agrees; 64 entries of one map field decode, 65 are DEFER"""
     for label, msgs, frames in nested_decoder_cases():
         if label.startswith("maps"):
-            rows, meta = TM._decode_model_emu(msgs, 0, frames)
-            TM._check_python_parse(msgs, 0, frames, rows, meta)
+            rows, meta = H.decode_model_emu(msgs, 0, frames)
+            H.check_python_parse(msgs, 0, frames, rows, meta)
             if label == "maps: non-canonical":
                 assert meta[-2:] == [OK, DEFER]
         else:
-            TN._decode_three_ways(msgs, 0, frames)
+            H.decode_three_ways(msgs, 0, frames)
 
 
 def _gpu_nested_decoder(eng):
@@ -707,7 +706,7 @@ def _gpu_nested_decoder(eng):
         want = reference("ndec", (msgs, 0), raw, off)
         check_equal(gpu_run(eng, "ndec", (msgs, 0), raw, off, len(want[0]) + 16), want, "nested decoder " + label)
         n += len(frames)
-    return "nested decoder: %d frames equal to the oracle / the maps model" % n
+    return "nested decoder: %d frames equal to the oracle / the model" % n
 
 
 # ---------------------------------------------------------------------------------------------------------------
@@ -722,24 +721,24 @@ def capacity_inputs():
     rows, off = S.pack_proto_rows(fields, msgs)
     out, o, _ = O.proto_encode(fields, rows, off)
     f_raw, f_off = _pack([fr for fr in TP._frames(out, o)])
-    values = [TN._rand_value(rnd, TN.MSGS, 0) for _ in range(1000)]
+    values = [H.rand_value(rnd, H.MSGS, 0) for _ in range(1000)]
     for v in values[7::50]:
         v[2] = b"\xff"                                  # PAGE.3, a string: BAD_UTF8, no frame
-    n_rows, n_off = S.pack_proto_nested_rows(TN.MSGS, 0, values)
-    out, o, _ = O.proto_encode_nested(TN.MSGS, 0, n_rows, n_off)
-    nf_raw, nf_off = _pack(TN._frames(out, o))
-    mm = TM._rand_map_types(rnd)
-    values = [TM._rand_map_value(rnd, mm, 0) for _ in range(800)]
+    n_rows, n_off = S.pack_proto_nested_rows(H.MSGS, 0, values)
+    out, o, _ = O.proto_encode_nested(H.MSGS, 0, n_rows, n_off)
+    nf_raw, nf_off = _pack(H.frames_of(out, o))
+    mm = H.rand_map_types(rnd)
+    values = [H.rand_map_value(rnd, mm, 0) for _ in range(800)]
     for v in values[::23]:                              # a duplicate key: BAD_ROW, no frame
         k = next((j for j, f in enumerate(mm[0]) if f.type == S.PB_MAP and v[j]), None)
         if k is not None:
             key = next(iter(v[k]))
             v[k] = [(key, v[k][key])] * 2
     m_rows, m_off = S.pack_proto_nested_rows(mm, 0, values)
-    frames, _ = PM.encode(mm, 0, m_rows, m_off)
+    frames, _ = M.encode(mm, 0, m_rows, m_off)
     mf_raw, mf_off = _pack(frames)
     return [("hello", "hello", None, h_raw, h_off), ("flat encoder", "enc", fields, rows, off), ("flat decoder", "dec", fields, f_raw, f_off),
-            ("nested encoder", "nenc", (TN.MSGS, 0), n_rows, n_off), ("nested decoder", "ndec", (TN.MSGS, 0), nf_raw, nf_off),
+            ("nested encoder", "nenc", (H.MSGS, 0), n_rows, n_off), ("nested decoder", "ndec", (H.MSGS, 0), nf_raw, nf_off),
             ("maps encoder", "nenc", (mm, 0), m_rows, m_off), ("maps decoder", "ndec", (mm, 0), mf_raw, mf_off)]
 
 

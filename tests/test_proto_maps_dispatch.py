@@ -6,26 +6,25 @@ import numpy as np
 
 from gofr_b200 import spec as S
 from gofr_b200 import _abi
-from tests.test_proto_nested import MSGS
+from tests import proto_nested_harness as H
 
 F = S.ProtoNField
 INVALID, CAP = 1, 7   # GOFR_ERR_INVALID; GOFR_ERR_CAPACITY = "valid, but no room to write the descriptor"
 
 
-def _describe(nm, n_msgs, nf, k, root=0, desc=None):
-    return _abi.lib().gofr_proto_nested_describe(nm.ctypes.data, n_msgs, nf.ctypes.data, k, root,
-                                                 None if desc is None else desc.ctypes.data, 0 if desc is None else desc.size)
+def _describe(nm, n_msgs, nf, k):
+    """the ABI call on hand-edited tables (spec.proto_nested_tables cannot make them)"""
+    return _abi.lib().gofr_proto_nested_describe(nm.ctypes.data, n_msgs, nf.ctypes.data, k, 0, None, 0)
 
 
 def _maps_word(msgs):
-    nm, nf, k = S.proto_nested_tables(msgs)
     desc = np.zeros(512, np.uint8)
-    assert _describe(nm, len(msgs), nf, k, 0, desc) == 0
+    assert H.describe(msgs, 0, desc) == 0
     return int(desc[2]) | int(desc[3]) << 8
 
 
 def test_descriptor_marks_descriptions_with_maps():
-    assert _maps_word(MSGS) == 0
+    assert _maps_word(H.MSGS) == 0
     assert _maps_word([[F(1, S.PB_INT32), F(2, S.PB_MESSAGE, True, 1)], [F(1, S.PB_STRING)]]) == 0
     assert _maps_word([[F(1, S.PB_MAP, False, 1)], [F(1, S.PB_STRING), F(2, S.PB_INT32)]]) == 1
     # a map two levels down marks the whole description

@@ -6,7 +6,8 @@ Reference behaviour: proto.Marshal of the message a unary handler returns + grpc
   python google.protobuf with descriptors built at run time (independent implementation, deterministic field order)
   the oracle (oracle/orc_proto_nested.c: recursive, a message marshalled into its own buffer)
   the device code (proto_nested_device.cuh: explicit stack, nested lengths from a sizing walk) on the CPU via tests/emu,
-  and the CUDA kernel with -m gpu."""
+  and the CUDA kernel with -m gpu.
+Generators, fixtures and the python protobuf classes are shared with the map and presence tests (tests/proto_nested_harness.py)."""
 import random
 import struct
 
@@ -14,70 +15,19 @@ import numpy as np
 import pytest
 
 from gofr_b200 import spec as S
-from gofr_b200 import _abi
 from tests import oracle as O
+from tests import proto_nested_harness as H
 from tests.emu import emu
 
-SCALARS = [S.PB_DOUBLE, S.PB_FLOAT, S.PB_INT64, S.PB_UINT64, S.PB_INT32, S.PB_FIXED64, S.PB_FIXED32, S.PB_BOOL, S.PB_STRING,
-           S.PB_BYTES, S.PB_UINT32, S.PB_SFIXED32, S.PB_SFIXED64, S.PB_SINT32, S.PB_SINT64]
 F = S.ProtoNField
-
-
-def _py_classes(msgs):
-    from google.protobuf import descriptor_pb2, descriptor_pool, message_factory
-    fdp = descriptor_pb2.FileDescriptorProto(name="n.proto", package="n", syntax="proto3")
-    for m, fields in enumerate(msgs):
-        mt = fdp.message_type.add(name="M%d" % m)
-        for f in fields:
-            # an enum field encodes exactly like int32 (and would need an enum type here)
-            kw = dict(name="f%d" % f.number, number=f.number, type=S.PB_INT32 if f.type == S.PB_ENUM else f.type, label=3 if f.repeated else 1)
-            if f.type == S.PB_MESSAGE:
-                kw["type_name"] = ".n.M%d" % f.msg
-            mt.field.add(**kw)
-    pool = descriptor_pool.DescriptorPool()
-    pool.Add(fdp)
-    return [message_factory.GetMessageClass(pool.FindMessageTypeByName("n.M%d" % m)) for m in range(len(msgs))]
-
-
-def _py_fill(classes, msgs, m, value):
-    obj = classes[m]()
-    for f, v in zip(msgs[m], value):
-        name = "f%d" % f.number
-        conv = (lambda x: x.decode("utf-8") if isinstance(x, (bytes, bytearray)) else x) if f.type == S.PB_STRING else (lambda x: x)
-        if f.repeated:
-            if f.type == S.PB_MESSAGE:
-                for e in v:
-                    getattr(obj, name).add().CopyFrom(_py_fill(classes, msgs, f.msg, e))
-            else:
-                getattr(obj, name).extend([conv(e) for e in v])
-        elif f.type == S.PB_MESSAGE:
-            if v is not None:
-                getattr(obj, name).CopyFrom(_py_fill(classes, msgs, f.msg, v))
-                getattr(obj, name).SetInParent()
-        else:
-            setattr(obj, name, conv(v))
-    return obj
-
-
-def _py_frames(msgs, root, values):
-    classes = _py_classes(msgs)
-    out = []
-    for v in values:
-        body = _py_fill(classes, msgs, root, v).SerializeToString(deterministic=True)
-        out.append(b"\x00" + len(body).to_bytes(4, "big") + body)
-    return out
-
-
-def _frames(out, off):
-    return [out[int(off[i]):int(off[i + 1])].tobytes() for i in range(len(off) - 1)]
 
 
 def _three_ways(msgs, root, values):
     rows, off = S.pack_proto_nested_rows(msgs, root, values)
     o_out, o_off, o_meta = O.proto_encode_nested(msgs, root, rows, off)
     assert not o_meta.any(), o_meta
-    want = _py_frames(msgs, root, values)
-    got = _frames(o_out, o_off)
+    want = H.py_frames(msgs, root, values)
+    got = H.frames_of(o_out, o_off)
     for i in range(len(values)):
         assert got[i] == want[i], (i, values[i], got[i].hex(), want[i].hex())
     for mis in (0, 3):
@@ -87,14 +37,6 @@ def _three_ways(msgs, root, values):
     return rows, off, o_out, o_off
 
 
-# the shapes of a typical API: a page of items with tags, an optional owner, per-item attributes and histograms
-ITEM = [F(1, S.PB_INT64), F(2, S.PB_STRING), F(3, S.PB_STRING, True), F(4, S.PB_DOUBLE, True), F(5, S.PB_MESSAGE, False, 2), F(7, S.PB_SINT32, True)]
-PAGE = [F(1, S.PB_MESSAGE, True, 1), F(2, S.PB_UINT32), F(3, S.PB_STRING), F(15, S.PB_MESSAGE, False, 2), F(16, S.PB_BOOL, True), F(2047, S.PB_FIXED64, True)]
-OWNER = [F(1, S.PB_STRING), F(2, S.PB_BYTES, True), F(3, S.PB_MESSAGE, False, 3)]
-GEO = [F(1, S.PB_FLOAT), F(2, S.PB_FLOAT), F(9, S.PB_ENUM, True)]
-MSGS = [PAGE, ITEM, OWNER, GEO]
-
-
 def test_known_answers_and_python_protobuf():
     geo = [1.5, -2.25, [1, 0, -1]]
     owner = ["ann", [b"\x00\xff", b""], geo]
@@ -102,8 +44,8 @@ def test_known_answers_and_python_protobuf():
     item2 = [0, "", [], [], None, []]                                   # an element that encodes to nothing: tag + length 0
     page = [[item1, item2], 2, "next", [ "", [], None], [True, False, True], [1, 2 ** 64 - 1]]
     empty = [[], 0, "", None, [], []]
-    rows, off, out, o = _three_ways(MSGS, 0, [page, empty, [[item2] * 3, 0, "", None, [], []]])
-    fr = _frames(out, o)
+    rows, off, out, o = _three_ways(H.MSGS, 0, [page, empty, [[item2] * 3, 0, "", None, [], []]])
+    fr = H.frames_of(out, o)
     assert fr[1] == b"\x00\x00\x00\x00\x00"                             # nothing set: an empty message, still a frame
     assert fr[2] == b"\x00\x00\x00\x00\x06" + b"\x0a\x00" * 3           # three empty items: tag 1/LEN + length 0 each
     # a set but empty singular message is written (field 15 = tag 0x7a, length 0); packed bools; packed fixed64 under a
@@ -112,66 +54,11 @@ def test_known_answers_and_python_protobuf():
     assert (2047 << 3 | 2).to_bytes(2, "little") != b"" and bytes([0xFA, 0x7F, 0x10]) in fr[0]
 
 
-def _rand_types(rnd):
-    """up to 5 acyclic message types (type m may use types > m), at most 4 levels deep from the root"""
-    n = rnd.randint(1, 5)
-    msgs = []
-    depth_below = [1] * n
-    for m in reversed(range(n)):
-        fields, numbers = [], sorted(rnd.sample(range(1, 40), rnd.randint(1, 6)) + ([rnd.choice([100, 2047, 2048, 70000])] if rnd.random() < 0.3 else []))
-        for num in sorted(set(numbers)):
-            usable = [k for k in range(m + 1, n) if 1 + depth_below[k] <= 4 - 0]
-            if usable and rnd.random() < 0.35:
-                k = rnd.choice(usable)
-                fields.append(F(num, S.PB_MESSAGE, rnd.random() < 0.5, k))
-                depth_below[m] = max(depth_below[m], 1 + depth_below[k])
-            else:
-                fields.append(F(num, rnd.choice(SCALARS), rnd.random() < 0.4))
-        msgs.insert(0, fields)
-    # the indices used above refer to final positions m+1..n-1: types were built back to front into position m
-    if depth_below[0] > 4:
-        return _rand_types(rnd)
-    return msgs
-
-
-def _rand_scalar(rnd, t):
-    if t == S.PB_DOUBLE:
-        return rnd.choice([0.0, -0.0, 1.5, -1e300, 5e-324, float(rnd.randint(-5, 5))])
-    if t == S.PB_FLOAT:
-        return rnd.choice([0.0, -0.0, 1.5, -2.25, 3.0e38, float(rnd.randint(-5, 5))])
-    if t in (S.PB_INT64, S.PB_SINT64, S.PB_SFIXED64):
-        return rnd.choice([0, 1, -1, 2 ** 63 - 1, -2 ** 63, rnd.randint(-10 ** 6, 10 ** 6)])
-    if t in (S.PB_UINT64, S.PB_FIXED64):
-        return rnd.choice([0, 1, 2 ** 64 - 1, 127, 128, rnd.randint(0, 10 ** 12)])
-    if t in (S.PB_INT32, S.PB_SINT32, S.PB_SFIXED32, S.PB_ENUM):
-        return rnd.choice([0, 1, -1, 2 ** 31 - 1, -2 ** 31, rnd.randint(-1000, 1000)])
-    if t in (S.PB_UINT32, S.PB_FIXED32):
-        return rnd.choice([0, 1, 2 ** 32 - 1, 16383, 16384])
-    if t == S.PB_BOOL:
-        return rnd.random() < 0.5
-    if t == S.PB_STRING:
-        return rnd.choice(["", "a", "héllo", "x" * 130, "日本", "tab\t"])
-    return rnd.choice([b"", b"\x00", b"\xff\xfe", b"b" * 200])
-
-
-def _rand_value(rnd, msgs, m, depth=0):
-    v = []
-    for f in msgs[m]:
-        one = (lambda: _rand_value(rnd, msgs, f.msg, depth + 1)) if f.type == S.PB_MESSAGE else (lambda: _rand_scalar(rnd, f.type))
-        if f.repeated:
-            v.append([one() for _ in range(rnd.choice([0, 0, 1, 2, 5]))])
-        elif f.type == S.PB_MESSAGE:
-            v.append(None if rnd.random() < 0.4 else one())
-        else:
-            v.append(one())
-    return v
-
-
 @pytest.mark.parametrize("seed", range(25))
 def test_random_types_three_ways(seed):
     rnd = random.Random(500 + seed)
-    msgs = _rand_types(rnd)
-    values = [_rand_value(rnd, msgs, 0) for _ in range(60)]
+    msgs = H.rand_types(rnd)
+    values = [H.rand_value(rnd, msgs, 0) for _ in range(60)]
     _three_ways(msgs, 0, values)
 
 
@@ -201,23 +88,9 @@ def test_invalid_utf8_and_malformed_rows():
 
 
 def test_descriptions_outside_the_limits_are_refused():
-    L = _abi.lib()
-
-    def describe(msgs, root=0):
-        nm, nf, k = S.proto_nested_tables(msgs)
-        return L.gofr_proto_nested_describe(nm.ctypes.data, len(msgs), nf.ctypes.data, k, root, None, 0)
-    CAP = 7   # GOFR_ERR_CAPACITY: "valid, but no room to write the descriptor"
-    assert describe(MSGS) == CAP
-    assert describe([[F(1, S.PB_MESSAGE, False, 0)]]) != CAP                                   # recursive type
-    assert describe([[F(1, S.PB_MESSAGE, False, 1)], [F(1, S.PB_MESSAGE, True, 0)]]) != CAP    # mutually recursive
-    assert describe([[F(2, S.PB_INT32), F(1, S.PB_INT32)]]) != CAP                             # not in field-number order
-    assert describe([[F(1, S.PB_MESSAGE, False, 3)]]) != CAP                                   # unknown message type
-    assert describe([[F(1, 10)]]) != CAP                                                       # TYPE_GROUP
-    assert describe([[F(0, S.PB_INT32)]]) != CAP and describe([[F(19500, S.PB_INT32)]]) != CAP  # reserved numbers
-    chain = [[F(1, S.PB_MESSAGE, False, m + 1)] for m in range(4)] + [[F(1, S.PB_INT32)]]
-    assert describe(chain) != CAP and describe(chain[1:4] + [[F(1, S.PB_INT32)]]) != CAP - 99  # 5 levels: too deep
-    ok4 = [[F(1, S.PB_MESSAGE, False, 1)], [F(1, S.PB_MESSAGE, False, 2)], [F(1, S.PB_MESSAGE, False, 3)], [F(1, S.PB_INT32)]]
-    assert describe(ok4) == CAP
+    """recursive types, field order, unknown types, groups, reserved numbers and depth (the table: H.LIMIT_DESCRIPTIONS)"""
+    for msgs, root, want in H.LIMIT_DESCRIPTIONS:
+        assert H.describe(msgs, root) == want, msgs
 
 
 @pytest.mark.gpu
@@ -229,8 +102,8 @@ def test_gpu_matches_oracle():
     assert torch.cuda.is_available()
     rnd = random.Random(77)
     eng = Engine(Table(synth.config1_spec()), 0)
-    for msgs in (MSGS, _rand_types(rnd), _rand_types(rnd)):
-        values = [_rand_value(rnd, msgs, 0) for _ in range(5000)]
+    for msgs in (H.MSGS, H.rand_types(rnd), H.rand_types(rnd)):
+        values = [H.rand_value(rnd, msgs, 0) for _ in range(5000)]
         rows, off = S.pack_proto_nested_rows(msgs, 0, values)
         o_out, o_off, o_meta = O.proto_encode_nested(msgs, 0, rows, off)
         d_out, d_off, d_meta = eng.proto_encode_nested_device(msgs, 0, rows, off)
@@ -244,95 +117,15 @@ def test_gpu_matches_oracle():
 # ---------------------------------------------------------------------------------------------------------------
 # the other direction: frames -> rows (gofr_proto_decode_nested_device)
 # ---------------------------------------------------------------------------------------------------------------
-def _py_to_value(msgs, m, obj):
-    """the value list pack_proto_nested_rows takes, from a parsed python protobuf message"""
-    v = []
-    for f in msgs[m]:
-        x = getattr(obj, "f%d" % f.number)
-        conv = (lambda e: e.encode("utf-8")) if f.type == S.PB_STRING else (lambda e: e)
-        if f.repeated:
-            v.append([_py_to_value(msgs, f.msg, e) for e in x] if f.type == S.PB_MESSAGE else [conv(e) for e in x])
-        elif f.type == S.PB_MESSAGE:
-            v.append(_py_to_value(msgs, f.msg, x) if obj.HasField("f%d" % f.number) else None)
-        else:
-            v.append(conv(x))
-    return v
-
-
-def _frame(body: bytes) -> bytes:
-    return b"\x00" + len(body).to_bytes(4, "big") + body
-
-
-def _pack_frames(frames):
-    blob, offs = bytearray(), [0]
-    for fr in frames:
-        blob += fr
-        offs.append(len(blob))
-    return np.frombuffer(bytes(blob) + b"\0" * 16, dtype=np.uint8).copy(), np.array(offs, dtype=np.uint32)
-
-
-def _varint(v):
-    out = bytearray()
-    while v >= 0x80:
-        out.append(v & 0x7F | 0x80)
-        v >>= 7
-    out.append(v)
-    return bytes(out)
-
-
-def _has_overlong_varint(body: bytes) -> bool:
-    run = 0
-    for b in body:
-        if b >= 0x80:
-            run += 1
-        else:
-            if run >= 9 and b > 1:
-                return True
-            run = 0
-        if run >= 10:
-            return True
-    return False
-
-
-def _decode_three_ways(msgs, root, frames):
-    """oracle == device code on everything; python protobuf decides what the rows of well-formed frames must be"""
-    raw, off = _pack_frames(frames)
-    o_rows, o_off, o_meta = O.proto_decode_nested(msgs, root, raw, off)
-    e_rows, e_off, e_meta = emu.proto_decode_nested(msgs, root, raw, off)
-    assert np.array_equal(o_meta, e_meta), (o_meta, e_meta)
-    assert np.array_equal(o_off, e_off)
-    assert o_rows[:int(o_off[-1])].tobytes() == e_rows[:int(o_off[-1])].tobytes()
-    classes = _py_classes(msgs)
-    from google.protobuf.message import DecodeError
-    for i, fr in enumerate(frames):
-        body = fr[5:]
-        try:
-            obj = classes[root]()
-            obj.ParseFromString(body)
-            ok = True
-        except DecodeError:
-            ok = False
-        if o_meta[i] in (S.GRPC_COMPRESSED, S.GRPC_BAD_LENGTH, S.GRPC_DEFER):
-            continue
-        if ok and o_meta[i] == S.GRPC_BAD_PROTO and _has_overlong_varint(body):
-            continue      # protowire.ConsumeVarint refuses a tenth byte above 1; upb silently truncates it
-        assert ok == (o_meta[i] == S.GRPC_OK), (i, fr.hex(), o_meta[i], ok)
-        if ok:
-            want, _ = S.pack_proto_nested_rows(msgs, root, [_py_to_value(msgs, root, obj)])
-            got = o_rows[int(o_off[i]):int(o_off[i + 1])].tobytes()
-            assert got == want[:len(got)].tobytes() and len(got) == (len(want) - 8 + 3) // 4 * 4, (i, fr.hex())
-    return o_rows, o_off, o_meta
-
-
 def test_decode_canonical_frames_round_trip():
     """decode(encode(row)) == row, and python protobuf parses the frames to the same values"""
     rnd = random.Random(9)
-    for msgs in (MSGS, _rand_types(rnd), _rand_types(rnd), _rand_types(rnd)):
-        values = [_rand_value(rnd, msgs, 0) for _ in range(80)]
+    for msgs in (H.MSGS, H.rand_types(rnd), H.rand_types(rnd), H.rand_types(rnd)):
+        values = [H.rand_value(rnd, msgs, 0) for _ in range(80)]
         rows, off = S.pack_proto_nested_rows(msgs, 0, values)
         out, o, meta = O.proto_encode_nested(msgs, 0, rows, off)
-        frames = _frames(out, o)
-        d_rows, d_off, d_meta = _decode_three_ways(msgs, 0, frames)
+        frames = H.frames_of(out, o)
+        d_rows, d_off, d_meta = H.decode_three_ways(msgs, 0, frames)
         assert not d_meta.any()
         for i in range(len(values)):
             a = rows[int(off[i]):int(off[i + 1])].tobytes()
@@ -341,41 +134,10 @@ def test_decode_canonical_frames_round_trip():
             assert a == b, (i, values[i])
 
 
-# message types and frames, well-formed but not canonical, or hostile: statuses as test_decode_noncanonical_and_hostile_frames
-# states them (the singular message sent twice is DEFER; the four header frames come last)
-HOSTILE_MSGS = [[F(1, S.PB_INT32), F(2, S.PB_STRING), F(3, S.PB_SINT64, True), F(4, S.PB_MESSAGE, False, 1), F(5, S.PB_MESSAGE, True, 1),
-                 F(6, S.PB_FIXED32, True), F(7, S.PB_STRING, True), F(8, S.PB_DOUBLE, True), F(9, S.PB_BOOL)],
-                [F(1, S.PB_STRING), F(2, S.PB_UINT64, True), F(3, S.PB_BYTES)]]
-_SUB = b"\x0a\x02hi" + b"\x10\x05" + b"\x12\x02\x01\x02" + b"\x1a\x01\xff"         # name, unpacked + packed uint64, bytes
-HOSTILE_BODIES = [
-    b"",                                                           # nothing
-    b"\x08\x01\x08\x02",                                           # singular scalar twice: last wins
-    b"\x12\x01a\x12\x02bc",                                        # string twice: last wins
-    b"\x18\x01\x18\x03" + b"\x1a\x02\x05\x07" + b"\x18\x09",       # repeated sint64: unpacked, packed, unpacked — wire order
-    b"\x22" + _varint(len(_SUB)) + _SUB,                             # singular message
-    b"\x2a\x00" + b"\x2a" + _varint(len(_SUB)) + _SUB + b"\x2a\x00",  # three elements, two empty
-    b"\x35\x01\x00\x00\x00" + b"\x32\x08\x02\x00\x00\x00\x03\x00\x00\x00",  # fixed32 unpacked then packed
-    b"\x3a\x00\x3a\x01x",                                          # repeated strings incl. an empty one
-    b"\x42\x10" + struct.pack("<dd", 1.5, -0.0) + b"\x41" + struct.pack("<d", 2.5),  # doubles packed + unpacked
-    b"\x48\x02",                                                   # bool from a varint that is not 0 / 1
-    b"\x0d\x01\x00\x00\x00" + b"\x10\x07" + b"\xf8\x07\x01" + b"\x92\x03\x03abc",    # foreign wire types and unknown numbers: skipped
-    b"\x0b\x08\x01\x13\x14\x0c" + b"\x08\x05",                      # unknown groups, nested, balanced
-    b"\x22\x02\x0a\x00" + b"\x08\x03",                             # message with an explicit empty string
-    b"\x22\x00\x22\x00",                                           # singular message twice: protobuf-go merges -> DEFER
-    b"\x2a\x04\x22\x02\x08\x01",                                   # element with fields the sub-message does not know
-    # malformed
-    b"\x08", b"\x12\x05ab", b"\x22\x03\x0a\x05a", b"\x0b\x08\x01", b"\x0c", b"\x32\x03\x01\x00\x00", b"\x1a\x02\x80\x80",
-    b"\x00\x01", b"\x0e\x01", b"\x42\x07" + b"\0" * 7, b"\x2a\x02\x12\x05",
-    # invalid UTF-8: top level, in an element, in an occurrence that is overwritten later
-    b"\x12\x01\xff", b"\x2a\x03\x0a\x01\xc3", b"\x12\x01\xff\x12\x01a", b"\x3a\x02\xed\xa0",
-]
-HOSTILE_HEADER_FRAMES = [b"\x01\x00\x00\x00\x00", b"\x00\x00\x00\x00\x05\x08", b"\x00\x00", b"\x02\x00\x00\x00\x00"]   # header problems
-
-
 def test_decode_noncanonical_and_hostile_frames():
-    msgs = HOSTILE_MSGS
-    frames = [_frame(b) for b in HOSTILE_BODIES] + HOSTILE_HEADER_FRAMES
-    rows, off, meta = _decode_three_ways(msgs, 0, frames)
+    msgs = H.HOSTILE_MSGS
+    frames = [H.frame(b) for b in H.HOSTILE_BODIES] + H.HOSTILE_HEADER_FRAMES
+    rows, off, meta = H.decode_three_ways(msgs, 0, frames)
     assert list(meta[:15]) == [S.GRPC_OK] * 13 + [S.GRPC_DEFER, S.GRPC_OK]
     assert all(m == S.GRPC_BAD_PROTO for m in meta[15:26]) and all(m == S.GRPC_BAD_UTF8 for m in meta[26:30])
     assert list(meta[30:]) == [S.GRPC_COMPRESSED, S.GRPC_BAD_LENGTH, S.GRPC_BAD_LENGTH, S.GRPC_BAD_LENGTH]
@@ -390,12 +152,12 @@ def test_decode_mutated_frames_device_code_equals_oracle(seed):
     """frames of random message types with bytes flipped, inserted and cut: oracle == device code on status and row, and
     python protobuf agrees on which frames parse (DEFER aside)"""
     rnd = random.Random(800 + seed)
-    msgs = _rand_types(rnd)
-    values = [_rand_value(rnd, msgs, 0) for _ in range(60)]
+    msgs = H.rand_types(rnd)
+    values = [H.rand_value(rnd, msgs, 0) for _ in range(60)]
     rows, off = S.pack_proto_nested_rows(msgs, 0, values)
     out, o, meta = O.proto_encode_nested(msgs, 0, rows, off)
     frames = []
-    for fr in _frames(out, o):
+    for fr in H.frames_of(out, o):
         body = bytearray(fr[5:])
         for _ in range(rnd.randint(0, 2)):
             r = rnd.random()
@@ -409,8 +171,8 @@ def test_decode_mutated_frames_device_code_equals_oracle(seed):
             else:      # reorder: move the tail in front (fields may arrive in any order)
                 p = rnd.randrange(len(body) + 1)
                 body = body[p:] + body[:p]
-        frames.append(_frame(bytes(body)))
-    _decode_three_ways(msgs, 0, frames)
+        frames.append(H.frame(bytes(body)))
+    H.decode_three_ways(msgs, 0, frames)
 
 
 def _gpu_decode_check():
@@ -422,17 +184,17 @@ def _gpu_decode_check():
     assert torch.cuda.is_available()
     rnd = random.Random(78)
     eng = Engine(Table(synth.config1_spec()), 0)
-    for msgs in (MSGS, _rand_types(rnd), _rand_types(rnd)):
-        values = [_rand_value(rnd, msgs, 0) for _ in range(4000)]
+    for msgs in (H.MSGS, H.rand_types(rnd), H.rand_types(rnd)):
+        values = [H.rand_value(rnd, msgs, 0) for _ in range(4000)]
         rows, off = S.pack_proto_nested_rows(msgs, 0, values)
         out, o, _ = O.proto_encode_nested(msgs, 0, rows, off)
-        frames = _frames(out, o)
+        frames = H.frames_of(out, o)
         for i in range(0, len(frames), 7):          # every seventh frame damaged: statuses and empty rows must agree too
             body = bytearray(frames[i][5:])
             if body:
                 body[rnd.randrange(len(body))] ^= 1 << rnd.randrange(8)
-            frames[i] = _frame(bytes(body))
-        raw, in_off = _pack_frames(frames)
+            frames[i] = H.frame(bytes(body))
+        raw, in_off = H.pack_frames(frames)
         o_rows, o_off, o_meta = O.proto_decode_nested(msgs, 0, raw, in_off)
         d_rows, d_off, d_meta = eng.proto_decode_nested_device(msgs, 0, raw, in_off)
         torch.cuda.synchronize()
@@ -450,10 +212,4 @@ def _gpu_decode_check():
 def test_gpu_decode_matches_oracle():
     """gofr_proto_decode_nested_device on the GPU == oracle (statuses, offsets, rows) — in a child process, so that a fault
     in the kernel cannot leave a sticky CUDA error in the process the other GPU tests run in"""
-    import os
-    import subprocess
-    import sys
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    r = subprocess.run([sys.executable, "-c", "import tests.test_proto_nested as t; t._gpu_decode_check()"], cwd=root,
-                       capture_output=True, text=True, timeout=600)
-    assert r.returncode == 0, r.stdout[-2000:] + r.stderr[-4000:]
+    H.run_child("import tests.test_proto_nested as t; t._gpu_decode_check()", timeout=600)
