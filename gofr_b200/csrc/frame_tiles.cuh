@@ -1,7 +1,6 @@
 // frame_tiles.cuh — the tile loop shared by the frame codecs of the gRPC message path (grpc_kernel.cu: Hello, proto3 encoder /
-// decoder for flat messages; proto_nested_kernel.cu: the encoder for nested / repeated message types): persistent
-// co-resident CTAs, one thread per frame, the tile's input bytes staged with one TMA bulk copy, exact output sizes scanned in
-// the CTA and chained across CTAs by the decoupled look-back, frames packed in order through the staging Writer.
+// decoder for flat messages; proto_nested_*kernel.cu: the nested codecs), one thread per frame, on the tile skeleton of
+// tile_common.cuh; frames are packed in order through the staging Writer.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -27,65 +26,28 @@ struct GrpcShared {
 // The tile loop shared by the two frame codecs (Hello request → response, row → proto3 message).
 template <class Codec>
 __device__ __forceinline__ void frame_tiles(const GrpcParams& p, const Codec& cd, GrpcShared& sh) {
-    const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    if (tid == 0) {
-        mbar_init(&sh.bar, 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
+    const uint32_t tid = threadIdx.x;
+    if (tid == 0) tile_barrier_init(&sh.bar);
     __syncthreads();
     uint32_t parity = 0;
     for (uint32_t tile = blockIdx.x; tile < p.n_tiles; tile += gridDim.x) {
         const uint32_t i = tile * GT + tid;
         const bool valid = i < p.n;
-        const uint32_t t0 = tile * GT, t1 = min(p.n, t0 + GT);
-        const uint32_t lo = __ldg(p.in_off + t0) & ~15u, hi = (__ldg(p.in_off + t1) + 15u) & ~15u;
-        const bool staged = hi > lo && hi - lo <= kGrpcStage;
+        const ByteRange in = offset_range(p.in_off, tile * GT, min(p.n, tile * GT + GT));
         __syncthreads();  // previous tile's reads of sh.in are done
-        if (staged && tid == 0) {
-            mbar_expect_tx(&sh.bar, hi - lo);
-            bulk_g2s(sh.in, p.in + lo, hi - lo, &sh.bar);
-        }
+        stage_start(&sh.bar, sh.in, p.in, in, kGrpcStage);
         uint32_t fo = 0, fn = 0;
         if (valid) { fo = __ldg(p.in_off + i); fn = __ldg(p.in_off + i + 1) - fo; }
-        const uint8_t* base = p.in;
-        if (staged) {
-            mbar_wait(&sh.bar, parity);
-            parity ^= 1;
-            base = launder_after_sync((const uint8_t*)sh.in) - lo;
-        }
+        const uint8_t* base = stage_wait(&sh.bar, parity, sh.in, p.in, in, kGrpcStage);
         typename Codec::R r = cd.none();
         if (valid) r = cd.parse(base + fo, fn, fo);
 
-        uint32_t incl = r.out_len;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            uint32_t v = __shfl_up_sync(0xFFFFFFFFu, incl, o);
-            if (lane >= (uint32_t)o) incl += v;
-        }
-        if (lane == 31) sh.warp_sum[warp] = incl;
-        __syncthreads();
-        uint32_t warp_excl = 0, tile_total = 0;
-#pragma unroll
-        for (int w = 0; w < GNW; w++) {
-            uint32_t s = sh.warp_sum[w];
-            if ((uint32_t)w < warp) warp_excl += s;
-            tile_total += s;
-        }
-        const uint32_t excl = warp_excl + incl - r.out_len;
-        if (warp == 0) {
-            unsigned long long b = lookback(p.tile_state, p.epoch, tile, tile_total, lane);
-            if (lane == 0) sh.tile_base = b;
-        }
-        __syncthreads();
-        const unsigned long long tile_base = sh.tile_base;
-        const bool fits = tile_base + tile_total <= p.out_cap && tile_base + tile_total <= 0xFFFFFFFFull;
-        if (!fits && tid == 0) atomicExch(p.overflow, 1u);
+        const TilePlace t = place_tile(p, tile, r.out_len, sh.warp_sum, sh.tile_base);
         if (valid) {
-            p.out_off[i] = (uint32_t)(tile_base + excl);
+            put_offsets(p.out_off, i, p.n, t, r.out_len);
             p.meta[i] = r.status;
-            if (i == p.n - 1) p.out_off[p.n] = (uint32_t)(tile_base + excl + r.out_len);
         }
-        if (fits && valid && r.out_len) cd.emit(base + fo, r, p.out + tile_base + excl, &sh.stage[tid]);
+        if (t.fits && valid && r.out_len) cd.emit(base + fo, r, p.out + t.base + t.excl, &sh.stage[tid]);
     }
 }
 

@@ -1,10 +1,6 @@
 // grpc_kernel.cu — the gRPC message path over batches of length-prefixed frames, sm_90a: the unary Hello of config 5
 // (request frame → response frame) and the proto3 encoder / decoder for any flat message type (rows ↔ frames).
-//
-// Same execution model as serve_kernel.cu: persistent co-resident CTAs, one thread per frame, the tile's contiguous
-// input byte range pulled into shared memory with one TMA bulk copy, exact output sizes scanned in the CTA and chained
-// across CTAs by the decoupled look-back, responses packed in request order and written through the aligned staging
-// Writer (16-byte st.global.cs.v4).  Per-frame logic: grpc_device.cuh.
+// The tile loop is frame_tiles.cuh, on the skeleton of tile_common.cuh.  Per-frame logic: grpc_device.cuh.
 #include "frame_tiles.cuh"
 
 namespace gofr {

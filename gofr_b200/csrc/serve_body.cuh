@@ -94,8 +94,7 @@ __device__ __forceinline__ void serve_body(const ServeParams& p) {
         uint4* dst = (uint4*)tbl;
         for (uint32_t i = tid; i < p.hot_bytes / 16; i += T) dst[i] = src[i];
         if (tid == 0) {
-            mbar_init(&sh.bar, 1);
-            asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+            tile_barrier_init(&sh.bar);
             sh.defer_n = 0;
         }
     }
@@ -126,58 +125,13 @@ __device__ __forceinline__ void serve_body(const ServeParams& p) {
         const uint32_t end = data_off + data_len;
 
         // ---- the tile's arena byte range ----
-        uint32_t lo = valid ? arena_off : 0xFFFFFFFFu, hi = valid ? end : 0u;
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {
-            lo = min(lo, __shfl_xor_sync(0xFFFFFFFFu, lo, o));
-            hi = max(hi, __shfl_xor_sync(0xFFFFFFFFu, hi, o));
-        }
-        if (lane == 0) { sh.warp_lo[warp] = lo; sh.warp_hi[warp] = hi; }
+        warp_range(valid ? arena_off : 0xFFFFFFFFu, valid ? end : 0u, sh.warp_lo, sh.warp_hi);
         __syncthreads();  // also: every thread is done reading the previous tile's in_stage
-        if (tid == 0) {
-            uint32_t l = sh.warp_lo[0], h = sh.warp_hi[0];
-#pragma unroll
-            for (int w = 1; w < NW; w++) { l = min(l, sh.warp_lo[w]); h = max(h, sh.warp_hi[w]); }
-            l &= ~15u;
-            h = (h + 15u) & ~15u;
-            sh.in_lo = l;
-            sh.in_hi = h;
-            if (h > l && h - l <= p.in_cap) {
-                mbar_expect_tx(&sh.bar, h - l);
-                bulk_g2s(in_stage, p.arena + l, h - l, &sh.bar);
-            }
-#if defined(GOFR_PREFETCH_NEXT)
-            // the tile this CTA takes next: ask for its bytes in L2 now (a hint — the range is guessed from its first and
-            // last descriptor, which is exact whenever requests lie in the arena in index order)
-            const uint32_t nt = tile + gridDim.x;
-            if (nt < p.n_tiles) {
-                const uint32_t i0 = nt * T, i1 = min(p.n, i0 + T) - 1;
-                const uint4 d0 = __ldg((const uint4*)p.desc + i0), d1 = __ldg((const uint4*)p.desc + i1);
-                const uint32_t plo = d0.x & ~15u;
-                const uint32_t phi = (((d1.x + (d1.y & 0xFFFFu) + (d1.y >> 16) + 3u) & ~3u) + d1.z + 15u) & ~15u;
-                if (phi > plo && phi - plo <= 2u * p.in_cap)
-                    asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(p.arena + plo), "r"(phi - plo) : "memory");
-            }
-#endif
-        }
-#if defined(GOFR_PREFETCH_NEXT)
-        {   // next tile's descriptors and trace ids: one lane per 128-byte line
-            const uint32_t ni = (tile + gridDim.x) * T + tid;
-            if (ni < p.n && (lane & 7u) == 0) {
-                asm volatile("prefetch.global.L2 [%0];" ::"l"((const uint4*)p.desc + ni));
-                asm volatile("prefetch.global.L2 [%0];" ::"l"((const uint4*)p.ids + ni));
-            }
-        }
-#endif
+        if (tid == 0) stage_start(&sh.bar, in_stage, p.arena, cta_range(sh.warp_lo, sh.warp_hi, 0u, sh.in_lo, sh.in_hi), p.in_cap);
         __syncthreads();
-        const uint32_t in_lo = sh.in_lo, in_hi = sh.in_hi;
-        const bool in_staged = in_hi > in_lo && in_hi - in_lo <= p.in_cap;
-        const uint8_t* abase = p.arena;
-        if (in_staged) {
-            mbar_wait(&sh.bar, parity);
-            parity ^= 1;
-            abase = launder_after_sync((const uint8_t*)in_stage) - in_lo;  // abase + arena_off lands in the staged copy
-        }
+        const ByteRange in{sh.in_lo, sh.in_hi};
+        const bool in_staged = stageable(in, p.in_cap);
+        const uint8_t* abase = stage_wait(&sh.bar, parity, in_stage, p.arena, in, p.in_cap);  // abase + arena_off: the request
 
         // ---- stage 1: route ----
         ReqCtx c;
@@ -214,13 +168,7 @@ __device__ __forceinline__ void serve_body(const ServeParams& p) {
                 __syncthreads();
                 if (warp == 0) {
                     const uint32_t v = hist[lane];
-                    uint32_t incl = v;
-#pragma unroll
-                    for (int o = 1; o < 32; o <<= 1) {
-                        const uint32_t u = __shfl_up_sync(0xFFFFFFFFu, incl, o);
-                        if (lane >= (uint32_t)o) incl += u;
-                    }
-                    hist[lane] = incl - v;
+                    hist[lane] = warp_inclusive_sum(v, lane) - v;
                 }
                 __syncthreads();
                 const uint32_t pos = hist[cls] + rank;
@@ -261,43 +209,16 @@ __device__ __forceinline__ void serve_body(const ServeParams& p) {
             continue;
         }
         if (valid) size_routed(tv, br, c);
-        // ---- block scan of response sizes ----
-        uint32_t incl = c.total_len;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            uint32_t v = __shfl_up_sync(0xFFFFFFFFu, incl, o);
-            if (lane >= (uint32_t)o) incl += v;
-        }
-        if (lane == 31) sh.warp_sum[warp] = incl;
-        __syncthreads();
-        uint32_t warp_excl = 0, tile_total = 0;
-#pragma unroll
-        for (int w = 0; w < NW; w++) {
-            uint32_t s = sh.warp_sum[w];
-            if ((uint32_t)w < warp) warp_excl += s;
-            tile_total += s;
-        }
-        const uint32_t excl = warp_excl + incl - c.total_len;
-
-        // ---- chain tiles (warp 0) ----
-        if (warp == 0) {
-            unsigned long long base = (p.debug_flags & 1u) ? (unsigned long long)tile * tile_total
-                                                           : lookback(p.tile_state, p.epoch, tile, tile_total, lane);
-            if (lane == 0) sh.tile_base = base;
-        }
-        __syncthreads();
-        // host-batch path: the chunk starts at the same offset mod 16 as its destination in the caller's buffer
-        const unsigned long long tile_base = sh.tile_base + chain0;
-        const bool fits = tile_base + tile_total <= p.out_cap && tile_base + tile_total <= 0xFFFFFFFFull;
-        if (!fits && tid == 0) atomicExch(p.overflow, 1u);
+        // ---- place the tile: block scan of response sizes, chained by the look-back; on the host-batch path (chain0) the
+        // chunk starts at the same offset mod 16 as its destination in the caller's buffer ----
+        const TilePlace t = place_tile(p, tile, c.total_len, sh.warp_sum, sh.tile_base, p.debug_flags & 1u, chain0);
         if (valid) {
-            p.out_off[i] = (uint32_t)(tile_base + excl);
+            put_offsets(p.out_off, i, p.n, t, c.total_len);
             p.meta[i] = request_status(tv, c) | (c.route << 16);
-            if (i == p.n - 1) p.out_off[p.n] = (uint32_t)(tile_base + excl + c.total_len);
         }
 
         // ---- stage 3: emit straight to HBM in 16-byte chunks ----
-        if (fits && valid && c.total_len) emit_request(tv, br, c, p.out + tile_base + excl, &sh.ring[tid]);
+        if (t.fits && valid && c.total_len) emit_request(tv, br, c, p.out + t.base + t.excl, &sh.ring[tid]);
         // the next iteration's first __syncthreads orders this tile's shared-memory reads before any overwrite
     }
     if (SLOTS) {
