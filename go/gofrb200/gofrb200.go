@@ -405,6 +405,27 @@ func (e *Engine) ProtoDecodeNestedExDevice(msgs []ProtoNMsg, fields []ProtoNFiel
 		"gofr_proto_decode_nested_ex_device")
 }
 
+// ProtoDecodeNestedDeferredDevice is the second pass after ProtoDecodeNestedExDevice
+// (gofr_proto_decode_nested_deferred_device): the frames whose status in dMetaIn is 6 (GOFR_GRPC_DEFER) are decoded
+// again with map fields of up to 4096 entries; every other frame gets an empty row and keeps its status.  Same
+// description, frames and offsets as the first call; dMeta may be dMetaIn.  Row i comes from this call's dRows when
+// dMetaIn[i] was 6 and dMeta[i] is 0 (GOFR_GRPC_OK), else from the first call's.
+func (e *Engine) ProtoDecodeNestedDeferredDevice(msgs []ProtoNMsg, fields []ProtoNField, root uint32, presence []uint8, dIn, dInOff unsafe.Pointer,
+	n int, dMetaIn, dRows unsafe.Pointer, rowsCap uint64, dRowOff, dMeta unsafe.Pointer, stream unsafe.Pointer) error {
+	if len(msgs) == 0 || len(fields) == 0 {
+		return errors.New("gofrb200: empty message description")
+	}
+	pp, err := presenceArg(presence, fields)
+	if err != nil {
+		return err
+	}
+	return check(C.gofr_proto_decode_nested_deferred_device(e.e, (*C.gofr_proto_nmsg)(unsafe.Pointer(&msgs[0])), C.uint32_t(len(msgs)),
+		(*C.gofr_proto_nfield)(unsafe.Pointer(&fields[0])), C.uint32_t(len(fields)), C.uint32_t(root), pp, (*C.uint8_t)(dIn),
+		(*C.uint32_t)(dInOff), C.uint32_t(n), (*C.uint32_t)(dMetaIn), (*C.uint8_t)(dRows), C.uint64_t(rowsCap), (*C.uint32_t)(dRowOff),
+		(*C.uint32_t)(dMeta), stream),
+		"gofr_proto_decode_nested_deferred_device")
+}
+
 // ProtoNestedDescribeEx validates a description with presence bytes without a GPU (gofr_proto_nested_describe_ex): nil
 // when the encode and decode calls would accept it.
 func ProtoNestedDescribeEx(msgs []ProtoNMsg, fields []ProtoNField, root uint32, presence []uint8) error {

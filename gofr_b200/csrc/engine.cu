@@ -63,6 +63,7 @@ __global__ void proto_encode_nested_maps_kernel(const GrpcParams p, const PbnDes
 __global__ void proto_decode_nested_maps_kernel(const GrpcParams p, const PbnDesc D);  // same for descriptions with maps
 __global__ void proto_encode_nested_presence_kernel(const GrpcParams p, const PbnDesc D);  // proto_nested_presence_kernel.cu:
 __global__ void proto_decode_nested_presence_kernel(const GrpcParams p, const PbnDesc D);  // with explicit presence (and maps)
+__global__ void proto_decode_nested_deferred_kernel(const GrpcParams p, const uint32_t* meta_in, const PbnDesc D);  // proto_nested_deferred_kernel.cu
 __global__ void reqlog_kernel(const LogParams p);                // reqlog_kernel.cu
 __global__ void http_parse_kernel(const HttpParams p);           // http_kernel.cu
 __global__ void route_kernel(const RouteParams p);               // route_kernel.cu
@@ -73,7 +74,7 @@ namespace {
 
 enum Kern {
     K_SERVE, K_SERVE_VALUES, K_SLOTS, K_SLOTS_WIDE, K_SLOTS_VALUES, K_HELLO, K_PROTO_ENC, K_PROTO_DEC, K_PBN_ENC, K_PBN_DEC,
-    K_PBN_ENC_MAPS, K_PBN_DEC_MAPS, K_PBN_ENC_PRES, K_PBN_DEC_PRES, K_REQLOG, K_HTTP, K_ROUTE, K_BIND, K_COUNT
+    K_PBN_ENC_MAPS, K_PBN_DEC_MAPS, K_PBN_ENC_PRES, K_PBN_DEC_PRES, K_PBN_DEC_DEFERRED, K_REQLOG, K_HTTP, K_ROUTE, K_BIND, K_COUNT
 };
 struct KernelRec {
     const void* fn;
@@ -95,6 +96,7 @@ const KernelRec kKernels[K_COUNT] = {
     {(const void*)proto_decode_nested_maps_kernel, "proto", kServeThreads},
     {(const void*)proto_encode_nested_presence_kernel, "proto", kServeThreads},
     {(const void*)proto_decode_nested_presence_kernel, "proto", kServeThreads},
+    {(const void*)proto_decode_nested_deferred_kernel, "proto", kServeThreads},
     {(const void*)reqlog_kernel, "request-log", kServeThreads},
     {(const void*)http_parse_kernel, "http", kServeThreads},
     {(const void*)route_kernel, "route", kRouteThreads},
@@ -525,23 +527,32 @@ static int grow_bind_scratch(gofr_engine* e, uint32_t n) {
 // The launch of the frame kernels (Hello, proto3 encode / decode, flat and nested, the request log): one thread per record,
 // tiles of kServeThreads chained by the look-back over the engine's resident scratch.  The caller has validated its own
 // arguments and filled the input fields of `p`; `extra` are the kernel's parameters after it (schema or descriptor).
+// launch_frames_smem: the same with `smem` bytes of dynamic shared memory per CTA, the resident grid asked for that size.
 template <class Params, class... Extra>
-static int launch_frames(gofr_engine* e, Kern k, Params p, uint32_t n, uint8_t* d_out, uint64_t out_cap, uint32_t* d_out_off,
-                         void* stream, const Extra&... extra) {
+static int launch_frames_smem(gofr_engine* e, Kern k, uint32_t smem, Params p, uint32_t n, uint8_t* d_out, uint64_t out_cap,
+                              uint32_t* d_out_off, void* stream, const Extra&... extra) {
     std::lock_guard<std::mutex> g(e->mu);
     CUDA_TRY(cudaSetDevice(e->device));
     cudaStream_t st = (cudaStream_t)stream;
     if (n == 0) { if (d_out_off) CUDA_TRY(cudaMemsetAsync(d_out_off, 0, 4, st)); return GOFR_OK; }
     const uint32_t tiles = (n + kServeThreads - 1) / kServeThreads;
     { int rc = grow_state(e->state, tiles); if (rc) return rc; }
-    const int resident = resident_grid(e, k);
+    int resident = 0;
+    if (!smem) resident = resident_grid(e, k);
+    else if ((resident = std::max(0, blocks_per_sm(k, e->device, smem)) * e->sm_count) <= 0)
+        set_last_error("%s kernel cannot be resident with %u bytes of shared memory", kKernels[k].what, smem);
     if (!resident) return GOFR_ERR_CUDA;
     p.n = n; p.n_tiles = tiles;
     { int rc = next_epoch(e, &p.epoch); if (rc) return rc; }
     p.out = d_out; p.out_cap = out_cap; p.out_off = d_out_off;
     p.tile_state = e->state.words; p.overflow = e->d_flag;
     const int grid = (int)std::min<uint32_t>((uint32_t)std::max(1, resident / engines_on_device(e->device)), tiles);
-    return launch(e, k, grid, 0, st, p, extra...);
+    return launch(e, k, grid, smem, st, p, extra...);
+}
+template <class Params, class... Extra>
+static int launch_frames(gofr_engine* e, Kern k, Params p, uint32_t n, uint8_t* d_out, uint64_t out_cap, uint32_t* d_out_off,
+                         void* stream, const Extra&... extra) {
+    return launch_frames_smem(e, k, 0, p, n, d_out, out_cap, d_out_off, stream, extra...);
 }
 
 // The schema index of a Bind target, or an error: not part of the engine's table, or not a struct Bind takes.
@@ -1274,6 +1285,31 @@ int gofr_proto_decode_nested_ex_device(gofr_engine* e, const gofr_proto_nmsg* ms
                                        uint32_t* d_meta, void* stream) {
     return proto_nested_run(e, msgs, n_msgs, fields, n_fields, root, presence, d_in, d_in_off, n, d_rows, rows_cap, d_row_off, d_meta,
                             stream, true);
+}
+
+// Map fields on the deepest path from message type m: how many sorted entry lists the second pass keeps at once
+static uint32_t pbn_map_levels(const PbnDesc& D, uint32_t m) {
+    uint32_t most = 0;
+    for (uint32_t k = 0; k < D.count[m]; k++) {
+        const PbnField& F = D.f[D.first[m] + k];
+        if (F.msg != 0xFF) most = std::max(most, ((F.flags & PBN_MAP) ? 1u : 0u) + pbn_map_levels(D, F.msg));
+    }
+    return most;
+}
+
+int gofr_proto_decode_nested_deferred_device(gofr_engine* e, const gofr_proto_nmsg* msgs, uint32_t n_msgs, const gofr_proto_nfield* fields,
+                                             uint32_t n_fields, uint32_t root, const uint8_t* presence, const uint8_t* d_in,
+                                             const uint32_t* d_in_off, uint32_t n, const uint32_t* d_meta_in, uint8_t* d_rows,
+                                             uint64_t rows_cap, uint32_t* d_row_off, uint32_t* d_meta, void* stream) {
+    if (!e || (n && (!d_in || !d_in_off || !d_meta_in || !d_rows || !d_row_off || !d_meta))) return GOFR_ERR_INVALID;
+    PbnDesc D;
+    { int rc = pbn_build(msgs, n_msgs, fields, n_fields, root, presence, &D); if (rc) return rc; }
+    const uint32_t levels = pbn_map_levels(D, D.root);  // (the depth limit keeps it at kPdnMaxMapLevels or below)
+    if (levels > kPdnMaxMapLevels) { set_last_error("map fields nest %u deep", levels); return GOFR_ERR_UNSUPPORTED; }
+    GrpcParams p;
+    memset(&p, 0, sizeof p);
+    p.in = d_in; p.in_off = d_in_off; p.meta = d_meta;
+    return launch_frames_smem(e, K_PBN_DEC_DEFERRED, pdn_sort_bytes(levels), p, n, d_rows, rows_cap, d_row_off, stream, d_meta_in, D);
 }
 
 // the descriptor gofr_proto_encode_nested_device would hand to its kernel (tests/emu drives the device code with it)

@@ -96,6 +96,12 @@ struct GrpcParams {
 // message field of its entry type; the decoder takes at most kPbnMaxMapEntries entries of one map field in one message
 // (selection of the canonical order is quadratic) and answers GOFR_GRPC_DEFER beyond that.
 constexpr int kPbnMaxMsgs = 8, kPbnMaxFields = 48, kPbnMaxDepth = 4, kPbnMaxMapEntries = 64;
+// The second pass (gofr_proto_decode_nested_deferred_device, proto_nested_deferred_kernel.cu) decodes the frames the first
+// pass deferred, one per CTA, with up to kPdnMaxSortedEntries entries of one map field in one message: each active map level
+// (at most kPdnMaxMapLevels under kPbnMaxDepth) has a sorted entry list of 16 bytes per entry in dynamic shared memory,
+// behind a head of kPdnSortHeadBytes.
+constexpr uint32_t kPdnMaxSortedEntries = 4096, kPdnMaxMapLevels = 2, kPdnSortHeadBytes = 144;
+constexpr uint32_t pdn_sort_bytes(uint32_t levels) { return kPdnSortHeadBytes + levels * kPdnMaxSortedEntries * 16u; }
 enum : uint8_t {
     PBN_REPEATED = 1u,  // a count word in the fixed part, the elements in the variable part (map fields too)
     PBN_MAP = 2u,       // a map field (GOFR_PB_MAP; always with PBN_REPEATED): entries in ascending key order

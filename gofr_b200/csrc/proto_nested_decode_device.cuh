@@ -15,7 +15,8 @@
 //     value message sent twice is merged -> DEFER as above); across entries a later equal key replaces the earlier entry.
 //     The row holds the map in the encoder's canonical form: keys ascending, each once.  The walks find it by SELECTION —
 //     per output slot, the smallest key above the previous one among all entries, the last entry carrying it — no scratch,
-//     quadratic, so more than kPbnMaxMapEntries entries of one map field in one message (duplicates counted) are DEFER;
+//     quadratic, so more than kPbnMaxMapEntries entries of one map field in one message (duplicates counted) are DEFER
+//     (the second pass, proto_nested_deferred_device.cuh, takes those frames with sorted lists instead: the MapStep policy);
 //   * explicit presence: an optional field is set iff it occurs (with its own wire type), the last occurrence winning; of a
 //     oneof group the member occurring last among all the group's members is the set one, with its last value.  A message
 //     member sent twice (even with another member between) is DEFER, by the rule for singular message fields above.
@@ -168,6 +169,32 @@ GOFR_HD bool pdn_map_next(const PbnDesc& D, const uint8_t* f, uint32_t lo, uint3
     return found;
 }
 
+// The map step of the field-order walk (pdn_walk's MapStep), a policy of static functions:
+//   begin(D, f, lo, hi, mt, q, E, level, it)  the number of distinct keys of map field q (entry type E) of the message
+//                                          [lo, hi) of type mt; `level` counts the maps active around it (0 outermost);
+//                                          *it is the walk's item, free to be used as scratch
+//   next(..., level, have, cursor, out)    the next entry in canonical order after the one *cursor stands for (the first
+//                                          when !have): its payload in out->poff / plen, *cursor moved on; false at the end
+//   store()                                whether this thread makes the emitting walk's stores
+//   kMaxEntries                            the most entries of one map field in one message it takes (more: DEFER)
+// PdnSelect is the selection above: no scratch, quadratic, one thread per frame.  (proto_nested_deferred_device.cuh has the
+// sorted-list policy, for one CTA per frame.)
+struct PdnSelect {
+    static constexpr uint32_t kMaxEntries = (uint32_t)kPbnMaxMapEntries;
+    static GOFR_HD uint32_t begin(const PbnDesc& D, const uint8_t* f, uint32_t lo, uint32_t hi, uint32_t mt, uint32_t q, uint32_t E, int,
+                                  PdnItem* it) {
+        uint32_t n = 0;
+        uint64_t key = 0;
+        while (pdn_map_next(D, f, lo, hi, mt, q, E, n != 0, &key, it)) n++;
+        return n;
+    }
+    static GOFR_HD bool next(const PbnDesc& D, const uint8_t* f, uint32_t lo, uint32_t hi, uint32_t mt, uint32_t q, uint32_t E, int,
+                             bool have, uint64_t* cursor, PdnItem* out) {
+        return pdn_map_next(D, f, lo, hi, mt, q, E, have, cursor, out);
+    }
+    static constexpr GOFR_HD bool store() { return true; }
+};
+
 // elements of a packed payload [lo, hi) of class cls: count them, or fail when the payload is not a whole number of elements
 GOFR_HD bool pdn_packed_count(const uint8_t* f, uint32_t lo, uint32_t hi, uint32_t cls, uint32_t* n) {
     const uint32_t wire = cls & PC_WIRE;
@@ -186,8 +213,9 @@ GOFR_HD bool pdn_packed_count(const uint8_t* f, uint32_t lo, uint32_t hi, uint32
 }
 
 // ---- walk 1: validate, in wire order ----
-// (MAPS == false: the instance for descriptions without map fields, as for the walks below)
-template <bool MAPS>
+// (MAPS == false: the instance for descriptions without map fields, as for the walks below.  MAXE: the most entries one map
+// field may have in one message, duplicates counted; more are DEFER)
+template <bool MAPS, uint32_t MAXE = (uint32_t)kPbnMaxMapEntries>
 GOFR_HD_NOINLINE uint32_t pdn_validate(const PbnDesc& D, const uint8_t* f, uint32_t lo, uint32_t hi) {
     struct Lv { uint32_t end; uint64_t seen; uint8_t mt; uint8_t gbase; } lv[kPbnMaxDepth + 1];
     uint32_t groups[kMaxGroupDepth];
@@ -224,7 +252,7 @@ GOFR_HD_NOINLINE uint32_t pdn_validate(const PbnDesc& D, const uint8_t* f, uint3
                 L.seen |= 1ull << q;
             } else if (MAPS && (F.flags & PBN_MAP) && !(L.seen >> q & 1u)) {  // first entry of a map field: count them all once
                 L.seen |= 1ull << q;
-                if (1u + pdn_count_after(D, f, i, L.end, L.mt, (uint32_t)q) > (uint32_t)kPbnMaxMapEntries) defer = true;
+                if (1u + pdn_count_after(D, f, i, L.end, L.mt, (uint32_t)q) > MAXE) defer = true;
             }
             if (depth > kPbnMaxDepth) return GOFR_GRPC_BAD_PROTO;  // cannot happen: the schema's depth was checked
             i = it.poff;  // descend: the payload is parsed as a message of type F.msg
@@ -243,13 +271,16 @@ GOFR_HD void pdn_st32(uint8_t* p, uint32_t v) { p[0] = (uint8_t)v; p[1] = (uint8
 
 // ---- walks 2 and 3: field order; EMIT stores into row[] ----
 // Returns the row's byte count before padding.  The frame has been validated: no check can fail here.  PRES == true (with
-// MAPS): the instance for descriptions with explicit-presence fields.
-template <bool EMIT, bool MAPS, bool PRES = false>
+// MAPS): the instance for descriptions with explicit-presence fields.  MapStep: how map entries are put in key order (see
+// PdnSelect); only the threads whose MapStep::store() holds make the emitting walk's stores.
+template <bool EMIT, bool MAPS, bool PRES = false, class MapStep = PdnSelect>
 GOFR_HD_NOINLINE uint32_t pdn_walk(const PbnDesc& D, const uint8_t* f, uint32_t lo, uint32_t hi, uint8_t* row) {
     // in_rep: 1 elements of a repeated message field in wire order (scan: where to look on), 2 / 3 entries of a map field in
-    // key order (3: keys[frame] = the key of the entry taken last)
+    // key order (3: keys[frame] = MapStep's cursor at the entry taken last)
     struct Fr { uint32_t lo, hi, fx, scan; uint8_t mt, fi, in_rep; } st[kPbnMaxDepth + 1];
     uint64_t keys[kPbnMaxDepth + 1];
+    const bool stores = EMIT && MapStep::store();  // the emitting walk, and this thread makes its stores
+    int maps = 0;  // map fields whose entries are being walked (the innermost one's level is maps - 1)
     int depth = 0;
     uint32_t vc = (uint32_t)D.fixed_words[D.root] * 4u;  // append position of the variable part
     st[0].lo = lo; st[0].hi = hi; st[0].fx = 0; st[0].scan = 0; st[0].mt = (uint8_t)D.root; st[0].fi = 0; st[0].in_rep = 0;
@@ -277,8 +308,9 @@ GOFR_HD_NOINLINE uint32_t pdn_walk(const PbnDesc& D, const uint8_t* f, uint32_t 
             bool more;
             if (!MAPS || fr.in_rep == 1) more = find(fr.mt, fr.fi - 1u, &fr.scan, fr.hi, &it);
             else {
-                more = pdn_map_next(D, f, fr.lo, fr.hi, fr.mt, fr.fi - 1u, F.msg, fr.in_rep == 3, &keys[depth - 1], &it);
+                more = MapStep::next(D, f, fr.lo, fr.hi, fr.mt, fr.fi - 1u, F.msg, maps - 1, fr.in_rep == 3, &keys[depth - 1], &it);
                 fr.in_rep = 3;
+                if (!more) maps--;
             }
             if (more) {
                 const uint32_t efx = vc;
@@ -315,15 +347,15 @@ GOFR_HD_NOINLINE uint32_t pdn_walk(const PbnDesc& D, const uint8_t* f, uint32_t 
                     if (o == (int)q) { set = true; it = x; }
                     else if (group && o >= 0 && ((uint32_t)fields[o].flags >> PBN_ONEOF_SHIFT) == group) set = false;
                 }
-                if (EMIT) pdn_st32(row + fxo, set ? 1u : 0u);
+                if (stores) pdn_st32(row + fxo, set ? 1u : 0u);
                 if (F.msg != 0xFF) {  // a oneof member of message type: its fixed part inline (zeros when unset)
                     if (set) {
                         Fr& ch = st[depth++];
                         ch.lo = it.poff; ch.hi = it.poff + it.plen; ch.fx = fxo + 4u; ch.scan = 0; ch.mt = F.msg; ch.fi = 0; ch.in_rep = 0;
-                    } else if (EMIT) for (uint32_t k = 0; k < (uint32_t)D.fixed_words[F.msg] * 4u; k++) row[fxo + 4u + k] = 0;
+                    } else if (stores) for (uint32_t k = 0; k < (uint32_t)D.fixed_words[F.msg] * 4u; k++) row[fxo + 4u + k] = 0;
                 } else if ((cls & PC_WIRE) == 2) {
                     const uint32_t plen = set ? it.plen : 0u;
-                    if (EMIT) {
+                    if (stores) {
                         pdn_st32(row + fxo + 4u, plen);
                         for (uint32_t k = 0; k < plen; k++) row[vc + k] = f[it.poff + k];
                     }
@@ -331,7 +363,7 @@ GOFR_HD_NOINLINE uint32_t pdn_walk(const PbnDesc& D, const uint8_t* f, uint32_t 
                 } else {
                     uint32_t w0 = 0, w1 = 0;
                     if (set) pdn_scalar_words(cls, it.wt, it.v, &w0, &w1);
-                    if (EMIT) { pdn_st32(row + fxo + 4u, w0); if (cls & PC_64) pdn_st32(row + fxo + 8u, w1); }
+                    if (stores) { pdn_st32(row + fxo + 4u, w0); if (cls & PC_64) pdn_st32(row + fxo + 8u, w1); }
                 }
                 continue;
             }
@@ -340,7 +372,7 @@ GOFR_HD_NOINLINE uint32_t pdn_walk(const PbnDesc& D, const uint8_t* f, uint32_t 
             if (F.msg != 0xFF) {  // singular message: presence word + its fixed part inline (zeros when absent)
                 // (a map value is always present: a missing one is an empty message)
                 const bool present = find(fr.mt, q, &i, fr.hi, &it);
-                if (EMIT) {
+                if (stores) {
                     pdn_st32(row + fxo, present || (MAPS && (F.flags & PBN_ENTRY)) ? 1u : 0u);
                     if (!present) for (uint32_t k = 0; k < (uint32_t)D.fixed_words[F.msg] * 4u; k++) row[fxo + 4u + k] = 0;
                 }
@@ -351,7 +383,7 @@ GOFR_HD_NOINLINE uint32_t pdn_walk(const PbnDesc& D, const uint8_t* f, uint32_t 
             } else if ((cls & PC_WIRE) == 2) {  // string / bytes: the last occurrence
                 uint32_t poff = 0, plen = 0;
                 while (find(fr.mt, q, &i, fr.hi, &it)) { poff = it.poff; plen = it.plen; }
-                if (EMIT) {
+                if (stores) {
                     pdn_st32(row + fxo, plen);
                     for (uint32_t k = 0; k < plen; k++) row[vc + k] = f[poff + k];
                 }
@@ -359,33 +391,31 @@ GOFR_HD_NOINLINE uint32_t pdn_walk(const PbnDesc& D, const uint8_t* f, uint32_t 
             } else {
                 uint32_t w0 = 0, w1 = 0;
                 while (find(fr.mt, q, &i, fr.hi, &it)) pdn_scalar_words(cls, it.wt, it.v, &w0, &w1);
-                if (EMIT) { pdn_st32(row + fxo, w0); if (cls & PC_64) pdn_st32(row + fxo + 4u, w1); }
+                if (stores) { pdn_st32(row + fxo, w0); if (cls & PC_64) pdn_st32(row + fxo + 4u, w1); }
             }
             continue;
         }
         // repeated: the count word, the elements appended
         if (MAPS && (F.flags & PBN_MAP)) {  // the distinct keys
-            uint32_t n = 0;
-            uint64_t key = 0;
-            while (pdn_map_next(D, f, fr.lo, fr.hi, fr.mt, q, F.msg, n != 0, &key, &it)) n++;
-            if (EMIT) pdn_st32(row + fxo, n);
-            if (n) fr.in_rep = 2;
+            const uint32_t n = MapStep::begin(D, f, fr.lo, fr.hi, fr.mt, q, F.msg, maps, &it);
+            if (stores) pdn_st32(row + fxo, n);
+            if (n) { fr.in_rep = 2; maps++; }
         } else if (F.msg != 0xFF) {
             uint32_t n = 0;
             while (find(fr.mt, q, &i, fr.hi, &it)) n++;
-            if (EMIT) pdn_st32(row + fxo, n);
+            if (stores) pdn_st32(row + fxo, n);
             if (n) { fr.in_rep = 1; fr.scan = fr.lo; }
         } else if ((cls & PC_WIRE) == 2) {
             uint32_t n = 0;
             while (find(fr.mt, q, &i, fr.hi, &it)) {
-                if (EMIT) {
+                if (stores) {
                     pdn_st32(row + vc, it.plen);
                     for (uint32_t k = 0; k < it.plen; k++) row[vc + 4u + k] = f[it.poff + k];
                 }
                 vc += 4u + it.plen;
                 n++;
             }
-            if (EMIT) pdn_st32(row + fxo, n);
+            if (stores) pdn_st32(row + fxo, n);
         } else {
             const uint32_t eb = (cls & PC_64) ? 8u : 4u, ewt = cls & PC_WIRE;
             uint32_t n = 0;
@@ -397,7 +427,7 @@ GOFR_HD_NOINLINE uint32_t pdn_walk(const PbnDesc& D, const uint8_t* f, uint32_t 
                         uint64_t v = 0;
                         if (ewt == 0) { j += (uint32_t)grpc_varint(f + j, end - j, &v); }
                         else { for (int b = (int)eb - 1; b >= 0; b--) v = v << 8 | f[j + (uint32_t)b]; j += eb; }
-                        if (EMIT) {
+                        if (stores) {
                             uint32_t w0, w1;
                             pdn_scalar_words(cls, ewt, v, &w0, &w1);
                             pdn_st32(row + vc, w0);
@@ -407,7 +437,7 @@ GOFR_HD_NOINLINE uint32_t pdn_walk(const PbnDesc& D, const uint8_t* f, uint32_t 
                         n++;
                     }
                 } else {
-                    if (EMIT) {
+                    if (stores) {
                         uint32_t w0, w1;
                         pdn_scalar_words(cls, it.wt, it.v, &w0, &w1);
                         pdn_st32(row + vc, w0);
@@ -417,7 +447,7 @@ GOFR_HD_NOINLINE uint32_t pdn_walk(const PbnDesc& D, const uint8_t* f, uint32_t 
                     n++;
                 }
             }
-            if (EMIT) pdn_st32(row + fxo, n);
+            if (stores) pdn_st32(row + fxo, n);
         }
     }
     return vc;
@@ -426,8 +456,9 @@ GOFR_HD_NOINLINE uint32_t pdn_walk(const PbnDesc& D, const uint8_t* f, uint32_t 
 // size pass of one frame.  The kernels instantiate it for MAPS == D.maps and PRES == D.presence (one kernel per choice,
 // picked on the host: the map-free kernel contains no map code, only the presence kernels presence code); pdn_decode_size
 // dispatches at run time.  Validation is the same for both values of PRES: a oneof member of message type is a singular
-// message field (sent twice: DEFER), the other members and optional fields are checked like any singular field.
-template <bool MAPS, bool PRES = false>
+// message field (sent twice: DEFER), the other members and optional fields are checked like any singular field.  MapStep:
+// the map step of the walks, whose entry limit validation applies.
+template <bool MAPS, bool PRES = false, class MapStep = PdnSelect>
 GOFR_HD PdnRow pdn_decode_size_as(const PbnDesc& D, const uint8_t* f, uint32_t fn) {
     PdnRow r = {GOFR_GRPC_OK, 0};
     if (fn < 5) { r.status = GOFR_GRPC_BAD_LENGTH; return r; }
@@ -435,18 +466,18 @@ GOFR_HD PdnRow pdn_decode_size_as(const PbnDesc& D, const uint8_t* f, uint32_t f
     if (f[0] != 0) { r.status = GOFR_GRPC_BAD_LENGTH; return r; }
     const uint32_t L = (uint32_t)f[1] << 24 | (uint32_t)f[2] << 16 | (uint32_t)f[3] << 8 | f[4];
     if (L != fn - 5) { r.status = GOFR_GRPC_BAD_LENGTH; return r; }
-    r.status = pdn_validate<MAPS>(D, f, 5, 5 + L);
+    r.status = pdn_validate<MAPS, MapStep::kMaxEntries>(D, f, 5, 5 + L);
     if (r.status != GOFR_GRPC_OK) return r;
-    r.out_len = (pdn_walk<false, MAPS, PRES>(D, f, 5, 5 + L, nullptr) + 3u) & ~3u;
+    r.out_len = (pdn_walk<false, MAPS, PRES, MapStep>(D, f, 5, 5 + L, nullptr) + 3u) & ~3u;
     return r;
 }
 
 // emit pass: the row at dst (4-byte aligned: every row is a multiple of 4 bytes long)
-template <bool MAPS, bool PRES = false>
+template <bool MAPS, bool PRES = false, class MapStep = PdnSelect>
 GOFR_HD void pdn_decode_emit_as(const PbnDesc& D, const uint8_t* f, uint32_t fn, const PdnRow r, uint8_t* dst) {
     if (!r.out_len) return;
-    uint32_t end = pdn_walk<true, MAPS, PRES>(D, f, 5, fn, dst);
-    for (; end < r.out_len; end++) dst[end] = 0;
+    uint32_t end = pdn_walk<true, MAPS, PRES, MapStep>(D, f, 5, fn, dst);
+    if (MapStep::store()) for (; end < r.out_len; end++) dst[end] = 0;
 }
 
 GOFR_HD PdnRow pdn_decode_size(const PbnDesc& D, const uint8_t* f, uint32_t fn) {

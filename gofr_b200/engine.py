@@ -41,6 +41,17 @@ class DeviceResponses:
         return out, off, meta
 
 
+def row_growth_bound(msgs, root: int):
+    """(per_byte, per_frame): no frame of b bytes of the message types msgs decodes to a row longer than per_byte * b +
+    per_frame.  Each element of a repeated field or map takes at least two bytes on the wire (tag, then a length or a
+    value) and brings its fixed part (a message or map entry: its type's fixed words, absent singular messages inline as
+    zeros) or at most 8 bytes; a packed element takes one byte and brings at most 8; string bytes are copied once.  Later
+    equal keys of a map and repeated singular fields only replace."""
+    fixed = [S._pb_fixed_bytes(msgs, m) for m in range(len(msgs))]
+    elem = [fixed[f.msg] for fields in msgs for f in fields if f.type == S.PB_MAP or (f.repeated and f.type == S.PB_MESSAGE)]
+    return max([8] + [(b + 1) // 2 for b in elem]), fixed[root] + 3
+
+
 class Engine:
     def __init__(self, table: Table, device: int = 0):
         L = _abi.lib()
@@ -195,6 +206,38 @@ class Engine:
                                                                  None if pr is None else pr.ctypes.data, d_in.data_ptr(), d_off.data_ptr(), n,
                                                                  rows.data_ptr(), cap, off.data_ptr(), meta.data_ptr(), st.cuda_stream),
                    "gofr_proto_decode_nested_ex_device")
+        return rows, off, meta[:n]
+
+    def proto_decode_nested_deferred_device(self, msgs, root: int, frames: np.ndarray, in_off: np.ndarray, meta_in, rows_cap: Optional[int] = None,
+                                            stream=None, meta_out=None):
+        """gofr_proto_decode_nested_deferred_device: the second pass after proto_decode_nested_device on the same frames.
+        meta_in: that call's status column (a contiguous int32 device tensor of n words).  Frames whose status is
+        GOFR_GRPC_DEFER are decoded again with map fields of up to 4096 entries; the others get an empty row and keep their
+        status.  Returns (rows uint8, row_off, meta) on the device; meta is the merged status column, written to meta_out
+        when given (meta_in itself is allowed).  Row i of this call replaces the first call's when meta_in[i] was DEFER and
+        meta[i] is OK.  The default capacity covers the longest rows the frames can decode to (row_growth_bound)."""
+        import torch
+        dev = torch.device("cuda", self.device)
+        st = stream if stream is not None else torch.cuda.current_stream(self.device)
+        n = len(in_off) - 1
+        nm, nf, k = S.proto_nested_tables(msgs)
+        d_in = torch.from_numpy(np.concatenate([np.ascontiguousarray(frames), np.zeros(16, np.uint8)])).to(dev)
+        d_off = torch.from_numpy(in_off.view(np.int32)).to(dev)
+        if rows_cap is None:
+            per_byte, per_frame = row_growth_bound(msgs, root)
+            rows_cap = per_byte * int(in_off[-1] - in_off[0]) + per_frame * n
+        cap = max(int(rows_cap), 0)
+        rows = torch.empty(max(cap, 1), dtype=torch.uint8, device=dev)
+        off = torch.zeros(n + 1, dtype=torch.int32, device=dev)
+        meta = meta_out if meta_out is not None else torch.zeros(max(n, 1), dtype=torch.int32, device=dev)
+        for t in (meta_in, meta):
+            assert t.is_cuda and t.dtype == torch.int32 and t.is_contiguous() and t.numel() >= n
+        pr = S.proto_nested_presence(msgs)
+        _abi.check(_abi.lib().gofr_proto_decode_nested_deferred_device(self._e, nm.ctypes.data, len(msgs), nf.ctypes.data, k, root,
+                                                                       None if pr is None else pr.ctypes.data, d_in.data_ptr(), d_off.data_ptr(), n,
+                                                                       meta_in.data_ptr() if n else None, rows.data_ptr(), cap, off.data_ptr(),
+                                                                       meta.data_ptr(), st.cuda_stream),
+                   "gofr_proto_decode_nested_deferred_device")
         return rows, off, meta[:n]
 
     def proto_decode_device(self, fields, frames: np.ndarray, in_off: np.ndarray, rows_cap: Optional[int] = None, stream=None):

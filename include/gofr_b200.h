@@ -361,7 +361,9 @@ void gofr_free_pinned(void*);
 enum { GOFR_GRPC_OK = 0, GOFR_GRPC_COMPRESSED = 1, GOFR_GRPC_BAD_LENGTH = 2, GOFR_GRPC_BAD_PROTO = 3, GOFR_GRPC_BAD_UTF8 = 4,
        GOFR_GRPC_BAD_ROW = 5,
        GOFR_GRPC_DEFER = 6 /* gofr_proto_decode_nested_device: a valid frame outside its subset (a singular message field sent
-                              more than once, which protobuf-go merges): decode it on the host */ };
+                              more than once, which protobuf-go merges; a map field with more than 64 entries).  Pass the
+                              batch through gofr_proto_decode_nested_deferred_device, which decodes maps of up to 4096
+                              entries; what is still DEFER after it, decode on the host */ };
 int gofr_grpc_hello_device(gofr_engine*, const uint8_t* d_in, const uint32_t* d_in_off, uint32_t n, uint8_t* d_out,
                            uint64_t out_cap, uint32_t* d_out_off, uint32_t* d_meta, void* stream);
 
@@ -488,6 +490,27 @@ int gofr_proto_decode_nested_ex_device(gofr_engine*, const gofr_proto_nmsg* msgs
                                        uint32_t* d_meta, void* stream);
 int gofr_proto_nested_describe_ex(const gofr_proto_nmsg* msgs, uint32_t n_msgs, const gofr_proto_nfield* fields, uint32_t n_fields,
                                   uint32_t root, const uint8_t* presence, void* desc_out, uint32_t desc_cap);
+
+/* LARGE MAPS: the second pass of the nested decoder.  Same description (presence may be NULL), frames and offsets as the
+ * gofr_proto_decode_nested_ex_device call before it; d_meta_in is that call's status column.
+ *   selection   frame i is decoded again when d_meta_in[i] == GOFR_GRPC_DEFER.  Any other frame gets an empty row and
+ *               d_meta[i] = d_meta_in[i], so d_meta is the merged status column; d_meta may be d_meta_in itself.
+ *   decoding    from scratch, by the rules of the _ex call, with one difference: a map field may have up to 4096 entries on
+ *               the wire in one message (duplicates counted).  Still GOFR_GRPC_DEFER: a singular message (or a message
+ *               member of a oneof, or a map's value message inside one entry) sent twice, and more than 4096 entries.
+ *               Statuses and their precedence as for the _ex call.  Every selected frame is validated again, so a frame
+ *               selected by mistake costs time but gets the answer of the _ex call: the same row, byte for byte.
+ *   output      rows packed in frame order, d_row_off[n + 1], under the packed-output contract of the other frame calls
+ *               (whole tiles of 128 frames dropped past rows_cap, the overflow flag set, offsets and statuses written in
+ *               full).  d_in follows the rule for device input buffers at the top of this file.
+ * A description without map fields is taken; its selected frames stay DEFER.  Each CTA decodes one selected frame at a
+ * time, map entries put in key order by a sort in shared memory (64 KiB per level of maps inside map values).
+ * Combining the two calls: row i is the first call's row unless d_meta_in[i] == GOFR_GRPC_DEFER and d_meta[i] ==
+ * GOFR_GRPC_OK, in which case it is row i of this call; d_meta[i] is the final status either way. */
+int gofr_proto_decode_nested_deferred_device(gofr_engine*, const gofr_proto_nmsg* msgs, uint32_t n_msgs, const gofr_proto_nfield* fields,
+                                             uint32_t n_fields, uint32_t root, const uint8_t* presence, const uint8_t* d_in,
+                                             const uint32_t* d_in_off, uint32_t n, const uint32_t* d_meta_in, uint8_t* d_rows,
+                                             uint64_t rows_cap, uint32_t* d_row_off, uint32_t* d_meta, void* stream);
 
 /* Bind as a stage of the split API: Context.Bind(&v) for closures that stay on the host (pkg/gofr/context.go:52-54 ->
  * pkg/gofr/http/request.go:40-47 -> json.Unmarshal(body, &v), v a struct of a registered schema).  Body i is the data

@@ -6,12 +6,16 @@ Workloads (1 Mi messages each; 1024 distinct rows repeated):
    b  M { map<string, string> labels = 1; map<int64, Item> items = 2; } with 8 labels and 8 items
    c  the same type with 64 labels and 64 items (short strings, no tags): the decoder's worst case (selection over 64
       entries per map)
+   e  the type of b with 200..400 labels and 200..400 items per message (256 distinct rows, --n-large messages): beyond
+      the first pass's 64 entries, so its frames are DEFER and the second pass
+      (gofr_proto_decode_nested_deferred_device) decodes them
    d  Event { int64 id = 1; optional string note = 2; optional int64 parent = 3;
               oneof payload { Click click = 4; string text = 5; int64 code = 6; } repeated Tag tags = 7; }
       (field presence: the *_presence kernels through the _ex calls) with about half of the optional fields set and the
       oneof cases (none, click, text, code) spread evenly
 A workload named twice in --only (a,d,a,d) runs again on the same rows: alternate two workloads to see the noise.
-The decoder runs on the encoder's output.  CUDA events around `steps` launches after 3 warm-up launches; one JSON line per
+The decoder runs on the encoder's output, then the second pass on the decoder's status column ("deferred"; with
+--select-all every frame is selected, as if the first pass had deferred them all).  CUDA events around `steps` launches after 3 warm-up launches; one JSON line per
 workload and direction, after the card's name, power limit and max SM clock (nvidia-smi, read-only query)."""
 import argparse
 import json
@@ -98,6 +102,8 @@ def main():
     ap.add_argument("--n", type=int, default=1 << 20)
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--only", default="a,b,c")
+    ap.add_argument("--n-large", type=int, default=32768)
+    ap.add_argument("--select-all", action="store_true")
     ap.add_argument("--tag", default=os.environ.get("GOFR_LIB_PATH", "tree"))
     a = ap.parse_args()
     smi = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"], capture_output=True, text=True)
@@ -106,7 +112,8 @@ def main():
     work = {"a": (MSGS, lambda: [rand_value(rnd, MSGS, 0) for _ in range(1024)]),
             "b": (MAP_MSGS, lambda: [map_value(rnd, 8) for _ in range(1024)]),
             "c": (MAP_MSGS, lambda: [map_value(rnd, 64, compact=True) for _ in range(1024)]),
-            "d": (EVENT_MSGS, lambda: [event_value(rnd, i) for i in range(1024)])}
+            "d": (EVENT_MSGS, lambda: [event_value(rnd, i) for i in range(1024)]),
+            "e": (MAP_MSGS, lambda: [map_value(rnd, rnd.randint(200, 400)) for _ in range(256)])}
     cache = {}
     eng = Engine(Table(synth.config1_spec()), 0)
     L = _abi.lib()
@@ -114,9 +121,9 @@ def main():
     for w in a.only.split(","):
         msgs, gen = work[w]
         if w not in cache:
-            cache[w] = tiled_rows(msgs, gen(), a.n)
+            cache[w] = tiled_rows(msgs, gen(), a.n_large if w == "e" else a.n)
         rows, off = cache[w]
-        n = a.n
+        n = len(off) - 1
         nm, nf, k = S.proto_nested_tables(msgs)
         pr = S.proto_nested_presence(msgs)
         d_rows = torch.from_numpy(rows).cuda()
@@ -153,12 +160,27 @@ def main():
                                                          d_out_off.data_ptr(), n, d_back.data_ptr(), rows_cap, d_back_off.data_ptr(),
                                                          d_meta2.data_ptr(), st), "decode")
         t_dec = timed(dec, a.steps)
-        assert not d_meta2.any().item()
-        same = bool(torch.equal(d_back[:int(off[-1])], d_rows[:int(off[-1])]))   # decode(encode(rows)) == rows
-        for direction, t in (("encode", t_enc), ("decode", t_dec)):
+        large = w == "e"
+        assert bool((d_meta2 == 6).all().item()) if large else not d_meta2.any().item()
+        same = large or bool(torch.equal(d_back[:int(off[-1])], d_rows[:int(off[-1])]))   # decode(encode(rows)) == rows
+        # the second pass on the first pass's statuses (or every frame selected)
+        d_sel = torch.full_like(d_meta2, 6) if a.select_all else d_meta2.clone()
+        n_sel = int((d_sel == 6).sum().item())
+        d_meta3 = torch.zeros(n, dtype=torch.int32, device="cuda")
+
+        def dec2():
+            _abi.check(L.gofr_proto_decode_nested_deferred_device(eng._e, nm.ctypes.data, len(msgs), nf.ctypes.data, k, 0,
+                                                                  None if pr is None else pr.ctypes.data, d_out.data_ptr(),
+                                                                  d_out_off.data_ptr(), n, d_sel.data_ptr(), d_back.data_ptr(), rows_cap,
+                                                                  d_back_off.data_ptr(), d_meta3.data_ptr(), st), "deferred")
+        t_dec2 = timed(dec2, a.steps)
+        assert not d_meta3.any().item()
+        if n_sel == n:
+            same = same and bool(torch.equal(d_back[:int(off[-1])], d_rows[:int(off[-1])]))
+        for direction, t in (("encode", t_enc), ("decode", t_dec), ("deferred", t_dec2)):
             print(json.dumps({"workload": w, "dir": direction, "n": n, "ms": round(t, 4), "Mmsg_per_s": round(n / t / 1e3, 1),
                               "frame_GBps": round(out_bytes / t / 1e6, 1), "row_bytes": int(off[-1]), "frame_bytes": out_bytes,
-                              "round_trip_equal": same, "lib": a.tag}), flush=True)
+                              "round_trip_equal": same, "selected": n_sel if direction == "deferred" else None, "lib": a.tag}), flush=True)
         del d_rows, d_out, d_back
         torch.cuda.empty_cache()
     eng.close()
