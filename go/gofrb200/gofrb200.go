@@ -443,3 +443,88 @@ func ProtoNestedDescribeEx(msgs []ProtoNMsg, fields []ProtoNField, root uint32, 
 	}
 	return check(rc, "gofr_proto_nested_describe_ex")
 }
+
+// ProtoNestedBound returns (perByte, perRecord) such that no record of b bytes yields more than perByte*b + perRecord
+// output bytes (gofr_proto_nested_bound; no GPU): a row when decode is true, a whole frame when encoding.  Sum it over a
+// batch to size the out buffer of ProtoDecodeBatch / ProtoEncodeBatch.
+func ProtoNestedBound(msgs []ProtoNMsg, fields []ProtoNField, root uint32, presence []uint8, decode bool) (perByte, perRecord uint32, err error) {
+	if len(msgs) == 0 || len(fields) == 0 {
+		return 0, 0, errors.New("gofrb200: empty message description")
+	}
+	pp, err := presenceArg(presence, fields)
+	if err != nil {
+		return 0, 0, err
+	}
+	d := C.int(0)
+	if decode {
+		d = 1
+	}
+	var pb, pr C.uint32_t
+	err = check(C.gofr_proto_nested_bound((*C.gofr_proto_nmsg)(unsafe.Pointer(&msgs[0])), C.uint32_t(len(msgs)),
+		(*C.gofr_proto_nfield)(unsafe.Pointer(&fields[0])), C.uint32_t(len(fields)), C.uint32_t(root), pp, d, &pb, &pr),
+		"gofr_proto_nested_bound")
+	return uint32(pb), uint32(pr), err
+}
+
+// protoBatch runs gofr_proto_batch_decode / _encode on host buffers and waits for it: record i = data[off[i]:off[i+1]],
+// results into out (ideally from gofr_alloc_pinned), outOff (n+1) and meta (n).  Returns the bytes written.
+func (e *Engine) protoBatch(decode bool, msgs []ProtoNMsg, fields []ProtoNField, root uint32, presence []uint8, data []byte, off []uint32,
+	out []byte, outOff, meta []uint32) (int, error) {
+	if len(msgs) == 0 || len(fields) == 0 || len(off) == 0 {
+		return 0, errors.New("gofrb200: empty message description or offsets")
+	}
+	n := len(off) - 1
+	if n == 0 {
+		return 0, nil
+	}
+	if len(outOff) < n+1 || len(meta) < n || len(out) == 0 {
+		return 0, errors.New("gofrb200: out/outOff/meta too small")
+	}
+	pp, err := presenceArg(presence, fields)
+	if err != nil {
+		return 0, err
+	}
+	var in C.gofr_proto_batch
+	if len(data) > 0 {
+		in.data = (*C.uint8_t)(unsafe.Pointer(&data[0]))
+	}
+	in.data_bytes = C.uint64_t(len(data))
+	in.off = (*C.uint32_t)(unsafe.Pointer(&off[0]))
+	in.n = C.uint32_t(n)
+	var o C.gofr_resp_batch
+	o.out = (*C.uint8_t)(unsafe.Pointer(&out[0]))
+	o.out_cap = C.uint64_t(len(out))
+	o.out_off = (*C.uint32_t)(unsafe.Pointer(&outOff[0]))
+	o.meta = (*C.uint32_t)(unsafe.Pointer(&meta[0]))
+	var ticket C.gofr_ticket
+	cm, cf := (*C.gofr_proto_nmsg)(unsafe.Pointer(&msgs[0])), (*C.gofr_proto_nfield)(unsafe.Pointer(&fields[0]))
+	if decode {
+		err = check(C.gofr_proto_batch_decode(e.e, cm, C.uint32_t(len(msgs)), cf, C.uint32_t(len(fields)), C.uint32_t(root), pp, &in, &o, &ticket),
+			"gofr_proto_batch_decode")
+	} else {
+		err = check(C.gofr_proto_batch_encode(e.e, cm, C.uint32_t(len(msgs)), cf, C.uint32_t(len(fields)), C.uint32_t(root), pp, &in, &o, &ticket),
+			"gofr_proto_batch_encode")
+	}
+	if err != nil {
+		return 0, err
+	}
+	if err := check(C.gofr_batch_wait(e.e, ticket), "gofr_batch_wait"); err != nil {
+		return 0, err
+	}
+	return int(o.out_bytes), nil
+}
+
+// ProtoDecodeBatch decodes a batch of request frames held in host memory (gofr_proto_batch_decode): both decode passes,
+// merged, so row i = out[outOff[i]:outOff[i+1]] and meta[i] are final.  meta[i] == 6 (GOFR_GRPC_DEFER): hand frame i
+// to proto.Unmarshal on the host; its row is empty, as is a failed frame's.
+func (e *Engine) ProtoDecodeBatch(msgs []ProtoNMsg, fields []ProtoNField, root uint32, presence []uint8, frames []byte, off []uint32,
+	out []byte, outOff, meta []uint32) (int, error) {
+	return e.protoBatch(true, msgs, fields, root, presence, frames, off, out, outOff, meta)
+}
+
+// ProtoEncodeBatch marshals a batch of response rows held in host memory into gRPC frames (gofr_proto_batch_encode): what
+// ProtoEncodeNestedExDevice gives, status for status.  Row offsets are multiples of 4.
+func (e *Engine) ProtoEncodeBatch(msgs []ProtoNMsg, fields []ProtoNField, root uint32, presence []uint8, rows []byte, off []uint32,
+	out []byte, outOff, meta []uint32) (int, error) {
+	return e.protoBatch(false, msgs, fields, root, presence, rows, off, out, outOff, meta)
+}

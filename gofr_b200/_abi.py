@@ -45,6 +45,10 @@ ERR_NAMES = {0: "OK", 1: "INVALID", 2: "UNSUPPORTED", 3: "NOMEM", 4: "CUDA", 5: 
              8: "NO_DEVICE"}
 
 
+class ProtoBatch(C.Structure):
+    _fields_ = [("data", C.c_void_p), ("data_bytes", C.c_uint64), ("off", C.c_void_p), ("n", C.c_uint32)]
+
+
 class ProtoField(C.Structure):
     _fields_ = [("number", C.c_uint32), ("type", C.c_uint32)]
 
@@ -107,6 +111,9 @@ def lib():
     L.gofr_proto_decode_nested_ex_device.argtypes = [vp, vp, u32, vp, u32, u32, vp, vp, vp, u32, vp, u64, vp, vp, vp]
     L.gofr_proto_encode_nested_ex_device.argtypes = [vp, vp, u32, vp, u32, u32, vp, vp, vp, u32, vp, u64, vp, vp, vp]
     L.gofr_proto_decode_nested_deferred_device.argtypes = [vp, vp, u32, vp, u32, u32, vp, vp, vp, u32, vp, vp, u64, vp, vp, vp]
+    L.gofr_proto_batch_decode.argtypes = [vp, vp, u32, vp, u32, u32, vp, C.POINTER(ProtoBatch), C.POINTER(RespBatch), C.POINTER(u64)]
+    L.gofr_proto_batch_encode.argtypes = [vp, vp, u32, vp, u32, u32, vp, C.POINTER(ProtoBatch), C.POINTER(RespBatch), C.POINTER(u64)]
+    L.gofr_proto_nested_bound.argtypes = [vp, u32, vp, u32, u32, vp, i32, C.POINTER(u32), C.POINTER(u32)]
     L.gofr_table_slot_ctas.argtypes = [vp, C.POINTER(C.c_int)]
     L.gofr_engine_slot_ctas.argtypes = [vp, C.c_int, C.POINTER(C.c_int)]
     L.gofr_engine_geometry.argtypes = [vp, C.POINTER(u32), C.POINTER(u32), C.POINTER(u32), C.POINTER(u32)]
@@ -152,7 +159,7 @@ DECLARED_SYMBOLS = [
     "gofr_table_route_count", "gofr_table_max_response_bytes", "gofr_engine_create", "gofr_engine_destroy",
     "gofr_serve_device", "gofr_serve_device_slots", "gofr_batch_submit", "gofr_batch_wait", "gofr_batch_submit_slots", "gofr_engine_set_chunk", "gofr_engine_set_tile",
     "gofr_engine_set_timing", "gofr_engine_overflowed", "gofr_engine_geometry", "gofr_engine_slot_ctas", "gofr_table_slot_ctas", "gofr_alloc_pinned", "gofr_free_pinned", "gofr_bind_host_thread", "gofr_bind_device", "gofr_batch_bind",
-    "gofr_grpc_hello_device", "gofr_requestlog_device", "gofr_http_parse_device", "gofr_batch_route", "gofr_proto_encode_device", "gofr_proto_decode_device", "gofr_proto_encode_nested_device", "gofr_proto_decode_nested_device", "gofr_proto_nested_describe", "gofr_proto_encode_nested_ex_device", "gofr_proto_decode_nested_ex_device", "gofr_proto_nested_describe_ex", "gofr_proto_decode_nested_deferred_device", "gofr_table_response_bound", "gofr_frontend_create", "gofr_frontend_destroy", "gofr_frontend_set_clock",
+    "gofr_grpc_hello_device", "gofr_requestlog_device", "gofr_http_parse_device", "gofr_batch_route", "gofr_proto_encode_device", "gofr_proto_decode_device", "gofr_proto_encode_nested_device", "gofr_proto_decode_nested_device", "gofr_proto_nested_describe", "gofr_proto_encode_nested_ex_device", "gofr_proto_decode_nested_ex_device", "gofr_proto_nested_describe_ex", "gofr_proto_decode_nested_deferred_device", "gofr_proto_batch_decode", "gofr_proto_batch_encode", "gofr_proto_nested_bound", "gofr_table_response_bound", "gofr_frontend_create", "gofr_frontend_destroy", "gofr_frontend_set_clock",
     "gofr_frontend_stats", "gofr_frontend_serve", "gofr_route_device", "gofr_engine_launch_count", "gofr_engine_kernel_time_ms", "gofr_last_error",
     "gofr_abi_version", "gofr_format_http_date",
 ]

@@ -68,13 +68,15 @@ __global__ void reqlog_kernel(const LogParams p);                // reqlog_kerne
 __global__ void http_parse_kernel(const HttpParams p);           // http_kernel.cu
 __global__ void route_kernel(const RouteParams p);               // route_kernel.cu
 __global__ void bind_kernel(const BindParams p);                 // bind_kernel.cu
+__global__ void chunk_pack_kernel(const PackParams p);           // pack_kernel.cu
 }  // namespace gofr
 
 namespace {
 
 enum Kern {
     K_SERVE, K_SERVE_VALUES, K_SLOTS, K_SLOTS_WIDE, K_SLOTS_VALUES, K_HELLO, K_PROTO_ENC, K_PROTO_DEC, K_PBN_ENC, K_PBN_DEC,
-    K_PBN_ENC_MAPS, K_PBN_DEC_MAPS, K_PBN_ENC_PRES, K_PBN_DEC_PRES, K_PBN_DEC_DEFERRED, K_REQLOG, K_HTTP, K_ROUTE, K_BIND, K_COUNT
+    K_PBN_ENC_MAPS, K_PBN_DEC_MAPS, K_PBN_ENC_PRES, K_PBN_DEC_PRES, K_PBN_DEC_DEFERRED, K_REQLOG, K_HTTP, K_ROUTE, K_BIND, K_PACK,
+    K_COUNT
 };
 struct KernelRec {
     const void* fn;
@@ -101,6 +103,7 @@ const KernelRec kKernels[K_COUNT] = {
     {(const void*)http_parse_kernel, "http", kServeThreads},
     {(const void*)route_kernel, "route", kRouteThreads},
     {(const void*)bind_kernel, "bind", kBindThreads},
+    {(const void*)chunk_pack_kernel, "pack", kServeThreads},
 };
 
 constexpr int kSlots = 3;  // pipeline depth of the host-batch path
@@ -122,10 +125,16 @@ struct Slot {
     uint32_t* d_flag = nullptr; uint32_t* d_bind = nullptr;
     TileState state;  // packed layout only
     size_t cap_n = 0, cap_arena = 0, cap_out = 0;
+    // proto host path (grown on demand): the input offsets, the codec kernels' own outputs and offset columns (decode: [0]
+    // the first pass, [1] the second) and the first pass's statuses
+    uint32_t* d_in_off = nullptr; uint32_t* d_meta1 = nullptr;
+    uint8_t* d_codec[2] = {nullptr, nullptr}; uint32_t* d_codec_off[2] = {nullptr, nullptr};
+    size_t cap_codec_n = 0, cap_codec[2] = {0, 0};
     // pinned staging for the tiny per-chunk read-backs
     uint32_t* h_tail = nullptr;  // [0] = chunk total bytes, [1] = overflow flag
 
     int reserve(gofr_engine* e, uint32_t requests, size_t arena_bytes, size_t out_bytes);
+    int reserve_codec(uint32_t records, size_t a_bytes, size_t b_bytes);
 };
 
 }  // namespace
@@ -369,6 +378,8 @@ void gofr_engine_destroy(gofr_engine* e) {
         if (s.ev_egress) cudaEventDestroy(s.ev_egress);
         cudaFree(s.d_desc); cudaFree(s.d_ids); cudaFree(s.d_arena); cudaFree(s.d_out); cudaFree(s.d_off); cudaFree(s.d_meta);
         cudaFree(s.state.words); cudaFree(s.d_flag); cudaFree(s.d_bind);
+        cudaFree(s.d_in_off); cudaFree(s.d_meta1);
+        for (int k = 0; k < 2; k++) { cudaFree(s.d_codec[k]); cudaFree(s.d_codec_off[k]); }
         if (s.h_tail) cudaFreeHost(s.h_tail);
     }
     for (auto& ev : e->timing) { cudaEventDestroy(ev.first); cudaEventDestroy(ev.second); }
@@ -524,19 +535,17 @@ static int grow_bind_scratch(gofr_engine* e, uint32_t n) {
     return GOFR_OK;
 }
 
-// The launch of the frame kernels (Hello, proto3 encode / decode, flat and nested, the request log): one thread per record,
-// tiles of kServeThreads chained by the look-back over the engine's resident scratch.  The caller has validated its own
-// arguments and filled the input fields of `p`; `extra` are the kernel's parameters after it (schema or descriptor).
-// launch_frames_smem: the same with `smem` bytes of dynamic shared memory per CTA, the resident grid asked for that size.
+// The launch of the frame kernels (Hello, proto3 encode / decode, flat and nested, the request log, the chunk pack kernel):
+// one thread per record, tiles of kServeThreads chained by the look-back over the scratch `state`, overflow reported in
+// `d_flag`, `smem` bytes of dynamic shared memory per CTA and the resident grid asked for that size.  Called with the
+// engine lock held.  The caller has validated its own arguments and filled the input fields of `p`; `extra` are the
+// kernel's parameters after it (schema or descriptor).
 template <class Params, class... Extra>
-static int launch_frames_smem(gofr_engine* e, Kern k, uint32_t smem, Params p, uint32_t n, uint8_t* d_out, uint64_t out_cap,
-                              uint32_t* d_out_off, void* stream, const Extra&... extra) {
-    std::lock_guard<std::mutex> g(e->mu);
-    CUDA_TRY(cudaSetDevice(e->device));
-    cudaStream_t st = (cudaStream_t)stream;
+static int launch_frames_locked(gofr_engine* e, Kern k, uint32_t smem, Params p, uint32_t n, uint8_t* d_out, uint64_t out_cap,
+                                uint32_t* d_out_off, TileState& state, uint32_t* d_flag, cudaStream_t st, const Extra&... extra) {
     if (n == 0) { if (d_out_off) CUDA_TRY(cudaMemsetAsync(d_out_off, 0, 4, st)); return GOFR_OK; }
     const uint32_t tiles = (n + kServeThreads - 1) / kServeThreads;
-    { int rc = grow_state(e->state, tiles); if (rc) return rc; }
+    { int rc = grow_state(state, tiles); if (rc) return rc; }
     int resident = 0;
     if (!smem) resident = resident_grid(e, k);
     else if ((resident = std::max(0, blocks_per_sm(k, e->device, smem)) * e->sm_count) <= 0)
@@ -545,9 +554,17 @@ static int launch_frames_smem(gofr_engine* e, Kern k, uint32_t smem, Params p, u
     p.n = n; p.n_tiles = tiles;
     { int rc = next_epoch(e, &p.epoch); if (rc) return rc; }
     p.out = d_out; p.out_cap = out_cap; p.out_off = d_out_off;
-    p.tile_state = e->state.words; p.overflow = e->d_flag;
+    p.tile_state = state.words; p.overflow = d_flag;
     const int grid = (int)std::min<uint32_t>((uint32_t)std::max(1, resident / engines_on_device(e->device)), tiles);
     return launch(e, k, grid, smem, st, p, extra...);
+}
+// The device calls: the engine's resident scratch, on the caller's stream
+template <class Params, class... Extra>
+static int launch_frames_smem(gofr_engine* e, Kern k, uint32_t smem, Params p, uint32_t n, uint8_t* d_out, uint64_t out_cap,
+                              uint32_t* d_out_off, void* stream, const Extra&... extra) {
+    std::lock_guard<std::mutex> g(e->mu);
+    CUDA_TRY(cudaSetDevice(e->device));
+    return launch_frames_locked(e, k, smem, p, n, d_out, out_cap, d_out_off, e->state, e->d_flag, (cudaStream_t)stream, extra...);
 }
 template <class Params, class... Extra>
 static int launch_frames(gofr_engine* e, Kern k, Params p, uint32_t n, uint8_t* d_out, uint64_t out_cap, uint32_t* d_out_off,
@@ -701,7 +718,7 @@ static int grow(void** p, size_t* cap, size_t need, size_t slack) {
 // (include/gofr_b200.h states the same for device-resident callers), so a staging arena is never sized to the byte.
 static constexpr size_t kArenaSlack = 16;
 
-// A chunk = contiguous request range [lo, hi) and the arena byte range it covers.
+// A chunk = contiguous record range [lo, hi), the input (arena) byte range it covers and a bound on its device output.
 struct ChunkPlan { uint32_t lo, hi; uint32_t arena_lo, arena_hi; uint64_t out_bound; };
 
 // The arena byte range [*alo, *ahi) (16-byte granular) that requests [lo, hi) reference: their whole requests, or their paths
@@ -791,6 +808,26 @@ int Slot::reserve(gofr_engine* e, uint32_t requests, size_t arena_bytes, size_t 
     return rc ? rc : grow((void**)&d_out, &cap_out, out_bytes, 256);
 }
 
+// The proto host path's buffers for a chunk of `records` records whose codec outputs take a_bytes and b_bytes.  Only the
+// chunk's own kernels use them, and a buffer that grows is freed by cudaFree, which waits for the device.  The copy of the
+// pack kernel reads a source word past its last byte: grow's slack covers it.
+int Slot::reserve_codec(uint32_t records, size_t a_bytes, size_t b_bytes) {
+    if (records > cap_codec_n) {
+        cudaFree(d_in_off); cudaFree(d_meta1); cudaFree(d_codec_off[0]); cudaFree(d_codec_off[1]);
+        d_in_off = d_meta1 = d_codec_off[0] = d_codec_off[1] = nullptr;
+        cap_codec_n = 0;
+        const size_t c = (size_t)records + records / 4 + 256;
+        if (cudaMalloc(&d_in_off, (c + 1) * 4) != cudaSuccess || cudaMalloc(&d_meta1, c * 4) != cudaSuccess ||
+            cudaMalloc(&d_codec_off[0], (c + 1) * 4) != cudaSuccess || cudaMalloc(&d_codec_off[1], (c + 1) * 4) != cudaSuccess) {
+            set_last_error("cudaMalloc failed for a %zu-record chunk", c);
+            return GOFR_ERR_NOMEM;
+        }
+        cap_codec_n = c;
+    }
+    int rc = grow((void**)&d_codec[0], &cap_codec[0], a_bytes, 256);
+    return rc ? rc : grow((void**)&d_codec[1], &cap_codec[1], b_bytes, 256);
+}
+
 // Waits for everything enqueued on the egress stream.  A large batch takes milliseconds: the thread sleeps on a
 // blocking-sync event.  A small one (the per-request front-end's batches) is back in tens of microseconds: spinning is
 // the faster wake-up there.
@@ -826,9 +863,24 @@ int gofr_batch_submit(gofr_engine* e, const gofr_req_batch* in, gofr_resp_batch*
     return rc;
 }
 
-static int batch_submit_locked(gofr_engine* e, const gofr_req_batch* in, gofr_resp_batch* out, gofr_ticket* ticket) {
+// The chunk pipeline of the host-batch calls with a packed output (gofr_batch_submit, gofr_proto_batch_decode / _encode).
+// What differs between them:
+//   plan     the chunk that starts at record lo: its end, its input byte range and a bound on its device output; the
+//            records' input is validated here, chunk by chunk (an up-front scan of 1 Mi records is milliseconds of pure
+//            latency), so an error can surface with earlier chunks in flight (the caller drains the streams);
+//   upload   the H2D copies of the chunk's input into the slot (and any buffers of the caller's own it needs);
+//   compute  the kernels that leave the chunk's packed output in the slot's d_out / d_off / d_meta, placed at
+//            *chain_pos & 15 when chain_pos is given (the serve kernel's convention), at 0 otherwise.
+// The pipeline reserves the slot, then runs upload, compute, advance and egress (pinned caller buffers) or an exact-size
+// copy (pageable ones).
+struct ChunkSteps {
+    std::function<int(uint32_t lo, ChunkPlan* c)> plan;
+    std::function<int(Slot& s, const ChunkPlan& c, cudaStream_t st)> upload;
+    std::function<int(Slot& s, const ChunkPlan& c, cudaStream_t st, const unsigned long long* chain_pos)> compute;
+};
+
+static int run_chunks(gofr_engine* e, uint32_t n, const ChunkSteps& steps, gofr_resp_batch* out, gofr_ticket* ticket) {
     out->out_bytes = 0;
-    const uint32_t n = in->n;
     int final_rc = GOFR_OK;
     if (n == 0) {  // nothing to do; the caller may have passed no buffers at all
         if (out->out_off) out->out_off[0] = 0;
@@ -836,46 +888,29 @@ static int batch_submit_locked(gofr_engine* e, const gofr_req_batch* in, gofr_re
         e->done_tickets.emplace_back(*ticket, GOFR_OK);
         return GOFR_OK;
     }
-
-    // Chunks are contiguous request ranges; a chunk's arena range is the min/max over its descriptors.  The scan is done
-    // lazily, right before a chunk is enqueued, so it overlaps with the GPU work of the chunks already in flight
-    // (scanning all descriptors up front costs milliseconds of pure latency on a 1 Mi-request batch).
-    const size_t nchunks_total = n ? (n + e->chunk - 1) / e->chunk : 0;
-    std::vector<ChunkPlan> plan(nchunks_total);
-    std::vector<char> planned(nchunks_total, 0);
-    auto plan_chunk = [&](size_t ci) -> int {
-        if (planned[ci]) return GOFR_OK;
-        uint32_t lo = (uint32_t)(ci * e->chunk), hi = std::min<uint32_t>(n, lo + e->chunk);
-        uint32_t alo = 0, ahi = 0;
-        uint64_t sizes[2];
-        int prc = chunk_arena_range(in, lo, hi, false, &alo, &ahi, sizes);
-        if (prc) return prc;
-        plan[ci] = {lo, hi, alo, ahi, chunk_out_bound(e, hi - lo, sizes)};
-        planned[ci] = 1;
-        return GOFR_OK;
-    };
     // ---- streaming path: caller buffers are pinned → egress is device driven, the host never blocks mid-batch ----
     auto device_visible = [](const void* p) {
         cudaPointerAttributes a;
         if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); return false; }
         return a.type == cudaMemoryTypeHost || a.type == cudaMemoryTypeManaged;
     };
-    if (n && device_visible(out->out) && device_visible(out->out_off) && device_visible(out->meta)) {
+    if (device_visible(out->out) && device_visible(out->out_off) && device_visible(out->meta)) {
         // growing buffers frees memory: make sure nothing from an earlier batch is still using them
         CUDA_TRY(cudaMemsetAsync(e->d_chain, 0, 8, e->st_compute));
         e->h_status[0] = 0; e->h_status[1] = 0;
-        for (size_t ci = 0; ci < plan.size(); ci++) {
+        size_t ci = 0;
+        for (uint32_t lo = 0; lo < n; ci++) {
             Slot& s = e->slots[ci % kSlots];
-            { int prc = plan_chunk(ci); if (prc) return prc; }
-            const ChunkPlan& c = plan[ci];
+            ChunkPlan c;
+            { int prc = steps.plan(lo, &c); if (prc) return prc; }
+            lo = c.hi;
             uint32_t cn = c.hi - c.lo;
             int rc = s.reserve(e, cn, (size_t)c.arena_hi - c.arena_lo, c.out_bound);
-            if (!rc) rc = upload_chunk(in, c.lo, cn, c.arena_lo, c.arena_hi, s.d_desc, s.d_ids, s.d_arena, e->st_h2d);
+            if (!rc) rc = steps.upload(s, c, e->st_h2d);
             if (rc) return rc;
             CUDA_TRY(cudaEventRecord(s.ev_h2d, e->st_h2d));
             CUDA_TRY(cudaStreamWaitEvent(e->st_compute, s.ev_h2d, 0));
-            rc = launch_serve(e, s.d_desc, s.d_ids, s.d_arena - c.arena_lo, cn, in->date, s.d_out, s.cap_out, s.d_off, s.d_meta,
-                              &s.state, s.d_flag, s.d_bind, e->st_compute, e->d_chain);
+            rc = steps.compute(s, c, e->st_compute, e->d_chain);
             if (rc) return rc;
             if (launch_advance(e->d_chain, s.d_off, cn, s.d_flag, e->d_info + (ci % kSlots), out->out_cap, e->st_compute) != 0) {
                 set_last_error("advance kernel launch failed"); return GOFR_ERR_CUDA;
@@ -904,23 +939,22 @@ static int batch_submit_locked(gofr_engine* e, const gofr_req_batch* in, gofr_re
 
     // ---- pageable caller buffers: 3-slot software pipeline, each chunk's exact size copied back once it is known ----
     size_t issued = 0, finished = 0;
+    uint32_t next_lo = 0;
+    ChunkPlan inflight[kSlots];
     uint64_t write_pos = 0;
-    const size_t nchunks = plan.size();
     // issue order == completion order == chunk order; out offsets are rebased on the host as chunks complete
-    while (finished < nchunks) {
+    while (next_lo < n || finished < issued) {
         // keep up to kSlots chunks in flight
-        while (issued < nchunks && issued - finished < (size_t)kSlots) {
+        while (next_lo < n && issued - finished < (size_t)kSlots) {
             int si = (int)(issued % kSlots);
             Slot& s = e->slots[si];
-            { int prc = plan_chunk(issued); if (prc) return prc; }
-            const ChunkPlan& c = plan[issued];
+            ChunkPlan& c = inflight[si];
+            { int prc = steps.plan(next_lo, &c); if (prc) return prc; }
+            next_lo = c.hi;
             uint32_t cn = c.hi - c.lo;
             int rc = s.reserve(e, cn, (size_t)c.arena_hi - c.arena_lo, c.out_bound);
-            if (!rc) rc = upload_chunk(in, c.lo, cn, c.arena_lo, c.arena_hi, s.d_desc, s.d_ids, s.d_arena, s.stream);
-            if (rc) return rc;
-            // descriptors keep absolute arena offsets: pass a rebased arena pointer
-            rc = launch_serve(e, s.d_desc, s.d_ids, s.d_arena - c.arena_lo, cn, in->date, s.d_out, s.cap_out, s.d_off, s.d_meta,
-                              &s.state, s.d_flag, s.d_bind, s.stream);
+            if (!rc) rc = steps.upload(s, c, s.stream);
+            if (!rc) rc = steps.compute(s, c, s.stream, nullptr);
             if (rc) return rc;
             CUDA_TRY(cudaMemcpyAsync(out->out_off + c.lo, s.d_off, (size_t)cn * 4, cudaMemcpyDeviceToHost, s.stream));
             CUDA_TRY(cudaMemcpyAsync(out->meta + c.lo, s.d_meta, (size_t)cn * 4, cudaMemcpyDeviceToHost, s.stream));
@@ -932,7 +966,7 @@ static int batch_submit_locked(gofr_engine* e, const gofr_req_batch* in, gofr_re
         // retire the oldest chunk: learn its size, then pull exactly that many bytes
         int si = (int)(finished % kSlots);
         Slot& s = e->slots[si];
-        const ChunkPlan& c = plan[finished];
+        const ChunkPlan& c = inflight[si];
         CUDA_TRY(cudaEventSynchronize(s.done));
         uint32_t total = s.h_tail[0];
         if (s.h_tail[1]) { CUDA_TRY(cudaMemsetAsync(s.d_flag, 0, 4, s.stream)); final_rc = GOFR_ERR_CAPACITY; set_last_error("device output buffer too small for chunk %zu", finished); total = 0; }
@@ -949,6 +983,29 @@ static int batch_submit_locked(gofr_engine* e, const gofr_req_batch* in, gofr_re
     *ticket = e->next_ticket++;
     e->done_tickets.emplace_back(*ticket, final_rc);
     return GOFR_OK;
+}
+
+static int batch_submit_locked(gofr_engine* e, const gofr_req_batch* in, gofr_resp_batch* out, gofr_ticket* ticket) {
+    ChunkSteps steps;
+    // Chunks are contiguous request ranges of e->chunk requests; a chunk's arena range is the min/max over its descriptors.
+    steps.plan = [&](uint32_t lo, ChunkPlan* c) -> int {
+        const uint32_t hi = std::min<uint32_t>(in->n, lo + e->chunk);
+        uint32_t alo = 0, ahi = 0;
+        uint64_t sizes[2];
+        int prc = chunk_arena_range(in, lo, hi, false, &alo, &ahi, sizes);
+        if (prc) return prc;
+        *c = {lo, hi, alo, ahi, chunk_out_bound(e, hi - lo, sizes)};
+        return GOFR_OK;
+    };
+    steps.upload = [&](Slot& s, const ChunkPlan& c, cudaStream_t st) -> int {
+        return upload_chunk(in, c.lo, c.hi - c.lo, c.arena_lo, c.arena_hi, s.d_desc, s.d_ids, s.d_arena, st);
+    };
+    // descriptors keep absolute arena offsets: pass a rebased arena pointer
+    steps.compute = [&](Slot& s, const ChunkPlan& c, cudaStream_t st, const unsigned long long* chain_pos) -> int {
+        return launch_serve(e, s.d_desc, s.d_ids, s.d_arena - c.arena_lo, c.hi - c.lo, in->date, s.d_out, s.cap_out, s.d_off,
+                            s.d_meta, &s.state, s.d_flag, s.d_bind, st, chain_pos);
+    };
+    return run_chunks(e, in->n, steps, out, ticket);
 }
 
 int gofr_batch_submit_slots(gofr_engine* e, const gofr_req_batch* in, gofr_slot_batch* out, gofr_ticket* ticket) {
@@ -1242,6 +1299,12 @@ static int pbn_build(const gofr_proto_nmsg* msgs, uint32_t n_msgs, const gofr_pr
     return GOFR_OK;
 }
 
+// The nested codec's instance for a description: presence-free, no presence code; map-free too, no map code
+static Kern pbn_kernel(const PbnDesc& D, bool decode) {
+    return D.presence ? (decode ? K_PBN_DEC_PRES : K_PBN_ENC_PRES)
+         : D.maps     ? (decode ? K_PBN_DEC_MAPS : K_PBN_ENC_MAPS) : (decode ? K_PBN_DEC : K_PBN_ENC);
+}
+
 static int proto_nested_run(gofr_engine* e, const gofr_proto_nmsg* msgs, uint32_t n_msgs, const gofr_proto_nfield* fields, uint32_t n_fields,
                             uint32_t root, const uint8_t* presence, const uint8_t* d_in, const uint32_t* d_in_off, uint32_t n,
                             uint8_t* d_out, uint64_t out_cap, uint32_t* d_out_off, uint32_t* d_meta, void* stream, bool decode) {
@@ -1251,10 +1314,7 @@ static int proto_nested_run(gofr_engine* e, const gofr_proto_nmsg* msgs, uint32_
     GrpcParams p;
     memset(&p, 0, sizeof p);
     p.in = d_in; p.in_off = d_in_off; p.meta = d_meta;
-    // presence-free: no presence code; map-free too: no map code
-    const Kern k = D.presence ? (decode ? K_PBN_DEC_PRES : K_PBN_ENC_PRES)
-                 : D.maps     ? (decode ? K_PBN_DEC_MAPS : K_PBN_ENC_MAPS) : (decode ? K_PBN_DEC : K_PBN_ENC);
-    return launch_frames(e, k, p, n, d_out, out_cap, d_out_off, stream, D);
+    return launch_frames(e, pbn_kernel(D, decode), p, n, d_out, out_cap, d_out_off, stream, D);
 }
 
 int gofr_proto_encode_nested_device(gofr_engine* e, const gofr_proto_nmsg* msgs, uint32_t n_msgs, const gofr_proto_nfield* fields,
@@ -1310,6 +1370,162 @@ int gofr_proto_decode_nested_deferred_device(gofr_engine* e, const gofr_proto_nm
     memset(&p, 0, sizeof p);
     p.in = d_in; p.in_off = d_in_off; p.meta = d_meta;
     return launch_frames_smem(e, K_PBN_DEC_DEFERRED, pdn_sort_bytes(levels), p, n, d_rows, rows_cap, d_row_off, stream, d_meta_in, D);
+}
+
+// gofr_proto_nested_bound: (per_byte, per_record) such that no record of b bytes yields more than per_byte * b + per_record
+// output bytes, from the description alone.
+// Decode (frame → row; the rule of engine.row_growth_bound in Python, which calls this): every element of a repeated field
+// or map takes at least two bytes on the wire (a tag, then a length or a value) and brings its fixed part (a message or map
+// entry: its type's fixed words, absent singular messages inline as zeros) or at most 8 bytes; a packed element takes one
+// byte and brings at most 8; string bytes are copied once; later equal keys of a map and repeated singular fields only
+// replace.  So per_byte = max(8, ceil(fixed bytes of an element type / 2)), and an empty frame still gives the root's
+// fixed part, rounded up to a word: per_record = its fixed bytes + 3.
+// Encode (row → frame with its 5-byte prefix): each byte written is charged to a row word or to a string byte.  String and
+// bytes contents are copied once (1 per byte).  A word is charged what its own field writes:
+//   scalar                  tag (tl bytes) + at most 10 (a varint: a negative int32 takes ten), 8 or 4;
+//   string / bytes length,  tag + a length of at most 5 (a frame's length fits 32 bits);
+//   singular message presence word, packed repeated count word, repeated string element: the same, tl + 5;
+//   packed element          at most 10 (a 64-bit kind spreads its ten over two words);
+//   presence word of an explicit-presence scalar: nothing (its value word pays);
+// plus, on the first word of an element of a repeated message field or a map (an entry: key, then value, both written
+// even at zero values, each a scalar or message of its own above), that element's tag and length, tl + 5.  An element's
+// fixed part is at least one word, because pbn_build refuses a message type with no fields, and a word is the first word
+// of at most one element.  So with W the most a word pays for itself and H the largest element header, per_byte =
+// ceil((W + H) / 4) (at least 1, for string bytes), per_record = 5.  tl is the varint length of the field's tag: 5 bytes
+// for field numbers from 2^25 on.
+static void pbn_bound(const PbnDesc& D, bool decode, uint32_t* per_byte, uint32_t* per_record) {
+    auto vlen = [](uint32_t v) { return v < 0x80u ? 1u : v < 0x4000u ? 2u : v < 0x200000u ? 3u : v < 0x10000000u ? 4u : 5u; };
+    uint32_t elem = 0, W = 0, H = 0;
+    for (uint32_t m = 0; m < D.n_msgs; m++) {
+        for (uint32_t k = 0; k < D.count[m]; k++) {
+            const PbnField& F = D.f[D.first[m] + k];
+            const bool sub = F.msg != 0xFF, rep = (F.flags & PBN_REPEATED) != 0;
+            const uint32_t tl = vlen(F.tag), wire = F.cls & PC_WIRE;
+            const uint32_t scalar = wire == 0 ? 10u : wire == 1 ? 8u : wire == 5 ? 4u : 5u;  // what follows the tag
+            if (rep && sub) {  // a repeated message field or a map
+                elem = std::max<uint32_t>(elem, 4u * D.fixed_words[F.msg]);
+                H = std::max(H, tl + 5u);
+            } else if (rep) {
+                W = std::max(W, std::max(tl + 5u, wire == 2 ? tl + 5u : scalar));
+            } else {
+                W = std::max(W, sub ? tl + 5u : tl + scalar);
+            }
+        }
+    }
+    if (decode) {
+        *per_byte = std::max(8u, (elem + 1u) / 2u);
+        *per_record = 4u * D.fixed_words[D.root] + 3u;
+    } else {
+        *per_byte = std::max(1u, (W + H + 3u) / 4u);
+        *per_record = 5u;
+    }
+}
+
+int gofr_proto_nested_bound(const gofr_proto_nmsg* msgs, uint32_t n_msgs, const gofr_proto_nfield* fields, uint32_t n_fields,
+                            uint32_t root, const uint8_t* presence, int decode, uint32_t* per_byte, uint32_t* per_record) {
+    if (!per_byte || !per_record) return GOFR_ERR_INVALID;
+    PbnDesc D;
+    { int rc = pbn_build(msgs, n_msgs, fields, n_fields, root, presence, &D); if (rc) return rc; }
+    pbn_bound(D, decode != 0, per_byte, per_record);
+    return GOFR_OK;
+}
+
+// Device bytes a proto chunk's output bound may take per slot: a chunk holds at most e->chunk records and, unless it is a
+// single record, records whose bounds sum to no more than this.  Decode grows by up to a few hundred bytes per wire byte
+// in the worst case, so a record count alone could ask for gigabytes.  Each slot holds three buffers of this size when
+// decoding (the two passes' rows and the packed chunk).
+static constexpr uint64_t kProtoChunkBudget = 256ull << 20;
+
+// The host-buffer calls of the nested codec: the chunk pipeline (run_chunks) with the codec kernels, then the pack kernel.
+static int proto_batch_locked(gofr_engine* e, const PbnDesc& D, bool decode, const gofr_proto_batch* in, gofr_resp_batch* out,
+                              gofr_ticket* ticket) {
+    uint32_t per_byte = 0, per_record = 0;
+    pbn_bound(D, decode, &per_byte, &per_record);
+    const uint32_t levels = pbn_map_levels(D, D.root);
+    if (decode && levels > kPdnMaxMapLevels) { set_last_error("map fields nest %u deep", levels); return GOFR_ERR_UNSUPPORTED; }
+    const uint32_t* off = in->off;
+    ChunkSteps steps;
+    // Offsets come from the caller: validated here in 64 bits, a chunk at a time (non-decreasing, within data_bytes, rows
+    // on 4-byte boundaries).  The chunk's output bound includes the 16 bytes the packed output may start into its buffer.
+    steps.plan = [&](uint32_t lo, ChunkPlan* c) -> int {
+        const uint32_t lim = lo + std::min<uint32_t>(e->chunk, in->n - lo);
+        const uint64_t start = off[lo];
+        if (start > in->data_bytes || (!decode && (start & 3u))) {
+            set_last_error("record %u starts at %llu: outside the data or not a multiple of 4", lo, (unsigned long long)start);
+            return GOFR_ERR_INVALID;
+        }
+        uint64_t bound = 0;
+        uint32_t hi = lo;
+        for (; hi < lim; hi++) {
+            const uint64_t a = off[hi], b = off[hi + 1];
+            if (b < a || b > in->data_bytes || (!decode && (b & 3u))) {
+                set_last_error("record %u: offsets %llu .. %llu are decreasing, outside the data or not multiples of 4", hi,
+                               (unsigned long long)a, (unsigned long long)b);
+                return GOFR_ERR_INVALID;
+            }
+            const uint64_t rb = (uint64_t)per_byte * (b - a) + per_record;
+            if (hi > lo && bound + rb > kProtoChunkBudget) break;
+            bound += rb;
+        }
+        // a single record with a larger bound gets a chunk of its own; no output offset passes 32 bits, so neither does a
+        // buffer (a record that would is reported as a capacity error by the kernels)
+        *c = {lo, hi, (uint32_t)(start & ~15ull), off[hi], std::min<uint64_t>(bound, 1ull << 32) + 16};
+        return GOFR_OK;
+    };
+    steps.upload = [&](Slot& s, const ChunkPlan& c, cudaStream_t st) -> int {
+        const uint32_t cn = c.hi - c.lo;
+        { int rc = s.reserve_codec(cn, c.out_bound, decode ? c.out_bound : 0); if (rc) return rc; }
+        CUDA_TRY(cudaMemcpyAsync(s.d_in_off, off + c.lo, (size_t)(cn + 1) * 4, cudaMemcpyHostToDevice, st));
+        if (c.arena_hi > c.arena_lo) CUDA_TRY(cudaMemcpyAsync(s.d_arena, in->data + c.arena_lo, c.arena_hi - c.arena_lo, cudaMemcpyHostToDevice, st));
+        return GOFR_OK;
+    };
+    // records keep their absolute offsets: pass a rebased input pointer.  The codec kernels write from byte 0 of their own
+    // buffers (16 bytes short of their end: the pack kernel's copy reads a word past a record's last byte).
+    steps.compute = [&](Slot& s, const ChunkPlan& c, cudaStream_t st, const unsigned long long* chain_pos) -> int {
+        const uint32_t cn = c.hi - c.lo;
+        GrpcParams p;
+        memset(&p, 0, sizeof p);
+        p.in = s.d_arena - c.arena_lo; p.in_off = s.d_in_off;
+        PackParams q;
+        memset(&q, 0, sizeof q);
+        q.a = s.d_codec[0]; q.a_off = s.d_codec_off[0]; q.a_cap = s.cap_codec[0] - 16; q.chain_pos = chain_pos;
+        p.meta = decode ? s.d_meta1 : s.d_meta;
+        int rc = launch_frames_locked(e, pbn_kernel(D, decode), 0, p, cn, s.d_codec[0], q.a_cap, s.d_codec_off[0], s.state, s.d_flag, st, D);
+        if (!rc && decode) {  // the second pass over the first one's statuses, always: with nothing DEFER it is a scan
+            p.meta = s.d_meta;
+            q.b = s.d_codec[1]; q.b_off = s.d_codec_off[1]; q.b_cap = s.cap_codec[1] - 16; q.sel = s.d_meta1;
+            rc = launch_frames_locked(e, K_PBN_DEC_DEFERRED, pdn_sort_bytes(levels), p, cn, s.d_codec[1], q.b_cap, s.d_codec_off[1],
+                                      s.state, s.d_flag, st, (const uint32_t*)s.d_meta1, D);
+        }
+        if (!rc) rc = launch_frames_locked(e, K_PACK, 0, q, cn, s.d_out, s.cap_out, s.d_off, s.state, s.d_flag, st);
+        return rc;
+    };
+    return run_chunks(e, in->n, steps, out, ticket);
+}
+
+static int proto_batch(gofr_engine* e, const gofr_proto_nmsg* msgs, uint32_t n_msgs, const gofr_proto_nfield* fields, uint32_t n_fields,
+                       uint32_t root, const uint8_t* presence, const gofr_proto_batch* in, gofr_resp_batch* out, gofr_ticket* ticket,
+                       bool decode) {
+    if (!e || !in || !out || !ticket) return GOFR_ERR_INVALID;
+    if (in->n && (!in->off || !out->out || !out->out_off || !out->meta)) return GOFR_ERR_INVALID;
+    if (in->data_bytes && !in->data) return GOFR_ERR_INVALID;
+    PbnDesc D;
+    { int rc = pbn_build(msgs, n_msgs, fields, n_fields, root, presence, &D); if (rc) return rc; }
+    std::lock_guard<std::mutex> g(e->mu);
+    CUDA_TRY(cudaSetDevice(e->device));
+    const int rc = proto_batch_locked(e, D, decode, in, out, ticket);
+    if (rc != GOFR_OK) drain_streams(e);  // see gofr_batch_submit
+    return rc;
+}
+
+int gofr_proto_batch_decode(gofr_engine* e, const gofr_proto_nmsg* msgs, uint32_t n_msgs, const gofr_proto_nfield* fields, uint32_t n_fields,
+                            uint32_t root, const uint8_t* presence, const gofr_proto_batch* in, gofr_resp_batch* out, gofr_ticket* ticket) {
+    return proto_batch(e, msgs, n_msgs, fields, n_fields, root, presence, in, out, ticket, true);
+}
+
+int gofr_proto_batch_encode(gofr_engine* e, const gofr_proto_nmsg* msgs, uint32_t n_msgs, const gofr_proto_nfield* fields, uint32_t n_fields,
+                            uint32_t root, const uint8_t* presence, const gofr_proto_batch* in, gofr_resp_batch* out, gofr_ticket* ticket) {
+    return proto_batch(e, msgs, n_msgs, fields, n_fields, root, presence, in, out, ticket, false);
 }
 
 // the descriptor gofr_proto_encode_nested_device would hand to its kernel (tests/emu drives the device code with it)

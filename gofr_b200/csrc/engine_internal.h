@@ -89,6 +89,28 @@ struct GrpcParams {
     unsigned long long* tile_state;
     uint32_t* overflow;
 };
+// Launch parameters of the chunk pack kernel (pack_kernel.cu): the host-batch path of the proto calls packs each record's
+// bytes from the codec's output buffer (source A) or, where the selector column says so, from a second buffer (source B)
+// into the slot's output buffer, starting at *chain_pos & 15 as the serve kernel does.
+struct PackParams {
+    const uint8_t* a;        // source A: record i = a[a_off[i] .. a_off[i + 1]), a_cap bytes written at most
+    const uint32_t* a_off;
+    uint64_t a_cap;
+    const uint8_t* b;        // source B (null: none), the same; record i comes from it when sel[i] == GOFR_GRPC_DEFER
+    const uint32_t* b_off;
+    uint64_t b_cap;
+    const uint32_t* sel;
+    uint32_t n;
+    uint32_t n_tiles;
+    uint32_t epoch;
+    uint8_t* out;
+    uint64_t out_cap;
+    uint32_t* out_off;       // n + 1
+    unsigned long long* tile_state;
+    uint32_t* overflow;
+    const unsigned long long* chain_pos;  // pinned-buffer path: packed position of the batch so far (else null)
+};
+
 // message types of gofr_proto_encode_nested_device (kernel parameter, by value): up to 8 message types with 48 fields in
 // all; fields of a type are consecutive, in ascending field-number order.  Rows use the layout of the wider data model
 // (include/gofr_b200.h "Row format"): a singular message field is a presence word + the message's fixed part inline, a

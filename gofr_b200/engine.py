@@ -41,15 +41,23 @@ class DeviceResponses:
         return out, off, meta
 
 
+def nested_bound(msgs, root: int, decode: bool):
+    """gofr_proto_nested_bound: (per_byte, per_record) such that no record of b bytes of the message types msgs yields more
+    than per_byte * b + per_record bytes: a row when decoding, a frame with its 5-byte prefix when encoding.  The
+    derivation is at the C function."""
+    nm, nf, k = S.proto_nested_tables(msgs)
+    pr = S.proto_nested_presence(msgs)
+    pb, prec = C.c_uint32(), C.c_uint32()
+    _abi.check(_abi.lib().gofr_proto_nested_bound(nm.ctypes.data, len(msgs), nf.ctypes.data, k, root,
+                                                  None if pr is None else pr.ctypes.data, 1 if decode else 0,
+                                                  C.byref(pb), C.byref(prec)), "gofr_proto_nested_bound")
+    return pb.value, prec.value
+
+
 def row_growth_bound(msgs, root: int):
     """(per_byte, per_frame): no frame of b bytes of the message types msgs decodes to a row longer than per_byte * b +
-    per_frame.  Each element of a repeated field or map takes at least two bytes on the wire (tag, then a length or a
-    value) and brings its fixed part (a message or map entry: its type's fixed words, absent singular messages inline as
-    zeros) or at most 8 bytes; a packed element takes one byte and brings at most 8; string bytes are copied once.  Later
-    equal keys of a map and repeated singular fields only replace."""
-    fixed = [S._pb_fixed_bytes(msgs, m) for m in range(len(msgs))]
-    elem = [fixed[f.msg] for fields in msgs for f in fields if f.type == S.PB_MAP or (f.repeated and f.type == S.PB_MESSAGE)]
-    return max([8] + [(b + 1) // 2 for b in elem]), fixed[root] + 3
+    per_frame (nested_bound when decoding)."""
+    return nested_bound(msgs, root, True)
 
 
 class Engine:
@@ -239,6 +247,44 @@ class Engine:
                                                                        meta.data_ptr(), st.cuda_stream),
                    "gofr_proto_decode_nested_deferred_device")
         return rows, off, meta[:n]
+
+    # ---- the nested codec on host buffers (gofr_proto_batch_decode / _encode) ----
+    def _proto_batch(self, msgs, root: int, data: np.ndarray, off: np.ndarray, out_cap: Optional[int], pinned: bool, decode: bool):
+        n = len(off) - 1
+        data = np.ascontiguousarray(data, dtype=np.uint8)
+        off = np.ascontiguousarray(off, dtype=np.uint32)
+        if out_cap is None:
+            per_byte, per_record = nested_bound(msgs, root, decode)
+            out_cap = per_byte * int(off[-1] - off[0]) + per_record * n if n else 0
+        if pinned:
+            out, out_off, meta = pinned_array(out_cap), pinned_array(4 * (n + 1), np.uint32), pinned_array(4 * max(n, 1), np.uint32)
+        else:
+            out, out_off, meta = np.empty(max(out_cap, 1), np.uint8), np.zeros(n + 1, np.uint32), np.zeros(max(n, 1), np.uint32)
+        nm, nf, k = S.proto_nested_tables(msgs)
+        pr = S.proto_nested_presence(msgs)
+        L = _abi.lib()
+        pb = _abi.ProtoBatch(data=data.ctypes.data, data_bytes=data.size, off=off.ctypes.data, n=n)
+        ob = _abi.RespBatch(out=out.ctypes.data, out_cap=out_cap, out_off=out_off.ctypes.data, meta=meta.ctypes.data, out_bytes=0)
+        t = C.c_uint64()
+        fn = L.gofr_proto_batch_decode if decode else L.gofr_proto_batch_encode
+        name = "gofr_proto_batch_decode" if decode else "gofr_proto_batch_encode"
+        _abi.check(fn(self._e, nm.ctypes.data, len(msgs), nf.ctypes.data, k, root, None if pr is None else pr.ctypes.data,
+                      C.byref(pb), C.byref(ob), C.byref(t)), name)
+        _abi.check(L.gofr_batch_wait(self._e, t.value), "gofr_batch_wait")
+        return out[:int(ob.out_bytes)], out_off, meta[:n]
+
+    def proto_decode_batch(self, msgs, root: int, frames: np.ndarray, in_off: np.ndarray, out_cap: Optional[int] = None,
+                           pinned: bool = False):
+        """gofr_proto_batch_decode: frames in host memory → (rows uint8, row_off uint32[n + 1], meta uint32[n]), both decode
+        passes combined; a frame still GOFR_GRPC_DEFER, or failed, has an empty row.  out_cap defaults to the bound; pinned
+        puts the outputs in pinned memory (device-driven egress)."""
+        return self._proto_batch(msgs, root, frames, in_off, out_cap, pinned, True)
+
+    def proto_encode_batch(self, msgs, root: int, rows: np.ndarray, row_off: np.ndarray, out_cap: Optional[int] = None,
+                           pinned: bool = False):
+        """gofr_proto_batch_encode: rows (spec.pack_proto_nested_rows) in host memory → (frames uint8, out_off uint32[n + 1],
+        meta uint32[n]), what gofr_proto_encode_nested_ex_device gives."""
+        return self._proto_batch(msgs, root, rows, row_off, out_cap, pinned, False)
 
     def proto_decode_device(self, fields, frames: np.ndarray, in_off: np.ndarray, rows_cap: Optional[int] = None, stream=None):
         """gofr_proto_decode_device: packed gRPC frames → rows.  Returns (rows uint8, row_off, meta) on the device."""

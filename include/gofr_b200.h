@@ -512,6 +512,39 @@ int gofr_proto_decode_nested_deferred_device(gofr_engine*, const gofr_proto_nmsg
                                              const uint32_t* d_in_off, uint32_t n, const uint32_t* d_meta_in, uint8_t* d_rows,
                                              uint64_t rows_cap, uint32_t* d_row_off, uint32_t* d_meta, void* stream);
 
+/* HOST BUFFERS for the nested codec: what a gRPC server holds (request frames, its handlers' responses) goes in and comes
+ * back in host memory, through the chunk pipeline of gofr_batch_submit (three device slots, three streams).  Same
+ * description arguments as the _ex calls (presence may be NULL).
+ *   in     record i = data[off[i] .. off[i + 1]); off has n + 1 entries, non-decreasing, off[n] <= data_bytes; for encode
+ *          the records are rows (the layout above) and every offset is a multiple of 4.  Offsets are checked on the host a
+ *          chunk at a time: a bad batch returns GOFR_ERR_INVALID with nothing still writing into the caller's buffers.
+ *   out    a gofr_resp_batch, collected with gofr_batch_wait: records packed in order, out_off[n + 1], meta[n], out_bytes.
+ *          Pinned buffers (gofr_alloc_pinned) are streamed by the device; pageable ones are copied back at each chunk's
+ *          exact size.
+ * gofr_proto_batch_decode: frames → rows.  Row i and meta[i] are what gofr_proto_decode_nested_ex_device followed by
+ * gofr_proto_decode_nested_deferred_device give, combined by the rule above; meta[i] is the final status.  A frame still
+ * GOFR_GRPC_DEFER (a singular message sent twice, a map field with more than 4096 entries: decode it on the host) and a
+ * failed frame get an empty row.  Rows are 4-byte aligned within out.
+ * gofr_proto_batch_encode: rows → frames, byte for byte and status for status what gofr_proto_encode_nested_ex_device gives.
+ * out_cap: gofr_proto_nested_bound sizes it.  When it is too small, gofr_batch_wait returns GOFR_ERR_CAPACITY, as for
+ * gofr_batch_submit: nothing is written at or past out_cap, meta is complete, out_bytes = out_off[n] = the bytes written, and
+ * out_off is meaningful only for the records of chunks that were written (a chunk that does not fit is dropped whole; the
+ * offsets of its records are unspecified).  n == 0 takes no buffers. */
+typedef struct gofr_proto_batch {
+    const uint8_t* data;   /* frames (decode) or rows (encode) */
+    uint64_t data_bytes;
+    const uint32_t* off;   /* n + 1 */
+    uint32_t n;
+} gofr_proto_batch;
+int gofr_proto_batch_decode(gofr_engine*, const gofr_proto_nmsg* msgs, uint32_t n_msgs, const gofr_proto_nfield* fields, uint32_t n_fields,
+                            uint32_t root, const uint8_t* presence, const gofr_proto_batch* in, gofr_resp_batch* out, gofr_ticket* ticket);
+int gofr_proto_batch_encode(gofr_engine*, const gofr_proto_nmsg* msgs, uint32_t n_msgs, const gofr_proto_nfield* fields, uint32_t n_fields,
+                            uint32_t root, const uint8_t* presence, const gofr_proto_batch* in, gofr_resp_batch* out, gofr_ticket* ticket);
+/* No GPU needed: (per_byte, per_record) such that no record of b bytes yields more than per_byte * b + per_record output
+ * bytes — a row when decode != 0, a whole frame with its 5-byte prefix when encoding.  Sum it over a batch for out_cap. */
+int gofr_proto_nested_bound(const gofr_proto_nmsg* msgs, uint32_t n_msgs, const gofr_proto_nfield* fields, uint32_t n_fields,
+                            uint32_t root, const uint8_t* presence, int decode, uint32_t* per_byte, uint32_t* per_record);
+
 /* Bind as a stage of the split API: Context.Bind(&v) for closures that stay on the host (pkg/gofr/context.go:52-54 ->
  * pkg/gofr/http/request.go:40-47 -> json.Unmarshal(body, &v), v a struct of a registered schema).  Body i is the data
  * section of request i (same descriptors / arena as the serve calls); result i lies in its own slot d_rows + i * slot_bytes

@@ -732,6 +732,87 @@ private:
     std::vector<std::unique_ptr<StructType>> types_;
     std::vector<RouteInfo> routes_;
     std::mt19937_64 rng_{0x9E3779B97F4A7C15ull};
+    friend class ProtoCodec;
+};
+
+// grpc-go's proto codec for a batch of unary calls on the app's engine (gofr_proto_batch_decode / _encode, host buffers):
+// Decode turns request frames (5-byte prefix + message) into rows in the layout of include/gofr_b200.h ("Row format"),
+// the handlers run on the host, Encode turns their response rows into frames.  Built from message types: msgs[m] lists the
+// fields of type m in ascending number order (a GOFR_PB_MESSAGE or GOFR_PB_MAP field names a type by its index in msgs),
+// `root` is the type of the records.  The app must be running (App::Run).
+class ProtoCodec {
+public:
+    struct Field {
+        uint32_t number;
+        uint32_t type;          // GOFR_PB_*, GOFR_PB_MESSAGE or GOFR_PB_MAP
+        bool repeated = false;
+        uint16_t msg = 0;       // GOFR_PB_MESSAGE / GOFR_PB_MAP: the message or entry type
+        uint8_t presence = 0;   // 0, GOFR_PB_OPTIONAL or a oneof group 1..7
+    };
+    struct Batch {
+        std::vector<std::string> records;  // rows (Decode) or frames (Encode); empty where status is not GOFR_GRPC_OK
+        std::vector<uint32_t> status;      // GOFR_GRPC_*: a frame still GOFR_GRPC_DEFER is for the host's own decoder
+    };
+
+    ProtoCodec(const App& app, const std::vector<std::vector<Field>>& msgs, uint32_t root) : engine_(app.engine_), root_(root) {
+        if (!engine_) throw std::logic_error("gofr::ProtoCodec: call App::Run first");
+        bool any_presence = false;
+        for (auto& fields : msgs) {
+            msgs_.push_back(gofr_proto_nmsg{(uint16_t)fields_.size(), (uint16_t)fields.size()});
+            for (auto& f : fields) {
+                fields_.push_back(gofr_proto_nfield{f.number, (uint8_t)f.type, (uint8_t)(f.repeated ? 1 : 0), f.msg});
+                presence_.push_back(f.presence);
+                any_presence |= f.presence != 0;
+            }
+        }
+        if (!any_presence) presence_.clear();
+        uint32_t pb = 0, pr = 0;  // validates the description
+        check(gofr_proto_nested_bound(msgs_.data(), (uint32_t)msgs_.size(), fields_.data(), (uint32_t)fields_.size(), root_,
+                                      presence(), 1, &pb, &pr), "gofr_proto_nested_bound");
+    }
+    Batch Decode(const std::vector<std::string>& frames) const { return run(frames, true); }
+    // rows are padded with zero bytes to a multiple of 4
+    Batch Encode(const std::vector<std::string>& rows) const { return run(rows, false); }
+
+private:
+    const uint8_t* presence() const { return presence_.empty() ? nullptr : presence_.data(); }
+    static void check(int rc, const char* where) {
+        if (rc != GOFR_OK) throw std::runtime_error(std::string(where) + ": " + gofr_last_error());
+    }
+    Batch run(const std::vector<std::string>& in, bool decode) const {
+        std::string data;
+        std::vector<uint32_t> off{0};
+        for (auto& r : in) {
+            data += r;
+            if (!decode) data.append((4 - data.size() % 4) % 4, '\0');
+            off.push_back((uint32_t)data.size());
+        }
+        uint32_t pb = 0, pr = 0;
+        check(gofr_proto_nested_bound(msgs_.data(), (uint32_t)msgs_.size(), fields_.data(), (uint32_t)fields_.size(), root_,
+                                      presence(), decode ? 1 : 0, &pb, &pr), "gofr_proto_nested_bound");
+        const uint64_t cap = (uint64_t)pb * data.size() + (uint64_t)pr * in.size();
+        std::vector<uint8_t> out(cap ? cap : 1);
+        std::vector<uint32_t> out_off(in.size() + 1), meta(in.size() ? in.size() : 1);
+        gofr_proto_batch b{reinterpret_cast<const uint8_t*>(data.data()), data.size(), off.data(), (uint32_t)in.size()};
+        gofr_resp_batch rb{out.data(), cap, out_off.data(), meta.data(), 0};
+        gofr_ticket t = 0;
+        auto call = decode ? gofr_proto_batch_decode : gofr_proto_batch_encode;
+        check(call(engine_, msgs_.data(), (uint32_t)msgs_.size(), fields_.data(), (uint32_t)fields_.size(), root_, presence(), &b, &rb, &t),
+              decode ? "gofr_proto_batch_decode" : "gofr_proto_batch_encode");
+        check(gofr_batch_wait(engine_, t), "gofr_batch_wait");
+        Batch r;
+        for (size_t i = 0; i < in.size(); i++) {
+            r.records.emplace_back(reinterpret_cast<const char*>(out.data()) + out_off[i], out_off[i + 1] - out_off[i]);
+            r.status.push_back(meta[i]);
+        }
+        return r;
+    }
+
+    gofr_engine* engine_;
+    uint32_t root_;
+    std::vector<gofr_proto_nmsg> msgs_;
+    std::vector<gofr_proto_nfield> fields_;
+    std::vector<uint8_t> presence_;
 };
 
 }  // namespace gofr
