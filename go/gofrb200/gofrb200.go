@@ -528,3 +528,69 @@ func (e *Engine) ProtoEncodeBatch(msgs []ProtoNMsg, fields []ProtoNField, root u
 	out []byte, outOff, meta []uint32) (int, error) {
 	return e.protoBatch(false, msgs, fields, root, presence, rows, off, out, outOff, meta)
 }
+
+// ProtoFrontend batches single messages from many goroutines through the nested codec (gofr_proto_frontend_*): the
+// per-message call grpc-go makes on its codec (encoding.Codec.Unmarshal for a request, Marshal for a response, on the
+// RPC's goroutine).  One message type, one direction.  Several ProtoFrontends and a Frontend may share one Engine.
+type ProtoFrontend struct {
+	f         *C.gofr_proto_frontend
+	perByte   uint32
+	perRecord uint32
+}
+
+// ErrProtoRecordTooLarge is what ProtoFrontend.Call returns, before anything is queued, for a record longer than the
+// front-end's maxRecordBytes: marshal or unmarshal that one with protobuf-go.
+var ErrProtoRecordTooLarge = errors.New("gofrb200: record exceeds the front-end's maxRecordBytes")
+
+// NewProtoFrontend creates the decode (decode == true) or encode front-end of message type msgs[root].  maxBatch and
+// maxWaitMicros mean what they mean for NewFrontend; a record longer than maxRecordBytes is refused
+// (ErrProtoRecordTooLarge) before it is queued.
+func NewProtoFrontend(e *Engine, msgs []ProtoNMsg, fields []ProtoNField, root uint32, presence []uint8, decode bool,
+	maxBatch, maxWaitMicros, maxRecordBytes int) (*ProtoFrontend, error) {
+	perByte, perRecord, err := ProtoNestedBound(msgs, fields, root, presence, decode)
+	if err != nil {
+		return nil, err
+	}
+	pp, err := presenceArg(presence, fields)
+	if err != nil {
+		return nil, err
+	}
+	d := C.int(0)
+	if decode {
+		d = 1
+	}
+	var f *C.gofr_proto_frontend
+	if err := check(C.gofr_proto_frontend_create(&f, e.e, (*C.gofr_proto_nmsg)(unsafe.Pointer(&msgs[0])), C.uint32_t(len(msgs)),
+		(*C.gofr_proto_nfield)(unsafe.Pointer(&fields[0])), C.uint32_t(len(fields)), C.uint32_t(root), pp, d, C.uint32_t(maxBatch),
+		C.uint32_t(maxWaitMicros), C.uint32_t(maxRecordBytes)), "gofr_proto_frontend_create"); err != nil {
+		return nil, err
+	}
+	return &ProtoFrontend{f, perByte, perRecord}, nil
+}
+
+// Close must not run while a Call is in progress.
+func (p *ProtoFrontend) Close() { C.gofr_proto_frontend_destroy(p.f); p.f = nil }
+
+// Stats returns the batches run and the records they held.
+func (p *ProtoFrontend) Stats() (batches, records uint64, err error) {
+	var b, r C.uint64_t
+	err = check(C.gofr_proto_frontend_stats(p.f, &b, &r), "gofr_proto_frontend_stats")
+	return uint64(b), uint64(r), err
+}
+
+// Call blocks until the batch this record joined has come back.  Decode: in is the message as Unmarshal receives it (no
+// 5-byte prefix), the result is its row.  Encode: in is a row, the result is the marshalled message without the prefix, as
+// Marshal returns it.  status is a GOFR_GRPC_* code: 6 (GOFR_GRPC_DEFER) means "decode this one with proto.Unmarshal", as
+// does ErrProtoRecordTooLarge.  out has room for the record's bound, so the result always fits.
+func (p *ProtoFrontend) Call(in []byte) (out []byte, status uint32, err error) {
+	buf := make([]byte, uint64(p.perByte)*uint64(len(in)+5)+uint64(p.perRecord))
+	var n, st C.uint32_t
+	rc := C.gofr_proto_frontend_call(p.f, bytesPtr(in), C.uint32_t(len(in)), bytesPtr(buf), C.uint32_t(len(buf)), &n, &st)
+	if rc == C.GOFR_ERR_CAPACITY {
+		return nil, 0, ErrProtoRecordTooLarge
+	}
+	if err = check(rc, "gofr_proto_frontend_call"); err != nil {
+		return nil, 0, err
+	}
+	return buf[:n], uint32(st), nil
+}

@@ -4,61 +4,19 @@
 // The reference serves one request per goroutine (net/http conn.serve → router.ServeHTTP, pkg/gofr/httpServer.go:29-33);
 // the GPU path wants batches.  This is the piece in between, host C++ only: any number of producer threads (connection
 // goroutines through cgo, or the threads of the C++ stand-in) hand in single requests and block until their response is
-// ready; one dispatcher thread closes a batch when it is full or when its oldest request has waited max_wait_us, runs it
-// through the engine's slot-layout host path and wakes the producers, each of which copies its own slot out.
-// A small ring of pinned batches rotates: while one is in flight the next fills, and a batch whose producers are slow to
-// pick their responses up (a descheduled thread) is skipped instead of stalling everybody.
-//
-// No lock on the request path (a mutex + condition variable version spent 5–10 µs per woken thread handing the mutex
-// around: 93 k req/s at 256 threads):
-//   claim     one CAS on the batch's claim word (closed bit | request count | arena bytes) reserves slot i and its arena
-//             range; the request bytes are copied in afterwards, outside any critical section (`filled` counts them in)
-//   close     the dispatcher sets the closed bit with fetch_or — the count is frozen at that instant
-//   complete  the dispatcher publishes the round number in one futex word per group of 32 slots and wakes group 0;
-//             the first thread of group g to notice wakes groups 2g+1 and 2g+2 (a wake tree: the dispatcher does not
-//             pay one wake per thread)
-//   recycle   the last producer to copy its response out reopens the batch
-#include <atomic>
-#include <chrono>
-#include <climits>
+// ready; the dispatcher of frontend_ring.h closes a batch, this file runs it through the engine's slot-layout host path,
+// and each producer copies its own slot out.  The ring (claim, close, timer, wake tree, recycle) is shared with the gRPC
+// front-end, proto_frontend.cpp; what is here is the HTTP payload: the pinned staging in the ABI layout, the Date of a
+// batch and the re-serve of a response too long for its slot.
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
-#include <thread>
 #include <vector>
 #include <time.h>
 
-#include <linux/futex.h>
-#include <sys/syscall.h>
-#include <unistd.h>
-
 #include "../../include/gofr_b200.h"
 #include "engine_internal.h"
-
-namespace {
-
-using Word = std::atomic<uint32_t>;
-static_assert(sizeof(Word) == 4, "futex words are 32-bit");
-
-void futex_wait(Word* w, uint32_t expect, const struct timespec* rel = nullptr) {
-    syscall(SYS_futex, reinterpret_cast<uint32_t*>(w), FUTEX_WAIT_PRIVATE, expect, rel, nullptr, 0);
-}
-void futex_wake_all(Word* w) { syscall(SYS_futex, reinterpret_cast<uint32_t*>(w), FUTEX_WAKE_PRIVATE, INT_MAX, nullptr, nullptr, 0); }
-void bump(Word* w) {
-    w->fetch_add(1, std::memory_order_release);
-    futex_wake_all(w);
-}
-int64_t mono_ns() {
-    return std::chrono::duration_cast<std::chrono::nanoseconds>(std::chrono::steady_clock::now().time_since_epoch()).count();
-}
-
-constexpr uint64_t kClosed = 1ull << 63;
-inline uint32_t claim_count(uint64_t w) { return (uint32_t)(w >> 32) & 0x7FFFFFFFu; }
-inline uint32_t claim_arena(uint64_t w) { return (uint32_t)w; }
-constexpr uint32_t kGroup = 32;  // slots per wake word
-constexpr int kBatches = 4;      // ring of batches
-
-}  // namespace
+#include "frontend_ring.h"
 
 struct gofr_frontend_batch {
     // pinned staging in the ABI layout (gofr_req_batch / gofr_slot_batch)
@@ -68,134 +26,41 @@ struct gofr_frontend_batch {
     uint8_t* out = nullptr;
     uint32_t* out_len = nullptr;
     uint32_t* meta = nullptr;
-    std::atomic<uint64_t> claim{0};       // closed bit | count << 32 | arena bytes
-    std::atomic<uint32_t> filled{0};      // requests whose bytes are in place
-    std::atomic<uint32_t> collected{0};   // producers that have copied their response out
-    std::atomic<uint32_t> round{0};       // bumped at recycle; round r is complete when done[g] == r + 1
-    std::atomic<int64_t> first_ns{0};     // arrival of the round's first request (0: not stored yet)
-    uint32_t closed_count = 0;            // count at close (written by the dispatcher before done[] is published)
     char date[29] = {0};                  // the round's Date header (a response too long for its slot is served again, alone)
-    int rc = GOFR_OK;
-    Word* done = nullptr;                 // per group of kGroup slots: last completed round + 1
-    Word* woke = nullptr;                 // per group: somebody already woke this group's children
 };
 using Batch = gofr_frontend_batch;
 
 struct gofr_frontend {
+    gofr_frontend(uint32_t max_batch, uint32_t max_wait_us) : ring(max_batch, max_wait_us) {}
     gofr_engine* eng = nullptr;
-    uint32_t max_batch = 0, max_wait_us = 0, slot_bytes = 0, per_request = 0, groups = 0;
+    uint32_t max_batch = 0, slot_bytes = 0, per_request = 0;
     std::atomic<int64_t> fixed_clock{0};  // tests: the Date of every batch; 0 = wall clock
-    Batch b[kBatches];
-    std::atomic<int> filling{0};          // the batch producers try first
-    std::atomic<bool> stop{false};
-    Word disp_seq{0};                     // dispatcher sleeps on this: first claim of a round, full batch, recycle, stop
-    Word room_seq{0};                     // producers without a slot sleep on this: batch closed (flip) or recycled
-    std::thread worker;
-    std::atomic<uint64_t> batches{0}, requests{0};
-    // GOFR_FRONTEND_DEBUG=1: where the dispatcher's time goes (printed at destroy)
-    bool debug = false;
-    int64_t dbg_spin_ns = 0, dbg_spin_max = 0, dbg_eng_ns = 0, dbg_eng_max = 0, dbg_wake_ns = 0, dbg_wake_max = 0, dbg_idle_ns = 0;
-    uint64_t dbg_eng_slow = 0;
+    Batch b[gofr_ring::kBatches];
+    gofr_ring::Ring ring;                 // GOFR_FRONTEND_DEBUG=1: where the dispatcher's time goes (printed at destroy)
 };
 
 static void free_batch(Batch& x) {
     gofr_free_pinned(x.desc); gofr_free_pinned(x.ids); gofr_free_pinned(x.arena);
     gofr_free_pinned(x.out); gofr_free_pinned(x.out_len); gofr_free_pinned(x.meta);
-    delete[] x.done;
-    delete[] x.woke;
 }
 
-static void dispatcher(gofr_frontend* f) {
-    for (;;) {
-        const uint32_t seq = f->disp_seq.load(std::memory_order_acquire);
-        int k = f->filling.load(std::memory_order_relaxed);
-        uint64_t w = f->b[k].claim.load(std::memory_order_acquire);
-        if ((w & kClosed) || claim_count(w) == 0) {
-            // Nothing to serve in the current batch.  Another one may hold requests (a producer that read `filling` just
-            // before a flip can claim a slot in a batch that was recycled in between); and if the current batch is still
-            // handing out its previous round, any open batch is a better place for producers to go.
-            int best = -1;
-            for (int j = 1; j < kBatches && best < 0; j++) {
-                const uint64_t wj = f->b[(k + j) % kBatches].claim.load(std::memory_order_acquire);
-                if (!(wj & kClosed) && claim_count(wj) > 0) best = (k + j) % kBatches;
-            }
-            for (int j = 1; j < kBatches && best < 0 && (w & kClosed); j++)
-                if (!(f->b[(k + j) % kBatches].claim.load(std::memory_order_acquire) & kClosed)) best = (k + j) % kBatches;
-            if (best >= 0) {
-                k = best;
-                f->filling.store(k, std::memory_order_release);
-                bump(&f->room_seq);
-                w = f->b[k].claim.load(std::memory_order_acquire);
-            }
-        }
-        Batch& x = f->b[k];
-        const bool stopping = f->stop.load(std::memory_order_acquire);
-        if ((w & kClosed) || claim_count(w) == 0) {  // still being collected by its previous round / nothing to do
-            if (stopping && !(w & kClosed)) return;
-            futex_wait(&f->disp_seq, seq);
-            continue;
-        }
-        if (claim_count(w) < f->max_batch && !stopping) {
-            // not full: wait until the oldest request has been here max_wait_us (or the batch fills up)
-            const int64_t first = x.first_ns.load(std::memory_order_acquire), now = mono_ns();
-            const int64_t deadline = (first ? first : now) + (int64_t)f->max_wait_us * 1000;
-            if (now < deadline) {
-                struct timespec rel;
-                rel.tv_sec = (deadline - now) / 1000000000;
-                rel.tv_nsec = (deadline - now) % 1000000000;
-                futex_wait(&f->disp_seq, seq, &rel);
-                continue;
-            }
-        }
-        // close: the count is frozen by the fetch_or; producers move on to the next open batch of the ring
-        w = x.claim.fetch_or(kClosed, std::memory_order_acq_rel);
-        const uint32_t n = claim_count(w);
-        x.closed_count = n;
-        int next = (k + 1) % kBatches;
-        for (int j = 1; j < kBatches; j++)
-            if (!(f->b[(k + j) % kBatches].claim.load(std::memory_order_acquire) & kClosed)) { next = (k + j) % kBatches; break; }
-        f->filling.store(next, std::memory_order_release);
-        bump(&f->room_seq);
-        const int64_t t_close = f->debug ? mono_ns() : 0;
-        while (x.filled.load(std::memory_order_acquire) != n) {  // the last claimants are still copying their bytes in
-#if defined(__x86_64__)
-            __builtin_ia32_pause();
-#endif
-        }
-        const int64_t t_filled = f->debug ? mono_ns() : 0;
-        gofr_req_batch in;
-        memset(&in, 0, sizeof in);
-        in.desc = x.desc; in.trace_ids = x.ids; in.arena = x.arena; in.arena_bytes = (claim_arena(w) + 15u) & ~15u; in.n = n;
-        int64_t now = f->fixed_clock.load(std::memory_order_relaxed);
-        if (!now) { struct timespec ts; clock_gettime(CLOCK_REALTIME, &ts); now = (int64_t)ts.tv_sec; }
-        gofr_format_http_date(now, in.date);
-        memcpy(x.date, in.date, sizeof x.date);
-        gofr_slot_batch out;
-        memset(&out, 0, sizeof out);
-        out.out = x.out; out.slot_bytes = f->slot_bytes; out.out_len = x.out_len; out.meta = x.meta;
-        gofr_ticket t = 0;
-        int rc = gofr_batch_submit_slots(f->eng, &in, &out, &t);
-        if (rc == GOFR_OK) rc = gofr_batch_wait(f->eng, t);
-        const int64_t t_eng = f->debug ? mono_ns() : 0;
-        x.rc = rc;
-        f->batches.fetch_add(1, std::memory_order_relaxed);
-        f->requests.fetch_add(n, std::memory_order_relaxed);
-        // publish the round in every group's word, then start the wake tree at its root.  DESCENDING group order: a
-        // caller of group g that is already awake may see done[g] == r1 at any moment and wake its children 2g+1 and
-        // 2g+2 exactly once (woke[g]); with release stores from the highest group down, seeing done[g] implies both
-        // children's words are already stored, so a child woken by that futex_wake cannot read the old value and go back
-        // to sleep with nobody left to wake it.
-        const uint32_t r1 = x.round.load(std::memory_order_relaxed) + 1, g_used = (n + kGroup - 1) / kGroup;
-        for (uint32_t g = g_used; g-- > 0;) x.done[g].store(r1, std::memory_order_release);
-        futex_wake_all(&x.done[0]);
-        if (f->debug) {
-            const int64_t t_end = mono_ns();
-            f->dbg_spin_ns += t_filled - t_close; if (t_filled - t_close > f->dbg_spin_max) f->dbg_spin_max = t_filled - t_close;
-            f->dbg_eng_ns += t_eng - t_filled; if (t_eng - t_filled > f->dbg_eng_max) f->dbg_eng_max = t_eng - t_filled;
-            if (t_eng - t_filled > 5000000) f->dbg_eng_slow++;
-            f->dbg_wake_ns += t_end - t_eng; if (t_end - t_eng > f->dbg_wake_max) f->dbg_wake_max = t_end - t_eng;
-        }
-    }
+// the dispatcher's step: batch k's n requests (arena_bytes of path, query and body) through the slot-layout host path
+static int serve_batch(gofr_frontend* f, int k, uint32_t n, uint32_t arena_bytes) {
+    Batch& x = f->b[k];
+    gofr_req_batch in;
+    memset(&in, 0, sizeof in);
+    in.desc = x.desc; in.trace_ids = x.ids; in.arena = x.arena; in.arena_bytes = (arena_bytes + 15u) & ~15u; in.n = n;
+    int64_t now = f->fixed_clock.load(std::memory_order_relaxed);
+    if (!now) { struct timespec ts; clock_gettime(CLOCK_REALTIME, &ts); now = (int64_t)ts.tv_sec; }
+    gofr_format_http_date(now, in.date);
+    memcpy(x.date, in.date, sizeof x.date);
+    gofr_slot_batch out;
+    memset(&out, 0, sizeof out);
+    out.out = x.out; out.slot_bytes = f->slot_bytes; out.out_len = x.out_len; out.meta = x.meta;
+    gofr_ticket t = 0;
+    int rc = gofr_batch_submit_slots(f->eng, &in, &out, &t);
+    if (rc == GOFR_OK) rc = gofr_batch_wait(f->eng, t);
+    return rc;
 }
 
 extern "C" {
@@ -203,15 +68,13 @@ extern "C" {
 int gofr_frontend_create(gofr_frontend** out, gofr_engine* e, uint32_t max_batch, uint32_t max_wait_us, uint32_t slot_bytes,
                          uint32_t max_request_bytes) {
     if (!out || !e || max_batch == 0 || max_batch > 0x7FFFFFFFu || slot_bytes == 0 || (slot_bytes & 15u)) return GOFR_ERR_INVALID;
-    gofr_frontend* f = new gofr_frontend();
-    f->eng = e;
-    f->max_batch = max_batch;
-    f->max_wait_us = max_wait_us;
-    f->slot_bytes = slot_bytes;
-    f->groups = (max_batch + kGroup - 1) / kGroup;
     const uint64_t per = ((uint64_t)max_request_bytes + 7u) & ~(uint64_t)3u;  // path|query and body are each padded to 4
     const uint64_t cap = (uint64_t)max_batch * per + 64;
-    if (cap > 0xFFFFFFF0ull) { delete f; return GOFR_ERR_CAPACITY; }
+    if (cap > 0xFFFFFFF0ull) return GOFR_ERR_CAPACITY;
+    gofr_frontend* f = new gofr_frontend(max_batch, max_wait_us);
+    f->eng = e;
+    f->max_batch = max_batch;
+    f->slot_bytes = slot_bytes;
     f->per_request = (uint32_t)per;
     for (auto& x : f->b) {
         x.desc = (gofr_req_desc*)gofr_alloc_pinned((size_t)max_batch * sizeof(gofr_req_desc));
@@ -220,32 +83,27 @@ int gofr_frontend_create(gofr_frontend** out, gofr_engine* e, uint32_t max_batch
         x.out = (uint8_t*)gofr_alloc_pinned((size_t)max_batch * slot_bytes);
         x.out_len = (uint32_t*)gofr_alloc_pinned((size_t)max_batch * 4);
         x.meta = (uint32_t*)gofr_alloc_pinned((size_t)max_batch * 4);
-        x.done = new Word[f->groups];
-        x.woke = new Word[f->groups];
-        for (uint32_t g = 0; g < f->groups; g++) { x.done[g].store(0); x.woke[g].store(0); }
         if (!x.desc || !x.ids || !x.arena || !x.out || !x.out_len || !x.meta) {
             for (auto& y : f->b) free_batch(y);
             delete f;
             return GOFR_ERR_NOMEM;
         }
     }
-    { const char* dbg = getenv("GOFR_FRONTEND_DEBUG"); f->debug = dbg && dbg[0] == '1'; }
-    f->worker = std::thread(dispatcher, f);
+    { const char* dbg = getenv("GOFR_FRONTEND_DEBUG"); f->ring.debug = dbg && dbg[0] == '1'; }
+    f->ring.start([f](int k, uint32_t n, uint32_t arena_bytes) { return serve_batch(f, k, n, arena_bytes); });
     *out = f;
     return GOFR_OK;
 }
 
 void gofr_frontend_destroy(gofr_frontend* f) {
     if (!f) return;
-    f->stop.store(true, std::memory_order_release);
-    bump(&f->disp_seq);
-    bump(&f->room_seq);
-    if (f->worker.joinable()) f->worker.join();
-    if (f->debug) {
-        const double nb = (double)(f->batches.load() ? f->batches.load() : 1);
+    gofr_ring::Ring& r = f->ring;
+    r.stop();
+    if (r.debug) {
+        const double nb = (double)(r.batches.load() ? r.batches.load() : 1);
         fprintf(stderr, "[gofr frontend] batches %llu  fill-spin avg %.1f max %.1f us  engine avg %.1f max %.1f us (>5ms: %llu)  publish+wake avg %.1f max %.1f us\n",
-                (unsigned long long)f->batches.load(), f->dbg_spin_ns / nb / 1e3, f->dbg_spin_max / 1e3, f->dbg_eng_ns / nb / 1e3,
-                f->dbg_eng_max / 1e3, (unsigned long long)f->dbg_eng_slow, f->dbg_wake_ns / nb / 1e3, f->dbg_wake_max / 1e3);
+                (unsigned long long)r.batches.load(), r.dbg_spin_ns / nb / 1e3, r.dbg_spin_max / 1e3, r.dbg_eng_ns / nb / 1e3,
+                r.dbg_eng_max / 1e3, (unsigned long long)r.dbg_eng_slow, r.dbg_wake_ns / nb / 1e3, r.dbg_wake_max / 1e3);
     }
     for (auto& x : f->b) free_batch(x);
     delete f;
@@ -259,8 +117,8 @@ int gofr_frontend_set_clock(gofr_frontend* f, int64_t unix_seconds) {
 
 int gofr_frontend_stats(gofr_frontend* f, uint64_t* batches, uint64_t* requests) {
     if (!f) return GOFR_ERR_INVALID;
-    if (batches) *batches = f->batches.load(std::memory_order_relaxed);
-    if (requests) *requests = f->requests.load(std::memory_order_relaxed);
+    if (batches) *batches = f->ring.batches.load(std::memory_order_relaxed);
+    if (requests) *requests = f->ring.records.load(std::memory_order_relaxed);
     return GOFR_OK;
 }
 
@@ -274,26 +132,12 @@ int gofr_frontend_serve(gofr_frontend* f, uint8_t method, const uint8_t* path, u
         return GOFR_ERR_CAPACITY;
     }
     const uint32_t need = (uint32_t)need64;
-    // ---- claim slot i and `need` arena bytes in the filling batch ----
-    Batch* xp;
-    uint32_t i, a;
-    for (;;) {
-        if (f->stop.load(std::memory_order_acquire)) return GOFR_ERR_INVALID;
-        const uint32_t rs = f->room_seq.load(std::memory_order_acquire);
-        Batch& c = f->b[f->filling.load(std::memory_order_acquire)];
-        uint64_t w = c.claim.load(std::memory_order_acquire);
-        if (!(w & kClosed) && claim_count(w) < f->max_batch) {
-            // arena bytes never run out first: the arena holds max_batch requests of the largest admissible size
-            if (!c.claim.compare_exchange_weak(w, w + (1ull << 32) + need, std::memory_order_acq_rel)) continue;
-            xp = &c; i = claim_count(w); a = claim_arena(w);
-            break;
-        }
-        if (!(w & kClosed)) bump(&f->disp_seq);  // full: the dispatcher should close it now
-        futex_wait(&f->room_seq, rs);            // until a batch is closed (the other one becomes current) or recycled
-    }
-    Batch& x = *xp;
-    const uint32_t round = x.round.load(std::memory_order_acquire);  // stable until this producer has collected
-    if (i == 0) x.first_ns.store(mono_ns(), std::memory_order_release);
+    // ---- claim slot i and `need` arena bytes in the filling batch (arena bytes never run out first: the arena holds
+    //      max_batch requests of the largest admissible size) ----
+    gofr_ring::Seat s;
+    if (!f->ring.claim(need, &s)) return GOFR_ERR_INVALID;
+    Batch& x = f->b[s.k];
+    const uint32_t i = s.i, a = s.a;
     gofr_req_desc d;
     memset(&d, 0, sizeof d);
     d.arena_off = a; d.path_len = path_len; d.query_len = query_len; d.data_len = data_len; d.method = method; d.flags = flags;
@@ -303,23 +147,11 @@ int gofr_frontend_serve(gofr_frontend* f, uint8_t method, const uint8_t* path, u
     if (data_len) memcpy(x.arena + body_at, data, data_len);
     x.desc[i] = d;
     memcpy(x.ids + (size_t)i * 16, trace_id, 16);
-    x.filled.fetch_add(1, std::memory_order_release);
-    if (i == 0 || i + 1 == f->max_batch) bump(&f->disp_seq);  // start the round's timer / close a full batch
+    f->ring.filled(s);
 
     // ---- wait for the round to come back ----
-    const uint32_t g = i / kGroup;
-    for (;;) {
-        const uint32_t v = x.done[g].load(std::memory_order_acquire);
-        if (v == round + 1) break;
-        futex_wait(&x.done[g], v);
-    }
-    const uint32_t n = x.closed_count;
-    const uint32_t g_used = (n + kGroup - 1) / kGroup;
-    if (2 * g + 1 < g_used && x.woke[g].exchange(1, std::memory_order_acq_rel) == 0) {
-        futex_wake_all(&x.done[2 * g + 1]);
-        if (2 * g + 2 < g_used) futex_wake_all(&x.done[2 * g + 2]);
-    }
-    int rc = x.rc;
+    const uint32_t n = f->ring.wait(s);
+    int rc = f->ring.b[s.k].rc;
     const uint32_t len = x.out_len[i];
     if (meta) *meta = x.meta[i];
     *resp_len = len;
@@ -331,16 +163,7 @@ int gofr_frontend_serve(gofr_frontend* f, uint8_t method, const uint8_t* path, u
         else if (len) memcpy(resp, x.out + (size_t)i * f->slot_bytes, len);
     }
     // ---- the last producer to leave reopens the batch ----
-    if (x.collected.fetch_add(1, std::memory_order_acq_rel) + 1 == n) {
-        for (uint32_t k = 0; k < g_used; k++) x.woke[k].store(0, std::memory_order_relaxed);
-        x.filled.store(0, std::memory_order_relaxed);
-        x.collected.store(0, std::memory_order_relaxed);
-        x.first_ns.store(0, std::memory_order_relaxed);
-        x.round.store(round + 1, std::memory_order_release);
-        x.claim.store(0, std::memory_order_release);
-        bump(&f->room_seq);
-        bump(&f->disp_seq);
-    }
+    f->ring.leave(s, n);
     if (alone) {
         // The slot layout reports the length of a response that does not fit but writes nothing: serve this one request
         // again through the packed call, straight into the caller's buffer, with the Date of the batch it belonged to.

@@ -22,6 +22,8 @@
  *                                 hello_grpc.pb.go:73-89           gofr_grpc_hello_device
  *   dec(in) / proto.Marshal of any flat proto3 message type (the codec grpc-go calls around a unary handler)
  *                                 hello_grpc.pb.go:73-89           gofr_proto_decode_device / gofr_proto_encode_device
+ *   encoding.Codec.Unmarshal / Marshal once per message on the RPC's goroutine
+ *                                 hello_grpc.pb.go:73-89           gofr_proto_frontend_call (batches the concurrent callers)
  *   Router.Match + mux.Vars (routing only, closures on the host)
  *                                 pkg/gofr/http/router.go:14,30-33 gofr_route_device / gofr_batch_route
  *   router.ServeHTTP per request under net/http's conn goroutine
@@ -633,6 +635,35 @@ int gofr_frontend_stats(gofr_frontend*, uint64_t* batches, uint64_t* requests);
 int gofr_frontend_serve(gofr_frontend*, uint8_t method, const uint8_t* path, uint16_t path_len, const uint8_t* query,
                         uint16_t query_len, uint8_t flags, const uint8_t* data, uint32_t data_len, const uint8_t trace_id[16],
                         uint8_t* resp, uint32_t resp_cap, uint32_t* resp_len, uint32_t* meta);
+
+/* Batching front-end of the nested proto3 codec: grpc-go calls its codec once per message (encoding.Codec.Unmarshal for a
+ * request, Marshal for a response, on the RPC's goroutine; hello_grpc.pb.go:73-89 runs dec(in) between them); the GPU codec
+ * wants batches.  Any number of threads call gofr_proto_frontend_call with ONE record each and block until its result is
+ * ready; batches close and rotate as gofr_frontend_create's max_batch and max_wait_us say, and run through
+ * gofr_proto_batch_decode when decode != 0, else gofr_proto_batch_encode.  One front-end serves one message type (the _ex description, presence may be
+ * NULL) in one direction; several front-ends and a gofr_frontend may share an engine (their batches take turns on it).
+ *   decode   in is the message as Unmarshal receives it: no 5-byte prefix, already decompressed; out receives the row.  Row
+ *            and *status are what gofr_proto_batch_decode gives for the frame 00 | len_be32(m) | m, whatever else is in
+ *            the batch: GOFR_GRPC_OK, BAD_PROTO, BAD_UTF8 or DEFER ("decode this one with protobuf-go").
+ *   encode   in is a row, zero padded to a multiple of 4 by the front-end; out receives the marshalled message WITHOUT the
+ *            prefix (what Marshal returns): gofr_proto_batch_encode's frame for that row minus its first 5 bytes, and its
+ *            status: GOFR_GRPC_OK, BAD_UTF8 or BAD_ROW.
+ * A failed record has *out_len = 0.  Returns GOFR_OK; GOFR_ERR_CAPACITY before anything is queued when in_len >
+ * max_record_bytes (hand the message to protobuf-go); GOFR_ERR_CAPACITY with *out_len (and *status) set when the result does
+ * not fit out_cap (the front-end keeps serving); the batch call's own error for every caller of that batch; GOFR_ERR_INVALID
+ * for bad arguments and once destroy has started.
+ * create checks the description as gofr_proto_nested_bound does (same codes) and refuses (GOFR_ERR_CAPACITY) a max_batch *
+ * (per_byte * (max_record_bytes + 5) + per_record) beyond 32 bits (the batch call's output offsets), with per_byte and
+ * per_record the bound of the direction.  A batch's pinned output grows to the sum of its records' bounds when that is
+ * larger and never shrinks.  destroy may only be called when no thread is inside gofr_proto_frontend_call. */
+typedef struct gofr_proto_frontend gofr_proto_frontend;
+int gofr_proto_frontend_create(gofr_proto_frontend** out, gofr_engine*, const gofr_proto_nmsg* msgs, uint32_t n_msgs,
+                               const gofr_proto_nfield* fields, uint32_t n_fields, uint32_t root, const uint8_t* presence,
+                               int decode, uint32_t max_batch, uint32_t max_wait_us, uint32_t max_record_bytes);
+void gofr_proto_frontend_destroy(gofr_proto_frontend*);
+int gofr_proto_frontend_stats(gofr_proto_frontend*, uint64_t* batches, uint64_t* records);
+int gofr_proto_frontend_call(gofr_proto_frontend*, const uint8_t* in, uint32_t in_len, uint8_t* out, uint32_t out_cap,
+                             uint32_t* out_len, uint32_t* status);
 
 /* HTTP/1.1 request heads (SURVEY.md §8f rank 2): what net/http's readRequest + url.ParseRequestURI hand to
  * Router.ServeHTTP, for a batch of raw request messages resident in HBM, in the layout the serve calls consume.

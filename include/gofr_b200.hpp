@@ -30,6 +30,7 @@
 #include <random>
 #include <stdexcept>
 #include <string>
+#include <tuple>
 #include <utility>
 #include <variant>
 #include <vector>
@@ -754,31 +755,46 @@ public:
         std::vector<uint32_t> status;      // GOFR_GRPC_*: a frame still GOFR_GRPC_DEFER is for the host's own decoder
     };
 
-    ProtoCodec(const App& app, const std::vector<std::vector<Field>>& msgs, uint32_t root) : engine_(app.engine_), root_(root) {
-        if (!engine_) throw std::logic_error("gofr::ProtoCodec: call App::Run first");
-        bool any_presence = false;
-        for (auto& fields : msgs) {
-            msgs_.push_back(gofr_proto_nmsg{(uint16_t)fields_.size(), (uint16_t)fields.size()});
-            for (auto& f : fields) {
-                fields_.push_back(gofr_proto_nfield{f.number, (uint8_t)f.type, (uint8_t)(f.repeated ? 1 : 0), f.msg});
-                presence_.push_back(f.presence);
-                any_presence |= f.presence != 0;
+    // the description in the ABI's form, checked (gofr_proto_nested_bound) on construction
+    struct Description {
+        Description(const std::vector<std::vector<Field>>& msgs, uint32_t root_) : root(root_) {
+            bool any_presence = false;
+            for (auto& fs : msgs) {
+                this->msgs.push_back(gofr_proto_nmsg{(uint16_t)fields.size(), (uint16_t)fs.size()});
+                for (auto& f : fs) {
+                    fields.push_back(gofr_proto_nfield{f.number, (uint8_t)f.type, (uint8_t)(f.repeated ? 1 : 0), f.msg});
+                    presence_.push_back(f.presence);
+                    any_presence |= f.presence != 0;
+                }
             }
+            if (!any_presence) presence_.clear();
+            bound(true);
         }
-        if (!any_presence) presence_.clear();
-        uint32_t pb = 0, pr = 0;  // validates the description
-        check(gofr_proto_nested_bound(msgs_.data(), (uint32_t)msgs_.size(), fields_.data(), (uint32_t)fields_.size(), root_,
-                                      presence(), 1, &pb, &pr), "gofr_proto_nested_bound");
+        const uint8_t* presence() const { return presence_.empty() ? nullptr : presence_.data(); }
+        // (per_byte, per_record) of gofr_proto_nested_bound for the direction
+        std::pair<uint32_t, uint32_t> bound(bool decode) const {
+            uint32_t pb = 0, pr = 0;
+            check(gofr_proto_nested_bound(msgs.data(), (uint32_t)msgs.size(), fields.data(), (uint32_t)fields.size(), root,
+                                          presence(), decode ? 1 : 0, &pb, &pr), "gofr_proto_nested_bound");
+            return {pb, pr};
+        }
+        uint32_t root;
+        std::vector<gofr_proto_nmsg> msgs;
+        std::vector<gofr_proto_nfield> fields;
+        std::vector<uint8_t> presence_;
+    };
+    static void check(int rc, const char* where) {
+        if (rc != GOFR_OK) throw std::runtime_error(std::string(where) + ": " + gofr_last_error());
+    }
+
+    ProtoCodec(const App& app, const std::vector<std::vector<Field>>& msgs, uint32_t root) : engine_(app.engine_), d_(msgs, root) {
+        if (!engine_) throw std::logic_error("gofr::ProtoCodec: call App::Run first");
     }
     Batch Decode(const std::vector<std::string>& frames) const { return run(frames, true); }
     // rows are padded with zero bytes to a multiple of 4
     Batch Encode(const std::vector<std::string>& rows) const { return run(rows, false); }
 
 private:
-    const uint8_t* presence() const { return presence_.empty() ? nullptr : presence_.data(); }
-    static void check(int rc, const char* where) {
-        if (rc != GOFR_OK) throw std::runtime_error(std::string(where) + ": " + gofr_last_error());
-    }
     Batch run(const std::vector<std::string>& in, bool decode) const {
         std::string data;
         std::vector<uint32_t> off{0};
@@ -787,9 +803,7 @@ private:
             if (!decode) data.append((4 - data.size() % 4) % 4, '\0');
             off.push_back((uint32_t)data.size());
         }
-        uint32_t pb = 0, pr = 0;
-        check(gofr_proto_nested_bound(msgs_.data(), (uint32_t)msgs_.size(), fields_.data(), (uint32_t)fields_.size(), root_,
-                                      presence(), decode ? 1 : 0, &pb, &pr), "gofr_proto_nested_bound");
+        const auto [pb, pr] = d_.bound(decode);
         const uint64_t cap = (uint64_t)pb * data.size() + (uint64_t)pr * in.size();
         std::vector<uint8_t> out(cap ? cap : 1);
         std::vector<uint32_t> out_off(in.size() + 1), meta(in.size() ? in.size() : 1);
@@ -797,7 +811,8 @@ private:
         gofr_resp_batch rb{out.data(), cap, out_off.data(), meta.data(), 0};
         gofr_ticket t = 0;
         auto call = decode ? gofr_proto_batch_decode : gofr_proto_batch_encode;
-        check(call(engine_, msgs_.data(), (uint32_t)msgs_.size(), fields_.data(), (uint32_t)fields_.size(), root_, presence(), &b, &rb, &t),
+        check(call(engine_, d_.msgs.data(), (uint32_t)d_.msgs.size(), d_.fields.data(), (uint32_t)d_.fields.size(), d_.root, d_.presence(),
+                   &b, &rb, &t),
               decode ? "gofr_proto_batch_decode" : "gofr_proto_batch_encode");
         check(gofr_batch_wait(engine_, t), "gofr_batch_wait");
         Batch r;
@@ -809,10 +824,60 @@ private:
     }
 
     gofr_engine* engine_;
-    uint32_t root_;
-    std::vector<gofr_proto_nmsg> msgs_;
-    std::vector<gofr_proto_nfield> fields_;
-    std::vector<uint8_t> presence_;
+    Description d_;
+};
+
+// grpc-go's codec one message at a time (gofr_proto_frontend_call): Call blocks until the batch the record joined has come
+// back, so each RPC's thread calls it the way grpc-go calls encoding.Codec.Unmarshal / Marshal.  Decode: the message
+// without its 5-byte prefix → the row; encode: a row (padded with zero bytes to a multiple of 4) → the marshalled message
+// without the prefix.  One message type, one direction; any number of threads may call one ProtoFrontend.  Built from the
+// same Field lists as ProtoCodec; the app must be running (App::Run).
+class ProtoFrontend {
+public:
+    using Field = ProtoCodec::Field;
+    struct Result {
+        int rc = GOFR_OK;      // GOFR_ERR_CAPACITY: the record exceeds max_record_bytes, nothing was queued (use the host codec)
+        uint32_t status = 0;   // GOFR_GRPC_*: GOFR_GRPC_DEFER is for the host's own decoder
+        std::string record;    // the row (decode) or the message (encode); empty where status is not GOFR_GRPC_OK
+    };
+
+    ProtoFrontend(const App& app, const std::vector<std::vector<Field>>& msgs, uint32_t root, bool decode, uint32_t max_batch = 1024,
+                  uint32_t max_wait_us = 200, uint32_t max_record_bytes = 4096)
+        : d_(msgs, root) {
+        if (!app.engine()) throw std::logic_error("gofr::ProtoFrontend: call App::Run first");
+        std::tie(per_byte_, per_record_) = d_.bound(decode);
+        ProtoCodec::check(gofr_proto_frontend_create(&f_, app.engine(), d_.msgs.data(), (uint32_t)d_.msgs.size(), d_.fields.data(),
+                                                     (uint32_t)d_.fields.size(), root, d_.presence(), decode ? 1 : 0, max_batch,
+                                                     max_wait_us, max_record_bytes),
+                          "gofr_proto_frontend_create");
+    }
+    ~ProtoFrontend() { gofr_proto_frontend_destroy(f_); }
+    ProtoFrontend(const ProtoFrontend&) = delete;
+    ProtoFrontend& operator=(const ProtoFrontend&) = delete;
+
+    Result Call(const std::string& in) const {
+        Result r;
+        // room for the bound of this record: the front-end never answers GOFR_ERR_CAPACITY for the output
+        std::vector<uint8_t> out((size_t)per_byte_ * (in.size() + 5) + per_record_);
+        uint32_t len = 0;
+        r.rc = in.size() > UINT32_MAX ? GOFR_ERR_CAPACITY
+                                      : gofr_proto_frontend_call(f_, reinterpret_cast<const uint8_t*>(in.data()), (uint32_t)in.size(),
+                                                                 out.data(), (uint32_t)out.size(), &len, &r.status);
+        if (r.rc == GOFR_ERR_CAPACITY) return r;
+        ProtoCodec::check(r.rc, "gofr_proto_frontend_call");
+        r.record.assign(reinterpret_cast<const char*>(out.data()), len);
+        return r;
+    }
+    std::pair<uint64_t, uint64_t> Stats() const {
+        uint64_t b = 0, n = 0;
+        ProtoCodec::check(gofr_proto_frontend_stats(f_, &b, &n), "gofr_proto_frontend_stats");
+        return {b, n};
+    }
+
+private:
+    ProtoCodec::Description d_;
+    uint32_t per_byte_ = 0, per_record_ = 0;
+    gofr_proto_frontend* f_ = nullptr;
 };
 
 }  // namespace gofr
