@@ -239,6 +239,22 @@ func (e *Engine) HTTPParseDevice(dRaw, dRawOff unsafe.Pointer, n int, dDesc, dAr
 		(*C.uint8_t)(dArena), (*C.uint32_t)(dStatus), (*C.uint64_t)(dSpans), stream), "gofr_http_parse_device")
 }
 
+// Connection statuses of HTTPFrameDevice (GOFR_HTTP_CONN_*).
+const (
+	HTTPConnDone  = 0 // every byte belongs to a whole request
+	HTTPConnMore  = 1 // the last record is the beginning of a request: keep it and append the next read
+	HTTPConnDefer = 2 // the last record starts with a request outside the subset: hand the bytes from consumed on to net/http
+)
+
+// HTTPFrameDevice cuts connection receive buffers (connection c = dBuf[off[c]:off[c+1]]) into the record column
+// HTTPParseDevice takes as dRawOff (gofr_http_frame_device): a connection's whole requests in order, then one tail record
+// when bytes are left over.  Connection c owns records dFirst[c] .. dFirst[c+1]; dFirst[nConns] is the record count.
+func (e *Engine) HTTPFrameDevice(dBuf, dBufOff unsafe.Pointer, nConns int, dRecOff unsafe.Pointer, recCap int, dFirst, dConsumed,
+	dConnStatus unsafe.Pointer, stream unsafe.Pointer) error {
+	return check(C.gofr_http_frame_device(e.e, (*C.uint8_t)(dBuf), (*C.uint32_t)(dBufOff), C.uint32_t(nConns), (*C.uint32_t)(dRecOff),
+		C.uint32_t(recCap), (*C.uint32_t)(dFirst), (*C.uint32_t)(dConsumed), (*C.uint32_t)(dConnStatus), stream), "gofr_http_frame_device")
+}
+
 // Frontend gathers single requests from many goroutines into batches (gofr_frontend_*): the per-request call that stands
 // where router.ServeHTTP stands in the reference (pkg/gofr/httpServer.go:29-33).
 type Frontend struct{ f *C.gofr_frontend }

@@ -66,6 +66,7 @@ __global__ void proto_decode_nested_presence_kernel(const GrpcParams p, const Pb
 __global__ void proto_decode_nested_deferred_kernel(const GrpcParams p, const uint32_t* meta_in, const PbnDesc D);  // proto_nested_deferred_kernel.cu
 __global__ void reqlog_kernel(const LogParams p);                // reqlog_kernel.cu
 __global__ void http_parse_kernel(const HttpParams p);           // http_kernel.cu
+__global__ void http_frame_kernel(const HttpFrameParams p);      // http_frame_kernel.cu
 __global__ void route_kernel(const RouteParams p);               // route_kernel.cu
 __global__ void bind_kernel(const BindParams p);                 // bind_kernel.cu
 __global__ void chunk_pack_kernel(const PackParams p);           // pack_kernel.cu
@@ -75,7 +76,7 @@ namespace {
 
 enum Kern {
     K_SERVE, K_SERVE_VALUES, K_SLOTS, K_SLOTS_WIDE, K_SLOTS_VALUES, K_HELLO, K_PROTO_ENC, K_PROTO_DEC, K_PBN_ENC, K_PBN_DEC,
-    K_PBN_ENC_MAPS, K_PBN_DEC_MAPS, K_PBN_ENC_PRES, K_PBN_DEC_PRES, K_PBN_DEC_DEFERRED, K_REQLOG, K_HTTP, K_ROUTE, K_BIND, K_PACK,
+    K_PBN_ENC_MAPS, K_PBN_DEC_MAPS, K_PBN_ENC_PRES, K_PBN_DEC_PRES, K_PBN_DEC_DEFERRED, K_REQLOG, K_HTTP, K_HTTP_FRAME, K_ROUTE, K_BIND, K_PACK,
     K_COUNT
 };
 struct KernelRec {
@@ -101,6 +102,7 @@ const KernelRec kKernels[K_COUNT] = {
     {(const void*)proto_decode_nested_deferred_kernel, "proto", kServeThreads},
     {(const void*)reqlog_kernel, "request-log", kServeThreads},
     {(const void*)http_parse_kernel, "http", kServeThreads},
+    {(const void*)http_frame_kernel, "http-frame", kServeThreads},
     {(const void*)route_kernel, "route", kRouteThreads},
     {(const void*)bind_kernel, "bind", kBindThreads},
     {(const void*)chunk_pack_kernel, "pack", kServeThreads},
@@ -1646,6 +1648,23 @@ int gofr_http_parse_device(gofr_engine* e, const uint8_t* d_raw, const uint32_t*
     p.desc = d_desc; p.arena = d_arena; p.status = d_status; p.spans = (unsigned long long*)d_spans;
     // no look-back: every message's result lands in the bytes it occupies, so the whole resident grid runs
     return launch(e, K_HTTP, (int)std::min<uint32_t>((uint32_t)resident, p.n_tiles), 0, (cudaStream_t)stream, p);
+}
+
+int gofr_http_frame_device(gofr_engine* e, const uint8_t* d_buf, const uint32_t* d_buf_off, uint32_t n_conns, uint32_t* d_rec_off,
+                           uint32_t rec_cap, uint32_t* d_first, uint32_t* d_consumed, uint32_t* d_conn_status, void* stream) {
+    if (!e) return GOFR_ERR_INVALID;
+    if (n_conns == 0) return GOFR_OK;
+    if (!d_buf || !d_buf_off || !d_rec_off || !d_first || !d_consumed || !d_conn_status) return GOFR_ERR_INVALID;
+    if (((uintptr_t)d_buf & 15u) || (((uintptr_t)d_buf_off | (uintptr_t)d_rec_off | (uintptr_t)d_first | (uintptr_t)d_consumed |
+                                      (uintptr_t)d_conn_status) & 3u)) {
+        set_last_error("d_buf must be 16-byte aligned and the offset, record and per-connection columns 4-byte aligned");
+        return GOFR_ERR_INVALID;
+    }
+    HttpFrameParams p;
+    memset(&p, 0, sizeof p);
+    p.buf = d_buf; p.buf_off = d_buf_off; p.consumed = d_consumed; p.status = d_conn_status;
+    // the record column is the packed output (rec_cap records), d_first its offset column
+    return launch_frames(e, K_HTTP_FRAME, p, n_conns, (uint8_t*)d_rec_off, rec_cap, d_first, stream);
 }
 
 int gofr_requestlog_device(gofr_engine* e, const gofr_log_desc* d_desc, const uint8_t* d_trace_ids, const uint8_t* d_arena,

@@ -227,6 +227,22 @@ struct HttpParams {
     unsigned long long* spans;  // n * GOFR_HTTP_SPANS
 };
 
+// http_frame_kernel.cu: a packed-output kernel whose output is the record column (words, not bytes)
+struct HttpFrameParams {
+    const uint8_t* buf;
+    const uint32_t* buf_off;  // n + 1
+    uint32_t n;               // connections
+    uint32_t n_tiles;
+    uint32_t epoch;
+    uint8_t* out;             // d_rec_off: out_cap + 1 words
+    uint64_t out_cap;         // records
+    uint32_t* out_off;        // d_first: n + 1
+    uint32_t* consumed;       // n
+    uint32_t* status;         // n
+    unsigned long long* tile_state;
+    uint32_t* overflow;
+};
+
 struct LogParams {
     const void* desc;   // gofr_log_desc[n]
     const void* ids;    // n * 16 trace id bytes

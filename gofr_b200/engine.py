@@ -323,11 +323,42 @@ class Engine:
         n = len(raw_off) - 1
         d_raw = torch.from_numpy(np.concatenate([raw, np.zeros(32, dtype=np.uint8)])).to(dev)
         d_off = torch.from_numpy(raw_off.astype(np.uint32).view(np.int32)).to(dev)
+        return self.http_parse_resident(d_raw, d_off, n, stream)
+
+    def http_frame_device(self, buf: np.ndarray, buf_off: np.ndarray, rec_cap: Optional[int] = None, stream=None):
+        """gofr_http_frame_device on host arrays (uploaded here): connection c's received bytes are
+        buf[buf_off[c]:buf_off[c+1]].  Returns torch tensors (d_buf uint8 with its slack, rec_off int32[rec_cap+1],
+        first int32[n+1], consumed int32[n], status int32[n]); first[n] is the record count, and (d_buf, rec_off, first[n])
+        goes to http_parse_resident as it is.  rec_cap defaults to what always suffices: the shortest request of the subset is
+        longer than 16 bytes, and a connection has at most one tail record."""
+        import torch
+        dev = torch.device("cuda", self.device)
+        st = stream if stream is not None else torch.cuda.current_stream(self.device)
+        n = len(buf_off) - 1
+        if rec_cap is None:
+            rec_cap = int(buf.size) // 16 + n + 1
+        d_buf = torch.from_numpy(np.concatenate([buf, np.zeros(32, dtype=np.uint8)])).to(dev)
+        d_off = torch.from_numpy(np.ascontiguousarray(buf_off, dtype=np.uint32).view(np.int32)).to(dev)
+        rec_off = torch.zeros(rec_cap + 1, dtype=torch.int32, device=dev)
+        first = torch.zeros(n + 1, dtype=torch.int32, device=dev)
+        consumed = torch.zeros(max(n, 1), dtype=torch.int32, device=dev)
+        status = torch.zeros(max(n, 1), dtype=torch.int32, device=dev)
+        _abi.check(_abi.lib().gofr_http_frame_device(self._e, d_buf.data_ptr(), d_off.data_ptr(), n, rec_off.data_ptr(), rec_cap,
+                                                     first.data_ptr(), consumed.data_ptr(), status.data_ptr(), st.cuda_stream),
+                   "gofr_http_frame_device")
+        return d_buf, rec_off, first, consumed[:n], status[:n]
+
+    def http_parse_resident(self, d_raw, d_raw_off, n: int, stream=None):
+        """gofr_http_parse_device on tensors already in HBM (d_raw with 16 bytes of slack, d_raw_off int32[n+1]): returns
+        (desc uint8[n*16], arena uint8, status int32[n], spans int64[n, 6])."""
+        import torch
+        dev = torch.device("cuda", self.device)
+        st = stream if stream is not None else torch.cuda.current_stream(self.device)
         desc = torch.zeros(max(n, 1) * 16, dtype=torch.uint8, device=dev)
-        arena = torch.zeros(int(raw.size) + 48, dtype=torch.uint8, device=dev)
+        arena = torch.zeros(int(d_raw.numel()) + 16, dtype=torch.uint8, device=dev)
         status = torch.zeros(max(n, 1), dtype=torch.int32, device=dev)
         spans = torch.zeros((max(n, 1), 6), dtype=torch.int64, device=dev)
-        _abi.check(_abi.lib().gofr_http_parse_device(self._e, d_raw.data_ptr(), d_off.data_ptr(), n, desc.data_ptr(),
+        _abi.check(_abi.lib().gofr_http_parse_device(self._e, d_raw.data_ptr(), d_raw_off.data_ptr(), n, desc.data_ptr(),
                                                      arena.data_ptr(), status.data_ptr(), spans.data_ptr(), st.cuda_stream),
                    "gofr_http_parse_device")
         return desc[:n * 16], arena, status[:n], spans[:n]

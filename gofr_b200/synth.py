@@ -384,3 +384,32 @@ def http_messages(n: int, start: int = 0, seed: int = SEED, n_routes: int = 16, 
     raw = np.frombuffer(b"".join(msgs), dtype=np.uint8).copy()
     off = np.cumsum([0] + [len(m) for m in msgs]).astype(np.uint32)
     return raw, off
+
+
+def http_streams(n_conns: int, seed: int = SEED, reqs=(0, 5), tail_every: int = 0, defer_every: int = 0, seed_msgs=None):
+    """n_conns connection receive buffers back to back: (buf uint8, buf_off uint32[n_conns+1]).  The http_messages stream cut
+    into connections of reqs[0]..reqs[1] requests each (seeded).  tail_every: every such connection ends with the first part
+    of one more request, cut at a seeded byte; defer_every: every such connection gets a request outside the subset at a
+    seeded place among its own.  seed_msgs: as in http_messages."""
+    r = rand_u64(seed, np.arange(n_conns, dtype=np.uint64), 22)
+    counts = (reqs[0] + r % np.uint64(reqs[1] - reqs[0] + 1)).astype(np.int64)
+    starts = np.concatenate([[0], np.cumsum(counts)])
+    total = int(starts[-1])
+    raw, off = http_messages(total + 1, seed=seed, seed_msgs=seed_msgs)
+    rawb = raw.tobytes()
+    if not tail_every and not defer_every:   # whole messages only: the connections are slices of the stream as it is
+        return raw[:int(off[total])].copy(), off[starts].astype(np.uint32)
+    old = b"GET /legacy HTTP/1.0\r\nHost: api.example.com\r\n\r\n"
+    conns = []
+    for c in range(n_conns):
+        a = int(r[c]) >> 8
+        lo, hi = int(starts[c]), int(starts[c + 1])
+        parts = [rawb[int(off[k]):int(off[k + 1])] for k in range(lo, hi)]
+        if defer_every and c % defer_every == defer_every // 2:
+            parts.insert(a % (len(parts) + 1), old)
+        if tail_every and c % tail_every == tail_every - 1:
+            nxt = rawb[int(off[hi]):int(off[hi + 1])]
+            parts.append(nxt[:1 + (a >> 8) % (len(nxt) - 1)])
+        conns.append(b"".join(parts))
+    buf = np.frombuffer(b"".join(conns), dtype=np.uint8).copy()
+    return buf, np.cumsum([0] + [len(x) for x in conns]).astype(np.uint32)

@@ -668,7 +668,8 @@ int gofr_proto_frontend_call(gofr_proto_frontend*, const uint8_t* in, uint32_t i
 /* HTTP/1.1 request heads (SURVEY.md §8f rank 2): what net/http's readRequest + url.ParseRequestURI hand to
  * Router.ServeHTTP, for a batch of raw request messages resident in HBM, in the layout the serve calls consume.
  *   d_raw / d_raw_off: message i = d_raw[d_raw_off[i] .. d_raw_off[i+1]) — exactly one request (head + body) as framed
- *                      by the connection reader; d_raw needs 16 readable bytes after the last message.
+ *                      by the connection reader (gofr_http_frame_device below is one: its record column is a d_raw_off);
+ *                      d_raw needs 16 readable bytes after the last message.
  *   d_status[i]      : GOFR_HTTP_OK, or GOFR_HTTP_DEFER = "not in the subset below: parse it on the host" (nothing is
  *                      claimed about such a message — it may be perfectly valid).  Never a different answer.
  *   d_desc[i], d_arena: for OK messages the gofr_req_desc and its bytes (decoded URL.Path | URL.RawQuery | pad4 | body) at
@@ -691,6 +692,40 @@ enum { GOFR_HTTP_SPAN_METHOD = 0, GOFR_HTTP_SPAN_TARGET = 1, GOFR_HTTP_SPAN_USER
        GOFR_HTTP_SPAN_HOST = 4, GOFR_HTTP_SPAN_BODY = 5, GOFR_HTTP_SPANS = 6 };
 int gofr_http_parse_device(gofr_engine*, const uint8_t* d_raw, const uint32_t* d_raw_off, uint32_t n, gofr_req_desc* d_desc,
                            uint8_t* d_arena, uint32_t* d_status, uint64_t* d_spans, void* stream);
+
+/* Connection byte streams → request messages: the connection reader in front of gofr_http_parse_device (net/http's
+ * conn.serve looping readRequest over one bufio.Reader).  A receive buffer holds zero, one or several requests (HTTP/1.1
+ * pipelining, or two requests that arrived in one read), then nothing or the first part of the next request.
+ *   d_buf / d_buf_off: connection c's received bytes = d_buf[d_buf_off[c] .. d_buf_off[c+1]), back to back; d_buf is 16-byte
+ *                      aligned with 16 readable bytes after the last connection (the same buffer is then passed on as d_raw).
+ *   d_rec_off        : a record column that TILES the buffer: d_rec_off[0 .. total], ascending, d_rec_off[0] = d_buf_off[0],
+ *                      d_rec_off[total] = d_buf_off[n_conns].  A connection's records are its whole requests in order, then
+ *                      — only when bytes are left over — one TAIL record with the rest of its buffer.  Records have no gaps,
+ *                      so (d_buf, d_rec_off, total) is a valid (d_raw, d_raw_off, n) of gofr_http_parse_device.
+ *   d_first          : n_conns + 1 entries; connection c owns records d_first[c] .. d_first[c+1]); d_first[n_conns] = total.
+ *   d_consumed[c]    : bytes of the connection covered by whole requests (= the tail's offset in the connection, or the
+ *                      connection's length when there is no tail).
+ *   d_conn_status[c] : GOFR_HTTP_CONN_DONE  every byte belongs to a whole request; no tail (an empty buffer: no records);
+ *                      GOFR_HTTP_CONN_MORE  the last record is a tail that can still become a request of the subset: keep
+ *                                           those bytes and append the next read;
+ *                      GOFR_HTTP_CONN_DEFER the last record is a tail the subset excludes already (HTTP/1.0, a control byte
+ *                                           in a header value, Connection: close, ...): hand the connection's bytes from
+ *                                           d_consumed[c] on to net/http.  The framer never resumes behind such a request:
+ *                                           where the next one starts is only known when this one's framing is.
+ *                      Bytes are judged as they arrive, header lines when they are complete (their CRLF is there).
+ *   rec_cap          : d_rec_off has rec_cap + 1 entries.  One record per 16 buffer bytes plus one per connection always
+ *                      suffices (the shortest request of the subset is longer).  When total > rec_cap the call behaves like
+ *                      the packed-output calls: gofr_engine_overflowed reports it, d_first is still written in full
+ *                      (d_first[n_conns] = the capacity needed), records are dropped by whole tiles of 128 connections and
+ *                      no entry at or past rec_cap + 1 is written.
+ * What makes the column safe to pass on: every non-tail record, given alone to gofr_http_parse_device, is GOFR_HTTP_OK, and
+ * every tail record is GOFR_HTTP_DEFER (a zero descriptor) — the host skips the last record of a MORE / DEFER connection.
+ * Conversely a message gofr_http_parse_device accepts, followed by anything, is cut at its own length.
+ * n_conns == 0 touches no buffer.  GOFR_ERR_INVALID: a null argument, d_buf not 16-byte aligned, a column not 4-byte aligned. */
+enum { GOFR_HTTP_CONN_DONE = 0, GOFR_HTTP_CONN_MORE = 1, GOFR_HTTP_CONN_DEFER = 2 };
+int gofr_http_frame_device(gofr_engine*, const uint8_t* d_buf, const uint32_t* d_buf_off, uint32_t n_conns,
+                           uint32_t* d_rec_off, uint32_t rec_cap, uint32_t* d_first, uint32_t* d_consumed,
+                           uint32_t* d_conn_status, void* stream);
 
 /* number of kernels launched by this engine so far (bench.py reports it as gpu_launches) */
 uint64_t gofr_engine_launch_count(const gofr_engine*);
