@@ -15,9 +15,9 @@
 //     with a decoupled look-back (single pass — inputs are read from HBM exactly once);
 //   * each thread streams its response through a funnel-shift word writer (serve_device.cuh) whose completed words
 //     collect in a conflict-free shared-memory ring and leave for HBM as whole 32-byte sectors, two 16-byte
-//     st.global.cs.v4 each; in the slot layout's fast path lane pairs share those stores, so every warp store
-//     covers whole sectors (the PairStores store policy).  No output tile lives in shared
-//     memory, which keeps 5 CTAs (20 warps) resident per SM for this latency-bound byte work.
+//     st.global.cs.v4 each; in the wide slot instance's fast path they leave as whole 128-byte lines, four lines per
+//     warp store (the LineStores store policy).  No output tile lives in shared memory, which keeps 5 CTAs (20 warps)
+//     resident per SM for this latency-bound byte work.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -36,6 +36,9 @@ constexpr int NW = T / 32;
 
 constexpr uint32_t kDeferred = 0xFFFFFFFFu;  // length-column mark of a request left for the general pass (never a length)
 
+// RING: words of the Writer's staging ring — GOFR_SOLO_WORDS rows of T for SoloStores; the wide slot instance's
+// LineStores columns need GOFR_LINE_WORDS rows of T + 1 (serve_device.cuh).  Only that instance has the larger ring.
+template <uint32_t RING>
 struct TileShared {
     uint64_t bar;  // mbarrier for the arena bulk load
     uint32_t warp_sum[NW];
@@ -46,8 +49,10 @@ struct TileShared {
     uint32_t defer_n;         // slot layout: requests waiting for the general pass; their indices (at most 2 T: one tile's
                               // worth is added between two checks) live in the request staging area, which is idle once
                               // the tile loop is over — as static shared memory the list cost every instance its fifth CTA
-    uint32_t ring[GOFR_STAGE_WORDS * T];  // word-major staging buffer of the Writer (serve_device.cuh)
+    uint32_t ring[RING];  // word-major staging buffer of the Writer (serve_device.cuh)
 };
+constexpr uint32_t kSoloRing = GOFR_SOLO_WORDS * T, kLineRing = GOFR_LINE_WORDS * (T + 1);
+static_assert(LineStores::kRowWords == T + 1, "LineStores rows are T + 1 words");
 
 // Slot layout, general pass.  The tile loop of serve_slots_kernel runs only the fast path (size_fast / emit_fast); a request
 // it cannot take — a program outside the fast path, a value that needs escaping or decoding, HEAD, an unstaged tile — is
@@ -57,7 +62,8 @@ struct TileShared {
 // the other three wait for it at the next barrier (barrier stall 5.5 cycles per issue on the 64-route workload).  The
 // request bytes are read from HBM here (the tile that staged them is gone); the code is out of line so that the tile loop
 // keeps its registers and its instruction-cache footprint.
-static __device__ __noinline__ void general_pass(const ServeParams* pp, const TableView tv, const BatchRefs br, TileShared* sh,
+template <class TS>
+static __device__ __noinline__ void general_pass(const ServeParams* pp, const TableView tv, const BatchRefs br, TS* sh,
                                           const uint32_t* defer, uint32_t first, uint32_t count) {
     const ServeParams& p = *pp;
     const uint32_t tid = threadIdx.x;
@@ -74,15 +80,16 @@ static __device__ __noinline__ void general_pass(const ServeParams* pp, const Ta
         emit_request_general<true>(tv, br, c, p.out + (size_t)r * p.slot_bytes, &sh->ring[tid]);
 }
 
-// PAIRS (slot layout): the fast path stores sectors in lane pairs (emit_fast with PairStores).  Its store rounds are
-// warp-uniform, so a warp whose lanes run different programs makes every lane take every other lane's rounds: on mixed
-// traffic (config 4: 0.31 -> 0.35 ms on an H100 SXM at 400 W) that costs more than whole-sector stores gain.  Only the
-// wide instance, which the engine runs for tables with one fast-path program shape, pairs.
-template <bool SLOTS, bool PAIRS = false>
+// LINES (slot layout): the fast path stores whole 128-byte lines (emit_fast with LineStores).  Its votes and store rounds
+// are warp-uniform, so a warp whose lanes run different programs makes every lane take part in every other lane's: on
+// mixed traffic that costs more than whole lines gain (lane pairs, the earlier warp-uniform policy, took config 4 from
+// 0.31 to 0.35 ms on an H100 SXM at 400 W).  Only the wide instance, which the engine runs for tables with one fast-path
+// program shape, stores lines; it alone carries the larger staging ring.
+template <bool SLOTS, bool LINES = false>
 __device__ __forceinline__ void serve_body(const ServeParams& p) {
     // (p is a __grid_constant__ kernel parameter: its address can be handed to the out-of-line general pass)
     extern __shared__ __align__(128) uint8_t smem[];
-    __shared__ __align__(16) TileShared sh;
+    __shared__ __align__(16) TileShared<LINES ? kLineRing : kSoloRing> sh;
 
     const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     uint8_t* tbl = smem;
@@ -194,17 +201,17 @@ __device__ __forceinline__ void serve_body(const ServeParams& p) {
                     p.out_off[r] = c.total_len;  // the length column; > slot_bytes tells the host the slot was too small
                     p.meta[r] = request_status(tv, c) | (c.route << 16);
                     if (c.total_len <= p.slot_bytes && c.total_len) {
-                        if (PAIRS) emit = true;
+                        if (LINES) emit = true;
                         else emit_fast(tv, br, c, p.out + (size_t)r * p.slot_bytes, &sh.ring[tid], SoloStores{});
                     }
                 } else {
                     p.out_off[r] = kDeferred;  // left for the general pass after the tile loop
                 }
             }
-            if (PAIRS) {
-                // every thread of the CTA is here: the lanes that write a response form the pair mask
-                const uint32_t pm = __ballot_sync(0xFFFFFFFFu, emit);
-                if (emit) emit_fast(tv, br, c, p.out + (size_t)r * p.slot_bytes, &sh.ring[tid], PairStores{pm});
+            if (LINES) {
+                // every thread of the CTA is here, and every lane of a warp runs the store rounds (eight lanes per line):
+                // a lane without a response to write runs an empty one
+                emit_fast(tv, br, c, emit ? p.out + (size_t)r * p.slot_bytes : p.out, &sh.ring[tid], LineStores{}, emit);
             }
             continue;
         }

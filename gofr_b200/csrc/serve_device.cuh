@@ -89,11 +89,11 @@ GOFR_HD bool warp_any(bool p) {
 // st.global.cs.v4.  When one lane issues both, a warp store touches 32 sectors 528 bytes apart (the config-2 slots) and
 // fills half of each.  Storing 1 Mi such slots and nothing else, at full occupancy (scratch/experiments/sector_stores,
 // H100 SXM at 400 W; the times rank store patterns, they are not the serve kernel's store cost), took 1.82 ms.  How
-// sectors leave is the store policy the caller passes to flush, copy and finish_padded (below): SoloStores, the default,
-// stores each lane's sector as two back-to-back halves; with PairStores (the fast path of the wide slot-layout instance,
-// serve_body.cuh PAIRS) lanes 2k and 2k+1 share both stores: the first writes the even lane's sector, the second the
-// odd lane's, each lane one half of each, and every warp store covers 16 whole sectors (0.60 ms for the same slots;
-// fully coalesced rows 0.17 ms).
+// bytes leave is the store policy the Writer is instantiated with (below): SoloStores, the default, stores each lane's
+// sector as two back-to-back halves; LineStores (the fast path of the wide slot-layout instance, serve_body.cuh LINES)
+// makes the destination alignment a 128-byte line and stores the complete lines of the warp's lanes four per warp store,
+// eight lanes per line (0.333 ms for the same slots; lane pairs on 16 whole sectors per warp store 0.599 ms, fully
+// coalesced rows 0.175 ms; H100 SXM at 700 W).
 //
 // Each thread owns a 16-word staging buffer in shared memory, laid out word-major (word k of thread t at
 // [k * CTA + t]): whatever word index a lane is at, its bank is its lane id, so accesses never conflict.  The buffer is
@@ -104,19 +104,32 @@ GOFR_HD bool warp_any(bool p) {
 //            bytes treated as a prefix of the source ("virtual source"): one aligned load + one funnel shift per
 //            output word regardless of source and destination alignment.
 //   flush:   decoupled from producing — between ops, when at least 8 words wait, whole sectors leave as
-//            8 conflict-free LDS + two st.global.cs.v4 (PairStores: shared by a lane pair as above); no shifting
-//            is needed because the buffer is already aligned.
+//            8 conflict-free LDS + two st.global.cs.v4; no shifting is needed because the buffer is already aligned.
 //   edges:   the first sector's leading `lead` bytes and the last sector's tail belong to neighbouring responses
 //            written by other threads; only this response's bytes are stored there.
+// With LineStores the column holds one 128-byte line plus what is appended before the next flush vote (39 words), and
+// its rows are T + 1 words apart: word k of thread t at [k * (T + 1) + t], so the bank of a word is (k + t) mod 32.
+// Appends of one word index by the lanes of a warp stay conflict-free, and the eight lanes that load the eight 16-byte
+// windows of one line (words 4w + j, w = 0..7) hit eight different banks (line_store_bank, tests/emu).
 // ---------------------------------------------------------------------------------------------------------------
 #if defined(__CUDA_ARCH__)
 #ifndef GOFR_RING_STRIDE_BYTES
 #define GOFR_RING_STRIDE_BYTES 512u  /* word-major staging: one word of every thread that shares the buffer per row */
 #endif
+#define GOFR_LINE_STRIDE_BYTES 516u  /* LineStores: one padding word per row */
 #else
 #define GOFR_RING_STRIDE_BYTES 4u
+#define GOFR_LINE_STRIDE_BYTES 4u
 #endif
-#define GOFR_STAGE_WORDS 16u
+#define GOFR_SOLO_WORDS 16u  /* SoloStores column */
+#define GOFR_LINE_WORDS 39u  /* LineStores column: < 32 words before an append of at most 8 */
+// Words a caller's staging column must hold.  Device kernels stage only with SoloStores (the wide slot instance sizes its
+// LineStores ring itself, serve_body.cuh); the host emulation (tests/emu) runs both policies through one column.
+#if defined(__CUDACC__)
+#define GOFR_STAGE_WORDS GOFR_SOLO_WORDS
+#else
+#define GOFR_STAGE_WORDS GOFR_LINE_WORDS
+#endif
 
 // ---- explicit address spaces -------------------------------------------------------------------------------------
 // The staging buffer, the table's literal pool and (for staged tiles) the request bytes all live in shared memory.
@@ -202,85 +215,112 @@ GOFR_HD void store16(uint8_t* addr, uint32_t v0, uint32_t v1, uint32_t v2, uint3
 #endif
 }
 
-// Store policies of the Writer's flush, copy and finish_padded, and of emit_fast: how the lanes that run them take a flush
-// decision (vote), how long a store round runs (round: while the lane, or its group, has something to store), and how
-// a whole 32-byte sector leaves (store32: the sector v0..v7 at the 32-byte aligned addr, if `have`).  kLockstep: every
-// lane of the group makes every call of these routines together, also with nothing to store.
+// Store policies of the Writer: its staging geometry (kStride: bytes between the rows of the column, kWords: words a
+// column holds, kLine: the destination alignment in bytes) and how the lanes that run flush, copy and finish_padded take
+// a flush decision (vote) and how long a loop over the group runs (round).  kLockstep: every lane of the group makes
+// every call of these routines together, also with nothing to store.
 //
-// SoloStores: each lane on its own, its sector as two back-to-back 16-byte stores; a flush decision is taken by all
-// active lanes of the warp.
+// SoloStores: each lane on its own, its 32-byte sector as two back-to-back 16-byte stores; a flush decision is taken by
+// all active lanes of the warp.
 struct SoloStores {
     static constexpr bool kLockstep = false;
+    static constexpr uint32_t kStride = GOFR_RING_STRIDE_BYTES, kWords = GOFR_SOLO_WORDS, kLine = 32;
     GOFR_HD bool vote(bool p) const { return warp_any(p); }
     GOFR_HD bool round(bool have) const { return have; }
+    // the sector v0..v7 at the 32-byte aligned addr, if `have`
     GOFR_HD void store32(bool have, uint8_t* addr, uint32_t v0, uint32_t v1, uint32_t v2, uint32_t v3, uint32_t v4,
                          uint32_t v5, uint32_t v6, uint32_t v7) const {
         if (have) { store16(addr, v0, v1, v2, v3); store16(addr + 16, v4, v5, v6, v7); }
     }
 };
-// PairStores: the lanes of the pair mask pm take every decision and run every round together, while any of them still
-// has something to store (a lane with nothing takes part with `have` false).  When lanes 2k and 2k+1 both have a
-// sector, they write them together: in each of the two 16-byte stores the even lane writes the lower and the odd lane
-// the upper half of one sector (first the even lane's, then the odd lane's), so each warp store covers whole sectors.  A
-// lane whose partner has no sector writes both halves of its own.  On the host (tests/emu) lanes run one at a time: pm
-// is ignored, and the vote is warp_any's so that the emulation replays extra flushes here too.
-struct PairStores {
-    uint32_t pm;
+// LineStores (slot layout only: every response starts 16-byte aligned): all 32 lanes of the warp take every decision
+// and run every round together — a line needs eight lanes, so a lane with no response to write takes part with an empty
+// one (emit_fast, live false).  A flush stores the complete 128-byte lines of all of them in rounds of four: lane group
+// g = lane >> 3 takes the g-th remaining lane with a line, and lane t = lane & 7 loads window t of that lane's column and
+// stores it, so one warp store is four aligned lines.  `wins` (bit w: window w) says which windows of a line belong to
+// the response: the first line skips the previous slot's, the last one ends at the zero-padded end.  On the host
+// (tests/emu) lanes run one at a time: a lane stores its own line, and the vote is warp_any's so that the emulation
+// replays extra flushes here too.
+struct LineStores {
+    static constexpr uint32_t wm = 0xFFFFFFFFu;
     static constexpr bool kLockstep = true;
+    static constexpr uint32_t kStride = GOFR_LINE_STRIDE_BYTES, kWords = GOFR_LINE_WORDS, kLine = 128;
+    static constexpr uint32_t kRowWords = 129;  // T + 1 (serve_body.cuh): the device row of the column
     GOFR_HD bool vote(bool p) const {
 #if defined(__CUDA_ARCH__)
-        return __any_sync(pm, p);
+        return __any_sync(wm, p);
 #else
         return warp_any(p);
 #endif
     }
     GOFR_HD bool round(bool have) const {
 #if defined(__CUDA_ARCH__)
-        return __any_sync(pm, have);
+        return __any_sync(wm, have);
 #else
         return have;
 #endif
     }
-    GOFR_HD void store32(bool have, uint8_t* addr, uint32_t v0, uint32_t v1, uint32_t v2, uint32_t v3, uint32_t v4,
-                         uint32_t v5, uint32_t v6, uint32_t v7) const {
-        uint8_t* a0 = addr;
-        uint8_t* a1 = addr + 16;
+    // ring word that holds word j of window w of the column of thread s
+    GOFR_HD static uint32_t window_word(uint32_t s, uint32_t w, uint32_t j) { return (4u * w + j) * kRowWords + s; }
+    // store windows `wins` of the line at `line` (128-byte aligned) from the column at col
+    GOFR_HD void lines(uint8_t* line, saddr_t col, uint32_t wins) const {
 #if defined(__CUDA_ARCH__)
-        {
-            const uint32_t lane = threadIdx.x & 31u, odd = lane & 1u;
-            const uint32_t haves = __ballot_sync(pm, have);  // by every lane of pm: not behind a short-circuit on `have`
-            const bool pair = have && ((haves >> (lane ^ 1u)) & 1u);
-            // the half the partner writes: the even lane's upper half, the odd lane's lower half
-            const uint32_t x0 = __shfl_xor_sync(pm, odd ? v0 : v4, 1), x1 = __shfl_xor_sync(pm, odd ? v1 : v5, 1);
-            const uint32_t x2 = __shfl_xor_sync(pm, odd ? v2 : v6, 1), x3 = __shfl_xor_sync(pm, odd ? v3 : v7, 1);
-            uint8_t* const pa = (uint8_t*)__shfl_xor_sync(pm, (unsigned long long)addr, 1);
-            if (pair && odd) { a0 = pa + 16; v0 = x0; v1 = x1; v2 = x2; v3 = x3; }
-            if (pair && !odd) { a1 = pa; v4 = x0; v5 = x1; v6 = x2; v7 = x3; }
-        }
+        const uint32_t lane = threadIdx.x & 31u, g = lane >> 3, t = lane & 7u;
+        uint32_t rem = __ballot_sync(wm, wins != 0u);
+        if (!rem) return;
+        __syncwarp(wm);  // the owners' column stores before the other lanes' loads
+        do {
+            const uint32_t m1 = rem & (rem - 1u), m2 = m1 & (m1 - 1u), m3 = m2 & (m2 - 1u);
+            const uint32_t sel = g == 0 ? rem : g == 1 ? m1 : g == 2 ? m2 : m3;
+            const uint32_t s = sel ? __ffs(sel) - 1u : lane;
+            uint8_t* const a = (uint8_t*)__shfl_sync(wm, (unsigned long long)line, s);
+            const uint32_t ws = __shfl_sync(wm, wins, s);
+            if (sel && ((ws >> t) & 1u)) {
+                const saddr_t rp = col + 4u * (window_word(s, t, 0) - lane);
+                store16(a + 16u * t, stg_ld(rp), stg_ld(rp + kStride), stg_ld(rp + 2u * kStride), stg_ld(rp + 3u * kStride));
+            }
+            rem = m3 & (m3 - 1u);
+        } while (rem);
+        __syncwarp(wm);  // every load of a column before its owner moves or overwrites words in it
+#else
+        for (uint32_t t = 0; t < 8; t++)
+            if ((wins >> t) & 1u) {
+                const saddr_t rp = col + 4u * t * kStride;
+                store16(line + 16u * t, stg_ld(rp), stg_ld(rp + kStride), stg_ld(rp + 2u * kStride), stg_ld(rp + 3u * kStride));
+            }
 #endif
-        if (have) { store16(a0, v0, v1, v2, v3); store16(a1, v4, v5, v6, v7); }
     }
 };
 
-struct Writer {
-    uint8_t* chunk;  // 32-byte aligned global address that staging word 0 maps to
+#if !defined(__CUDACC__)
+// The host emulation (tests/emu) selects the wide instance's policy by the name of the lane-pair policy LineStores
+// replaced, with that policy's lane mask, which lines do not use.
+struct PairStores : LineStores {
+    explicit PairStores(uint32_t) {}
+};
+#endif
+
+template <typename P>
+struct WriterT {
+    static constexpr uint32_t kStride = P::kStride, kWords = P::kWords, kLine = P::kLine;
+    uint8_t* chunk;  // kLine-aligned global address that staging word 0 maps to
     saddr_t base;    // this thread's column of the staging buffer
     saddr_t wp;      // base + wl * stride: where the next complete word goes
-    uint32_t wl;     // complete words staged (0 .. GOFR_STAGE_WORDS)
+    uint32_t wl;     // complete words staged (0 .. kWords)
     uint32_t pend, nb;
-    uint32_t lead;   // bytes at the start of the first sector owned by the previous response(s)
+    uint32_t lead;   // bytes at the start of the first sector (line) owned by the previous response(s)
 
     GOFR_HD void init(uint8_t* dst, uint32_t* col) {
         uintptr_t x = (uintptr_t)dst;
-        chunk = (uint8_t*)(x & ~(uintptr_t)31);
-        lead = (uint32_t)(x & 31);
+        chunk = (uint8_t*)(x & ~(uintptr_t)(kLine - 1));
+        lead = (uint32_t)(x & (kLine - 1));
         wl = lead >> 2;  // phantom words of the neighbour: never stored
         nb = lead & 3;
         base = to_saddr(col);
-        wp = base + wl * GOFR_RING_STRIDE_BYTES;
+        wp = base + wl * kStride;
         pend = 0;
     }
-    GOFR_HD uint32_t word(uint32_t k) const { return stg_ld(base + k * GOFR_RING_STRIDE_BYTES); }
+    GOFR_HD uint32_t word(uint32_t k) const { return stg_ld(base + k * kStride); }
 
     // Write bytes [lo, hi) of the 32-byte sector at addr from the eight staging words at rp: a 16-byte half where one is
     // whole, else words, else single bytes.  Runs twice per response at most (first and last sector), so it is a loop,
@@ -290,64 +330,79 @@ struct Writer {
     GOFR_HD static void store_partial(uint8_t* addr, saddr_t rp, uint32_t lo, uint32_t hi) {
         uint32_t b = lo;
 #pragma unroll 1
-        for (; b < hi && (b & 3u); b++) st8(addr + b, stg_ld8(rp + (b >> 2) * GOFR_RING_STRIDE_BYTES + (b & 3u)));
+        for (; b < hi && (b & 3u); b++) st8(addr + b, stg_ld8(rp + (b >> 2) * kStride + (b & 3u)));
 #pragma unroll 1
-        for (; b + 4 <= hi && (b & 15u); b += 4) st32(addr + b, stg_ld(rp + (b >> 2) * GOFR_RING_STRIDE_BYTES));
+        for (; b + 4 <= hi && (b & 15u); b += 4) st32(addr + b, stg_ld(rp + (b >> 2) * kStride));
 #pragma unroll 1
         for (; b + 16 <= hi; b += 16) {
-            const saddr_t q = rp + (b >> 2) * GOFR_RING_STRIDE_BYTES;
-            store16(addr + b, stg_ld(q), stg_ld(q + GOFR_RING_STRIDE_BYTES), stg_ld(q + 2 * GOFR_RING_STRIDE_BYTES),
-                    stg_ld(q + 3 * GOFR_RING_STRIDE_BYTES));
+            const saddr_t q = rp + (b >> 2) * kStride;
+            store16(addr + b, stg_ld(q), stg_ld(q + kStride), stg_ld(q + 2 * kStride),
+                    stg_ld(q + 3 * kStride));
         }
 #pragma unroll 1
-        for (; b + 4 <= hi; b += 4) st32(addr + b, stg_ld(rp + (b >> 2) * GOFR_RING_STRIDE_BYTES));
+        for (; b + 4 <= hi; b += 4) st32(addr + b, stg_ld(rp + (b >> 2) * kStride));
 #pragma unroll 1
-        for (; b < hi; b++) st8(addr + b, stg_ld8(rp + (b >> 2) * GOFR_RING_STRIDE_BYTES + (b & 3u)));
+        for (; b < hi; b++) st8(addr + b, stg_ld8(rp + (b >> 2) * kStride + (b & 3u)));
     }
-    // store every complete sector, move the (< 8) left-over words to the front
-    template <typename P = SoloStores>
+    // store every complete sector (LineStores: line), move the (< 8) left-over words to the front
     GOFR_HD void flush(P p = P()) {
-        uint32_t n = wl >> 3;
-        saddr_t rp = base;
-        if (n && lead) {  // first sector of the response: skip the neighbour's bytes
-            store_partial(chunk, rp, lead, 32);
-            lead = 0;
-            chunk += 32;
-            rp += 8 * GOFR_RING_STRIDE_BYTES;
-            n--;
-        }
-#pragma unroll 1
-        while (p.round(n != 0)) {
-            const bool have = n != 0;
-            uint8_t* const at = chunk;
-            uint32_t v[8] = {0u, 0u, 0u, 0u, 0u, 0u, 0u, 0u};
-            if (have) {  // a lane without a sector may be at the end of its column: it reads nothing
+        if constexpr (P::kLockstep) {
+            // a line is complete at 32 words; a column holds fewer than 40, so there is at most one
+            const bool full = wl >= 32u;
+            p.lines(chunk, base, full ? (0xFFu << (lead >> 4)) & 0xFFu : 0u);
+            if (full) {
+                const uint32_t r = wl - 32u;
 #pragma unroll
-                for (uint32_t j = 0; j < 8; j++) v[j] = stg_ld(rp + j * GOFR_RING_STRIDE_BYTES);
+                for (uint32_t j = 0; j < 7; j++)
+                    if (r > j) stg_st(base + j * kStride, stg_ld(base + (32u + j) * kStride));
+                wl = r;
+                wp = base + r * kStride;
+                chunk += 128;
+                lead = 0;
             }
-            p.store32(have, at, v[0], v[1], v[2], v[3], v[4], v[5], v[6], v[7]);
-            if (have) {
+        } else {
+            uint32_t n = wl >> 3;
+            saddr_t rp = base;
+            if (n && lead) {  // first sector of the response: skip the neighbour's bytes
+                store_partial(chunk, rp, lead, 32);
+                lead = 0;
                 chunk += 32;
-                rp += 8 * GOFR_RING_STRIDE_BYTES;
+                rp += 8 * kStride;
                 n--;
             }
-        }
-        const uint32_t r = wl & 7;
-        if (wl >= 8 && r) {
+#pragma unroll 1
+            while (p.round(n != 0)) {
+                const bool have = n != 0;
+                uint8_t* const at = chunk;
+                uint32_t v[8] = {0u, 0u, 0u, 0u, 0u, 0u, 0u, 0u};
+                if (have) {
 #pragma unroll
-            for (uint32_t j = 0; j < 7; j++)
-                if (r > j) stg_st(base + j * GOFR_RING_STRIDE_BYTES, stg_ld(rp + j * GOFR_RING_STRIDE_BYTES));
+                    for (uint32_t j = 0; j < 8; j++) v[j] = stg_ld(rp + j * kStride);
+                }
+                p.store32(have, at, v[0], v[1], v[2], v[3], v[4], v[5], v[6], v[7]);
+                if (have) {
+                    chunk += 32;
+                    rp += 8 * kStride;
+                    n--;
+                }
+            }
+            const uint32_t r = wl & 7;
+            if (wl >= 8 && r) {
+#pragma unroll
+                for (uint32_t j = 0; j < 7; j++)
+                    if (r > j) stg_st(base + j * kStride, stg_ld(rp + j * kStride));
+            }
+            wl = r;
+            wp = base + r * kStride;
         }
-        wl = r;
-        wp = base + r * GOFR_RING_STRIDE_BYTES;
     }
     // make room for n more words (n <= 8); the decision is taken together by all active lanes
     GOFR_HD void reserve(uint32_t n) {
-        if (warp_any(wl + n > GOFR_STAGE_WORDS)) flush();
+        if (warp_any(wl + n > kWords)) flush();
     }
     GOFR_HD void store_word(uint32_t x) {
         stg_st(wp, x);
-        wp += GOFR_RING_STRIDE_BYTES;
+        wp += kStride;
         wl++;
     }
     GOFR_HD void put4(uint32_t v) {
@@ -384,10 +439,10 @@ struct Writer {
 #pragma unroll
         for (int i = 0; i < K; i++) n[i] = M::ld(Y + 4 * i);
 #pragma unroll
-        for (int i = 0; i < K; i++) stg_st(wp + i * GOFR_RING_STRIDE_BYTES, fsr(i ? n[i - 1] : cur, n[i], sh));
+        for (int i = 0; i < K; i++) stg_st(wp + i * kStride, fsr(i ? n[i - 1] : cur, n[i], sh));
         cur = n[K - 1];
         Y += 4 * K;
-        wp += K * GOFR_RING_STRIDE_BYTES;
+        wp += K * kStride;
         wl += K;
     }
 
@@ -396,9 +451,9 @@ struct Writer {
     // previous one is carried) and one funnel shift.  Only word 0 mixes in `pend`.
     // Sources must be readable up to the end of the aligned word following their last byte (literal pool, staged
     // arena and blobs are padded accordingly); no byte before the source is ever read.
-    // With PairStores every lane of the pair mask makes the call, also with len 0, and takes the flush and long-copy
-    // rounds below.
-    template <bool SH, typename P = SoloStores>
+    // With LineStores every lane of the write mask makes the call, also with len 0, and takes the flush votes and the
+    // long-copy rounds below.
+    template <bool SH>
     GOFR_HD void copy(typename SrcMem<SH>::A src, uint32_t len, P p = P()) {
         typedef SrcMem<SH> M;
         if (!P::kLockstep && !len) return;
@@ -424,14 +479,27 @@ struct Writer {
             if (!P::kLockstep) return;
         }
         // at most 8 words staged from here on: this word + (head <= 7 | a short copy <= 7)
-        if (p.vote(wl + 8 > GOFR_STAGE_WORDS)) flush(p);
+        if (p.vote(wl + 8 > kWords)) flush(p);
         if (words) {
             store_word(w0);
             cur = nxt;
             Y += 8;  // Y now points at the NEXT word to load
             nwords--;
         }
-        if (p.round(nwords >= 8)) {
+        if constexpr (P::kLockstep) {
+            // Long copy: 8 words at a time through the column, a flush vote before each step and after the last one
+            if (p.round(nwords >= 8)) {
+#pragma unroll 1
+                do {
+                    if (p.vote(wl + 8 > kWords)) flush(p);
+                    if (nwords >= 8) {
+                        stream_words<M, 8>(Y, cur, sh);
+                        nwords -= 8;
+                    }
+                } while (p.round(nwords >= 8));
+                if (p.vote(wl + 8 > kWords)) flush(p);
+            }
+        } else if (p.round(nwords >= 8)) {
             if (nwords >= 8) {
                 // Long copy.  Head: complete the sector under construction (<= 7 more words), store it; from then on
                 // the staging buffer is empty and whole sectors go from registers straight to HBM.
@@ -475,25 +543,33 @@ struct Writer {
     }
     // Slot layout (gofr_serve_device_slots): the response owns its 16-byte aligned slot, so the last 16-byte chunk is
     // stored whole, zero padded — no byte stores, nothing of a neighbour to preserve.  A slot starts either on a sector
-    // boundary or in the middle of one (lead 0 or 16).
-    template <typename P = SoloStores>
+    // boundary or in the middle of one (lead 0 or 16); with LineStores at any 16-byte window of a line, and the last line
+    // is stored in whole windows up to the padded end.
     GOFR_HD void finish_padded(P p = P()) {
         flush(p);
-        const uint32_t end = 4 * wl + nb;  // bytes of the last sector in use, phantom lead included
+        const uint32_t end = 4 * wl + nb;  // bytes of the last sector (line) in use, phantom lead included
         const bool some = end > lead;
-        uint32_t v[8] = {0u, 0u, 0u, 0u, 0u, 0u, 0u, 0u};
-        if (some) {
-            const uint32_t tail = nb ? pend >> (8 * (4 - nb)) : 0u;
+        if constexpr (P::kLockstep) {
+            uint32_t wins = 0u;
+            if (some) {
+                const uint32_t ew = (end + 15u) >> 4;  // windows in use: 1..8
+                if (nb) stg_st(wp, pend >> (8 * (4 - nb)));
+#pragma unroll 1
+                for (uint32_t k = wl + (nb ? 1u : 0u); k < 4u * ew; k++) stg_st(base + k * kStride, 0u);
+                wins = (0xFFu >> (8u - ew)) & (0xFFu << (lead >> 4));
+            }
+            p.lines(chunk, base, wins);
+        } else {
+            uint32_t v[8] = {0u, 0u, 0u, 0u, 0u, 0u, 0u, 0u};
+            if (some) {
+                const uint32_t tail = nb ? pend >> (8 * (4 - nb)) : 0u;
 #pragma unroll
-            for (uint32_t j = 0; j < 8; j++) v[j] = j < wl ? word(j) : (j == wl ? tail : 0u);
-            if (lead) store16(chunk + 16, v[4], v[5], v[6], v[7]);  // upper half only: the lower one is the neighbour's
-            else if (end > 16) { if (!P::kLockstep) p.store32(true, chunk, v[0], v[1], v[2], v[3], v[4], v[5], v[6], v[7]); }
-            else store16(chunk, v[0], v[1], v[2], v[3]);  // the upper half may be the next slot's
+                for (uint32_t j = 0; j < 8; j++) v[j] = j < wl ? word(j) : (j == wl ? tail : 0u);
+                if (lead) store16(chunk + 16, v[4], v[5], v[6], v[7]);  // upper half only: the lower one is the neighbour's
+                else if (end > 16) p.store32(true, chunk, v[0], v[1], v[2], v[3], v[4], v[5], v[6], v[7]);
+                else store16(chunk, v[0], v[1], v[2], v[3]);  // the upper half may be the next slot's
+            }
         }
-        // The whole last sector (the `end > 16` case above).  A lane on its own stores it in that branch; a lockstep
-        // group makes the call with every lane, outside the per-lane branches.  (One `whole` flag and one call after
-        // the branches would read better, but it changes the solo code: Bind's kernel grows by 8 to 16 instructions.)
-        if (P::kLockstep) p.store32(some && !lead && end > 16, chunk, v[0], v[1], v[2], v[3], v[4], v[5], v[6], v[7]);
     }
     GOFR_HD void finish() {
         flush();
@@ -504,15 +580,19 @@ struct Writer {
     }
 };
 
+typedef WriterT<SoloStores> Writer;
+
 // The slow paths (rune-by-rune escapes, Location, Bind errors) share one out-of-line flush: they already work on a
 // local-memory copy of the Writer, and inlining the flush into every byte loop made the kernel's code several times
 // larger than its instruction cache.
 GOFR_HD_NOINLINE void flush_out(Writer* w) { w->flush(); }
-GOFR_HD void Writer::reserve_out(uint32_t n) {
-    if (warp_any(wl + n > GOFR_STAGE_WORDS)) flush_out(this);
+template <typename P>
+GOFR_HD void WriterT<P>::reserve_out(uint32_t n) {
+    if (warp_any(wl + n > GOFR_SOLO_WORDS)) flush_out(this);
 }
-GOFR_HD void Writer::put1(uint32_t c) {
-    if (warp_any(wl >= GOFR_STAGE_WORDS - 2)) flush_out(this);
+template <typename P>
+GOFR_HD void WriterT<P>::put1(uint32_t c) {
+    if (warp_any(wl >= GOFR_SOLO_WORDS - 2)) flush_out(this);
     putk(c, 1);
 }
 
@@ -655,7 +735,8 @@ GOFR_HD uint32_t ascii4(uint32_t q) {
 }
 
 // v < 10^8 with nd digits (nd = 1..8): at most two four-digit groups — what Content-Length, counters and most ids need
-GOFR_HD void emit_small_digits(Writer* w, uint32_t v, uint32_t nd) {
+template <typename W>
+GOFR_HD void emit_small_digits(W* w, uint32_t v, uint32_t nd) {
     const uint32_t hi = v / 10000u, lo = v - hi * 10000u;
     const uint32_t wlo = ascii4(lo);
     if (nd <= 4) {
@@ -667,8 +748,10 @@ GOFR_HD void emit_small_digits(Writer* w, uint32_t v, uint32_t nd) {
     w->put4(wlo);
 }
 
-template <bool EMIT>
-GOFR_HD uint32_t emit_i64(Writer* w, int64_t sv) {
+// (WT: the Writer instance; the size pass passes a null Writer*)
+template <typename X> struct NoDeduce { typedef X T; };
+template <bool EMIT, typename WT = Writer>
+GOFR_HD uint32_t emit_i64(typename NoDeduce<WT>::T* w, int64_t sv) {
     uint64_t v = sv < 0 ? (uint64_t)0 - (uint64_t)sv : (uint64_t)sv;
     uint32_t nd = ndigits_u64(v);
     uint32_t total = nd + (sv < 0 ? 1u : 0u);
@@ -693,8 +776,8 @@ GOFR_HD uint32_t emit_i64(Writer* w, int64_t sv) {
     return total;
 }
 
-template <bool EMIT>
-GOFR_HD uint32_t emit_u32(Writer* w, uint32_t v) {
+template <bool EMIT, typename WT = Writer>
+GOFR_HD uint32_t emit_u32(typename NoDeduce<WT>::T* w, uint32_t v) {
     uint32_t nd = v < 10 ? 1 : v < 100 ? 2 : v < 1000 ? 3 : v < 10000 ? 4 : v < 100000 ? 5 : v < 1000000 ? 6
                 : v < 10000000 ? 7 : v < 100000000 ? 8 : v < 1000000000 ? 9 : 10;
     if (!EMIT) return nd;
@@ -1301,7 +1384,7 @@ GOFR_HD bool run_prog(const TableView& tv, const BatchRefs& br, ReqCtx& c, Write
         csrc = nullptr;
         clen = 0;
         cshared = true;
-        if (EMIT && warp_any(w->wl >= GOFR_STAGE_WORDS - 8)) w->flush();  // every non-copy action appends at most 8 words
+        if (EMIT && warp_any(w->wl >= GOFR_SOLO_WORDS - 8)) w->flush();  // every non-copy action appends at most 8 words
         if (code == OP_LIT) {
             if (!(governed && skip)) {
                 csrc = lits + ooff;
@@ -1542,26 +1625,15 @@ GOFR_HD bool size_fast(const TableView& tv, const BatchRefs& br, ReqCtx& c) {
     return true;
 }
 
-// Window i (16 bytes) of a source: TMPL, a template in the literal pool (16-byte aligned); else a staging column.
-template <bool TMPL>
-GOFR_HD uint4 window_ld(saddr_t src, uint32_t i) {
-    if (TMPL) return src_ld128(src + 16 * i);
-    const saddr_t rp = src + 4 * i * GOFR_RING_STRIDE_BYTES;
-    uint4 v;
-    v.x = stg_ld(rp); v.y = stg_ld(rp + GOFR_RING_STRIDE_BYTES); v.z = stg_ld(rp + 2 * GOFR_RING_STRIDE_BYTES); v.w = stg_ld(rp + 3 * GOFR_RING_STRIDE_BYTES);
-    return v;
-}
-
-// Windows [k0, k1) of a response into its slot, window k0 + i from window i of src: whole 32-byte sectors wherever the
-// destination allows (a slot starts on a sector boundary or in the middle of one), single 16-byte windows at the ends.
-// With PairStores every lane of the pair mask makes the call (k0 == k1: nothing to store).
-template <bool TMPL, typename P>
-GOFR_HD void copy_windows(uint8_t* dst, saddr_t src, uint32_t k0, uint32_t k1, P p) {
+// Windows [k0, k1) of a response into its slot, window k0 + i from window i of the template at src (16-byte aligned, in
+// the literal pool): whole 32-byte sectors wherever the destination allows (a slot starts on a sector boundary or in the
+// middle of one), single 16-byte windows at the ends.
+GOFR_HD void copy_windows(uint8_t* dst, saddr_t src, uint32_t k0, uint32_t k1, SoloStores p) {
     const uint32_t n = k1 - k0;
     uint8_t* const d = dst + 16 * k0;
     uint32_t i = 0;
     if (n && ((uintptr_t)d & 16u)) {
-        const uint4 v = window_ld<TMPL>(src, 0);
+        const uint4 v = src_ld128(src);
         store16(d, v.x, v.y, v.z, v.w);
         i = 1;
     }
@@ -1569,75 +1641,91 @@ GOFR_HD void copy_windows(uint8_t* dst, saddr_t src, uint32_t k0, uint32_t k1, P
     while (p.round(i + 2 <= n)) {
         const bool have = i + 2 <= n;
         uint4 a = {0u, 0u, 0u, 0u}, b = {0u, 0u, 0u, 0u};
-        if (have) { a = window_ld<TMPL>(src, i); b = window_ld<TMPL>(src, i + 1); }
+        if (have) { a = src_ld128(src + 16 * i); b = src_ld128(src + 16 * (i + 1)); }
         p.store32(have, d + 16 * i, a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w);
         if (have) i += 2;
     }
     if (i < n) {
-        const uint4 v = window_ld<TMPL>(src, i);
+        const uint4 v = src_ld128(src + 16 * i);
         store16(d + 16 * i, v.x, v.y, v.z, v.w);
     }
 }
 
-// Writes a response sized by size_fast into its 16-byte aligned slot: the template with aligned 16-byte loads and
-// stores, the trace id patched into the windows it touches, then the tail ops through the Writer.  With PairStores every
-// lane of the pair mask runs every store round below, also when its program has no template or no tail: a lane past its
-// last op, or on an op that writes nothing, copies 0 bytes.  Only the appending of words differs between lanes.
+// Writes a response sized by size_fast into its 16-byte aligned slot.  SoloStores: the template with aligned 16-byte
+// loads and stores, the trace id patched into the windows it touches, then the tail ops through the Writer.
+// LineStores: everything goes through the Writer's column — the template as a copy from the literal pool with the 8
+// words of the trace id put in at hex_pos — and every lane of the write mask runs every vote and store round below,
+// also when its program has no template or no tail: a lane past its last op, or on an op that writes nothing, copies 0
+// bytes.  Only the appending of words differs between lanes.
+// live false (LineStores): the lane has no response and runs an empty one — votes and store rounds, no loads, no stores.
 template <typename P>
-GOFR_HD void emit_fast(const TableView& tv, const BatchRefs& br, ReqCtx& c, uint8_t* dst, uint32_t* ring_col, P p) {
-    const FastRec F = *(tv.fast() + c.prog);
+GOFR_HD void emit_fast(const TableView& tv, const BatchRefs& br, ReqCtx& c, uint8_t* dst, uint32_t* ring_col, P p,
+                       bool live = true) {
+    const FastRec F = live ? *(tv.fast() + c.prog) : FastRec{0u, 0, 0, 0xFFFFu, 0, 0, 0u};
     const uint32_t nwin = F.tmpl_windows;
     // the trace id is needed after the template copy: ask for it now
     uint4 id = {0u, 0u, 0u, 0u};
     if (F.hex_pos != 0xFFFFu) id = *(const uint4*)(br.ids + (size_t)c.index * 16);
-    if (P::kLockstep || nwin) {
-        const saddr_t tp = to_saddr(tv.lits() + F.tmpl_off);
-        const saddr_t col = to_saddr(ring_col);
-        uint32_t h0 = nwin, h1 = nwin;  // [h0, h1): windows the 32 hex characters touch
-        if (nwin && F.hex_pos != 0xFFFFu) { h0 = (uint32_t)F.hex_pos >> 4; h1 = (((uint32_t)F.hex_pos + 31u) >> 4) + 1u; }
-        copy_windows<true>(dst, tp, 0, h0, p);
-        copy_windows<true>(dst, tp + 16 * h1, h1, nwin, p);
-        if (h0 < nwin) {
-            // the 2 or 3 windows around the trace id: template words into the (idle) staging column, the 8 hex words
-            // shifted to their byte offset on top, then whole windows out
-            const uint32_t nw = (h1 - h0) * 4;  // 8 or 12 words
-#pragma unroll 1
-            for (uint32_t k = 0; k < nw; k++) stg_st(col + k * GOFR_RING_STRIDE_BYTES, src_ld(tp + 16 * h0 + 4 * k));
+    WriterT<P> w;
+    // the Writer's room check before a value: SoloStores flushes whole sectors once 8 words wait, LineStores has a line
+    constexpr uint32_t kFull = P::kLockstep ? 32u : GOFR_SOLO_WORDS - 8;
+    if constexpr (P::kLockstep) {
+        w.init(dst, ring_col);
+        const uint8_t* const tp = tv.lits() + F.tmpl_off;
+        const bool hex = nwin && F.hex_pos != 0xFFFFu;
+        const uint32_t h = hex ? (uint32_t)F.hex_pos : 16 * nwin;  // template bytes before the trace id
+        w.template copy<true>(SrcMem<true>::from(tp), h, p);
+        if (p.vote(w.wl >= kFull)) w.flush(p);
+        if (hex) {
             uint32_t H[8];
             hex8(id.x, H[0], H[1]); hex8(id.y, H[2], H[3]); hex8(id.z, H[4], H[5]); hex8(id.w, H[6], H[7]);
-            const uint32_t o = (uint32_t)F.hex_pos & 15u, q = o >> 2, sh = (o & 3u) * 8;
-            const saddr_t hp = col + q * GOFR_RING_STRIDE_BYTES;
-            if (sh == 0) {
 #pragma unroll
-                for (uint32_t j = 0; j < 8; j++) stg_st(hp + j * GOFR_RING_STRIDE_BYTES, H[j]);
-            } else {
-                const uint32_t lowmask = (1u << sh) - 1u;
-                stg_st(hp, (stg_ld(hp) & lowmask) | (H[0] << sh));
-#pragma unroll
-                for (uint32_t j = 1; j < 8; j++) stg_st(hp + j * GOFR_RING_STRIDE_BYTES, fsr(H[j - 1], H[j], 32 - sh));
-                stg_st(hp + 8 * GOFR_RING_STRIDE_BYTES, (H[7] >> (32 - sh)) | (stg_ld(hp + 8 * GOFR_RING_STRIDE_BYTES) & ~lowmask));
-            }
+            for (uint32_t j = 0; j < 8; j++) w.put4(H[j]);
         }
-        // a lane on its own stores the 2 or 3 trace-id windows one at a time: through copy_windows the 5-CTA slot
-        // instance took 4 % longer on config 4, well outside the run-to-run spread (DESIGN §6 has the A/B)
-        if (P::kLockstep) {
-            copy_windows<false>(dst, col, h0, h0 < nwin ? h1 : h0, p);
-        } else if (h0 < nwin) {
+        w.template copy<true>(SrcMem<true>::from(hex ? tp + h + 32 : tp), hex ? 16 * nwin - h - 32 : 0u, p);
+    } else {
+        if (nwin) {
+            const saddr_t tp = to_saddr(tv.lits() + F.tmpl_off);
+            const saddr_t col = to_saddr(ring_col);
+            uint32_t h0 = nwin, h1 = nwin;  // [h0, h1): windows the 32 hex characters touch
+            if (F.hex_pos != 0xFFFFu) { h0 = (uint32_t)F.hex_pos >> 4; h1 = (((uint32_t)F.hex_pos + 31u) >> 4) + 1u; }
+            copy_windows(dst, tp, 0, h0, p);
+            copy_windows(dst, tp + 16 * h1, h1, nwin, p);
+            if (h0 < nwin) {
+                // the 2 or 3 windows around the trace id: template words into the (idle) staging column, the 8 hex words
+                // shifted to their byte offset on top, then whole windows out, one at a time (as whole sectors the
+                // 5-CTA slot instance took 4 % longer on config 4, well outside the run-to-run spread: DESIGN §6)
+                const uint32_t nw = (h1 - h0) * 4;  // 8 or 12 words
 #pragma unroll 1
-            for (uint32_t k = h0; k < h1; k++) {
-                const saddr_t rp = col + (k - h0) * 4 * GOFR_RING_STRIDE_BYTES;
-                store16(dst + 16 * k, stg_ld(rp), stg_ld(rp + GOFR_RING_STRIDE_BYTES), stg_ld(rp + 2 * GOFR_RING_STRIDE_BYTES),
-                        stg_ld(rp + 3 * GOFR_RING_STRIDE_BYTES));
+                for (uint32_t k = 0; k < nw; k++) stg_st(col + k * GOFR_RING_STRIDE_BYTES, src_ld(tp + 16 * h0 + 4 * k));
+                uint32_t H[8];
+                hex8(id.x, H[0], H[1]); hex8(id.y, H[2], H[3]); hex8(id.z, H[4], H[5]); hex8(id.w, H[6], H[7]);
+                const uint32_t o = (uint32_t)F.hex_pos & 15u, q = o >> 2, sh = (o & 3u) * 8;
+                const saddr_t hp = col + q * GOFR_RING_STRIDE_BYTES;
+                if (sh == 0) {
+#pragma unroll
+                    for (uint32_t j = 0; j < 8; j++) stg_st(hp + j * GOFR_RING_STRIDE_BYTES, H[j]);
+                } else {
+                    const uint32_t lowmask = (1u << sh) - 1u;
+                    stg_st(hp, (stg_ld(hp) & lowmask) | (H[0] << sh));
+#pragma unroll
+                    for (uint32_t j = 1; j < 8; j++) stg_st(hp + j * GOFR_RING_STRIDE_BYTES, fsr(H[j - 1], H[j], 32 - sh));
+                    stg_st(hp + 8 * GOFR_RING_STRIDE_BYTES, (H[7] >> (32 - sh)) | (stg_ld(hp + 8 * GOFR_RING_STRIDE_BYTES) & ~lowmask));
+                }
+#pragma unroll 1
+                for (uint32_t k = h0; k < h1; k++) {
+                    const saddr_t rp = col + (k - h0) * 4 * GOFR_RING_STRIDE_BYTES;
+                    store16(dst + 16 * k, stg_ld(rp), stg_ld(rp + GOFR_RING_STRIDE_BYTES), stg_ld(rp + 2 * GOFR_RING_STRIDE_BYTES),
+                            stg_ld(rp + 3 * GOFR_RING_STRIDE_BYTES));
+                }
             }
         }
+        if (F.flags & FR_COMPLETE) return;
+        w.init(dst + 16 * nwin, ring_col);
     }
-    // a template-only program: with PairStores its Writer runs the tail with no ops, storing nothing but taking part in
-    // the store rounds
-    if (!P::kLockstep && (F.flags & FR_COMPLETE)) return;
+    // a template-only program: with LineStores its Writer runs the tail with no ops, appending nothing but taking part in
+    // the votes and store rounds
     const uint32_t n_ops = (F.flags & FR_COMPLETE) ? 0u : F.n_tail_ops;
-
-    Writer w;
-    w.init(dst + 16 * nwin, ring_col);
     const Op* ops = tv.ops() + F.tail_op;
     const uint8_t* const lits = tv.lits();
     RowReader row;
@@ -1664,7 +1752,7 @@ GOFR_HD void emit_fast(const TableView& tv, const BatchRefs& br, ReqCtx& c, uint
             live = false;
         }
         if (!P::kLockstep && !live) continue;
-        if ((P::kLockstep || comma) && p.vote(w.wl >= GOFR_STAGE_WORDS - 8)) w.flush(p);  // room for the comma
+        if ((P::kLockstep || comma) && p.vote(w.wl >= kFull)) w.flush(p);  // room for the comma
         if (comma) w.putc(',');
         const bool lit_only = code == OP_LIT || code == OP_KEY;
         // step 0: the op's literal bytes (OP_LIT / OP_KEY: the literal itself, else the folded prefix); step 1: its value
@@ -1675,7 +1763,7 @@ GOFR_HD void emit_fast(const TableView& tv, const BatchRefs& br, ReqCtx& c, uint
             if (step == 1) {
                 if (!P::kLockstep && lit_only) break;
                 clen = 0;
-                if (p.vote(w.wl >= GOFR_STAGE_WORDS - 8)) w.flush(p);  // a generated value appends at most 8 words
+                if (p.vote(w.wl >= kFull)) w.flush(p);  // a generated value appends at most 8 words
                 if (!live || lit_only) {
                     // no value: the copy below stores nothing
                 } else if (code == OP_STR) {
@@ -1683,14 +1771,14 @@ GOFR_HD void emit_fast(const TableView& tv, const BatchRefs& br, ReqCtx& c, uint
                     csrc = c.data() + c.str_base + str_cursor;
                     str_cursor += clen;
                 } else if (code == OP_I64) {
-                    emit_i64<true>(&w, (int64_t)((uint64_t)row[ooff] | (uint64_t)row[ooff + 1] << 32));
+                    emit_i64<true, WriterT<P>>(&w, (int64_t)((uint64_t)row[ooff] | (uint64_t)row[ooff + 1] << 32));
                 } else if (code == OP_I32) {
-                    emit_i64<true>(&w, (int64_t)(int32_t)row[ooff]);
+                    emit_i64<true, WriterT<P>>(&w, (int64_t)(int32_t)row[ooff]);
                 } else if (code == OP_BOOL) {
                     if (row[ooff]) w.put4('t' | 'r' << 8 | 'u' << 16 | 'e' << 24);
                     else { w.put4('f' | 'a' << 8 | 'l' << 16 | 's' << 24); w.putc('e'); }
                 } else if (code == OP_CLEN) {
-                    emit_u32<true>(&w, c.body_len);
+                    emit_u32<true, WriterT<P>>(&w, c.body_len);
                 } else if (code == OP_HEXID) {
                     const uint4 id = *(const uint4*)(br.ids + (size_t)c.index * 16);
                     const uint32_t idw[4] = {id.x, id.y, id.z, id.w};
@@ -1704,7 +1792,7 @@ GOFR_HD void emit_fast(const TableView& tv, const BatchRefs& br, ReqCtx& c, uint
                     clen = row[ooff + 1];
                 }
             }
-            if (P::kLockstep || clen) w.copy<true>(SrcMem<true>::from(csrc), clen, p);
+            if (P::kLockstep || clen) w.template copy<true>(SrcMem<true>::from(csrc), clen, p);
         }
     }
     w.finish_padded(p);

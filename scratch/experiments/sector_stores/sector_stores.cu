@@ -8,6 +8,9 @@
 //      slot, then of the odd lane's; a warp store covers 16 whole sectors
 //   c  the warp's 32 slots as one contiguous row, 512 bytes per warp store (the floor: fully coalesced)
 //   d  lane quads: four lanes write two whole sectors (64 bytes) of one slot per instruction
+//   e  line rounds: one lane per slot stages its bytes in a line-aligned shared-memory column; the lanes holding a whole
+//      128-byte line store four such lines per warp store, eight lanes per line (the LineStores policy of the serve
+//      kernel's wide slot instance)
 // Every pattern must produce the same bytes (checked against pattern a).  Prints one JSON line per pattern: CUDA-event
 // time per launch over `steps` launches after a warm-up.
 //
@@ -131,6 +134,64 @@ __global__ void __launch_bounds__(T) pat_d(uint8_t* out) {
     if (t0 < PADDED) st16(s + t0, val(r, t0));
 }
 
+// e: one lane per slot, its bytes staged 8 words at a time in a line-aligned shared-memory column (word k of thread t at
+//    [k * LS + t]; LS = T + 1 keeps the appends and a group's window loads conflict-free), then a vote; the lanes with a
+//    complete 128-byte line are stored in rounds of four lines per warp store: lane group g = lane >> 3 takes the g-th
+//    remaining ready lane, lane t = lane & 7 its 16-byte window t.  Edge lines store only the windows of the response.
+constexpr uint32_t LW = 39, LS = T + 1;  // column words (< 32 before an append of at most 8), row stride in words
+
+__device__ __forceinline__ void line_rounds(const uint32_t* ring, bool ready, uint8_t* chunk, uint32_t lo, uint32_t hi) {
+    const uint32_t lane = threadIdx.x & 31u, g = lane >> 3, t = lane & 7u, warp0 = threadIdx.x & ~31u;
+    uint32_t rem = __ballot_sync(~0u, ready);
+    __syncwarp();  // the owners' column stores before the other lanes' loads
+#pragma unroll 1
+    while (rem) {
+        const uint32_t m1 = rem & (rem - 1u), m2 = m1 & (m1 - 1u), m3 = m2 & (m2 - 1u);
+        const uint32_t sel = g == 0 ? rem : g == 1 ? m1 : g == 2 ? m2 : m3;
+        const uint32_t s = sel ? __ffs(sel) - 1u : lane;
+        uint8_t* const c = (uint8_t*)__shfl_sync(~0u, (unsigned long long)chunk, s);
+        const uint32_t l = __shfl_sync(~0u, lo, s), h = __shfl_sync(~0u, hi, s);
+        if (sel && t >= l && t < h) {
+            const uint32_t* p = ring + 4u * t * LS + warp0 + s;
+            st16(c + 16u * t, make_uint4(p[0], p[LS], p[2 * LS], p[3 * LS]));
+        }
+        rem = m3 & (m3 - 1u);
+    }
+    __syncwarp();  // every load of a column before its owner moves or overwrites it
+}
+
+__global__ void __launch_bounds__(T) pat_e(uint8_t* out) {
+    __shared__ uint32_t ring[LW * LS];
+    const uint32_t r = blockIdx.x * T + threadIdx.x;  // N is a multiple of T: every lane has a slot
+    uint32_t* const col = ring + threadIdx.x;
+    uint8_t* const s = out + (size_t)r * SLOT;
+    uint8_t* chunk = (uint8_t*)((uintptr_t)s & ~(uintptr_t)127);
+    uint32_t lead = (uint32_t)((uintptr_t)s & 127u), wl = lead >> 2, o = 0;
+#pragma unroll 1
+    while (__any_sync(~0u, o < PADDED)) {
+        if (o < PADDED) {
+            const uint4 a = val(r, o);
+            col[wl * LS] = a.x; col[(wl + 1) * LS] = a.y; col[(wl + 2) * LS] = a.z; col[(wl + 3) * LS] = a.w;
+            wl += 4; o += 16;
+            if (o < PADDED) {
+                const uint4 b = val(r, o);
+                col[wl * LS] = b.x; col[(wl + 1) * LS] = b.y; col[(wl + 2) * LS] = b.z; col[(wl + 3) * LS] = b.w;
+                wl += 4; o += 16;
+            }
+        }
+        const bool ready = wl >= 32u;
+        if (__any_sync(~0u, ready)) {
+            line_rounds(ring, ready, chunk, lead >> 4, 8u);
+            if (ready) {
+#pragma unroll 1
+                for (uint32_t k = 32; k < wl; k++) col[(k - 32) * LS] = col[k * LS];
+                wl -= 32; chunk += 128; lead = 0;
+            }
+        }
+    }
+    line_rounds(ring, 4 * wl > lead, chunk, lead >> 4, (wl + 3) >> 2);  // the last, partial line
+}
+
 int main(int argc, char** argv) {
     const int steps = argc > 1 ? atoi(argv[1]) : 50;
     const size_t bytes = (size_t)N * SLOT;
@@ -139,14 +200,14 @@ int main(int argc, char** argv) {
     cudaDeviceProp prop;
     CK(cudaGetDeviceProperties(&prop, 0));
     std::vector<uint8_t> ref(bytes), got(bytes);
-    void (*kern[4])(uint8_t*) = {pat_a, pat_b, pat_c, pat_d};
-    const char* names[4] = {"a_lane_per_slot", "b_lane_pairs", "c_coalesced_rows", "d_lane_quads"};
+    void (*kern[5])(uint8_t*) = {pat_a, pat_b, pat_c, pat_d, pat_e};
+    const char* names[5] = {"a_lane_per_slot", "b_lane_pairs", "c_coalesced_rows", "d_lane_quads", "e_line_rounds"};
     cudaEvent_t e0, e1;
     CK(cudaEventCreate(&e0));
     CK(cudaEventCreate(&e1));
     const uint32_t grid = (N + T - 1) / T;
     for (int rep = 0; rep < 2; rep++)
-        for (int k = 0; k < 4; k++) {
+        for (int k = 0; k < 5; k++) {
             CK(cudaMemset(out, 0xA5, bytes));
             kern[k]<<<grid, T>>>(out);
             CK(cudaGetLastError());
