@@ -255,6 +255,70 @@ func (e *Engine) HTTPFrameDevice(dBuf, dBufOff unsafe.Pointer, nConns int, dRecO
 		C.uint32_t(recCap), (*C.uint32_t)(dFirst), (*C.uint32_t)(dConsumed), (*C.uint32_t)(dConnStatus), stream), "gofr_http_frame_device")
 }
 
+// ConnResponses receives what ServeConnections returns; the caller owns the slices (ideally from gofr_alloc_pinned) and
+// sizes them with ConnBound.  Request k's response is Out[OutOff[k]:OutOff[k+1]]; connection c owns requests
+// ReqFirst[c] .. ReqFirst[c+1].  TraceIDs may be nil.
+type ConnResponses struct {
+	Out                            []byte
+	OutOff, Meta, ReqAt            []uint32 // req_cap + 1, req_cap, req_cap
+	TraceIDs                       []byte   // req_cap * 16, or nil
+	ReqFirst, Consumed, ConnStatus []uint32 // n + 1, n, n
+}
+
+// ConnBound gives the request and byte capacities that always suffice for connections with these offsets
+// (gofr_conn_batch_bound; no GPU needed).
+func (t *Table) ConnBound(bufOff []uint32) (reqCap uint32, outCap uint64, err error) {
+	if len(bufOff) == 0 {
+		return 0, 0, errors.New("gofrb200: bufOff needs n + 1 entries")
+	}
+	var rc C.uint32_t
+	var oc C.uint64_t
+	err = check(C.gofr_conn_batch_bound(t.t, (*C.uint32_t)(unsafe.Pointer(&bufOff[0])), C.uint32_t(len(bufOff)-1), &rc, &oc),
+		"gofr_conn_batch_bound")
+	return uint32(rc), uint64(oc), err
+}
+
+// ServeConnections serves every whole request in the connections' receive buffers (connection c = buf[bufOff[c]:bufOff[c+1]])
+// with gofr_conn_batch_submit + wait and returns the response bytes written.  Write Out[OutOff[ReqFirst[c]]:OutOff[ReqFirst[c+1]]]
+// to connection c, splicing in the host's responses for GOFR_H_HOST requests (status 0 in Meta); then keep its bytes from
+// Consumed[c] on (HTTPConnMore) or hand them to net/http (HTTPConnDefer).  traceSeed must be fresh per batch.
+func (e *Engine) ServeConnections(buf []byte, bufOff []uint32, now time.Time, traceSeed uint64, r *ConnResponses) (uint64, error) {
+	n := len(bufOff) - 1
+	if n <= 0 {
+		return 0, nil
+	}
+	if len(buf) == 0 || len(r.Out) == 0 || len(r.Meta) == 0 || len(r.OutOff) < len(r.Meta)+1 || len(r.ReqAt) < len(r.Meta) ||
+		(r.TraceIDs != nil && len(r.TraceIDs) < 16*len(r.Meta)) || len(r.ReqFirst) < n+1 || len(r.Consumed) < n || len(r.ConnStatus) < n {
+		return 0, errors.New("gofrb200: ConnResponses columns too small")
+	}
+	var in C.gofr_conn_batch
+	in.buf = (*C.uint8_t)(unsafe.Pointer(&buf[0]))
+	in.buf_off = (*C.uint32_t)(unsafe.Pointer(&bufOff[0]))
+	in.buf_bytes = C.uint64_t(len(buf))
+	in.n_conns = C.uint32_t(n)
+	in.trace_seed = C.uint64_t(traceSeed)
+	C.gofr_format_http_date(C.int64_t(now.Unix()), &in.date[0])
+	var o C.gofr_conn_resp
+	o.out = (*C.uint8_t)(unsafe.Pointer(&r.Out[0]))
+	o.out_cap = C.uint64_t(len(r.Out))
+	o.req_cap = C.uint32_t(len(r.Meta))
+	o.out_off = (*C.uint32_t)(unsafe.Pointer(&r.OutOff[0]))
+	o.meta = (*C.uint32_t)(unsafe.Pointer(&r.Meta[0]))
+	o.req_at = (*C.uint32_t)(unsafe.Pointer(&r.ReqAt[0]))
+	if r.TraceIDs != nil {
+		o.trace_ids = (*C.uint8_t)(unsafe.Pointer(&r.TraceIDs[0]))
+	}
+	o.req_first = (*C.uint32_t)(unsafe.Pointer(&r.ReqFirst[0]))
+	o.consumed = (*C.uint32_t)(unsafe.Pointer(&r.Consumed[0]))
+	o.conn_status = (*C.uint32_t)(unsafe.Pointer(&r.ConnStatus[0]))
+	var ticket C.gofr_ticket
+	if err := check(C.gofr_conn_batch_submit(e.e, &in, &o, &ticket), "gofr_conn_batch_submit"); err != nil {
+		return 0, err
+	}
+	err := check(C.gofr_batch_wait(e.e, ticket), "gofr_batch_wait")
+	return uint64(o.out_bytes), err
+}
+
 // Frontend gathers single requests from many goroutines into batches (gofr_frontend_*): the per-request call that stands
 // where router.ServeHTTP stands in the reference (pkg/gofr/httpServer.go:29-33).
 type Frontend struct{ f *C.gofr_frontend }

@@ -67,6 +67,7 @@ __global__ void proto_decode_nested_deferred_kernel(const GrpcParams p, const ui
 __global__ void reqlog_kernel(const LogParams p);                // reqlog_kernel.cu
 __global__ void http_parse_kernel(const HttpParams p);           // http_kernel.cu
 __global__ void http_frame_kernel(const HttpFrameParams p);      // http_frame_kernel.cu
+__global__ void conn_compact_kernel(const ConnParams p);         // conn_kernel.cu
 __global__ void route_kernel(const RouteParams p);               // route_kernel.cu
 __global__ void bind_kernel(const BindParams p);                 // bind_kernel.cu
 __global__ void chunk_pack_kernel(const PackParams p);           // pack_kernel.cu
@@ -77,6 +78,7 @@ namespace {
 enum Kern {
     K_SERVE, K_SERVE_VALUES, K_SLOTS, K_SLOTS_WIDE, K_SLOTS_VALUES, K_HELLO, K_PROTO_ENC, K_PROTO_DEC, K_PBN_ENC, K_PBN_DEC,
     K_PBN_ENC_MAPS, K_PBN_DEC_MAPS, K_PBN_ENC_PRES, K_PBN_DEC_PRES, K_PBN_DEC_DEFERRED, K_REQLOG, K_HTTP, K_HTTP_FRAME, K_ROUTE, K_BIND, K_PACK,
+    K_CONN,
     K_COUNT
 };
 struct KernelRec {
@@ -106,6 +108,7 @@ const KernelRec kKernels[K_COUNT] = {
     {(const void*)route_kernel, "route", kRouteThreads},
     {(const void*)bind_kernel, "bind", kBindThreads},
     {(const void*)chunk_pack_kernel, "pack", kServeThreads},
+    {(const void*)conn_compact_kernel, "connection compact", kServeThreads},
 };
 
 constexpr int kSlots = 3;  // pipeline depth of the host-batch path
@@ -132,11 +135,20 @@ struct Slot {
     uint32_t* d_in_off = nullptr; uint32_t* d_meta1 = nullptr;
     uint8_t* d_codec[2] = {nullptr, nullptr}; uint32_t* d_codec_off[2] = {nullptr, nullptr};
     size_t cap_codec_n = 0, cap_codec[2] = {0, 0};
+    // connection host path (grown on demand): the staged receive buffers and their offsets, the framer's per-connection
+    // columns and compacted req_first (per connection), its record column, and the request-head kernel's outputs and the
+    // compacted req_at (per record)
+    uint8_t* d_buf = nullptr; uint32_t* d_buf_off = nullptr;
+    uint32_t* d_first = nullptr; uint32_t* d_cstatus = nullptr; uint32_t* d_consumed = nullptr; uint32_t* d_req_first = nullptr;
+    uint32_t* d_rec = nullptr; void* d_pdesc = nullptr; uint32_t* d_pstatus = nullptr; unsigned long long* d_spans = nullptr;
+    uint32_t* d_req_at = nullptr;
+    size_t cap_buf = 0, cap_conns = 0, cap_recs = 0;
     // pinned staging for the tiny per-chunk read-backs
     uint32_t* h_tail = nullptr;  // [0] = chunk total bytes, [1] = overflow flag
 
     int reserve(gofr_engine* e, uint32_t requests, size_t arena_bytes, size_t out_bytes);
     int reserve_codec(uint32_t records, size_t a_bytes, size_t b_bytes);
+    int reserve_conn(uint32_t conns, uint32_t records, size_t buf_bytes);
 };
 
 }  // namespace
@@ -171,6 +183,8 @@ struct gofr_engine {
     unsigned long long* d_chain = nullptr;  // packed position of the batch in flight
     ChunkInfo* d_info = nullptr;            // one per slot
     unsigned long long* h_status = nullptr; // pinned: [0] total bytes, [1] overflow
+    uint32_t* h_ends = nullptr;             // pinned, gofr_conn_batch_submit: per chunk its first and end response offsets
+    size_t ends_cap = 0;                    // (words)
     int egress_grid = 37;
     uint32_t chunk = 65536;
     std::mutex mu;
@@ -382,6 +396,8 @@ void gofr_engine_destroy(gofr_engine* e) {
         cudaFree(s.state.words); cudaFree(s.d_flag); cudaFree(s.d_bind);
         cudaFree(s.d_in_off); cudaFree(s.d_meta1);
         for (int k = 0; k < 2; k++) { cudaFree(s.d_codec[k]); cudaFree(s.d_codec_off[k]); }
+        cudaFree(s.d_buf); cudaFree(s.d_buf_off); cudaFree(s.d_first); cudaFree(s.d_cstatus); cudaFree(s.d_consumed);
+        cudaFree(s.d_req_first); cudaFree(s.d_rec); cudaFree(s.d_pdesc); cudaFree(s.d_pstatus); cudaFree(s.d_spans); cudaFree(s.d_req_at);
         if (s.h_tail) cudaFreeHost(s.h_tail);
     }
     for (auto& ev : e->timing) { cudaEventDestroy(ev.first); cudaEventDestroy(ev.second); }
@@ -391,6 +407,7 @@ void gofr_engine_destroy(gofr_engine* e) {
     if (e->ev_batch_done) cudaEventDestroy(e->ev_batch_done);
     cudaFree(e->d_chain); cudaFree(e->d_info);
     if (e->h_status) cudaFreeHost(e->h_status);
+    if (e->h_ends) cudaFreeHost(e->h_ends);
     cudaFree(e->d_image); cudaFree(e->state.words); cudaFree(e->d_flag); cudaFree(e->d_bind);
     cudaFree(e->d_rt_desc); cudaFree(e->d_rt_arena); cudaFree(e->d_rt_meta); cudaFree(e->d_rt_vars); cudaFree(e->d_rt_rows);
     delete e;
@@ -881,6 +898,13 @@ struct ChunkSteps {
     std::function<int(Slot& s, const ChunkPlan& c, cudaStream_t st, const unsigned long long* chain_pos)> compute;
 };
 
+// Host memory the device can write (pinned or managed): the egress kernel stores into it directly
+static bool device_visible(const void* p) {
+    cudaPointerAttributes a;
+    if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); return false; }
+    return a.type == cudaMemoryTypeHost || a.type == cudaMemoryTypeManaged;
+}
+
 static int run_chunks(gofr_engine* e, uint32_t n, const ChunkSteps& steps, gofr_resp_batch* out, gofr_ticket* ticket) {
     out->out_bytes = 0;
     int final_rc = GOFR_OK;
@@ -891,11 +915,6 @@ static int run_chunks(gofr_engine* e, uint32_t n, const ChunkSteps& steps, gofr_
         return GOFR_OK;
     }
     // ---- streaming path: caller buffers are pinned → egress is device driven, the host never blocks mid-batch ----
-    auto device_visible = [](const void* p) {
-        cudaPointerAttributes a;
-        if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); return false; }
-        return a.type == cudaMemoryTypeHost || a.type == cudaMemoryTypeManaged;
-    };
     if (device_visible(out->out) && device_visible(out->out_off) && device_visible(out->meta)) {
         // growing buffers frees memory: make sure nothing from an earlier batch is still using them
         CUDA_TRY(cudaMemsetAsync(e->d_chain, 0, 8, e->st_compute));
@@ -1054,6 +1073,269 @@ static int batch_submit_slots_locked(gofr_engine* e, const gofr_req_batch* in, g
     }
     *ticket = e->next_ticket++;
     e->done_tickets.emplace_back(*ticket, final_rc);
+    return GOFR_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// connection receive buffers in host memory (gofr_conn_batch_submit)
+// ---------------------------------------------------------------------------------------------------------------
+
+// Receive-buffer bytes one chunk stages at most; a connection larger than this gets a chunk of its own.
+static constexpr uint32_t kConnChunkBudget = 8u << 20;
+
+// The buffers of a chunk of `conns` connections, `records` records at most and `buf_bytes` staged buffer bytes (plus the
+// 16 readable bytes the framer and the request-head kernel need, and 16 more for the bulk copies' rounding).
+int Slot::reserve_conn(uint32_t conns, uint32_t records, size_t buf_bytes) {
+    if (conns > cap_conns) {
+        cudaFree(d_buf_off); cudaFree(d_first); cudaFree(d_cstatus); cudaFree(d_consumed); cudaFree(d_req_first);
+        d_buf_off = d_first = d_cstatus = d_consumed = d_req_first = nullptr;
+        cap_conns = 0;
+        const size_t c = (size_t)conns + conns / 4 + 256;
+        if (cudaMalloc(&d_buf_off, (c + 1) * 4) != cudaSuccess || cudaMalloc(&d_first, (c + 1) * 4) != cudaSuccess ||
+            cudaMalloc(&d_cstatus, c * 4) != cudaSuccess || cudaMalloc(&d_consumed, c * 4) != cudaSuccess ||
+            cudaMalloc(&d_req_first, (c + 1) * 4) != cudaSuccess) {
+            set_last_error("cudaMalloc failed for a %zu-connection chunk", c);
+            return GOFR_ERR_NOMEM;
+        }
+        cap_conns = c;
+    }
+    if (records > cap_recs) {
+        cudaFree(d_rec); cudaFree(d_pdesc); cudaFree(d_pstatus); cudaFree(d_spans); cudaFree(d_req_at);
+        d_rec = d_pstatus = d_req_at = nullptr; d_pdesc = nullptr; d_spans = nullptr;
+        cap_recs = 0;
+        const size_t c = (size_t)records + records / 4 + 256;
+        if (cudaMalloc(&d_rec, (c + 1) * 4) != cudaSuccess || cudaMalloc(&d_pdesc, c * 16) != cudaSuccess ||
+            cudaMalloc(&d_pstatus, c * 4) != cudaSuccess || cudaMalloc(&d_spans, c * GOFR_HTTP_SPANS * 8) != cudaSuccess ||
+            cudaMalloc(&d_req_at, c * 4) != cudaSuccess) {
+            set_last_error("cudaMalloc failed for a %zu-record chunk", c);
+            return GOFR_ERR_NOMEM;
+        }
+        cap_recs = c;
+    }
+    return grow((void**)&d_buf, &cap_buf, buf_bytes + 32, 256);
+}
+
+// A chunk: connections [lo, hi), staged from buffer byte alo (buf_off[lo] rounded down to 16, so that the absolute offsets
+// address the staged copy through a rebased pointer), with room for rec_cap records.
+struct ConnChunk { uint32_t lo, hi, alo, rec_cap; };
+
+// The chunk that starts at connection lo: at most e->chunk connections whose bytes fit kConnChunkBudget, at least one.  The
+// offsets are validated here, chunk by chunk.
+static int conn_plan(const gofr_engine* e, const gofr_conn_batch* in, uint32_t lo, ConnChunk* c) {
+    const uint32_t* o = in->buf_off;
+    uint32_t hi = lo;
+    while (hi < in->n_conns && hi - lo < e->chunk) {
+        if (o[hi + 1] < o[hi] || o[hi + 1] > in->buf_bytes) {
+            set_last_error("buf_off[%u] decreases or passes buf_bytes", hi + 1);
+            return GOFR_ERR_INVALID;
+        }
+        if (hi > lo && o[hi + 1] - o[lo] > kConnChunkBudget) break;
+        hi++;
+    }
+    c->lo = lo; c->hi = hi; c->alo = o[lo] & ~15u;
+    c->rec_cap = (o[hi] - o[lo]) / 16 + (hi - lo);  // one record per 16 bytes plus one per connection (the framer's bound)
+    return GOFR_OK;
+}
+
+// First half of a chunk: stage its bytes, frame them, and bring back its record count (s.h_tail[0]) and its per-connection
+// columns.  s.done marks the moment the host may read them.
+static int conn_frame(gofr_engine* e, const gofr_conn_batch* in, gofr_conn_resp* out, Slot& s, const ConnChunk& c) {
+    const uint32_t cn = c.hi - c.lo, bytes = in->buf_off[c.hi] - c.alo;
+    const uint64_t sizes[2] = {0, bytes};  // the chunk's paths, queries and bodies: never more than its bytes
+    int rc = s.reserve(e, c.rec_cap, (size_t)bytes + 16, chunk_out_bound(e, c.rec_cap, sizes));
+    if (!rc) rc = s.reserve_conn(cn, c.rec_cap, bytes);
+    if (rc) return rc;
+    CUDA_TRY(cudaMemcpyAsync(s.d_buf, in->buf + c.alo, bytes, cudaMemcpyHostToDevice, e->st_h2d));
+    CUDA_TRY(cudaMemsetAsync(s.d_buf + bytes, 0, 32, e->st_h2d));
+    CUDA_TRY(cudaMemcpyAsync(s.d_buf_off, in->buf_off + c.lo, (size_t)(cn + 1) * 4, cudaMemcpyHostToDevice, e->st_h2d));
+    CUDA_TRY(cudaEventRecord(s.ev_h2d, e->st_h2d));
+    CUDA_TRY(cudaStreamWaitEvent(e->st_compute, s.ev_h2d, 0));
+    HttpFrameParams p;
+    memset(&p, 0, sizeof p);
+    p.buf = s.d_buf - c.alo; p.buf_off = s.d_buf_off; p.consumed = s.d_consumed; p.status = s.d_cstatus;
+    rc = launch_frames_locked(e, K_HTTP_FRAME, 0, p, cn, (uint8_t*)s.d_rec, c.rec_cap, s.d_first, s.state, s.d_flag, e->st_compute);
+    if (rc) return rc;
+    CUDA_TRY(cudaMemcpyAsync(&s.h_tail[0], s.d_first + cn, 4, cudaMemcpyDeviceToHost, e->st_compute));
+    CUDA_TRY(cudaMemcpyAsync(out->conn_status + c.lo, s.d_cstatus, (size_t)cn * 4, cudaMemcpyDeviceToHost, e->st_compute));
+    CUDA_TRY(cudaMemcpyAsync(out->consumed + c.lo, s.d_consumed, (size_t)cn * 4, cudaMemcpyDeviceToHost, e->st_compute));
+    CUDA_TRY(cudaEventRecord(s.done, e->st_compute));
+    return GOFR_OK;
+}
+
+// The state of a connection batch between its chunks
+struct ConnRun {
+    bool pinned;
+    bool req_short = false;     // req_cap was too small for a chunk: no per-request column is written from there on
+    bool bytes_short = false;   // out_cap was too small (pageable path; the pinned path learns it from the egress kernel)
+    uint64_t req_base = 0;      // requests of the chunks before
+    uint64_t write_pos = 0;     // pageable path: response bytes written so far
+};
+
+// Second half of chunk ci: parse its records, compact the whole requests, serve them, and send the results to the caller's
+// columns.  The record count and the connection states are on the host by now: they size the launches.
+static int conn_serve(gofr_engine* e, const gofr_conn_batch* in, gofr_conn_resp* out, Slot& s, size_t ci, const ConnChunk& c,
+                      ConnRun& r) {
+    CUDA_TRY(cudaEventSynchronize(s.done));
+    const uint32_t cn = c.hi - c.lo, n_rec = s.h_tail[0];
+    uint32_t n_req = n_rec;
+    for (uint32_t k = c.lo; k < c.hi; k++) n_req -= out->conn_status[k] != GOFR_HTTP_CONN_DONE ? 1u : 0u;
+    cudaStream_t st = e->st_compute;
+    if (n_rec) {  // every record's result lands in the bytes it occupies: no look-back, the whole resident grid runs
+        const int resident = resident_grid(e, K_HTTP);
+        if (!resident) return GOFR_ERR_CUDA;
+        HttpParams p;
+        memset(&p, 0, sizeof p);
+        p.raw = s.d_buf - c.alo; p.raw_off = s.d_rec; p.n = n_rec; p.n_tiles = (n_rec + kServeThreads - 1) / kServeThreads;
+        p.desc = s.d_pdesc; p.arena = s.d_arena - c.alo; p.status = s.d_pstatus; p.spans = s.d_spans;
+        int rc = launch(e, K_HTTP, (int)std::min<uint32_t>((uint32_t)resident, p.n_tiles), 0, st, p);
+        if (rc) return rc;
+    }
+    ConnParams q;
+    memset(&q, 0, sizeof q);
+    q.first = s.d_first; q.conn_status = s.d_cstatus; q.rec_off = s.d_rec; q.desc_in = s.d_pdesc;
+    q.trace_seed = in->trace_seed; q.conn0 = c.lo; q.req0 = (uint32_t)r.req_base; q.req_at = s.d_req_at; q.ids = (uint8_t*)s.d_ids;
+    int rc = launch_frames_locked(e, K_CONN, 0, q, cn, (uint8_t*)s.d_desc, n_rec, s.d_req_first, s.state, s.d_flag, st);
+    if (rc) return rc;
+    if (r.req_base + n_req > out->req_cap) r.req_short = true;
+    const bool put = !r.req_short && n_req;  // this chunk's per-request columns go to the caller
+    uint32_t* ends = e->h_ends + 2 * ci;     // the chunk's first and end response offsets: what it needs of out_cap
+    ends[0] = ends[1] = 0;
+    if (n_req) {
+        rc = launch_serve(e, s.d_desc, s.d_ids, s.d_arena - c.alo, n_req, in->date, s.d_out, s.cap_out, s.d_off, s.d_meta, &s.state,
+                          s.d_flag, s.d_bind, st, r.pinned ? e->d_chain : nullptr);
+        if (rc) return rc;
+        CUDA_TRY(cudaMemcpyAsync(&ends[0], s.d_off, 4, cudaMemcpyDeviceToHost, st));
+        CUDA_TRY(cudaMemcpyAsync(&ends[1], s.d_off + n_req, 4, cudaMemcpyDeviceToHost, st));
+    }
+    const size_t si = ci % kSlots;
+    if (r.pinned) {
+        if (put && launch_advance(e->d_chain, s.d_off, n_req, s.d_flag, e->d_info + si, out->out_cap, st) != 0) {
+            set_last_error("advance kernel launch failed"); return GOFR_ERR_CUDA;
+        }
+        CUDA_TRY(cudaEventRecord(s.ev_served, st));
+        CUDA_TRY(cudaStreamWaitEvent(e->st_egress, s.ev_served, 0));
+        cudaStream_t eg = e->st_egress;
+        if (put) {
+            if (launch_egress(e->d_info + si, s.d_out, s.d_off, s.d_meta, n_req, out->out, out->out_off + r.req_base,
+                              out->meta + r.req_base, e->h_status, e->egress_grid, eg) != 0) {
+                set_last_error("egress kernel launch failed"); return GOFR_ERR_CUDA;
+            }
+            e->launches += 2;
+            CUDA_TRY(cudaMemcpyAsync(out->req_at + r.req_base, s.d_req_at, (size_t)n_req * 4, cudaMemcpyDeviceToHost, eg));
+            if (out->trace_ids) CUDA_TRY(cudaMemcpyAsync(out->trace_ids + r.req_base * 16, s.d_ids, (size_t)n_req * 16, cudaMemcpyDeviceToHost, eg));
+        }
+        CUDA_TRY(cudaMemcpyAsync(out->req_first + c.lo, s.d_req_first, (size_t)cn * 4, cudaMemcpyDeviceToHost, eg));
+        CUDA_TRY(cudaEventRecord(s.ev_egress, eg));
+        s.egress_pending = true;
+    } else {  // pageable: the chunk's exact size first, then exactly that many bytes
+        CUDA_TRY(cudaStreamSynchronize(st));
+        const uint32_t total = ends[1];
+        if (put && r.write_pos + total > out->out_cap) r.bytes_short = true;
+        if (put && !r.bytes_short) {
+            if (total) CUDA_TRY(cudaMemcpyAsync(out->out + r.write_pos, s.d_out, total, cudaMemcpyDeviceToHost, st));
+            CUDA_TRY(cudaMemcpyAsync(out->out_off + r.req_base, s.d_off, (size_t)n_req * 4, cudaMemcpyDeviceToHost, st));
+            CUDA_TRY(cudaMemcpyAsync(out->meta + r.req_base, s.d_meta, (size_t)n_req * 4, cudaMemcpyDeviceToHost, st));
+            CUDA_TRY(cudaMemcpyAsync(out->req_at + r.req_base, s.d_req_at, (size_t)n_req * 4, cudaMemcpyDeviceToHost, st));
+            if (out->trace_ids) CUDA_TRY(cudaMemcpyAsync(out->trace_ids + r.req_base * 16, s.d_ids, (size_t)n_req * 16, cudaMemcpyDeviceToHost, st));
+        }
+        CUDA_TRY(cudaMemcpyAsync(out->req_first + c.lo, s.d_req_first, (size_t)cn * 4, cudaMemcpyDeviceToHost, st));
+        CUDA_TRY(cudaStreamSynchronize(st));
+        if (put && !r.bytes_short) {
+            if (r.write_pos) for (uint64_t k = r.req_base; k < r.req_base + n_req; k++) out->out_off[k] += (uint32_t)r.write_pos;
+            r.write_pos += total;
+        }
+    }
+    r.req_base += n_req;
+    return GOFR_OK;
+}
+
+// The chunks of a connection batch, one framed ahead of the one being served: the host learns a chunk's record count while
+// the next chunk's bytes are on their way.
+static int conn_batch_locked(gofr_engine* e, const gofr_conn_batch* in, gofr_conn_resp* out, gofr_ticket* ticket) {
+    const uint32_t n = in->n_conns;
+    out->out_bytes = 0;
+    if (n == 0) {  // touches no buffer
+        *ticket = e->next_ticket++;
+        e->done_tickets.emplace_back(*ticket, GOFR_OK);
+        return GOFR_OK;
+    }
+    // chunks end at e->chunk connections or at the byte budget, where two neighbours together pass it
+    const uint64_t max_chunks = (n + (uint64_t)e->chunk - 1) / e->chunk + 2 * (std::min<uint64_t>(in->buf_bytes, 1ull << 32) / kConnChunkBudget) + 2;
+    if (2 * max_chunks > e->ends_cap) {
+        if (e->h_ends) cudaFreeHost(e->h_ends);
+        e->h_ends = nullptr;
+        e->ends_cap = 0;
+        CUDA_TRY(cudaMallocHost(&e->h_ends, 2 * max_chunks * 4));
+        e->ends_cap = 2 * max_chunks;
+    }
+    ConnRun r;
+    r.pinned = device_visible(out->out) && device_visible(out->out_off) && device_visible(out->meta);
+    if (r.pinned) {
+        CUDA_TRY(cudaMemsetAsync(e->d_chain, 0, 8, e->st_compute));
+        e->h_status[0] = 0; e->h_status[1] = 0;
+    }
+    ConnChunk chunks[kSlots];
+    size_t issued = 0, served = 0;
+    for (uint32_t lo = 0; lo < n || served < issued;) {
+        while (lo < n && issued < served + 2) {
+            ConnChunk& c = chunks[issued % kSlots];
+            int rc = conn_plan(e, in, lo, &c);
+            if (!rc) rc = conn_frame(e, in, out, e->slots[issued % kSlots], c);
+            if (rc) return rc;
+            lo = c.hi;
+            issued++;
+        }
+        int rc = conn_serve(e, in, out, e->slots[served % kSlots], served, chunks[served % kSlots], r);
+        if (rc) return rc;
+        served++;
+    }
+    uint64_t need = 0, written = r.write_pos;
+    bool short_ = r.req_short || r.bytes_short;
+    if (r.pinned) {
+        CUDA_TRY(cudaMemcpyAsync((void*)&e->h_status[0], e->d_chain, 8, cudaMemcpyDeviceToHost, e->st_egress));
+        CUDA_TRY(wait_batch(e, n));
+        for (auto& s : e->slots) s.egress_pending = false;
+        written = e->h_status[0];
+        short_ |= e->h_status[1] != 0;
+    }
+    for (size_t ci = 0; ci < served; ci++) need += e->h_ends[2 * ci + 1] - e->h_ends[2 * ci];
+    out->req_first[n] = (uint32_t)r.req_base;
+    out->out_bytes = need;
+    int final_rc = GOFR_OK;
+    if (short_) {
+        final_rc = GOFR_ERR_CAPACITY;
+        set_last_error("the batch needs %llu requests and %llu response bytes: req_cap %u, out_cap %llu", (unsigned long long)r.req_base,
+                       (unsigned long long)need, out->req_cap, (unsigned long long)out->out_cap);
+    } else {
+        out->out_off[r.req_base] = (uint32_t)written;
+    }
+    *ticket = e->next_ticket++;
+    e->done_tickets.emplace_back(*ticket, final_rc);
+    return GOFR_OK;
+}
+
+int gofr_conn_batch_submit(gofr_engine* e, const gofr_conn_batch* in, gofr_conn_resp* out, gofr_ticket* ticket) {
+    if (!e || !in || !out || !ticket) return GOFR_ERR_INVALID;
+    if (in->n_conns && (!in->buf || !in->buf_off || !out->out || !out->out_off || !out->meta || !out->req_at || !out->req_first ||
+                        !out->consumed || !out->conn_status)) return GOFR_ERR_INVALID;
+    std::lock_guard<std::mutex> g(e->mu);
+    CUDA_TRY(cudaSetDevice(e->device));
+    const int rc = conn_batch_locked(e, in, out, ticket);
+    if (rc != GOFR_OK) drain_streams(e);  // see gofr_batch_submit
+    return rc;
+}
+
+int gofr_conn_batch_bound(const gofr_table* t, const uint32_t* buf_off, uint32_t n_conns, uint32_t* req_cap, uint64_t* out_cap) {
+    if (!t || !req_cap || !out_cap || (n_conns && !buf_off)) return GOFR_ERR_INVALID;
+    const uint64_t r0 = gofr_table_response_bound(t, 0, 0, 0);
+    if (!r0) { set_last_error("the table is not sealed"); return GOFR_ERR_NOT_SEALED; }
+    // a response grows by at most this much per path, query or body byte of its request
+    const uint64_t per_byte = std::max(gofr_table_response_bound(t, 1, 0, 0), gofr_table_response_bound(t, 0, 0, 1)) - r0;
+    for (uint32_t c = 0; c < n_conns; c++)
+        if (buf_off[c + 1] < buf_off[c]) { set_last_error("buf_off[%u] decreases", c + 1); return GOFR_ERR_INVALID; }
+    const uint64_t bytes = n_conns ? buf_off[n_conns] - buf_off[0] : 0, reqs = bytes / 16 + n_conns;
+    *req_cap = (uint32_t)std::min<uint64_t>(reqs, 0xFFFFFFFFull);
+    *out_cap = reqs * r0 + per_byte * bytes;
     return GOFR_OK;
 }
 

@@ -243,6 +243,28 @@ struct HttpFrameParams {
     uint32_t* overflow;
 };
 
+// conn_kernel.cu: gofr_conn_batch_submit's compact step, a packed-output kernel over connections whose output is the
+// compacted request columns (a connection's length is its number of whole requests)
+struct ConnParams {
+    const uint32_t* first;        // n + 1: the framer's record column of the chunk (d_first)
+    const uint32_t* conn_status;  // n
+    const uint32_t* rec_off;      // the framer's record starts (absolute buffer offsets)
+    const void* desc_in;          // gofr_req_desc per record (the request-head kernel's output)
+    uint64_t trace_seed;
+    uint32_t conn0;               // the batch index of the chunk's first connection (trace ids)
+    uint32_t req0;                // the batch index of the chunk's first request (req_first)
+    uint32_t n;                   // connections
+    uint32_t n_tiles;
+    uint32_t epoch;
+    uint8_t* out;                 // gofr_req_desc per request (out_cap requests)
+    uint64_t out_cap;
+    uint32_t* out_off;            // req_first: n + 1, rebased by req0
+    uint32_t* req_at;             // per request
+    uint8_t* ids;                 // 16 bytes per request
+    unsigned long long* tile_state;
+    uint32_t* overflow;
+};
+
 struct LogParams {
     const void* desc;   // gofr_log_desc[n]
     const void* ids;    // n * 16 trace id bytes

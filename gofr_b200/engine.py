@@ -429,6 +429,65 @@ class Engine:
         return int(ob.out_bytes)
 
 
+@dataclass
+class ConnResponses:
+    """What gofr_conn_batch_submit returns for a batch of connection buffers (numpy arrays, sliced to what was written).
+    Connection c's bytes to write are out[out_off[req_first[c]]:out_off[req_first[c + 1]]]."""
+    out: np.ndarray          # uint8[out_bytes]
+    out_off: np.ndarray      # uint32[requests + 1]
+    meta: np.ndarray         # uint32[requests]
+    req_at: np.ndarray       # uint32[requests]: the request's first byte in buf
+    trace_ids: np.ndarray    # uint8[requests, 16]
+    req_first: np.ndarray    # uint32[n_conns + 1]
+    consumed: np.ndarray     # uint32[n_conns]
+    conn_status: np.ndarray  # uint32[n_conns]: GOFR_HTTP_CONN_DONE / MORE / DEFER
+
+
+def conn_batch_bound(table: Table, buf_off: np.ndarray):
+    """gofr_conn_batch_bound: (req_cap, out_cap) that always suffice for connection buffers with these offsets."""
+    off = np.ascontiguousarray(buf_off, dtype=np.uint32)
+    rc, oc = C.c_uint32(), C.c_uint64()
+    _abi.check(_abi.lib().gofr_conn_batch_bound(table.handle, off.ctypes.data, len(off) - 1, C.byref(rc), C.byref(oc)),
+               "gofr_conn_batch_bound")
+    return rc.value, oc.value
+
+
+def _serve_connections(self, buf: np.ndarray, buf_off: np.ndarray, date: bytes, trace_seed: int, pinned: bool = True,
+                       req_cap: Optional[int] = None, out_cap: Optional[int] = None):
+    """gofr_conn_batch_submit + wait: connection c's received bytes are buf[buf_off[c]:buf_off[c + 1]] (host memory).
+    Returns ConnResponses.  The capacities default to conn_batch_bound; pinned puts the outputs in pinned memory (egress
+    driven by the device), else in pageable numpy arrays."""
+    buf = np.ascontiguousarray(buf, dtype=np.uint8)
+    off = np.ascontiguousarray(buf_off, dtype=np.uint32)
+    n = len(off) - 1
+    if req_cap is None or out_cap is None:
+        rc, oc = conn_batch_bound(self.table, off)
+        req_cap = rc if req_cap is None else req_cap
+        out_cap = oc if out_cap is None else out_cap
+    if pinned:
+        alloc = lambda count, dt: pinned_array(max(count, 1) * np.dtype(dt).itemsize).view(dt)
+    else:
+        alloc = lambda count, dt: np.zeros(max(count, 1), dt)
+    out, out_off, meta = alloc(out_cap, np.uint8), alloc(req_cap + 1, np.uint32), alloc(req_cap, np.uint32)
+    req_at, ids = alloc(req_cap, np.uint32), alloc(req_cap * 16, np.uint8)
+    req_first, consumed, status = alloc(n + 1, np.uint32), alloc(n, np.uint32), alloc(n, np.uint32)
+    assert len(date) == 29
+    cb = _abi.ConnBatch(buf=buf.ctypes.data, buf_off=off.ctypes.data, buf_bytes=buf.size, n_conns=n, date=date, trace_seed=trace_seed)
+    cr = _abi.ConnResp(out=out.ctypes.data, out_cap=out_cap, req_cap=req_cap, out_off=out_off.ctypes.data, meta=meta.ctypes.data,
+                       req_at=req_at.ctypes.data, trace_ids=ids.ctypes.data, req_first=req_first.ctypes.data,
+                       consumed=consumed.ctypes.data, conn_status=status.ctypes.data, out_bytes=0)
+    L = _abi.lib()
+    t = C.c_uint64()
+    _abi.check(L.gofr_conn_batch_submit(self._e, C.byref(cb), C.byref(cr), C.byref(t)), "gofr_conn_batch_submit")
+    _abi.check(L.gofr_batch_wait(self._e, t.value), "gofr_batch_wait")
+    k = int(req_first[n]) if n else 0
+    return ConnResponses(out[:int(cr.out_bytes)], out_off[:k + 1], meta[:k], req_at[:k], ids[:k * 16].reshape(k, 16),
+                         req_first[:n + 1] if n else np.zeros(1, np.uint32), consumed[:n], status[:n])
+
+
+Engine.serve_connections = _serve_connections
+
+
 def _serve_host_slots(self, batch: S.RequestBatch, date: bytes, slot_bytes: int, out: np.ndarray, out_len: np.ndarray,
                       meta: np.ndarray) -> None:
     """gofr_batch_submit_slots + wait: host buffers in, response i in out[i * slot_bytes:], its length in out_len[i]."""

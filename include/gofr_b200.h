@@ -727,6 +727,67 @@ int gofr_http_frame_device(gofr_engine*, const uint8_t* d_buf, const uint32_t* d
                            uint32_t* d_rec_off, uint32_t rec_cap, uint32_t* d_first, uint32_t* d_consumed,
                            uint32_t* d_conn_status, void* stream);
 
+/* Connection receive buffers in HOST memory → the bytes to write back to every connection, in one call: frame
+ * (gofr_http_frame_device), parse (gofr_http_parse_device), drop the tail records, serve every whole request (the packed
+ * layout of gofr_batch_submit), all on the device, chunk after chunk over the engine's streams.  Collect with
+ * gofr_batch_wait.
+ *   in   buf / buf_off: connection c's received bytes = buf[buf_off[c] .. buf_off[c+1]); buf_off has n_conns + 1
+ *        non-decreasing entries, buf_off[n_conns] <= buf_bytes.  date: the batch's IMF-fixdate.  trace_seed: see below.
+ *   out  per request k (requests are numbered across the batch, connection after connection, in request order):
+ *          out[out_off[k] .. out_off[k+1])  its response (out_off has req_cap + 1 entries);
+ *          meta[k]                           as gofr_batch_submit's meta; status 0 = a GOFR_H_HOST route: a hole of no bytes;
+ *          req_at[k]                         the request's first byte in buf;
+ *          trace_ids[16k .. 16k+16)          its trace id (may be NULL);
+ *        per connection c:
+ *          req_first[c] .. req_first[c+1])   its requests (req_first has n_conns + 1 entries);
+ *          consumed[c], conn_status[c]       as gofr_http_frame_device's d_consumed / d_conn_status;
+ *        out_bytes: the response bytes of the batch (filled by submit, reported by wait).
+ * Connection c's bytes to write are out[out_off[req_first[c]] .. out_off[req_first[c+1]]), its requests' responses in
+ * request order.  A GOFR_H_HOST request is a hole: the caller runs that closure and splices its response in at the request's
+ * place; the request's bytes are buf[req_at[k] .. end), end = req_at[k+1] within the connection, or buf_off[c] + consumed[c]
+ * for its last request.  Tail records (the last record of a MORE / DEFER connection) are never served and never appear in a
+ * per-request column.  A DEFER connection's requests before the deferred one are answered: write their responses, then hand
+ * buf[buf_off[c] + consumed[c] ..] to net/http.
+ * Trace ids: request j of connection c (j from 0 within the connection, c the connection's index in the batch) gets
+ *   x = splitmix64(trace_seed ^ splitmix64(c)), bytes 0-7 = splitmix64(x + 2j), bytes 8-15 = splitmix64(x + 2j + 1),
+ * little-endian; a pure function of (trace_seed, c, j), so chunking does not change it.  Pass a fresh seed per batch.
+ * Capacity: when req_cap or out_cap is too small, wait returns GOFR_ERR_CAPACITY and nothing is written at or past either
+ * capacity; the per-connection columns are still complete, and req_first[n_conns] and out_bytes are what the batch needed.
+ * gofr_conn_batch_bound (host only) gives capacities that always suffice for the given offsets.
+ * n_conns == 0 touches no buffer.  GOFR_ERR_INVALID: a null argument or column (trace_ids excepted), offsets that decrease
+ * or pass buf_bytes.  Offsets are checked chunk by chunk as the batch is enqueued; when a later chunk is refused, the work
+ * already enqueued is drained before the call returns and the engine stays usable. */
+typedef struct gofr_conn_batch {
+    const uint8_t* buf;
+    const uint32_t* buf_off;  /* n_conns + 1 */
+    uint64_t buf_bytes;
+    uint32_t n_conns;
+    char date[29];
+    uint8_t pad[3];
+    uint64_t trace_seed;
+} gofr_conn_batch;
+
+typedef struct gofr_conn_resp {
+    uint8_t* out;
+    uint64_t out_cap;
+    uint32_t req_cap;
+    uint32_t reserved;
+    uint32_t* out_off;      /* req_cap + 1 */
+    uint32_t* meta;         /* req_cap */
+    uint32_t* req_at;       /* req_cap */
+    uint8_t* trace_ids;     /* req_cap * 16, or NULL */
+    uint32_t* req_first;    /* n_conns + 1 */
+    uint32_t* consumed;     /* n_conns */
+    uint32_t* conn_status;  /* n_conns: GOFR_HTTP_CONN_DONE / MORE / DEFER */
+    uint64_t out_bytes;
+} gofr_conn_resp;
+
+int gofr_conn_batch_submit(gofr_engine*, const gofr_conn_batch* in, gofr_conn_resp* out, gofr_ticket* ticket);
+/* Capacities that always suffice for connections with these offsets: one request per 16 buffer bytes plus one per
+ * connection, and for the bytes gofr_table_response_bound summed over them (a request's path, query and body are never
+ * longer than its record).  No GPU needed.  GOFR_ERR_INVALID: null arguments, offsets that decrease. */
+int gofr_conn_batch_bound(const gofr_table*, const uint32_t* buf_off, uint32_t n_conns, uint32_t* req_cap, uint64_t* out_cap);
+
 /* number of kernels launched by this engine so far (bench.py reports it as gpu_launches) */
 uint64_t gofr_engine_launch_count(const gofr_engine*);
 /* duration in ms of the kernels launched since the last reset, measured with CUDA events on the launch stream.  Every
