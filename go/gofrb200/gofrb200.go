@@ -257,12 +257,42 @@ func (e *Engine) HTTPFrameDevice(dBuf, dBufOff unsafe.Pointer, nConns int, dRecO
 
 // ConnResponses receives what ServeConnections returns; the caller owns the slices (ideally from gofr_alloc_pinned) and
 // sizes them with ConnBound.  Request k's response is Out[OutOff[k]:OutOff[k+1]]; connection c owns requests
-// ReqFirst[c] .. ReqFirst[c+1].  TraceIDs may be nil.
+// ReqFirst[c] .. ReqFirst[c+1].  TraceIDs may be nil.  With Log set, ServeConnections also writes middleware.Logging's
+// lines for the requests answered on the device (gofr_conn_batch_submit_log).
 type ConnResponses struct {
 	Out                            []byte
 	OutOff, Meta, ReqAt            []uint32 // req_cap + 1, req_cap, req_cap
 	TraceIDs                       []byte   // req_cap * 16, or nil
 	ReqFirst, Consumed, ConnStatus []uint32 // n + 1, n, n
+	Log                            *ConnLog
+}
+
+// ConnLog is the request log of a connection batch.  Inputs: connection c's req.RemoteAddr is
+// Remote[RemoteOff[c]:RemoteOff[c+1]] (at most 255 bytes) and its requests' start clock Start[c]; every line is logged at
+// LogTime.  Outputs, sized with ConnLogBound: line m is Out[LogOff[m]:LogOff[m+1]] and belongs to request LogReq[m]; Lines
+// and OutBytes are what the batch needed.  A request with status 0 (GOFR_H_HOST) has no line: log it once its closure ran.
+type ConnLog struct {
+	Remote         []byte
+	RemoteOff      []uint32 // n + 1
+	Start          []time.Time
+	LogTime        time.Time
+	Out            []byte
+	LogOff, LogReq []uint32 // line_cap + 1, line_cap
+	Lines          uint32
+	OutBytes       uint64
+}
+
+// ConnLogBound gives the line and byte capacities that always suffice for the request log of connections with these
+// offsets (gofr_conn_log_bound; no GPU needed).
+func ConnLogBound(bufOff, remoteOff []uint32) (lineCap uint32, outCap uint64, err error) {
+	if len(bufOff) == 0 || len(remoteOff) != len(bufOff) {
+		return 0, 0, errors.New("gofrb200: bufOff and remoteOff need n + 1 entries")
+	}
+	var lc C.uint32_t
+	var oc C.uint64_t
+	err = check(C.gofr_conn_log_bound((*C.uint32_t)(unsafe.Pointer(&bufOff[0])), (*C.uint32_t)(unsafe.Pointer(&remoteOff[0])),
+		C.uint32_t(len(bufOff)-1), &lc, &oc), "gofr_conn_log_bound")
+	return uint32(lc), uint64(oc), err
 }
 
 // ConnBound gives the request and byte capacities that always suffice for connections with these offsets
@@ -311,11 +341,39 @@ func (e *Engine) ServeConnections(buf []byte, bufOff []uint32, now time.Time, tr
 	o.req_first = (*C.uint32_t)(unsafe.Pointer(&r.ReqFirst[0]))
 	o.consumed = (*C.uint32_t)(unsafe.Pointer(&r.Consumed[0]))
 	o.conn_status = (*C.uint32_t)(unsafe.Pointer(&r.ConnStatus[0]))
+	var lg *C.gofr_conn_log
+	var start []int64
+	if l := r.Log; l != nil {
+		if len(l.RemoteOff) < n+1 || len(l.Start) < n || len(l.Out) == 0 || len(l.LogReq) == 0 || len(l.LogOff) < len(l.LogReq)+1 {
+			return 0, errors.New("gofrb200: ConnLog columns too small")
+		}
+		start = make([]int64, n)
+		for c := 0; c < n; c++ {
+			start[c] = l.Start[c].UnixNano()
+		}
+		_, tz := l.LogTime.Zone()
+		lg = &C.gofr_conn_log{}
+		if len(l.Remote) > 0 {
+			lg.remote = (*C.uint8_t)(unsafe.Pointer(&l.Remote[0]))
+		}
+		lg.remote_off = (*C.uint32_t)(unsafe.Pointer(&l.RemoteOff[0]))
+		lg.start_unix_ns = (*C.int64_t)(unsafe.Pointer(&start[0]))
+		lg.log_unix_ns = C.int64_t(l.LogTime.UnixNano())
+		lg.tz_offset_s = C.int32_t(tz)
+		lg.line_cap = C.uint32_t(len(l.LogReq))
+		lg.out = (*C.uint8_t)(unsafe.Pointer(&l.Out[0]))
+		lg.out_cap = C.uint64_t(len(l.Out))
+		lg.log_off = (*C.uint32_t)(unsafe.Pointer(&l.LogOff[0]))
+		lg.log_req = (*C.uint32_t)(unsafe.Pointer(&l.LogReq[0]))
+	}
 	var ticket C.gofr_ticket
-	if err := check(C.gofr_conn_batch_submit(e.e, &in, &o, &ticket), "gofr_conn_batch_submit"); err != nil {
+	if err := check(C.gofr_conn_batch_submit_log(e.e, &in, &o, lg, &ticket), "gofr_conn_batch_submit_log"); err != nil {
 		return 0, err
 	}
 	err := check(C.gofr_batch_wait(e.e, ticket), "gofr_batch_wait")
+	if lg != nil {
+		r.Log.Lines, r.Log.OutBytes = uint32(lg.lines), uint64(lg.out_bytes)
+	}
 	return uint64(o.out_bytes), err
 }
 

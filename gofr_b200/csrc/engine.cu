@@ -68,6 +68,7 @@ __global__ void reqlog_kernel(const LogParams p);                // reqlog_kerne
 __global__ void http_parse_kernel(const HttpParams p);           // http_kernel.cu
 __global__ void http_frame_kernel(const HttpFrameParams p);      // http_frame_kernel.cu
 __global__ void conn_compact_kernel(const ConnParams p);         // conn_kernel.cu
+__global__ void conn_log_kernel(const ConnLogParams p);          // conn_log_kernel.cu
 __global__ void route_kernel(const RouteParams p);               // route_kernel.cu
 __global__ void bind_kernel(const BindParams p);                 // bind_kernel.cu
 __global__ void chunk_pack_kernel(const PackParams p);           // pack_kernel.cu
@@ -78,7 +79,7 @@ namespace {
 enum Kern {
     K_SERVE, K_SERVE_VALUES, K_SLOTS, K_SLOTS_WIDE, K_SLOTS_VALUES, K_HELLO, K_PROTO_ENC, K_PROTO_DEC, K_PBN_ENC, K_PBN_DEC,
     K_PBN_ENC_MAPS, K_PBN_DEC_MAPS, K_PBN_ENC_PRES, K_PBN_DEC_PRES, K_PBN_DEC_DEFERRED, K_REQLOG, K_HTTP, K_HTTP_FRAME, K_ROUTE, K_BIND, K_PACK,
-    K_CONN,
+    K_CONN, K_CONN_LOG,
     K_COUNT
 };
 struct KernelRec {
@@ -109,6 +110,7 @@ const KernelRec kKernels[K_COUNT] = {
     {(const void*)bind_kernel, "bind", kBindThreads},
     {(const void*)chunk_pack_kernel, "pack", kServeThreads},
     {(const void*)conn_compact_kernel, "connection compact", kServeThreads},
+    {(const void*)conn_log_kernel, "connection log", kServeThreads},
 };
 
 constexpr int kSlots = 3;  // pipeline depth of the host-batch path
@@ -143,12 +145,20 @@ struct Slot {
     uint32_t* d_rec = nullptr; void* d_pdesc = nullptr; uint32_t* d_pstatus = nullptr; unsigned long long* d_spans = nullptr;
     uint32_t* d_req_at = nullptr;
     size_t cap_buf = 0, cap_conns = 0, cap_recs = 0;
+    // its request-log lines (grown on demand): the staged remote strings, their offsets and the start clocks (per
+    // connection), the gather's per-connection line column, its descriptors, trace ids and request indices and the
+    // reqlog and pack offset columns (per line), the log arena, the reqlog kernel's lines and the packed lines
+    uint8_t* d_remote = nullptr; uint32_t* d_remote_off = nullptr; int64_t* d_start = nullptr; uint32_t* d_lfirst = nullptr;
+    void* d_ldesc = nullptr; uint8_t* d_lids = nullptr; uint32_t* d_lreq = nullptr; uint32_t* d_lraw_off = nullptr; uint32_t* d_loff = nullptr;
+    uint8_t* d_larena = nullptr; uint8_t* d_lraw = nullptr; uint8_t* d_lout = nullptr;
+    size_t cap_remote = 0, cap_lconns = 0, cap_lrecs = 0, cap_larena = 0, cap_lraw = 0, cap_lout = 0;
     // pinned staging for the tiny per-chunk read-backs
-    uint32_t* h_tail = nullptr;  // [0] = chunk total bytes, [1] = overflow flag
+    uint32_t* h_tail = nullptr;  // [0] = chunk total bytes, [1] = overflow flag; connection log: [2] lines, [3] overflow
 
     int reserve(gofr_engine* e, uint32_t requests, size_t arena_bytes, size_t out_bytes);
     int reserve_codec(uint32_t records, size_t a_bytes, size_t b_bytes);
     int reserve_conn(uint32_t conns, uint32_t records, size_t buf_bytes);
+    int reserve_log(uint32_t conns, uint32_t records, size_t remote_bytes);
 };
 
 }  // namespace
@@ -181,9 +191,10 @@ struct gofr_engine {
     cudaEvent_t ev_batch_done = nullptr;  // blocking-sync event: the caller's thread SLEEPS until its batch is back (a
                                           // spinning cudaStreamSynchronize per rank burns the CPU quota eight ranks share)
     unsigned long long* d_chain = nullptr;  // packed position of the batch in flight
-    ChunkInfo* d_info = nullptr;            // one per slot
-    unsigned long long* h_status = nullptr; // pinned: [0] total bytes, [1] overflow
-    uint32_t* h_ends = nullptr;             // pinned, gofr_conn_batch_submit: per chunk its first and end response offsets
+    ChunkInfo* d_info = nullptr;            // two per slot: [slot] the responses, [kSlots + slot] the request-log lines
+    unsigned long long* h_status = nullptr; // pinned: [0] total bytes, [1] overflow; [2], [3] the same for the log lines
+    uint32_t* h_ends = nullptr;             // pinned, gofr_conn_batch_submit: per chunk its first and end response offsets,
+                                            // then its first and end log line offsets
     size_t ends_cap = 0;                    // (words)
     int egress_grid = 37;
     uint32_t chunk = 65536;
@@ -372,7 +383,7 @@ static int engine_init(gofr_engine* e, const std::vector<uint8_t>& img, int devi
     CUDA_TRY(cudaStreamCreateWithFlags(&e->st_egress, cudaStreamNonBlocking));
     CUDA_TRY(cudaEventCreateWithFlags(&e->ev_batch_done, cudaEventBlockingSync | cudaEventDisableTiming));
     CUDA_TRY(cudaMalloc(&e->d_chain, 64));
-    CUDA_TRY(cudaMalloc(&e->d_info, sizeof(ChunkInfo) * kSlots));
+    CUDA_TRY(cudaMalloc(&e->d_info, sizeof(ChunkInfo) * 2 * kSlots));
     CUDA_TRY(cudaMallocHost(&e->h_status, 64));
     if (const char* w = getenv("GOFR_DEBUG_EPOCH_START")) e->epoch = (uint32_t)strtoul(w, nullptr, 0) & kEpochMask;  // tests: start next to the wrap
     if (getenv("GOFR_DEBUG_NO_LOOKBACK")) e->debug_flags |= 1u;  // diagnostic only: offsets are wrong unless every response has the same size
@@ -398,6 +409,8 @@ void gofr_engine_destroy(gofr_engine* e) {
         for (int k = 0; k < 2; k++) { cudaFree(s.d_codec[k]); cudaFree(s.d_codec_off[k]); }
         cudaFree(s.d_buf); cudaFree(s.d_buf_off); cudaFree(s.d_first); cudaFree(s.d_cstatus); cudaFree(s.d_consumed);
         cudaFree(s.d_req_first); cudaFree(s.d_rec); cudaFree(s.d_pdesc); cudaFree(s.d_pstatus); cudaFree(s.d_spans); cudaFree(s.d_req_at);
+        cudaFree(s.d_remote); cudaFree(s.d_remote_off); cudaFree(s.d_start); cudaFree(s.d_lfirst); cudaFree(s.d_ldesc); cudaFree(s.d_lids);
+        cudaFree(s.d_lreq); cudaFree(s.d_lraw_off); cudaFree(s.d_loff); cudaFree(s.d_larena); cudaFree(s.d_lraw); cudaFree(s.d_lout);
         if (s.h_tail) cudaFreeHost(s.h_tail);
     }
     for (auto& ev : e->timing) { cudaEventDestroy(ev.first); cudaEventDestroy(ev.second); }
@@ -1115,39 +1128,98 @@ int Slot::reserve_conn(uint32_t conns, uint32_t records, size_t buf_bytes) {
     return grow((void**)&d_buf, &cap_buf, buf_bytes + 32, 256);
 }
 
+// The request-log buffers of a chunk of `conns` connections with `records` records at most and `remote_bytes` of remote
+// strings: the inputs and every per-line column (a chunk has no more lines than records).  The byte buffers whose size is
+// only known once the chunk is served grow in conn_log_chunk.
+int Slot::reserve_log(uint32_t conns, uint32_t records, size_t remote_bytes) {
+    if (conns > cap_lconns) {
+        cudaFree(d_remote_off); cudaFree(d_start); cudaFree(d_lfirst);
+        d_remote_off = d_lfirst = nullptr; d_start = nullptr;
+        cap_lconns = 0;
+        const size_t c = (size_t)conns + conns / 4 + 256;
+        if (cudaMalloc(&d_remote_off, (c + 1) * 4) != cudaSuccess || cudaMalloc(&d_start, c * 8) != cudaSuccess ||
+            cudaMalloc(&d_lfirst, (c + 1) * 4) != cudaSuccess) {
+            set_last_error("cudaMalloc failed for a %zu-connection chunk's log", c);
+            return GOFR_ERR_NOMEM;
+        }
+        cap_lconns = c;
+    }
+    if (records > cap_lrecs) {
+        cudaFree(d_ldesc); cudaFree(d_lids); cudaFree(d_lreq); cudaFree(d_lraw_off); cudaFree(d_loff);
+        d_ldesc = nullptr; d_lids = nullptr; d_lreq = d_lraw_off = d_loff = nullptr;
+        cap_lrecs = 0;
+        const size_t c = (size_t)records + records / 4 + 256;
+        if (cudaMalloc(&d_ldesc, c * sizeof(gofr_log_desc)) != cudaSuccess || cudaMalloc(&d_lids, c * 16) != cudaSuccess ||
+            cudaMalloc(&d_lreq, c * 4) != cudaSuccess || cudaMalloc(&d_lraw_off, (c + 1) * 4) != cudaSuccess ||
+            cudaMalloc(&d_loff, (c + 1) * 4) != cudaSuccess) {
+            set_last_error("cudaMalloc failed for a %zu-line chunk's log", c);
+            return GOFR_ERR_NOMEM;
+        }
+        cap_lrecs = c;
+    }
+    return grow((void**)&d_remote, &cap_remote, remote_bytes + 16, 256);
+}
+
 // A chunk: connections [lo, hi), staged from buffer byte alo (buf_off[lo] rounded down to 16, so that the absolute offsets
-// address the staged copy through a rebased pointer), with room for rec_cap records.
-struct ConnChunk { uint32_t lo, hi, alo, rec_cap; };
+// address the staged copy through a rebased pointer), with room for rec_cap records.  With logging: its remote strings
+// remote[rlo .. rhi), the longest of them remote_max bytes.
+struct ConnChunk { uint32_t lo, hi, alo, rec_cap, rlo, rhi, remote_max; };
+
+// The longest line of a request besides 6 bytes per byte of its strings (reqlog_device.cuh): the literals, two times of 35
+// bytes, the id, a response_time of 20 characters and a status of 5 digits take 264 bytes.
+static constexpr uint64_t kConnLogFrame = 320;
 
 // The chunk that starts at connection lo: at most e->chunk connections whose bytes fit kConnChunkBudget, at least one.  The
-// offsets are validated here, chunk by chunk.
-static int conn_plan(const gofr_engine* e, const gofr_conn_batch* in, uint32_t lo, ConnChunk* c) {
+// offsets are validated here, chunk by chunk, and with logging the remote offsets too.
+static int conn_plan(const gofr_engine* e, const gofr_conn_batch* in, const gofr_conn_log* log, uint32_t lo, ConnChunk* c) {
     const uint32_t* o = in->buf_off;
-    uint32_t hi = lo;
+    const uint32_t* ro = log ? log->remote_off : nullptr;
+    uint32_t hi = lo, rmax = 0;
     while (hi < in->n_conns && hi - lo < e->chunk) {
         if (o[hi + 1] < o[hi] || o[hi + 1] > in->buf_bytes) {
             set_last_error("buf_off[%u] decreases or passes buf_bytes", hi + 1);
             return GOFR_ERR_INVALID;
         }
         if (hi > lo && o[hi + 1] - o[lo] > kConnChunkBudget) break;
+        if (ro) {
+            if (ro[hi + 1] < ro[hi] || ro[hi + 1] - ro[hi] > 255u) {
+                set_last_error("remote_off[%u] decreases or ends a remote string longer than 255 bytes", hi + 1);
+                return GOFR_ERR_INVALID;
+            }
+            rmax = std::max(rmax, ro[hi + 1] - ro[hi]);
+        }
         hi++;
     }
     c->lo = lo; c->hi = hi; c->alo = o[lo] & ~15u;
     c->rec_cap = (o[hi] - o[lo]) / 16 + (hi - lo);  // one record per 16 bytes plus one per connection (the framer's bound)
+    c->rlo = ro ? ro[lo] : 0; c->rhi = ro ? ro[hi] : 0; c->remote_max = rmax;
+    if (ro && c->rhi > c->rlo && !log->remote) { set_last_error("remote strings without a remote buffer"); return GOFR_ERR_INVALID; }
+    // the log arena of the chunk is addressed with 32-bit offsets (conn_log_device.cuh): its bytes plus R per request
+    if (ro && (uint64_t)(o[hi] - c->alo) + (uint64_t)c->rec_cap * rmax + 64 > 0xFFFFFFFFull) {
+        set_last_error("the log strings of connections %u..%u could pass 4 GiB", lo, hi);
+        return GOFR_ERR_UNSUPPORTED;
+    }
     return GOFR_OK;
 }
 
 // First half of a chunk: stage its bytes, frame them, and bring back its record count (s.h_tail[0]) and its per-connection
 // columns.  s.done marks the moment the host may read them.
-static int conn_frame(gofr_engine* e, const gofr_conn_batch* in, gofr_conn_resp* out, Slot& s, const ConnChunk& c) {
+static int conn_frame(gofr_engine* e, const gofr_conn_batch* in, gofr_conn_resp* out, const gofr_conn_log* log, Slot& s,
+                      const ConnChunk& c) {
     const uint32_t cn = c.hi - c.lo, bytes = in->buf_off[c.hi] - c.alo;
     const uint64_t sizes[2] = {0, bytes};  // the chunk's paths, queries and bodies: never more than its bytes
     int rc = s.reserve(e, c.rec_cap, (size_t)bytes + 16, chunk_out_bound(e, c.rec_cap, sizes));
     if (!rc) rc = s.reserve_conn(cn, c.rec_cap, bytes);
+    if (!rc && log) rc = s.reserve_log(cn, c.rec_cap, c.rhi - c.rlo);
     if (rc) return rc;
     CUDA_TRY(cudaMemcpyAsync(s.d_buf, in->buf + c.alo, bytes, cudaMemcpyHostToDevice, e->st_h2d));
     CUDA_TRY(cudaMemsetAsync(s.d_buf + bytes, 0, 32, e->st_h2d));
     CUDA_TRY(cudaMemcpyAsync(s.d_buf_off, in->buf_off + c.lo, (size_t)(cn + 1) * 4, cudaMemcpyHostToDevice, e->st_h2d));
+    if (log) {
+        if (c.rhi > c.rlo) CUDA_TRY(cudaMemcpyAsync(s.d_remote, log->remote + c.rlo, c.rhi - c.rlo, cudaMemcpyHostToDevice, e->st_h2d));
+        CUDA_TRY(cudaMemcpyAsync(s.d_remote_off, log->remote_off + c.lo, (size_t)(cn + 1) * 4, cudaMemcpyHostToDevice, e->st_h2d));
+        CUDA_TRY(cudaMemcpyAsync(s.d_start, log->start_unix_ns + c.lo, (size_t)cn * 8, cudaMemcpyHostToDevice, e->st_h2d));
+    }
     CUDA_TRY(cudaEventRecord(s.ev_h2d, e->st_h2d));
     CUDA_TRY(cudaStreamWaitEvent(e->st_compute, s.ev_h2d, 0));
     HttpFrameParams p;
@@ -1169,7 +1241,103 @@ struct ConnRun {
     bool bytes_short = false;   // out_cap was too small (pageable path; the pinned path learns it from the egress kernel)
     uint64_t req_base = 0;      // requests of the chunks before
     uint64_t write_pos = 0;     // pageable path: response bytes written so far
+    // the request-log lines (gofr_conn_batch_submit_log), the same per line
+    gofr_conn_log* log = nullptr;
+    bool log_pinned = false;
+    bool lines_short = false;
+    bool log_bytes_short = false;
+    uint64_t line_base = 0;
+    uint64_t log_pos = 0;
 };
+
+// The request-log lines of chunk ci, after its serve kernel: the gather (conn_log_kernel.cu), then the existing reqlog_kernel
+// and chunk_pack_kernel, then the caller's columns as for the responses (advance and egress on the log's own chain word
+// when they are pinned, an exact-size copy when they are pageable).  The reqlog and pack kernels take the chunk's line count
+// from the host: it is read back after the gather.  The log kernels report overflow in their own flag word, so that the
+// responses' advance never sees it.
+static int conn_log_chunk(gofr_engine* e, const gofr_conn_batch* in, Slot& s, size_t ci, const ConnChunk& c, ConnRun& r,
+                          uint32_t n_req) {
+    gofr_conn_log* log = r.log;
+    cudaStream_t st = e->st_compute;
+    uint32_t* ends = e->h_ends + 4 * ci + 2;  // the chunk's first and end line offsets: what it needs of out_cap
+    ends[0] = ends[1] = 0;
+    if (!n_req) return GOFR_OK;
+    const uint32_t cn = c.hi - c.lo, bytes = in->buf_off[c.hi] - c.alo;
+    uint32_t* flag = s.d_flag + 1;
+    // the log arena: the chunk's bytes plus R per request (conn_plan has checked that this stays below 4 GiB), and the 32
+    // readable bytes the reqlog kernel needs after the last string
+    int rc = grow((void**)&s.d_larena, &s.cap_larena, (size_t)bytes + (size_t)n_req * c.remote_max + 64, 256);
+    if (rc) return rc;
+    ConnLogParams g;
+    memset(&g, 0, sizeof g);
+    g.first = s.d_first; g.conn_status = s.d_cstatus; g.req_first = s.d_req_first; g.rec_off = s.d_rec; g.spans = s.d_spans;
+    g.meta = s.d_meta; g.ids = (const uint8_t*)s.d_ids; g.buf = s.d_buf - c.alo; g.remote = s.d_remote - c.rlo;
+    g.remote_off = s.d_remote_off; g.start_ns = s.d_start; g.log_ns = log->log_unix_ns; g.tz_offset_s = log->tz_offset_s;
+    g.alo = c.alo; g.remote_max = c.remote_max; g.req0 = (uint32_t)r.req_base;
+    g.line_ids = s.d_lids; g.line_req = s.d_lreq; g.arena = s.d_larena;
+    rc = launch_frames_locked(e, K_CONN_LOG, 0, g, cn, (uint8_t*)s.d_ldesc, n_req, s.d_lfirst, s.state, flag, st);
+    if (rc) return rc;
+    CUDA_TRY(cudaMemcpyAsync(&s.h_tail[2], s.d_lfirst + cn, 4, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaEventRecord(s.done, st));
+    CUDA_TRY(cudaEventSynchronize(s.done));
+    const uint32_t lines = s.h_tail[2];
+    if (!lines) return GOFR_OK;
+    // a line is at most kConnLogFrame bytes plus 6 per byte of its strings: its head's (disjoint spans of its record) and
+    // its remote string
+    const uint64_t bound = std::min<uint64_t>((uint64_t)lines * (kConnLogFrame + 6ull * c.remote_max) + 6ull * bytes, 0xFFFFFFF0ull);
+    rc = grow((void**)&s.d_lraw, &s.cap_lraw, bound + 16, 256);  // + the word the pack kernel's copy reads past a line
+    if (!rc) rc = grow((void**)&s.d_lout, &s.cap_lout, bound + 16, 256);  // + the packed start at *chain_pos & 15
+    if (rc) return rc;
+    LogParams lp;
+    memset(&lp, 0, sizeof lp);
+    lp.desc = s.d_ldesc; lp.ids = s.d_lids; lp.arena = s.d_larena;
+    rc = launch_frames_locked(e, K_REQLOG, 0, lp, lines, s.d_lraw, s.cap_lraw - 16, s.d_lraw_off, s.state, flag, st);
+    if (rc) return rc;
+    PackParams q;
+    memset(&q, 0, sizeof q);
+    q.a = s.d_lraw; q.a_off = s.d_lraw_off; q.a_cap = s.cap_lraw - 16; q.chain_pos = r.log_pinned ? e->d_chain + 1 : nullptr;
+    rc = launch_frames_locked(e, K_PACK, 0, q, lines, s.d_lout, s.cap_lout, s.d_loff, s.state, flag, st);
+    if (rc) return rc;
+    CUDA_TRY(cudaMemcpyAsync(&ends[0], s.d_loff, 4, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(&ends[1], s.d_loff + lines, 4, cudaMemcpyDeviceToHost, st));
+    if (r.line_base + lines > log->line_cap) r.lines_short = true;
+    const bool put = !r.lines_short;
+    const size_t si = kSlots + ci % kSlots;
+    if (r.log_pinned) {
+        if (put && launch_advance(e->d_chain + 1, s.d_loff, lines, flag, e->d_info + si, log->out_cap, st) != 0) {
+            set_last_error("advance kernel launch failed"); return GOFR_ERR_CUDA;
+        }
+        if (!put) CUDA_TRY(cudaMemsetAsync(flag, 0, 4, st));
+        CUDA_TRY(cudaEventRecord(s.ev_served, st));
+        CUDA_TRY(cudaStreamWaitEvent(e->st_egress, s.ev_served, 0));
+        if (put) {
+            if (launch_egress(e->d_info + si, s.d_lout, s.d_loff, s.d_lreq, lines, log->out, log->log_off + r.line_base,
+                              log->log_req + r.line_base, e->h_status + 2, e->egress_grid, e->st_egress) != 0) {
+                set_last_error("egress kernel launch failed"); return GOFR_ERR_CUDA;
+            }
+            e->launches += 2;
+        }
+        CUDA_TRY(cudaEventRecord(s.ev_egress, e->st_egress));
+        s.egress_pending = true;
+    } else {  // pageable: the chunk's exact size first, then exactly that many bytes
+        CUDA_TRY(cudaMemcpyAsync(&s.h_tail[3], flag, 4, cudaMemcpyDeviceToHost, st));
+        CUDA_TRY(cudaStreamSynchronize(st));
+        if (s.h_tail[3]) { CUDA_TRY(cudaMemsetAsync(flag, 0, 4, st)); r.log_bytes_short = true; }
+        const uint32_t total = ends[1];
+        // log_off is 32-bit: lines past 4 GiB are a capacity error, as advance_kernel makes them on the pinned path
+        if (put && (r.log_pos + total > log->out_cap || r.log_pos + total > 0xFFFFFFFFull)) r.log_bytes_short = true;
+        if (put && !r.log_bytes_short) {
+            if (total) CUDA_TRY(cudaMemcpyAsync(log->out + r.log_pos, s.d_lout, total, cudaMemcpyDeviceToHost, st));
+            CUDA_TRY(cudaMemcpyAsync(log->log_off + r.line_base, s.d_loff, (size_t)lines * 4, cudaMemcpyDeviceToHost, st));
+            CUDA_TRY(cudaMemcpyAsync(log->log_req + r.line_base, s.d_lreq, (size_t)lines * 4, cudaMemcpyDeviceToHost, st));
+            CUDA_TRY(cudaStreamSynchronize(st));
+            if (r.log_pos) for (uint64_t m = r.line_base; m < r.line_base + lines; m++) log->log_off[m] += (uint32_t)r.log_pos;
+            r.log_pos += total;
+        }
+    }
+    r.line_base += lines;
+    return GOFR_OK;
+}
 
 // Second half of chunk ci: parse its records, compact the whole requests, serve them, and send the results to the caller's
 // columns.  The record count and the connection states are on the host by now: they size the launches.
@@ -1198,7 +1366,7 @@ static int conn_serve(gofr_engine* e, const gofr_conn_batch* in, gofr_conn_resp*
     if (rc) return rc;
     if (r.req_base + n_req > out->req_cap) r.req_short = true;
     const bool put = !r.req_short && n_req;  // this chunk's per-request columns go to the caller
-    uint32_t* ends = e->h_ends + 2 * ci;     // the chunk's first and end response offsets: what it needs of out_cap
+    uint32_t* ends = e->h_ends + 4 * ci;     // the chunk's first and end response offsets: what it needs of out_cap
     ends[0] = ends[1] = 0;
     if (n_req) {
         rc = launch_serve(e, s.d_desc, s.d_ids, s.d_arena - c.alo, n_req, in->date, s.d_out, s.cap_out, s.d_off, s.d_meta, &s.state,
@@ -1245,15 +1413,20 @@ static int conn_serve(gofr_engine* e, const gofr_conn_batch* in, gofr_conn_resp*
             r.write_pos += total;
         }
     }
+    if (r.log) {
+        const int rc = conn_log_chunk(e, in, s, ci, c, r, n_req);
+        if (rc) return rc;
+    }
     r.req_base += n_req;
     return GOFR_OK;
 }
 
 // The chunks of a connection batch, one framed ahead of the one being served: the host learns a chunk's record count while
 // the next chunk's bytes are on their way.
-static int conn_batch_locked(gofr_engine* e, const gofr_conn_batch* in, gofr_conn_resp* out, gofr_ticket* ticket) {
+static int conn_batch_locked(gofr_engine* e, const gofr_conn_batch* in, gofr_conn_resp* out, gofr_conn_log* log, gofr_ticket* ticket) {
     const uint32_t n = in->n_conns;
     out->out_bytes = 0;
+    if (log) { log->lines = 0; log->out_bytes = 0; }
     if (n == 0) {  // touches no buffer
         *ticket = e->next_ticket++;
         e->done_tickets.emplace_back(*ticket, GOFR_OK);
@@ -1261,12 +1434,12 @@ static int conn_batch_locked(gofr_engine* e, const gofr_conn_batch* in, gofr_con
     }
     // chunks end at e->chunk connections or at the byte budget, where two neighbours together pass it
     const uint64_t max_chunks = (n + (uint64_t)e->chunk - 1) / e->chunk + 2 * (std::min<uint64_t>(in->buf_bytes, 1ull << 32) / kConnChunkBudget) + 2;
-    if (2 * max_chunks > e->ends_cap) {
+    if (4 * max_chunks > e->ends_cap) {
         if (e->h_ends) cudaFreeHost(e->h_ends);
         e->h_ends = nullptr;
         e->ends_cap = 0;
-        CUDA_TRY(cudaMallocHost(&e->h_ends, 2 * max_chunks * 4));
-        e->ends_cap = 2 * max_chunks;
+        CUDA_TRY(cudaMallocHost(&e->h_ends, 4 * max_chunks * 4));
+        e->ends_cap = 4 * max_chunks;
     }
     ConnRun r;
     r.pinned = device_visible(out->out) && device_visible(out->out_off) && device_visible(out->meta);
@@ -1274,13 +1447,19 @@ static int conn_batch_locked(gofr_engine* e, const gofr_conn_batch* in, gofr_con
         CUDA_TRY(cudaMemsetAsync(e->d_chain, 0, 8, e->st_compute));
         e->h_status[0] = 0; e->h_status[1] = 0;
     }
+    r.log = log;
+    r.log_pinned = log && device_visible(log->out) && device_visible(log->log_off) && device_visible(log->log_req);
+    if (r.log_pinned) {
+        CUDA_TRY(cudaMemsetAsync(e->d_chain + 1, 0, 8, e->st_compute));
+        e->h_status[2] = 0; e->h_status[3] = 0;
+    }
     ConnChunk chunks[kSlots];
     size_t issued = 0, served = 0;
     for (uint32_t lo = 0; lo < n || served < issued;) {
         while (lo < n && issued < served + 2) {
             ConnChunk& c = chunks[issued % kSlots];
-            int rc = conn_plan(e, in, lo, &c);
-            if (!rc) rc = conn_frame(e, in, out, e->slots[issued % kSlots], c);
+            int rc = conn_plan(e, in, log, lo, &c);
+            if (!rc) rc = conn_frame(e, in, out, log, e->slots[issued % kSlots], c);
             if (rc) return rc;
             lo = c.hi;
             issued++;
@@ -1291,14 +1470,17 @@ static int conn_batch_locked(gofr_engine* e, const gofr_conn_batch* in, gofr_con
     }
     uint64_t need = 0, written = r.write_pos;
     bool short_ = r.req_short || r.bytes_short;
-    if (r.pinned) {
-        CUDA_TRY(cudaMemcpyAsync((void*)&e->h_status[0], e->d_chain, 8, cudaMemcpyDeviceToHost, e->st_egress));
+    if (r.pinned || r.log_pinned) {
+        if (r.pinned) CUDA_TRY(cudaMemcpyAsync((void*)&e->h_status[0], e->d_chain, 8, cudaMemcpyDeviceToHost, e->st_egress));
+        if (r.log_pinned) CUDA_TRY(cudaMemcpyAsync((void*)&e->h_status[2], e->d_chain + 1, 8, cudaMemcpyDeviceToHost, e->st_egress));
         CUDA_TRY(wait_batch(e, n));
         for (auto& s : e->slots) s.egress_pending = false;
+    }
+    if (r.pinned) {
         written = e->h_status[0];
         short_ |= e->h_status[1] != 0;
     }
-    for (size_t ci = 0; ci < served; ci++) need += e->h_ends[2 * ci + 1] - e->h_ends[2 * ci];
+    for (size_t ci = 0; ci < served; ci++) need += e->h_ends[4 * ci + 1] - e->h_ends[4 * ci];
     out->req_first[n] = (uint32_t)r.req_base;
     out->out_bytes = need;
     int final_rc = GOFR_OK;
@@ -1309,18 +1491,36 @@ static int conn_batch_locked(gofr_engine* e, const gofr_conn_batch* in, gofr_con
     } else {
         out->out_off[r.req_base] = (uint32_t)written;
     }
+    if (log) {
+        uint64_t lneed = 0;
+        for (size_t ci = 0; ci < served; ci++) lneed += e->h_ends[4 * ci + 3] - e->h_ends[4 * ci + 2];
+        log->lines = (uint32_t)r.line_base;
+        log->out_bytes = lneed;
+        if (r.lines_short || r.log_bytes_short || (r.log_pinned && e->h_status[3] != 0)) {
+            final_rc = GOFR_ERR_CAPACITY;
+            set_last_error("the batch needs %llu log lines and %llu log bytes: line_cap %u, out_cap %llu", (unsigned long long)r.line_base,
+                           (unsigned long long)lneed, log->line_cap, (unsigned long long)log->out_cap);
+        } else {
+            log->log_off[r.line_base] = (uint32_t)(r.log_pinned ? e->h_status[2] : r.log_pos);
+        }
+    }
     *ticket = e->next_ticket++;
     e->done_tickets.emplace_back(*ticket, final_rc);
     return GOFR_OK;
 }
 
 int gofr_conn_batch_submit(gofr_engine* e, const gofr_conn_batch* in, gofr_conn_resp* out, gofr_ticket* ticket) {
+    return gofr_conn_batch_submit_log(e, in, out, nullptr, ticket);
+}
+
+int gofr_conn_batch_submit_log(gofr_engine* e, const gofr_conn_batch* in, gofr_conn_resp* out, gofr_conn_log* log, gofr_ticket* ticket) {
     if (!e || !in || !out || !ticket) return GOFR_ERR_INVALID;
     if (in->n_conns && (!in->buf || !in->buf_off || !out->out || !out->out_off || !out->meta || !out->req_at || !out->req_first ||
                         !out->consumed || !out->conn_status)) return GOFR_ERR_INVALID;
+    if (log && in->n_conns && (!log->remote_off || !log->start_unix_ns || !log->out || !log->log_off || !log->log_req)) return GOFR_ERR_INVALID;
     std::lock_guard<std::mutex> g(e->mu);
     CUDA_TRY(cudaSetDevice(e->device));
-    const int rc = conn_batch_locked(e, in, out, ticket);
+    const int rc = conn_batch_locked(e, in, out, log, ticket);
     if (rc != GOFR_OK) drain_streams(e);  // see gofr_batch_submit
     return rc;
 }
@@ -1336,6 +1536,25 @@ int gofr_conn_batch_bound(const gofr_table* t, const uint32_t* buf_off, uint32_t
     const uint64_t bytes = n_conns ? buf_off[n_conns] - buf_off[0] : 0, reqs = bytes / 16 + n_conns;
     *req_cap = (uint32_t)std::min<uint64_t>(reqs, 0xFFFFFFFFull);
     *out_cap = reqs * r0 + per_byte * bytes;
+    return GOFR_OK;
+}
+
+int gofr_conn_log_bound(const uint32_t* buf_off, const uint32_t* remote_off, uint32_t n_conns, uint32_t* line_cap, uint64_t* out_cap) {
+    if (!line_cap || !out_cap || (n_conns && (!buf_off || !remote_off))) return GOFR_ERR_INVALID;
+    uint64_t reqs = 0, remote = 0;
+    for (uint32_t c = 0; c < n_conns; c++) {
+        if (buf_off[c + 1] < buf_off[c]) { set_last_error("buf_off[%u] decreases", c + 1); return GOFR_ERR_INVALID; }
+        if (remote_off[c + 1] < remote_off[c] || remote_off[c + 1] - remote_off[c] > 255u) {
+            set_last_error("remote_off[%u] decreases or ends a remote string longer than 255 bytes", c + 1);
+            return GOFR_ERR_INVALID;
+        }
+        const uint64_t r = (buf_off[c + 1] - buf_off[c]) / 16 + 1;  // the connection's requests at most
+        reqs += r;
+        remote += r * (remote_off[c + 1] - remote_off[c]);
+    }
+    const uint64_t bytes = n_conns ? buf_off[n_conns] - buf_off[0] : 0;
+    *line_cap = (uint32_t)std::min<uint64_t>(reqs, 0xFFFFFFFFull);
+    *out_cap = reqs * kConnLogFrame + 6 * (bytes + remote);
     return GOFR_OK;
 }
 

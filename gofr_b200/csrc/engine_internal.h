@@ -265,6 +265,39 @@ struct ConnParams {
     uint32_t* overflow;
 };
 
+// conn_log_kernel.cu: gofr_conn_batch_submit_log's gather step, a packed-output kernel over connections whose output is the
+// line column (a connection's length is its number of logged requests): per line a gofr_log_desc, its trace id and its
+// batch request index, and the line's five strings in the log arena (conn_log_device.cuh)
+struct ConnLogParams {
+    const uint32_t* first;               // n + 1: the framer's record column of the chunk
+    const uint32_t* conn_status;         // n
+    const uint32_t* req_first;           // n + 1: the compact step's output (batch request indices)
+    const uint32_t* rec_off;             // the framer's record starts (absolute buffer offsets)
+    const unsigned long long* spans;     // per record: the request-head kernel's spans (absolute buffer offsets)
+    const uint32_t* meta;                // per request of the chunk: the serve kernel's meta
+    const uint8_t* ids;                  // per request of the chunk: 16 trace id bytes
+    const uint8_t* buf;                  // the staged chunk, addressed by absolute buffer offsets
+    const uint8_t* remote;               // the staged remote strings, addressed by absolute remote offsets
+    const uint32_t* remote_off;          // n + 1
+    const int64_t* start_ns;             // n
+    int64_t log_ns;
+    int32_t tz_offset_s;
+    uint32_t alo;                        // the chunk's first staged buffer byte
+    uint32_t remote_max;                 // R: the chunk's longest remote string
+    uint32_t req0;                       // the batch index of the chunk's first request
+    uint32_t n;                          // connections
+    uint32_t n_tiles;
+    uint32_t epoch;
+    uint8_t* out;                        // gofr_log_desc per line (out_cap lines)
+    uint64_t out_cap;
+    uint32_t* out_off;                   // n + 1: the connection's first line in the chunk
+    uint8_t* line_ids;                   // 16 bytes per line
+    uint32_t* line_req;                  // per line
+    uint8_t* arena;                      // the log arena
+    unsigned long long* tile_state;
+    uint32_t* overflow;
+};
+
 struct LogParams {
     const void* desc;   // gofr_log_desc[n]
     const void* ids;    // n * 16 trace id bytes

@@ -441,6 +441,32 @@ class ConnResponses:
     req_first: np.ndarray    # uint32[n_conns + 1]
     consumed: np.ndarray     # uint32[n_conns]
     conn_status: np.ndarray  # uint32[n_conns]: GOFR_HTTP_CONN_DONE / MORE / DEFER
+    log: Optional["ConnLogLines"] = None  # the request-log lines, when serve_connections was given a ConnLog
+
+
+@dataclass
+class ConnLog:
+    """The inputs of gofr_conn_batch_submit_log besides the connections' bytes: connection c's req.RemoteAddr is
+    remote[remote_off[c]:remote_off[c + 1]] (at most 255 bytes) and its requests' start clock start_unix_ns[c]; every line
+    is logged at log_unix_ns in a zone tz_offset_s east of UTC.  The capacities default to conn_log_bound."""
+    remote: np.ndarray         # uint8
+    remote_off: np.ndarray     # uint32[n_conns + 1]
+    start_unix_ns: np.ndarray  # int64[n_conns]
+    log_unix_ns: int
+    tz_offset_s: int = 0
+    line_cap: Optional[int] = None
+    out_cap: Optional[int] = None
+
+
+@dataclass
+class ConnLogLines:
+    """middleware.Logging's lines for the requests answered on the device, in request order: line m is
+    out[log_off[m]:log_off[m + 1]] and belongs to batch request log_req[m].  lines / out_bytes: what the batch needed."""
+    out: np.ndarray          # uint8[out_bytes]
+    log_off: np.ndarray      # uint32[lines + 1]
+    log_req: np.ndarray      # uint32[lines]
+    lines: int
+    out_bytes: int
 
 
 def conn_batch_bound(table: Table, buf_off: np.ndarray):
@@ -452,11 +478,22 @@ def conn_batch_bound(table: Table, buf_off: np.ndarray):
     return rc.value, oc.value
 
 
+def conn_log_bound(buf_off: np.ndarray, remote_off: np.ndarray):
+    """gofr_conn_log_bound: (line_cap, out_cap) that always suffice for the request-log lines of these connections."""
+    off = np.ascontiguousarray(buf_off, dtype=np.uint32)
+    roff = np.ascontiguousarray(remote_off, dtype=np.uint32)
+    lc, oc = C.c_uint32(), C.c_uint64()
+    _abi.check(_abi.lib().gofr_conn_log_bound(off.ctypes.data, roff.ctypes.data, len(off) - 1, C.byref(lc), C.byref(oc)),
+               "gofr_conn_log_bound")
+    return lc.value, oc.value
+
+
 def _serve_connections(self, buf: np.ndarray, buf_off: np.ndarray, date: bytes, trace_seed: int, pinned: bool = True,
-                       req_cap: Optional[int] = None, out_cap: Optional[int] = None):
+                       req_cap: Optional[int] = None, out_cap: Optional[int] = None, log: Optional[ConnLog] = None):
     """gofr_conn_batch_submit + wait: connection c's received bytes are buf[buf_off[c]:buf_off[c + 1]] (host memory).
     Returns ConnResponses.  The capacities default to conn_batch_bound; pinned puts the outputs in pinned memory (egress
-    driven by the device), else in pageable numpy arrays."""
+    driven by the device), else in pageable numpy arrays.  With log (a ConnLog), gofr_conn_batch_submit_log: the result's
+    .log holds the request-log lines, in the same kind of memory."""
     buf = np.ascontiguousarray(buf, dtype=np.uint8)
     off = np.ascontiguousarray(buf_off, dtype=np.uint32)
     n = len(off) - 1
@@ -478,11 +515,33 @@ def _serve_connections(self, buf: np.ndarray, buf_off: np.ndarray, date: bytes, 
                        consumed=consumed.ctypes.data, conn_status=status.ctypes.data, out_bytes=0)
     L = _abi.lib()
     t = C.c_uint64()
-    _abi.check(L.gofr_conn_batch_submit(self._e, C.byref(cb), C.byref(cr), C.byref(t)), "gofr_conn_batch_submit")
+    if log is None:
+        _abi.check(L.gofr_conn_batch_submit(self._e, C.byref(cb), C.byref(cr), C.byref(t)), "gofr_conn_batch_submit")
+    else:
+        remote = np.ascontiguousarray(log.remote, dtype=np.uint8)
+        roff = np.ascontiguousarray(log.remote_off, dtype=np.uint32)
+        start = np.ascontiguousarray(log.start_unix_ns, dtype=np.int64)
+        assert len(roff) == n + 1 and len(start) == n
+        line_cap, lout_cap = log.line_cap, log.out_cap
+        if line_cap is None or lout_cap is None:
+            lc, oc = conn_log_bound(off, roff)
+            line_cap = lc if line_cap is None else line_cap
+            lout_cap = oc if lout_cap is None else lout_cap
+        lout, log_off, log_req = alloc(lout_cap, np.uint8), alloc(line_cap + 1, np.uint32), alloc(line_cap, np.uint32)
+        cl = _abi.ConnLog(remote=remote.ctypes.data, remote_off=roff.ctypes.data, start_unix_ns=start.ctypes.data,
+                          log_unix_ns=log.log_unix_ns, tz_offset_s=log.tz_offset_s, line_cap=line_cap, out=lout.ctypes.data,
+                          out_cap=lout_cap, log_off=log_off.ctypes.data, log_req=log_req.ctypes.data)
+        _abi.check(L.gofr_conn_batch_submit_log(self._e, C.byref(cb), C.byref(cr), C.byref(cl), C.byref(t)),
+                   "gofr_conn_batch_submit_log")
     _abi.check(L.gofr_batch_wait(self._e, t.value), "gofr_batch_wait")
     k = int(req_first[n]) if n else 0
+    lines = None
+    if log is not None:
+        m = cl.lines
+        lines = ConnLogLines(lout[:int(cl.out_bytes)], log_off[:m + 1] if n else np.zeros(1, np.uint32), log_req[:m], m,
+                             int(cl.out_bytes))
     return ConnResponses(out[:int(cr.out_bytes)], out_off[:k + 1], meta[:k], req_at[:k], ids[:k * 16].reshape(k, 16),
-                         req_first[:n + 1] if n else np.zeros(1, np.uint32), consumed[:n], status[:n])
+                         req_first[:n + 1] if n else np.zeros(1, np.uint32), consumed[:n], status[:n], lines)
 
 
 Engine.serve_connections = _serve_connections

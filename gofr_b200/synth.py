@@ -413,3 +413,24 @@ def http_streams(n_conns: int, seed: int = SEED, reqs=(0, 5), tail_every: int = 
         conns.append(b"".join(parts))
     buf = np.frombuffer(b"".join(conns), dtype=np.uint8).copy()
     return buf, np.cumsum([0] + [len(x) for x in conns]).astype(np.uint32)
+
+
+def conn_clients(n_conns: int, seed: int = SEED, t0: int = 1_700_000_000_000_000_000):
+    """What gofr_conn_batch_submit_log takes per connection besides its bytes, seeded: the remote addresses (IPv4 host:port
+    and bracketed IPv6, as net/http's req.RemoteAddr) back to back, their offsets uint32[n_conns + 1], and each
+    connection's start clock (int64 unix ns, some on whole seconds, some with a nanosecond fraction)."""
+    idx = np.arange(n_conns, dtype=np.uint64)
+    r, r2 = rand_u64(seed, idx, 31), rand_u64(seed, idx, 32)
+    addrs = []
+    for a, b in zip(r.tolist(), r2.tolist()):
+        port = 1024 + (b >> 40) % 64000
+        if a % 5 == 0:
+            addrs.append(b"[2001:db8:%x::%x]:%d" % ((a >> 8) % 65536, (a >> 24) % 65536, port))
+        else:
+            addrs.append(b"%d.%d.%d.%d:%d" % ((a >> 8) % 256, (a >> 16) % 256, (a >> 24) % 256, (a >> 32) % 256, port))
+    remote = np.frombuffer(b"".join(addrs), dtype=np.uint8).copy()
+    remote_off = np.cumsum([0] + [len(x) for x in addrs]).astype(np.uint32)
+    start = (np.int64(t0) + idx.astype(np.int64) * 1_000_003 + (r2 % np.uint64(1_000_000)).astype(np.int64) * 1000
+             + np.where(r % np.uint64(7) == 0, (r2 >> np.uint64(20)) % np.uint64(1000), 0).astype(np.int64))
+    start = np.where(r % np.uint64(31) == 0, start - start % 1_000_000_000, start)
+    return remote, remote_off, start.astype(np.int64)

@@ -788,6 +788,55 @@ int gofr_conn_batch_submit(gofr_engine*, const gofr_conn_batch* in, gofr_conn_re
  * longer than its record).  No GPU needed.  GOFR_ERR_INVALID: null arguments, offsets that decrease. */
 int gofr_conn_batch_bound(const gofr_table*, const uint32_t* buf_off, uint32_t n_conns, uint32_t* req_cap, uint64_t* out_cap);
 
+/* gofr_conn_batch_submit plus middleware.Logging's RequestLog line (gofr_requestlog_device's format) for every request it
+ * answers on the device, in the same call.  With log == NULL it is gofr_conn_batch_submit.
+ * Which requests get a line: request k has one exactly when GOFR_META_ROUTE(meta[k]) != GOFR_ROUTE_NONE,
+ * GOFR_META_STATUS(meta[k]) != 0, and its method, User-Agent, first X-Forwarded-For value and target are each at most
+ * 65535 bytes (gofr_log_desc's length fields; the caller logs a longer one, as it logs a hole).  gorilla/mux wraps
+ * middleware around matched routes only, so the cleanPath 301 and mux's 404 / 405 are not logged; an OPTIONS request answered by CORS is (status 200: CORS runs inside Logging).  A hole
+ * (status 0: a GOFR_H_HOST closure) has no line here: the caller writes it once its closure has set the status.
+ * Each line's fields: method, user_agent and uri from the request head (its first User-Agent value, the request target);
+ * ip = getIPAddress of the first X-Forwarded-For value, or of the connection's remote string when its first element is
+ * empty; response = the status; start_time = start_unix_ns[c] of the request's connection; time = log_unix_ns; id = the
+ * request's trace id (the bytes of its X-Correlation-Id header).
+ *   in   remote / remote_off: connection c's req.RemoteAddr = remote[remote_off[c] .. remote_off[c+1]), n_conns + 1
+ *        non-decreasing offsets, each string at most 255 bytes.  start_unix_ns: n_conns clock readings.
+ *        log_unix_ns, tz_offset_s: the logger's clock and time.Local's offset at that instant, for every line.
+ *   out  line m = out[log_off[m] .. log_off[m+1]) (log_off has line_cap + 1 entries), lines in request order;
+ *        log_req[m] = the batch request index k of line m (ascending; line_cap entries);
+ *        lines, out_bytes: the lines and bytes of the batch (filled by submit, reported by wait).
+ * Capacity: when line_cap or out_cap is too small, wait returns GOFR_ERR_CAPACITY, nothing is written at or past either
+ * capacity, and lines / out_bytes are what the batch needed.  The response columns are complete whenever their own
+ * capacities suffice.  gofr_conn_log_bound gives capacities that always suffice.  log_off holds 32-bit offsets: a batch
+ * whose lines pass 4 GiB gets GOFR_ERR_CAPACITY whatever out_cap is.
+ * A chunk's log strings are placed in one buffer addressed with 32-bit offsets: a chunk whose staged bytes plus one remote
+ * string per possible request (one per 16 bytes plus one per connection) would pass 4 GiB is refused with
+ * GOFR_ERR_UNSUPPORTED (it takes a single connection of some hundred megabytes).
+ * GOFR_ERR_INVALID: gofr_conn_batch_submit's cases, a null log column (remote may be NULL when every string is empty),
+ * remote offsets that decrease or a string longer than 255 bytes. */
+typedef struct gofr_conn_log {
+    const uint8_t* remote;
+    const uint32_t* remote_off;    /* n_conns + 1 */
+    const int64_t* start_unix_ns;  /* n_conns: Logging's `start := time.Now()` for the connection's requests */
+    int64_t log_unix_ns;           /* the logger's time.Now(): response_time = (log_unix_ns - start) / 1000 µs */
+    int32_t tz_offset_s;           /* time.Local's offset at that instant, seconds east of UTC */
+    uint32_t line_cap;
+    uint8_t* out;
+    uint64_t out_cap;
+    uint32_t* log_off;             /* line_cap + 1 */
+    uint32_t* log_req;             /* line_cap */
+    uint32_t lines;
+    uint32_t reserved;
+    uint64_t out_bytes;
+} gofr_conn_log;
+int gofr_conn_batch_submit_log(gofr_engine*, const gofr_conn_batch* in, gofr_conn_resp* out, gofr_conn_log* log,
+                               gofr_ticket* ticket);
+/* Capacities that always suffice for gofr_conn_batch_submit_log's lines: one request per 16 buffer bytes plus one per
+ * connection, each a line of at most 320 bytes plus 6 per byte of its head and of its connection's remote string.  No GPU
+ * needed.  GOFR_ERR_INVALID: null arguments, offsets that decrease, a remote string longer than 255 bytes. */
+int gofr_conn_log_bound(const uint32_t* buf_off, const uint32_t* remote_off, uint32_t n_conns, uint32_t* line_cap,
+                        uint64_t* out_cap);
+
 /* number of kernels launched by this engine so far (bench.py reports it as gpu_launches) */
 uint64_t gofr_engine_launch_count(const gofr_engine*);
 /* duration in ms of the kernels launched since the last reset, measured with CUDA events on the launch stream.  Every
