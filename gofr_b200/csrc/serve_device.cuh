@@ -290,6 +290,59 @@ struct LineStores {
             }
 #endif
     }
+    // Windows [0, nwin) of every lane's template into its slot at dst, straight from the literal pool (tp), except windows
+    // [h0, h1), which the lane has staged from row 0 of its column at col (stage_trace_id).  The warp numbers the windows
+    // of its 32 responses in request order (an exclusive sum of nwin) and lane L stores windows L, L + 32, ... of that
+    // sequence, so consecutive lanes store consecutive windows of a response and one warp store covers the templates of
+    // two or three whole responses.  The owner of window g is the lane whose range holds it: g / nwin when every lane has
+    // the same count, else a search over the shuffled prefix.  A lane with nothing to write passes nwin 0.  On the host
+    // (tests/emu) a lane stores its own windows.
+    GOFR_HD void templates(uint8_t* dst, saddr_t tp, uint32_t nwin, uint32_t h0, uint32_t h1, saddr_t col) const {
+#if defined(__CUDA_ARCH__)
+        const uint32_t lane = threadIdx.x & 31u;
+        uint32_t incl = nwin;
+#pragma unroll
+        for (uint32_t o = 1; o < 32; o <<= 1) {
+            const uint32_t u = __shfl_up_sync(wm, incl, o);
+            if (lane >= o) incl += u;
+        }
+        const uint32_t total = __shfl_sync(wm, incl, 31);
+        if (!total) return;
+        const uint32_t first = incl - nwin, n0 = __shfl_sync(wm, nwin, 0);
+        const bool uniform = __all_sync(wm, nwin == n0);
+        const uint32_t rec = first | h0 << 16 | h1 << 24;  // first < 32 * 256; h0 <= h1 <= nwin < 256
+        __syncwarp(wm);  // the owners' staged windows before the other lanes' loads
+#pragma unroll 1
+        for (uint32_t g0 = 0; g0 < total; g0 += 32u) {
+            const uint32_t g = g0 + lane;
+            const bool have = g < total;
+            uint32_t s = 0;
+            if (uniform) {
+                s = have ? g / n0 : lane;
+            } else {
+#pragma unroll
+                for (uint32_t b = 16; b; b >>= 1)
+                    if (__shfl_sync(wm, first, s + b) <= g) s += b;
+            }
+            const uint32_t r = __shfl_sync(wm, rec, s);
+            const saddr_t src = __shfl_sync(wm, tp, s);
+            uint8_t* const d = (uint8_t*)__shfl_sync(wm, (unsigned long long)dst, s);
+            const uint32_t k = g - (r & 0xFFFFu), k0 = (r >> 16) & 0xFFu, k1 = r >> 24;
+            const bool staged = k >= k0 && k < k1;
+            const saddr_t rp = staged ? col + 4u * (s - lane) + (k - k0) * 4u * kStride : src + 16u * k;
+            const uint32_t st = staged ? kStride : 4u;
+            if (have) store16(d + 16u * k, stg_ld(rp), stg_ld(rp + st), stg_ld(rp + 2u * st), stg_ld(rp + 3u * st));
+        }
+        __syncwarp(wm);  // every load of a column before its owner appends the tail to it
+#else
+        for (uint32_t k = 0; k < nwin; k++) {
+            const bool staged = k >= h0 && k < h1;
+            const saddr_t rp = staged ? col + (k - h0) * 4u * kStride : tp + 16u * k;
+            const uint32_t st = staged ? kStride : 4u;
+            store16(dst + 16u * k, stg_ld(rp), stg_ld(rp + st), stg_ld(rp + 2u * st), stg_ld(rp + 3u * st));
+        }
+#endif
+    }
 };
 
 #if !defined(__CUDACC__)
@@ -1651,12 +1704,37 @@ GOFR_HD void copy_windows(uint8_t* dst, saddr_t src, uint32_t k0, uint32_t k1, S
     }
 }
 
-// Writes a response sized by size_fast into its 16-byte aligned slot.  SoloStores: the template with aligned 16-byte
-// loads and stores, the trace id patched into the windows it touches, then the tail ops through the Writer.
-// LineStores: everything goes through the Writer's column — the template as a copy from the literal pool with the 8
-// words of the trace id put in at hex_pos — and every lane of the write mask runs every vote and store round below,
-// also when its program has no template or no tail: a lane past its last op, or on an op that writes nothing, copies 0
-// bytes.  Only the appending of words differs between lanes.
+// Windows [h0, h1) of the template at tp, the 2 or 3 that the 32 hex characters of the trace id touch, staged in the lane's
+// (idle) Writer column at col, whose rows are S bytes apart: the template's words from row 0 on, then the 8 hex words of
+// `id` shifted to byte hex_pos & 15 of window h0 on top.  The store policy stores the windows from there (emit_fast).
+template <uint32_t S>
+GOFR_HD void stage_trace_id(saddr_t col, saddr_t tp, uint32_t hex_pos, uint32_t h0, uint32_t h1, uint4 id) {
+    const uint32_t nw = (h1 - h0) * 4;  // 8 or 12 words
+#pragma unroll 1
+    for (uint32_t k = 0; k < nw; k++) stg_st(col + k * S, src_ld(tp + 16 * h0 + 4 * k));
+    uint32_t H[8];
+    hex8(id.x, H[0], H[1]); hex8(id.y, H[2], H[3]); hex8(id.z, H[4], H[5]); hex8(id.w, H[6], H[7]);
+    const uint32_t o = hex_pos & 15u, q = o >> 2, sh = (o & 3u) * 8;
+    const saddr_t hp = col + q * S;
+    if (sh == 0) {
+#pragma unroll
+        for (uint32_t j = 0; j < 8; j++) stg_st(hp + j * S, H[j]);
+    } else {
+        const uint32_t lowmask = (1u << sh) - 1u;
+        stg_st(hp, (stg_ld(hp) & lowmask) | (H[0] << sh));
+#pragma unroll
+        for (uint32_t j = 1; j < 8; j++) stg_st(hp + j * S, fsr(H[j - 1], H[j], 32 - sh));
+        stg_st(hp + 8 * S, (H[7] >> (32 - sh)) | (stg_ld(hp + 8 * S) & ~lowmask));
+    }
+}
+
+// Writes a response sized by size_fast into its 16-byte aligned slot: the template as whole 16-byte windows from the
+// literal pool, the windows the trace id touches staged in the lane's column first (stage_trace_id), then the tail ops
+// through the Writer, which starts right after the template.  The store policies differ only in how the template windows
+// leave.  SoloStores: each lane its own, the plain windows in whole sectors where the slot allows (copy_windows).
+// LineStores: the warp stores the templates of all its lanes together (LineStores::templates), and every lane of the
+// write mask runs every vote and store round of the tail, also when its program has no template or no tail: a lane past
+// its last op, or on an op that writes nothing, copies 0 bytes.  Only the appending of words differs between lanes.
 // live false (LineStores): the lane has no response and runs an empty one — votes and store rounds, no loads, no stores.
 template <typename P>
 GOFR_HD void emit_fast(const TableView& tv, const BatchRefs& br, ReqCtx& c, uint8_t* dst, uint32_t* ring_col, P p,
@@ -1669,60 +1747,31 @@ GOFR_HD void emit_fast(const TableView& tv, const BatchRefs& br, ReqCtx& c, uint
     WriterT<P> w;
     // the Writer's room check before a value: SoloStores flushes whole sectors once 8 words wait, LineStores has a line
     constexpr uint32_t kFull = P::kLockstep ? 32u : GOFR_SOLO_WORDS - 8;
-    if constexpr (P::kLockstep) {
-        w.init(dst, ring_col);
-        const uint8_t* const tp = tv.lits() + F.tmpl_off;
-        const bool hex = nwin && F.hex_pos != 0xFFFFu;
-        const uint32_t h = hex ? (uint32_t)F.hex_pos : 16 * nwin;  // template bytes before the trace id
-        w.template copy<true>(SrcMem<true>::from(tp), h, p);
-        if (p.vote(w.wl >= kFull)) w.flush(p);
-        if (hex) {
-            uint32_t H[8];
-            hex8(id.x, H[0], H[1]); hex8(id.y, H[2], H[3]); hex8(id.z, H[4], H[5]); hex8(id.w, H[6], H[7]);
-#pragma unroll
-            for (uint32_t j = 0; j < 8; j++) w.put4(H[j]);
-        }
-        w.template copy<true>(SrcMem<true>::from(hex ? tp + h + 32 : tp), hex ? 16 * nwin - h - 32 : 0u, p);
-    } else {
-        if (nwin) {
-            const saddr_t tp = to_saddr(tv.lits() + F.tmpl_off);
-            const saddr_t col = to_saddr(ring_col);
-            uint32_t h0 = nwin, h1 = nwin;  // [h0, h1): windows the 32 hex characters touch
-            if (F.hex_pos != 0xFFFFu) { h0 = (uint32_t)F.hex_pos >> 4; h1 = (((uint32_t)F.hex_pos + 31u) >> 4) + 1u; }
+    if (P::kLockstep || nwin) {
+        const saddr_t tp = to_saddr(tv.lits() + F.tmpl_off);
+        const saddr_t col = to_saddr(ring_col);
+        uint32_t h0 = nwin, h1 = nwin;  // [h0, h1): windows the 32 hex characters touch
+        if (F.hex_pos != 0xFFFFu) { h0 = (uint32_t)F.hex_pos >> 4; h1 = (((uint32_t)F.hex_pos + 31u) >> 4) + 1u; }
+        if constexpr (P::kLockstep) {
+            if (h0 < nwin) stage_trace_id<P::kStride>(col, tp, F.hex_pos, h0, h1, id);
+            p.templates(dst, tp, nwin, h0, h1, col);
+        } else {
             copy_windows(dst, tp, 0, h0, p);
             copy_windows(dst, tp + 16 * h1, h1, nwin, p);
             if (h0 < nwin) {
-                // the 2 or 3 windows around the trace id: template words into the (idle) staging column, the 8 hex words
-                // shifted to their byte offset on top, then whole windows out, one at a time (as whole sectors the
-                // 5-CTA slot instance took 4 % longer on config 4, well outside the run-to-run spread: DESIGN §6)
-                const uint32_t nw = (h1 - h0) * 4;  // 8 or 12 words
-#pragma unroll 1
-                for (uint32_t k = 0; k < nw; k++) stg_st(col + k * GOFR_RING_STRIDE_BYTES, src_ld(tp + 16 * h0 + 4 * k));
-                uint32_t H[8];
-                hex8(id.x, H[0], H[1]); hex8(id.y, H[2], H[3]); hex8(id.z, H[4], H[5]); hex8(id.w, H[6], H[7]);
-                const uint32_t o = (uint32_t)F.hex_pos & 15u, q = o >> 2, sh = (o & 3u) * 8;
-                const saddr_t hp = col + q * GOFR_RING_STRIDE_BYTES;
-                if (sh == 0) {
-#pragma unroll
-                    for (uint32_t j = 0; j < 8; j++) stg_st(hp + j * GOFR_RING_STRIDE_BYTES, H[j]);
-                } else {
-                    const uint32_t lowmask = (1u << sh) - 1u;
-                    stg_st(hp, (stg_ld(hp) & lowmask) | (H[0] << sh));
-#pragma unroll
-                    for (uint32_t j = 1; j < 8; j++) stg_st(hp + j * GOFR_RING_STRIDE_BYTES, fsr(H[j - 1], H[j], 32 - sh));
-                    stg_st(hp + 8 * GOFR_RING_STRIDE_BYTES, (H[7] >> (32 - sh)) | (stg_ld(hp + 8 * GOFR_RING_STRIDE_BYTES) & ~lowmask));
-                }
+                // the 2 or 3 windows around the trace id go out whole, one at a time (as whole sectors the 5-CTA slot
+                // instance took 4 % longer on config 4, well outside the run-to-run spread: DESIGN §6)
+                stage_trace_id<P::kStride>(col, tp, F.hex_pos, h0, h1, id);
 #pragma unroll 1
                 for (uint32_t k = h0; k < h1; k++) {
-                    const saddr_t rp = col + (k - h0) * 4 * GOFR_RING_STRIDE_BYTES;
-                    store16(dst + 16 * k, stg_ld(rp), stg_ld(rp + GOFR_RING_STRIDE_BYTES), stg_ld(rp + 2 * GOFR_RING_STRIDE_BYTES),
-                            stg_ld(rp + 3 * GOFR_RING_STRIDE_BYTES));
+                    const saddr_t rp = col + (k - h0) * 4 * P::kStride;
+                    store16(dst + 16 * k, stg_ld(rp), stg_ld(rp + P::kStride), stg_ld(rp + 2 * P::kStride), stg_ld(rp + 3 * P::kStride));
                 }
             }
         }
-        if (F.flags & FR_COMPLETE) return;
-        w.init(dst + 16 * nwin, ring_col);
     }
+    if (!P::kLockstep && (F.flags & FR_COMPLETE)) return;
+    w.init(dst + 16 * nwin, ring_col);
     // a template-only program: with LineStores its Writer runs the tail with no ops, appending nothing but taking part in
     // the votes and store rounds
     const uint32_t n_ops = (F.flags & FR_COMPLETE) ? 0u : F.n_tail_ops;
