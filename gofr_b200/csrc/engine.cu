@@ -19,6 +19,7 @@
 
 #include <algorithm>
 #include <functional>
+#include <initializer_list>
 #include <mutex>
 #include <string>
 #include <vector>
@@ -153,7 +154,7 @@ struct Slot {
     uint8_t* d_larena = nullptr; uint8_t* d_lraw = nullptr; uint8_t* d_lout = nullptr;
     size_t cap_remote = 0, cap_lconns = 0, cap_lrecs = 0, cap_larena = 0, cap_lraw = 0, cap_lout = 0;
     // pinned staging for the tiny per-chunk read-backs
-    uint32_t* h_tail = nullptr;  // [0] = chunk total bytes, [1] = overflow flag; connection log: [2] lines, [3] overflow
+    uint32_t* h_tail = nullptr;  // [0] = chunk total bytes (connections: records), [1] = overflow flag; log: [2] lines, [3] overflow
 
     int reserve(gofr_engine* e, uint32_t requests, size_t arena_bytes, size_t out_bytes);
     int reserve_codec(uint32_t records, size_t a_bytes, size_t b_bytes);
@@ -746,6 +747,26 @@ static int grow(void** p, size_t* cap, size_t need, size_t slack) {
     return GOFR_OK;
 }
 
+// One per-element device column of a group: per bytes per element plus extra bytes (none allocated when both are 0).
+struct Col { void* p; size_t per, extra; };
+
+// Grows a group of per-element columns (capacity *cap elements, `what` names the elements in the error) to hold n: all of
+// them are freed and reallocated at n + n/4 + 256 elements.  Columns of n + 1 entries ask for one element extra; the
+// kernels rely on every extra byte.
+static int grow_cols(size_t* cap, size_t n, const char* what, std::initializer_list<Col> cols) {
+    if (n <= *cap) return GOFR_OK;
+    for (const Col& k : cols) { cudaFree(*(void**)k.p); *(void**)k.p = nullptr; }
+    *cap = 0;
+    const size_t c = n + n / 4 + 256;
+    for (const Col& k : cols)
+        if ((k.per || k.extra) && cudaMalloc((void**)k.p, c * k.per + k.extra) != cudaSuccess) {
+            set_last_error("cudaMalloc failed for a chunk of %zu %s", c, what);
+            return GOFR_ERR_NOMEM;
+        }
+    *cap = c;
+    return GOFR_OK;
+}
+
 // The copy loops read their source in whole aligned words: up to 16 bytes past the last byte a request names may be touched
 // (include/gofr_b200.h states the same for device-resident callers), so a staging arena is never sized to the byte.
 static constexpr size_t kArenaSlack = 16;
@@ -819,19 +840,9 @@ static int wait_egress(gofr_engine* e, Slot& s, bool grows) {
 // Makes the slot's buffers ready for a chunk of `requests` requests, `arena_bytes` arena bytes and `out_bytes` of output.
 int Slot::reserve(gofr_engine* e, uint32_t requests, size_t arena_bytes, size_t out_bytes) {
     { int rc = wait_egress(e, *this, requests > cap_n || arena_bytes + kArenaSlack > cap_arena || out_bytes > cap_out); if (rc) return rc; }
-    if (requests > cap_n) {
-        cudaFree(d_desc); cudaFree(d_ids); cudaFree(d_off); cudaFree(d_meta); cudaFree(d_bind);
-        d_desc = d_ids = nullptr; d_off = d_meta = nullptr; d_bind = nullptr;
-        cap_n = 0;
-        const size_t c = (size_t)requests + requests / 4 + 256;
-        if (cudaMalloc(&d_desc, c * 16) != cudaSuccess || cudaMalloc(&d_ids, c * 16) != cudaSuccess ||
-            cudaMalloc(&d_off, (c + 1) * 4) != cudaSuccess || cudaMalloc(&d_meta, c * 4) != cudaSuccess ||
-            (e->hdr.bind_row_words && cudaMalloc(&d_bind, c * e->hdr.bind_row_words * 4 + 256) != cudaSuccess)) {
-            set_last_error("cudaMalloc failed for a %zu-request chunk", c);
-            return GOFR_ERR_NOMEM;
-        }
-        cap_n = c;
-    }
+    const size_t bind = (size_t)e->hdr.bind_row_words * 4;
+    { int rc = grow_cols(&cap_n, requests, "requests", {{&d_desc, 16, 0}, {&d_ids, 16, 0}, {&d_off, 4, 4}, {&d_meta, 4, 0},
+                                                         {&d_bind, bind, bind ? 256u : 0u}}); if (rc) return rc; }
     if (!d_flag && (cudaMalloc(&d_flag, 64) != cudaSuccess || cudaMemset(d_flag, 0, 64) != cudaSuccess)) {
         set_last_error("cudaMalloc failed for a chunk's overflow flag");
         return GOFR_ERR_NOMEM;
@@ -844,19 +855,9 @@ int Slot::reserve(gofr_engine* e, uint32_t requests, size_t arena_bytes, size_t 
 // chunk's own kernels use them, and a buffer that grows is freed by cudaFree, which waits for the device.  The copy of the
 // pack kernel reads a source word past its last byte: grow's slack covers it.
 int Slot::reserve_codec(uint32_t records, size_t a_bytes, size_t b_bytes) {
-    if (records > cap_codec_n) {
-        cudaFree(d_in_off); cudaFree(d_meta1); cudaFree(d_codec_off[0]); cudaFree(d_codec_off[1]);
-        d_in_off = d_meta1 = d_codec_off[0] = d_codec_off[1] = nullptr;
-        cap_codec_n = 0;
-        const size_t c = (size_t)records + records / 4 + 256;
-        if (cudaMalloc(&d_in_off, (c + 1) * 4) != cudaSuccess || cudaMalloc(&d_meta1, c * 4) != cudaSuccess ||
-            cudaMalloc(&d_codec_off[0], (c + 1) * 4) != cudaSuccess || cudaMalloc(&d_codec_off[1], (c + 1) * 4) != cudaSuccess) {
-            set_last_error("cudaMalloc failed for a %zu-record chunk", c);
-            return GOFR_ERR_NOMEM;
-        }
-        cap_codec_n = c;
-    }
-    int rc = grow((void**)&d_codec[0], &cap_codec[0], a_bytes, 256);
+    int rc = grow_cols(&cap_codec_n, records, "records", {{&d_in_off, 4, 4}, {&d_meta1, 4, 0}, {&d_codec_off[0], 4, 4},
+                                                          {&d_codec_off[1], 4, 4}});
+    if (!rc) rc = grow((void**)&d_codec[0], &cap_codec[0], a_bytes, 256);
     return rc ? rc : grow((void**)&d_codec[1], &cap_codec[1], b_bytes, 256);
 }
 
@@ -879,37 +880,22 @@ static void drain_streams(gofr_engine* e) {
     cudaGetLastError();
 }
 
-static int batch_submit_locked(gofr_engine* e, const gofr_req_batch* in, gofr_resp_batch* out, gofr_ticket* ticket);
-static int batch_submit_slots_locked(gofr_engine* e, const gofr_req_batch* in, gofr_slot_batch* out, gofr_ticket* ticket);
-
-int gofr_batch_submit(gofr_engine* e, const gofr_req_batch* in, gofr_resp_batch* out, gofr_ticket* ticket) {
-    if (!e || !in || !out || !ticket) return GOFR_ERR_INVALID;
-    if (in->n && (!in->desc || !in->trace_ids || !out->out || !out->out_off || !out->meta)) return GOFR_ERR_INVALID;
+// Runs a host-batch call under the engine lock.  Its input is validated chunk by chunk as the batch is enqueued (an
+// up-front scan of 1 Mi records is milliseconds of pure latency), so an error can surface with earlier chunks in flight:
+// nothing may still be writing into the caller's buffers when the error is returned.
+static int host_batch(gofr_engine* e, const std::function<int()>& run) {
     std::lock_guard<std::mutex> g(e->mu);
     CUDA_TRY(cudaSetDevice(e->device));
-    // Descriptors are validated chunk by chunk as the batch is enqueued (an up-front scan of 1 Mi descriptors is
-    // milliseconds of pure latency), so an error can surface with earlier chunks in flight: nothing may still be
-    // writing into the caller's buffers when the error is returned.
-    const int rc = batch_submit_locked(e, in, out, ticket);
+    const int rc = run();
     if (rc != GOFR_OK) drain_streams(e);
     return rc;
 }
 
-// The chunk pipeline of the host-batch calls with a packed output (gofr_batch_submit, gofr_proto_batch_decode / _encode).
-// What differs between them:
-//   plan     the chunk that starts at record lo: its end, its input byte range and a bound on its device output; the
-//            records' input is validated here, chunk by chunk (an up-front scan of 1 Mi records is milliseconds of pure
-//            latency), so an error can surface with earlier chunks in flight (the caller drains the streams);
-//   upload   the H2D copies of the chunk's input into the slot (and any buffers of the caller's own it needs);
-//   compute  the kernels that leave the chunk's packed output in the slot's d_out / d_off / d_meta, placed at
-//            *chain_pos & 15 when chain_pos is given (the serve kernel's convention), at 0 otherwise.
-// The pipeline reserves the slot, then runs upload, compute, advance and egress (pinned caller buffers) or an exact-size
-// copy (pageable ones).
-struct ChunkSteps {
-    std::function<int(uint32_t lo, ChunkPlan* c)> plan;
-    std::function<int(Slot& s, const ChunkPlan& c, cudaStream_t st)> upload;
-    std::function<int(Slot& s, const ChunkPlan& c, cudaStream_t st, const unsigned long long* chain_pos)> compute;
-};
+// A finished submit: its result waits for gofr_batch_wait under a new ticket.
+static void complete(gofr_engine* e, gofr_ticket* ticket, int rc) {
+    *ticket = e->next_ticket++;
+    e->done_tickets.emplace_back(*ticket, rc);
+}
 
 // Host memory the device can write (pinned or managed): the egress kernel stores into it directly
 static bool device_visible(const void* p) {
@@ -918,20 +904,107 @@ static bool device_visible(const void* p) {
     return a.type == cudaMemoryTypeHost || a.type == cudaMemoryTypeManaged;
 }
 
-static int run_chunks(gofr_engine* e, uint32_t n, const ChunkSteps& steps, gofr_resp_batch* out, gofr_ticket* ticket) {
-    out->out_bytes = 0;
-    int final_rc = GOFR_OK;
-    if (n == 0) {  // nothing to do; the caller may have passed no buffers at all
-        if (out->out_off) out->out_off[0] = 0;
-        *ticket = e->next_ticket++;
-        e->done_tickets.emplace_back(*ticket, GOFR_OK);
+// A packed output of a host-batch call: the caller's bytes, their offsets and the one per-record column egress carries
+// (meta, or log_req).  Output k (0: responses or proto rows, 1: request-log lines) owns d_chain[k], h_status[2k..],
+// d_info[k * kSlots ..], each slot's overflow word d_flag[k] and h_ends[4 ci + 2k ..].  Pinned buffers are filled by
+// advance and egress without the host waiting (deliver), pageable ones get each chunk's exact bytes (retire).  Both skip a
+// chunk's bytes when the device overflowed or when they would pass cap or 4 GiB (32-bit offsets): the batch then fails.
+struct PackedOut {
+    uint8_t* out = nullptr;
+    uint64_t cap = 0;
+    uint32_t* off = nullptr;
+    uint32_t* col = nullptr;
+    int k = 0;
+    bool pinned = false;
+    uint64_t written = 0, at = 0;  // bytes written (pinned: after finish); pageable: where the last retired chunk went
+    bool overflow = false;         // some chunk's bytes were skipped (pinned: after finish)
+
+    PackedOut() = default;
+    PackedOut(uint8_t* o, uint64_t c, uint32_t* f, uint32_t* m, int k_)
+        : out(o), cap(c), off(f), col(m), k(k_), pinned(device_visible(o) && device_visible(f) && device_visible(m)) {}
+    unsigned long long* chain(gofr_engine* e) const { return pinned ? e->d_chain + k : nullptr; }
+    uint32_t* ends(gofr_engine* e, size_t ci) const { return e->h_ends + 4 * ci + 2 * k; }  // chunk ci's first, end offset
+    uint64_t needed(gofr_engine* e, size_t chunks) const {
+        uint64_t b = 0;
+        for (size_t ci = 0; ci < chunks; ci++) b += ends(e, ci)[1] - ends(e, ci)[0];
+        return b;
+    }
+    int start(gofr_engine* e) {
+        if (!pinned) return GOFR_OK;
+        CUDA_TRY(cudaMemsetAsync(e->d_chain + k, 0, 8, e->st_compute));
+        e->h_status[2 * k] = e->h_status[2 * k + 1] = 0;
         return GOFR_OK;
     }
-    // ---- streaming path: caller buffers are pinned → egress is device driven, the host never blocks mid-batch ----
-    if (device_visible(out->out) && device_visible(out->out_off) && device_visible(out->meta)) {
-        // growing buffers frees memory: make sure nothing from an earlier batch is still using them
-        CUDA_TRY(cudaMemsetAsync(e->d_chain, 0, 8, e->st_compute));
-        e->h_status[0] = 0; e->h_status[1] = 0;
+    // After the chunk's kernels on st_compute: advance, then egress of its n records to the caller's from `first` on
+    // st_egress.  Without put (a count capacity is short) neither runs and the overflow word is cleared.  The caller adds
+    // its own columns on st_egress, then records s.ev_egress.
+    int deliver(gofr_engine* e, Slot& s, size_t ci, const uint8_t* d_out, const uint32_t* d_off, const uint32_t* d_col,
+                uint32_t n, uint64_t first, bool put) {
+        ChunkInfo* info = e->d_info + k * kSlots + ci % kSlots;
+        if (put && launch_advance(e->d_chain + k, d_off, n, s.d_flag + k, info, cap, e->st_compute) != 0) {
+            set_last_error("advance kernel launch failed"); return GOFR_ERR_CUDA;
+        }
+        if (!put) CUDA_TRY(cudaMemsetAsync(s.d_flag + k, 0, 4, e->st_compute));
+        CUDA_TRY(cudaEventRecord(s.ev_served, e->st_compute));
+        CUDA_TRY(cudaStreamWaitEvent(e->st_egress, s.ev_served, 0));
+        if (put && launch_egress(info, d_out, d_off, d_col, n, out, off + first, col + first, e->h_status + 2 * k,
+                                 e->egress_grid, e->st_egress) != 0) {
+            set_last_error("egress kernel launch failed"); return GOFR_ERR_CUDA;
+        }
+        if (put) e->launches += 2;
+        return GOFR_OK;
+    }
+    // A chunk of `total` bytes at d_out, with the overflow word `flag` the caller read back (cleared here when set): unless
+    // put is false or the rule skips it, its bytes are copied to out + written on st and rebase() places its offsets.
+    int retire(Slot& s, const uint8_t* d_out, uint32_t total, uint32_t flag, bool put, cudaStream_t st, bool* wrote) {
+        if (flag) CUDA_TRY(cudaMemsetAsync(s.d_flag + k, 0, 4, st));
+        *wrote = put && !flag && written + total <= cap && written + total <= 0xFFFFFFFFull;
+        overflow |= flag || (put && !*wrote);
+        if (*wrote && total) CUDA_TRY(cudaMemcpyAsync(out + written, d_out, total, cudaMemcpyDeviceToHost, st));
+        if (*wrote) { at = written; written += total; }
+        return GOFR_OK;
+    }
+    void rebase(uint64_t first, uint32_t n) const { if (at) for (uint64_t i = first; i < first + n; i++) off[i] += (uint32_t)at; }
+    // Reads the pinned outputs' chain words back behind their egress and waits for it once.
+    static int finish(gofr_engine* e, uint32_t n, std::initializer_list<PackedOut*> outs) {
+        bool wait = false;
+        for (PackedOut* o : outs) {
+            if (o->pinned) CUDA_TRY(cudaMemcpyAsync(&e->h_status[2 * o->k], e->d_chain + o->k, 8, cudaMemcpyDeviceToHost, e->st_egress));
+            wait |= o->pinned;
+        }
+        if (!wait) return GOFR_OK;
+        CUDA_TRY(wait_batch(e, n));
+        for (auto& s : e->slots) s.egress_pending = false;
+        for (PackedOut* o : outs)
+            if (o->pinned) { o->written = e->h_status[2 * o->k]; o->overflow = e->h_status[2 * o->k + 1] != 0; }
+        return GOFR_OK;
+    }
+};
+
+// The chunk pipeline of the host-batch calls with a packed output (gofr_batch_submit, gofr_proto_batch_decode / _encode).
+// What differs between them:
+//   plan     the chunk that starts at record lo: its end, its input byte range and a bound on its device output; the
+//            records' input is validated here, chunk by chunk (see host_batch);
+//   upload   the H2D copies of the chunk's input into the slot (and any buffers of the caller's own it needs);
+//   compute  the kernels that leave the chunk's packed output in the slot's d_out / d_off / d_meta, placed at
+//            *chain_pos & 15 when chain_pos is given (the serve kernel's convention), at 0 otherwise.
+// The pipeline reserves the slot, then runs upload and compute and hands the chunk to its PackedOut.
+struct ChunkSteps {
+    std::function<int(uint32_t lo, ChunkPlan* c)> plan;
+    std::function<int(Slot& s, const ChunkPlan& c, cudaStream_t st)> upload;
+    std::function<int(Slot& s, const ChunkPlan& c, cudaStream_t st, const unsigned long long* chain_pos)> compute;
+};
+
+static int run_chunks(gofr_engine* e, uint32_t n, const ChunkSteps& steps, gofr_resp_batch* out, gofr_ticket* ticket) {
+    out->out_bytes = 0;
+    if (n == 0) {  // nothing to do; the caller may have passed no buffers at all
+        if (out->out_off) out->out_off[0] = 0;
+        complete(e, ticket, GOFR_OK);
+        return GOFR_OK;
+    }
+    PackedOut o(out->out, out->out_cap, out->out_off, out->meta, 0);
+    { int rc = o.start(e); if (rc) return rc; }
+    if (o.pinned) {  // ---- streaming path: egress is device driven, the host never blocks mid-batch ----
         size_t ci = 0;
         for (uint32_t lo = 0; lo < n; ci++) {
             Slot& s = e->slots[ci % kSlots];
@@ -944,78 +1017,53 @@ static int run_chunks(gofr_engine* e, uint32_t n, const ChunkSteps& steps, gofr_
             if (rc) return rc;
             CUDA_TRY(cudaEventRecord(s.ev_h2d, e->st_h2d));
             CUDA_TRY(cudaStreamWaitEvent(e->st_compute, s.ev_h2d, 0));
-            rc = steps.compute(s, c, e->st_compute, e->d_chain);
+            rc = steps.compute(s, c, e->st_compute, o.chain(e));
+            if (!rc) rc = o.deliver(e, s, ci, s.d_out, s.d_off, s.d_meta, cn, c.lo, true);
             if (rc) return rc;
-            if (launch_advance(e->d_chain, s.d_off, cn, s.d_flag, e->d_info + (ci % kSlots), out->out_cap, e->st_compute) != 0) {
-                set_last_error("advance kernel launch failed"); return GOFR_ERR_CUDA;
-            }
-            CUDA_TRY(cudaEventRecord(s.ev_served, e->st_compute));
-            CUDA_TRY(cudaStreamWaitEvent(e->st_egress, s.ev_served, 0));
-            if (launch_egress(e->d_info + (ci % kSlots), s.d_out, s.d_off, s.d_meta, cn, out->out, out->out_off + c.lo,
-                              out->meta + c.lo, e->h_status, e->egress_grid, e->st_egress) != 0) {
-                set_last_error("egress kernel launch failed"); return GOFR_ERR_CUDA;
-            }
             CUDA_TRY(cudaEventRecord(s.ev_egress, e->st_egress));
             s.egress_pending = true;
-            e->launches += 2;
         }
-        CUDA_TRY(cudaMemcpyAsync((void*)&e->h_status[0], e->d_chain, 8, cudaMemcpyDeviceToHost, e->st_egress));
-        CUDA_TRY(wait_batch(e, n));
-        for (auto& s : e->slots) s.egress_pending = false;
-        uint64_t total = e->h_status[0];
-        if (e->h_status[1]) { final_rc = GOFR_ERR_CAPACITY; set_last_error("output capacity too small (device chunk buffer or caller buffer)"); }
-        out->out_off[n] = (uint32_t)total;
-        out->out_bytes = total;
-        *ticket = e->next_ticket++;
-        e->done_tickets.emplace_back(*ticket, final_rc);
-        return GOFR_OK;
-    }
-
-    // ---- pageable caller buffers: 3-slot software pipeline, each chunk's exact size copied back once it is known ----
-    size_t issued = 0, finished = 0;
-    uint32_t next_lo = 0;
-    ChunkPlan inflight[kSlots];
-    uint64_t write_pos = 0;
-    // issue order == completion order == chunk order; out offsets are rebased on the host as chunks complete
-    while (next_lo < n || finished < issued) {
-        // keep up to kSlots chunks in flight
-        while (next_lo < n && issued - finished < (size_t)kSlots) {
-            int si = (int)(issued % kSlots);
-            Slot& s = e->slots[si];
-            ChunkPlan& c = inflight[si];
-            { int prc = steps.plan(next_lo, &c); if (prc) return prc; }
-            next_lo = c.hi;
-            uint32_t cn = c.hi - c.lo;
-            int rc = s.reserve(e, cn, (size_t)c.arena_hi - c.arena_lo, c.out_bound);
-            if (!rc) rc = steps.upload(s, c, s.stream);
-            if (!rc) rc = steps.compute(s, c, s.stream, nullptr);
-            if (rc) return rc;
-            CUDA_TRY(cudaMemcpyAsync(out->out_off + c.lo, s.d_off, (size_t)cn * 4, cudaMemcpyDeviceToHost, s.stream));
-            CUDA_TRY(cudaMemcpyAsync(out->meta + c.lo, s.d_meta, (size_t)cn * 4, cudaMemcpyDeviceToHost, s.stream));
-            CUDA_TRY(cudaMemcpyAsync(&s.h_tail[0], s.d_off + cn, 4, cudaMemcpyDeviceToHost, s.stream));
-            CUDA_TRY(cudaMemcpyAsync(&s.h_tail[1], s.d_flag, 4, cudaMemcpyDeviceToHost, s.stream));
-            CUDA_TRY(cudaEventRecord(s.done, s.stream));
-            issued++;
+    } else {  // ---- pageable: 3-slot software pipeline, each chunk's exact size copied back once it is known ----
+        size_t issued = 0, finished = 0;
+        uint32_t next_lo = 0;
+        ChunkPlan inflight[kSlots];
+        // issue order == completion order == chunk order; out offsets are rebased on the host as chunks complete
+        while (next_lo < n || finished < issued) {
+            // keep up to kSlots chunks in flight
+            while (next_lo < n && issued - finished < (size_t)kSlots) {
+                int si = (int)(issued % kSlots);
+                Slot& s = e->slots[si];
+                ChunkPlan& c = inflight[si];
+                { int prc = steps.plan(next_lo, &c); if (prc) return prc; }
+                next_lo = c.hi;
+                uint32_t cn = c.hi - c.lo;
+                int rc = s.reserve(e, cn, (size_t)c.arena_hi - c.arena_lo, c.out_bound);
+                if (!rc) rc = steps.upload(s, c, s.stream);
+                if (!rc) rc = steps.compute(s, c, s.stream, nullptr);
+                if (rc) return rc;
+                CUDA_TRY(cudaMemcpyAsync(out->out_off + c.lo, s.d_off, (size_t)cn * 4, cudaMemcpyDeviceToHost, s.stream));
+                CUDA_TRY(cudaMemcpyAsync(out->meta + c.lo, s.d_meta, (size_t)cn * 4, cudaMemcpyDeviceToHost, s.stream));
+                CUDA_TRY(cudaMemcpyAsync(&s.h_tail[0], s.d_off + cn, 4, cudaMemcpyDeviceToHost, s.stream));
+                CUDA_TRY(cudaMemcpyAsync(&s.h_tail[1], s.d_flag, 4, cudaMemcpyDeviceToHost, s.stream));
+                CUDA_TRY(cudaEventRecord(s.done, s.stream));
+                issued++;
+            }
+            // retire the oldest chunk: learn its size, then pull exactly that many bytes
+            Slot& s = e->slots[finished % kSlots];
+            const ChunkPlan& c = inflight[finished % kSlots];
+            CUDA_TRY(cudaEventSynchronize(s.done));
+            bool wrote = false;
+            { int rc = o.retire(s, s.d_out, s.h_tail[0], s.h_tail[1], true, s.stream, &wrote); if (rc) return rc; }
+            if (wrote) o.rebase(c.lo, c.hi - c.lo);  // while the copy runs
+            CUDA_TRY(cudaStreamSynchronize(s.stream));
+            finished++;
         }
-        // retire the oldest chunk: learn its size, then pull exactly that many bytes
-        int si = (int)(finished % kSlots);
-        Slot& s = e->slots[si];
-        const ChunkPlan& c = inflight[si];
-        CUDA_TRY(cudaEventSynchronize(s.done));
-        uint32_t total = s.h_tail[0];
-        if (s.h_tail[1]) { CUDA_TRY(cudaMemsetAsync(s.d_flag, 0, 4, s.stream)); final_rc = GOFR_ERR_CAPACITY; set_last_error("device output buffer too small for chunk %zu", finished); total = 0; }
-        if (write_pos + total > out->out_cap) { final_rc = GOFR_ERR_CAPACITY; set_last_error("output capacity %llu too small", (unsigned long long)out->out_cap); total = 0; }
-        if (total) CUDA_TRY(cudaMemcpyAsync(out->out + write_pos, s.d_out, total, cudaMemcpyDeviceToHost, s.stream));
-        // rebase this chunk's offsets while the copy runs
-        if (write_pos) for (uint32_t i = c.lo; i < c.hi; i++) out->out_off[i] += (uint32_t)write_pos;
-        CUDA_TRY(cudaStreamSynchronize(s.stream));
-        write_pos += total;
-        finished++;
     }
-    out->out_off[n] = (uint32_t)write_pos;
-    out->out_bytes = write_pos;
-    *ticket = e->next_ticket++;
-    e->done_tickets.emplace_back(*ticket, final_rc);
+    { int rc = PackedOut::finish(e, n, {&o}); if (rc) return rc; }
+    if (o.overflow) set_last_error("output capacity too small (device chunk buffer or caller buffer)");
+    out->out_off[n] = (uint32_t)o.written;
+    out->out_bytes = o.written;
+    complete(e, ticket, o.overflow ? GOFR_ERR_CAPACITY : GOFR_OK);
     return GOFR_OK;
 }
 
@@ -1042,20 +1090,14 @@ static int batch_submit_locked(gofr_engine* e, const gofr_req_batch* in, gofr_re
     return run_chunks(e, in->n, steps, out, ticket);
 }
 
-int gofr_batch_submit_slots(gofr_engine* e, const gofr_req_batch* in, gofr_slot_batch* out, gofr_ticket* ticket) {
+int gofr_batch_submit(gofr_engine* e, const gofr_req_batch* in, gofr_resp_batch* out, gofr_ticket* ticket) {
     if (!e || !in || !out || !ticket) return GOFR_ERR_INVALID;
-    if (in->n && (!in->desc || !in->trace_ids || !out->out || !out->out_len || !out->meta)) return GOFR_ERR_INVALID;
-    if (out->slot_bytes == 0 || (out->slot_bytes & 15u)) { set_last_error("slot_bytes must be a positive multiple of 16"); return GOFR_ERR_INVALID; }
-    std::lock_guard<std::mutex> g(e->mu);
-    CUDA_TRY(cudaSetDevice(e->device));
-    const int rc = batch_submit_slots_locked(e, in, out, ticket);
-    if (rc != GOFR_OK) drain_streams(e);  // see gofr_batch_submit
-    return rc;
+    if (in->n && (!in->desc || !in->trace_ids || !out->out || !out->out_off || !out->meta)) return GOFR_ERR_INVALID;
+    return host_batch(e, [&] { return batch_submit_locked(e, in, out, ticket); });
 }
 
 static int batch_submit_slots_locked(gofr_engine* e, const gofr_req_batch* in, gofr_slot_batch* out, gofr_ticket* ticket) {
     const uint32_t n = in->n, slot = out->slot_bytes;
-    int final_rc = GOFR_OK;
     const size_t nchunks = n ? (n + e->chunk - 1) / e->chunk : 0;
     for (size_t ci = 0; ci < nchunks; ci++) {
         Slot& s = e->slots[ci % kSlots];
@@ -1084,9 +1126,15 @@ static int batch_submit_slots_locked(gofr_engine* e, const gofr_req_batch* in, g
         CUDA_TRY(wait_batch(e, n));
         for (auto& s : e->slots) s.egress_pending = false;
     }
-    *ticket = e->next_ticket++;
-    e->done_tickets.emplace_back(*ticket, final_rc);
+    complete(e, ticket, GOFR_OK);
     return GOFR_OK;
+}
+
+int gofr_batch_submit_slots(gofr_engine* e, const gofr_req_batch* in, gofr_slot_batch* out, gofr_ticket* ticket) {
+    if (!e || !in || !out || !ticket) return GOFR_ERR_INVALID;
+    if (in->n && (!in->desc || !in->trace_ids || !out->out || !out->out_len || !out->meta)) return GOFR_ERR_INVALID;
+    if (out->slot_bytes == 0 || (out->slot_bytes & 15u)) { set_last_error("slot_bytes must be a positive multiple of 16"); return GOFR_ERR_INVALID; }
+    return host_batch(e, [&] { return batch_submit_slots_locked(e, in, out, ticket); });
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -1099,65 +1147,21 @@ static constexpr uint32_t kConnChunkBudget = 8u << 20;
 // The buffers of a chunk of `conns` connections, `records` records at most and `buf_bytes` staged buffer bytes (plus the
 // 16 readable bytes the framer and the request-head kernel need, and 16 more for the bulk copies' rounding).
 int Slot::reserve_conn(uint32_t conns, uint32_t records, size_t buf_bytes) {
-    if (conns > cap_conns) {
-        cudaFree(d_buf_off); cudaFree(d_first); cudaFree(d_cstatus); cudaFree(d_consumed); cudaFree(d_req_first);
-        d_buf_off = d_first = d_cstatus = d_consumed = d_req_first = nullptr;
-        cap_conns = 0;
-        const size_t c = (size_t)conns + conns / 4 + 256;
-        if (cudaMalloc(&d_buf_off, (c + 1) * 4) != cudaSuccess || cudaMalloc(&d_first, (c + 1) * 4) != cudaSuccess ||
-            cudaMalloc(&d_cstatus, c * 4) != cudaSuccess || cudaMalloc(&d_consumed, c * 4) != cudaSuccess ||
-            cudaMalloc(&d_req_first, (c + 1) * 4) != cudaSuccess) {
-            set_last_error("cudaMalloc failed for a %zu-connection chunk", c);
-            return GOFR_ERR_NOMEM;
-        }
-        cap_conns = c;
-    }
-    if (records > cap_recs) {
-        cudaFree(d_rec); cudaFree(d_pdesc); cudaFree(d_pstatus); cudaFree(d_spans); cudaFree(d_req_at);
-        d_rec = d_pstatus = d_req_at = nullptr; d_pdesc = nullptr; d_spans = nullptr;
-        cap_recs = 0;
-        const size_t c = (size_t)records + records / 4 + 256;
-        if (cudaMalloc(&d_rec, (c + 1) * 4) != cudaSuccess || cudaMalloc(&d_pdesc, c * 16) != cudaSuccess ||
-            cudaMalloc(&d_pstatus, c * 4) != cudaSuccess || cudaMalloc(&d_spans, c * GOFR_HTTP_SPANS * 8) != cudaSuccess ||
-            cudaMalloc(&d_req_at, c * 4) != cudaSuccess) {
-            set_last_error("cudaMalloc failed for a %zu-record chunk", c);
-            return GOFR_ERR_NOMEM;
-        }
-        cap_recs = c;
-    }
-    return grow((void**)&d_buf, &cap_buf, buf_bytes + 32, 256);
+    int rc = grow_cols(&cap_conns, conns, "connections", {{&d_buf_off, 4, 4}, {&d_first, 4, 4}, {&d_cstatus, 4, 0},
+                                                          {&d_consumed, 4, 0}, {&d_req_first, 4, 4}});
+    if (!rc) rc = grow_cols(&cap_recs, records, "records", {{&d_rec, 4, 4}, {&d_pdesc, 16, 0}, {&d_pstatus, 4, 0},
+                                                            {&d_spans, GOFR_HTTP_SPANS * 8, 0}, {&d_req_at, 4, 0}});
+    return rc ? rc : grow((void**)&d_buf, &cap_buf, buf_bytes + 32, 256);
 }
 
 // The request-log buffers of a chunk of `conns` connections with `records` records at most and `remote_bytes` of remote
 // strings: the inputs and every per-line column (a chunk has no more lines than records).  The byte buffers whose size is
 // only known once the chunk is served grow in conn_log_chunk.
 int Slot::reserve_log(uint32_t conns, uint32_t records, size_t remote_bytes) {
-    if (conns > cap_lconns) {
-        cudaFree(d_remote_off); cudaFree(d_start); cudaFree(d_lfirst);
-        d_remote_off = d_lfirst = nullptr; d_start = nullptr;
-        cap_lconns = 0;
-        const size_t c = (size_t)conns + conns / 4 + 256;
-        if (cudaMalloc(&d_remote_off, (c + 1) * 4) != cudaSuccess || cudaMalloc(&d_start, c * 8) != cudaSuccess ||
-            cudaMalloc(&d_lfirst, (c + 1) * 4) != cudaSuccess) {
-            set_last_error("cudaMalloc failed for a %zu-connection chunk's log", c);
-            return GOFR_ERR_NOMEM;
-        }
-        cap_lconns = c;
-    }
-    if (records > cap_lrecs) {
-        cudaFree(d_ldesc); cudaFree(d_lids); cudaFree(d_lreq); cudaFree(d_lraw_off); cudaFree(d_loff);
-        d_ldesc = nullptr; d_lids = nullptr; d_lreq = d_lraw_off = d_loff = nullptr;
-        cap_lrecs = 0;
-        const size_t c = (size_t)records + records / 4 + 256;
-        if (cudaMalloc(&d_ldesc, c * sizeof(gofr_log_desc)) != cudaSuccess || cudaMalloc(&d_lids, c * 16) != cudaSuccess ||
-            cudaMalloc(&d_lreq, c * 4) != cudaSuccess || cudaMalloc(&d_lraw_off, (c + 1) * 4) != cudaSuccess ||
-            cudaMalloc(&d_loff, (c + 1) * 4) != cudaSuccess) {
-            set_last_error("cudaMalloc failed for a %zu-line chunk's log", c);
-            return GOFR_ERR_NOMEM;
-        }
-        cap_lrecs = c;
-    }
-    return grow((void**)&d_remote, &cap_remote, remote_bytes + 16, 256);
+    int rc = grow_cols(&cap_lconns, conns, "logged connections", {{&d_remote_off, 4, 4}, {&d_start, 8, 0}, {&d_lfirst, 4, 4}});
+    if (!rc) rc = grow_cols(&cap_lrecs, records, "log lines", {{&d_ldesc, sizeof(gofr_log_desc), 0}, {&d_lids, 16, 0},
+                                                               {&d_lreq, 4, 0}, {&d_lraw_off, 4, 4}, {&d_loff, 4, 4}});
+    return rc ? rc : grow((void**)&d_remote, &cap_remote, remote_bytes + 16, 256);
 }
 
 // A chunk: connections [lo, hi), staged from buffer byte alo (buf_off[lo] rounded down to 16, so that the absolute offsets
@@ -1236,30 +1240,21 @@ static int conn_frame(gofr_engine* e, const gofr_conn_batch* in, gofr_conn_resp*
 
 // The state of a connection batch between its chunks
 struct ConnRun {
-    bool pinned;
     bool req_short = false;     // req_cap was too small for a chunk: no per-request column is written from there on
-    bool bytes_short = false;   // out_cap was too small (pageable path; the pinned path learns it from the egress kernel)
     uint64_t req_base = 0;      // requests of the chunks before
-    uint64_t write_pos = 0;     // pageable path: response bytes written so far
     // the request-log lines (gofr_conn_batch_submit_log), the same per line
-    gofr_conn_log* log = nullptr;
-    bool log_pinned = false;
     bool lines_short = false;
-    bool log_bytes_short = false;
     uint64_t line_base = 0;
-    uint64_t log_pos = 0;
 };
 
 // The request-log lines of chunk ci, after its serve kernel: the gather (conn_log_kernel.cu), then the existing reqlog_kernel
-// and chunk_pack_kernel, then the caller's columns as for the responses (advance and egress on the log's own chain word
-// when they are pinned, an exact-size copy when they are pageable).  The reqlog and pack kernels take the chunk's line count
-// from the host: it is read back after the gather.  The log kernels report overflow in their own flag word, so that the
-// responses' advance never sees it.
-static int conn_log_chunk(gofr_engine* e, const gofr_conn_batch* in, Slot& s, size_t ci, const ConnChunk& c, ConnRun& r,
-                          uint32_t n_req) {
-    gofr_conn_log* log = r.log;
+// and chunk_pack_kernel, then the caller's columns through the lines' PackedOut (output 1).  The reqlog and pack kernels
+// take the chunk's line count from the host: it is read back after the gather.  The log kernels report overflow in their
+// own flag word, so that the responses' advance never sees it.
+static int conn_log_chunk(gofr_engine* e, const gofr_conn_batch* in, const gofr_conn_log* log, Slot& s, size_t ci,
+                          const ConnChunk& c, ConnRun& r, PackedOut& lo, uint32_t n_req) {
     cudaStream_t st = e->st_compute;
-    uint32_t* ends = e->h_ends + 4 * ci + 2;  // the chunk's first and end line offsets: what it needs of out_cap
+    uint32_t* ends = lo.ends(e, ci);  // the chunk's first and end line offsets: what it needs of out_cap
     ends[0] = ends[1] = 0;
     if (!n_req) return GOFR_OK;
     const uint32_t cn = c.hi - c.lo, bytes = in->buf_off[c.hi] - c.alo;
@@ -1295,44 +1290,29 @@ static int conn_log_chunk(gofr_engine* e, const gofr_conn_batch* in, Slot& s, si
     if (rc) return rc;
     PackParams q;
     memset(&q, 0, sizeof q);
-    q.a = s.d_lraw; q.a_off = s.d_lraw_off; q.a_cap = s.cap_lraw - 16; q.chain_pos = r.log_pinned ? e->d_chain + 1 : nullptr;
+    q.a = s.d_lraw; q.a_off = s.d_lraw_off; q.a_cap = s.cap_lraw - 16; q.chain_pos = lo.chain(e);
     rc = launch_frames_locked(e, K_PACK, 0, q, lines, s.d_lout, s.cap_lout, s.d_loff, s.state, flag, st);
     if (rc) return rc;
     CUDA_TRY(cudaMemcpyAsync(&ends[0], s.d_loff, 4, cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaMemcpyAsync(&ends[1], s.d_loff + lines, 4, cudaMemcpyDeviceToHost, st));
     if (r.line_base + lines > log->line_cap) r.lines_short = true;
     const bool put = !r.lines_short;
-    const size_t si = kSlots + ci % kSlots;
-    if (r.log_pinned) {
-        if (put && launch_advance(e->d_chain + 1, s.d_loff, lines, flag, e->d_info + si, log->out_cap, st) != 0) {
-            set_last_error("advance kernel launch failed"); return GOFR_ERR_CUDA;
-        }
-        if (!put) CUDA_TRY(cudaMemsetAsync(flag, 0, 4, st));
-        CUDA_TRY(cudaEventRecord(s.ev_served, st));
-        CUDA_TRY(cudaStreamWaitEvent(e->st_egress, s.ev_served, 0));
-        if (put) {
-            if (launch_egress(e->d_info + si, s.d_lout, s.d_loff, s.d_lreq, lines, log->out, log->log_off + r.line_base,
-                              log->log_req + r.line_base, e->h_status + 2, e->egress_grid, e->st_egress) != 0) {
-                set_last_error("egress kernel launch failed"); return GOFR_ERR_CUDA;
-            }
-            e->launches += 2;
-        }
+    if (lo.pinned) {
+        rc = lo.deliver(e, s, ci, s.d_lout, s.d_loff, s.d_lreq, lines, r.line_base, put);
+        if (rc) return rc;
         CUDA_TRY(cudaEventRecord(s.ev_egress, e->st_egress));
         s.egress_pending = true;
     } else {  // pageable: the chunk's exact size first, then exactly that many bytes
         CUDA_TRY(cudaMemcpyAsync(&s.h_tail[3], flag, 4, cudaMemcpyDeviceToHost, st));
         CUDA_TRY(cudaStreamSynchronize(st));
-        if (s.h_tail[3]) { CUDA_TRY(cudaMemsetAsync(flag, 0, 4, st)); r.log_bytes_short = true; }
-        const uint32_t total = ends[1];
-        // log_off is 32-bit: lines past 4 GiB are a capacity error, as advance_kernel makes them on the pinned path
-        if (put && (r.log_pos + total > log->out_cap || r.log_pos + total > 0xFFFFFFFFull)) r.log_bytes_short = true;
-        if (put && !r.log_bytes_short) {
-            if (total) CUDA_TRY(cudaMemcpyAsync(log->out + r.log_pos, s.d_lout, total, cudaMemcpyDeviceToHost, st));
+        bool wrote = false;
+        rc = lo.retire(s, s.d_lout, ends[1], s.h_tail[3], put, st, &wrote);
+        if (rc) return rc;
+        if (wrote) {
             CUDA_TRY(cudaMemcpyAsync(log->log_off + r.line_base, s.d_loff, (size_t)lines * 4, cudaMemcpyDeviceToHost, st));
             CUDA_TRY(cudaMemcpyAsync(log->log_req + r.line_base, s.d_lreq, (size_t)lines * 4, cudaMemcpyDeviceToHost, st));
             CUDA_TRY(cudaStreamSynchronize(st));
-            if (r.log_pos) for (uint64_t m = r.line_base; m < r.line_base + lines; m++) log->log_off[m] += (uint32_t)r.log_pos;
-            r.log_pos += total;
+            lo.rebase(r.line_base, lines);
         }
     }
     r.line_base += lines;
@@ -1341,8 +1321,8 @@ static int conn_log_chunk(gofr_engine* e, const gofr_conn_batch* in, Slot& s, si
 
 // Second half of chunk ci: parse its records, compact the whole requests, serve them, and send the results to the caller's
 // columns.  The record count and the connection states are on the host by now: they size the launches.
-static int conn_serve(gofr_engine* e, const gofr_conn_batch* in, gofr_conn_resp* out, Slot& s, size_t ci, const ConnChunk& c,
-                      ConnRun& r) {
+static int conn_serve(gofr_engine* e, const gofr_conn_batch* in, gofr_conn_resp* out, const gofr_conn_log* log, Slot& s,
+                      size_t ci, const ConnChunk& c, ConnRun& r, PackedOut& ro, PackedOut& lo) {
     CUDA_TRY(cudaEventSynchronize(s.done));
     const uint32_t cn = c.hi - c.lo, n_rec = s.h_tail[0];
     uint32_t n_req = n_rec;
@@ -1366,55 +1346,46 @@ static int conn_serve(gofr_engine* e, const gofr_conn_batch* in, gofr_conn_resp*
     if (rc) return rc;
     if (r.req_base + n_req > out->req_cap) r.req_short = true;
     const bool put = !r.req_short && n_req;  // this chunk's per-request columns go to the caller
-    uint32_t* ends = e->h_ends + 4 * ci;     // the chunk's first and end response offsets: what it needs of out_cap
+    uint32_t* ends = ro.ends(e, ci);         // the chunk's first and end response offsets: what it needs of out_cap
     ends[0] = ends[1] = 0;
     if (n_req) {
         rc = launch_serve(e, s.d_desc, s.d_ids, s.d_arena - c.alo, n_req, in->date, s.d_out, s.cap_out, s.d_off, s.d_meta, &s.state,
-                          s.d_flag, s.d_bind, st, r.pinned ? e->d_chain : nullptr);
+                          s.d_flag, s.d_bind, st, ro.chain(e));
         if (rc) return rc;
         CUDA_TRY(cudaMemcpyAsync(&ends[0], s.d_off, 4, cudaMemcpyDeviceToHost, st));
         CUDA_TRY(cudaMemcpyAsync(&ends[1], s.d_off + n_req, 4, cudaMemcpyDeviceToHost, st));
     }
-    const size_t si = ci % kSlots;
-    if (r.pinned) {
-        if (put && launch_advance(e->d_chain, s.d_off, n_req, s.d_flag, e->d_info + si, out->out_cap, st) != 0) {
-            set_last_error("advance kernel launch failed"); return GOFR_ERR_CUDA;
-        }
-        CUDA_TRY(cudaEventRecord(s.ev_served, st));
-        CUDA_TRY(cudaStreamWaitEvent(e->st_egress, s.ev_served, 0));
-        cudaStream_t eg = e->st_egress;
-        if (put) {
-            if (launch_egress(e->d_info + si, s.d_out, s.d_off, s.d_meta, n_req, out->out, out->out_off + r.req_base,
-                              out->meta + r.req_base, e->h_status, e->egress_grid, eg) != 0) {
-                set_last_error("egress kernel launch failed"); return GOFR_ERR_CUDA;
-            }
-            e->launches += 2;
-            CUDA_TRY(cudaMemcpyAsync(out->req_at + r.req_base, s.d_req_at, (size_t)n_req * 4, cudaMemcpyDeviceToHost, eg));
-            if (out->trace_ids) CUDA_TRY(cudaMemcpyAsync(out->trace_ids + r.req_base * 16, s.d_ids, (size_t)n_req * 16, cudaMemcpyDeviceToHost, eg));
-        }
-        CUDA_TRY(cudaMemcpyAsync(out->req_first + c.lo, s.d_req_first, (size_t)cn * 4, cudaMemcpyDeviceToHost, eg));
-        CUDA_TRY(cudaEventRecord(s.ev_egress, eg));
-        s.egress_pending = true;
+    // the per-request columns go next to the responses: behind the egress when pinned, behind their bytes when pageable
+    bool wrote = put;
+    cudaStream_t cs = e->st_egress;
+    if (ro.pinned) {
+        rc = ro.deliver(e, s, ci, s.d_out, s.d_off, s.d_meta, n_req, r.req_base, put);
+        if (rc) return rc;
     } else {  // pageable: the chunk's exact size first, then exactly that many bytes
+        cs = st;
+        CUDA_TRY(cudaMemcpyAsync(&s.h_tail[1], s.d_flag, 4, cudaMemcpyDeviceToHost, st));
         CUDA_TRY(cudaStreamSynchronize(st));
-        const uint32_t total = ends[1];
-        if (put && r.write_pos + total > out->out_cap) r.bytes_short = true;
-        if (put && !r.bytes_short) {
-            if (total) CUDA_TRY(cudaMemcpyAsync(out->out + r.write_pos, s.d_out, total, cudaMemcpyDeviceToHost, st));
+        rc = ro.retire(s, s.d_out, ends[1], s.h_tail[1], put, st, &wrote);
+        if (rc) return rc;
+        if (wrote) {
             CUDA_TRY(cudaMemcpyAsync(out->out_off + r.req_base, s.d_off, (size_t)n_req * 4, cudaMemcpyDeviceToHost, st));
             CUDA_TRY(cudaMemcpyAsync(out->meta + r.req_base, s.d_meta, (size_t)n_req * 4, cudaMemcpyDeviceToHost, st));
-            CUDA_TRY(cudaMemcpyAsync(out->req_at + r.req_base, s.d_req_at, (size_t)n_req * 4, cudaMemcpyDeviceToHost, st));
-            if (out->trace_ids) CUDA_TRY(cudaMemcpyAsync(out->trace_ids + r.req_base * 16, s.d_ids, (size_t)n_req * 16, cudaMemcpyDeviceToHost, st));
-        }
-        CUDA_TRY(cudaMemcpyAsync(out->req_first + c.lo, s.d_req_first, (size_t)cn * 4, cudaMemcpyDeviceToHost, st));
-        CUDA_TRY(cudaStreamSynchronize(st));
-        if (put && !r.bytes_short) {
-            if (r.write_pos) for (uint64_t k = r.req_base; k < r.req_base + n_req; k++) out->out_off[k] += (uint32_t)r.write_pos;
-            r.write_pos += total;
         }
     }
-    if (r.log) {
-        const int rc = conn_log_chunk(e, in, s, ci, c, r, n_req);
+    if (wrote) {
+        CUDA_TRY(cudaMemcpyAsync(out->req_at + r.req_base, s.d_req_at, (size_t)n_req * 4, cudaMemcpyDeviceToHost, cs));
+        if (out->trace_ids) CUDA_TRY(cudaMemcpyAsync(out->trace_ids + r.req_base * 16, s.d_ids, (size_t)n_req * 16, cudaMemcpyDeviceToHost, cs));
+    }
+    CUDA_TRY(cudaMemcpyAsync(out->req_first + c.lo, s.d_req_first, (size_t)cn * 4, cudaMemcpyDeviceToHost, cs));
+    if (ro.pinned) {
+        CUDA_TRY(cudaEventRecord(s.ev_egress, cs));
+        s.egress_pending = true;
+    } else {
+        CUDA_TRY(cudaStreamSynchronize(st));
+        if (wrote) ro.rebase(r.req_base, n_req);
+    }
+    if (log) {
+        const int rc = conn_log_chunk(e, in, log, s, ci, c, r, lo, n_req);
         if (rc) return rc;
     }
     r.req_base += n_req;
@@ -1428,8 +1399,7 @@ static int conn_batch_locked(gofr_engine* e, const gofr_conn_batch* in, gofr_con
     out->out_bytes = 0;
     if (log) { log->lines = 0; log->out_bytes = 0; }
     if (n == 0) {  // touches no buffer
-        *ticket = e->next_ticket++;
-        e->done_tickets.emplace_back(*ticket, GOFR_OK);
+        complete(e, ticket, GOFR_OK);
         return GOFR_OK;
     }
     // chunks end at e->chunk connections or at the byte budget, where two neighbours together pass it
@@ -1442,70 +1412,53 @@ static int conn_batch_locked(gofr_engine* e, const gofr_conn_batch* in, gofr_con
         e->ends_cap = 4 * max_chunks;
     }
     ConnRun r;
-    r.pinned = device_visible(out->out) && device_visible(out->out_off) && device_visible(out->meta);
-    if (r.pinned) {
-        CUDA_TRY(cudaMemsetAsync(e->d_chain, 0, 8, e->st_compute));
-        e->h_status[0] = 0; e->h_status[1] = 0;
-    }
-    r.log = log;
-    r.log_pinned = log && device_visible(log->out) && device_visible(log->log_off) && device_visible(log->log_req);
-    if (r.log_pinned) {
-        CUDA_TRY(cudaMemsetAsync(e->d_chain + 1, 0, 8, e->st_compute));
-        e->h_status[2] = 0; e->h_status[3] = 0;
+    PackedOut ro(out->out, out->out_cap, out->out_off, out->meta, 0), lo;
+    { int rc = ro.start(e); if (rc) return rc; }
+    if (log) {
+        lo = PackedOut(log->out, log->out_cap, log->log_off, log->log_req, 1);
+        int rc = lo.start(e);
+        if (rc) return rc;
     }
     ConnChunk chunks[kSlots];
     size_t issued = 0, served = 0;
-    for (uint32_t lo = 0; lo < n || served < issued;) {
-        while (lo < n && issued < served + 2) {
+    for (uint32_t next = 0; next < n || served < issued;) {
+        while (next < n && issued < served + 2) {
             ConnChunk& c = chunks[issued % kSlots];
-            int rc = conn_plan(e, in, log, lo, &c);
+            int rc = conn_plan(e, in, log, next, &c);
             if (!rc) rc = conn_frame(e, in, out, log, e->slots[issued % kSlots], c);
             if (rc) return rc;
-            lo = c.hi;
+            next = c.hi;
             issued++;
         }
-        int rc = conn_serve(e, in, out, e->slots[served % kSlots], served, chunks[served % kSlots], r);
+        int rc = conn_serve(e, in, out, log, e->slots[served % kSlots], served, chunks[served % kSlots], r, ro, lo);
         if (rc) return rc;
         served++;
     }
-    uint64_t need = 0, written = r.write_pos;
-    bool short_ = r.req_short || r.bytes_short;
-    if (r.pinned || r.log_pinned) {
-        if (r.pinned) CUDA_TRY(cudaMemcpyAsync((void*)&e->h_status[0], e->d_chain, 8, cudaMemcpyDeviceToHost, e->st_egress));
-        if (r.log_pinned) CUDA_TRY(cudaMemcpyAsync((void*)&e->h_status[2], e->d_chain + 1, 8, cudaMemcpyDeviceToHost, e->st_egress));
-        CUDA_TRY(wait_batch(e, n));
-        for (auto& s : e->slots) s.egress_pending = false;
-    }
-    if (r.pinned) {
-        written = e->h_status[0];
-        short_ |= e->h_status[1] != 0;
-    }
-    for (size_t ci = 0; ci < served; ci++) need += e->h_ends[4 * ci + 1] - e->h_ends[4 * ci];
+    { int rc = PackedOut::finish(e, n, {&ro, &lo}); if (rc) return rc; }
+    const uint64_t need = ro.needed(e, served);
     out->req_first[n] = (uint32_t)r.req_base;
     out->out_bytes = need;
     int final_rc = GOFR_OK;
-    if (short_) {
+    if (r.req_short || ro.overflow) {
         final_rc = GOFR_ERR_CAPACITY;
         set_last_error("the batch needs %llu requests and %llu response bytes: req_cap %u, out_cap %llu", (unsigned long long)r.req_base,
                        (unsigned long long)need, out->req_cap, (unsigned long long)out->out_cap);
     } else {
-        out->out_off[r.req_base] = (uint32_t)written;
+        out->out_off[r.req_base] = (uint32_t)ro.written;
     }
     if (log) {
-        uint64_t lneed = 0;
-        for (size_t ci = 0; ci < served; ci++) lneed += e->h_ends[4 * ci + 3] - e->h_ends[4 * ci + 2];
+        const uint64_t lneed = lo.needed(e, served);
         log->lines = (uint32_t)r.line_base;
         log->out_bytes = lneed;
-        if (r.lines_short || r.log_bytes_short || (r.log_pinned && e->h_status[3] != 0)) {
+        if (r.lines_short || lo.overflow) {
             final_rc = GOFR_ERR_CAPACITY;
             set_last_error("the batch needs %llu log lines and %llu log bytes: line_cap %u, out_cap %llu", (unsigned long long)r.line_base,
                            (unsigned long long)lneed, log->line_cap, (unsigned long long)log->out_cap);
         } else {
-            log->log_off[r.line_base] = (uint32_t)(r.log_pinned ? e->h_status[2] : r.log_pos);
+            log->log_off[r.line_base] = (uint32_t)lo.written;
         }
     }
-    *ticket = e->next_ticket++;
-    e->done_tickets.emplace_back(*ticket, final_rc);
+    complete(e, ticket, final_rc);
     return GOFR_OK;
 }
 
@@ -1518,11 +1471,7 @@ int gofr_conn_batch_submit_log(gofr_engine* e, const gofr_conn_batch* in, gofr_c
     if (in->n_conns && (!in->buf || !in->buf_off || !out->out || !out->out_off || !out->meta || !out->req_at || !out->req_first ||
                         !out->consumed || !out->conn_status)) return GOFR_ERR_INVALID;
     if (log && in->n_conns && (!log->remote_off || !log->start_unix_ns || !log->out || !log->log_off || !log->log_req)) return GOFR_ERR_INVALID;
-    std::lock_guard<std::mutex> g(e->mu);
-    CUDA_TRY(cudaSetDevice(e->device));
-    const int rc = conn_batch_locked(e, in, out, log, ticket);
-    if (rc != GOFR_OK) drain_streams(e);  // see gofr_batch_submit
-    return rc;
+    return host_batch(e, [&] { return conn_batch_locked(e, in, out, log, ticket); });
 }
 
 int gofr_conn_batch_bound(const gofr_table* t, const uint32_t* buf_off, uint32_t n_conns, uint32_t* req_cap, uint64_t* out_cap) {
@@ -2014,11 +1963,7 @@ static int proto_batch(gofr_engine* e, const gofr_proto_nmsg* msgs, uint32_t n_m
     if (in->data_bytes && !in->data) return GOFR_ERR_INVALID;
     PbnDesc D;
     { int rc = pbn_build(msgs, n_msgs, fields, n_fields, root, presence, &D); if (rc) return rc; }
-    std::lock_guard<std::mutex> g(e->mu);
-    CUDA_TRY(cudaSetDevice(e->device));
-    const int rc = proto_batch_locked(e, D, decode, in, out, ticket);
-    if (rc != GOFR_OK) drain_streams(e);  // see gofr_batch_submit
-    return rc;
+    return host_batch(e, [&] { return proto_batch_locked(e, D, decode, in, out, ticket); });
 }
 
 int gofr_proto_batch_decode(gofr_engine* e, const gofr_proto_nmsg* msgs, uint32_t n_msgs, const gofr_proto_nfield* fields, uint32_t n_fields,
