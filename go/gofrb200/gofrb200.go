@@ -313,6 +313,91 @@ func (t *Table) ConnBound(bufOff []uint32) (reqCap uint32, outCap uint64, err er
 // to connection c, splicing in the host's responses for GOFR_H_HOST requests (status 0 in Meta); then keep its bytes from
 // Consumed[c] on (HTTPConnMore) or hand them to net/http (HTTPConnDefer).  traceSeed must be fresh per batch.
 func (e *Engine) ServeConnections(buf []byte, bufOff []uint32, now time.Time, traceSeed uint64, r *ConnResponses) (uint64, error) {
+	return e.respondConnections(buf, bufOff, now, traceSeed, nil, r)
+}
+
+// ConnRoute receives what RouteConnections returns; the caller owns the slices and sizes them with ConnBound (reqCap) and
+// len(buf) + 64 (Arena).  Request k: Meta[k] = status | route id << 16 (status 0: the closure of that route runs), its path
+// variables Vars[8k:8k+8] (offset | length << 16 inside its path, 0xFFFFFFFF unused), ReqAt[k], TraceIDs[16k:16k+16] and
+// its parsed request Desc[k], whose bytes are Arena[Desc[k].arena_off:] (decoded path | query | pad4 | body).
+type ConnRoute struct {
+	Desc                           []C.gofr_req_desc // req_cap
+	Arena                          []byte            // len(buf) + 64
+	Meta, ReqAt                    []uint32          // req_cap
+	Vars                           []uint32          // req_cap * 8
+	TraceIDs                       []byte            // req_cap * 16
+	ReqFirst, Consumed, ConnStatus []uint32          // n + 1, n, n
+}
+
+// RouteConnections is stage 1 of serving connection buffers with handler closures (gofr_conn_batch_route, synchronous):
+// frame, parse and route on the device.  Run the closures of the requests whose status is 0, encode each (data, err) as a
+// GOFR_H_RESULT record, and pass the records to RespondConnections with the same buf, bufOff and traceSeed.
+func (e *Engine) RouteConnections(buf []byte, bufOff []uint32, traceSeed uint64, r *ConnRoute) error {
+	n := len(bufOff) - 1
+	if n <= 0 {
+		return nil
+	}
+	k := len(r.Meta)
+	if len(buf) == 0 || k == 0 || len(r.Desc) < k || len(r.Arena) < len(buf)+64 || len(r.ReqAt) < k || len(r.Vars) < 8*k ||
+		len(r.TraceIDs) < 16*k || len(r.ReqFirst) < n+1 || len(r.Consumed) < n || len(r.ConnStatus) < n {
+		return errors.New("gofrb200: ConnRoute columns too small")
+	}
+	var in C.gofr_conn_batch
+	in.buf = (*C.uint8_t)(unsafe.Pointer(&buf[0]))
+	in.buf_off = (*C.uint32_t)(unsafe.Pointer(&bufOff[0]))
+	in.buf_bytes = C.uint64_t(len(buf))
+	in.n_conns = C.uint32_t(n)
+	in.trace_seed = C.uint64_t(traceSeed)
+	var o C.gofr_conn_route
+	o.req_cap = C.uint32_t(k)
+	o.desc = &r.Desc[0]
+	o.arena = (*C.uint8_t)(unsafe.Pointer(&r.Arena[0]))
+	o.meta = (*C.uint32_t)(unsafe.Pointer(&r.Meta[0]))
+	o.vars = (*C.uint32_t)(unsafe.Pointer(&r.Vars[0]))
+	o.req_at = (*C.uint32_t)(unsafe.Pointer(&r.ReqAt[0]))
+	o.trace_ids = (*C.uint8_t)(unsafe.Pointer(&r.TraceIDs[0]))
+	o.req_first = (*C.uint32_t)(unsafe.Pointer(&r.ReqFirst[0]))
+	o.consumed = (*C.uint32_t)(unsafe.Pointer(&r.Consumed[0]))
+	o.conn_status = (*C.uint32_t)(unsafe.Pointer(&r.ConnStatus[0]))
+	return check(C.gofr_conn_batch_route(e.e, &in, &o), "gofr_conn_batch_route")
+}
+
+// RespondConnections is stage 2 (gofr_conn_batch_respond + wait): ServeConnections with request k's data section replaced by
+// its closure's record rec[recOff[k]:recOff[k+1]] where that is not empty.  recOff has one entry per request of stage 1 plus
+// one.  Size r.Out with RespondBound.
+func (e *Engine) RespondConnections(buf []byte, bufOff []uint32, now time.Time, traceSeed uint64, rec []byte, recOff []uint32,
+	r *ConnResponses) (uint64, error) {
+	if len(recOff) == 0 {
+		return 0, errors.New("gofrb200: recOff needs one entry per request plus one")
+	}
+	res := &C.gofr_conn_results{}
+	if len(rec) > 0 {
+		res.rec = (*C.uint8_t)(unsafe.Pointer(&rec[0]))
+	}
+	res.rec_off = (*C.uint32_t)(unsafe.Pointer(&recOff[0]))
+	res.rec_bytes = C.uint64_t(len(rec))
+	res.n_req = C.uint32_t(len(recOff) - 1)
+	return e.respondConnections(buf, bufOff, now, traceSeed, res, r)
+}
+
+// RespondBound gives an output capacity that always suffices for RespondConnections on the requests stage 1 described
+// (gofr_conn_respond_bound; no GPU needed).
+func (t *Table) RespondBound(desc []C.gofr_req_desc, recOff []uint32) (uint64, error) {
+	if len(recOff) != len(desc)+1 {
+		return 0, errors.New("gofrb200: recOff needs len(desc) + 1 entries")
+	}
+	var oc C.uint64_t
+	var d *C.gofr_req_desc
+	if len(desc) > 0 {
+		d = &desc[0]
+	}
+	err := check(C.gofr_conn_respond_bound(t.t, d, C.uint32_t(len(desc)), (*C.uint32_t)(unsafe.Pointer(&recOff[0])), &oc),
+		"gofr_conn_respond_bound")
+	return uint64(oc), err
+}
+
+func (e *Engine) respondConnections(buf []byte, bufOff []uint32, now time.Time, traceSeed uint64, res *C.gofr_conn_results,
+	r *ConnResponses) (uint64, error) {
 	n := len(bufOff) - 1
 	if n <= 0 {
 		return 0, nil
@@ -367,7 +452,7 @@ func (e *Engine) ServeConnections(buf []byte, bufOff []uint32, now time.Time, tr
 		lg.log_req = (*C.uint32_t)(unsafe.Pointer(&l.LogReq[0]))
 	}
 	var ticket C.gofr_ticket
-	if err := check(C.gofr_conn_batch_submit_log(e.e, &in, &o, lg, &ticket), "gofr_conn_batch_submit_log"); err != nil {
+	if err := check(C.gofr_conn_batch_respond(e.e, &in, res, &o, lg, &ticket), "gofr_conn_batch_respond"); err != nil {
 		return 0, err
 	}
 	err := check(C.gofr_batch_wait(e.e, ticket), "gofr_batch_wait")

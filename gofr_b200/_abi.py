@@ -63,6 +63,17 @@ class ConnLog(C.Structure):
                 ("out_bytes", C.c_uint64)]
 
 
+class ConnRoute(C.Structure):
+    _fields_ = [("req_cap", C.c_uint32), ("reserved", C.c_uint32), ("desc", C.c_void_p), ("arena", C.c_void_p),
+                ("meta", C.c_void_p), ("vars", C.c_void_p), ("req_at", C.c_void_p), ("trace_ids", C.c_void_p),
+                ("req_first", C.c_void_p), ("consumed", C.c_void_p), ("conn_status", C.c_void_p)]
+
+
+class ConnResults(C.Structure):
+    _fields_ = [("rec", C.c_void_p), ("rec_off", C.c_void_p), ("rec_bytes", C.c_uint64), ("n_req", C.c_uint32),
+                ("reserved", C.c_uint32)]
+
+
 class ProtoBatch(C.Structure):
     _fields_ = [("data", C.c_void_p), ("data_bytes", C.c_uint64), ("off", C.c_void_p), ("n", C.c_uint32)]
 
@@ -150,6 +161,7 @@ def lib():
     L.gofr_proto_encode_device.argtypes = [vp, vp, u32, vp, vp, u32, vp, u64, vp, vp, vp]
     L.gofr_proto_decode_device.argtypes = [vp, vp, u32, vp, vp, u32, vp, u64, vp, vp, vp]
     L.gofr_batch_route.argtypes = [vp, C.POINTER(ReqBatch), vp, vp]
+    L.gofr_batch_bind.argtypes = [vp, u32, C.POINTER(ReqBatch), vp, u32, vp, vp]
     L.gofr_frontend_create.argtypes = [C.POINTER(vp), vp, u32, u32, u32, u32]
     L.gofr_frontend_destroy.argtypes = [vp]
     L.gofr_frontend_destroy.restype = None
@@ -168,6 +180,10 @@ def lib():
     L.gofr_conn_batch_bound.argtypes = [vp, vp, u32, C.POINTER(u32), C.POINTER(u64)]
     L.gofr_conn_batch_submit_log.argtypes = [vp, C.POINTER(ConnBatch), C.POINTER(ConnResp), C.POINTER(ConnLog), C.POINTER(u64)]
     L.gofr_conn_log_bound.argtypes = [vp, vp, u32, C.POINTER(u32), C.POINTER(u64)]
+    L.gofr_conn_batch_route.argtypes = [vp, C.POINTER(ConnBatch), C.POINTER(ConnRoute)]
+    L.gofr_conn_batch_respond.argtypes = [vp, C.POINTER(ConnBatch), C.POINTER(ConnResults), C.POINTER(ConnResp), C.POINTER(ConnLog),
+                                          C.POINTER(u64)]
+    L.gofr_conn_respond_bound.argtypes = [vp, vp, u32, vp, C.POINTER(u64)]
     L.gofr_requestlog_device.argtypes = [vp, vp, vp, vp, u32, vp, u64, vp, vp]
     L.gofr_engine_launch_count.argtypes = [vp]
     L.gofr_engine_launch_count.restype = u64
@@ -187,7 +203,7 @@ DECLARED_SYMBOLS = [
     "gofr_table_route_count", "gofr_table_max_response_bytes", "gofr_engine_create", "gofr_engine_destroy",
     "gofr_serve_device", "gofr_serve_device_slots", "gofr_batch_submit", "gofr_batch_wait", "gofr_batch_submit_slots", "gofr_engine_set_chunk", "gofr_engine_set_tile",
     "gofr_engine_set_timing", "gofr_engine_overflowed", "gofr_engine_geometry", "gofr_engine_slot_ctas", "gofr_table_slot_ctas", "gofr_alloc_pinned", "gofr_free_pinned", "gofr_bind_host_thread", "gofr_bind_device", "gofr_batch_bind",
-    "gofr_grpc_hello_device", "gofr_requestlog_device", "gofr_http_parse_device", "gofr_http_frame_device", "gofr_conn_batch_submit", "gofr_conn_batch_bound", "gofr_conn_batch_submit_log", "gofr_conn_log_bound", "gofr_batch_route", "gofr_proto_encode_device", "gofr_proto_decode_device", "gofr_proto_encode_nested_device", "gofr_proto_decode_nested_device", "gofr_proto_nested_describe", "gofr_proto_encode_nested_ex_device", "gofr_proto_decode_nested_ex_device", "gofr_proto_nested_describe_ex", "gofr_proto_decode_nested_deferred_device", "gofr_proto_batch_decode", "gofr_proto_batch_encode", "gofr_proto_nested_bound", "gofr_table_response_bound", "gofr_frontend_create", "gofr_frontend_destroy", "gofr_frontend_set_clock",
+    "gofr_grpc_hello_device", "gofr_requestlog_device", "gofr_http_parse_device", "gofr_http_frame_device", "gofr_conn_batch_submit", "gofr_conn_batch_bound", "gofr_conn_batch_submit_log", "gofr_conn_log_bound", "gofr_conn_batch_route", "gofr_conn_batch_respond", "gofr_conn_respond_bound", "gofr_batch_route", "gofr_proto_encode_device", "gofr_proto_decode_device", "gofr_proto_encode_nested_device", "gofr_proto_decode_nested_device", "gofr_proto_nested_describe", "gofr_proto_encode_nested_ex_device", "gofr_proto_decode_nested_ex_device", "gofr_proto_nested_describe_ex", "gofr_proto_decode_nested_deferred_device", "gofr_proto_batch_decode", "gofr_proto_batch_encode", "gofr_proto_nested_bound", "gofr_table_response_bound", "gofr_frontend_create", "gofr_frontend_destroy", "gofr_frontend_set_clock",
     "gofr_frontend_stats", "gofr_frontend_serve", "gofr_proto_frontend_create", "gofr_proto_frontend_destroy",
     "gofr_proto_frontend_stats", "gofr_proto_frontend_call", "gofr_route_device", "gofr_engine_launch_count", "gofr_engine_kernel_time_ms", "gofr_last_error",
     "gofr_abi_version", "gofr_format_http_date",

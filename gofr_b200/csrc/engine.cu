@@ -70,6 +70,7 @@ __global__ void http_parse_kernel(const HttpParams p);           // http_kernel.
 __global__ void http_frame_kernel(const HttpFrameParams p);      // http_frame_kernel.cu
 __global__ void conn_compact_kernel(const ConnParams p);         // conn_kernel.cu
 __global__ void conn_log_kernel(const ConnLogParams p);          // conn_log_kernel.cu
+__global__ void conn_result_kernel(const ConnResultParams p);    // conn_result_kernel.cu
 __global__ void route_kernel(const RouteParams p);               // route_kernel.cu
 __global__ void bind_kernel(const BindParams p);                 // bind_kernel.cu
 __global__ void chunk_pack_kernel(const PackParams p);           // pack_kernel.cu
@@ -80,7 +81,7 @@ namespace {
 enum Kern {
     K_SERVE, K_SERVE_VALUES, K_SLOTS, K_SLOTS_WIDE, K_SLOTS_VALUES, K_HELLO, K_PROTO_ENC, K_PROTO_DEC, K_PBN_ENC, K_PBN_DEC,
     K_PBN_ENC_MAPS, K_PBN_DEC_MAPS, K_PBN_ENC_PRES, K_PBN_DEC_PRES, K_PBN_DEC_DEFERRED, K_REQLOG, K_HTTP, K_HTTP_FRAME, K_ROUTE, K_BIND, K_PACK,
-    K_CONN, K_CONN_LOG,
+    K_CONN, K_CONN_LOG, K_CONN_RESULT,
     K_COUNT
 };
 struct KernelRec {
@@ -112,6 +113,7 @@ const KernelRec kKernels[K_COUNT] = {
     {(const void*)chunk_pack_kernel, "pack", kServeThreads},
     {(const void*)conn_compact_kernel, "connection compact", kServeThreads},
     {(const void*)conn_log_kernel, "connection log", kServeThreads},
+    {(const void*)conn_result_kernel, "connection result", kServeThreads},
 };
 
 constexpr int kSlots = 3;  // pipeline depth of the host-batch path
@@ -153,6 +155,11 @@ struct Slot {
     void* d_ldesc = nullptr; uint8_t* d_lids = nullptr; uint32_t* d_lreq = nullptr; uint32_t* d_lraw_off = nullptr; uint32_t* d_loff = nullptr;
     uint8_t* d_larena = nullptr; uint8_t* d_lraw = nullptr; uint8_t* d_lout = nullptr;
     size_t cap_remote = 0, cap_lconns = 0, cap_lrecs = 0, cap_larena = 0, cap_lraw = 0, cap_lout = 0;
+    // the closures' results (gofr_conn_batch_respond, grown on demand): the chunk's record bytes, their offsets and the
+    // spliced arena's offset column (per request), the spliced arena; gofr_conn_batch_route: the path variables
+    uint8_t* d_rbytes = nullptr; uint32_t* d_roff = nullptr; uint32_t* d_soff = nullptr; uint8_t* d_sarena = nullptr;
+    uint32_t* d_vars = nullptr;
+    size_t cap_rbytes = 0, cap_rreqs = 0, cap_sarena = 0, cap_vars = 0;
     // pinned staging for the tiny per-chunk read-backs
     uint32_t* h_tail = nullptr;  // [0] = chunk total bytes (connections: records), [1] = overflow flag; log: [2] lines, [3] overflow
 
@@ -412,6 +419,7 @@ void gofr_engine_destroy(gofr_engine* e) {
         cudaFree(s.d_req_first); cudaFree(s.d_rec); cudaFree(s.d_pdesc); cudaFree(s.d_pstatus); cudaFree(s.d_spans); cudaFree(s.d_req_at);
         cudaFree(s.d_remote); cudaFree(s.d_remote_off); cudaFree(s.d_start); cudaFree(s.d_lfirst); cudaFree(s.d_ldesc); cudaFree(s.d_lids);
         cudaFree(s.d_lreq); cudaFree(s.d_lraw_off); cudaFree(s.d_loff); cudaFree(s.d_larena); cudaFree(s.d_lraw); cudaFree(s.d_lout);
+        cudaFree(s.d_rbytes); cudaFree(s.d_roff); cudaFree(s.d_soff); cudaFree(s.d_sarena); cudaFree(s.d_vars);
         if (s.h_tail) cudaFreeHost(s.h_tail);
     }
     for (auto& ev : e->timing) { cudaEventDestroy(ev.first); cudaEventDestroy(ev.second); }
@@ -1207,9 +1215,9 @@ static int conn_plan(const gofr_engine* e, const gofr_conn_batch* in, const gofr
 }
 
 // First half of a chunk: stage its bytes, frame them, and bring back its record count (s.h_tail[0]) and its per-connection
-// columns.  s.done marks the moment the host may read them.
-static int conn_frame(gofr_engine* e, const gofr_conn_batch* in, gofr_conn_resp* out, const gofr_conn_log* log, Slot& s,
-                      const ConnChunk& c) {
+// columns (the caller's consumed and conn_status).  s.done marks the moment the host may read them.
+static int conn_frame(gofr_engine* e, const gofr_conn_batch* in, uint32_t* consumed, uint32_t* conn_status, const gofr_conn_log* log,
+                      Slot& s, const ConnChunk& c) {
     const uint32_t cn = c.hi - c.lo, bytes = in->buf_off[c.hi] - c.alo;
     const uint64_t sizes[2] = {0, bytes};  // the chunk's paths, queries and bodies: never more than its bytes
     int rc = s.reserve(e, c.rec_cap, (size_t)bytes + 16, chunk_out_bound(e, c.rec_cap, sizes));
@@ -1232,8 +1240,8 @@ static int conn_frame(gofr_engine* e, const gofr_conn_batch* in, gofr_conn_resp*
     rc = launch_frames_locked(e, K_HTTP_FRAME, 0, p, cn, (uint8_t*)s.d_rec, c.rec_cap, s.d_first, s.state, s.d_flag, e->st_compute);
     if (rc) return rc;
     CUDA_TRY(cudaMemcpyAsync(&s.h_tail[0], s.d_first + cn, 4, cudaMemcpyDeviceToHost, e->st_compute));
-    CUDA_TRY(cudaMemcpyAsync(out->conn_status + c.lo, s.d_cstatus, (size_t)cn * 4, cudaMemcpyDeviceToHost, e->st_compute));
-    CUDA_TRY(cudaMemcpyAsync(out->consumed + c.lo, s.d_consumed, (size_t)cn * 4, cudaMemcpyDeviceToHost, e->st_compute));
+    CUDA_TRY(cudaMemcpyAsync(conn_status + c.lo, s.d_cstatus, (size_t)cn * 4, cudaMemcpyDeviceToHost, e->st_compute));
+    CUDA_TRY(cudaMemcpyAsync(consumed + c.lo, s.d_consumed, (size_t)cn * 4, cudaMemcpyDeviceToHost, e->st_compute));
     CUDA_TRY(cudaEventRecord(s.done, e->st_compute));
     return GOFR_OK;
 }
@@ -1319,14 +1327,16 @@ static int conn_log_chunk(gofr_engine* e, const gofr_conn_batch* in, const gofr_
     return GOFR_OK;
 }
 
-// Second half of chunk ci: parse its records, compact the whole requests, serve them, and send the results to the caller's
-// columns.  The record count and the connection states are on the host by now: they size the launches.
-static int conn_serve(gofr_engine* e, const gofr_conn_batch* in, gofr_conn_resp* out, const gofr_conn_log* log, Slot& s,
-                      size_t ci, const ConnChunk& c, ConnRun& r, PackedOut& ro, PackedOut& lo) {
+// The chunk's framing is back: parse its records and compact its whole requests into s.d_desc, s.d_req_at, s.d_ids and
+// s.d_req_first (batch request indices from req0).  The record count and the connection states (conn_status, on the host
+// by now) size the launches; *n_req receives the chunk's request count.
+static int conn_parse(gofr_engine* e, const gofr_conn_batch* in, const uint32_t* conn_status, Slot& s, const ConnChunk& c,
+                      uint32_t req0, uint32_t* n_req_out) {
     CUDA_TRY(cudaEventSynchronize(s.done));
     const uint32_t cn = c.hi - c.lo, n_rec = s.h_tail[0];
     uint32_t n_req = n_rec;
-    for (uint32_t k = c.lo; k < c.hi; k++) n_req -= out->conn_status[k] != GOFR_HTTP_CONN_DONE ? 1u : 0u;
+    for (uint32_t k = c.lo; k < c.hi; k++) n_req -= conn_status[k] != GOFR_HTTP_CONN_DONE ? 1u : 0u;
+    *n_req_out = n_req;
     cudaStream_t st = e->st_compute;
     if (n_rec) {  // every record's result lands in the bytes it occupies: no look-back, the whole resident grid runs
         const int resident = resident_grid(e, K_HTTP);
@@ -1341,15 +1351,72 @@ static int conn_serve(gofr_engine* e, const gofr_conn_batch* in, gofr_conn_resp*
     ConnParams q;
     memset(&q, 0, sizeof q);
     q.first = s.d_first; q.conn_status = s.d_cstatus; q.rec_off = s.d_rec; q.desc_in = s.d_pdesc;
-    q.trace_seed = in->trace_seed; q.conn0 = c.lo; q.req0 = (uint32_t)r.req_base; q.req_at = s.d_req_at; q.ids = (uint8_t*)s.d_ids;
-    int rc = launch_frames_locked(e, K_CONN, 0, q, cn, (uint8_t*)s.d_desc, n_rec, s.d_req_first, s.state, s.d_flag, st);
+    q.trace_seed = in->trace_seed; q.conn0 = c.lo; q.req0 = req0; q.req_at = s.d_req_at; q.ids = (uint8_t*)s.d_ids;
+    return launch_frames_locked(e, K_CONN, 0, q, cn, (uint8_t*)s.d_desc, n_rec, s.d_req_first, s.state, s.d_flag, st);
+}
+
+// The closures' results of chunk c (gofr_conn_batch_respond), after its compact step: the chunk's records, those of batch
+// requests [req_base, req_base + n_req), go up, and the splice kernel writes every request of the chunk into the slot's
+// spliced arena, in request order, rewriting the descriptors in place.  *d_arena receives the arena the serve kernel reads.
+static int conn_splice_chunk(gofr_engine* e, const gofr_conn_batch* in, const gofr_conn_results* res, Slot& s, const ConnChunk& c,
+                             uint64_t req_base, uint32_t n_req, const uint8_t** d_arena) {
+    if (req_base + n_req > res->n_req || (c.hi == in->n_conns && req_base + n_req != res->n_req)) {
+        set_last_error("the results are for %u requests, the connections hold %s%llu", res->n_req,
+                       c.hi == in->n_conns ? "" : "at least ", (unsigned long long)(req_base + n_req));
+        return GOFR_ERR_INVALID;
+    }
+    if (!n_req) return GOFR_OK;
+    const uint32_t* ro = res->rec_off + req_base;
+    for (uint32_t k = 0; k < n_req; k++)
+        if (ro[k + 1] < ro[k] || ro[k + 1] > res->rec_bytes) {
+            set_last_error("rec_off[%llu] decreases or passes rec_bytes", (unsigned long long)(req_base + k + 1));
+            return GOFR_ERR_INVALID;
+        }
+    // the spliced arena is addressed with 32-bit offsets: each request takes its path, query and data section plus two pads
+    // of at most 3 bytes, and its path, query and body are never longer than its message
+    const uint32_t rlo = ro[0] & ~15u, rhi = ro[n_req], bytes = in->buf_off[c.hi] - c.alo;
+    const uint64_t spliced = (uint64_t)bytes + (rhi - ro[0]) + 8ull * n_req;
+    if (spliced + 64 > 0xFFFFFFFFull) {
+        set_last_error("the spliced requests of connections %u..%u could pass 4 GiB", c.lo, c.hi);
+        return GOFR_ERR_UNSUPPORTED;
+    }
+    // the serve kernel's output bound: the data sections are the chunk's bytes and records now (a path byte is bounded by
+    // a data byte's expansion)
+    const uint64_t sizes[2] = {0, spliced};
+    int rc = grow_cols(&s.cap_rreqs, n_req, "requests", {{&s.d_roff, 4, 4}, {&s.d_soff, 4, 4}});
+    if (!rc) rc = grow((void**)&s.d_rbytes, &s.cap_rbytes, (size_t)(rhi - rlo) + 16, 256);
+    if (!rc) rc = grow((void**)&s.d_sarena, &s.cap_sarena, (size_t)spliced + 16, 256);
+    if (!rc) rc = grow((void**)&s.d_out, &s.cap_out, chunk_out_bound(e, n_req, sizes), 256);
     if (rc) return rc;
+    cudaStream_t st = e->st_compute;
+    if (rhi > rlo) CUDA_TRY(cudaMemcpyAsync(s.d_rbytes, res->rec + rlo, rhi - rlo, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(s.d_roff, ro, (size_t)(n_req + 1) * 4, cudaMemcpyHostToDevice, st));
+    ConnResultParams p;
+    memset(&p, 0, sizeof p);
+    p.desc = s.d_desc; p.arena = s.d_arena - c.alo; p.rec = s.d_rbytes - rlo; p.rec_off = s.d_roff;
+    rc = launch_frames_locked(e, K_CONN_RESULT, 0, p, n_req, s.d_sarena, s.cap_sarena, s.d_soff, s.state, s.d_flag, st);
+    if (rc) return rc;
+    *d_arena = s.d_sarena;
+    return GOFR_OK;
+}
+
+// Second half of chunk ci: parse its records, compact the whole requests, splice the closures' results in (res not null),
+// serve them, and send the results to the caller's columns.
+static int conn_serve(gofr_engine* e, const gofr_conn_batch* in, const gofr_conn_results* res, gofr_conn_resp* out,
+                      const gofr_conn_log* log, Slot& s, size_t ci, const ConnChunk& c, ConnRun& r, PackedOut& ro, PackedOut& lo) {
+    const uint32_t cn = c.hi - c.lo;
+    uint32_t n_req = 0;
+    int rc = conn_parse(e, in, out->conn_status, s, c, (uint32_t)r.req_base, &n_req);
+    if (rc) return rc;
+    cudaStream_t st = e->st_compute;
+    const uint8_t* d_arena = s.d_arena - c.alo;
+    if (res && (rc = conn_splice_chunk(e, in, res, s, c, r.req_base, n_req, &d_arena)) != 0) return rc;
     if (r.req_base + n_req > out->req_cap) r.req_short = true;
     const bool put = !r.req_short && n_req;  // this chunk's per-request columns go to the caller
     uint32_t* ends = ro.ends(e, ci);         // the chunk's first and end response offsets: what it needs of out_cap
     ends[0] = ends[1] = 0;
     if (n_req) {
-        rc = launch_serve(e, s.d_desc, s.d_ids, s.d_arena - c.alo, n_req, in->date, s.d_out, s.cap_out, s.d_off, s.d_meta, &s.state,
+        rc = launch_serve(e, s.d_desc, s.d_ids, d_arena, n_req, in->date, s.d_out, s.cap_out, s.d_off, s.d_meta, &s.state,
                           s.d_flag, s.d_bind, st, ro.chain(e));
         if (rc) return rc;
         CUDA_TRY(cudaMemcpyAsync(&ends[0], s.d_off, 4, cudaMemcpyDeviceToHost, st));
@@ -1394,7 +1461,8 @@ static int conn_serve(gofr_engine* e, const gofr_conn_batch* in, gofr_conn_resp*
 
 // The chunks of a connection batch, one framed ahead of the one being served: the host learns a chunk's record count while
 // the next chunk's bytes are on their way.
-static int conn_batch_locked(gofr_engine* e, const gofr_conn_batch* in, gofr_conn_resp* out, gofr_conn_log* log, gofr_ticket* ticket) {
+static int conn_batch_locked(gofr_engine* e, const gofr_conn_batch* in, const gofr_conn_results* res, gofr_conn_resp* out,
+                             gofr_conn_log* log, gofr_ticket* ticket) {
     const uint32_t n = in->n_conns;
     out->out_bytes = 0;
     if (log) { log->lines = 0; log->out_bytes = 0; }
@@ -1425,12 +1493,12 @@ static int conn_batch_locked(gofr_engine* e, const gofr_conn_batch* in, gofr_con
         while (next < n && issued < served + 2) {
             ConnChunk& c = chunks[issued % kSlots];
             int rc = conn_plan(e, in, log, next, &c);
-            if (!rc) rc = conn_frame(e, in, out, log, e->slots[issued % kSlots], c);
+            if (!rc) rc = conn_frame(e, in, out->consumed, out->conn_status, log, e->slots[issued % kSlots], c);
             if (rc) return rc;
             next = c.hi;
             issued++;
         }
-        int rc = conn_serve(e, in, out, log, e->slots[served % kSlots], served, chunks[served % kSlots], r, ro, lo);
+        int rc = conn_serve(e, in, res, out, log, e->slots[served % kSlots], served, chunks[served % kSlots], r, ro, lo);
         if (rc) return rc;
         served++;
     }
@@ -1467,11 +1535,83 @@ int gofr_conn_batch_submit(gofr_engine* e, const gofr_conn_batch* in, gofr_conn_
 }
 
 int gofr_conn_batch_submit_log(gofr_engine* e, const gofr_conn_batch* in, gofr_conn_resp* out, gofr_conn_log* log, gofr_ticket* ticket) {
+    return gofr_conn_batch_respond(e, in, nullptr, out, log, ticket);
+}
+
+int gofr_conn_batch_respond(gofr_engine* e, const gofr_conn_batch* in, const gofr_conn_results* res, gofr_conn_resp* out,
+                            gofr_conn_log* log, gofr_ticket* ticket) {
     if (!e || !in || !out || !ticket) return GOFR_ERR_INVALID;
     if (in->n_conns && (!in->buf || !in->buf_off || !out->out || !out->out_off || !out->meta || !out->req_at || !out->req_first ||
                         !out->consumed || !out->conn_status)) return GOFR_ERR_INVALID;
     if (log && in->n_conns && (!log->remote_off || !log->start_unix_ns || !log->out || !log->log_off || !log->log_req)) return GOFR_ERR_INVALID;
-    return host_batch(e, [&] { return conn_batch_locked(e, in, out, log, ticket); });
+    if (res && in->n_conns && (!res->rec_off || (res->rec_bytes && !res->rec))) return GOFR_ERR_INVALID;
+    if (res && !in->n_conns && res->n_req) { set_last_error("the results are for %u requests, the batch has none", res->n_req); return GOFR_ERR_INVALID; }
+    return host_batch(e, [&] { return conn_batch_locked(e, in, res, out, log, ticket); });
+}
+
+// Stage 1 of the closure path (gofr_conn_batch_route): chunk after chunk, synchronously — frame, parse and compact as the
+// connection pipeline does, route the compacted requests, and bring the chunk's columns and its parse-arena bytes back.
+// A request's parsed form lies inside its own message (include/gofr_b200.h), so a chunk's arena bytes are exactly its
+// connections' byte range, copied to the same offsets of the caller's arena.
+static int conn_route_locked(gofr_engine* e, const gofr_conn_batch* in, gofr_conn_route* out) {
+    const uint32_t n = in->n_conns;
+    const cudaStream_t st = e->st_compute;
+    Slot& s = e->slots[0];
+    uint64_t req_base = 0;
+    bool req_short = false;
+    for (uint32_t lo = 0; lo < n;) {
+        ConnChunk c;
+        uint32_t n_req = 0;
+        int rc = conn_plan(e, in, nullptr, lo, &c);
+        if (!rc) rc = conn_frame(e, in, out->consumed, out->conn_status, nullptr, s, c);
+        if (!rc) rc = conn_parse(e, in, out->conn_status, s, c, (uint32_t)req_base, &n_req);
+        if (rc) return rc;
+        if (req_base + n_req > out->req_cap) req_short = true;
+        if (!req_short && n_req) {
+            const size_t vbytes = (size_t)n_req * 4 * GOFR_MAX_PATH_VARS;
+            rc = grow((void**)&s.d_vars, &s.cap_vars, vbytes, 256);
+            if (!rc) rc = launch_route_kernel(e, s.d_desc, s.d_arena - c.alo, n_req, s.d_meta, s.d_vars, st);
+            if (rc) return rc;
+            const uint32_t a0 = in->buf_off[c.lo], a1 = in->buf_off[c.hi];
+            CUDA_TRY(cudaMemcpyAsync(out->desc + req_base, s.d_desc, (size_t)n_req * 16, cudaMemcpyDeviceToHost, st));
+            CUDA_TRY(cudaMemcpyAsync(out->meta + req_base, s.d_meta, (size_t)n_req * 4, cudaMemcpyDeviceToHost, st));
+            CUDA_TRY(cudaMemcpyAsync(out->vars + req_base * GOFR_MAX_PATH_VARS, s.d_vars, vbytes, cudaMemcpyDeviceToHost, st));
+            CUDA_TRY(cudaMemcpyAsync(out->req_at + req_base, s.d_req_at, (size_t)n_req * 4, cudaMemcpyDeviceToHost, st));
+            CUDA_TRY(cudaMemcpyAsync(out->trace_ids + req_base * 16, s.d_ids, (size_t)n_req * 16, cudaMemcpyDeviceToHost, st));
+            CUDA_TRY(cudaMemcpyAsync(out->arena + a0, s.d_arena + (a0 - c.alo), a1 - a0, cudaMemcpyDeviceToHost, st));
+        }
+        CUDA_TRY(cudaMemcpyAsync(out->req_first + c.lo, s.d_req_first, (size_t)(c.hi - c.lo) * 4, cudaMemcpyDeviceToHost, st));
+        CUDA_TRY(cudaStreamSynchronize(st));
+        req_base += n_req;
+        lo = c.hi;
+    }
+    out->req_first[n] = (uint32_t)req_base;
+    if (req_short) {
+        set_last_error("the batch needs %llu requests: req_cap %u", (unsigned long long)req_base, out->req_cap);
+        return GOFR_ERR_CAPACITY;
+    }
+    return GOFR_OK;
+}
+
+int gofr_conn_batch_route(gofr_engine* e, const gofr_conn_batch* in, gofr_conn_route* out) {
+    if (!e || !in || !out) return GOFR_ERR_INVALID;
+    if (in->n_conns && (!in->buf || !in->buf_off || !out->desc || !out->arena || !out->meta || !out->vars || !out->req_at ||
+                        !out->trace_ids || !out->req_first || !out->consumed || !out->conn_status)) return GOFR_ERR_INVALID;
+    if (!in->n_conns) return GOFR_OK;
+    return host_batch(e, [&] { return conn_route_locked(e, in, out); });
+}
+
+int gofr_conn_respond_bound(const gofr_table* t, const gofr_req_desc* desc, uint32_t n_req, const uint32_t* rec_off, uint64_t* out_cap) {
+    if (!t || !out_cap || (n_req && (!desc || !rec_off))) return GOFR_ERR_INVALID;
+    if (!gofr_table_response_bound(t, 0, 0, 0)) { set_last_error("the table is not sealed"); return GOFR_ERR_NOT_SEALED; }
+    uint64_t b = 0;
+    for (uint32_t k = 0; k < n_req; k++) {
+        if (rec_off[k + 1] < rec_off[k]) { set_last_error("rec_off[%u] decreases", k + 1); return GOFR_ERR_INVALID; }
+        const uint32_t len = rec_off[k + 1] > rec_off[k] ? rec_off[k + 1] - rec_off[k] : desc[k].data_len;
+        b += gofr_table_response_bound(t, desc[k].path_len, desc[k].query_len, len);
+    }
+    *out_cap = b;
+    return GOFR_OK;
 }
 
 int gofr_conn_batch_bound(const gofr_table* t, const uint32_t* buf_off, uint32_t n_conns, uint32_t* req_cap, uint64_t* out_cap) {

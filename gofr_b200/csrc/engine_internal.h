@@ -298,6 +298,24 @@ struct ConnLogParams {
     uint32_t* overflow;
 };
 
+// conn_result_kernel.cu: gofr_conn_batch_respond's splice step, a packed-output kernel over the requests of a chunk whose
+// output is the spliced arena (conn_result_device.cuh): request i's decoded path | query | pad4 | data section, its data
+// section the closure's record rec[rec_off[i] .. rec_off[i + 1]) when that is not empty, else its own body
+struct ConnResultParams {
+    void* desc;                 // gofr_req_desc per request (parse-arena offsets), rewritten in place to spliced-arena ones
+    const uint8_t* arena;       // the parse arena, addressed by absolute buffer offsets
+    const uint8_t* rec;         // the chunk's records, addressed by the caller's record offsets
+    const uint32_t* rec_off;    // n + 1: the caller's rec_off from the chunk's first request on
+    uint32_t n;
+    uint32_t n_tiles;
+    uint32_t epoch;
+    uint8_t* out;               // the spliced arena
+    uint64_t out_cap;
+    uint32_t* out_off;          // n + 1: request i's spliced form starts at out_off[i] (a multiple of 4)
+    unsigned long long* tile_state;
+    uint32_t* overflow;
+};
+
 struct LogParams {
     const void* desc;   // gofr_log_desc[n]
     const void* ids;    // n * 16 trace id bytes

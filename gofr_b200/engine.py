@@ -488,23 +488,101 @@ def conn_log_bound(buf_off: np.ndarray, remote_off: np.ndarray):
     return lc.value, oc.value
 
 
-def _serve_connections(self, buf: np.ndarray, buf_off: np.ndarray, date: bytes, trace_seed: int, pinned: bool = True,
-                       req_cap: Optional[int] = None, out_cap: Optional[int] = None, log: Optional[ConnLog] = None):
-    """gofr_conn_batch_submit + wait: connection c's received bytes are buf[buf_off[c]:buf_off[c + 1]] (host memory).
-    Returns ConnResponses.  The capacities default to conn_batch_bound; pinned puts the outputs in pinned memory (egress
-    driven by the device), else in pageable numpy arrays.  With log (a ConnLog), gofr_conn_batch_submit_log: the result's
-    .log holds the request-log lines, in the same kind of memory."""
+@dataclass
+class ConnRoute:
+    """What gofr_conn_batch_route returns (numpy arrays, sliced to the batch's requests): per request k its route decision
+    (meta[k], vars[k]: as route_host gives them; status 0 = the closure of route meta[k] >> 16 runs), its first byte in buf,
+    its trace id and its parsed form, desc[k] into arena; per connection req_first / consumed / conn_status.  .batch is the
+    requests as a RequestBatch (desc, trace_ids, arena): what gofr_batch_bind takes and what Param / PathParam read."""
+    desc: np.ndarray         # DESC_DTYPE[requests]
+    arena: np.ndarray        # uint8[buf_bytes + 64]
+    meta: np.ndarray         # uint32[requests]
+    vars: np.ndarray         # uint32[requests, 8]: off | len << 16 inside the request's path, 0xFFFFFFFF unused
+    req_at: np.ndarray       # uint32[requests]
+    trace_ids: np.ndarray    # uint8[requests, 16]
+    req_first: np.ndarray    # uint32[n_conns + 1]
+    consumed: np.ndarray     # uint32[n_conns]
+    conn_status: np.ndarray  # uint32[n_conns]
+
+    @property
+    def batch(self) -> S.RequestBatch:
+        return S.RequestBatch(self.desc, self.trace_ids, self.arena)
+
+
+def _alloc(pinned: bool):
+    if pinned:
+        return lambda count, dt: pinned_array(max(count, 1) * np.dtype(dt).itemsize).view(dt)
+    return lambda count, dt: np.zeros(max(count, 1), dt)
+
+
+def _route_connections(self, buf: np.ndarray, buf_off: np.ndarray, trace_seed: int, pinned: bool = True,
+                       req_cap: Optional[int] = None) -> ConnRoute:
+    """gofr_conn_batch_route: stage 1 of serving connection buffers with handler closures (frame, parse and route on the
+    device).  Run the closures of the requests whose status is 0, then hand their GOFR_H_RESULT records to
+    serve_connections(..., results=(rec, rec_off)) with the same buf, buf_off and trace_seed.  req_cap defaults to
+    conn_batch_bound's; pinned puts the outputs in pinned memory, else in pageable numpy arrays."""
     buf = np.ascontiguousarray(buf, dtype=np.uint8)
     off = np.ascontiguousarray(buf_off, dtype=np.uint32)
     n = len(off) - 1
+    if req_cap is None:
+        req_cap, _ = conn_batch_bound(self.table, off)
+    alloc = _alloc(pinned)
+    desc, arena = alloc(req_cap, S.DESC_DTYPE), alloc(buf.size + 64, np.uint8)
+    meta, vars_, req_at = alloc(req_cap, np.uint32), alloc(req_cap * 8, np.uint32), alloc(req_cap, np.uint32)
+    ids = alloc(req_cap * 16, np.uint8)
+    req_first, consumed, status = alloc(n + 1, np.uint32), alloc(n, np.uint32), alloc(n, np.uint32)
+    cb = _abi.ConnBatch(buf=buf.ctypes.data, buf_off=off.ctypes.data, buf_bytes=buf.size, n_conns=n, date=b"", trace_seed=trace_seed)
+    cr = _abi.ConnRoute(req_cap=req_cap, desc=desc.ctypes.data, arena=arena.ctypes.data, meta=meta.ctypes.data,
+                        vars=vars_.ctypes.data, req_at=req_at.ctypes.data, trace_ids=ids.ctypes.data,
+                        req_first=req_first.ctypes.data, consumed=consumed.ctypes.data, conn_status=status.ctypes.data)
+    _abi.check(_abi.lib().gofr_conn_batch_route(self._e, C.byref(cb), C.byref(cr)), "gofr_conn_batch_route")
+    k = int(req_first[n]) if n else 0
+    return ConnRoute(desc[:k], arena[:buf.size + 64], meta[:k], vars_[:k * 8].reshape(k, 8), req_at[:k], ids[:k * 16].reshape(k, 16),
+                     req_first[:n + 1] if n else np.zeros(1, np.uint32), consumed[:n], status[:n])
+
+
+Engine.route_connections = _route_connections
+
+
+def conn_respond_bound(table: Table, desc: np.ndarray, rec_off: np.ndarray) -> int:
+    """gofr_conn_respond_bound: an out_cap that always suffices for serve_connections(..., results=(rec, rec_off)) on the
+    requests stage 1 described (desc: ConnRoute.desc)."""
+    d = np.ascontiguousarray(desc).view(S.DESC_DTYPE)
+    ro = np.ascontiguousarray(rec_off, dtype=np.uint32)
+    assert len(ro) == len(d) + 1
+    oc = C.c_uint64()
+    _abi.check(_abi.lib().gofr_conn_respond_bound(table.handle, d.ctypes.data, len(d), ro.ctypes.data, C.byref(oc)),
+               "gofr_conn_respond_bound")
+    return oc.value
+
+
+def _serve_connections(self, buf: np.ndarray, buf_off: np.ndarray, date: bytes, trace_seed: int, pinned: bool = True,
+                       req_cap: Optional[int] = None, out_cap: Optional[int] = None, log: Optional[ConnLog] = None,
+                       results=None):
+    """gofr_conn_batch_submit + wait: connection c's received bytes are buf[buf_off[c]:buf_off[c + 1]] (host memory).
+    Returns ConnResponses.  The capacities default to conn_batch_bound; pinned puts the outputs in pinned memory (egress
+    driven by the device), else in pageable numpy arrays.  With log (a ConnLog), gofr_conn_batch_submit_log: the result's
+    .log holds the request-log lines, in the same kind of memory.  With results = (rec uint8, rec_off uint32[requests + 1]),
+    gofr_conn_batch_respond: stage 2 after route_connections on the same buffers and seed, request k's data section is its
+    closure's record rec[rec_off[k]:rec_off[k + 1]] where that is not empty; out_cap then defaults to the larger of
+    conn_batch_bound's and what the records need (conn_respond_bound over the requests the table's bound assumes)."""
+    buf = np.ascontiguousarray(buf, dtype=np.uint8)
+    off = np.ascontiguousarray(buf_off, dtype=np.uint32)
+    n = len(off) - 1
+    rres = None
+    if results is not None:
+        rec = np.ascontiguousarray(results[0], dtype=np.uint8)
+        roff = np.ascontiguousarray(results[1], dtype=np.uint32)
+        rres = _abi.ConnResults(rec=rec.ctypes.data if rec.size else None, rec_off=roff.ctypes.data, rec_bytes=rec.size,
+                                n_req=len(roff) - 1)
     if req_cap is None or out_cap is None:
         rc, oc = conn_batch_bound(self.table, off)
+        if results is not None:   # every request's data section may be a record: per byte of a record, the table's bound
+            rb = lambda dl: _abi.lib().gofr_table_response_bound(self.table.handle, 0, 0, dl)
+            oc += (rb(1) - rb(0)) * rec.size
         req_cap = rc if req_cap is None else req_cap
         out_cap = oc if out_cap is None else out_cap
-    if pinned:
-        alloc = lambda count, dt: pinned_array(max(count, 1) * np.dtype(dt).itemsize).view(dt)
-    else:
-        alloc = lambda count, dt: np.zeros(max(count, 1), dt)
+    alloc = _alloc(pinned)
     out, out_off, meta = alloc(out_cap, np.uint8), alloc(req_cap + 1, np.uint32), alloc(req_cap, np.uint32)
     req_at, ids = alloc(req_cap, np.uint32), alloc(req_cap * 16, np.uint8)
     req_first, consumed, status = alloc(n + 1, np.uint32), alloc(n, np.uint32), alloc(n, np.uint32)
@@ -515,7 +593,10 @@ def _serve_connections(self, buf: np.ndarray, buf_off: np.ndarray, date: bytes, 
                        consumed=consumed.ctypes.data, conn_status=status.ctypes.data, out_bytes=0)
     L = _abi.lib()
     t = C.c_uint64()
-    if log is None:
+    if results is not None and log is None:
+        _abi.check(L.gofr_conn_batch_respond(self._e, C.byref(cb), C.byref(rres), C.byref(cr), None, C.byref(t)),
+                   "gofr_conn_batch_respond")
+    elif log is None:
         _abi.check(L.gofr_conn_batch_submit(self._e, C.byref(cb), C.byref(cr), C.byref(t)), "gofr_conn_batch_submit")
     else:
         remote = np.ascontiguousarray(log.remote, dtype=np.uint8)
@@ -531,8 +612,12 @@ def _serve_connections(self, buf: np.ndarray, buf_off: np.ndarray, date: bytes, 
         cl = _abi.ConnLog(remote=remote.ctypes.data, remote_off=roff.ctypes.data, start_unix_ns=start.ctypes.data,
                           log_unix_ns=log.log_unix_ns, tz_offset_s=log.tz_offset_s, line_cap=line_cap, out=lout.ctypes.data,
                           out_cap=lout_cap, log_off=log_off.ctypes.data, log_req=log_req.ctypes.data)
-        _abi.check(L.gofr_conn_batch_submit_log(self._e, C.byref(cb), C.byref(cr), C.byref(cl), C.byref(t)),
-                   "gofr_conn_batch_submit_log")
+        if results is not None:
+            _abi.check(L.gofr_conn_batch_respond(self._e, C.byref(cb), C.byref(rres), C.byref(cr), C.byref(cl), C.byref(t)),
+                       "gofr_conn_batch_respond")
+        else:
+            _abi.check(L.gofr_conn_batch_submit_log(self._e, C.byref(cb), C.byref(cr), C.byref(cl), C.byref(t)),
+                       "gofr_conn_batch_submit_log")
     _abi.check(L.gofr_batch_wait(self._e, t.value), "gofr_batch_wait")
     k = int(req_first[n]) if n else 0
     lines = None

@@ -837,6 +837,73 @@ int gofr_conn_batch_submit_log(gofr_engine*, const gofr_conn_batch* in, gofr_con
 int gofr_conn_log_bound(const uint32_t* buf_off, const uint32_t* remote_off, uint32_t n_conns, uint32_t* line_cap,
                         uint64_t* out_cap);
 
+/* Connection buffers served with the app's handler closures, in two calls.  Stage 1 frames, parses and routes the buffers
+ * on the device and hands back everything a closure needs; the caller runs the closures of the requests whose status is 0
+ * and encodes their (data, err) as GOFR_H_RESULT records; stage 2 splices those records in on the device and answers every
+ * request of every connection, as gofr_conn_batch_submit_log does.
+ *
+ * Stage 1 (synchronous): requests are numbered as gofr_conn_batch_submit numbers them, and their trace ids are the same
+ * function of (trace_seed, c, j).
+ *   out  per request k:
+ *          meta[k], vars[k * GOFR_MAX_PATH_VARS ..]  as gofr_route_device gives them: status 301 / 404 / 405 / 200 (OPTIONS),
+ *                                                   or 0 = the handler of route GOFR_META_ROUTE(meta[k]) runs;
+ *          req_at[k], trace_ids[16k ..]              as gofr_conn_batch_submit's;
+ *          desc[k]                                   the parsed request: arena[desc[k].arena_off ..] holds its decoded
+ *                                                   URL.Path | URL.RawQuery | pad4 | body (de-chunked), the layout of
+ *                                                   gofr_http_parse_device; so (desc, trace_ids, arena) is a valid
+ *                                                   gofr_req_batch, which gofr_batch_bind takes for Context.Bind;
+ *        per connection c: req_first, consumed, conn_status as gofr_conn_batch_submit's.
+ *   arena has buf_bytes + 64 bytes.  A request's parsed form starts at its first byte in buf rounded up to 4 and ends
+ *   inside its own message (a message of the subset is longer than its target plus its body plus 6 bytes), so each chunk
+ *   copies back exactly the bytes [buf_off[lo], buf_off[hi]) of its connections, at their own offsets; arena bytes that
+ *   belong to no request's parsed form are unspecified.
+ * Capacity: req_cap as for gofr_conn_batch_submit (gofr_conn_batch_bound).  When it is too small the call returns
+ * GOFR_ERR_CAPACITY, req_first[n_conns] is what the batch needed, the per-connection columns are complete and no
+ * per-request entry at or past req_cap is written.  GOFR_ERR_INVALID: gofr_conn_batch_submit's cases, a null column.
+ *
+ * Stage 2 (collect with gofr_batch_wait): in must be the buffers, offsets and trace_seed stage 1 saw.  Record k (requests
+ * numbered as in stage 1) is rec[rec_off[k] .. rec_off[k+1]); rec_off has n_req + 1 entries and n_req is stage 1's request
+ * count.  A non-empty record replaces request k's data section: a GOFR_H_RESULT record (include/gofr_b200.h, handler kinds),
+ * answered by Responder.Respond on the device.  An empty record leaves the request's own body in place, so fused kinds, the
+ * router's own answers and GOFR_H_HOST holes are answered exactly as gofr_conn_batch_submit answers them.  out and log are
+ * gofr_conn_batch_submit_log's; a request whose record produced a status gets its log line by that call's rule.  With
+ * res == NULL the call is gofr_conn_batch_submit_log.
+ * Nothing is kept between the stages: stage 2 uploads, frames and parses the buffers again.  It cannot tell buffers that
+ * changed since stage 1 from the ones stage 1 saw, other than by their request count: res->n_req must equal it
+ * (GOFR_ERR_INVALID otherwise, checked before the last chunk is served).
+ * GOFR_ERR_INVALID also for gofr_conn_batch_submit_log's cases, a null rec_off (or a null rec with rec_bytes > 0), record
+ * offsets that decrease or pass rec_bytes; these are checked chunk by chunk, and a refused batch leaves the engine usable.
+ * GOFR_ERR_UNSUPPORTED: a chunk whose spliced requests (its buffer bytes plus its record bytes plus 8 per request) could
+ * pass 4 GiB.  gofr_conn_respond_bound (host only) gives an out_cap that always suffices: the sum of
+ * gofr_table_response_bound(path_len, query_len, len) over stage 1's descriptors, len the record's length when it is not
+ * empty, else data_len. */
+typedef struct gofr_conn_route {
+    uint32_t req_cap;
+    uint32_t reserved;
+    gofr_req_desc* desc;    /* req_cap */
+    uint8_t* arena;         /* buf_bytes + 64 */
+    uint32_t* meta;         /* req_cap */
+    uint32_t* vars;         /* req_cap * GOFR_MAX_PATH_VARS */
+    uint32_t* req_at;       /* req_cap */
+    uint8_t* trace_ids;     /* req_cap * 16 */
+    uint32_t* req_first;    /* n_conns + 1 */
+    uint32_t* consumed;     /* n_conns */
+    uint32_t* conn_status;  /* n_conns */
+} gofr_conn_route;
+int gofr_conn_batch_route(gofr_engine*, const gofr_conn_batch* in, gofr_conn_route* out);
+
+typedef struct gofr_conn_results {
+    const uint8_t* rec;
+    const uint32_t* rec_off;  /* n_req + 1 */
+    uint64_t rec_bytes;
+    uint32_t n_req;
+    uint32_t reserved;
+} gofr_conn_results;
+int gofr_conn_batch_respond(gofr_engine*, const gofr_conn_batch* in, const gofr_conn_results* res, gofr_conn_resp* out,
+                            gofr_conn_log* log, gofr_ticket* ticket);
+int gofr_conn_respond_bound(const gofr_table*, const gofr_req_desc* desc, uint32_t n_req, const uint32_t* rec_off,
+                            uint64_t* out_cap);
+
 /* number of kernels launched by this engine so far (bench.py reports it as gpu_launches) */
 uint64_t gofr_engine_launch_count(const gofr_engine*);
 /* duration in ms of the kernels launched since the last reset, measured with CUDA events on the launch stream.  Every

@@ -447,6 +447,127 @@ public:
         return out;
     }
 
+    // What ServeConnections hands back for one connection: the bytes to write, how many of its received bytes they answer,
+    // and GOFR_HTTP_CONN_DONE / MORE (keep the bytes from `consumed` on and append the next read) / DEFER (hand the bytes
+    // from `consumed` on to net/http).
+    struct ConnResponse {
+        std::string bytes;
+        uint32_t consumed = 0;
+        uint32_t conn_status = GOFR_HTTP_CONN_DONE;
+    };
+
+    // net/http's conn.serve → router.ServeHTTP for a batch of connections: buffers[c] is what connection c received (pipelined
+    // requests, maybe the first part of the next one).  Frames, parses and routes them on the GPU (gofr_conn_batch_route),
+    // binds the bodies of the routes that declared a struct type (gofr_batch_bind on the exported requests), runs the closures
+    // with a Context built from the parsed request, then splices their results in and answers every request on the GPU
+    // (gofr_conn_batch_respond).  Request j of connection c gets the trace id include/gofr_b200.h states for (trace_seed, c, j).
+    std::vector<ConnResponse> ServeConnections(const std::vector<std::string>& buffers, uint64_t trace_seed, int64_t unix_now = 0) {
+        if (!engine_) throw std::logic_error("gofr::App: call Run before ServeConnections");
+        const uint32_t nc = (uint32_t)buffers.size();
+        std::vector<ConnResponse> out(nc);
+        if (!nc) return out;
+        std::string buf;
+        std::vector<uint32_t> boff(nc + 1);
+        for (uint32_t c = 0; c < nc; c++) {
+            boff[c] = (uint32_t)buf.size();
+            buf += buffers[c];
+            if (buf.size() > 0xFFFFFFF0u) throw std::invalid_argument("gofr::App::ServeConnections: more than 4 GiB of buffers");
+        }
+        boff[nc] = (uint32_t)buf.size();
+        buf.append(16, '\0');
+        gofr_conn_batch in;
+        memset(&in, 0, sizeof in);
+        in.buf = (const uint8_t*)buf.data(); in.buf_off = boff.data(); in.buf_bytes = boff[nc]; in.n_conns = nc;
+        in.trace_seed = trace_seed;
+        gofr_format_http_date(unix_now ? unix_now : (int64_t)time(nullptr), in.date);
+        uint32_t req_cap = 0;
+        uint64_t cap0 = 0;
+        check(gofr_conn_batch_bound(table_, boff.data(), nc, &req_cap, &cap0), "gofr_conn_batch_bound");
+        const size_t rc1 = std::max<uint32_t>(req_cap, 1);
+        // ---- stage 1 (GPU): frame, parse, route; the parsed requests come back ----
+        std::vector<gofr_req_desc> desc(rc1);
+        std::vector<uint8_t> arena((size_t)boff[nc] + 64), ids(rc1 * 16);
+        std::vector<uint32_t> meta(rc1), vars(rc1 * GOFR_MAX_PATH_VARS), req_at(rc1), req_first(nc + 1), consumed(nc), cstat(nc);
+        gofr_conn_route rt;
+        memset(&rt, 0, sizeof rt);
+        rt.req_cap = req_cap; rt.desc = desc.data(); rt.arena = arena.data(); rt.meta = meta.data(); rt.vars = vars.data();
+        rt.req_at = req_at.data(); rt.trace_ids = ids.data(); rt.req_first = req_first.data(); rt.consumed = consumed.data();
+        rt.conn_status = cstat.data();
+        check(gofr_conn_batch_route(engine_, &in, &rt), "gofr_conn_batch_route");
+        const uint32_t n = req_first[nc];
+        auto bytes_at = [&](uint32_t off, uint32_t len) { return std::string((const char*)arena.data() + off, len); };
+        std::vector<Parsed> ps(n);
+        std::vector<Request> rq(n);
+        for (uint32_t i = 0; i < n; i++) {
+            const gofr_req_desc& d = desc[i];
+            ps[i].path = bytes_at(d.arena_off, d.path_len);
+            ps[i].query = bytes_at(d.arena_off + d.path_len, d.query_len);
+            ps[i].force_query = (d.flags & GOFR_REQ_FORCE_QUERY) != 0;
+            rq[i].method = method_name(d.method);
+            rq[i].body = bytes_at(d.arena_off + ((d.path_len + d.query_len + 3u) & ~3u), d.data_len);
+        }
+        // ---- stage 1b (GPU): Context.Bind on the exported requests, per struct type ----
+        std::vector<Bound> bound(n);
+        for (auto& t : types_) {
+            std::vector<uint32_t> who;
+            for (uint32_t i = 0; i < n; i++) {
+                const uint32_t status = meta[i] & 0xFFFFu, route = meta[i] >> 16;
+                if (status == 0 && route < routes_.size() && routes_[route].bind_type == t->id_) who.push_back(i);
+            }
+            if (who.empty()) continue;
+            std::vector<gofr_req_desc> bd(who.size());
+            size_t longest = 0;
+            for (size_t k = 0; k < who.size(); k++) {
+                bd[k] = desc[who[k]];
+                longest = std::max<size_t>(longest, bd[k].data_len);
+            }
+            gofr_req_batch bin;
+            memset(&bin, 0, sizeof bin);
+            bin.desc = bd.data(); bin.arena = arena.data(); bin.arena_bytes = arena.size(); bin.n = (uint32_t)who.size();
+            const uint32_t slot = (uint32_t)((8 * t->fields_.size() + longest + 256 + 15) & ~(size_t)15);
+            std::vector<uint8_t> rows((size_t)who.size() * slot);
+            std::vector<uint32_t> blen(who.size()), bstat(who.size());
+            check(gofr_batch_bind(engine_, t->id_, &bin, rows.data(), slot, blen.data(), bstat.data()), "gofr_batch_bind");
+            for (size_t k = 0; k < who.size(); k++) {
+                bound[who[k]].status = blen[k] > slot ? (uint32_t)GOFR_BIND_HOST : bstat[k];
+                bound[who[k]].row.assign((const char*)rows.data() + k * slot, std::min<uint32_t>(blen[k], slot));
+            }
+        }
+        // ---- the closures (host), only where the reference would have called one ----
+        std::string rec;
+        std::vector<uint32_t> rec_off(n + 1);
+        for (uint32_t i = 0; i < n; i++) {
+            rec_off[i] = (uint32_t)rec.size();
+            const uint32_t status = meta[i] & 0xFFFFu, route = meta[i] >> 16;
+            if (status == 0 && route < routes_.size()) rec += run_handler(routes_[route], rq[i], ps[i], &vars[(size_t)i * GOFR_MAX_PATH_VARS], bound[i]);
+            if (rec.size() > 0xFFFFFFF0u) throw std::invalid_argument("gofr::App::ServeConnections: more than 4 GiB of handler results");
+        }
+        rec_off[n] = (uint32_t)rec.size();
+        // ---- stage 2 (GPU): the results spliced in, Responder.Respond + framing for every request ----
+        uint64_t cap = 0;
+        check(gofr_conn_respond_bound(table_, desc.data(), n, rec_off.data(), &cap), "gofr_conn_respond_bound");
+        cap += 4096;
+        gofr_conn_results res;
+        memset(&res, 0, sizeof res);
+        res.rec = (const uint8_t*)rec.data(); res.rec_off = rec_off.data(); res.rec_bytes = rec.size(); res.n_req = n;
+        std::vector<uint8_t> bytes(cap);
+        std::vector<uint32_t> off(rc1 + 1);
+        gofr_conn_resp o;
+        memset(&o, 0, sizeof o);
+        o.out = bytes.data(); o.out_cap = cap; o.req_cap = req_cap; o.out_off = off.data(); o.meta = meta.data();
+        o.req_at = req_at.data(); o.req_first = req_first.data(); o.consumed = consumed.data(); o.conn_status = cstat.data();
+        gofr_ticket tk = 0;
+        check(gofr_conn_batch_respond(engine_, &in, &res, &o, nullptr, &tk), "gofr_conn_batch_respond");
+        check(gofr_batch_wait(engine_, tk), "gofr_batch_wait");
+        for (uint32_t c = 0; c < nc; c++) {
+            const uint32_t a = off[req_first[c]], b = off[req_first[c + 1]];
+            out[c].bytes.assign((const char*)bytes.data() + a, b - a);
+            out[c].consumed = consumed[c];
+            out[c].conn_status = cstat[c];
+        }
+        return out;
+    }
+
     // url.ParseRequestURI as Serve applies it to Request::target (tests): false for what httptest.NewRequest would refuse
     static bool ParseTarget(const std::string& target, std::string* path, std::string* raw_query, bool* force_query) {
         try {
@@ -478,11 +599,16 @@ private:
     static void check(int rc, const char* where) {
         if (rc != GOFR_OK) throw std::runtime_error(std::string(where) + ": " + gofr_last_error());
     }
-    static uint8_t method_code(const std::string& m) {
+    static const char* const* method_names() {
         static const char* names[] = {"GET", "HEAD", "POST", "PUT", "PATCH", "DELETE", "CONNECT", "OPTIONS", "TRACE"};
-        for (uint8_t k = 0; k < 9; k++) if (m == names[k]) return k;
+        return names;
+    }
+    static uint8_t method_code(const std::string& m) {
+        for (uint8_t k = 0; k < 9; k++) if (m == method_names()[k]) return k;
         return GOFR_M_OTHER;
     }
+    // the request-head parser only accepts the methods with a code below 9
+    static std::string method_name(uint8_t code) { return code < 9 ? method_names()[code] : ""; }
     // url.ParseRequestURI for an origin-form target: Path is the unescaped part before the first '?', RawQuery the rest
     static Parsed parse_target(const std::string& target) {
         if (target.empty() || target[0] != '/') throw std::invalid_argument("gofr::App: request target must be in origin form: " + target);
