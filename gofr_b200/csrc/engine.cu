@@ -161,7 +161,7 @@ struct Slot {
     uint32_t* d_vars = nullptr;
     size_t cap_rbytes = 0, cap_rreqs = 0, cap_sarena = 0, cap_vars = 0;
     // pinned staging for the tiny per-chunk read-backs
-    uint32_t* h_tail = nullptr;  // [0] = chunk total bytes (connections: records), [1] = overflow flag; log: [2] lines, [3] overflow
+    uint32_t* h_tail = nullptr;  // [0] = chunk total bytes (connections: records), [2] = log lines; [2k + 1] = output k's overflow word
 
     int reserve(gofr_engine* e, uint32_t requests, size_t arena_bytes, size_t out_bytes);
     int reserve_codec(uint32_t records, size_t a_bytes, size_t b_bytes);
@@ -201,8 +201,8 @@ struct gofr_engine {
     unsigned long long* d_chain = nullptr;  // packed position of the batch in flight
     ChunkInfo* d_info = nullptr;            // two per slot: [slot] the responses, [kSlots + slot] the request-log lines
     unsigned long long* h_status = nullptr; // pinned: [0] total bytes, [1] overflow; [2], [3] the same for the log lines
-    uint32_t* h_ends = nullptr;             // pinned, gofr_conn_batch_submit: per chunk its first and end response offsets,
-                                            // then its first and end log line offsets
+    uint32_t* h_ends = nullptr;             // pinned, gofr_conn_batch_submit: per shipped chunk its first and end response
+                                            // offsets, then its first and end log line offsets (PackedOut::ship)
     size_t ends_cap = 0;                    // (words)
     int egress_grid = 37;
     uint32_t chunk = 65536;
@@ -912,11 +912,26 @@ static bool device_visible(const void* p) {
     return a.type == cudaMemoryTypeHost || a.type == cudaMemoryTypeManaged;
 }
 
+// The records of a batch counted against the caller's record capacity: a chunk's per-record columns are written only
+// while every record so far fits.  From the first chunk that does not, none are (short: the batch fails), and the count
+// goes on, so that the batch reports what it needed.
+struct RecCount {
+    uint64_t cap = 0, base = 0;  // the capacity; the records of the chunks before
+    bool short_ = false;
+    // Counts a chunk of n records, which start at the old base; whether its columns are written.
+    bool add(uint32_t n) { short_ |= base + n > cap; base += n; return !short_; }
+};
+
+// A device→host copy to one of the caller's columns that goes with a chunk besides its offsets and per-record column:
+// per record (made only when the chunk's records are written) or always (a per-connection column).  No dst: none.
+struct ColCopy { void* dst; const void* src; size_t bytes; bool per_record; };
+
 // A packed output of a host-batch call: the caller's bytes, their offsets and the one per-record column egress carries
-// (meta, or log_req).  Output k (0: responses or proto rows, 1: request-log lines) owns d_chain[k], h_status[2k..],
-// d_info[k * kSlots ..], each slot's overflow word d_flag[k] and h_ends[4 ci + 2k ..].  Pinned buffers are filled by
-// advance and egress without the host waiting (deliver), pageable ones get each chunk's exact bytes (retire).  Both skip a
-// chunk's bytes when the device overflowed or when they would pass cap or 4 GiB (32-bit offsets): the batch then fails.
+// (meta, or log_req), and its record count.  Output k (0: responses or proto rows, 1: request-log lines) owns d_chain[k],
+// h_status[2k..], d_info[k * kSlots ..], each slot's overflow word d_flag[k] and its read-back h_tail[2k + 1], and
+// h_ends[4 j + 2k ..] for its j-th shipped chunk.  Pinned buffers are filled by advance and egress without the host
+// waiting (deliver), pageable ones get each chunk's exact bytes (retire).  Both skip a chunk's bytes when the device
+// overflowed or when they would pass cap or 4 GiB (32-bit offsets): the batch then fails.
 struct PackedOut {
     uint8_t* out = nullptr;
     uint64_t cap = 0;
@@ -924,19 +939,16 @@ struct PackedOut {
     uint32_t* col = nullptr;
     int k = 0;
     bool pinned = false;
+    RecCount recs;
     uint64_t written = 0, at = 0;  // bytes written (pinned: after finish); pageable: where the last retired chunk went
     bool overflow = false;         // some chunk's bytes were skipped (pinned: after finish)
+    size_t shipped = 0;            // chunks through ship
 
     PackedOut() = default;
-    PackedOut(uint8_t* o, uint64_t c, uint32_t* f, uint32_t* m, int k_)
-        : out(o), cap(c), off(f), col(m), k(k_), pinned(device_visible(o) && device_visible(f) && device_visible(m)) {}
+    PackedOut(uint8_t* o, uint64_t c, uint32_t* f, uint32_t* m, uint64_t rec_cap, int k_)
+        : out(o), cap(c), off(f), col(m), k(k_), pinned(device_visible(o) && device_visible(f) && device_visible(m)), recs{rec_cap} {}
     unsigned long long* chain(gofr_engine* e) const { return pinned ? e->d_chain + k : nullptr; }
-    uint32_t* ends(gofr_engine* e, size_t ci) const { return e->h_ends + 4 * ci + 2 * k; }  // chunk ci's first, end offset
-    uint64_t needed(gofr_engine* e, size_t chunks) const {
-        uint64_t b = 0;
-        for (size_t ci = 0; ci < chunks; ci++) b += ends(e, ci)[1] - ends(e, ci)[0];
-        return b;
-    }
+    uint32_t* h_flag(Slot& s) const { return s.h_tail + 2 * k + 1; }
     int start(gofr_engine* e) {
         if (!pinned) return GOFR_OK;
         CUDA_TRY(cudaMemsetAsync(e->d_chain + k, 0, 8, e->st_compute));
@@ -973,6 +985,62 @@ struct PackedOut {
         return GOFR_OK;
     }
     void rebase(uint64_t first, uint32_t n) const { if (at) for (uint64_t i = first; i < first + n; i++) off[i] += (uint32_t)at; }
+    // Hands chunk ci's n records to the caller after the kernels on st_compute that left them in d_out / d_off (at
+    // *chain(e) & 15 when pinned, at 0 otherwise) and d_col, with the caller's copies.  The chunk's first and end offsets
+    // come back to h_ends, so that a batch short of cap still reports what it needed.  Pinned: deliver, the copies on
+    // st_egress behind the egress, then s.ev_egress.  Pageable: the overflow word and the chunk's size first, then exactly
+    // its bytes, its offsets and column and the copies on st_compute, then its offsets rebased.
+    int ship(gofr_engine* e, Slot& s, size_t ci, const uint8_t* d_out, const uint32_t* d_off, const uint32_t* d_col, uint32_t n,
+             std::initializer_list<ColCopy> copies) {
+        const uint64_t first = recs.base;
+        const bool put = recs.add(n) && n;
+        cudaStream_t st = e->st_compute;
+        uint32_t* ends = e->h_ends + 4 * shipped++ + 2 * k;
+        ends[0] = ends[1] = 0;
+        if (n) {
+            CUDA_TRY(cudaMemcpyAsync(&ends[0], d_off, 4, cudaMemcpyDeviceToHost, st));
+            CUDA_TRY(cudaMemcpyAsync(&ends[1], d_off + n, 4, cudaMemcpyDeviceToHost, st));
+        }
+        bool wrote = put;
+        if (pinned) {
+            int rc = deliver(e, s, ci, d_out, d_off, d_col, n, first, put);
+            if (rc) return rc;
+            st = e->st_egress;
+        } else {
+            CUDA_TRY(cudaMemcpyAsync(h_flag(s), s.d_flag + k, 4, cudaMemcpyDeviceToHost, st));
+            CUDA_TRY(cudaStreamSynchronize(st));
+            int rc = retire(s, d_out, ends[1], *h_flag(s), put, st, &wrote);
+            if (rc) return rc;
+            if (wrote) {
+                CUDA_TRY(cudaMemcpyAsync(off + first, d_off, (size_t)n * 4, cudaMemcpyDeviceToHost, st));
+                CUDA_TRY(cudaMemcpyAsync(col + first, d_col, (size_t)n * 4, cudaMemcpyDeviceToHost, st));
+            }
+        }
+        for (const ColCopy& c : copies)
+            if (c.dst && (wrote || !c.per_record)) CUDA_TRY(cudaMemcpyAsync(c.dst, c.src, c.bytes, cudaMemcpyDeviceToHost, st));
+        if (pinned) {
+            CUDA_TRY(cudaEventRecord(s.ev_egress, st));
+            s.egress_pending = true;
+        } else {
+            CUDA_TRY(cudaStreamSynchronize(st));
+            if (wrote) rebase(first, n);
+        }
+        return GOFR_OK;
+    }
+    // The end of a shipped batch, after finish: *bytes receives the bytes its chunks needed.  The closing offset
+    // off[recs.base] is stored when every chunk was written; otherwise the error is fmt with the records, the bytes, the
+    // record capacity and cap (all unsigned long long), and the result GOFR_ERR_CAPACITY.
+    int report(gofr_engine* e, uint64_t* bytes, const char* fmt) const {
+        uint64_t b = 0;
+        for (size_t j = 0; j < shipped; j++) b += e->h_ends[4 * j + 2 * k + 1] - e->h_ends[4 * j + 2 * k];
+        *bytes = b;
+        if (recs.short_ || overflow) {
+            set_last_error(fmt, (unsigned long long)recs.base, (unsigned long long)b, (unsigned long long)recs.cap, (unsigned long long)cap);
+            return GOFR_ERR_CAPACITY;
+        }
+        off[recs.base] = (uint32_t)written;
+        return GOFR_OK;
+    }
     // Reads the pinned outputs' chain words back behind their egress and waits for it once.
     static int finish(gofr_engine* e, uint32_t n, std::initializer_list<PackedOut*> outs) {
         bool wait = false;
@@ -1010,7 +1078,7 @@ static int run_chunks(gofr_engine* e, uint32_t n, const ChunkSteps& steps, gofr_
         complete(e, ticket, GOFR_OK);
         return GOFR_OK;
     }
-    PackedOut o(out->out, out->out_cap, out->out_off, out->meta, 0);
+    PackedOut o(out->out, out->out_cap, out->out_off, out->meta, n, 0);
     { int rc = o.start(e); if (rc) return rc; }
     if (o.pinned) {  // ---- streaming path: egress is device driven, the host never blocks mid-batch ----
         size_t ci = 0;
@@ -1052,7 +1120,7 @@ static int run_chunks(gofr_engine* e, uint32_t n, const ChunkSteps& steps, gofr_
                 CUDA_TRY(cudaMemcpyAsync(out->out_off + c.lo, s.d_off, (size_t)cn * 4, cudaMemcpyDeviceToHost, s.stream));
                 CUDA_TRY(cudaMemcpyAsync(out->meta + c.lo, s.d_meta, (size_t)cn * 4, cudaMemcpyDeviceToHost, s.stream));
                 CUDA_TRY(cudaMemcpyAsync(&s.h_tail[0], s.d_off + cn, 4, cudaMemcpyDeviceToHost, s.stream));
-                CUDA_TRY(cudaMemcpyAsync(&s.h_tail[1], s.d_flag, 4, cudaMemcpyDeviceToHost, s.stream));
+                CUDA_TRY(cudaMemcpyAsync(o.h_flag(s), s.d_flag, 4, cudaMemcpyDeviceToHost, s.stream));
                 CUDA_TRY(cudaEventRecord(s.done, s.stream));
                 issued++;
             }
@@ -1061,7 +1129,7 @@ static int run_chunks(gofr_engine* e, uint32_t n, const ChunkSteps& steps, gofr_
             const ChunkPlan& c = inflight[finished % kSlots];
             CUDA_TRY(cudaEventSynchronize(s.done));
             bool wrote = false;
-            { int rc = o.retire(s, s.d_out, s.h_tail[0], s.h_tail[1], true, s.stream, &wrote); if (rc) return rc; }
+            { int rc = o.retire(s, s.d_out, s.h_tail[0], *o.h_flag(s), true, s.stream, &wrote); if (rc) return rc; }
             if (wrote) o.rebase(c.lo, c.hi - c.lo);  // while the copy runs
             CUDA_TRY(cudaStreamSynchronize(s.stream));
             finished++;
@@ -1181,6 +1249,21 @@ struct ConnChunk { uint32_t lo, hi, alo, rec_cap, rlo, rhi, remote_max; };
 // bytes, the id, a response_time of 20 characters and a status of 5 digits take 264 bytes.
 static constexpr uint64_t kConnLogFrame = 320;
 
+// The rule of the caller's offset columns: off[i + 1] is not below off[i] and not past limit, for i in [i0, i1).
+static int check_offsets(const char* what, const uint32_t* off, uint64_t i0, uint64_t i1, uint64_t limit) {
+    for (uint64_t i = i0; i < i1; i++)
+        if (off[i + 1] < off[i] || off[i + 1] > limit) {
+            set_last_error("%s[%llu] decreases or passes %llu", what, (unsigned long long)(i + 1), (unsigned long long)limit);
+            return GOFR_ERR_INVALID;
+        }
+    return GOFR_OK;
+}
+
+// The rule of gofr_conn_log's remote offsets, checked at connection c: its remote string is at most 255 bytes long.
+static int check_remote(const uint32_t* remote_off, uint32_t c) {
+    return check_offsets("remote_off", remote_off, c, c + 1, (uint64_t)remote_off[c] + 255u);
+}
+
 // The chunk that starts at connection lo: at most e->chunk connections whose bytes fit kConnChunkBudget, at least one.  The
 // offsets are validated here, chunk by chunk, and with logging the remote offsets too.
 static int conn_plan(const gofr_engine* e, const gofr_conn_batch* in, const gofr_conn_log* log, uint32_t lo, ConnChunk* c) {
@@ -1188,16 +1271,10 @@ static int conn_plan(const gofr_engine* e, const gofr_conn_batch* in, const gofr
     const uint32_t* ro = log ? log->remote_off : nullptr;
     uint32_t hi = lo, rmax = 0;
     while (hi < in->n_conns && hi - lo < e->chunk) {
-        if (o[hi + 1] < o[hi] || o[hi + 1] > in->buf_bytes) {
-            set_last_error("buf_off[%u] decreases or passes buf_bytes", hi + 1);
-            return GOFR_ERR_INVALID;
-        }
+        if (int rc = check_offsets("buf_off", o, hi, hi + 1, in->buf_bytes)) return rc;
         if (hi > lo && o[hi + 1] - o[lo] > kConnChunkBudget) break;
         if (ro) {
-            if (ro[hi + 1] < ro[hi] || ro[hi + 1] - ro[hi] > 255u) {
-                set_last_error("remote_off[%u] decreases or ends a remote string longer than 255 bytes", hi + 1);
-                return GOFR_ERR_INVALID;
-            }
+            if (int rc = check_remote(ro, hi)) return rc;
             rmax = std::max(rmax, ro[hi + 1] - ro[hi]);
         }
         hi++;
@@ -1246,24 +1323,13 @@ static int conn_frame(gofr_engine* e, const gofr_conn_batch* in, uint32_t* consu
     return GOFR_OK;
 }
 
-// The state of a connection batch between its chunks
-struct ConnRun {
-    bool req_short = false;     // req_cap was too small for a chunk: no per-request column is written from there on
-    uint64_t req_base = 0;      // requests of the chunks before
-    // the request-log lines (gofr_conn_batch_submit_log), the same per line
-    bool lines_short = false;
-    uint64_t line_base = 0;
-};
-
 // The request-log lines of chunk ci, after its serve kernel: the gather (conn_log_kernel.cu), then the existing reqlog_kernel
-// and chunk_pack_kernel, then the caller's columns through the lines' PackedOut (output 1).  The reqlog and pack kernels
-// take the chunk's line count from the host: it is read back after the gather.  The log kernels report overflow in their
-// own flag word, so that the responses' advance never sees it.
+// and chunk_pack_kernel, then the lines' PackedOut (output 1).  The reqlog and pack kernels take the chunk's line count
+// from the host: it is read back after the gather.  The log kernels report overflow in their own flag word, so that the
+// responses' advance never sees it.  The chunk's requests are batch requests [req0, req0 + n_req).
 static int conn_log_chunk(gofr_engine* e, const gofr_conn_batch* in, const gofr_conn_log* log, Slot& s, size_t ci,
-                          const ConnChunk& c, ConnRun& r, PackedOut& lo, uint32_t n_req) {
+                          const ConnChunk& c, PackedOut& lo, uint64_t req0, uint32_t n_req) {
     cudaStream_t st = e->st_compute;
-    uint32_t* ends = lo.ends(e, ci);  // the chunk's first and end line offsets: what it needs of out_cap
-    ends[0] = ends[1] = 0;
     if (!n_req) return GOFR_OK;
     const uint32_t cn = c.hi - c.lo, bytes = in->buf_off[c.hi] - c.alo;
     uint32_t* flag = s.d_flag + 1;
@@ -1276,7 +1342,7 @@ static int conn_log_chunk(gofr_engine* e, const gofr_conn_batch* in, const gofr_
     g.first = s.d_first; g.conn_status = s.d_cstatus; g.req_first = s.d_req_first; g.rec_off = s.d_rec; g.spans = s.d_spans;
     g.meta = s.d_meta; g.ids = (const uint8_t*)s.d_ids; g.buf = s.d_buf - c.alo; g.remote = s.d_remote - c.rlo;
     g.remote_off = s.d_remote_off; g.start_ns = s.d_start; g.log_ns = log->log_unix_ns; g.tz_offset_s = log->tz_offset_s;
-    g.alo = c.alo; g.remote_max = c.remote_max; g.req0 = (uint32_t)r.req_base;
+    g.alo = c.alo; g.remote_max = c.remote_max; g.req0 = (uint32_t)req0;
     g.line_ids = s.d_lids; g.line_req = s.d_lreq; g.arena = s.d_larena;
     rc = launch_frames_locked(e, K_CONN_LOG, 0, g, cn, (uint8_t*)s.d_ldesc, n_req, s.d_lfirst, s.state, flag, st);
     if (rc) return rc;
@@ -1300,31 +1366,7 @@ static int conn_log_chunk(gofr_engine* e, const gofr_conn_batch* in, const gofr_
     memset(&q, 0, sizeof q);
     q.a = s.d_lraw; q.a_off = s.d_lraw_off; q.a_cap = s.cap_lraw - 16; q.chain_pos = lo.chain(e);
     rc = launch_frames_locked(e, K_PACK, 0, q, lines, s.d_lout, s.cap_lout, s.d_loff, s.state, flag, st);
-    if (rc) return rc;
-    CUDA_TRY(cudaMemcpyAsync(&ends[0], s.d_loff, 4, cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaMemcpyAsync(&ends[1], s.d_loff + lines, 4, cudaMemcpyDeviceToHost, st));
-    if (r.line_base + lines > log->line_cap) r.lines_short = true;
-    const bool put = !r.lines_short;
-    if (lo.pinned) {
-        rc = lo.deliver(e, s, ci, s.d_lout, s.d_loff, s.d_lreq, lines, r.line_base, put);
-        if (rc) return rc;
-        CUDA_TRY(cudaEventRecord(s.ev_egress, e->st_egress));
-        s.egress_pending = true;
-    } else {  // pageable: the chunk's exact size first, then exactly that many bytes
-        CUDA_TRY(cudaMemcpyAsync(&s.h_tail[3], flag, 4, cudaMemcpyDeviceToHost, st));
-        CUDA_TRY(cudaStreamSynchronize(st));
-        bool wrote = false;
-        rc = lo.retire(s, s.d_lout, ends[1], s.h_tail[3], put, st, &wrote);
-        if (rc) return rc;
-        if (wrote) {
-            CUDA_TRY(cudaMemcpyAsync(log->log_off + r.line_base, s.d_loff, (size_t)lines * 4, cudaMemcpyDeviceToHost, st));
-            CUDA_TRY(cudaMemcpyAsync(log->log_req + r.line_base, s.d_lreq, (size_t)lines * 4, cudaMemcpyDeviceToHost, st));
-            CUDA_TRY(cudaStreamSynchronize(st));
-            lo.rebase(r.line_base, lines);
-        }
-    }
-    r.line_base += lines;
-    return GOFR_OK;
+    return rc ? rc : lo.ship(e, s, ci, s.d_lout, s.d_loff, s.d_lreq, lines, {});
 }
 
 // The chunk's framing is back: parse its records and compact its whole requests into s.d_desc, s.d_req_at, s.d_ids and
@@ -1366,12 +1408,8 @@ static int conn_splice_chunk(gofr_engine* e, const gofr_conn_batch* in, const go
         return GOFR_ERR_INVALID;
     }
     if (!n_req) return GOFR_OK;
+    if (int rc = check_offsets("rec_off", res->rec_off, req_base, req_base + n_req, res->rec_bytes)) return rc;
     const uint32_t* ro = res->rec_off + req_base;
-    for (uint32_t k = 0; k < n_req; k++)
-        if (ro[k + 1] < ro[k] || ro[k + 1] > res->rec_bytes) {
-            set_last_error("rec_off[%llu] decreases or passes rec_bytes", (unsigned long long)(req_base + k + 1));
-            return GOFR_ERR_INVALID;
-        }
     // the spliced arena is addressed with 32-bit offsets: each request takes its path, query and data section plus two pads
     // of at most 3 bytes, and its path, query and body are never longer than its message
     const uint32_t rlo = ro[0] & ~15u, rhi = ro[n_req], bytes = in->buf_off[c.hi] - c.alo;
@@ -1403,64 +1441,47 @@ static int conn_splice_chunk(gofr_engine* e, const gofr_conn_batch* in, const go
 // Second half of chunk ci: parse its records, compact the whole requests, splice the closures' results in (res not null),
 // serve them, and send the results to the caller's columns.
 static int conn_serve(gofr_engine* e, const gofr_conn_batch* in, const gofr_conn_results* res, gofr_conn_resp* out,
-                      const gofr_conn_log* log, Slot& s, size_t ci, const ConnChunk& c, ConnRun& r, PackedOut& ro, PackedOut& lo) {
-    const uint32_t cn = c.hi - c.lo;
+                      const gofr_conn_log* log, Slot& s, size_t ci, const ConnChunk& c, PackedOut& ro, PackedOut& lo) {
+    const uint64_t req0 = ro.recs.base;
     uint32_t n_req = 0;
-    int rc = conn_parse(e, in, out->conn_status, s, c, (uint32_t)r.req_base, &n_req);
+    int rc = conn_parse(e, in, out->conn_status, s, c, (uint32_t)req0, &n_req);
     if (rc) return rc;
-    cudaStream_t st = e->st_compute;
     const uint8_t* d_arena = s.d_arena - c.alo;
-    if (res && (rc = conn_splice_chunk(e, in, res, s, c, r.req_base, n_req, &d_arena)) != 0) return rc;
-    if (r.req_base + n_req > out->req_cap) r.req_short = true;
-    const bool put = !r.req_short && n_req;  // this chunk's per-request columns go to the caller
-    uint32_t* ends = ro.ends(e, ci);         // the chunk's first and end response offsets: what it needs of out_cap
-    ends[0] = ends[1] = 0;
-    if (n_req) {
-        rc = launch_serve(e, s.d_desc, s.d_ids, d_arena, n_req, in->date, s.d_out, s.cap_out, s.d_off, s.d_meta, &s.state,
-                          s.d_flag, s.d_bind, st, ro.chain(e));
-        if (rc) return rc;
-        CUDA_TRY(cudaMemcpyAsync(&ends[0], s.d_off, 4, cudaMemcpyDeviceToHost, st));
-        CUDA_TRY(cudaMemcpyAsync(&ends[1], s.d_off + n_req, 4, cudaMemcpyDeviceToHost, st));
-    }
-    // the per-request columns go next to the responses: behind the egress when pinned, behind their bytes when pageable
-    bool wrote = put;
-    cudaStream_t cs = e->st_egress;
-    if (ro.pinned) {
-        rc = ro.deliver(e, s, ci, s.d_out, s.d_off, s.d_meta, n_req, r.req_base, put);
-        if (rc) return rc;
-    } else {  // pageable: the chunk's exact size first, then exactly that many bytes
-        cs = st;
-        CUDA_TRY(cudaMemcpyAsync(&s.h_tail[1], s.d_flag, 4, cudaMemcpyDeviceToHost, st));
-        CUDA_TRY(cudaStreamSynchronize(st));
-        rc = ro.retire(s, s.d_out, ends[1], s.h_tail[1], put, st, &wrote);
-        if (rc) return rc;
-        if (wrote) {
-            CUDA_TRY(cudaMemcpyAsync(out->out_off + r.req_base, s.d_off, (size_t)n_req * 4, cudaMemcpyDeviceToHost, st));
-            CUDA_TRY(cudaMemcpyAsync(out->meta + r.req_base, s.d_meta, (size_t)n_req * 4, cudaMemcpyDeviceToHost, st));
+    if (res && (rc = conn_splice_chunk(e, in, res, s, c, req0, n_req, &d_arena)) != 0) return rc;
+    if (n_req && (rc = launch_serve(e, s.d_desc, s.d_ids, d_arena, n_req, in->date, s.d_out, s.cap_out, s.d_off, s.d_meta,
+                                    &s.state, s.d_flag, s.d_bind, e->st_compute, ro.chain(e))) != 0) return rc;
+    rc = ro.ship(e, s, ci, s.d_out, s.d_off, s.d_meta, n_req,
+                 {{out->req_at + req0, s.d_req_at, (size_t)n_req * 4, true},
+                  {out->trace_ids ? out->trace_ids + req0 * 16 : nullptr, s.d_ids, (size_t)n_req * 16, true},
+                  {out->req_first + c.lo, s.d_req_first, (size_t)(c.hi - c.lo) * 4, false}});
+    if (!rc && log) rc = conn_log_chunk(e, in, log, s, ci, c, lo, req0, n_req);
+    return rc;
+}
+
+// The chunks of a connection batch in order, one framed ahead of the one being stepped: the host learns a chunk's record
+// count while the next chunk's bytes are on their way.  step(s, ci, c) finishes chunk ci, framed in slot s.
+using ConnStep = std::function<int(Slot& s, size_t ci, const ConnChunk& c)>;
+static int conn_chunks(gofr_engine* e, const gofr_conn_batch* in, uint32_t* consumed, uint32_t* conn_status, const gofr_conn_log* log,
+                       const ConnStep& step) {
+    const uint32_t n = in->n_conns;
+    ConnChunk chunks[kSlots];
+    size_t issued = 0, stepped = 0;
+    for (uint32_t next = 0; next < n || stepped < issued;) {
+        while (next < n && issued < stepped + 2) {
+            ConnChunk& c = chunks[issued % kSlots];
+            int rc = conn_plan(e, in, log, next, &c);
+            if (!rc) rc = conn_frame(e, in, consumed, conn_status, log, e->slots[issued % kSlots], c);
+            if (rc) return rc;
+            next = c.hi;
+            issued++;
         }
-    }
-    if (wrote) {
-        CUDA_TRY(cudaMemcpyAsync(out->req_at + r.req_base, s.d_req_at, (size_t)n_req * 4, cudaMemcpyDeviceToHost, cs));
-        if (out->trace_ids) CUDA_TRY(cudaMemcpyAsync(out->trace_ids + r.req_base * 16, s.d_ids, (size_t)n_req * 16, cudaMemcpyDeviceToHost, cs));
-    }
-    CUDA_TRY(cudaMemcpyAsync(out->req_first + c.lo, s.d_req_first, (size_t)cn * 4, cudaMemcpyDeviceToHost, cs));
-    if (ro.pinned) {
-        CUDA_TRY(cudaEventRecord(s.ev_egress, cs));
-        s.egress_pending = true;
-    } else {
-        CUDA_TRY(cudaStreamSynchronize(st));
-        if (wrote) ro.rebase(r.req_base, n_req);
-    }
-    if (log) {
-        const int rc = conn_log_chunk(e, in, log, s, ci, c, r, lo, n_req);
+        int rc = step(e->slots[stepped % kSlots], stepped, chunks[stepped % kSlots]);
         if (rc) return rc;
+        stepped++;
     }
-    r.req_base += n_req;
     return GOFR_OK;
 }
 
-// The chunks of a connection batch, one framed ahead of the one being served: the host learns a chunk's record count while
-// the next chunk's bytes are on their way.
 static int conn_batch_locked(gofr_engine* e, const gofr_conn_batch* in, const gofr_conn_results* res, gofr_conn_resp* out,
                              gofr_conn_log* log, gofr_ticket* ticket) {
     const uint32_t n = in->n_conns;
@@ -1479,52 +1500,24 @@ static int conn_batch_locked(gofr_engine* e, const gofr_conn_batch* in, const go
         CUDA_TRY(cudaMallocHost(&e->h_ends, 4 * max_chunks * 4));
         e->ends_cap = 4 * max_chunks;
     }
-    ConnRun r;
-    PackedOut ro(out->out, out->out_cap, out->out_off, out->meta, 0), lo;
+    PackedOut ro(out->out, out->out_cap, out->out_off, out->meta, out->req_cap, 0), lo;
     { int rc = ro.start(e); if (rc) return rc; }
     if (log) {
-        lo = PackedOut(log->out, log->out_cap, log->log_off, log->log_req, 1);
+        lo = PackedOut(log->out, log->out_cap, log->log_off, log->log_req, log->line_cap, 1);
         int rc = lo.start(e);
         if (rc) return rc;
     }
-    ConnChunk chunks[kSlots];
-    size_t issued = 0, served = 0;
-    for (uint32_t next = 0; next < n || served < issued;) {
-        while (next < n && issued < served + 2) {
-            ConnChunk& c = chunks[issued % kSlots];
-            int rc = conn_plan(e, in, log, next, &c);
-            if (!rc) rc = conn_frame(e, in, out->consumed, out->conn_status, log, e->slots[issued % kSlots], c);
-            if (rc) return rc;
-            next = c.hi;
-            issued++;
-        }
-        int rc = conn_serve(e, in, res, out, log, e->slots[served % kSlots], served, chunks[served % kSlots], r, ro, lo);
-        if (rc) return rc;
-        served++;
-    }
-    { int rc = PackedOut::finish(e, n, {&ro, &lo}); if (rc) return rc; }
-    const uint64_t need = ro.needed(e, served);
-    out->req_first[n] = (uint32_t)r.req_base;
-    out->out_bytes = need;
-    int final_rc = GOFR_OK;
-    if (r.req_short || ro.overflow) {
-        final_rc = GOFR_ERR_CAPACITY;
-        set_last_error("the batch needs %llu requests and %llu response bytes: req_cap %u, out_cap %llu", (unsigned long long)r.req_base,
-                       (unsigned long long)need, out->req_cap, (unsigned long long)out->out_cap);
-    } else {
-        out->out_off[r.req_base] = (uint32_t)ro.written;
-    }
+    int rc = conn_chunks(e, in, out->consumed, out->conn_status, log, [&](Slot& s, size_t ci, const ConnChunk& c) {
+        return conn_serve(e, in, res, out, log, s, ci, c, ro, lo);
+    });
+    if (!rc) rc = PackedOut::finish(e, n, {&ro, &lo});
+    if (rc) return rc;
+    out->req_first[n] = (uint32_t)ro.recs.base;
+    int final_rc = ro.report(e, &out->out_bytes, "the batch needs %llu requests and %llu response bytes: req_cap %llu, out_cap %llu");
     if (log) {
-        const uint64_t lneed = lo.needed(e, served);
-        log->lines = (uint32_t)r.line_base;
-        log->out_bytes = lneed;
-        if (r.lines_short || lo.overflow) {
-            final_rc = GOFR_ERR_CAPACITY;
-            set_last_error("the batch needs %llu log lines and %llu log bytes: line_cap %u, out_cap %llu", (unsigned long long)r.line_base,
-                           (unsigned long long)lneed, log->line_cap, (unsigned long long)log->out_cap);
-        } else {
-            log->log_off[r.line_base] = (uint32_t)lo.written;
-        }
+        log->lines = (uint32_t)lo.recs.base;
+        rc = lo.report(e, &log->out_bytes, "the batch needs %llu log lines and %llu log bytes: line_cap %llu, out_cap %llu");
+        if (rc) final_rc = rc;
     }
     complete(e, ticket, final_rc);
     return GOFR_OK;
@@ -1549,45 +1542,39 @@ int gofr_conn_batch_respond(gofr_engine* e, const gofr_conn_batch* in, const gof
     return host_batch(e, [&] { return conn_batch_locked(e, in, res, out, log, ticket); });
 }
 
-// Stage 1 of the closure path (gofr_conn_batch_route): chunk after chunk, synchronously — frame, parse and compact as the
-// connection pipeline does, route the compacted requests, and bring the chunk's columns and its parse-arena bytes back.
-// A request's parsed form lies inside its own message (include/gofr_b200.h), so a chunk's arena bytes are exactly its
-// connections' byte range, copied to the same offsets of the caller's arena.
+// Stage 1 of the closure path (gofr_conn_batch_route), synchronous: the connection chunks of conn_chunks, each framed,
+// parsed and compacted as the connection pipeline does, its requests routed, and its columns and parse-arena bytes
+// brought back before the next one is stepped.  A request's parsed form lies inside its own message (include/gofr_b200.h),
+// so a chunk's arena bytes are exactly its connections' byte range, copied to the same offsets of the caller's arena.
 static int conn_route_locked(gofr_engine* e, const gofr_conn_batch* in, gofr_conn_route* out) {
-    const uint32_t n = in->n_conns;
     const cudaStream_t st = e->st_compute;
-    Slot& s = e->slots[0];
-    uint64_t req_base = 0;
-    bool req_short = false;
-    for (uint32_t lo = 0; lo < n;) {
-        ConnChunk c;
+    RecCount r{out->req_cap};
+    int rc = conn_chunks(e, in, out->consumed, out->conn_status, nullptr, [&](Slot& s, size_t, const ConnChunk& c) -> int {
+        const uint64_t req0 = r.base;
         uint32_t n_req = 0;
-        int rc = conn_plan(e, in, nullptr, lo, &c);
-        if (!rc) rc = conn_frame(e, in, out->consumed, out->conn_status, nullptr, s, c);
-        if (!rc) rc = conn_parse(e, in, out->conn_status, s, c, (uint32_t)req_base, &n_req);
+        int rc = conn_parse(e, in, out->conn_status, s, c, (uint32_t)req0, &n_req);
         if (rc) return rc;
-        if (req_base + n_req > out->req_cap) req_short = true;
-        if (!req_short && n_req) {
+        if (r.add(n_req) && n_req) {
             const size_t vbytes = (size_t)n_req * 4 * GOFR_MAX_PATH_VARS;
             rc = grow((void**)&s.d_vars, &s.cap_vars, vbytes, 256);
             if (!rc) rc = launch_route_kernel(e, s.d_desc, s.d_arena - c.alo, n_req, s.d_meta, s.d_vars, st);
             if (rc) return rc;
             const uint32_t a0 = in->buf_off[c.lo], a1 = in->buf_off[c.hi];
-            CUDA_TRY(cudaMemcpyAsync(out->desc + req_base, s.d_desc, (size_t)n_req * 16, cudaMemcpyDeviceToHost, st));
-            CUDA_TRY(cudaMemcpyAsync(out->meta + req_base, s.d_meta, (size_t)n_req * 4, cudaMemcpyDeviceToHost, st));
-            CUDA_TRY(cudaMemcpyAsync(out->vars + req_base * GOFR_MAX_PATH_VARS, s.d_vars, vbytes, cudaMemcpyDeviceToHost, st));
-            CUDA_TRY(cudaMemcpyAsync(out->req_at + req_base, s.d_req_at, (size_t)n_req * 4, cudaMemcpyDeviceToHost, st));
-            CUDA_TRY(cudaMemcpyAsync(out->trace_ids + req_base * 16, s.d_ids, (size_t)n_req * 16, cudaMemcpyDeviceToHost, st));
+            CUDA_TRY(cudaMemcpyAsync(out->desc + req0, s.d_desc, (size_t)n_req * 16, cudaMemcpyDeviceToHost, st));
+            CUDA_TRY(cudaMemcpyAsync(out->meta + req0, s.d_meta, (size_t)n_req * 4, cudaMemcpyDeviceToHost, st));
+            CUDA_TRY(cudaMemcpyAsync(out->vars + req0 * GOFR_MAX_PATH_VARS, s.d_vars, vbytes, cudaMemcpyDeviceToHost, st));
+            CUDA_TRY(cudaMemcpyAsync(out->req_at + req0, s.d_req_at, (size_t)n_req * 4, cudaMemcpyDeviceToHost, st));
+            CUDA_TRY(cudaMemcpyAsync(out->trace_ids + req0 * 16, s.d_ids, (size_t)n_req * 16, cudaMemcpyDeviceToHost, st));
             CUDA_TRY(cudaMemcpyAsync(out->arena + a0, s.d_arena + (a0 - c.alo), a1 - a0, cudaMemcpyDeviceToHost, st));
         }
         CUDA_TRY(cudaMemcpyAsync(out->req_first + c.lo, s.d_req_first, (size_t)(c.hi - c.lo) * 4, cudaMemcpyDeviceToHost, st));
         CUDA_TRY(cudaStreamSynchronize(st));
-        req_base += n_req;
-        lo = c.hi;
-    }
-    out->req_first[n] = (uint32_t)req_base;
-    if (req_short) {
-        set_last_error("the batch needs %llu requests: req_cap %u", (unsigned long long)req_base, out->req_cap);
+        return GOFR_OK;
+    });
+    if (rc) return rc;
+    out->req_first[in->n_conns] = (uint32_t)r.base;
+    if (r.short_) {
+        set_last_error("the batch needs %llu requests: req_cap %u", (unsigned long long)r.base, out->req_cap);
         return GOFR_ERR_CAPACITY;
     }
     return GOFR_OK;
@@ -1604,9 +1591,9 @@ int gofr_conn_batch_route(gofr_engine* e, const gofr_conn_batch* in, gofr_conn_r
 int gofr_conn_respond_bound(const gofr_table* t, const gofr_req_desc* desc, uint32_t n_req, const uint32_t* rec_off, uint64_t* out_cap) {
     if (!t || !out_cap || (n_req && (!desc || !rec_off))) return GOFR_ERR_INVALID;
     if (!gofr_table_response_bound(t, 0, 0, 0)) { set_last_error("the table is not sealed"); return GOFR_ERR_NOT_SEALED; }
+    if (int rc = check_offsets("rec_off", rec_off, 0, n_req, 0xFFFFFFFFull)) return rc;
     uint64_t b = 0;
     for (uint32_t k = 0; k < n_req; k++) {
-        if (rec_off[k + 1] < rec_off[k]) { set_last_error("rec_off[%u] decreases", k + 1); return GOFR_ERR_INVALID; }
         const uint32_t len = rec_off[k + 1] > rec_off[k] ? rec_off[k + 1] - rec_off[k] : desc[k].data_len;
         b += gofr_table_response_bound(t, desc[k].path_len, desc[k].query_len, len);
     }
@@ -1620,8 +1607,7 @@ int gofr_conn_batch_bound(const gofr_table* t, const uint32_t* buf_off, uint32_t
     if (!r0) { set_last_error("the table is not sealed"); return GOFR_ERR_NOT_SEALED; }
     // a response grows by at most this much per path, query or body byte of its request
     const uint64_t per_byte = std::max(gofr_table_response_bound(t, 1, 0, 0), gofr_table_response_bound(t, 0, 0, 1)) - r0;
-    for (uint32_t c = 0; c < n_conns; c++)
-        if (buf_off[c + 1] < buf_off[c]) { set_last_error("buf_off[%u] decreases", c + 1); return GOFR_ERR_INVALID; }
+    if (int rc = check_offsets("buf_off", buf_off, 0, n_conns, 0xFFFFFFFFull)) return rc;
     const uint64_t bytes = n_conns ? buf_off[n_conns] - buf_off[0] : 0, reqs = bytes / 16 + n_conns;
     *req_cap = (uint32_t)std::min<uint64_t>(reqs, 0xFFFFFFFFull);
     *out_cap = reqs * r0 + per_byte * bytes;
@@ -1630,13 +1616,10 @@ int gofr_conn_batch_bound(const gofr_table* t, const uint32_t* buf_off, uint32_t
 
 int gofr_conn_log_bound(const uint32_t* buf_off, const uint32_t* remote_off, uint32_t n_conns, uint32_t* line_cap, uint64_t* out_cap) {
     if (!line_cap || !out_cap || (n_conns && (!buf_off || !remote_off))) return GOFR_ERR_INVALID;
+    if (int rc = check_offsets("buf_off", buf_off, 0, n_conns, 0xFFFFFFFFull)) return rc;
     uint64_t reqs = 0, remote = 0;
     for (uint32_t c = 0; c < n_conns; c++) {
-        if (buf_off[c + 1] < buf_off[c]) { set_last_error("buf_off[%u] decreases", c + 1); return GOFR_ERR_INVALID; }
-        if (remote_off[c + 1] < remote_off[c] || remote_off[c + 1] - remote_off[c] > 255u) {
-            set_last_error("remote_off[%u] decreases or ends a remote string longer than 255 bytes", c + 1);
-            return GOFR_ERR_INVALID;
-        }
+        if (int rc = check_remote(remote_off, c)) return rc;
         const uint64_t r = (buf_off[c + 1] - buf_off[c]) / 16 + 1;  // the connection's requests at most
         reqs += r;
         remote += r * (remote_off[c + 1] - remote_off[c]);
