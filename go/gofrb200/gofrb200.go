@@ -817,3 +817,103 @@ func (p *ProtoFrontend) Call(in []byte) (out []byte, status uint32, err error) {
 	}
 	return buf[:n], uint32(st), nil
 }
+
+// ConnFrontend batches single reads from many connection goroutines through the connection pipeline
+// (gofr_conn_frontend_*): the per-connection loop of net/http's conn.serve (pkg/gofr/httpServer.go:29-33) hands in what it
+// holds for its connection and gets that connection's answers back, framed, parsed and served on the GPU together with
+// the other goroutines' reads.  Several front-ends of any kind may share one Engine.
+type ConnFrontend struct {
+	f            *C.gofr_conn_frontend
+	maxConnBytes int
+	log          bool
+}
+
+// ErrConnReadTooLarge is what ConnFrontend.Serve returns, before anything is queued, for a read longer than the
+// front-end's maxConnBytes: serve that connection with net/http.
+var ErrConnReadTooLarge = errors.New("gofrb200: read exceeds the front-end's maxConnBytes")
+
+// NewConnFrontend: maxBatch and maxWaitMicros mean what they mean for NewFrontend; a read longer than maxConnBytes is
+// refused (ErrConnReadTooLarge).  With log, Serve also returns middleware.Logging's lines, logged in a zone
+// tzOffsetSeconds east of UTC.  Batch b draws its trace ids from splitmix64(splitmix64(seed) + b).
+func NewConnFrontend(e *Engine, maxBatch, maxWaitMicros, maxConnBytes int, log bool, tzOffsetSeconds int32, seed uint64) (*ConnFrontend, error) {
+	l := C.int(0)
+	if log {
+		l = 1
+	}
+	var f *C.gofr_conn_frontend
+	if err := check(C.gofr_conn_frontend_create(&f, e.e, C.uint32_t(maxBatch), C.uint32_t(maxWaitMicros), C.uint32_t(maxConnBytes), l,
+		C.int32_t(tzOffsetSeconds), C.uint64_t(seed)), "gofr_conn_frontend_create"); err != nil {
+		return nil, err
+	}
+	return &ConnFrontend{f, maxConnBytes, log}, nil
+}
+
+// Close must not run while a Serve is in progress.
+func (f *ConnFrontend) Close() { C.gofr_conn_frontend_destroy(f.f); f.f = nil }
+
+// SetClock pins the Date header and the log time of every batch (tests); the zero Time restores the wall clock.
+func (f *ConnFrontend) SetClock(t time.Time) error {
+	ns := int64(0)
+	if !t.IsZero() {
+		ns = t.UnixNano()
+	}
+	return check(C.gofr_conn_frontend_set_clock(f.f, C.int64_t(ns)), "gofr_conn_frontend_set_clock")
+}
+
+// Stats returns the batches run, the reads they held, and the batches served again after their outputs grew.
+func (f *ConnFrontend) Stats() (batches, conns, reruns uint64, err error) {
+	var b, c, r C.uint64_t
+	err = check(C.gofr_conn_frontend_stats(f.f, &b, &c, &r), "gofr_conn_frontend_stats")
+	return uint64(b), uint64(c), uint64(r), err
+}
+
+// Serve blocks until the batch this read joined has been served and fills r as ServeConnections fills it for a batch of
+// one connection: size its slices with Table.ConnBound([]uint32{0, len(buf)}) (ReqFirst 2, Consumed and ConnStatus 1).
+// With r.Log set on a front-end created with log, its output fields (Out, LogOff, LogReq, sized with ConnLogBound) receive
+// the connection's lines; its input fields are not used: remote and start are this read's req.RemoteAddr and Logging's
+// start clock.  Returns the response bytes written.  Then write Out[:n], running the closures of the holes (status 0 in
+// Meta) from buf[ReqAt[k]:]; keep buf[Consumed[0]:] on HTTPConnMore, hand it to net/http on HTTPConnDefer.
+func (f *ConnFrontend) Serve(buf, remote []byte, start time.Time, r *ConnResponses) (uint64, error) {
+	if len(buf) > f.maxConnBytes {
+		return 0, ErrConnReadTooLarge
+	}
+	if len(r.Out) == 0 || len(r.Meta) == 0 || len(r.OutOff) < len(r.Meta)+1 || len(r.ReqAt) < len(r.Meta) ||
+		(r.TraceIDs != nil && len(r.TraceIDs) < 16*len(r.Meta)) || len(r.ReqFirst) < 2 || len(r.Consumed) < 1 || len(r.ConnStatus) < 1 {
+		return 0, errors.New("gofrb200: ConnResponses columns too small")
+	}
+	var o C.gofr_conn_resp
+	o.out = (*C.uint8_t)(unsafe.Pointer(&r.Out[0]))
+	o.out_cap = C.uint64_t(len(r.Out))
+	o.req_cap = C.uint32_t(len(r.Meta))
+	o.out_off = (*C.uint32_t)(unsafe.Pointer(&r.OutOff[0]))
+	o.meta = (*C.uint32_t)(unsafe.Pointer(&r.Meta[0]))
+	o.req_at = (*C.uint32_t)(unsafe.Pointer(&r.ReqAt[0]))
+	if r.TraceIDs != nil {
+		o.trace_ids = (*C.uint8_t)(unsafe.Pointer(&r.TraceIDs[0]))
+	}
+	o.req_first = (*C.uint32_t)(unsafe.Pointer(&r.ReqFirst[0]))
+	o.consumed = (*C.uint32_t)(unsafe.Pointer(&r.Consumed[0]))
+	o.conn_status = (*C.uint32_t)(unsafe.Pointer(&r.ConnStatus[0]))
+	var lg *C.gofr_conn_log
+	if l := r.Log; l != nil && f.log {
+		if len(l.Out) == 0 || len(l.LogReq) == 0 || len(l.LogOff) < len(l.LogReq)+1 {
+			return 0, errors.New("gofrb200: ConnLog columns too small")
+		}
+		lg = &C.gofr_conn_log{}
+		lg.line_cap = C.uint32_t(len(l.LogReq))
+		lg.out = (*C.uint8_t)(unsafe.Pointer(&l.Out[0]))
+		lg.out_cap = C.uint64_t(len(l.Out))
+		lg.log_off = (*C.uint32_t)(unsafe.Pointer(&l.LogOff[0]))
+		lg.log_req = (*C.uint32_t)(unsafe.Pointer(&l.LogReq[0]))
+	}
+	ns := int64(0)
+	if !start.IsZero() {
+		ns = start.UnixNano()
+	}
+	rc := C.gofr_conn_frontend_serve(f.f, bytesPtr(buf), C.uint32_t(len(buf)), bytesPtr(remote), C.uint32_t(len(remote)), C.int64_t(ns),
+		&o, lg)
+	if lg != nil {
+		r.Log.Lines, r.Log.OutBytes = uint32(lg.lines), uint64(lg.out_bytes)
+	}
+	return uint64(o.out_bytes), check(rc, "gofr_conn_frontend_serve")
+}

@@ -174,6 +174,12 @@ def lib():
     L.gofr_proto_frontend_destroy.restype = None
     L.gofr_proto_frontend_stats.argtypes = [vp, C.POINTER(u64), C.POINTER(u64)]
     L.gofr_proto_frontend_call.argtypes = [vp, C.c_char_p, u32, vp, u32, C.POINTER(u32), C.POINTER(u32)]
+    L.gofr_conn_frontend_create.argtypes = [C.POINTER(vp), vp, u32, u32, u32, i32, C.c_int32, u64]
+    L.gofr_conn_frontend_destroy.argtypes = [vp]
+    L.gofr_conn_frontend_destroy.restype = None
+    L.gofr_conn_frontend_set_clock.argtypes = [vp, C.c_int64]
+    L.gofr_conn_frontend_stats.argtypes = [vp, C.POINTER(u64), C.POINTER(u64), C.POINTER(u64)]
+    L.gofr_conn_frontend_serve.argtypes = [vp, C.c_char_p, u32, C.c_char_p, u32, C.c_int64, C.POINTER(ConnResp), C.POINTER(ConnLog)]
     L.gofr_http_parse_device.argtypes = [vp, vp, vp, u32, vp, vp, vp, vp, vp]
     L.gofr_http_frame_device.argtypes = [vp, vp, vp, u32, vp, u32, vp, vp, vp, vp]
     L.gofr_conn_batch_submit.argtypes = [vp, C.POINTER(ConnBatch), C.POINTER(ConnResp), C.POINTER(u64)]
@@ -205,6 +211,7 @@ DECLARED_SYMBOLS = [
     "gofr_engine_set_timing", "gofr_engine_overflowed", "gofr_engine_geometry", "gofr_engine_slot_ctas", "gofr_table_slot_ctas", "gofr_alloc_pinned", "gofr_free_pinned", "gofr_bind_host_thread", "gofr_bind_device", "gofr_batch_bind",
     "gofr_grpc_hello_device", "gofr_requestlog_device", "gofr_http_parse_device", "gofr_http_frame_device", "gofr_conn_batch_submit", "gofr_conn_batch_bound", "gofr_conn_batch_submit_log", "gofr_conn_log_bound", "gofr_conn_batch_route", "gofr_conn_batch_respond", "gofr_conn_respond_bound", "gofr_batch_route", "gofr_proto_encode_device", "gofr_proto_decode_device", "gofr_proto_encode_nested_device", "gofr_proto_decode_nested_device", "gofr_proto_nested_describe", "gofr_proto_encode_nested_ex_device", "gofr_proto_decode_nested_ex_device", "gofr_proto_nested_describe_ex", "gofr_proto_decode_nested_deferred_device", "gofr_proto_batch_decode", "gofr_proto_batch_encode", "gofr_proto_nested_bound", "gofr_table_response_bound", "gofr_frontend_create", "gofr_frontend_destroy", "gofr_frontend_set_clock",
     "gofr_frontend_stats", "gofr_frontend_serve", "gofr_proto_frontend_create", "gofr_proto_frontend_destroy",
-    "gofr_proto_frontend_stats", "gofr_proto_frontend_call", "gofr_route_device", "gofr_engine_launch_count", "gofr_engine_kernel_time_ms", "gofr_last_error",
+    "gofr_proto_frontend_stats", "gofr_proto_frontend_call", "gofr_conn_frontend_create", "gofr_conn_frontend_destroy",
+    "gofr_conn_frontend_set_clock", "gofr_conn_frontend_stats", "gofr_conn_frontend_serve", "gofr_route_device", "gofr_engine_launch_count", "gofr_engine_kernel_time_ms", "gofr_last_error",
     "gofr_abi_version", "gofr_format_http_date",
 ]

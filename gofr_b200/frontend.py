@@ -3,16 +3,20 @@
 The reference serves one request per goroutine (net/http conn.serve → Router.ServeHTTP, pkg/gofr/httpServer.go:29-33);
 `Frontend.serve` is that per-request call (gofr_frontend_*): it blocks until the batch the request joined has come back.
 grpc-go calls its codec once per message; `ProtoFrontend.call` is that call for the nested proto3 codec
-(gofr_proto_frontend_*).  ctypes drops the GIL for the duration of a call, so Python threads can stand in for goroutines.
+(gofr_proto_frontend_*).  A connection goroutine reads raw bytes; `ConnFrontend.serve` takes one such read and answers it
+through the device framer, parser and serve chain (gofr_conn_frontend_*).  ctypes drops the GIL for the duration of a
+call, so Python threads can stand in for goroutines.
 """
 from __future__ import annotations
 
 import ctypes as C
 from typing import Optional, Tuple
 
+import numpy as np
+
 from . import _abi
 from . import spec as S
-from .engine import Engine, nested_bound
+from .engine import ConnLogLines, ConnResponses, Engine, conn_batch_bound, conn_log_bound, nested_bound
 
 
 class Frontend:
@@ -102,3 +106,69 @@ class ProtoFrontend:
         _abi.check(_abi.lib().gofr_proto_frontend_call(self._f, data, len(data), buf, out_cap, C.byref(n), C.byref(status)),
                    "gofr_proto_frontend_call")
         return buf.raw[:n.value], int(status.value)
+
+
+class ConnFrontend:
+    """One read of one connection per call: serve(bytes held for the connection) → ConnResponses of that connection alone
+    (n_conns = 1: req_first, consumed and conn_status have one connection's entries), with .log when the front-end was
+    created with log.  On MORE keep buf[consumed[0]:] and append the next read; on DEFER write the responses, then hand
+    buf[consumed[0]:] to net/http; a hole (status 0) is served from buf[req_at[k]:]."""
+
+    def __init__(self, engine: Engine, max_batch: int = 1024, max_wait_us: int = 200, max_conn_bytes: int = 16384,
+                 log: bool = False, tz_offset_s: int = 0, seed: int = 0):
+        self._f = C.c_void_p()
+        self.engine = engine
+        self.log = bool(log)
+        _abi.check(_abi.lib().gofr_conn_frontend_create(C.byref(self._f), engine._e, max_batch, max_wait_us, max_conn_bytes,
+                                                        int(self.log), tz_offset_s, seed), "gofr_conn_frontend_create")
+
+    def close(self):
+        if self._f:
+            _abi.lib().gofr_conn_frontend_destroy(self._f)
+            self._f = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def set_clock(self, unix_ns: int) -> None:
+        """pin the Date header and the log time of every batch (tests); 0 = wall clock"""
+        _abi.check(_abi.lib().gofr_conn_frontend_set_clock(self._f, unix_ns), "gofr_conn_frontend_set_clock")
+
+    def stats(self) -> Tuple[int, int, int]:
+        """(batches, connection reads served, batches served again after their outputs grew)"""
+        b, c, r = C.c_uint64(), C.c_uint64(), C.c_uint64()
+        _abi.check(_abi.lib().gofr_conn_frontend_stats(self._f, C.byref(b), C.byref(c), C.byref(r)), "gofr_conn_frontend_stats")
+        return int(b.value), int(c.value), int(r.value)
+
+    def serve(self, buf: bytes, remote: bytes = b"", start_unix_ns: int = 0) -> ConnResponses:
+        """Blocks until the batch this read joined has been served.  remote: the connection's req.RemoteAddr (at most 255
+        bytes); start_unix_ns: Logging's start clock for this read.  The outputs are sized with gofr_conn_batch_bound /
+        gofr_conn_log_bound on {0, len(buf)}, which always suffice; a read past max_conn_bytes raises
+        GofrError(GOFR_ERR_CAPACITY)."""
+        buf = bytes(buf)
+        off = np.array([0, len(buf)], np.uint32)
+        req_cap, out_cap = conn_batch_bound(self.engine.table, off)
+        out, out_off, meta = np.zeros(max(out_cap, 1), np.uint8), np.zeros(req_cap + 1, np.uint32), np.zeros(max(req_cap, 1), np.uint32)
+        req_at, ids = np.zeros(max(req_cap, 1), np.uint32), np.zeros(max(req_cap, 1) * 16, np.uint8)
+        req_first, consumed, status = np.zeros(2, np.uint32), np.zeros(1, np.uint32), np.zeros(1, np.uint32)
+        cr = _abi.ConnResp(out=out.ctypes.data, out_cap=out_cap, req_cap=req_cap, out_off=out_off.ctypes.data, meta=meta.ctypes.data,
+                           req_at=req_at.ctypes.data, trace_ids=ids.ctypes.data, req_first=req_first.ctypes.data,
+                           consumed=consumed.ctypes.data, conn_status=status.ctypes.data, out_bytes=0)
+        cl = None
+        if self.log:
+            line_cap, log_out_cap = conn_log_bound(off, np.array([0, len(remote)], np.uint32))
+            lout, log_off, log_req = np.zeros(max(log_out_cap, 1), np.uint8), np.zeros(line_cap + 1, np.uint32), np.zeros(max(line_cap, 1), np.uint32)
+            cl = _abi.ConnLog(line_cap=line_cap, out=lout.ctypes.data, out_cap=log_out_cap, log_off=log_off.ctypes.data,
+                              log_req=log_req.ctypes.data)
+        _abi.check(_abi.lib().gofr_conn_frontend_serve(self._f, buf, len(buf), remote, len(remote), start_unix_ns, C.byref(cr),
+                                                       C.byref(cl) if cl is not None else None), "gofr_conn_frontend_serve")
+        k = int(req_first[1])
+        lines = None
+        if cl is not None:
+            m = cl.lines
+            lines = ConnLogLines(lout[:int(cl.out_bytes)], log_off[:m + 1], log_req[:m], m, int(cl.out_bytes))
+        return ConnResponses(out[:int(cr.out_bytes)], out_off[:k + 1], meta[:k], req_at[:k], ids[:k * 16].reshape(k, 16), req_first,
+                             consumed, status, lines)

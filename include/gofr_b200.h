@@ -904,6 +904,42 @@ int gofr_conn_batch_respond(gofr_engine*, const gofr_conn_batch* in, const gofr_
 int gofr_conn_respond_bound(const gofr_table*, const gofr_req_desc* desc, uint32_t n_req, const uint32_t* rec_off,
                             uint64_t* out_cap);
 
+/* Batching front-end over gofr_conn_batch_submit_log: net/http runs one goroutine per connection (conn.serve looping
+ * readRequest, pkg/gofr/httpServer.go:29-33), each holding only its own received bytes.  Any number of threads call
+ * gofr_conn_frontend_serve with ONE read of one connection each (the kept tail plus the new bytes) and block until the batch
+ * it joined has been served; batches close and rotate as gofr_frontend_create's max_batch and max_wait_us say.
+ * What a call returns is what gofr_conn_batch_submit_log returns for that connection as a batch of one (n_conns = 1), except
+ * for the trace ids:
+ *   out  out[out_off[k] .. out_off[k+1]) is request k's response (offsets from the caller's out), meta[k], req_at[k] (the
+ *        request's first byte in buf), trace_ids[16k ..] (may be NULL); req_first[0..1] = {0, requests}, consumed[0],
+ *        conn_status[0] (GOFR_HTTP_CONN_DONE / MORE / DEFER) and out_bytes.  Holes (status 0) and DEFER mean what they mean
+ *        for the batch call: serve a hole from buf[req_at[k] ..]; on DEFER write the responses, then hand buf[consumed[0] ..]
+ *        to net/http; on MORE keep buf[consumed[0] ..] and append the next read to it.
+ *   log  when log != NULL and the front-end was created with log != 0: the connection's lines in the output fields of
+ *        gofr_conn_log, where log_req[m] indexes this call's requests; its input fields are ignored: remote (at most 255 bytes) and
+ *        start_unix_ns (Logging's `start := time.Now()` for this read) are arguments, log time and zone the front-end's.
+ *        Otherwise lines and out_bytes are 0.
+ * Per batch: Date and log_unix_ns are the wall clock at dispatch (gofr_conn_frontend_set_clock pins them, in ns; 0 = wall
+ * clock), and trace_seed = splitmix64(splitmix64(seed) + batch number), batches numbered from 0; the connection in slot c of
+ * the batch gets gofr_conn_batch_submit's ids for (trace_seed, c, j).  Each id is the bytes of its response's X-Correlation-Id.
+ * Returns GOFR_OK; at once, without joining a batch, for len == 0 (conn_status DONE, no requests); GOFR_ERR_CAPACITY before
+ * anything is queued when len > max_conn_bytes (hand the connection to net/http); GOFR_ERR_CAPACITY with req_first[1],
+ * out_bytes and the log's lines / out_bytes set to what the connection needed when the caller's req_cap, out_cap, line_cap
+ * or log out_cap is short (columns whose capacities suffice are complete; the front-end keeps serving;
+ * gofr_conn_batch_bound / gofr_conn_log_bound on {0, len} give capacities that always suffice); the batch call's own error
+ * for every caller of that batch; GOFR_ERR_INVALID for bad arguments and once destroy has started.
+ * One call per connection at a time.  A batch's response and log outputs grow when the batch call reports more than they
+ * hold (the batch is then served again, counted in stats' reruns) and never shrink.  create refuses (GOFR_ERR_CAPACITY) a
+ * max_batch * max_conn_bytes beyond 32 bits.  destroy may only be called when no thread is inside gofr_conn_frontend_serve. */
+typedef struct gofr_conn_frontend gofr_conn_frontend;
+int gofr_conn_frontend_create(gofr_conn_frontend** out, gofr_engine*, uint32_t max_batch, uint32_t max_wait_us,
+                              uint32_t max_conn_bytes, int log, int32_t tz_offset_s, uint64_t seed);
+void gofr_conn_frontend_destroy(gofr_conn_frontend*);
+int gofr_conn_frontend_set_clock(gofr_conn_frontend*, int64_t unix_ns);
+int gofr_conn_frontend_stats(gofr_conn_frontend*, uint64_t* batches, uint64_t* conns, uint64_t* reruns);
+int gofr_conn_frontend_serve(gofr_conn_frontend*, const uint8_t* buf, uint32_t len, const uint8_t* remote, uint32_t remote_len,
+                             int64_t start_unix_ns, gofr_conn_resp* out, gofr_conn_log* log);
+
 /* number of kernels launched by this engine so far (bench.py reports it as gpu_launches) */
 uint64_t gofr_engine_launch_count(const gofr_engine*);
 /* duration in ms of the kernels launched since the last reset, measured with CUDA events on the launch stream.  Every

@@ -1006,4 +1006,90 @@ private:
     gofr_proto_frontend* f_ = nullptr;
 };
 
+// net/http's conn.serve one read at a time (gofr_conn_frontend_serve): Serve takes the bytes a connection's thread holds (the
+// kept tail plus its new read) and blocks until the batch it joined has been framed, parsed and answered on the GPU.  A
+// request of a GOFR_H_HOST route (status 0 in meta) is a hole: the caller runs that route's closure and writes its response
+// at the hole's place.  On GOFR_HTTP_CONN_MORE keep buf[consumed ..] and append the next read; on GOFR_HTTP_CONN_DEFER write
+// the responses, then hand buf[consumed ..] to net/http.  Any number of threads may call one ConnFrontend, one call per
+// connection at a time.  The engine serves `table`; App's routes are GOFR_H_RESULT routes, which need their closures'
+// records (App::ServeConnections), so an App's table is not one to serve through this front-end.
+class ConnFrontend {
+public:
+    struct Read {
+        int rc = GOFR_OK;           // GOFR_ERR_CAPACITY: the read exceeds max_conn_bytes, nothing was queued (use net/http)
+        std::string bytes;          // the responses back to back: request k's is bytes[out_off[k] .. out_off[k+1]), a hole's empty
+        std::vector<uint32_t> out_off{0}, meta, req_at;  // meta as gofr_batch_submit's; req_at: the request's first byte in buf
+        std::vector<std::array<uint8_t, 16>> trace_ids;  // each the bytes of its response's X-Correlation-Id
+        uint32_t consumed = 0, conn_status = GOFR_HTTP_CONN_DONE;
+        std::string log;            // with log: middleware.Logging's lines, line m = log[log_off[m] .. log_off[m+1]) for request log_req[m]
+        std::vector<uint32_t> log_off{0}, log_req;
+    };
+
+    ConnFrontend(gofr_engine* engine, const gofr_table* table, uint32_t max_batch = 1024, uint32_t max_wait_us = 200,
+                 uint32_t max_conn_bytes = 16384, bool log = false, int32_t tz_offset_s = 0, uint64_t seed = 0)
+        : table_(table), max_conn_bytes_(max_conn_bytes), log_(log) {
+        ProtoCodec::check(gofr_conn_frontend_create(&f_, engine, max_batch, max_wait_us, max_conn_bytes, log ? 1 : 0, tz_offset_s, seed),
+                          "gofr_conn_frontend_create");
+    }
+    ~ConnFrontend() { gofr_conn_frontend_destroy(f_); }
+    ConnFrontend(const ConnFrontend&) = delete;
+    ConnFrontend& operator=(const ConnFrontend&) = delete;
+
+    // remote: the connection's req.RemoteAddr (at most 255 bytes); start_unix_ns: Logging's start clock for this read
+    Read Serve(const std::string& buf, const std::string& remote = std::string(), int64_t start_unix_ns = 0) const {
+        Read r;
+        if (buf.size() > max_conn_bytes_) { r.rc = GOFR_ERR_CAPACITY; return r; }
+        // capacities that always suffice for this read: the front-end never answers GOFR_ERR_CAPACITY for them
+        const uint32_t off[2] = {0, (uint32_t)buf.size()}, roff[2] = {0, (uint32_t)remote.size()};
+        uint32_t req_cap = 0, line_cap = 0;
+        uint64_t out_cap = 0, log_cap = 0;
+        ProtoCodec::check(gofr_conn_batch_bound(table_, off, 1, &req_cap, &out_cap), "gofr_conn_batch_bound");
+        if (log_) ProtoCodec::check(gofr_conn_log_bound(off, roff, 1, &line_cap, &log_cap), "gofr_conn_log_bound");
+        r.bytes.resize(out_cap);
+        r.out_off.resize(req_cap + 1);
+        r.meta.resize(req_cap);
+        r.req_at.resize(req_cap);
+        r.trace_ids.resize(req_cap);
+        r.log.resize(log_cap);
+        r.log_off.resize(line_cap + 1);
+        r.log_req.resize(line_cap);
+        uint32_t first[2] = {0, 0};
+        gofr_conn_resp o{};
+        o.out = reinterpret_cast<uint8_t*>(&r.bytes[0]); o.out_cap = out_cap; o.req_cap = req_cap; o.out_off = r.out_off.data();
+        o.meta = r.meta.data(); o.req_at = r.req_at.data(); o.trace_ids = r.trace_ids.empty() ? nullptr : r.trace_ids[0].data();
+        o.req_first = first; o.consumed = &r.consumed; o.conn_status = &r.conn_status;
+        gofr_conn_log l{};
+        l.line_cap = line_cap; l.out = reinterpret_cast<uint8_t*>(&r.log[0]); l.out_cap = log_cap; l.log_off = r.log_off.data();
+        l.log_req = r.log_req.data();
+        r.rc = gofr_conn_frontend_serve(f_, reinterpret_cast<const uint8_t*>(buf.data()), (uint32_t)buf.size(),
+                                        reinterpret_cast<const uint8_t*>(remote.data()), (uint32_t)remote.size(), start_unix_ns, &o,
+                                        log_ ? &l : nullptr);
+        ProtoCodec::check(r.rc, "gofr_conn_frontend_serve");
+        const uint32_t n = first[1];
+        r.bytes.resize(o.out_bytes);
+        r.out_off.resize(n + 1);
+        r.meta.resize(n);
+        r.req_at.resize(n);
+        r.trace_ids.resize(n);
+        r.log.resize(log_ ? l.out_bytes : 0);
+        r.log_off.resize((log_ ? l.lines : 0) + 1);
+        r.log_req.resize(log_ ? l.lines : 0);
+        return r;
+    }
+    // pin the Date header and the log time of every batch (tests); 0 = wall clock
+    void SetClock(int64_t unix_ns) { ProtoCodec::check(gofr_conn_frontend_set_clock(f_, unix_ns), "gofr_conn_frontend_set_clock"); }
+    // batches, connection reads served, batches served again after their outputs grew
+    std::array<uint64_t, 3> Stats() const {
+        std::array<uint64_t, 3> s{};
+        ProtoCodec::check(gofr_conn_frontend_stats(f_, &s[0], &s[1], &s[2]), "gofr_conn_frontend_stats");
+        return s;
+    }
+
+private:
+    const gofr_table* table_;
+    uint32_t max_conn_bytes_;
+    bool log_;
+    gofr_conn_frontend* f_ = nullptr;
+};
+
 }  // namespace gofr
