@@ -917,3 +917,168 @@ func (f *ConnFrontend) Serve(buf, remote []byte, start time.Time, r *ConnRespons
 	}
 	return uint64(o.out_bytes), check(rc, "gofr_conn_frontend_serve")
 }
+
+// ConnAppFrontend serves handler-closure apps one connection read per call (gofr_conn_app_frontend_*): Route hands in a
+// read and returns its requests routed, parsed and bound on the GPU together with the other goroutines' reads; the
+// goroutine runs the closures itself, as long as they take; Respond hands in the same read with the closures' records and
+// returns its responses.  Route batches and respond batches are independent, so no response waits for another
+// connection's closure.  Several front-ends of any kind may share one Engine.
+type ConnAppFrontend struct {
+	f            *C.gofr_conn_app_frontend
+	maxConnBytes int
+	log          bool
+	maxFields    int
+}
+
+// ConnAppRoute is what Route returns for one read: its requests as ServeConnections' stage 1 returns them for a batch of
+// one (Desc into Arena, ReqAt into the read), each request's bind status (GOFR_BIND_*, 0xFFFFFFFF when not bound) and row
+// Rows[RowOff[k]:RowOff[k+1]], and the read's trace key, which Respond takes.
+type ConnAppRoute struct {
+	Desc                 []C.gofr_req_desc
+	Arena                []byte
+	Meta, Vars, ReqAt    []uint32
+	TraceIDs             []byte
+	Consumed, ConnStatus uint32
+	BindStatus, RowOff   []uint32
+	Rows                 []byte
+	TraceKey             uint64
+}
+
+// NewConnAppFrontend: maxBatch and maxWaitMicros mean what they mean for NewFrontend; a read longer than maxConnBytes is
+// refused (ErrConnReadTooLarge).  routeSchema[r] is the schema route r binds (0: none) and schemaFields[r] that schema's
+// field count.  With log, Respond also returns middleware.Logging's lines.
+func NewConnAppFrontend(e *Engine, maxBatch, maxWaitMicros, maxConnBytes int, log bool, tzOffsetSeconds int32, seed uint64,
+	routeSchema, schemaFields []uint32) (*ConnAppFrontend, error) {
+	if len(routeSchema) != len(schemaFields) {
+		return nil, errors.New("gofrb200: routeSchema and schemaFields differ in length")
+	}
+	l := C.int(0)
+	if log {
+		l = 1
+	}
+	var rs, sf *C.uint32_t
+	maxFields := 0
+	if len(routeSchema) > 0 {
+		rs = (*C.uint32_t)(unsafe.Pointer(&routeSchema[0]))
+		sf = (*C.uint32_t)(unsafe.Pointer(&schemaFields[0]))
+		for _, n := range schemaFields {
+			if int(n) > maxFields {
+				maxFields = int(n)
+			}
+		}
+	}
+	var f *C.gofr_conn_app_frontend
+	if err := check(C.gofr_conn_app_frontend_create(&f, e.e, C.uint32_t(maxBatch), C.uint32_t(maxWaitMicros), C.uint32_t(maxConnBytes), l,
+		C.int32_t(tzOffsetSeconds), C.uint64_t(seed), rs, C.uint32_t(len(routeSchema)), sf), "gofr_conn_app_frontend_create"); err != nil {
+		return nil, err
+	}
+	return &ConnAppFrontend{f, maxConnBytes, log, maxFields}, nil
+}
+
+// Close must not run while a Route or Respond is in progress.
+func (f *ConnAppFrontend) Close() { C.gofr_conn_app_frontend_destroy(f.f); f.f = nil }
+
+// SetClock pins the Date header and the log time of every respond batch (tests); the zero Time restores the wall clock.
+func (f *ConnAppFrontend) SetClock(t time.Time) error {
+	ns := int64(0)
+	if !t.IsZero() {
+		ns = t.UnixNano()
+	}
+	return check(C.gofr_conn_app_frontend_set_clock(f.f, C.int64_t(ns)), "gofr_conn_app_frontend_set_clock")
+}
+
+// Stats returns gofr_conn_app_stats: route and respond batches and reads, reruns, isolated batches, record-gather time.
+func (f *ConnAppFrontend) Stats() (C.gofr_conn_app_stats, error) {
+	var st C.gofr_conn_app_stats
+	return st, check(C.gofr_conn_app_frontend_stats(f.f, &st), "gofr_conn_app_frontend_stats")
+}
+
+// Route blocks until the route batch this read joined has been routed and bound.
+func (f *ConnAppFrontend) Route(buf []byte) (*ConnAppRoute, error) {
+	if len(buf) > f.maxConnBytes {
+		return nil, ErrConnReadTooLarge
+	}
+	reqCap := len(buf)/16 + 1 // the framer's most for one connection
+	r := &ConnAppRoute{Desc: make([]C.gofr_req_desc, reqCap), Arena: make([]byte, len(buf)+80), Meta: make([]uint32, reqCap),
+		Vars: make([]uint32, reqCap*C.GOFR_MAX_PATH_VARS), ReqAt: make([]uint32, reqCap), TraceIDs: make([]byte, 16*reqCap),
+		BindStatus: make([]uint32, reqCap), RowOff: make([]uint32, reqCap+1), Rows: make([]byte, reqCap*(8*f.maxFields+272)+len(buf))}
+	var first [2]C.uint32_t
+	var rt C.gofr_conn_route
+	rt.req_cap = C.uint32_t(reqCap)
+	rt.desc = &r.Desc[0]
+	rt.arena = (*C.uint8_t)(unsafe.Pointer(&r.Arena[0]))
+	rt.meta = (*C.uint32_t)(unsafe.Pointer(&r.Meta[0]))
+	rt.vars = (*C.uint32_t)(unsafe.Pointer(&r.Vars[0]))
+	rt.req_at = (*C.uint32_t)(unsafe.Pointer(&r.ReqAt[0]))
+	rt.trace_ids = (*C.uint8_t)(unsafe.Pointer(&r.TraceIDs[0]))
+	rt.req_first = &first[0]
+	rt.consumed = (*C.uint32_t)(unsafe.Pointer(&r.Consumed))
+	rt.conn_status = (*C.uint32_t)(unsafe.Pointer(&r.ConnStatus))
+	var bd C.gofr_conn_app_bind
+	bd.status = (*C.uint32_t)(unsafe.Pointer(&r.BindStatus[0]))
+	bd.row_off = (*C.uint32_t)(unsafe.Pointer(&r.RowOff[0]))
+	bd.rows = (*C.uint8_t)(unsafe.Pointer(&r.Rows[0]))
+	bd.rows_cap = C.uint64_t(len(r.Rows))
+	var key C.uint64_t
+	if err := check(C.gofr_conn_app_frontend_route(f.f, bytesPtr(buf), C.uint32_t(len(buf)), &rt, &bd, &key), "gofr_conn_app_frontend_route"); err != nil {
+		return nil, err
+	}
+	n := int(first[1])
+	r.Desc, r.Meta, r.Vars, r.ReqAt = r.Desc[:n], r.Meta[:n], r.Vars[:n*C.GOFR_MAX_PATH_VARS], r.ReqAt[:n]
+	r.TraceIDs, r.BindStatus, r.RowOff, r.Rows = r.TraceIDs[:16*n], r.BindStatus[:n], r.RowOff[:n+1], r.Rows[:bd.rows_bytes]
+	r.TraceKey = uint64(key)
+	return r, nil
+}
+
+// Respond blocks until the respond batch this read joined has been served: buf is the read Route took, key its TraceKey,
+// request k's record recs[recOff[k]:recOff[k+1]] (GOFR_H_RESULT; empty: the request is answered as ServeConnections
+// answers it).  r and the return value are ConnFrontend.Serve's.
+func (f *ConnAppFrontend) Respond(buf []byte, key uint64, recs []byte, recOff []uint32, remote []byte, start time.Time, r *ConnResponses) (uint64, error) {
+	if len(buf) > f.maxConnBytes {
+		return 0, ErrConnReadTooLarge
+	}
+	if len(recOff) == 0 || len(r.Out) == 0 || len(r.Meta) == 0 || len(r.OutOff) < len(r.Meta)+1 || len(r.ReqAt) < len(r.Meta) ||
+		(r.TraceIDs != nil && len(r.TraceIDs) < 16*len(r.Meta)) || len(r.ReqFirst) < 2 || len(r.Consumed) < 1 || len(r.ConnStatus) < 1 {
+		return 0, errors.New("gofrb200: record offsets or ConnResponses columns too small")
+	}
+	var res C.gofr_conn_results
+	res.rec = bytesPtr(recs)
+	res.rec_off = (*C.uint32_t)(unsafe.Pointer(&recOff[0]))
+	res.rec_bytes = C.uint64_t(len(recs))
+	res.n_req = C.uint32_t(len(recOff) - 1)
+	var o C.gofr_conn_resp
+	o.out = (*C.uint8_t)(unsafe.Pointer(&r.Out[0]))
+	o.out_cap = C.uint64_t(len(r.Out))
+	o.req_cap = C.uint32_t(len(r.Meta))
+	o.out_off = (*C.uint32_t)(unsafe.Pointer(&r.OutOff[0]))
+	o.meta = (*C.uint32_t)(unsafe.Pointer(&r.Meta[0]))
+	o.req_at = (*C.uint32_t)(unsafe.Pointer(&r.ReqAt[0]))
+	if r.TraceIDs != nil {
+		o.trace_ids = (*C.uint8_t)(unsafe.Pointer(&r.TraceIDs[0]))
+	}
+	o.req_first = (*C.uint32_t)(unsafe.Pointer(&r.ReqFirst[0]))
+	o.consumed = (*C.uint32_t)(unsafe.Pointer(&r.Consumed[0]))
+	o.conn_status = (*C.uint32_t)(unsafe.Pointer(&r.ConnStatus[0]))
+	var lg *C.gofr_conn_log
+	if l := r.Log; l != nil && f.log {
+		if len(l.Out) == 0 || len(l.LogReq) == 0 || len(l.LogOff) < len(l.LogReq)+1 {
+			return 0, errors.New("gofrb200: ConnLog columns too small")
+		}
+		lg = &C.gofr_conn_log{}
+		lg.line_cap = C.uint32_t(len(l.LogReq))
+		lg.out = (*C.uint8_t)(unsafe.Pointer(&l.Out[0]))
+		lg.out_cap = C.uint64_t(len(l.Out))
+		lg.log_off = (*C.uint32_t)(unsafe.Pointer(&l.LogOff[0]))
+		lg.log_req = (*C.uint32_t)(unsafe.Pointer(&l.LogReq[0]))
+	}
+	ns := int64(0)
+	if !start.IsZero() {
+		ns = start.UnixNano()
+	}
+	rc := C.gofr_conn_app_frontend_respond(f.f, bytesPtr(buf), C.uint32_t(len(buf)), C.uint64_t(key), &res, bytesPtr(remote),
+		C.uint32_t(len(remote)), C.int64_t(ns), &o, lg)
+	if lg != nil {
+		r.Log.Lines, r.Log.OutBytes = uint32(lg.lines), uint64(lg.out_bytes)
+	}
+	return uint64(o.out_bytes), check(rc, "gofr_conn_app_frontend_respond")
+}

@@ -74,6 +74,16 @@ class ConnResults(C.Structure):
                 ("reserved", C.c_uint32)]
 
 
+class ConnAppBind(C.Structure):
+    _fields_ = [("status", C.c_void_p), ("row_off", C.c_void_p), ("rows", C.c_void_p), ("rows_cap", C.c_uint64),
+                ("rows_bytes", C.c_uint64)]
+
+
+class ConnAppStats(C.Structure):
+    _fields_ = [("route_batches", C.c_uint64), ("route_reads", C.c_uint64), ("respond_batches", C.c_uint64),
+                ("respond_reads", C.c_uint64), ("reruns", C.c_uint64), ("isolated", C.c_uint64), ("gather_ns", C.c_uint64)]
+
+
 class ProtoBatch(C.Structure):
     _fields_ = [("data", C.c_void_p), ("data_bytes", C.c_uint64), ("off", C.c_void_p), ("n", C.c_uint32)]
 
@@ -190,6 +200,16 @@ def lib():
     L.gofr_conn_batch_respond.argtypes = [vp, C.POINTER(ConnBatch), C.POINTER(ConnResults), C.POINTER(ConnResp), C.POINTER(ConnLog),
                                           C.POINTER(u64)]
     L.gofr_conn_respond_bound.argtypes = [vp, vp, u32, vp, C.POINTER(u64)]
+    L.gofr_conn_batch_respond_ex.argtypes = [vp, C.POINTER(ConnBatch), vp, C.POINTER(ConnResults), C.POINTER(ConnResp),
+                                             C.POINTER(ConnLog), C.POINTER(u64)]
+    L.gofr_conn_app_frontend_create.argtypes = [C.POINTER(vp), vp, u32, u32, u32, i32, C.c_int32, u64, vp, u32, vp]
+    L.gofr_conn_app_frontend_destroy.argtypes = [vp]
+    L.gofr_conn_app_frontend_destroy.restype = None
+    L.gofr_conn_app_frontend_set_clock.argtypes = [vp, C.c_int64]
+    L.gofr_conn_app_frontend_stats.argtypes = [vp, C.POINTER(ConnAppStats)]
+    L.gofr_conn_app_frontend_route.argtypes = [vp, C.c_char_p, u32, C.POINTER(ConnRoute), C.POINTER(ConnAppBind), C.POINTER(u64)]
+    L.gofr_conn_app_frontend_respond.argtypes = [vp, C.c_char_p, u32, u64, C.POINTER(ConnResults), C.c_char_p, u32, C.c_int64,
+                                                 C.POINTER(ConnResp), C.POINTER(ConnLog)]
     L.gofr_requestlog_device.argtypes = [vp, vp, vp, vp, u32, vp, u64, vp, vp]
     L.gofr_engine_launch_count.argtypes = [vp]
     L.gofr_engine_launch_count.restype = u64
@@ -209,9 +229,12 @@ DECLARED_SYMBOLS = [
     "gofr_table_route_count", "gofr_table_max_response_bytes", "gofr_engine_create", "gofr_engine_destroy",
     "gofr_serve_device", "gofr_serve_device_slots", "gofr_batch_submit", "gofr_batch_wait", "gofr_batch_submit_slots", "gofr_engine_set_chunk", "gofr_engine_set_tile",
     "gofr_engine_set_timing", "gofr_engine_overflowed", "gofr_engine_geometry", "gofr_engine_slot_ctas", "gofr_table_slot_ctas", "gofr_alloc_pinned", "gofr_free_pinned", "gofr_bind_host_thread", "gofr_bind_device", "gofr_batch_bind",
-    "gofr_grpc_hello_device", "gofr_requestlog_device", "gofr_http_parse_device", "gofr_http_frame_device", "gofr_conn_batch_submit", "gofr_conn_batch_bound", "gofr_conn_batch_submit_log", "gofr_conn_log_bound", "gofr_conn_batch_route", "gofr_conn_batch_respond", "gofr_conn_respond_bound", "gofr_batch_route", "gofr_proto_encode_device", "gofr_proto_decode_device", "gofr_proto_encode_nested_device", "gofr_proto_decode_nested_device", "gofr_proto_nested_describe", "gofr_proto_encode_nested_ex_device", "gofr_proto_decode_nested_ex_device", "gofr_proto_nested_describe_ex", "gofr_proto_decode_nested_deferred_device", "gofr_proto_batch_decode", "gofr_proto_batch_encode", "gofr_proto_nested_bound", "gofr_table_response_bound", "gofr_frontend_create", "gofr_frontend_destroy", "gofr_frontend_set_clock",
+    "gofr_grpc_hello_device", "gofr_requestlog_device", "gofr_http_parse_device", "gofr_http_frame_device", "gofr_conn_batch_submit", "gofr_conn_batch_bound", "gofr_conn_batch_submit_log", "gofr_conn_log_bound", "gofr_conn_batch_route", "gofr_conn_batch_respond", "gofr_conn_respond_bound", "gofr_conn_batch_respond_ex", "gofr_batch_route", "gofr_proto_encode_device", "gofr_proto_decode_device", "gofr_proto_encode_nested_device", "gofr_proto_decode_nested_device", "gofr_proto_nested_describe", "gofr_proto_encode_nested_ex_device", "gofr_proto_decode_nested_ex_device", "gofr_proto_nested_describe_ex", "gofr_proto_decode_nested_deferred_device", "gofr_proto_batch_decode", "gofr_proto_batch_encode", "gofr_proto_nested_bound", "gofr_table_response_bound", "gofr_frontend_create", "gofr_frontend_destroy", "gofr_frontend_set_clock",
     "gofr_frontend_stats", "gofr_frontend_serve", "gofr_proto_frontend_create", "gofr_proto_frontend_destroy",
     "gofr_proto_frontend_stats", "gofr_proto_frontend_call", "gofr_conn_frontend_create", "gofr_conn_frontend_destroy",
-    "gofr_conn_frontend_set_clock", "gofr_conn_frontend_stats", "gofr_conn_frontend_serve", "gofr_route_device", "gofr_engine_launch_count", "gofr_engine_kernel_time_ms", "gofr_last_error",
+    "gofr_conn_frontend_set_clock", "gofr_conn_frontend_stats", "gofr_conn_frontend_serve",
+    "gofr_conn_app_frontend_create", "gofr_conn_app_frontend_destroy", "gofr_conn_app_frontend_set_clock",
+    "gofr_conn_app_frontend_stats", "gofr_conn_app_frontend_route", "gofr_conn_app_frontend_respond",
+    "gofr_route_device", "gofr_engine_launch_count", "gofr_engine_kernel_time_ms", "gofr_last_error",
     "gofr_abi_version", "gofr_format_http_date",
 ]

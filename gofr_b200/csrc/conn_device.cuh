@@ -29,6 +29,11 @@ GOFR_CONN_HD uint64_t conn_splitmix64(uint64_t x) {
 // The trace id of request j of connection c (include/gofr_b200.h, gofr_conn_batch_submit): two splitmix64 draws keyed by
 // (seed, c, j), stored little-endian.  `key` is conn_trace_key(seed, c), computed once per connection.
 GOFR_CONN_HD uint64_t conn_trace_key(uint64_t seed, uint32_t c) { return conn_splitmix64(seed ^ conn_splitmix64((uint64_t)c)); }
+// The key of the chunk's connection i, batch connection conn0 + i: keys[i] when the caller gave a key column
+// (gofr_conn_batch_respond_ex), else conn_trace_key(seed, conn0 + i).
+GOFR_CONN_HD uint64_t conn_key(const uint64_t* keys, uint64_t seed, uint32_t conn0, uint32_t i) {
+    return keys ? keys[i] : conn_trace_key(seed, conn0 + i);
+}
 GOFR_CONN_HD void conn_trace_id(uint64_t key, uint32_t j, uint8_t* out16) {
     const uint64_t lo = conn_splitmix64(key + 2ull * j), hi = conn_splitmix64(key + 2ull * j + 1ull);
     memcpy(out16, &lo, 8);

@@ -29,7 +29,7 @@ __global__ void __launch_bounds__(CT) conn_compact_kernel(const ConnParams p) {
         p.out_off[i] = p.req0 + k0;
         if (i == p.n - 1) p.out_off[p.n] = p.req0 + k0 + count;
         if (!t.fits) continue;
-        conn_put((const gofr_req_desc*)p.desc_in, p.rec_off, p.first[i], count, conn_trace_key(p.trace_seed, p.conn0 + i),
+        conn_put((const gofr_req_desc*)p.desc_in, p.rec_off, p.first[i], count, conn_key(p.trace_key, p.trace_seed, p.conn0, i),
                  (gofr_req_desc*)p.out, p.req_at, p.ids, k0);
     }
 }

@@ -147,6 +147,7 @@ struct Slot {
     uint32_t* d_first = nullptr; uint32_t* d_cstatus = nullptr; uint32_t* d_consumed = nullptr; uint32_t* d_req_first = nullptr;
     uint32_t* d_rec = nullptr; void* d_pdesc = nullptr; uint32_t* d_pstatus = nullptr; unsigned long long* d_spans = nullptr;
     uint32_t* d_req_at = nullptr;
+    uint64_t* d_tkey = nullptr;  // gofr_conn_batch_respond_ex: the chunk's per-connection trace keys
     size_t cap_buf = 0, cap_conns = 0, cap_recs = 0;
     // its request-log lines (grown on demand): the staged remote strings, their offsets and the start clocks (per
     // connection), the gather's per-connection line column, its descriptors, trace ids and request indices and the
@@ -415,7 +416,7 @@ void gofr_engine_destroy(gofr_engine* e) {
         cudaFree(s.state.words); cudaFree(s.d_flag); cudaFree(s.d_bind);
         cudaFree(s.d_in_off); cudaFree(s.d_meta1);
         for (int k = 0; k < 2; k++) { cudaFree(s.d_codec[k]); cudaFree(s.d_codec_off[k]); }
-        cudaFree(s.d_buf); cudaFree(s.d_buf_off); cudaFree(s.d_first); cudaFree(s.d_cstatus); cudaFree(s.d_consumed);
+        cudaFree(s.d_buf); cudaFree(s.d_buf_off); cudaFree(s.d_first); cudaFree(s.d_cstatus); cudaFree(s.d_consumed); cudaFree(s.d_tkey);
         cudaFree(s.d_req_first); cudaFree(s.d_rec); cudaFree(s.d_pdesc); cudaFree(s.d_pstatus); cudaFree(s.d_spans); cudaFree(s.d_req_at);
         cudaFree(s.d_remote); cudaFree(s.d_remote_off); cudaFree(s.d_start); cudaFree(s.d_lfirst); cudaFree(s.d_ldesc); cudaFree(s.d_lids);
         cudaFree(s.d_lreq); cudaFree(s.d_lraw_off); cudaFree(s.d_loff); cudaFree(s.d_larena); cudaFree(s.d_lraw); cudaFree(s.d_lout);
@@ -1224,7 +1225,7 @@ static constexpr uint32_t kConnChunkBudget = 8u << 20;
 // 16 readable bytes the framer and the request-head kernel need, and 16 more for the bulk copies' rounding).
 int Slot::reserve_conn(uint32_t conns, uint32_t records, size_t buf_bytes) {
     int rc = grow_cols(&cap_conns, conns, "connections", {{&d_buf_off, 4, 4}, {&d_first, 4, 4}, {&d_cstatus, 4, 0},
-                                                          {&d_consumed, 4, 0}, {&d_req_first, 4, 4}});
+                                                          {&d_consumed, 4, 0}, {&d_req_first, 4, 4}, {&d_tkey, 8, 0}});
     if (!rc) rc = grow_cols(&cap_recs, records, "records", {{&d_rec, 4, 4}, {&d_pdesc, 16, 0}, {&d_pstatus, 4, 0},
                                                             {&d_spans, GOFR_HTTP_SPANS * 8, 0}, {&d_req_at, 4, 0}});
     return rc ? rc : grow((void**)&d_buf, &cap_buf, buf_bytes + 32, 256);
@@ -1293,8 +1294,8 @@ static int conn_plan(const gofr_engine* e, const gofr_conn_batch* in, const gofr
 
 // First half of a chunk: stage its bytes, frame them, and bring back its record count (s.h_tail[0]) and its per-connection
 // columns (the caller's consumed and conn_status).  s.done marks the moment the host may read them.
-static int conn_frame(gofr_engine* e, const gofr_conn_batch* in, uint32_t* consumed, uint32_t* conn_status, const gofr_conn_log* log,
-                      Slot& s, const ConnChunk& c) {
+static int conn_frame(gofr_engine* e, const gofr_conn_batch* in, const uint64_t* trace_key, uint32_t* consumed, uint32_t* conn_status,
+                      const gofr_conn_log* log, Slot& s, const ConnChunk& c) {
     const uint32_t cn = c.hi - c.lo, bytes = in->buf_off[c.hi] - c.alo;
     const uint64_t sizes[2] = {0, bytes};  // the chunk's paths, queries and bodies: never more than its bytes
     int rc = s.reserve(e, c.rec_cap, (size_t)bytes + 16, chunk_out_bound(e, c.rec_cap, sizes));
@@ -1304,6 +1305,7 @@ static int conn_frame(gofr_engine* e, const gofr_conn_batch* in, uint32_t* consu
     CUDA_TRY(cudaMemcpyAsync(s.d_buf, in->buf + c.alo, bytes, cudaMemcpyHostToDevice, e->st_h2d));
     CUDA_TRY(cudaMemsetAsync(s.d_buf + bytes, 0, 32, e->st_h2d));
     CUDA_TRY(cudaMemcpyAsync(s.d_buf_off, in->buf_off + c.lo, (size_t)(cn + 1) * 4, cudaMemcpyHostToDevice, e->st_h2d));
+    if (trace_key) CUDA_TRY(cudaMemcpyAsync(s.d_tkey, trace_key + c.lo, (size_t)cn * 8, cudaMemcpyHostToDevice, e->st_h2d));
     if (log) {
         if (c.rhi > c.rlo) CUDA_TRY(cudaMemcpyAsync(s.d_remote, log->remote + c.rlo, c.rhi - c.rlo, cudaMemcpyHostToDevice, e->st_h2d));
         CUDA_TRY(cudaMemcpyAsync(s.d_remote_off, log->remote_off + c.lo, (size_t)(cn + 1) * 4, cudaMemcpyHostToDevice, e->st_h2d));
@@ -1371,9 +1373,10 @@ static int conn_log_chunk(gofr_engine* e, const gofr_conn_batch* in, const gofr_
 
 // The chunk's framing is back: parse its records and compact its whole requests into s.d_desc, s.d_req_at, s.d_ids and
 // s.d_req_first (batch request indices from req0).  The record count and the connection states (conn_status, on the host
-// by now) size the launches; *n_req receives the chunk's request count.
-static int conn_parse(gofr_engine* e, const gofr_conn_batch* in, const uint32_t* conn_status, Slot& s, const ConnChunk& c,
-                      uint32_t req0, uint32_t* n_req_out) {
+// by now) size the launches; *n_req receives the chunk's request count.  With trace_key the ids come from the keys conn_frame
+// staged, else from (trace_seed, c).
+static int conn_parse(gofr_engine* e, const gofr_conn_batch* in, const uint64_t* trace_key, const uint32_t* conn_status, Slot& s,
+                      const ConnChunk& c, uint32_t req0, uint32_t* n_req_out) {
     CUDA_TRY(cudaEventSynchronize(s.done));
     const uint32_t cn = c.hi - c.lo, n_rec = s.h_tail[0];
     uint32_t n_req = n_rec;
@@ -1393,7 +1396,7 @@ static int conn_parse(gofr_engine* e, const gofr_conn_batch* in, const uint32_t*
     ConnParams q;
     memset(&q, 0, sizeof q);
     q.first = s.d_first; q.conn_status = s.d_cstatus; q.rec_off = s.d_rec; q.desc_in = s.d_pdesc;
-    q.trace_seed = in->trace_seed; q.conn0 = c.lo; q.req0 = req0; q.req_at = s.d_req_at; q.ids = (uint8_t*)s.d_ids;
+    q.trace_seed = in->trace_seed; q.trace_key = trace_key ? s.d_tkey : nullptr; q.conn0 = c.lo; q.req0 = req0; q.req_at = s.d_req_at; q.ids = (uint8_t*)s.d_ids;
     return launch_frames_locked(e, K_CONN, 0, q, cn, (uint8_t*)s.d_desc, n_rec, s.d_req_first, s.state, s.d_flag, st);
 }
 
@@ -1440,11 +1443,11 @@ static int conn_splice_chunk(gofr_engine* e, const gofr_conn_batch* in, const go
 
 // Second half of chunk ci: parse its records, compact the whole requests, splice the closures' results in (res not null),
 // serve them, and send the results to the caller's columns.
-static int conn_serve(gofr_engine* e, const gofr_conn_batch* in, const gofr_conn_results* res, gofr_conn_resp* out,
-                      const gofr_conn_log* log, Slot& s, size_t ci, const ConnChunk& c, PackedOut& ro, PackedOut& lo) {
+static int conn_serve(gofr_engine* e, const gofr_conn_batch* in, const uint64_t* trace_key, const gofr_conn_results* res,
+                      gofr_conn_resp* out, const gofr_conn_log* log, Slot& s, size_t ci, const ConnChunk& c, PackedOut& ro, PackedOut& lo) {
     const uint64_t req0 = ro.recs.base;
     uint32_t n_req = 0;
-    int rc = conn_parse(e, in, out->conn_status, s, c, (uint32_t)req0, &n_req);
+    int rc = conn_parse(e, in, trace_key, out->conn_status, s, c, (uint32_t)req0, &n_req);
     if (rc) return rc;
     const uint8_t* d_arena = s.d_arena - c.alo;
     if (res && (rc = conn_splice_chunk(e, in, res, s, c, req0, n_req, &d_arena)) != 0) return rc;
@@ -1461,8 +1464,8 @@ static int conn_serve(gofr_engine* e, const gofr_conn_batch* in, const gofr_conn
 // The chunks of a connection batch in order, one framed ahead of the one being stepped: the host learns a chunk's record
 // count while the next chunk's bytes are on their way.  step(s, ci, c) finishes chunk ci, framed in slot s.
 using ConnStep = std::function<int(Slot& s, size_t ci, const ConnChunk& c)>;
-static int conn_chunks(gofr_engine* e, const gofr_conn_batch* in, uint32_t* consumed, uint32_t* conn_status, const gofr_conn_log* log,
-                       const ConnStep& step) {
+static int conn_chunks(gofr_engine* e, const gofr_conn_batch* in, const uint64_t* trace_key, uint32_t* consumed, uint32_t* conn_status,
+                       const gofr_conn_log* log, const ConnStep& step) {
     const uint32_t n = in->n_conns;
     ConnChunk chunks[kSlots];
     size_t issued = 0, stepped = 0;
@@ -1470,7 +1473,7 @@ static int conn_chunks(gofr_engine* e, const gofr_conn_batch* in, uint32_t* cons
         while (next < n && issued < stepped + 2) {
             ConnChunk& c = chunks[issued % kSlots];
             int rc = conn_plan(e, in, log, next, &c);
-            if (!rc) rc = conn_frame(e, in, consumed, conn_status, log, e->slots[issued % kSlots], c);
+            if (!rc) rc = conn_frame(e, in, trace_key, consumed, conn_status, log, e->slots[issued % kSlots], c);
             if (rc) return rc;
             next = c.hi;
             issued++;
@@ -1482,8 +1485,8 @@ static int conn_chunks(gofr_engine* e, const gofr_conn_batch* in, uint32_t* cons
     return GOFR_OK;
 }
 
-static int conn_batch_locked(gofr_engine* e, const gofr_conn_batch* in, const gofr_conn_results* res, gofr_conn_resp* out,
-                             gofr_conn_log* log, gofr_ticket* ticket) {
+static int conn_batch_locked(gofr_engine* e, const gofr_conn_batch* in, const uint64_t* trace_key, const gofr_conn_results* res,
+                             gofr_conn_resp* out, gofr_conn_log* log, gofr_ticket* ticket) {
     const uint32_t n = in->n_conns;
     out->out_bytes = 0;
     if (log) { log->lines = 0; log->out_bytes = 0; }
@@ -1507,8 +1510,8 @@ static int conn_batch_locked(gofr_engine* e, const gofr_conn_batch* in, const go
         int rc = lo.start(e);
         if (rc) return rc;
     }
-    int rc = conn_chunks(e, in, out->consumed, out->conn_status, log, [&](Slot& s, size_t ci, const ConnChunk& c) {
-        return conn_serve(e, in, res, out, log, s, ci, c, ro, lo);
+    int rc = conn_chunks(e, in, trace_key, out->consumed, out->conn_status, log, [&](Slot& s, size_t ci, const ConnChunk& c) {
+        return conn_serve(e, in, trace_key, res, out, log, s, ci, c, ro, lo);
     });
     if (!rc) rc = PackedOut::finish(e, n, {&ro, &lo});
     if (rc) return rc;
@@ -1533,13 +1536,18 @@ int gofr_conn_batch_submit_log(gofr_engine* e, const gofr_conn_batch* in, gofr_c
 
 int gofr_conn_batch_respond(gofr_engine* e, const gofr_conn_batch* in, const gofr_conn_results* res, gofr_conn_resp* out,
                             gofr_conn_log* log, gofr_ticket* ticket) {
+    return gofr_conn_batch_respond_ex(e, in, nullptr, res, out, log, ticket);
+}
+
+int gofr_conn_batch_respond_ex(gofr_engine* e, const gofr_conn_batch* in, const uint64_t* trace_key, const gofr_conn_results* res,
+                               gofr_conn_resp* out, gofr_conn_log* log, gofr_ticket* ticket) {
     if (!e || !in || !out || !ticket) return GOFR_ERR_INVALID;
     if (in->n_conns && (!in->buf || !in->buf_off || !out->out || !out->out_off || !out->meta || !out->req_at || !out->req_first ||
                         !out->consumed || !out->conn_status)) return GOFR_ERR_INVALID;
     if (log && in->n_conns && (!log->remote_off || !log->start_unix_ns || !log->out || !log->log_off || !log->log_req)) return GOFR_ERR_INVALID;
     if (res && in->n_conns && (!res->rec_off || (res->rec_bytes && !res->rec))) return GOFR_ERR_INVALID;
     if (res && !in->n_conns && res->n_req) { set_last_error("the results are for %u requests, the batch has none", res->n_req); return GOFR_ERR_INVALID; }
-    return host_batch(e, [&] { return conn_batch_locked(e, in, res, out, log, ticket); });
+    return host_batch(e, [&] { return conn_batch_locked(e, in, trace_key, res, out, log, ticket); });
 }
 
 // Stage 1 of the closure path (gofr_conn_batch_route), synchronous: the connection chunks of conn_chunks, each framed,
@@ -1549,10 +1557,10 @@ int gofr_conn_batch_respond(gofr_engine* e, const gofr_conn_batch* in, const gof
 static int conn_route_locked(gofr_engine* e, const gofr_conn_batch* in, gofr_conn_route* out) {
     const cudaStream_t st = e->st_compute;
     RecCount r{out->req_cap};
-    int rc = conn_chunks(e, in, out->consumed, out->conn_status, nullptr, [&](Slot& s, size_t, const ConnChunk& c) -> int {
+    int rc = conn_chunks(e, in, nullptr, out->consumed, out->conn_status, nullptr, [&](Slot& s, size_t, const ConnChunk& c) -> int {
         const uint64_t req0 = r.base;
         uint32_t n_req = 0;
-        int rc = conn_parse(e, in, out->conn_status, s, c, (uint32_t)req0, &n_req);
+        int rc = conn_parse(e, in, nullptr, out->conn_status, s, c, (uint32_t)req0, &n_req);
         if (rc) return rc;
         if (r.add(n_req) && n_req) {
             const size_t vbytes = (size_t)n_req * 4 * GOFR_MAX_PATH_VARS;

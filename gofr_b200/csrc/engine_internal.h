@@ -251,6 +251,7 @@ struct ConnParams {
     const uint32_t* rec_off;      // the framer's record starts (absolute buffer offsets)
     const void* desc_in;          // gofr_req_desc per record (the request-head kernel's output)
     uint64_t trace_seed;
+    const uint64_t* trace_key;    // n: the connections' trace keys (gofr_conn_batch_respond_ex), or null: keys of (trace_seed, c)
     uint32_t conn0;               // the batch index of the chunk's first connection (trace ids)
     uint32_t req0;                // the batch index of the chunk's first request (req_first)
     uint32_t n;                   // connections

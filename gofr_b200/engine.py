@@ -558,14 +558,15 @@ def conn_respond_bound(table: Table, desc: np.ndarray, rec_off: np.ndarray) -> i
 
 def _serve_connections(self, buf: np.ndarray, buf_off: np.ndarray, date: bytes, trace_seed: int, pinned: bool = True,
                        req_cap: Optional[int] = None, out_cap: Optional[int] = None, log: Optional[ConnLog] = None,
-                       results=None):
+                       results=None, trace_key: Optional[np.ndarray] = None):
     """gofr_conn_batch_submit + wait: connection c's received bytes are buf[buf_off[c]:buf_off[c + 1]] (host memory).
     Returns ConnResponses.  The capacities default to conn_batch_bound; pinned puts the outputs in pinned memory (egress
     driven by the device), else in pageable numpy arrays.  With log (a ConnLog), gofr_conn_batch_submit_log: the result's
     .log holds the request-log lines, in the same kind of memory.  With results = (rec uint8, rec_off uint32[requests + 1]),
     gofr_conn_batch_respond: stage 2 after route_connections on the same buffers and seed, request k's data section is its
     closure's record rec[rec_off[k]:rec_off[k + 1]] where that is not empty; out_cap then defaults to the larger of
-    conn_batch_bound's and what the records need (conn_respond_bound over the requests the table's bound assumes)."""
+    conn_batch_bound's and what the records need (conn_respond_bound over the requests the table's bound assumes).  With
+    trace_key (uint64[n_conns]), gofr_conn_batch_respond_ex: connection c's ids come from trace_key[c], not (trace_seed, c)."""
     buf = np.ascontiguousarray(buf, dtype=np.uint8)
     off = np.ascontiguousarray(buf_off, dtype=np.uint32)
     n = len(off) - 1
@@ -593,7 +594,12 @@ def _serve_connections(self, buf: np.ndarray, buf_off: np.ndarray, date: bytes, 
                        consumed=consumed.ctypes.data, conn_status=status.ctypes.data, out_bytes=0)
     L = _abi.lib()
     t = C.c_uint64()
-    if results is not None and log is None:
+    keys = None if trace_key is None else np.ascontiguousarray(trace_key, dtype=np.uint64)
+    assert keys is None or len(keys) == n
+    if keys is not None and log is None:
+        _abi.check(L.gofr_conn_batch_respond_ex(self._e, C.byref(cb), keys.ctypes.data, None if rres is None else C.byref(rres),
+                                                C.byref(cr), None, C.byref(t)), "gofr_conn_batch_respond_ex")
+    elif results is not None and log is None:
         _abi.check(L.gofr_conn_batch_respond(self._e, C.byref(cb), C.byref(rres), C.byref(cr), None, C.byref(t)),
                    "gofr_conn_batch_respond")
     elif log is None:
@@ -612,7 +618,10 @@ def _serve_connections(self, buf: np.ndarray, buf_off: np.ndarray, date: bytes, 
         cl = _abi.ConnLog(remote=remote.ctypes.data, remote_off=roff.ctypes.data, start_unix_ns=start.ctypes.data,
                           log_unix_ns=log.log_unix_ns, tz_offset_s=log.tz_offset_s, line_cap=line_cap, out=lout.ctypes.data,
                           out_cap=lout_cap, log_off=log_off.ctypes.data, log_req=log_req.ctypes.data)
-        if results is not None:
+        if keys is not None:
+            _abi.check(L.gofr_conn_batch_respond_ex(self._e, C.byref(cb), keys.ctypes.data, None if rres is None else C.byref(rres),
+                                                    C.byref(cr), C.byref(cl), C.byref(t)), "gofr_conn_batch_respond_ex")
+        elif results is not None:
             _abi.check(L.gofr_conn_batch_respond(self._e, C.byref(cb), C.byref(rres), C.byref(cr), C.byref(cl), C.byref(t)),
                        "gofr_conn_batch_respond")
         else:

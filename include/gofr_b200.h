@@ -903,6 +903,14 @@ int gofr_conn_batch_respond(gofr_engine*, const gofr_conn_batch* in, const gofr_
                             gofr_conn_log* log, gofr_ticket* ticket);
 int gofr_conn_respond_bound(const gofr_table*, const gofr_req_desc* desc, uint32_t n_req, const uint32_t* rec_off,
                             uint64_t* out_cap);
+/* Stage 2 with the connections' trace keys given: trace_key[c] (n_conns entries) replaces x = splitmix64(trace_seed ^
+ * splitmix64(c)) in gofr_conn_batch_submit's id function for connection c, so request j of connection c gets bytes 0-7 =
+ * splitmix64(trace_key[c] + 2j), bytes 8-15 = splitmix64(trace_key[c] + 2j + 1).  That lets a stage 2 batch hold connections
+ * from different stage 1 batches, or in another order, and still answer each with the ids its stage 1 handed out (the
+ * closures' log lines and the X-Correlation-Id are the same bytes).  With trace_key == NULL it is gofr_conn_batch_respond;
+ * everything else is that call's contract. */
+int gofr_conn_batch_respond_ex(gofr_engine*, const gofr_conn_batch* in, const uint64_t* trace_key, const gofr_conn_results* res,
+                               gofr_conn_resp* out, gofr_conn_log* log, gofr_ticket* ticket);
 
 /* Batching front-end over gofr_conn_batch_submit_log: net/http runs one goroutine per connection (conn.serve looping
  * readRequest, pkg/gofr/httpServer.go:29-33), each holding only its own received bytes.  Any number of threads call
@@ -939,6 +947,77 @@ int gofr_conn_frontend_set_clock(gofr_conn_frontend*, int64_t unix_ns);
 int gofr_conn_frontend_stats(gofr_conn_frontend*, uint64_t* batches, uint64_t* conns, uint64_t* reruns);
 int gofr_conn_frontend_serve(gofr_conn_frontend*, const uint8_t* buf, uint32_t len, const uint8_t* remote, uint32_t remote_len,
                              int64_t start_unix_ns, gofr_conn_resp* out, gofr_conn_log* log);
+
+/* Batching front-end over the closure path (gofr_conn_batch_route → closures → gofr_conn_batch_respond_ex), one read of one
+ * connection per call, with the closures on the caller's thread: net/http's conn.serve runs the user's closure on the
+ * connection's goroutine (pkg/gofr/httpServer.go:29-33, handler.go:32-36).  A read takes two calls, each a blocking call
+ * that joins a batch of its own kind, batches closing and rotating as gofr_frontend_create's max_batch and max_wait_us say:
+ *   route    the read → its requests routed, parsed and, for routes that declared a bind schema, bound; and its trace key;
+ *   (the caller runs the closures of its status-0 requests and encodes their (data, err) as GOFR_H_RESULT records)
+ *   respond  the same read, its trace key and its records → its responses and log lines.
+ * Route batches and respond batches are independent: a respond batch holds connections from any route batches, and a
+ * connection's response never waits for another connection's closure (a closure may call back into the front-end).  The
+ * front-end holds nothing for a read between its two calls: a caller that routes and never responds costs nothing.
+ *
+ * route: what gofr_conn_batch_route returns for this connection as a batch of one, rebased to the caller's buffers:
+ *   out  desc[k], meta[k], vars[k * GOFR_MAX_PATH_VARS ..], req_at[k] (the request's first byte in buf), trace_ids[16k ..];
+ *        req_first[0..1] = {0, requests}, consumed[0], conn_status[0].  arena holds len + 80 bytes; desc[k].arena_off indexes
+ *        it, and each parsed form keeps the alignment gofr_conn_batch_route gives it (the forms are moved by a multiple of 16),
+ *        so (desc, trace_ids, arena) with arena_bytes = len + 80 is a valid gofr_req_batch.
+ *   bind (may be NULL) Context.Bind of every status-0 request whose route route_schema maps to a schema (done for the whole
+ *        batch with one gofr_batch_bind per schema): status[k] = GOFR_BIND_OK / ERROR / HOST, or 0xFFFFFFFF for a request
+ *        that was not bound; its row (GOFR_BIND_OK) or error text (GOFR_BIND_ERROR) is rows[row_off[k] .. row_off[k+1]).  A
+ *        row longer than its slot (8 bytes per schema field plus the body plus 256, rounded up to 16) is GOFR_BIND_HOST and
+ *        has no bytes.  rows_bytes is what the rows take; req_cap * (8 * fields + 272) + len always suffices.
+ *   *trace_key  splitmix64(trace_seed_b ^ splitmix64(slot)), the x of gofr_conn_batch_submit's id function for this read:
+ *        trace_seed_b = splitmix64(splitmix64(seed) + route batch number), batches numbered from 0, slot the read's place in
+ *        its route batch.  trace_ids are the ids of that key; hand it to respond.
+ * respond: what gofr_conn_frontend_serve returns for this read (out and log as there), with the records res spliced in as
+ *   gofr_conn_batch_respond splices them: res->n_req is the route call's request count and res->rec_off its n_req + 1 record
+ *   offsets into res->rec.  The ids are trace_key's, so each X-Correlation-Id and log line carries the id the route call
+ *   returned.  Date and log_unix_ns are the respond batch's (gofr_conn_app_frontend_set_clock pins them, in ns; 0 = wall
+ *   clock); start_unix_ns is this read's.
+ * Returns GOFR_OK; at once, without joining a batch, for len == 0 (conn_status DONE, no requests; respond wants n_req == 0);
+ * GOFR_ERR_CAPACITY before anything is queued when len > max_conn_bytes (hand the connection to net/http); GOFR_ERR_CAPACITY
+ * with req_first[1] (route), rows_bytes, out_bytes and the log's lines / out_bytes set to what the read needed when one of
+ * the caller's capacities is short (gofr_conn_batch_bound / gofr_conn_log_bound on {0, len} give capacities that always
+ * suffice); the batch call's own error for every caller of that batch; GOFR_ERR_INVALID for bad arguments and once destroy
+ * has started.  respond also returns GOFR_ERR_INVALID, before queuing, for records whose offsets decrease or pass rec_bytes,
+ * and, without failing its batch-mates, for records that do not match the read's requests (a wrong n_req, or bytes that
+ * changed the request count since the route call): such a batch is served once more without records to count each read's
+ * requests, and again without the offenders' records (stats: isolated).  A respond batch gathers its callers' records
+ * behind 32-bit offsets: a caller whose records, with those of the callers before it in the batch, would bring the batch's
+ * records plus its bytes plus 8 per possible request past 4 GiB gets GOFR_ERR_CAPACITY without failing the others (respond
+ * again; records that pass that alone are never served).
+ * One call per connection at a time.  Respond batches' outputs grow and are served again as gofr_conn_frontend's (stats:
+ * reruns).  create: route_schema[r] (n_routes entries, may be NULL when n_routes is 0) is the schema route r binds, 0 for
+ * none, and schema_fields[r] that schema's field count; refuses (GOFR_ERR_CAPACITY) a max_batch * max_conn_bytes beyond 32
+ * bits.  destroy may only be called when no thread is inside a route or respond call. */
+typedef struct gofr_conn_app_frontend gofr_conn_app_frontend;
+typedef struct gofr_conn_app_bind {
+    uint32_t* status;     /* req_cap */
+    uint32_t* row_off;    /* req_cap + 1 */
+    uint8_t* rows;
+    uint64_t rows_cap;
+    uint64_t rows_bytes;
+} gofr_conn_app_bind;
+typedef struct gofr_conn_app_stats {
+    uint64_t route_batches, route_reads, respond_batches, respond_reads;
+    uint64_t reruns;      /* respond batches served again after an output grew */
+    uint64_t isolated;    /* respond batches served once more to count their reads' requests */
+    uint64_t gather_ns;   /* the respond dispatcher's time gathering the callers' records */
+} gofr_conn_app_stats;
+int gofr_conn_app_frontend_create(gofr_conn_app_frontend** out, gofr_engine*, uint32_t max_batch, uint32_t max_wait_us,
+                                  uint32_t max_conn_bytes, int log, int32_t tz_offset_s, uint64_t seed, const uint32_t* route_schema,
+                                  uint32_t n_routes, const uint32_t* schema_fields);
+void gofr_conn_app_frontend_destroy(gofr_conn_app_frontend*);
+int gofr_conn_app_frontend_set_clock(gofr_conn_app_frontend*, int64_t unix_ns);
+int gofr_conn_app_frontend_stats(gofr_conn_app_frontend*, gofr_conn_app_stats* stats);
+int gofr_conn_app_frontend_route(gofr_conn_app_frontend*, const uint8_t* buf, uint32_t len, gofr_conn_route* out,
+                                 gofr_conn_app_bind* bind, uint64_t* trace_key);
+int gofr_conn_app_frontend_respond(gofr_conn_app_frontend*, const uint8_t* buf, uint32_t len, uint64_t trace_key,
+                                   const gofr_conn_results* res, const uint8_t* remote, uint32_t remote_len, int64_t start_unix_ns,
+                                   gofr_conn_resp* out, gofr_conn_log* log);
 
 /* number of kernels launched by this engine so far (bench.py reports it as gpu_launches) */
 uint64_t gofr_engine_launch_count(const gofr_engine*);

@@ -270,6 +270,7 @@ public:
 
     explicit App(uint32_t frame_mode = GOFR_FRAME_WIRE) { check(gofr_table_create(&table_, frame_mode), "gofr_table_create"); }
     ~App() {
+        gofr_conn_app_frontend_destroy(reads_);
         if (engine_) gofr_engine_destroy(engine_);
         if (table_) gofr_table_destroy(table_);
     }
@@ -495,17 +496,6 @@ public:
         rt.conn_status = cstat.data();
         check(gofr_conn_batch_route(engine_, &in, &rt), "gofr_conn_batch_route");
         const uint32_t n = req_first[nc];
-        auto bytes_at = [&](uint32_t off, uint32_t len) { return std::string((const char*)arena.data() + off, len); };
-        std::vector<Parsed> ps(n);
-        std::vector<Request> rq(n);
-        for (uint32_t i = 0; i < n; i++) {
-            const gofr_req_desc& d = desc[i];
-            ps[i].path = bytes_at(d.arena_off, d.path_len);
-            ps[i].query = bytes_at(d.arena_off + d.path_len, d.query_len);
-            ps[i].force_query = (d.flags & GOFR_REQ_FORCE_QUERY) != 0;
-            rq[i].method = method_name(d.method);
-            rq[i].body = bytes_at(d.arena_off + ((d.path_len + d.query_len + 3u) & ~3u), d.data_len);
-        }
         // ---- stage 1b (GPU): Context.Bind on the exported requests, per struct type ----
         std::vector<Bound> bound(n);
         for (auto& t : types_) {
@@ -535,14 +525,8 @@ public:
         }
         // ---- the closures (host), only where the reference would have called one ----
         std::string rec;
-        std::vector<uint32_t> rec_off(n + 1);
-        for (uint32_t i = 0; i < n; i++) {
-            rec_off[i] = (uint32_t)rec.size();
-            const uint32_t status = meta[i] & 0xFFFFu, route = meta[i] >> 16;
-            if (status == 0 && route < routes_.size()) rec += run_handler(routes_[route], rq[i], ps[i], &vars[(size_t)i * GOFR_MAX_PATH_VARS], bound[i]);
-            if (rec.size() > 0xFFFFFFF0u) throw std::invalid_argument("gofr::App::ServeConnections: more than 4 GiB of handler results");
-        }
-        rec_off[n] = (uint32_t)rec.size();
+        std::vector<uint32_t> rec_off;
+        run_closures(desc.data(), arena.data(), meta.data(), vars.data(), n, bound, &rec, &rec_off, "gofr::App::ServeConnections");
         // ---- stage 2 (GPU): the results spliced in, Responder.Respond + framing for every request ----
         uint64_t cap = 0;
         check(gofr_conn_respond_bound(table_, desc.data(), n, rec_off.data(), &cap), "gofr_conn_respond_bound");
@@ -566,6 +550,109 @@ public:
             out[c].conn_status = cstat[c];
         }
         return out;
+    }
+
+    // Starts the per-read entry ServeRead (after Run, before any ServeRead): a gofr_conn_app_frontend on this App's engine
+    // whose route batches bind the bodies of the routes registered with Binds, with max_batch / max_wait_us as
+    // gofr_frontend_create's, reads of at most max_conn_bytes, and middleware.Logging's lines when log is set.
+    void ServeReads(uint32_t max_batch = 1024, uint32_t max_wait_us = 200, uint32_t max_conn_bytes = 16384, uint64_t seed = 0,
+                    bool log = false, int32_t tz_offset_s = 0) {
+        if (!engine_) throw std::logic_error("gofr::App: call Run before ServeReads");
+        if (reads_) throw std::logic_error("gofr::App::ServeReads: already started");
+        std::vector<uint32_t> schema(routes_.size()), fields(routes_.size());
+        for (size_t r = 0; r < routes_.size(); r++) {
+            schema[r] = routes_[r].bind_type;
+            fields[r] = schema[r] ? (uint32_t)types_[schema[r] - 1]->fields_.size() : 0u;
+            max_fields_ = std::max(max_fields_, fields[r]);
+        }
+        check(gofr_conn_app_frontend_create(&reads_, engine_, max_batch, max_wait_us, max_conn_bytes, log ? 1 : 0, tz_offset_s, seed,
+                                            schema.data(), (uint32_t)schema.size(), fields.data()),
+              "gofr_conn_app_frontend_create");
+        reads_max_ = max_conn_bytes;
+        reads_log_ = log;
+    }
+    // pin the Date header and the log time of ServeRead's respond batches (tests); 0 = wall clock
+    void SetReadClock(int64_t unix_ns) { check(gofr_conn_app_frontend_set_clock(reads_, unix_ns), "gofr_conn_app_frontend_set_clock"); }
+    gofr_conn_app_stats ReadStats() const {
+        gofr_conn_app_stats st{};
+        check(gofr_conn_app_frontend_stats(reads_, &st), "gofr_conn_app_frontend_stats");
+        return st;
+    }
+
+    // What ServeRead hands back for one read: ServeConnections' ConnResponse for it, request k's response at bytes[out_off[k]
+    // .. out_off[k+1]), each request's trace id (the bytes of its X-Correlation-Id) and, with log, middleware.Logging's lines
+    // of the requests answered on the GPU.
+    struct ReadResponse : ConnResponse {
+        int rc = GOFR_OK;  // GOFR_ERR_CAPACITY: the read exceeds max_conn_bytes, nothing was queued (hand it to net/http)
+        std::vector<uint32_t> out_off{0};
+        std::vector<std::array<uint8_t, 16>> trace_ids;
+        std::string log;
+    };
+
+    // net/http's conn.serve for one read of one connection (the kept tail plus the new bytes), on the connection's own
+    // thread: the read is framed, parsed, routed and bound on the GPU with the other threads' reads (one route batch), the
+    // closures of its requests run here, on the calling thread, with the Context ServeConnections builds, and their results
+    // are spliced in and every request answered on the GPU (one respond batch, gofr_conn_batch_respond_ex under the trace
+    // key the route call returned).  Thread-safe: any number of threads, one call per connection at a time.  remote and
+    // start_unix_ns are Logging's req.RemoteAddr and start clock for this read.
+    ReadResponse ServeRead(const std::string& buf, const std::string& remote = std::string(), int64_t start_unix_ns = 0) const {
+        if (!reads_) throw std::logic_error("gofr::App: call ServeReads before ServeRead");
+        ReadResponse r;
+        if (buf.size() > reads_max_) { r.rc = GOFR_ERR_CAPACITY; return r; }
+        const uint32_t len = (uint32_t)buf.size(), off[2] = {0, len}, roff[2] = {0, (uint32_t)remote.size()};
+        uint32_t req_cap = 0;
+        uint64_t cap0 = 0;
+        check(gofr_conn_batch_bound(table_, off, 1, &req_cap, &cap0), "gofr_conn_batch_bound");
+        const size_t rc1 = std::max<uint32_t>(req_cap, 1);
+        // ---- route round: frame, parse, route and bind on the GPU ----
+        std::vector<gofr_req_desc> desc(rc1);
+        std::vector<uint8_t> arena((size_t)len + 80), ids(rc1 * 16);
+        std::vector<uint32_t> meta(rc1), vars(rc1 * GOFR_MAX_PATH_VARS), req_at(rc1), bstat(rc1), row_off(rc1 + 1);
+        std::vector<uint8_t> rows((size_t)req_cap * (8 * max_fields_ + 272) + len + 1);
+        uint32_t first[2] = {0, 0};
+        gofr_conn_route rt{};
+        rt.req_cap = req_cap; rt.desc = desc.data(); rt.arena = arena.data(); rt.meta = meta.data(); rt.vars = vars.data();
+        rt.req_at = req_at.data(); rt.trace_ids = ids.data(); rt.req_first = first; rt.consumed = &r.consumed; rt.conn_status = &r.conn_status;
+        gofr_conn_app_bind bd{bstat.data(), row_off.data(), rows.data(), rows.size(), 0};
+        uint64_t key = 0;
+        check(gofr_conn_app_frontend_route(reads_, (const uint8_t*)buf.data(), len, &rt, &bd, &key), "gofr_conn_app_frontend_route");
+        const uint32_t n = first[1];
+        std::vector<Bound> bound(n);
+        for (uint32_t i = 0; i < n; i++) {
+            bound[i].status = bstat[i];
+            bound[i].row.assign((const char*)rows.data() + row_off[i], row_off[i + 1] - row_off[i]);
+        }
+        // ---- the closures, on this thread ----
+        std::string rec;
+        std::vector<uint32_t> rec_off;
+        run_closures(desc.data(), arena.data(), meta.data(), vars.data(), n, bound, &rec, &rec_off, "gofr::App::ServeRead");
+        // ---- respond round: the results spliced in, every request answered on the GPU ----
+        uint64_t cap = 0;
+        check(gofr_conn_respond_bound(table_, desc.data(), n, rec_off.data(), &cap), "gofr_conn_respond_bound");
+        cap += 4096;
+        uint32_t line_cap = 0;
+        uint64_t log_cap = 0;
+        if (reads_log_) check(gofr_conn_log_bound(off, roff, 1, &line_cap, &log_cap), "gofr_conn_log_bound");
+        r.bytes.resize(cap);
+        r.trace_ids.resize(rc1);
+        r.log.resize(log_cap + 1);
+        r.out_off.resize(rc1 + 1);
+        std::vector<uint32_t> log_off(line_cap + 1), log_req(std::max<uint32_t>(line_cap, 1));
+        gofr_conn_results res{(const uint8_t*)rec.data(), rec_off.data(), rec.size(), n, 0};
+        gofr_conn_resp o{};
+        o.out = (uint8_t*)&r.bytes[0]; o.out_cap = cap; o.req_cap = req_cap; o.out_off = r.out_off.data(); o.meta = meta.data();
+        o.req_at = req_at.data(); o.trace_ids = r.trace_ids[0].data(); o.req_first = first; o.consumed = &r.consumed;
+        o.conn_status = &r.conn_status;
+        gofr_conn_log l{};
+        l.line_cap = line_cap; l.out = (uint8_t*)&r.log[0]; l.out_cap = log_cap; l.log_off = log_off.data(); l.log_req = log_req.data();
+        r.rc = gofr_conn_app_frontend_respond(reads_, (const uint8_t*)buf.data(), len, key, &res, (const uint8_t*)remote.data(),
+                                              (uint32_t)remote.size(), start_unix_ns, &o, reads_log_ ? &l : nullptr);
+        check(r.rc, "gofr_conn_app_frontend_respond");
+        r.bytes.resize(o.out_bytes);
+        r.trace_ids.resize(first[1]);
+        r.out_off.resize(first[1] + 1);
+        r.log.resize(reads_log_ ? l.out_bytes : 0);
+        return r;
     }
 
     // url.ParseRequestURI as Serve applies it to Request::target (tests): false for what httptest.NewRequest would refuse
@@ -630,6 +717,33 @@ private:
         }
         if (p.path.size() > 0xFFFF || p.query.size() > 0xFFFF) throw std::invalid_argument("gofr::App: request target too long");
         return p;
+    }
+
+    // handler.ServeHTTP for every request of a routed batch (desc into arena, meta / vars as gofr_route_device gives them,
+    // bound[i] its Context.Bind result), where the reference would call a closure: the request as net/http parsed it, the
+    // closure, and its (data, err) as the GOFR_H_RESULT record stage 2 splices in.  Record i is rec[rec_off[i] .. rec_off[i+1])
+    // (empty where no closure ran); ServeConnections and ServeRead share it.
+    void run_closures(const gofr_req_desc* desc, const uint8_t* arena, const uint32_t* meta, const uint32_t* vars, uint32_t n,
+                      const std::vector<Bound>& bound, std::string* rec, std::vector<uint32_t>* rec_off, const char* who) const {
+        rec_off->assign((size_t)n + 1, 0);
+        auto bytes_at = [&](uint32_t off, uint32_t len) { return std::string((const char*)arena + off, len); };
+        for (uint32_t i = 0; i < n; i++) {
+            (*rec_off)[i] = (uint32_t)rec->size();
+            const uint32_t status = meta[i] & 0xFFFFu, route = meta[i] >> 16;
+            if (status == 0 && route < routes_.size()) {
+                const gofr_req_desc& d = desc[i];
+                Parsed p;
+                p.path = bytes_at(d.arena_off, d.path_len);
+                p.query = bytes_at(d.arena_off + d.path_len, d.query_len);
+                p.force_query = (d.flags & GOFR_REQ_FORCE_QUERY) != 0;
+                Request rq;
+                rq.method = method_name(d.method);
+                rq.body = bytes_at(d.arena_off + ((d.path_len + d.query_len + 3u) & ~3u), d.data_len);
+                *rec += run_handler(routes_[route], rq, p, &vars[(size_t)i * GOFR_MAX_PATH_VARS], bound[i]);
+            }
+            if (rec->size() > 0xFFFFFFF0u) throw std::invalid_argument(std::string(who) + ": more than 4 GiB of handler results");
+        }
+        (*rec_off)[n] = (uint32_t)rec->size();
     }
 
     // handler.ServeHTTP (pkg/gofr/handler.go:32-36): build the Context, call the closure, describe (data, err) for Respond
@@ -859,6 +973,9 @@ private:
     std::vector<std::unique_ptr<StructType>> types_;
     std::vector<RouteInfo> routes_;
     std::mt19937_64 rng_{0x9E3779B97F4A7C15ull};
+    gofr_conn_app_frontend* reads_ = nullptr;  // ServeRead's front-end (ServeReads)
+    uint32_t reads_max_ = 0, max_fields_ = 0;
+    bool reads_log_ = false;
     friend class ProtoCodec;
 };
 
@@ -1011,8 +1128,8 @@ private:
 // request of a GOFR_H_HOST route (status 0 in meta) is a hole: the caller runs that route's closure and writes its response
 // at the hole's place.  On GOFR_HTTP_CONN_MORE keep buf[consumed ..] and append the next read; on GOFR_HTTP_CONN_DEFER write
 // the responses, then hand buf[consumed ..] to net/http.  Any number of threads may call one ConnFrontend, one call per
-// connection at a time.  The engine serves `table`; App's routes are GOFR_H_RESULT routes, which need their closures'
-// records (App::ServeConnections), so an App's table is not one to serve through this front-end.
+// connection at a time.  The engine serves `table`: fused routes and GOFR_H_HOST holes.  An App's routes are closures; serve
+// them one read at a time with App::ServeRead.
 class ConnFrontend {
 public:
     struct Read {
