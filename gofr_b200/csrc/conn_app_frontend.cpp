@@ -89,9 +89,6 @@ static bool grow_route(RouteStaging& r, uint32_t req_cap) {
     return ok;
 }
 
-// the row slot of a request bound for a schema of `fields` fields: its fixed words plus its body, and room for an error text
-static uint64_t row_slot(uint32_t fields, uint32_t data_len) { return (8ull * fields + data_len + 256 + 15) & ~15ull; }
-
 // the route dispatcher's step: batch k's n reads through gofr_conn_batch_route, then Context.Bind per schema
 static int route_batch(AppFrontend* f, int k, uint32_t n, uint32_t arena_bytes) {
     RouteStaging& r = f->rb[k];
@@ -115,8 +112,8 @@ static int route_batch(AppFrontend* f, int k, uint32_t n, uint32_t arena_bytes) 
     if (rc) return rc;
     const uint32_t nreq = x.req_first[n];
     for (uint32_t q = 0; q < nreq; q++) r.bstat[q] = kUnbound, r.blen[q] = 0, r.brow[q] = 0;
-    // Context.Bind for the batch: one gofr_batch_bind per schema over its routes' status-0 requests, rows in slots sized
-    // as App::ServeConnections sizes them
+    // Context.Bind for the batch: one gofr_batch_bind per schema over its routes' status-0 requests, rows in slots of
+    // GOFR_BIND_ROW_SLOT
     uint64_t at = 0;
     for (uint32_t s : f->schemas) {
         r.who.clear();
@@ -131,7 +128,7 @@ static int route_batch(AppFrontend* f, int k, uint32_t n, uint32_t arena_bytes) 
             longest = std::max(longest, r.desc[q].data_len);
         }
         if (r.who.empty()) continue;
-        const uint32_t slot = (uint32_t)row_slot(fields, longest);
+        const uint32_t slot = (uint32_t)GOFR_BIND_ROW_SLOT(fields, longest);
         const uint64_t need = at + (uint64_t)r.who.size() * slot;
         if (need > r.rows_cap) {
             // the rows of the schemas bound so far move along
@@ -151,7 +148,7 @@ static int route_batch(AppFrontend* f, int k, uint32_t n, uint32_t arena_bytes) 
         for (size_t j = 0; j < r.who.size(); j++) {
             const uint32_t q = r.who[j];
             // a row longer than its slot, or than this request's own slot, was not decided on the device
-            const bool host = len[j] > slot || len[j] > row_slot(fields, r.desc[q].data_len);
+            const bool host = len[j] > slot || len[j] > GOFR_BIND_ROW_SLOT(fields, r.desc[q].data_len);
             r.bstat[q] = host ? (uint32_t)GOFR_BIND_HOST : st[j];
             r.blen[q] = host ? 0 : len[j];
             r.brow[q] = at + (uint64_t)j * slot;

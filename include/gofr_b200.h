@@ -565,6 +565,10 @@ int gofr_proto_nested_bound(const gofr_proto_nmsg* msgs, uint32_t n_msgs, const 
  * d_len[i] = bytes of the result; a value above slot_bytes means it did not fit and nothing was written.
  * Pins: pkg/gofr/http/request_test.go:17-30, pkg/gofr/context_test.go:23-49. */
 enum { GOFR_BIND_OK = 0, GOFR_BIND_ERROR = 1, GOFR_BIND_HOST = 2 };
+/* The row slot gofr::App and gofr_conn_app_frontend bind a body of data_len bytes in, for a schema of `fields` fields: a
+ * row never exceeds its fixed words (at most 8 bytes per field) plus the body, and 256 bytes leave room for an error
+ * text; rounded up to 16 as slot_bytes must be.  64-bit. */
+#define GOFR_BIND_ROW_SLOT(fields, data_len) ((8 * (uint64_t)(fields) + (uint64_t)(data_len) + 256 + 15) & ~(uint64_t)15)
 int gofr_bind_device(gofr_engine* e, uint32_t schema_id, const gofr_req_desc* d_desc, const uint8_t* d_arena, uint32_t n,
                      uint8_t* d_rows, uint32_t slot_bytes, uint32_t* d_len, uint32_t* d_status, void* stream);
 /* The same stage with host buffers (what a host shim calls between gofr_batch_route and its closures); synchronous. */
@@ -967,8 +971,8 @@ int gofr_conn_frontend_serve(gofr_conn_frontend*, const uint8_t* buf, uint32_t l
  *   bind (may be NULL) Context.Bind of every status-0 request whose route route_schema maps to a schema (done for the whole
  *        batch with one gofr_batch_bind per schema): status[k] = GOFR_BIND_OK / ERROR / HOST, or 0xFFFFFFFF for a request
  *        that was not bound; its row (GOFR_BIND_OK) or error text (GOFR_BIND_ERROR) is rows[row_off[k] .. row_off[k+1]).  A
- *        row longer than its slot (8 bytes per schema field plus the body plus 256, rounded up to 16) is GOFR_BIND_HOST and
- *        has no bytes.  rows_bytes is what the rows take; req_cap * (8 * fields + 272) + len always suffices.
+ *        row longer than its slot (GOFR_BIND_ROW_SLOT of the schema's fields and the body) is GOFR_BIND_HOST and has no
+ *        bytes.  rows_bytes is what the rows take; req_cap * (8 * fields + 272) + len always suffices.
  *   *trace_key  splitmix64(trace_seed_b ^ splitmix64(slot)), the x of gofr_conn_batch_submit's id function for this read:
  *        trace_seed_b = splitmix64(splitmix64(seed) + route batch number), batches numbered from 0, slot the read's place in
  *        its route batch.  trace_ids are the ids of that key; hand it to respond.

@@ -351,22 +351,26 @@ public:
         const uint32_t n = (uint32_t)reqs.size();
         std::vector<Response> out(n);
         if (!n) return out;
-        // ---- stage 0: what net/http hands to the router: method, URL.Path (decoded), URL.RawQuery, body ----
-        std::vector<Parsed> ps(n);
+        // ---- stage 0: what net/http hands to the router, as a request batch: method, URL.Path (decoded) | URL.RawQuery,
+        // then the body ----
         std::vector<gofr_req_desc> desc(n);
         std::vector<uint8_t> ids((size_t)n * 16);
         std::string arena;
         for (uint32_t i = 0; i < n; i++) {
-            ps[i] = parse_target(reqs[i].target);
+            const Parsed p = parse_target(reqs[i].target);
             memset(&desc[i], 0, sizeof desc[i]);
             desc[i].arena_off = (uint32_t)arena.size();
-            desc[i].path_len = (uint16_t)ps[i].path.size();
-            desc[i].query_len = (uint16_t)ps[i].query.size();
+            desc[i].path_len = (uint16_t)p.path.size();
+            desc[i].query_len = (uint16_t)p.query.size();
+            desc[i].data_len = (uint32_t)reqs[i].body.size();
             desc[i].method = method_code(reqs[i].method);
-            desc[i].flags = ps[i].force_query ? GOFR_REQ_FORCE_QUERY : 0;
-            arena += ps[i].path;
-            arena += ps[i].query;
+            desc[i].flags = p.force_query ? GOFR_REQ_FORCE_QUERY : 0;
+            arena += p.path;
+            arena += p.query;
             arena.append((4 - arena.size() % 4) % 4, '\0');
+            arena += reqs[i].body;
+            arena.append((4 - arena.size() % 4) % 4, '\0');
+            if (arena.size() > 0xFFFFFFF0u) throw std::invalid_argument("gofr::App::Serve: more than 4 GiB of requests");
             if (reqs[i].trace_id) memcpy(&ids[(size_t)i * 16], reqs[i].trace_id->data(), 16);
             else for (int k = 0; k < 16; k += 8) { const uint64_t v = rng_(); memcpy(&ids[(size_t)i * 16 + k], &v, 8); }
         }
@@ -379,52 +383,19 @@ public:
         std::vector<uint32_t> meta(n), vars((size_t)n * GOFR_MAX_PATH_VARS);
         check(gofr_batch_route(engine_, &in, meta.data(), vars.data()), "gofr_batch_route");
         // ---- stage 1b (GPU): Context.Bind — json.Unmarshal of the bodies of the routes that declared a struct type ----
-        std::vector<Bound> bound(n);
-        for (auto& t : types_) {
-            std::vector<uint32_t> who;
-            for (uint32_t i = 0; i < n; i++) {
-                const uint32_t status = meta[i] & 0xFFFFu, route = meta[i] >> 16;
-                if (status == 0 && route < routes_.size() && routes_[route].bind_type == t->id_) who.push_back(i);
-            }
-            if (who.empty()) continue;
-            std::vector<gofr_req_desc> bd(who.size());
-            std::string ba;
-            size_t longest = 0;
-            for (size_t k = 0; k < who.size(); k++) {
-                const std::string& body = reqs[who[k]].body;
-                memset(&bd[k], 0, sizeof bd[k]);
-                bd[k].arena_off = (uint32_t)ba.size();
-                bd[k].data_len = (uint32_t)body.size();
-                ba += body;
-                ba.append((4 - ba.size() % 4) % 4, '\0');
-                longest = std::max(longest, body.size());
-            }
-            ba.append(64, '\0');
-            gofr_req_batch bin;
-            memset(&bin, 0, sizeof bin);
-            bin.desc = bd.data(); bin.arena = (const uint8_t*)ba.data(); bin.arena_bytes = ba.size(); bin.n = (uint32_t)who.size();
-            // a row is never longer than its fixed words plus the body; an error text is short
-            const uint32_t slot = (uint32_t)((8 * t->fields_.size() + longest + 256 + 15) & ~(size_t)15);
-            std::vector<uint8_t> rows((size_t)who.size() * slot);
-            std::vector<uint32_t> blen(who.size()), bstat(who.size());
-            check(gofr_batch_bind(engine_, t->id_, &bin, rows.data(), slot, blen.data(), bstat.data()), "gofr_batch_bind");
-            for (size_t k = 0; k < who.size(); k++) {
-                bound[who[k]].status = blen[k] > slot ? (uint32_t)GOFR_BIND_HOST : bstat[k];
-                bound[who[k]].row.assign((const char*)rows.data() + k * slot, std::min<uint32_t>(blen[k], slot));
-            }
-        }
+        const std::vector<Bound> bound = bind_batch(desc.data(), (const uint8_t*)arena.data(), arena.size(), meta.data(), n);
         // ---- the closures (host), only where the reference would have called one ----
+        std::string rec;
+        std::vector<uint32_t> rec_off;
+        run_closures(desc.data(), (const uint8_t*)arena.data(), meta.data(), vars.data(), n, bound, &rec, &rec_off, "gofr::App::Serve");
         std::string arena2;
         for (uint32_t i = 0; i < n; i++) {
-            std::string record;
-            const uint32_t status = meta[i] & 0xFFFFu, route = meta[i] >> 16;
-            if (status == 0 && route < routes_.size()) record = run_handler(routes_[route], reqs[i], ps[i], &vars[(size_t)i * GOFR_MAX_PATH_VARS], bound[i]);
+            const uint32_t at = desc[i].arena_off;
             desc[i].arena_off = (uint32_t)arena2.size();
-            desc[i].data_len = (uint32_t)record.size();
-            arena2 += ps[i].path;
-            arena2 += ps[i].query;
+            desc[i].data_len = rec_off[i + 1] - rec_off[i];
+            arena2.append(arena, at, (size_t)desc[i].path_len + desc[i].query_len);
             arena2.append((4 - arena2.size() % 4) % 4, '\0');
-            arena2 += record;
+            arena2.append(rec, rec_off[i], desc[i].data_len);
             arena2.append((4 - arena2.size() % 4) % 4, '\0');
         }
         arena2.append(64, '\0');
@@ -442,7 +413,7 @@ public:
         check(gofr_batch_submit(engine_, &in, &rb, &t), "gofr_batch_submit");
         check(gofr_batch_wait(engine_, t), "gofr_batch_wait");
         for (uint32_t i = 0; i < n; i++) {
-            out[i].status = (int)(meta2[i] & 0xFFFFu);
+            out[i].status = (int)GOFR_META_STATUS(meta2[i]);
             out[i].bytes.assign((const char*)bytes.data() + off[i], off[i + 1] - off[i]);
         }
         return out;
@@ -496,33 +467,8 @@ public:
         rt.conn_status = cstat.data();
         check(gofr_conn_batch_route(engine_, &in, &rt), "gofr_conn_batch_route");
         const uint32_t n = req_first[nc];
-        // ---- stage 1b (GPU): Context.Bind on the exported requests, per struct type ----
-        std::vector<Bound> bound(n);
-        for (auto& t : types_) {
-            std::vector<uint32_t> who;
-            for (uint32_t i = 0; i < n; i++) {
-                const uint32_t status = meta[i] & 0xFFFFu, route = meta[i] >> 16;
-                if (status == 0 && route < routes_.size() && routes_[route].bind_type == t->id_) who.push_back(i);
-            }
-            if (who.empty()) continue;
-            std::vector<gofr_req_desc> bd(who.size());
-            size_t longest = 0;
-            for (size_t k = 0; k < who.size(); k++) {
-                bd[k] = desc[who[k]];
-                longest = std::max<size_t>(longest, bd[k].data_len);
-            }
-            gofr_req_batch bin;
-            memset(&bin, 0, sizeof bin);
-            bin.desc = bd.data(); bin.arena = arena.data(); bin.arena_bytes = arena.size(); bin.n = (uint32_t)who.size();
-            const uint32_t slot = (uint32_t)((8 * t->fields_.size() + longest + 256 + 15) & ~(size_t)15);
-            std::vector<uint8_t> rows((size_t)who.size() * slot);
-            std::vector<uint32_t> blen(who.size()), bstat(who.size());
-            check(gofr_batch_bind(engine_, t->id_, &bin, rows.data(), slot, blen.data(), bstat.data()), "gofr_batch_bind");
-            for (size_t k = 0; k < who.size(); k++) {
-                bound[who[k]].status = blen[k] > slot ? (uint32_t)GOFR_BIND_HOST : bstat[k];
-                bound[who[k]].row.assign((const char*)rows.data() + k * slot, std::min<uint32_t>(blen[k], slot));
-            }
-        }
+        // ---- stage 1b (GPU): Context.Bind on the exported requests ----
+        const std::vector<Bound> bound = bind_batch(desc.data(), arena.data(), arena.size(), meta.data(), n);
         // ---- the closures (host), only where the reference would have called one ----
         std::string rec;
         std::vector<uint32_t> rec_off;
@@ -719,35 +665,58 @@ private:
         return p;
     }
 
+    // Context.Bind for every request of a routed batch (desc into arena, meta as gofr_route_device gives it) whose route
+    // declared a struct type: one gofr_batch_bind per type, rows in slots of GOFR_BIND_ROW_SLOT for the type's fields and
+    // the longest of those bodies.  bound[i].status stays 0xFFFFFFFF for a request that was not bound.
+    std::vector<Bound> bind_batch(const gofr_req_desc* desc, const uint8_t* arena, uint64_t arena_bytes, const uint32_t* meta, uint32_t n) const {
+        std::vector<Bound> bound(n);
+        for (auto& t : types_) {
+            std::vector<uint32_t> who;
+            std::vector<gofr_req_desc> bd;
+            uint32_t longest = 0;
+            for (uint32_t i = 0; i < n; i++) {
+                const uint32_t route = GOFR_META_ROUTE(meta[i]);
+                if (GOFR_META_STATUS(meta[i]) || route >= routes_.size() || routes_[route].bind_type != t->id_) continue;
+                who.push_back(i);
+                bd.push_back(desc[i]);
+                longest = std::max(longest, desc[i].data_len);
+            }
+            if (who.empty()) continue;
+            gofr_req_batch bin;
+            memset(&bin, 0, sizeof bin);
+            bin.desc = bd.data(); bin.arena = arena; bin.arena_bytes = arena_bytes; bin.n = (uint32_t)who.size();
+            const uint32_t slot = (uint32_t)GOFR_BIND_ROW_SLOT(t->fields_.size(), longest);
+            std::vector<uint8_t> rows((size_t)who.size() * slot);
+            std::vector<uint32_t> blen(who.size()), bstat(who.size());
+            check(gofr_batch_bind(engine_, t->id_, &bin, rows.data(), slot, blen.data(), bstat.data()), "gofr_batch_bind");
+            for (size_t k = 0; k < who.size(); k++) {
+                bound[who[k]].status = blen[k] > slot ? (uint32_t)GOFR_BIND_HOST : bstat[k];
+                bound[who[k]].row.assign((const char*)rows.data() + k * slot, std::min<uint32_t>(blen[k], slot));
+            }
+        }
+        return bound;
+    }
+
     // handler.ServeHTTP for every request of a routed batch (desc into arena, meta / vars as gofr_route_device gives them,
     // bound[i] its Context.Bind result), where the reference would call a closure: the request as net/http parsed it, the
     // closure, and its (data, err) as the GOFR_H_RESULT record stage 2 splices in.  Record i is rec[rec_off[i] .. rec_off[i+1])
-    // (empty where no closure ran); ServeConnections and ServeRead share it.
+    // (empty where no closure ran).
     void run_closures(const gofr_req_desc* desc, const uint8_t* arena, const uint32_t* meta, const uint32_t* vars, uint32_t n,
                       const std::vector<Bound>& bound, std::string* rec, std::vector<uint32_t>* rec_off, const char* who) const {
         rec_off->assign((size_t)n + 1, 0);
-        auto bytes_at = [&](uint32_t off, uint32_t len) { return std::string((const char*)arena + off, len); };
         for (uint32_t i = 0; i < n; i++) {
             (*rec_off)[i] = (uint32_t)rec->size();
-            const uint32_t status = meta[i] & 0xFFFFu, route = meta[i] >> 16;
-            if (status == 0 && route < routes_.size()) {
-                const gofr_req_desc& d = desc[i];
-                Parsed p;
-                p.path = bytes_at(d.arena_off, d.path_len);
-                p.query = bytes_at(d.arena_off + d.path_len, d.query_len);
-                p.force_query = (d.flags & GOFR_REQ_FORCE_QUERY) != 0;
-                Request rq;
-                rq.method = method_name(d.method);
-                rq.body = bytes_at(d.arena_off + ((d.path_len + d.query_len + 3u) & ~3u), d.data_len);
-                *rec += run_handler(routes_[route], rq, p, &vars[(size_t)i * GOFR_MAX_PATH_VARS], bound[i]);
-            }
+            const uint32_t route = GOFR_META_ROUTE(meta[i]);
+            if (GOFR_META_STATUS(meta[i]) == 0 && route < routes_.size())
+                *rec += run_handler(routes_[route], desc[i], arena, &vars[(size_t)i * GOFR_MAX_PATH_VARS], bound[i]);
             if (rec->size() > 0xFFFFFFF0u) throw std::invalid_argument(std::string(who) + ": more than 4 GiB of handler results");
         }
         (*rec_off)[n] = (uint32_t)rec->size();
     }
 
-    // handler.ServeHTTP (pkg/gofr/handler.go:32-36): build the Context, call the closure, describe (data, err) for Respond
-    std::string run_handler(const RouteInfo& r, const Request& rq, const Parsed& p, const uint32_t* vars, const Bound& bound) const {
+    // handler.ServeHTTP (pkg/gofr/handler.go:32-36): build the Context from request d (path | query, then the body, in
+    // arena), call the closure, describe (data, err) for Respond
+    std::string run_handler(const RouteInfo& r, const gofr_req_desc& d, const uint8_t* arena, const uint32_t* vars, const Bound& bound) const {
         Context c;
         if (r.bind_type) {
             c.bind_status_ = bound.status;
@@ -756,13 +725,14 @@ private:
             if (bound.status == GOFR_BIND_HOST) c.bind_status_ = GOFR_BIND_ERROR;
             for (auto& ty : types_) if (ty->id_ == r.bind_type) for (auto& f : ty->fields_) c.bind_kinds_.push_back(f.kind);
         }
-        c.method_ = rq.method;
-        c.path_ = p.path;
-        c.query_ = p.query;
-        c.body_ = rq.body;
+        const char* at = (const char*)arena + d.arena_off;
+        c.method_ = method_name(d.method);
+        c.path_.assign(at, d.path_len);
+        c.query_.assign(at + d.path_len, d.query_len);
+        c.body_.assign(at + ((d.path_len + d.query_len + 3u) & ~3u), d.data_len);
         for (size_t k = 0; k < r.var_names.size() && k < GOFR_MAX_PATH_VARS; k++) {
             if (vars[k] == 0xFFFFFFFFu) continue;
-            c.path_params_.emplace_back(r.var_names[k], p.path.substr(vars[k] & 0xFFFFu, vars[k] >> 16));
+            c.path_params_.emplace_back(r.var_names[k], c.path_.substr(vars[k] & 0xFFFFu, vars[k] >> 16));
         }
         Result res;
         try {
