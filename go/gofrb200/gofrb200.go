@@ -1001,7 +1001,7 @@ func (f *ConnAppFrontend) Route(buf []byte) (*ConnAppRoute, error) {
 	reqCap := len(buf)/16 + 1 // the framer's most for one connection
 	r := &ConnAppRoute{Desc: make([]C.gofr_req_desc, reqCap), Arena: make([]byte, len(buf)+80), Meta: make([]uint32, reqCap),
 		Vars: make([]uint32, reqCap*C.GOFR_MAX_PATH_VARS), ReqAt: make([]uint32, reqCap), TraceIDs: make([]byte, 16*reqCap),
-		BindStatus: make([]uint32, reqCap), RowOff: make([]uint32, reqCap+1), Rows: make([]byte, reqCap*(8*f.maxFields+272)+len(buf))}
+		BindStatus: make([]uint32, reqCap), RowOff: make([]uint32, reqCap+1)}
 	var first [2]C.uint32_t
 	var rt C.gofr_conn_route
 	rt.req_cap = C.uint32_t(reqCap)
@@ -1017,11 +1017,22 @@ func (f *ConnAppFrontend) Route(buf []byte) (*ConnAppRoute, error) {
 	var bd C.gofr_conn_app_bind
 	bd.status = (*C.uint32_t)(unsafe.Pointer(&r.BindStatus[0]))
 	bd.row_off = (*C.uint32_t)(unsafe.Pointer(&r.RowOff[0]))
-	bd.rows = (*C.uint8_t)(unsafe.Pointer(&r.Rows[0]))
-	bd.rows_cap = C.uint64_t(len(r.Rows))
 	var key C.uint64_t
-	if err := check(C.gofr_conn_app_frontend_route(f.f, bytesPtr(buf), C.uint32_t(len(buf)), &rt, &bd, &key), "gofr_conn_app_frontend_route"); err != nil {
-		return nil, err
+	// GOFR_BIND_ROW_BOUND without the schemas' names, which are not known here: a read whose error texts need more is
+	// routed again with the rows it reported
+	rowsCap := reqCap*(8*f.maxFields+70) + 3*len(buf)
+	for {
+		r.Rows = make([]byte, rowsCap)
+		bd.rows = (*C.uint8_t)(unsafe.Pointer(&r.Rows[0]))
+		bd.rows_cap = C.uint64_t(len(r.Rows))
+		rc := C.gofr_conn_app_frontend_route(f.f, bytesPtr(buf), C.uint32_t(len(buf)), &rt, &bd, &key)
+		if rc != C.GOFR_ERR_CAPACITY || int(bd.rows_bytes) <= rowsCap {
+			if err := check(rc, "gofr_conn_app_frontend_route"); err != nil {
+				return nil, err
+			}
+			break
+		}
+		rowsCap = int(bd.rows_bytes)
 	}
 	n := int(first[1])
 	r.Desc, r.Meta, r.Vars, r.ReqAt = r.Desc[:n], r.Meta[:n], r.Vars[:n*C.GOFR_MAX_PATH_VARS], r.ReqAt[:n]

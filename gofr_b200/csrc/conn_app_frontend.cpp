@@ -115,6 +115,16 @@ static int route_batch(AppFrontend* f, int k, uint32_t n, uint32_t arena_bytes) 
     // Context.Bind for the batch: one gofr_batch_bind per schema over its routes' status-0 requests, rows in slots of
     // GOFR_BIND_ROW_SLOT
     uint64_t at = 0;
+    auto reserve = [&](uint64_t need) {  // rows holds `need` bytes; the rows of the binds so far move along
+        if (need <= r.rows_cap) return true;
+        uint8_t* grown = (uint8_t*)gofr_alloc_pinned((size_t)need + (need >> 2));
+        if (!grown) { set_last_error("gofr_conn_app_frontend: no pinned rows of %llu bytes", (unsigned long long)need); return false; }
+        if (at) memcpy(grown, r.rows, (size_t)at);
+        gofr_free_pinned(r.rows);
+        r.rows = grown;
+        r.rows_cap = need + (need >> 2);
+        return true;
+    };
     for (uint32_t s : f->schemas) {
         r.who.clear();
         r.bd.clear();
@@ -129,31 +139,41 @@ static int route_batch(AppFrontend* f, int k, uint32_t n, uint32_t arena_bytes) 
         }
         if (r.who.empty()) continue;
         const uint32_t slot = (uint32_t)GOFR_BIND_ROW_SLOT(fields, longest);
-        const uint64_t need = at + (uint64_t)r.who.size() * slot;
-        if (need > r.rows_cap) {
-            // the rows of the schemas bound so far move along
-            uint8_t* grown = (uint8_t*)gofr_alloc_pinned((size_t)need + (need >> 2));
-            if (!grown) { set_last_error("gofr_conn_app_frontend: no pinned rows of %llu bytes", (unsigned long long)need); return GOFR_ERR_NOMEM; }
-            if (at) memcpy(grown, r.rows, (size_t)at);
-            gofr_free_pinned(r.rows);
-            r.rows = grown;
-            r.rows_cap = need + (need >> 2);
-        }
+        if (!reserve(at + (uint64_t)r.who.size() * slot)) return GOFR_ERR_NOMEM;
         gofr_req_batch b;
         memset(&b, 0, sizeof b);
         b.desc = r.bd.data(); b.arena = r.parsed; b.arena_bytes = (uint64_t)arena_bytes + 64; b.n = (uint32_t)r.who.size();
         std::vector<uint32_t> len(r.who.size()), st(r.who.size());
         rc = gofr_batch_bind(f->eng, s, &b, r.rows + at, slot, len.data(), st.data());
         if (rc) return rc;
+        std::vector<uint32_t> over;  // rows the slot did not hold: the bind reported their exact length
+        uint32_t wide = 0;
         for (size_t j = 0; j < r.who.size(); j++) {
             const uint32_t q = r.who[j];
-            // a row longer than its slot, or than this request's own slot, was not decided on the device
-            const bool host = len[j] > slot || len[j] > GOFR_BIND_ROW_SLOT(fields, r.desc[q].data_len);
-            r.bstat[q] = host ? (uint32_t)GOFR_BIND_HOST : st[j];
-            r.blen[q] = host ? 0 : len[j];
+            r.bstat[q] = st[j];
+            r.blen[q] = len[j];
             r.brow[q] = at + (uint64_t)j * slot;
+            if (len[j] > slot && st[j] != GOFR_BIND_HOST) { over.push_back(q); wide = std::max(wide, len[j]); }
         }
-        at = need;
+        at += (uint64_t)r.who.size() * slot;
+        if (over.empty()) continue;
+        // invalid UTF-8 triples a string, a long literal or name lengthens an error text: bind those requests once more in
+        // slots of the longest
+        const uint32_t slot2 = (wide + 15u) & ~15u;
+        if (!reserve(at + (uint64_t)over.size() * slot2)) return GOFR_ERR_NOMEM;
+        r.bd.clear();
+        for (uint32_t q : over) r.bd.push_back(r.desc[q]);
+        b.desc = r.bd.data(); b.n = (uint32_t)over.size();
+        rc = gofr_batch_bind(f->eng, s, &b, r.rows + at, slot2, len.data(), st.data());
+        if (rc) return rc;
+        for (size_t j = 0; j < over.size(); j++) {
+            // a bind that reports exact lengths always fits here; a row that does not is left to the host, alone
+            const bool host = len[j] > slot2;
+            r.bstat[over[j]] = host ? (uint32_t)GOFR_BIND_HOST : st[j];
+            r.blen[over[j]] = host ? 0 : len[j];
+            r.brow[over[j]] = at + (uint64_t)j * slot2;
+        }
+        at += (uint64_t)over.size() * slot2;
     }
     return GOFR_OK;
 }

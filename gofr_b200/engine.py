@@ -404,12 +404,14 @@ class Engine:
                                                       meta.data_ptr(), st.cuda_stream), "gofr_serve_device_slots")
         return out, out_len[:b.n], meta[:b.n]
 
-    def bind_device(self, b: DeviceBatch, schema_id: int, slot_bytes: int, stream=None):
-        """gofr_bind_device: Context.Bind for host closures.  Returns (rows uint8[n * slot_bytes], len int32[n], status int32[n])."""
+    def bind_device(self, b: DeviceBatch, schema_id: int, slot_bytes: int, stream=None, rows=None):
+        """gofr_bind_device: Context.Bind for host closures.  Returns (rows uint8[n * slot_bytes], len int32[n], status int32[n]);
+        pass rows to pre-fill them."""
         import torch
         dev = torch.device("cuda", self.device)
         st = stream if stream is not None else torch.cuda.current_stream(self.device)
-        rows = torch.zeros(max(b.n, 1) * slot_bytes, dtype=torch.uint8, device=dev)
+        if rows is None:
+            rows = torch.zeros(max(b.n, 1) * slot_bytes, dtype=torch.uint8, device=dev)
         ln = torch.zeros(max(b.n, 1), dtype=torch.int32, device=dev)
         status = torch.zeros(max(b.n, 1), dtype=torch.int32, device=dev)
         _abi.check(_abi.lib().gofr_bind_device(self._e, schema_id, b.desc.data_ptr(), b.arena.data_ptr(), b.n, rows.data_ptr(),

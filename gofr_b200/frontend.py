@@ -240,15 +240,22 @@ class ConnAppFrontend:
         desc, arena = np.zeros(rc1, S.DESC_DTYPE), np.zeros(len(buf) + 80, np.uint8)
         meta, vars_, req_at, ids = np.zeros(rc1, np.uint32), np.zeros(rc1 * 8, np.uint32), np.zeros(rc1, np.uint32), np.zeros(rc1 * 16, np.uint8)
         req_first, consumed, status = np.zeros(2, np.uint32), np.zeros(1, np.uint32), np.zeros(1, np.uint32)
-        rows_cap = req_cap * (8 * self.max_fields + 272) + len(buf)
-        bstat, row_off, rows = np.zeros(rc1, np.uint32), np.zeros(rc1 + 1, np.uint32), np.zeros(max(rows_cap, 1), np.uint8)
+        # GOFR_BIND_ROW_BOUND without the schemas' names, which this wrapper does not know: a read whose error texts need
+        # more is routed again with the rows it reported
+        rows_cap = req_cap * (8 * self.max_fields + 70) + 3 * len(buf)
+        bstat, row_off = np.zeros(rc1, np.uint32), np.zeros(rc1 + 1, np.uint32)
         cr = _abi.ConnRoute(req_cap=req_cap, desc=desc.ctypes.data, arena=arena.ctypes.data, meta=meta.ctypes.data,
                             vars=vars_.ctypes.data, req_at=req_at.ctypes.data, trace_ids=ids.ctypes.data,
                             req_first=req_first.ctypes.data, consumed=consumed.ctypes.data, conn_status=status.ctypes.data)
-        cb = _abi.ConnAppBind(status=bstat.ctypes.data, row_off=row_off.ctypes.data, rows=rows.ctypes.data, rows_cap=rows_cap)
         key = C.c_uint64()
-        _abi.check(_abi.lib().gofr_conn_app_frontend_route(self._f, buf, len(buf), C.byref(cr), C.byref(cb), C.byref(key)),
-                   "gofr_conn_app_frontend_route")
+        while True:
+            rows = np.zeros(max(rows_cap, 1), np.uint8)
+            cb = _abi.ConnAppBind(status=bstat.ctypes.data, row_off=row_off.ctypes.data, rows=rows.ctypes.data, rows_cap=rows_cap)
+            rc = _abi.lib().gofr_conn_app_frontend_route(self._f, buf, len(buf), C.byref(cr), C.byref(cb), C.byref(key))
+            if rc != 7 or cb.rows_bytes <= rows_cap:   # GOFR_ERR_CAPACITY for anything else: the read is too long
+                break
+            rows_cap = int(cb.rows_bytes)
+        _abi.check(rc, "gofr_conn_app_frontend_route")
         k = int(req_first[1])
         r = ConnRoute(desc[:k], arena, meta[:k], vars_[:k * 8].reshape(k, 8), req_at[:k], ids[:k * 16].reshape(k, 16), req_first,
                       consumed, status)

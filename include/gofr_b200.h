@@ -562,13 +562,22 @@ int gofr_proto_nested_bound(const gofr_proto_nmsg* msgs, uint32_t n_msgs, const 
  *                                  leaves behind in that case is not reported
  *   d_status[i] = GOFR_BIND_HOST   not decided on the device (nesting deeper than 64, or a number for a float64 member that
  *                                  is one of the rare literals left to Go's slow path — see GOFR_H_BIND_ECHO): run encoding/json on the host
- * d_len[i] = bytes of the result; a value above slot_bytes means it did not fit and nothing was written.
+ * d_len[i] = bytes of the result; a value above slot_bytes means it did not fit and nothing was written (bind it again in a
+ * slot of at least d_len[i] bytes).
  * Pins: pkg/gofr/http/request_test.go:17-30, pkg/gofr/context_test.go:23-49. */
 enum { GOFR_BIND_OK = 0, GOFR_BIND_ERROR = 1, GOFR_BIND_HOST = 2 };
-/* The row slot gofr::App and gofr_conn_app_frontend bind a body of data_len bytes in, for a schema of `fields` fields: a
- * row never exceeds its fixed words (at most 8 bytes per field) plus the body, and 256 bytes leave room for an error
- * text; rounded up to 16 as slot_bytes must be.  64-bit. */
+/* The first row slot gofr::App and gofr_conn_app_frontend bind a body of data_len bytes in, for a schema of `fields`
+ * fields: the fixed words (at most 8 bytes per field) plus the body, and 256 bytes for an error text; rounded up to 16 as
+ * slot_bytes must be.  It holds the rows of ordinary bodies; those it does not hold are bound again in a wider slot.  64-bit. */
 #define GOFR_BIND_ROW_SLOT(fields, data_len) ((8 * (uint64_t)(fields) + (uint64_t)(data_len) + 256 + 15) & ~(uint64_t)15)
+/* What a row or error text of a body of data_len bytes can take at most, for a schema of `fields` fields whose Go type
+ * name and longest JSON name take `names` bytes together.  A row is its fixed words (at most 8 bytes per field) and its
+ * decoded strings: those come from disjoint pieces of the body, and no body byte yields more than 3 bytes (an invalid
+ * UTF-8 byte becomes U+FFFD, EF BF BD; a valid sequence keeps its length; \uXXXX gives at most 3 bytes for 6, a surrogate
+ * pair 4 for 12, the other escapes 1 for 2).  An error text takes at most 70 bytes besides a number literal (a piece of
+ * the body) and the names: a syntax error ("invalid character '\u00XX' " and the longest scanner context) 69, "json:
+ * cannot unmarshal number <literal> into Go struct field <T>.<name> of type float64" 69.  64-bit. */
+#define GOFR_BIND_ROW_BOUND(fields, names, data_len) (8 * (uint64_t)(fields) + 3 * (uint64_t)(data_len) + 70 + (uint64_t)(names))
 int gofr_bind_device(gofr_engine* e, uint32_t schema_id, const gofr_req_desc* d_desc, const uint8_t* d_arena, uint32_t n,
                      uint8_t* d_rows, uint32_t slot_bytes, uint32_t* d_len, uint32_t* d_status, void* stream);
 /* The same stage with host buffers (what a host shim calls between gofr_batch_route and its closures); synchronous. */
@@ -970,9 +979,11 @@ int gofr_conn_frontend_serve(gofr_conn_frontend*, const uint8_t* buf, uint32_t l
  *        so (desc, trace_ids, arena) with arena_bytes = len + 80 is a valid gofr_req_batch.
  *   bind (may be NULL) Context.Bind of every status-0 request whose route route_schema maps to a schema (done for the whole
  *        batch with one gofr_batch_bind per schema): status[k] = GOFR_BIND_OK / ERROR / HOST, or 0xFFFFFFFF for a request
- *        that was not bound; its row (GOFR_BIND_OK) or error text (GOFR_BIND_ERROR) is rows[row_off[k] .. row_off[k+1]).  A
- *        row longer than its slot (GOFR_BIND_ROW_SLOT of the schema's fields and the body) is GOFR_BIND_HOST and has no
- *        bytes.  rows_bytes is what the rows take; req_cap * (8 * fields + 272) + len always suffices.
+ *        that was not bound; its row (GOFR_BIND_OK) or error text (GOFR_BIND_ERROR) is rows[row_off[k] .. row_off[k+1]).
+ *        A row longer than its first slot is bound again in a slot of the length reported for it (a row that would not fit
+ *        even that one comes back GOFR_BIND_HOST with no bytes; gofr_batch_bind reports exact lengths, so it never does).
+ *        rows_bytes is what the rows take; GOFR_BIND_ROW_BOUND summed over the requests always suffices, and so does
+ *        req_cap * (8 * fields + 70 + names) + 3 * len, with fields and names those of the widest schema.
  *   *trace_key  splitmix64(trace_seed_b ^ splitmix64(slot)), the x of gofr_conn_batch_submit's id function for this read:
  *        trace_seed_b = splitmix64(splitmix64(seed) + route batch number), batches numbered from 0, slot the read's place in
  *        its route batch.  trace_ids are the ids of that key; hand it to respond.

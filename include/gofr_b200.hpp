@@ -510,6 +510,11 @@ public:
             schema[r] = routes_[r].bind_type;
             fields[r] = schema[r] ? (uint32_t)types_[schema[r] - 1]->fields_.size() : 0u;
             max_fields_ = std::max(max_fields_, fields[r]);
+            if (!schema[r]) continue;
+            const StructType& t = *types_[schema[r] - 1];
+            size_t name = 0;
+            for (auto& f : t.fields_) name = std::max(name, (f.json.empty() ? f.go : f.json).size());
+            max_names_ = std::max<uint64_t>(max_names_, t.go_type_.size() + name);
         }
         check(gofr_conn_app_frontend_create(&reads_, engine_, max_batch, max_wait_us, max_conn_bytes, log ? 1 : 0, tz_offset_s, seed,
                                             schema.data(), (uint32_t)schema.size(), fields.data()),
@@ -554,7 +559,7 @@ public:
         std::vector<gofr_req_desc> desc(rc1);
         std::vector<uint8_t> arena((size_t)len + 80), ids(rc1 * 16);
         std::vector<uint32_t> meta(rc1), vars(rc1 * GOFR_MAX_PATH_VARS), req_at(rc1), bstat(rc1), row_off(rc1 + 1);
-        std::vector<uint8_t> rows((size_t)req_cap * (8 * max_fields_ + 272) + len + 1);
+        std::vector<uint8_t> rows((size_t)req_cap * (8 * max_fields_ + 70 + max_names_) + 3 * (size_t)len + 1);  // GOFR_BIND_ROW_BOUND over the read
         uint32_t first[2] = {0, 0};
         gofr_conn_route rt{};
         rt.req_cap = req_cap; rt.desc = desc.data(); rt.arena = arena.data(); rt.meta = meta.data(); rt.vars = vars.data();
@@ -667,7 +672,8 @@ private:
 
     // Context.Bind for every request of a routed batch (desc into arena, meta as gofr_route_device gives it) whose route
     // declared a struct type: one gofr_batch_bind per type, rows in slots of GOFR_BIND_ROW_SLOT for the type's fields and
-    // the longest of those bodies.  bound[i].status stays 0xFFFFFFFF for a request that was not bound.
+    // the longest of those bodies, and one more for the rows that outgrew it.  bound[i].status stays 0xFFFFFFFF for a
+    // request that was not bound.
     std::vector<Bound> bind_batch(const gofr_req_desc* desc, const uint8_t* arena, uint64_t arena_bytes, const uint32_t* meta, uint32_t n) const {
         std::vector<Bound> bound(n);
         for (auto& t : types_) {
@@ -689,9 +695,26 @@ private:
             std::vector<uint8_t> rows((size_t)who.size() * slot);
             std::vector<uint32_t> blen(who.size()), bstat(who.size());
             check(gofr_batch_bind(engine_, t->id_, &bin, rows.data(), slot, blen.data(), bstat.data()), "gofr_batch_bind");
+            std::vector<uint32_t> over;  // rows the slot did not hold: the bind reported their exact length
+            std::vector<gofr_req_desc> od;
+            uint32_t wide = 0;
             for (size_t k = 0; k < who.size(); k++) {
-                bound[who[k]].status = blen[k] > slot ? (uint32_t)GOFR_BIND_HOST : bstat[k];
-                bound[who[k]].row.assign((const char*)rows.data() + k * slot, std::min<uint32_t>(blen[k], slot));
+                bound[who[k]].status = bstat[k];
+                if (blen[k] <= slot) bound[who[k]].row.assign((const char*)rows.data() + k * slot, blen[k]);
+                else if (bstat[k] != GOFR_BIND_HOST) { over.push_back(who[k]); od.push_back(bd[k]); wide = std::max(wide, blen[k]); }
+            }
+            if (over.empty()) continue;
+            // invalid UTF-8 triples a string, a long literal or name lengthens an error text: bind those requests once more
+            // in slots of the longest
+            const uint32_t slot2 = (wide + 15u) & ~15u;
+            bin.desc = od.data(); bin.n = (uint32_t)over.size();
+            rows.assign((size_t)over.size() * slot2, 0);
+            check(gofr_batch_bind(engine_, t->id_, &bin, rows.data(), slot2, blen.data(), bstat.data()), "gofr_batch_bind");
+            for (size_t k = 0; k < over.size(); k++) {
+                // gofr_batch_bind reports exact lengths, so every row fits here; one that does not is left to the host
+                const bool host = blen[k] > slot2;
+                bound[over[k]].status = host ? (uint32_t)GOFR_BIND_HOST : bstat[k];
+                bound[over[k]].row.assign((const char*)rows.data() + k * slot2, host ? 0u : blen[k]);
             }
         }
         return bound;
@@ -945,6 +968,7 @@ private:
     std::mt19937_64 rng_{0x9E3779B97F4A7C15ull};
     gofr_conn_app_frontend* reads_ = nullptr;  // ServeRead's front-end (ServeReads)
     uint32_t reads_max_ = 0, max_fields_ = 0;
+    uint64_t max_names_ = 0;  // of the bound types: Go type name plus longest JSON name (GOFR_BIND_ROW_BOUND's names)
     bool reads_log_ = false;
     friend class ProtoCodec;
 };

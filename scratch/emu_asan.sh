@@ -19,5 +19,5 @@ cp /tmp/libgofr_emu_asan.so tests/emu/libgofr_emu.so
 trap 'cp /tmp/libgofr_emu_plain.so tests/emu/libgofr_emu.so; touch tests/emu/libgofr_emu.so' EXIT
 touch tests/emu/libgofr_emu.so
 LD_PRELOAD=$(gcc -print-file-name=libasan.so) ASAN_OPTIONS=detect_leaks=0 python -m pytest tests/test_values.py tests/test_proto_nested.py \
-    tests/test_proto.py tests/test_http_parse.py tests/test_http_frame.py tests/test_route.py tests/test_slots.py tests/test_emu_parity.py tests/test_bind.py \
+    tests/test_proto.py tests/test_http_parse.py tests/test_http_frame.py tests/test_route.py tests/test_slots.py tests/test_emu_parity.py tests/test_bind.py tests/test_bind_unmarshal.py \
     tests/test_result.py tests/test_reqlog.py tests/test_grpc.py tests/test_proto_presence.py tests/test_conn_log.py tests/test_conn_closures.py -x -q -m "not gpu" -p no:cacheprovider -W ignore

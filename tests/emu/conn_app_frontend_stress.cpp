@@ -130,20 +130,22 @@ int gofr_conn_batch_route(gofr_engine*, const gofr_conn_batch* in, gofr_conn_rou
     out->req_first[n] = k;
     return GOFR_OK;
 }
-// row of a bound request: the schema, its parsed form's first byte and data_len bytes; data_len 3 passes any slot
+// row of a bound request: the schema, its parsed form's first byte and data_len bytes; data_len 3 passes any slot (a bind
+// that does not keep to the length it reported), data_len 1 has 1024 bytes more (longer than the first slot of any batch
+// these reads make: the front-end binds it again in a wider one)
 int gofr_batch_bind(gofr_engine*, uint32_t schema, const gofr_req_batch* in, uint8_t* rows, uint32_t slot, uint32_t* len,
                     uint32_t* status) {
     for (uint32_t i = 0; i < in->n; i++) {
         const gofr_req_desc& d = in->desc[i];
         if (d.arena_off >= in->arena_bytes) { g_violations++; return GOFR_ERR_INVALID; }
-        const uint32_t l = d.data_len == 3 ? slot + 1 : 2 + d.data_len;
+        const uint32_t l = d.data_len == 3 ? slot + 1 : 2 + d.data_len + (d.data_len == 1 ? 1024u : 0u);
         len[i] = l;
         status[i] = d.data_len == 2 ? GOFR_BIND_ERROR : GOFR_BIND_OK;
         if (l > slot) continue;
         uint8_t* row = rows + (size_t)i * slot;
         row[0] = (uint8_t)schema;
         row[1] = in->arena[d.arena_off];
-        memset(row + 2, 'r', d.data_len);
+        memset(row + 2, 'r', l - 2);
     }
     return GOFR_OK;
 }
@@ -241,7 +243,7 @@ int main(int argc, char** argv) {
     gofr_conn_app_frontend_set_clock(fe, kClock);
     char date[29];
     gofr_format_http_date(kClock / 1000000000, date);
-    std::atomic<uint64_t> bad{0}, queued{0}, empty{0}, over{0}, invalid_got{0}, bound{0}, hosts{0}, finished{0}, parked_ok{0};
+    std::atomic<uint64_t> bad{0}, queued{0}, empty{0}, over{0}, invalid_got{0}, bound{0}, rebound{0}, hosts{0}, finished{0}, parked_ok{0};
     std::vector<std::vector<uint64_t>> keys(T);
 
     // one read through both calls; false when anything differs from what the stubs say this read must get
@@ -254,7 +256,7 @@ int main(int argc, char** argv) {
         const uint32_t nreq = (uint32_t)want.meta.size(), rc1 = nreq + 1;
         // ---- route ----
         std::vector<gofr_req_desc> desc(rc1);
-        std::vector<uint8_t> arena(len + 80), ids(rc1 * 16), rows(rc1 * 600 + len);
+        std::vector<uint8_t> arena(len + 80), ids(rc1 * 16), rows(rc1 * 600 + len + 1024);
         std::vector<uint32_t> meta(rc1), vars(rc1 * GOFR_MAX_PATH_VARS), at(rc1), bstat(rc1), row_off(rc1 + 1);
         uint32_t first[2] = {9, 9}, consumed = 9, status = 9;
         gofr_conn_route ro;
@@ -277,9 +279,10 @@ int main(int argc, char** argv) {
             if (!binds) ok = ok && bstat[j] == 0xFFFFFFFFu && rlen == 0;
             else if (j == 3) { ok = ok && bstat[j] == GOFR_BIND_HOST && rlen == 0; hosts++; }
             else {
-                ok = ok && bstat[j] == (j == 2 ? (uint32_t)GOFR_BIND_ERROR : (uint32_t)GOFR_BIND_OK) && rlen == 2 + j &&
-                     rows[row_off[j]] == kRouteSchema[route] && rows[row_off[j] + 1] == (buf[at[j]] ^ 0x5A);
+                ok = ok && bstat[j] == (j == 2 ? (uint32_t)GOFR_BIND_ERROR : (uint32_t)GOFR_BIND_OK) && rlen == 2 + j + (j == 1 ? 1024u : 0u) &&
+                     rows[row_off[j]] == kRouteSchema[route] && rows[row_off[j] + 1] == (buf[at[j]] ^ 0x5A) && (j == 0 || rows[row_off[j + 1] - 1] == 'r');
                 bound++;
+                if (j == 1) rebound++;
             }
         }
         if (len) keys[t].push_back(key);
@@ -382,14 +385,14 @@ int main(int argc, char** argv) {
     gofr_conn_app_frontend_destroy(fe);
     printf("{\"queued\": %llu, \"empty\": %llu, \"over\": %llu, \"route_batches\": %llu, \"route_reads\": %llu, \"respond_batches\": %llu, "
            "\"respond_reads\": %llu, \"reruns\": %llu, \"isolated\": %llu, \"refused\": %llu, \"mixed\": %llu, \"largest\": %llu, "
-           "\"respond_calls\": %llu, \"invalid_got\": %llu, \"bound\": %llu, \"hosts\": %llu, \"keys\": %llu, \"parked_ok\": %llu, "
+           "\"respond_calls\": %llu, \"invalid_got\": %llu, \"bound\": %llu, \"rebound\": %llu, \"hosts\": %llu, \"keys\": %llu, \"parked_ok\": %llu, "
            "\"violations\": %llu, \"bad\": %llu}\n",
            (unsigned long long)queued.load(), (unsigned long long)empty.load(), (unsigned long long)over.load(),
            (unsigned long long)st.route_batches, (unsigned long long)st.route_reads, (unsigned long long)st.respond_batches,
            (unsigned long long)st.respond_reads, (unsigned long long)st.reruns, (unsigned long long)st.isolated,
            (unsigned long long)g_refused.load(), (unsigned long long)g_mixed.load(), (unsigned long long)g_largest.load(),
            (unsigned long long)g_respond_calls.load(), (unsigned long long)invalid_got.load(), (unsigned long long)bound.load(),
-           (unsigned long long)hosts.load(), (unsigned long long)n_keys, (unsigned long long)parked_ok.load(),
+           (unsigned long long)rebound.load(), (unsigned long long)hosts.load(), (unsigned long long)n_keys, (unsigned long long)parked_ok.load(),
            (unsigned long long)g_violations.load(), (unsigned long long)bad.load());
     return bad.load() || g_violations.load() ? 1 : 0;
 }

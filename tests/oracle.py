@@ -153,8 +153,13 @@ class OracleTable:
         return None if n == -1 else b"" if n == -2 else out.raw[:n]
 
     def bind(self, schema_id: int, body: bytes):
-        out = C.create_string_buffer(len(body) * 4 + 4096)
-        n = lib().orc_bind(self._t, schema_id, body, len(body), out, len(out))
+        cap = len(body) * 4 + 4096
+        while True:
+            out = C.create_string_buffer(cap)
+            n = lib().orc_bind(self._t, schema_id, body, len(body), out, len(out))
+            if n != -1000000:   # -1000000: the row or error text did not fit (an error text names the type and the field)
+                break
+            cap *= 4
         if n >= 0:
             return True, out.raw[:n]
         return False, out.raw[:-n]

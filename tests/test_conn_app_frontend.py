@@ -81,7 +81,7 @@ def test_two_rounds_under_tsan(stress_exe, args):
     t, n, max_batch = (int(v) for v in args.split()[:3])
     park, bad = int(args.split()[7]), int(args.split()[8])
     assert res["bad"] == 0 and res["violations"] == 0 and res["largest"] <= max_batch
-    assert res["empty"] > 0 and res["over"] > 0 and res["bound"] > 0 and res["hosts"] > 0
+    assert res["empty"] > 0 and res["over"] > 0 and res["bound"] > 0 and res["rebound"] > 0 and res["hosts"] > 0
     assert res["keys"] == res["route_reads"]
     if max_batch > 1:
         assert res["reruns"] > 0 and res["reruns"] == res["refused"]
