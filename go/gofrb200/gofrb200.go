@@ -187,6 +187,52 @@ func (b *LogBatch) Append(start time.Time, elapsed time.Duration, now time.Time,
 	b.Arena = append(append(append(append(append(b.Arena, method...), userAgent...), xff...), remoteAddr...), requestURI...)
 }
 
+// SubmitLog serves one batch like Serve and writes middleware.Logging's line for each request in the same call
+// (gofr_batch_submit_log): log holds one record per request of b, appended with Append, whose status and clocks the call
+// fills from the response and from now; request i's line is lines[logOff[i]:logOff[i+1]], empty when mux answered it
+// without middleware (301 / 404 / 405) or it is a GOFR_H_HOST hole.  logOff needs len(b.Desc)+1 entries; a short lines
+// buffer is gofr_batch_wait's GOFR_ERR_CAPACITY (gofr_batch_log_bound sizes it).  Returns the response and line bytes.
+func (e *Engine) SubmitLog(b *Batch, log *LogBatch, now time.Time, out []byte, off, meta []uint32, lines []byte,
+	logOff []uint32) (int, int, error) {
+	n := len(b.Desc)
+	if n == 0 {
+		return 0, 0, nil
+	}
+	if len(off) < n+1 || len(meta) < n || len(log.Desc) != n || len(logOff) < n+1 || len(lines) == 0 {
+		return 0, 0, errors.New("gofrb200: SubmitLog columns too small")
+	}
+	var in C.gofr_req_batch
+	in.desc = &b.Desc[0]
+	in.trace_ids = (*C.uint8_t)(unsafe.Pointer(&b.TraceIDs[0]))
+	in.arena = (*C.uint8_t)(unsafe.Pointer(&b.Arena[0]))
+	in.arena_bytes = C.uint64_t(len(b.Arena))
+	in.n = C.uint32_t(n)
+	C.gofr_format_http_date(C.int64_t(now.Unix()), &in.date[0])
+	var o C.gofr_resp_batch
+	o.out = (*C.uint8_t)(unsafe.Pointer(&out[0]))
+	o.out_cap = C.uint64_t(len(out))
+	o.out_off = (*C.uint32_t)(unsafe.Pointer(&off[0]))
+	o.meta = (*C.uint32_t)(unsafe.Pointer(&meta[0]))
+	var l C.gofr_batch_log
+	l.desc = &log.Desc[0]
+	if len(log.Arena) > 0 {
+		l.arena = (*C.uint8_t)(unsafe.Pointer(&log.Arena[0]))
+	}
+	l.arena_bytes = C.uint64_t(len(log.Arena))
+	l.log_unix_ns = C.int64_t(now.UnixNano())
+	l.out = (*C.uint8_t)(unsafe.Pointer(&lines[0]))
+	l.out_cap = C.uint64_t(len(lines))
+	l.log_off = (*C.uint32_t)(unsafe.Pointer(&logOff[0]))
+	var ticket C.gofr_ticket
+	if err := check(C.gofr_batch_submit_log(e.e, &in, &o, &l, &ticket), "gofr_batch_submit_log"); err != nil {
+		return 0, 0, err
+	}
+	if err := check(C.gofr_batch_wait(e.e, ticket), "gofr_batch_wait"); err != nil {
+		return 0, 0, err
+	}
+	return int(o.out_bytes), int(l.out_bytes), nil
+}
+
 // RequestLogDevice runs gofr_requestlog_device on buffers that already live in device memory (the batcher uploads the
 // LogBatch next to the request batch); lines come back packed, line i = out[off[i]:off[i+1]].
 func (e *Engine) RequestLogDevice(dDesc, dTraceIDs, dArena unsafe.Pointer, n int, dOut unsafe.Pointer, outCap uint64,

@@ -63,6 +63,12 @@ class ConnLog(C.Structure):
                 ("out_bytes", C.c_uint64)]
 
 
+class BatchLog(C.Structure):
+    _fields_ = [("desc", C.c_void_p), ("arena", C.c_void_p), ("arena_bytes", C.c_uint64), ("log_unix_ns", C.c_int64),
+                ("out", C.c_void_p), ("out_cap", C.c_uint64), ("log_off", C.c_void_p), ("lines", C.c_uint32),
+                ("reserved", C.c_uint32), ("out_bytes", C.c_uint64)]
+
+
 class ConnRoute(C.Structure):
     _fields_ = [("req_cap", C.c_uint32), ("reserved", C.c_uint32), ("desc", C.c_void_p), ("arena", C.c_void_p),
                 ("meta", C.c_void_p), ("vars", C.c_void_p), ("req_at", C.c_void_p), ("trace_ids", C.c_void_p),
@@ -211,6 +217,14 @@ def lib():
     L.gofr_conn_app_frontend_respond.argtypes = [vp, C.c_char_p, u32, u64, C.POINTER(ConnResults), C.c_char_p, u32, C.c_int64,
                                                  C.POINTER(ConnResp), C.POINTER(ConnLog)]
     L.gofr_requestlog_device.argtypes = [vp, vp, vp, vp, u32, vp, u64, vp, vp]
+    L.gofr_batch_submit_log.argtypes = [vp, C.POINTER(ReqBatch), C.POINTER(RespBatch), C.POINTER(BatchLog), C.POINTER(u64)]
+    L.gofr_batch_submit_slots_log.argtypes = [vp, C.POINTER(ReqBatch), C.POINTER(SlotBatch), C.POINTER(BatchLog), C.POINTER(u64)]
+    L.gofr_batch_log_bound.argtypes = [vp, u32, C.POINTER(u64)]
+    L.gofr_frontend_create_log.argtypes = [C.POINTER(vp), vp, u32, u32, u32, u32, u32]
+    L.gofr_frontend_set_log_clock.argtypes = [vp, C.c_int64]
+    L.gofr_frontend_serve_log.argtypes = [vp, C.c_uint8, C.c_char_p, C.c_uint16, C.c_char_p, C.c_uint16, C.c_uint8, C.c_char_p,
+                                          u32, C.c_char_p, vp, C.c_char_p, C.c_char_p, u32, C.POINTER(u32), C.POINTER(u32),
+                                          C.c_char_p, u32, C.POINTER(u32)]
     L.gofr_engine_launch_count.argtypes = [vp]
     L.gofr_engine_launch_count.restype = u64
     L.gofr_engine_kernel_time_ms.argtypes = [vp, C.POINTER(C.c_double), C.POINTER(u64), i32]
@@ -229,8 +243,8 @@ DECLARED_SYMBOLS = [
     "gofr_table_route_count", "gofr_table_max_response_bytes", "gofr_engine_create", "gofr_engine_destroy",
     "gofr_serve_device", "gofr_serve_device_slots", "gofr_batch_submit", "gofr_batch_wait", "gofr_batch_submit_slots", "gofr_engine_set_chunk", "gofr_engine_set_tile",
     "gofr_engine_set_timing", "gofr_engine_overflowed", "gofr_engine_geometry", "gofr_engine_slot_ctas", "gofr_table_slot_ctas", "gofr_alloc_pinned", "gofr_free_pinned", "gofr_bind_host_thread", "gofr_bind_device", "gofr_batch_bind",
-    "gofr_grpc_hello_device", "gofr_requestlog_device", "gofr_http_parse_device", "gofr_http_frame_device", "gofr_conn_batch_submit", "gofr_conn_batch_bound", "gofr_conn_batch_submit_log", "gofr_conn_log_bound", "gofr_conn_batch_route", "gofr_conn_batch_respond", "gofr_conn_respond_bound", "gofr_conn_batch_respond_ex", "gofr_batch_route", "gofr_proto_encode_device", "gofr_proto_decode_device", "gofr_proto_encode_nested_device", "gofr_proto_decode_nested_device", "gofr_proto_nested_describe", "gofr_proto_encode_nested_ex_device", "gofr_proto_decode_nested_ex_device", "gofr_proto_nested_describe_ex", "gofr_proto_decode_nested_deferred_device", "gofr_proto_batch_decode", "gofr_proto_batch_encode", "gofr_proto_nested_bound", "gofr_table_response_bound", "gofr_frontend_create", "gofr_frontend_destroy", "gofr_frontend_set_clock",
-    "gofr_frontend_stats", "gofr_frontend_serve", "gofr_proto_frontend_create", "gofr_proto_frontend_destroy",
+    "gofr_grpc_hello_device", "gofr_requestlog_device", "gofr_batch_submit_log", "gofr_batch_submit_slots_log", "gofr_batch_log_bound", "gofr_http_parse_device", "gofr_http_frame_device", "gofr_conn_batch_submit", "gofr_conn_batch_bound", "gofr_conn_batch_submit_log", "gofr_conn_log_bound", "gofr_conn_batch_route", "gofr_conn_batch_respond", "gofr_conn_respond_bound", "gofr_conn_batch_respond_ex", "gofr_batch_route", "gofr_proto_encode_device", "gofr_proto_decode_device", "gofr_proto_encode_nested_device", "gofr_proto_decode_nested_device", "gofr_proto_nested_describe", "gofr_proto_encode_nested_ex_device", "gofr_proto_decode_nested_ex_device", "gofr_proto_nested_describe_ex", "gofr_proto_decode_nested_deferred_device", "gofr_proto_batch_decode", "gofr_proto_batch_encode", "gofr_proto_nested_bound", "gofr_table_response_bound", "gofr_frontend_create", "gofr_frontend_destroy", "gofr_frontend_set_clock",
+    "gofr_frontend_stats", "gofr_frontend_serve", "gofr_frontend_create_log", "gofr_frontend_set_log_clock", "gofr_frontend_serve_log", "gofr_proto_frontend_create", "gofr_proto_frontend_destroy",
     "gofr_proto_frontend_stats", "gofr_proto_frontend_call", "gofr_conn_frontend_create", "gofr_conn_frontend_destroy",
     "gofr_conn_frontend_set_clock", "gofr_conn_frontend_stats", "gofr_conn_frontend_serve",
     "gofr_conn_app_frontend_create", "gofr_conn_app_frontend_destroy", "gofr_conn_app_frontend_set_clock",

@@ -66,6 +66,7 @@ __global__ void proto_encode_nested_presence_kernel(const GrpcParams p, const Pb
 __global__ void proto_decode_nested_presence_kernel(const GrpcParams p, const PbnDesc D);  // with explicit presence (and maps)
 __global__ void proto_decode_nested_deferred_kernel(const GrpcParams p, const uint32_t* meta_in, const PbnDesc D);  // proto_nested_deferred_kernel.cu
 __global__ void reqlog_kernel(const LogParams p);                // reqlog_kernel.cu
+__global__ void batch_log_kernel(const LogParams p, const uint32_t* meta, int64_t log_ns, unsigned long long* lines);  // batch_log_kernel.cu
 __global__ void http_parse_kernel(const HttpParams p);           // http_kernel.cu
 __global__ void http_frame_kernel(const HttpFrameParams p);      // http_frame_kernel.cu
 __global__ void conn_compact_kernel(const ConnParams p);         // conn_kernel.cu
@@ -81,7 +82,7 @@ namespace {
 enum Kern {
     K_SERVE, K_SERVE_VALUES, K_SLOTS, K_SLOTS_WIDE, K_SLOTS_VALUES, K_HELLO, K_PROTO_ENC, K_PROTO_DEC, K_PBN_ENC, K_PBN_DEC,
     K_PBN_ENC_MAPS, K_PBN_DEC_MAPS, K_PBN_ENC_PRES, K_PBN_DEC_PRES, K_PBN_DEC_DEFERRED, K_REQLOG, K_HTTP, K_HTTP_FRAME, K_ROUTE, K_BIND, K_PACK,
-    K_CONN, K_CONN_LOG, K_CONN_RESULT,
+    K_CONN, K_CONN_LOG, K_CONN_RESULT, K_BATCH_LOG,
     K_COUNT
 };
 struct KernelRec {
@@ -114,6 +115,7 @@ const KernelRec kKernels[K_COUNT] = {
     {(const void*)conn_compact_kernel, "connection compact", kServeThreads},
     {(const void*)conn_log_kernel, "connection log", kServeThreads},
     {(const void*)conn_result_kernel, "connection result", kServeThreads},
+    {(const void*)batch_log_kernel, "batch log", kServeThreads},
 };
 
 constexpr int kSlots = 3;  // pipeline depth of the host-batch path
@@ -168,6 +170,8 @@ struct Slot {
     int reserve_codec(uint32_t records, size_t a_bytes, size_t b_bytes);
     int reserve_conn(uint32_t conns, uint32_t records, size_t buf_bytes);
     int reserve_log(uint32_t conns, uint32_t records, size_t remote_bytes);
+    int reserve_lines(uint32_t lines);
+    int reserve_line_bytes(size_t arena_bytes, uint64_t line_bytes);
 };
 
 }  // namespace
@@ -199,9 +203,10 @@ struct gofr_engine {
     cudaStream_t st_h2d = nullptr, st_compute = nullptr, st_egress = nullptr;
     cudaEvent_t ev_batch_done = nullptr;  // blocking-sync event: the caller's thread SLEEPS until its batch is back (a
                                           // spinning cudaStreamSynchronize per rank burns the CPU quota eight ranks share)
-    unsigned long long* d_chain = nullptr;  // packed position of the batch in flight
+    unsigned long long* d_chain = nullptr;  // packed position of the batch in flight; [2] its log lines (gofr_batch_submit_log)
     ChunkInfo* d_info = nullptr;            // two per slot: [slot] the responses, [kSlots + slot] the request-log lines
-    unsigned long long* h_status = nullptr; // pinned: [0] total bytes, [1] overflow; [2], [3] the same for the log lines
+    unsigned long long* h_status = nullptr; // pinned: [0] total bytes, [1] overflow; [2], [3] the same for the log lines;
+                                            // [4] the log line count of gofr_batch_submit_log
     uint32_t* h_ends = nullptr;             // pinned, gofr_conn_batch_submit: per shipped chunk its first and end response
                                             // offsets, then its first and end log line offsets (PackedOut::ship)
     size_t ends_cap = 0;                    // (words)
@@ -1058,6 +1063,17 @@ struct PackedOut {
     }
 };
 
+// PackedOut::ship's read-backs for a batch of up to max_chunks chunks
+static int reserve_ends(gofr_engine* e, uint64_t max_chunks) {
+    if (4 * max_chunks <= e->ends_cap) return GOFR_OK;
+    if (e->h_ends) cudaFreeHost(e->h_ends);
+    e->h_ends = nullptr;
+    e->ends_cap = 0;
+    CUDA_TRY(cudaMallocHost(&e->h_ends, 4 * max_chunks * 4));
+    e->ends_cap = 4 * max_chunks;
+    return GOFR_OK;
+}
+
 // The chunk pipeline of the host-batch calls with a packed output (gofr_batch_submit, gofr_proto_batch_decode / _encode).
 // What differs between them:
 //   plan     the chunk that starts at record lo: its end, its input byte range and a bound on its device output; the
@@ -1236,9 +1252,23 @@ int Slot::reserve_conn(uint32_t conns, uint32_t records, size_t buf_bytes) {
 // only known once the chunk is served grow in conn_log_chunk.
 int Slot::reserve_log(uint32_t conns, uint32_t records, size_t remote_bytes) {
     int rc = grow_cols(&cap_lconns, conns, "logged connections", {{&d_remote_off, 4, 4}, {&d_start, 8, 0}, {&d_lfirst, 4, 4}});
-    if (!rc) rc = grow_cols(&cap_lrecs, records, "log lines", {{&d_ldesc, sizeof(gofr_log_desc), 0}, {&d_lids, 16, 0},
-                                                               {&d_lreq, 4, 0}, {&d_lraw_off, 4, 4}, {&d_loff, 4, 4}});
+    if (!rc) rc = reserve_lines(records);
     return rc ? rc : grow((void**)&d_remote, &cap_remote, remote_bytes + 16, 256);
+}
+
+// The per-line columns: descriptors, trace ids, request indices and the reqlog and pack offset columns.
+int Slot::reserve_lines(uint32_t lines) {
+    return grow_cols(&cap_lrecs, lines, "log lines", {{&d_ldesc, sizeof(gofr_log_desc), 0}, {&d_lids, 16, 0}, {&d_lreq, 4, 0},
+                                                      {&d_lraw_off, 4, 4}, {&d_loff, 4, 4}});
+}
+
+// The log arena (plus the 32 readable bytes the reqlog kernel needs after the last string), and the reqlog kernel's lines
+// and the packed lines for `line_bytes` of lines (plus the word the pack kernel's copy reads past a line, and the packed
+// start at *chain_pos & 15).
+int Slot::reserve_line_bytes(size_t arena_bytes, uint64_t line_bytes) {
+    int rc = grow((void**)&d_larena, &cap_larena, arena_bytes + 64, 256);
+    if (!rc) rc = grow((void**)&d_lraw, &cap_lraw, line_bytes + 16, 256);
+    return rc ? rc : grow((void**)&d_lout, &cap_lout, line_bytes + 16, 256);
 }
 
 // A chunk: connections [lo, hi), staged from buffer byte alo (buf_off[lo] rounded down to 16, so that the absolute offsets
@@ -1496,13 +1526,7 @@ static int conn_batch_locked(gofr_engine* e, const gofr_conn_batch* in, const ui
     }
     // chunks end at e->chunk connections or at the byte budget, where two neighbours together pass it
     const uint64_t max_chunks = (n + (uint64_t)e->chunk - 1) / e->chunk + 2 * (std::min<uint64_t>(in->buf_bytes, 1ull << 32) / kConnChunkBudget) + 2;
-    if (4 * max_chunks > e->ends_cap) {
-        if (e->h_ends) cudaFreeHost(e->h_ends);
-        e->h_ends = nullptr;
-        e->ends_cap = 0;
-        CUDA_TRY(cudaMallocHost(&e->h_ends, 4 * max_chunks * 4));
-        e->ends_cap = 4 * max_chunks;
-    }
+    { int rc = reserve_ends(e, max_chunks); if (rc) return rc; }
     PackedOut ro(out->out, out->out_cap, out->out_off, out->meta, out->req_cap, 0), lo;
     { int rc = ro.start(e); if (rc) return rc; }
     if (log) {
@@ -1635,6 +1659,155 @@ int gofr_conn_log_bound(const uint32_t* buf_off, const uint32_t* remote_off, uin
     const uint64_t bytes = n_conns ? buf_off[n_conns] - buf_off[0] : 0;
     *line_cap = (uint32_t)std::min<uint64_t>(reqs, 0xFFFFFFFFull);
     *out_cap = reqs * kConnLogFrame + 6 * (bytes + remote);
+    return GOFR_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// host batches with request-log lines (gofr_batch_submit_log, gofr_batch_submit_slots_log)
+// ---------------------------------------------------------------------------------------------------------------
+
+// The log records of requests [lo, hi): each is checked (its kind, its strings inside the arena), and *alo / *ahi receive
+// the arena range of the records that may get a line (16-byte granular below), *bytes the bound of their lines.
+static int batch_log_plan(const gofr_batch_log* log, uint32_t lo, uint32_t hi, uint32_t* alo_out, uint32_t* ahi_out, uint64_t* bytes) {
+    uint64_t alo = ~0ull, ahi = 0, b = 0;
+    for (uint32_t i = lo; i < hi; i++) {
+        const gofr_log_desc& d = log->desc[i];
+        if (d.kind != GOFR_LOG_REQUEST && d.kind != GOFR_LOG_NONE) {
+            set_last_error("log record %u: kind %u (GOFR_LOG_REQUEST or GOFR_LOG_NONE)", i, d.kind);
+            return GOFR_ERR_INVALID;
+        }
+        const uint64_t len = (uint64_t)d.method_len + d.ua_len + d.xff_len + d.remote_len + d.uri_len, end = d.arena_off + len;
+        if (end > log->arena_bytes || (len && !log->arena)) {
+            set_last_error("log record %u: its strings pass the log arena", i);
+            return GOFR_ERR_INVALID;
+        }
+        if (d.kind == GOFR_LOG_NONE) continue;
+        alo = std::min<uint64_t>(alo, d.arena_off);
+        ahi = std::max(ahi, end);
+        b += kConnLogFrame + 6 * len;
+    }
+    if (ahi == 0) alo = 0;
+    *alo_out = (uint32_t)(alo & ~15ull);
+    *ahi_out = (uint32_t)ahi;
+    *bytes = b;
+    return GOFR_OK;
+}
+
+// One call for both layouts: packed responses into `out`, or slots into `slots`.  Per chunk: the requests and their log
+// records and strings go up, the serve kernel answers, the serve-fed request-log kernel (batch_log_kernel.cu) writes each
+// request's line (empty for a request without one) in its own overflow word d_flag[1], chunk_pack_kernel places the lines
+// on the batch's chained position, and the lines leave as output 1 (PackedOut).  Line offsets are per request, so no count
+// comes back mid-batch; the kernel counts the lines into d_chain[2], read once at the end.  The lines carry meta as their
+// per-record column: the slot layout's meta leaves with them (and once more as a plain copy, so that it is complete when
+// only the log's capacity is short).
+static int batch_log_locked(gofr_engine* e, const gofr_req_batch* in, gofr_resp_batch* out, gofr_slot_batch* slots,
+                            gofr_batch_log* log, gofr_ticket* ticket) {
+    const uint32_t n = in->n;
+    log->lines = 0;
+    log->out_bytes = 0;
+    if (out) out->out_bytes = 0;
+    if (n == 0) {  // nothing to do; the caller may have passed no buffers at all
+        if (log->log_off) log->log_off[0] = 0;
+        if (out && out->out_off) out->out_off[0] = 0;
+        complete(e, ticket, GOFR_OK);
+        return GOFR_OK;
+    }
+    { int rc = reserve_ends(e, (n + (uint64_t)e->chunk - 1) / e->chunk); if (rc) return rc; }
+    uint32_t* meta = out ? out->meta : slots->meta;
+    PackedOut ro, lo(log->out, log->out_cap, log->log_off, meta, n, 1);
+    if (out) {
+        ro = PackedOut(out->out, out->out_cap, out->out_off, out->meta, n, 0);
+        int rc = ro.start(e);
+        if (rc) return rc;
+    }
+    { int rc = lo.start(e); if (rc) return rc; }
+    cudaStream_t st = e->st_compute;
+    unsigned long long* d_lines = e->d_chain + 2;
+    CUDA_TRY(cudaMemsetAsync(d_lines, 0, 8, st));
+    const int64_t log_ns = log->log_unix_ns;
+    for (size_t ci = 0; ci * e->chunk < n; ci++) {
+        Slot& s = e->slots[ci % kSlots];
+        const uint32_t c0 = (uint32_t)(ci * e->chunk), c1 = std::min<uint32_t>(n, c0 + e->chunk), cn = c1 - c0;
+        uint32_t alo = 0, ahi = 0, llo = 0, lhi = 0;
+        uint64_t sizes[2], lbytes = 0;
+        int rc = chunk_arena_range(in, c0, c1, false, &alo, &ahi, sizes);
+        if (!rc) rc = batch_log_plan(log, c0, c1, &llo, &lhi, &lbytes);
+        if (rc) return rc;
+        if (lbytes > 0xFFFFFFF0ull) {
+            set_last_error("the log lines of requests %u..%u could pass 4 GiB", c0, c1);
+            return GOFR_ERR_UNSUPPORTED;
+        }
+        const uint64_t obytes = out ? chunk_out_bound(e, cn, sizes) : (uint64_t)cn * slots->slot_bytes;
+        rc = s.reserve(e, cn, (size_t)ahi - alo, obytes);
+        if (!rc) rc = s.reserve_lines(cn);
+        if (!rc) rc = s.reserve_line_bytes((size_t)lhi - llo, lbytes);
+        if (!rc) rc = upload_chunk(in, c0, cn, alo, ahi, s.d_desc, s.d_ids, s.d_arena, e->st_h2d);
+        if (rc) return rc;
+        CUDA_TRY(cudaMemcpyAsync(s.d_ldesc, log->desc + c0, (size_t)cn * sizeof(gofr_log_desc), cudaMemcpyHostToDevice, e->st_h2d));
+        if (lhi > llo)
+            CUDA_TRY(cudaMemcpyAsync(s.d_larena, log->arena + llo, std::min<uint64_t>(lhi, log->arena_bytes) - llo, cudaMemcpyHostToDevice, e->st_h2d));
+        CUDA_TRY(cudaEventRecord(s.ev_h2d, e->st_h2d));
+        CUDA_TRY(cudaStreamWaitEvent(st, s.ev_h2d, 0));
+        rc = out ? launch_serve(e, s.d_desc, s.d_ids, s.d_arena - alo, cn, in->date, s.d_out, s.cap_out, s.d_off, s.d_meta, &s.state,
+                                s.d_flag, s.d_bind, st, ro.chain(e))
+                 : launch_serve(e, s.d_desc, s.d_ids, s.d_arena - alo, cn, in->date, s.d_out, obytes, s.d_off, s.d_meta, nullptr,
+                                s.d_flag, s.d_bind, st, nullptr, slots->slot_bytes);
+        if (!rc && out) rc = ro.ship(e, s, ci, s.d_out, s.d_off, s.d_meta, cn, {});
+        if (rc) return rc;
+        uint32_t* flag = s.d_flag + 1;
+        const uint32_t* d_meta = s.d_meta;
+        LogParams lp;
+        memset(&lp, 0, sizeof lp);
+        lp.desc = s.d_ldesc; lp.ids = s.d_ids; lp.arena = s.d_larena - llo;
+        rc = launch_frames_locked(e, K_BATCH_LOG, 0, lp, cn, s.d_lraw, s.cap_lraw - 16, s.d_lraw_off, s.state, flag, st, d_meta, log_ns, d_lines);
+        if (rc) return rc;
+        PackParams q;
+        memset(&q, 0, sizeof q);
+        q.a = s.d_lraw; q.a_off = s.d_lraw_off; q.a_cap = s.cap_lraw - 16; q.chain_pos = lo.chain(e);
+        rc = launch_frames_locked(e, K_PACK, 0, q, cn, s.d_lout, s.cap_lout, s.d_loff, s.state, flag, st);
+        if (!rc && out) rc = lo.ship(e, s, ci, s.d_lout, s.d_loff, s.d_meta, cn, {});
+        if (!rc && !out)
+            rc = lo.ship(e, s, ci, s.d_lout, s.d_loff, s.d_meta, cn,
+                         {{slots->out + (size_t)c0 * slots->slot_bytes, s.d_out, (size_t)obytes, false},
+                          {slots->out_len + c0, s.d_off, (size_t)cn * 4, false},
+                          {slots->meta + c0, s.d_meta, (size_t)cn * 4, false}});
+        if (rc) return rc;
+    }
+    { int rc = out ? PackedOut::finish(e, n, {&ro, &lo}) : PackedOut::finish(e, n, {&lo}); if (rc) return rc; }
+    CUDA_TRY(cudaMemcpyAsync(&e->h_status[4], d_lines, 8, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    log->lines = (uint32_t)e->h_status[4];
+    int final_rc = GOFR_OK;
+    if (out) final_rc = ro.report(e, &out->out_bytes, "the batch needs %llu requests and %llu response bytes: n %llu, out_cap %llu");
+    const int lrc = lo.report(e, &log->out_bytes, "the batch needs %llu log records and %llu log bytes: n %llu, out_cap %llu");
+    complete(e, ticket, lrc ? lrc : final_rc);
+    return GOFR_OK;
+}
+
+static bool batch_log_valid(const gofr_req_batch* in, const gofr_batch_log* log) {
+    return log && (!in->n || (log->desc && log->out && log->log_off));
+}
+
+int gofr_batch_submit_log(gofr_engine* e, const gofr_req_batch* in, gofr_resp_batch* out, gofr_batch_log* log, gofr_ticket* ticket) {
+    if (!e || !in || !out || !ticket || !batch_log_valid(in, log)) return GOFR_ERR_INVALID;
+    if (in->n && (!in->desc || !in->trace_ids || !out->out || !out->out_off || !out->meta)) return GOFR_ERR_INVALID;
+    return host_batch(e, [&] { return batch_log_locked(e, in, out, nullptr, log, ticket); });
+}
+
+int gofr_batch_submit_slots_log(gofr_engine* e, const gofr_req_batch* in, gofr_slot_batch* out, gofr_batch_log* log, gofr_ticket* ticket) {
+    if (!e || !in || !out || !ticket || !batch_log_valid(in, log)) return GOFR_ERR_INVALID;
+    if (in->n && (!in->desc || !in->trace_ids || !out->out || !out->out_len || !out->meta)) return GOFR_ERR_INVALID;
+    if (out->slot_bytes == 0 || (out->slot_bytes & 15u)) { set_last_error("slot_bytes must be a positive multiple of 16"); return GOFR_ERR_INVALID; }
+    return host_batch(e, [&] { return batch_log_locked(e, in, nullptr, out, log, ticket); });
+}
+
+int gofr_batch_log_bound(const gofr_log_desc* desc, uint32_t n, uint64_t* out_cap) {
+    if (!out_cap || (n && !desc)) return GOFR_ERR_INVALID;
+    uint64_t b = 0;
+    for (uint32_t i = 0; i < n; i++)
+        if (desc[i].kind != GOFR_LOG_NONE)
+            b += kConnLogFrame + 6ull * ((uint64_t)desc[i].method_len + desc[i].ua_len + desc[i].xff_len + desc[i].remote_len + desc[i].uri_len);
+    *out_cap = b;
     return GOFR_OK;
 }
 

@@ -658,6 +658,89 @@ def _serve_host_slots(self, batch: S.RequestBatch, date: bytes, slot_bytes: int,
 Engine.serve_host_slots = _serve_host_slots
 
 
+def batch_log_bound(log: S.LogBatch) -> int:
+    """gofr_batch_log_bound: line bytes that always suffice for gofr_batch_submit_log on these records."""
+    cap = C.c_uint64()
+    _abi.check(_abi.lib().gofr_batch_log_bound(log.desc.ctypes.data, log.n, C.byref(cap)), "gofr_batch_log_bound")
+    return int(cap.value)
+
+
+@dataclass
+class BatchLogResult:
+    """What gofr_batch_submit_log / _slots_log return: the responses (packed: out[out_off[i]:out_off[i + 1]]; slots:
+    out[i * slot_bytes:][:out_len[i]]), meta, and request i's line lines_out[log_off[i]:log_off[i + 1]] (empty when it has
+    none).  lines / log_bytes: what the batch needed; rc: gofr_batch_wait's code (GOFR_ERR_CAPACITY = 7 when short)."""
+    out: np.ndarray
+    out_off: Optional[np.ndarray]   # packed layout
+    out_len: Optional[np.ndarray]   # slot layout
+    meta: np.ndarray
+    lines_out: np.ndarray
+    log_off: np.ndarray
+    lines: int
+    log_bytes: int
+    out_bytes: int
+    rc: int
+
+    def responses(self, slot_bytes: int = 0):
+        if self.out_off is not None:
+            b = self.out.tobytes()
+            return [b[int(self.out_off[i]):int(self.out_off[i + 1])] for i in range(len(self.meta))]
+        return [self.out[i * slot_bytes:i * slot_bytes + int(self.out_len[i])].tobytes() for i in range(len(self.meta))]
+
+    def line_list(self):
+        b = self.lines_out.tobytes()
+        return [b[int(self.log_off[i]):int(self.log_off[i + 1])] for i in range(len(self.log_off) - 1)]
+
+
+def _serve_host_log(self, batch: S.RequestBatch, date: bytes, log: S.LogBatch, log_unix_ns: int, slot_bytes: int = 0,
+                    pinned: bool = True, out_cap: Optional[int] = None, log_out_cap: Optional[int] = None,
+                    raise_on_capacity: bool = True) -> BatchLogResult:
+    """gofr_batch_submit_log (slot_bytes 0: packed layout) or gofr_batch_submit_slots_log + wait on a RequestBatch with
+    one LogBatch record per request (kind LOG_REQUEST or LOG_NONE; status and the clock fields are the call's).  The log
+    batch's trace ids are not used: a line's id is its request's.  Buffers are pinned (device-driven egress) or pageable."""
+    L = _abi.lib()
+    n = batch.n
+    assert log.n == n
+    alloc = _alloc(pinned)
+    if out_cap is None:
+        out_cap = sum(int(L.gofr_table_response_bound(self.table.handle, int(d["path_len"]), int(d["query_len"]),
+                                                      int(d["data_len"]))) for d in batch.desc)
+    if log_out_cap is None:
+        log_out_cap = batch_log_bound(log)
+    meta = alloc(n, np.uint32)
+    lout = alloc(log_out_cap + 16, np.uint8)
+    lout[log_out_cap:] = 0xAB   # 16 bytes past the capacity that the call must leave alone
+    log_off = alloc(n + 1, np.uint32)
+    rb = _abi.ReqBatch(desc=batch.desc.ctypes.data, trace_ids=batch.trace_ids.ctypes.data, arena=batch.arena.ctypes.data,
+                       arena_bytes=batch.arena.size, n=n, date=date)
+    lb = _abi.BatchLog(desc=log.desc.ctypes.data, arena=log.arena.ctypes.data if log.arena.size else None,
+                       arena_bytes=log.arena.size, log_unix_ns=log_unix_ns, out=lout.ctypes.data, out_cap=log_out_cap,
+                       log_off=log_off.ctypes.data, lines=0, reserved=0, out_bytes=0)
+    t = C.c_uint64()
+    out_off = out_len = None
+    if slot_bytes:
+        out = alloc(n * slot_bytes, np.uint8)
+        out_len = alloc(n, np.uint32)
+        sb = _abi.SlotBatch(out=out.ctypes.data, slot_bytes=slot_bytes, reserved=0, out_len=out_len.ctypes.data,
+                            meta=meta.ctypes.data)
+        _abi.check(L.gofr_batch_submit_slots_log(self._e, C.byref(rb), C.byref(sb), C.byref(lb), C.byref(t)),
+                   "gofr_batch_submit_slots_log")
+    else:
+        out = alloc(out_cap + 16, np.uint8)
+        out_off = alloc(n + 1, np.uint32)
+        ob = _abi.RespBatch(out=out.ctypes.data, out_cap=out_cap, out_off=out_off.ctypes.data, meta=meta.ctypes.data,
+                            out_bytes=0)
+        _abi.check(L.gofr_batch_submit_log(self._e, C.byref(rb), C.byref(ob), C.byref(lb), C.byref(t)), "gofr_batch_submit_log")
+    rc = int(L.gofr_batch_wait(self._e, t.value))
+    if rc and (raise_on_capacity or rc != 7):
+        _abi.check(rc, "gofr_batch_wait")
+    return BatchLogResult(out, out_off, out_len[:n] if slot_bytes else None, meta[:n], lout, log_off, int(lb.lines),
+                          int(lb.out_bytes), 0 if slot_bytes else int(ob.out_bytes), rc)
+
+
+Engine.serve_host_log = _serve_host_log
+
+
 def pinned_array(nbytes: int, dtype=np.uint8) -> np.ndarray:
     """numpy view over cudaMallocHost memory (gofr_alloc_pinned).  The memory lives until process exit."""
     L = _abi.lib()

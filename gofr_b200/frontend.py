@@ -23,12 +23,18 @@ from .engine import ConnLogLines, ConnResponses, ConnRoute, Engine, conn_batch_b
 
 class Frontend:
     def __init__(self, engine: Engine, max_batch: int = 4096, max_wait_us: int = 200, slot_bytes: int = 1024,
-                 max_request_bytes: int = 4096):
+                 max_request_bytes: int = 4096, max_log_bytes: Optional[int] = None):
+        """max_log_bytes: log staging per request (gofr_frontend_create_log), so that serve takes log=; None: none."""
         self._f = C.c_void_p()
         self.engine = engine
         self.slot_bytes = slot_bytes
-        _abi.check(_abi.lib().gofr_frontend_create(C.byref(self._f), engine._e, max_batch, max_wait_us, slot_bytes,
-                                                   max_request_bytes), "gofr_frontend_create")
+        self.max_log_bytes = max_log_bytes
+        if max_log_bytes is None:
+            _abi.check(_abi.lib().gofr_frontend_create(C.byref(self._f), engine._e, max_batch, max_wait_us, slot_bytes,
+                                                       max_request_bytes), "gofr_frontend_create")
+        else:
+            _abi.check(_abi.lib().gofr_frontend_create_log(C.byref(self._f), engine._e, max_batch, max_wait_us, slot_bytes,
+                                                           max_request_bytes, max_log_bytes), "gofr_frontend_create_log")
 
     def close(self):
         if self._f:
@@ -45,19 +51,36 @@ class Frontend:
         """pin the Date header of every batch (tests); 0 = wall clock"""
         _abi.check(_abi.lib().gofr_frontend_set_clock(self._f, unix_seconds), "gofr_frontend_set_clock")
 
+    def set_log_clock(self, unix_ns: int) -> None:
+        """pin the log time of every line (tests); 0 = wall clock"""
+        _abi.check(_abi.lib().gofr_frontend_set_log_clock(self._f, unix_ns), "gofr_frontend_set_log_clock")
+
     def stats(self) -> Tuple[int, int]:
         b, r = C.c_uint64(), C.c_uint64()
         _abi.check(_abi.lib().gofr_frontend_stats(self._f, C.byref(b), C.byref(r)), "gofr_frontend_stats")
         return int(b.value), int(r.value)
 
     def serve(self, method: int, path: bytes, query: bytes = b"", data: bytes = b"", trace_id: bytes = b"\0" * 16,
-              flags: int = 0, resp_cap: int = 0) -> Tuple[bytes, int]:
+              flags: int = 0, resp_cap: int = 0, log: Optional[S.LogRec] = None, line_cap: int = 0):
         """One request → (response bytes, meta).  Blocks until the batch it joined has been served.  resp_cap: size of
-        the caller's buffer (default: one slot); a response longer than the slot but within resp_cap is served alone."""
+        the caller's buffer (default: one slot); a response longer than the slot but within resp_cap is served alone.
+        With log (a LogRec: its start time, zone, strings and kind LOG_REQUEST / LOG_NONE; the rest is the call's) →
+        (response bytes, meta, line) through gofr_frontend_serve_log; line_cap defaults to the bound of the record."""
         assert len(trace_id) == 16
         cap = resp_cap or self.slot_bytes
         buf = C.create_string_buffer(cap)
         n, meta = C.c_uint32(), C.c_uint32()
+        if log is not None:
+            lb = S.LogBatch.pack([log])
+            strings = lb.arena.tobytes()
+            lcap = line_cap or 320 + 6 * len(strings)
+            line = C.create_string_buffer(max(lcap, 1))
+            ln = C.c_uint32()
+            _abi.check(_abi.lib().gofr_frontend_serve_log(self._f, method, path, len(path), query, len(query), flags, data,
+                                                          len(data), trace_id, lb.desc.ctypes.data, strings, buf, cap,
+                                                          C.byref(n), C.byref(meta), line, lcap, C.byref(ln)),
+                       "gofr_frontend_serve_log")
+            return buf.raw[:n.value], int(meta.value), line.raw[:ln.value]
         _abi.check(_abi.lib().gofr_frontend_serve(self._f, method, path, len(path), query, len(query), flags, data, len(data),
                                                   trace_id, buf, cap, C.byref(n), C.byref(meta)),
                    "gofr_frontend_serve")

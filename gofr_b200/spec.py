@@ -283,7 +283,7 @@ class RequestBatch:
         return RequestBatch(desc, ids, np.frombuffer(bytes(arena), dtype=np.uint8).copy())
 
 
-LOG_REQUEST, LOG_RPC = 0, 1
+LOG_REQUEST, LOG_RPC, LOG_NONE = 0, 1, 2   # LOG_NONE: this request gets no line from gofr_batch_submit_log
 
 # gofr_log_desc (include/gofr_b200.h): one RequestLog record (middleware/logger.go:24-33,41-70)
 LOG_DESC_DTYPE = np.dtype([("start_unix_ns", "<i8"), ("elapsed_ns", "<i8"), ("log_unix_ns", "<i8"), ("arena_off", "<u4"),

@@ -629,6 +629,49 @@ typedef struct gofr_log_desc { /* 48 bytes */
 int gofr_requestlog_device(gofr_engine*, const gofr_log_desc* d_desc, const uint8_t* d_trace_ids, const uint8_t* d_arena,
                            uint32_t n, uint8_t* d_out, uint64_t out_cap, uint32_t* d_out_off, void* stream);
 
+/* gofr_batch_submit / gofr_batch_submit_slots plus middleware.Logging's RequestLog line (gofr_requestlog_device's format)
+ * for every request of the batch the middleware wraps, in the same call: the lines are a second output of the host-batch
+ * chunk pipeline, written on the device from the statuses the serve kernel has just produced.  Responses, meta and the
+ * packed / slot outputs are byte for byte and status for status what the call without a log gives.
+ *   desc   one record per request of the batch (n = the gofr_req_batch's n).  Read: start_unix_ns, tz_offset_s, arena_off,
+ *          the five lengths and kind, which is GOFR_LOG_REQUEST or GOFR_LOG_NONE (this request gets no line from the call:
+ *          the caller logs it, or nobody does).  Filled by the call: status (the response's), log_unix_ns (the batch's)
+ *          and elapsed_ns = log_unix_ns - start_unix_ns.
+ *   arena  the five strings of each record, as gofr_requestlog_device takes them: method | User-Agent | first
+ *          X-Forwarded-For value | RemoteAddr | RequestURI back to back from arena_off; arena_bytes long.
+ * Which requests get a line: request i has one exactly when GOFR_META_ROUTE(meta[i]) != GOFR_ROUTE_NONE (gorilla/mux
+ * wraps middleware around matched routes only, so the cleanPath 301 and mux's own 404 / 405 are not logged),
+ * GOFR_META_STATUS(meta[i]) != 0 (a GOFR_H_HOST hole is logged by the call that serves its closure's result) and its kind
+ * is GOFR_LOG_REQUEST.  The line's id is the request's trace id.  Every other request has an empty line.
+ *   out    request i's line = out[log_off[i] .. log_off[i + 1]) (log_off has n + 1 entries), in request order; lines =
+ *          the requests that have one, out_bytes = the bytes of all of them.
+ * Capacity: a short out_cap makes gofr_batch_wait return GOFR_ERR_CAPACITY with lines and out_bytes set to what the batch
+ * needed; nothing is written at or past out_cap, and the response columns are complete whenever their own capacities
+ * suffice.  log_off holds 32-bit offsets: a batch whose lines pass 4 GiB is GOFR_ERR_CAPACITY too.  gofr_batch_log_bound
+ * gives an out_cap that always suffices.  Pinned buffers (gofr_alloc_pinned) are streamed by the device, pageable ones are
+ * copied back at each chunk's exact size.
+ * GOFR_ERR_INVALID: the batch call's cases, a null log column (arena may be NULL when every string is empty), a record
+ * whose strings pass arena_bytes, a kind other than GOFR_LOG_REQUEST / GOFR_LOG_NONE. */
+enum { GOFR_LOG_NONE = 2 };
+typedef struct gofr_batch_log {
+    const gofr_log_desc* desc;     /* n */
+    const uint8_t* arena;
+    uint64_t arena_bytes;
+    int64_t log_unix_ns;           /* the logger's time.Now() for every line of the batch */
+    uint8_t* out;
+    uint64_t out_cap;
+    uint32_t* log_off;             /* n + 1 */
+    uint32_t lines;                /* filled by submit, reported by wait */
+    uint32_t reserved;
+    uint64_t out_bytes;            /* filled by submit, reported by wait */
+} gofr_batch_log;
+int gofr_batch_submit_log(gofr_engine*, const gofr_req_batch* in, gofr_resp_batch* out, gofr_batch_log* log, gofr_ticket* ticket);
+int gofr_batch_submit_slots_log(gofr_engine*, const gofr_req_batch* in, gofr_slot_batch* out, gofr_batch_log* log,
+                                gofr_ticket* ticket);
+/* No GPU needed: an out_cap that always suffices for gofr_batch_submit_log's lines of these n records — 320 bytes plus 6
+ * per string byte for each record whose kind is not GOFR_LOG_NONE. */
+int gofr_batch_log_bound(const gofr_log_desc* desc, uint32_t n, uint64_t* out_cap);
+
 /* Batching front-end (SURVEY.md §8f rank 3): the reference serves one request per goroutine (net/http conn.serve →
  * router.ServeHTTP, pkg/gofr/httpServer.go:29-33); the GPU wants batches.  Any number of threads call
  * gofr_frontend_serve with ONE request each and block until its response is ready; a dispatcher thread closes a batch
@@ -648,6 +691,23 @@ int gofr_frontend_stats(gofr_frontend*, uint64_t* batches, uint64_t* requests);
 int gofr_frontend_serve(gofr_frontend*, uint8_t method, const uint8_t* path, uint16_t path_len, const uint8_t* query,
                         uint16_t query_len, uint8_t flags, const uint8_t* data, uint32_t data_len, const uint8_t trace_id[16],
                         uint8_t* resp, uint32_t resp_cap, uint32_t* resp_len, uint32_t* meta);
+/* A front-end whose callers may also ask for their request's RequestLog line: gofr_frontend_create plus log staging of
+ * max_log_bytes string bytes per request.  Its batches run through gofr_batch_submit_slots_log when some caller of the
+ * batch logs (callers of gofr_frontend_serve ride along as GOFR_LOG_NONE), else through gofr_batch_submit_slots. */
+int gofr_frontend_create_log(gofr_frontend** out, gofr_engine*, uint32_t max_batch, uint32_t max_wait_us, uint32_t slot_bytes,
+                             uint32_t max_request_bytes, uint32_t max_log_bytes);
+/* The log time of every line (unix ns; 0 = the wall clock at dispatch).  gofr_frontend_set_clock keeps pinning the Date. */
+int gofr_frontend_set_log_clock(gofr_frontend*, int64_t unix_ns);
+/* gofr_frontend_serve plus the request's line by gofr_batch_submit_log's rule.  log: start_unix_ns, tz_offset_s, the five
+ * lengths and kind (GOFR_LOG_REQUEST or GOFR_LOG_NONE) are read, arena_off is ignored; strings: the five strings back to
+ * back (at most max_log_bytes).  The line goes to line[0 .. *line_len) (empty when the request has none); a line longer
+ * than line_cap returns GOFR_ERR_CAPACITY with *line_len set, the response still delivered.  A response longer than its
+ * slot is served again alone as gofr_frontend_serve does; its line is the batch's, written once.  GOFR_ERR_INVALID on a
+ * front-end made by gofr_frontend_create. */
+int gofr_frontend_serve_log(gofr_frontend*, uint8_t method, const uint8_t* path, uint16_t path_len, const uint8_t* query,
+                            uint16_t query_len, uint8_t flags, const uint8_t* data, uint32_t data_len, const uint8_t trace_id[16],
+                            const gofr_log_desc* log, const uint8_t* strings, uint8_t* resp, uint32_t resp_cap, uint32_t* resp_len,
+                            uint32_t* meta, uint8_t* line, uint32_t line_cap, uint32_t* line_len);
 
 /* Batching front-end of the nested proto3 codec: grpc-go calls its codec once per message (encoding.Codec.Unmarshal for a
  * request, Marshal for a response, on the RPC's goroutine; hello_grpc.pb.go:73-89 runs dec(in) between them); the GPU codec
