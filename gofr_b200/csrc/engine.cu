@@ -127,9 +127,8 @@ struct TileState {
 };
 
 struct Slot {
-    cudaStream_t stream = nullptr;
     cudaEvent_t done = nullptr;
-    cudaEvent_t ev_h2d = nullptr, ev_served = nullptr, ev_egress = nullptr;  // streaming path
+    cudaEvent_t ev_h2d = nullptr, ev_served = nullptr, ev_egress = nullptr;  // the chunk pipeline
     bool egress_pending = false;
     // device buffers (grown on demand)
     void* d_desc = nullptr; void* d_ids = nullptr; uint8_t* d_arena = nullptr; uint8_t* d_out = nullptr;
@@ -164,7 +163,7 @@ struct Slot {
     uint32_t* d_vars = nullptr;
     size_t cap_rbytes = 0, cap_rreqs = 0, cap_sarena = 0, cap_vars = 0;
     // pinned staging for the tiny per-chunk read-backs
-    uint32_t* h_tail = nullptr;  // [0] = chunk total bytes (connections: records), [2] = log lines; [2k + 1] = output k's overflow word
+    uint32_t* h_tail = nullptr;  // [2k] = a pageable output k's chunk size (connections: [0] records, [2] log lines); [2k + 1] = output k's overflow word
 
     int reserve(gofr_engine* e, uint32_t requests, size_t arena_bytes, size_t out_bytes);
     int reserve_codec(uint32_t records, size_t a_bytes, size_t b_bytes);
@@ -207,8 +206,8 @@ struct gofr_engine {
     ChunkInfo* d_info = nullptr;            // two per slot: [slot] the responses, [kSlots + slot] the request-log lines
     unsigned long long* h_status = nullptr; // pinned: [0] total bytes, [1] overflow; [2], [3] the same for the log lines;
                                             // [4] the log line count of gofr_batch_submit_log
-    uint32_t* h_ends = nullptr;             // pinned, gofr_conn_batch_submit: per shipped chunk its first and end response
-                                            // offsets, then its first and end log line offsets (PackedOut::ship)
+    uint32_t* h_ends = nullptr;             // pinned, calls that report what they needed: per posted chunk its first and end
+                                            // response offsets, then its first and end log line offsets (PackedOut::post)
     size_t ends_cap = 0;                    // (words)
     int egress_grid = 37;
     uint32_t chunk = 65536;
@@ -385,7 +384,6 @@ static int engine_init(gofr_engine* e, const std::vector<uint8_t>& img, int devi
     for (uint32_t k = 0; k < e->hdr.n_progs; k++)
         e->has_values |= (reinterpret_cast<const ProgRec*>(img.data() + e->hdr.progs_off)[k].flags & PF_VALUES) != 0;
     for (auto& s : e->slots) {
-        CUDA_TRY(cudaStreamCreateWithFlags(&s.stream, cudaStreamNonBlocking));
         CUDA_TRY(cudaEventCreateWithFlags(&s.done, cudaEventDisableTiming));
         CUDA_TRY(cudaMallocHost(&s.h_tail, 64));
         CUDA_TRY(cudaEventCreateWithFlags(&s.ev_h2d, cudaEventDisableTiming));
@@ -412,7 +410,6 @@ void gofr_engine_destroy(gofr_engine* e) {
     cudaSetDevice(e->device);
     cudaDeviceSynchronize();
     for (auto& s : e->slots) {
-        if (s.stream) cudaStreamDestroy(s.stream);
         if (s.done) cudaEventDestroy(s.done);
         if (s.ev_h2d) cudaEventDestroy(s.ev_h2d);
         if (s.ev_served) cudaEventDestroy(s.ev_served);
@@ -785,8 +782,9 @@ static int grow_cols(size_t* cap, size_t n, const char* what, std::initializer_l
 // (include/gofr_b200.h states the same for device-resident callers), so a staging arena is never sized to the byte.
 static constexpr size_t kArenaSlack = 16;
 
-// A chunk = contiguous record range [lo, hi), the input (arena) byte range it covers and a bound on its device output.
-struct ChunkPlan { uint32_t lo, hi; uint32_t arena_lo, arena_hi; uint64_t out_bound; };
+// A chunk = contiguous record range [lo, hi), the input (arena) byte range it covers and a bound on its device output;
+// with a log, the log-arena byte range its records' strings cover and a bound on its lines.
+struct ChunkPlan { uint32_t lo, hi; uint32_t arena_lo, arena_hi; uint64_t out_bound; uint32_t log_lo, log_hi; uint64_t log_bound; };
 
 // The arena byte range [*alo, *ahi) (16-byte granular) that requests [lo, hi) reference: their whole requests, or their paths
 // only (what routing reads).  All arithmetic in 64 bits: a descriptor with a huge arena_off or data_len (say a data_len taken
@@ -890,7 +888,7 @@ static void drain_streams(gofr_engine* e) {
     cudaStreamSynchronize(e->st_h2d);
     cudaStreamSynchronize(e->st_compute);
     cudaStreamSynchronize(e->st_egress);
-    for (auto& s : e->slots) { if (s.stream) cudaStreamSynchronize(s.stream); s.egress_pending = false; }
+    for (auto& s : e->slots) s.egress_pending = false;
     cudaGetLastError();
 }
 
@@ -932,27 +930,47 @@ struct RecCount {
 // per record (made only when the chunk's records are written) or always (a per-connection column).  No dst: none.
 struct ColCopy { void* dst; const void* src; size_t bytes; bool per_record; };
 
+static int copy_cols(std::initializer_list<ColCopy> copies, bool records, cudaStream_t st) {
+    for (const ColCopy& c : copies)
+        if (c.dst && (records || !c.per_record)) CUDA_TRY(cudaMemcpyAsync(c.dst, c.src, c.bytes, cudaMemcpyDeviceToHost, st));
+    return GOFR_OK;
+}
+
+// The slot's chunk has been handed to the egress stream: its buffers wait for this before they are written again
+// (wait_egress).
+static int fence_egress(gofr_engine* e, Slot& s) {
+    CUDA_TRY(cudaEventRecord(s.ev_egress, e->st_egress));
+    s.egress_pending = true;
+    return GOFR_OK;
+}
+
 // A packed output of a host-batch call: the caller's bytes, their offsets and the one per-record column egress carries
 // (meta, or log_req), and its record count.  Output k (0: responses or proto rows, 1: request-log lines) owns d_chain[k],
 // h_status[2k..], d_info[k * kSlots ..], each slot's overflow word d_flag[k] and its read-back h_tail[2k + 1], and
-// h_ends[4 j + 2k ..] for its j-th shipped chunk.  Pinned buffers are filled by advance and egress without the host
-// waiting (deliver), pageable ones get each chunk's exact bytes (retire).  Both skip a chunk's bytes when the device
-// overflowed or when they would pass cap or 4 GiB (32-bit offsets): the batch then fails.
+// h_ends[4 j + 2k ..] for its j-th posted chunk.  A chunk is posted after the kernels that leave it on the device.
+// Pinned buffers are filled by advance and egress without the host waiting (deliver); a pageable chunk is retired later:
+// its exact bytes once the host has read its size.  Both skip a chunk's bytes when the device overflowed or when they
+// would pass cap or 4 GiB (32-bit offsets): the batch then fails.
+//
+// `needed` decides what the batch reports at its end (report): what it needed, from each chunk's first and end offsets
+// read back to h_ends (the log and connection calls), or what was written (gofr_batch_submit and the proto calls, whose
+// columns are then complete whatever the capacity).
 struct PackedOut {
     uint8_t* out = nullptr;
     uint64_t cap = 0;
     uint32_t* off = nullptr;
     uint32_t* col = nullptr;
     int k = 0;
-    bool pinned = false;
+    bool pinned = false, needed = false;
     RecCount recs;
     uint64_t written = 0, at = 0;  // bytes written (pinned: after finish); pageable: where the last retired chunk went
     bool overflow = false;         // some chunk's bytes were skipped (pinned: after finish)
-    size_t shipped = 0;            // chunks through ship
+    size_t shipped = 0;            // chunks posted with their ends read back (needed)
 
     PackedOut() = default;
-    PackedOut(uint8_t* o, uint64_t c, uint32_t* f, uint32_t* m, uint64_t rec_cap, int k_)
-        : out(o), cap(c), off(f), col(m), k(k_), pinned(device_visible(o) && device_visible(f) && device_visible(m)), recs{rec_cap} {}
+    PackedOut(uint8_t* o, uint64_t c, uint32_t* f, uint32_t* m, uint64_t rec_cap, int k_, bool needed_)
+        : out(o), cap(c), off(f), col(m), k(k_), pinned(device_visible(o) && device_visible(f) && device_visible(m)),
+          needed(needed_), recs{rec_cap} {}
     unsigned long long* chain(gofr_engine* e) const { return pinned ? e->d_chain + k : nullptr; }
     uint32_t* h_flag(Slot& s) const { return s.h_tail + 2 * k + 1; }
     int start(gofr_engine* e) {
@@ -961,9 +979,114 @@ struct PackedOut {
         e->h_status[2 * k] = e->h_status[2 * k + 1] = 0;
         return GOFR_OK;
     }
-    // After the chunk's kernels on st_compute: advance, then egress of its n records to the caller's from `first` on
-    // st_egress.  Without put (a count capacity is short) neither runs and the overflow word is cleared.  The caller adds
-    // its own columns on st_egress, then records s.ev_egress.
+    // Chunk ci's n records, left in slot s's d_out / d_off (at *chain(e) & 15 when pinned, at 0 otherwise) and d_col by the
+    // kernels on st_compute: the record-capacity test, and with `needed` the chunk's first and end offsets back to h_ends.
+    // Pinned: deliver, then `copies` on st_egress behind the egress, then s.ev_egress.  Pageable: the chunk's size and
+    // overflow word back to the host, then s.ev_served; retire(ci) takes it from there.
+    int post(gofr_engine* e, Slot& s, size_t ci, const uint8_t* d_out, const uint32_t* d_off, const uint32_t* d_col, uint32_t n,
+             std::initializer_list<ColCopy> copies = {}) {
+        Posted& p = posted[ci % kSlots];
+        p = {d_out, d_off, d_col, n, recs.base, s.h_tail + 2 * k, false, !pinned};
+        p.put = recs.add(n) && n;
+        const cudaStream_t st = e->st_compute;
+        if (needed) {
+            uint32_t* ends = e->h_ends + 4 * shipped++ + 2 * k;
+            ends[0] = ends[1] = 0;
+            if (n) {
+                CUDA_TRY(cudaMemcpyAsync(&ends[0], d_off, 4, cudaMemcpyDeviceToHost, st));
+                CUDA_TRY(cudaMemcpyAsync(&ends[1], d_off + n, 4, cudaMemcpyDeviceToHost, st));
+            }
+            p.size = &ends[1];
+        }
+        if (pinned) {
+            int rc = deliver(e, s, ci, d_out, d_off, d_col, n, p.first, p.put);
+            if (!rc) rc = copy_cols(copies, p.put, e->st_egress);
+            return rc ? rc : fence_egress(e, s);
+        }
+        if (!needed) CUDA_TRY(cudaMemcpyAsync(p.size, d_off + n, 4, cudaMemcpyDeviceToHost, st));
+        CUDA_TRY(cudaMemcpyAsync(h_flag(s), s.d_flag + k, 4, cudaMemcpyDeviceToHost, st));
+        CUDA_TRY(cudaEventRecord(s.ev_served, st));
+        return GOFR_OK;
+    }
+    // The pageable chunk posted in slot ci % kSlots, if one is still there: the host waits for its read-backs and clears
+    // the overflow word when set.  Unless the capacity test failed or the rule skips it, exactly its bytes go to
+    // out + written.  Its offsets and column go with its bytes (needed) or always (written), then the `copies`.  Everything
+    // goes on st_egress behind s.ev_egress; once it has landed the offsets are rebased.
+    int retire(gofr_engine* e, size_t ci, std::initializer_list<ColCopy> copies = {}) {
+        Posted& p = posted[ci % kSlots];
+        if (!p.live) return GOFR_OK;
+        p.live = false;
+        Slot& s = e->slots[ci % kSlots];
+        const cudaStream_t st = e->st_egress;
+        CUDA_TRY(cudaEventSynchronize(s.ev_served));
+        const uint32_t flag = *h_flag(s), total = *p.size;
+        if (flag) CUDA_TRY(cudaMemsetAsync(s.d_flag + k, 0, 4, st));
+        const bool wrote = p.put && !flag && written + total <= cap && written + total <= 0xFFFFFFFFull;
+        overflow |= flag || (p.put && !wrote);
+        if (wrote && total) CUDA_TRY(cudaMemcpyAsync(out + written, p.d_out, total, cudaMemcpyDeviceToHost, st));
+        if (wrote || (p.put && !needed)) {
+            CUDA_TRY(cudaMemcpyAsync(off + p.first, p.d_off, (size_t)p.n * 4, cudaMemcpyDeviceToHost, st));
+            CUDA_TRY(cudaMemcpyAsync(col + p.first, p.d_col, (size_t)p.n * 4, cudaMemcpyDeviceToHost, st));
+        }
+        int rc = copy_cols(copies, wrote, st);
+        if (!rc) rc = fence_egress(e, s);
+        if (rc) return rc;
+        CUDA_TRY(cudaEventSynchronize(s.ev_egress));
+        if (wrote) {
+            at = written;
+            written += total;
+            if (at) for (uint64_t i = p.first; i < p.first + p.n; i++) off[i] += (uint32_t)at;
+        }
+        return GOFR_OK;
+    }
+    // post, then for a pageable chunk retire at once: the connection calls, whose loop waits on each chunk anyway.
+    int ship(gofr_engine* e, Slot& s, size_t ci, const uint8_t* d_out, const uint32_t* d_off, const uint32_t* d_col, uint32_t n,
+             std::initializer_list<ColCopy> copies) {
+        int rc = post(e, s, ci, d_out, d_off, d_col, n, copies);
+        return rc || pinned ? rc : retire(e, ci, copies);
+    }
+    // The end of a batch, after finish: *bytes receives the bytes its chunks needed (needed) or the bytes written.  The
+    // closing offset off[recs.base] is stored when every chunk was written, and always when the output reports what was
+    // written; otherwise the error is fmt with the records, the bytes, the record capacity and cap (all unsigned long
+    // long), and the result GOFR_ERR_CAPACITY.
+    int report(gofr_engine* e, uint64_t* bytes, const char* fmt) const {
+        uint64_t b = written;
+        if (needed) {
+            b = 0;
+            for (size_t j = 0; j < shipped; j++) b += e->h_ends[4 * j + 2 * k + 1] - e->h_ends[4 * j + 2 * k];
+        }
+        *bytes = b;
+        const bool short_ = recs.short_ || overflow;
+        if (!short_ || !needed) off[recs.base] = (uint32_t)written;
+        if (!short_) return GOFR_OK;
+        set_last_error(fmt, (unsigned long long)recs.base, (unsigned long long)b, (unsigned long long)recs.cap, (unsigned long long)cap);
+        return GOFR_ERR_CAPACITY;
+    }
+    // Reads the pinned outputs' chain words back behind their egress and waits for it once (also when `wait`: other
+    // columns left on the egress stream).
+    static int finish(gofr_engine* e, uint32_t n, std::initializer_list<PackedOut*> outs, bool wait = false) {
+        for (PackedOut* o : outs) {
+            if (o->pinned) CUDA_TRY(cudaMemcpyAsync(&e->h_status[2 * o->k], e->d_chain + o->k, 8, cudaMemcpyDeviceToHost, e->st_egress));
+            wait |= o->pinned;
+        }
+        if (!wait) return GOFR_OK;
+        CUDA_TRY(wait_batch(e, n));
+        for (auto& s : e->slots) s.egress_pending = false;
+        for (PackedOut* o : outs)
+            if (o->pinned) { o->written = e->h_status[2 * o->k]; o->overflow = e->h_status[2 * o->k + 1] != 0; }
+        return GOFR_OK;
+    }
+
+private:
+    // A posted chunk: its device buffers and records, where its size is read back to, whether its records fit the record
+    // capacity (put) and whether it still waits for retire (live: pageable only).
+    struct Posted {
+        const uint8_t* d_out; const uint32_t* d_off; const uint32_t* d_col; uint32_t n; uint64_t first; uint32_t* size; bool put, live;
+    };
+    Posted posted[kSlots] = {};
+
+    // Advance on st_compute, then egress of the n records to the caller's from `first` on st_egress.  Without put
+    // neither runs and the overflow word is cleared.
     int deliver(gofr_engine* e, Slot& s, size_t ci, const uint8_t* d_out, const uint32_t* d_off, const uint32_t* d_col,
                 uint32_t n, uint64_t first, bool put) {
         ChunkInfo* info = e->d_info + k * kSlots + ci % kSlots;
@@ -980,90 +1103,9 @@ struct PackedOut {
         if (put) e->launches += 2;
         return GOFR_OK;
     }
-    // A chunk of `total` bytes at d_out, with the overflow word `flag` the caller read back (cleared here when set): unless
-    // put is false or the rule skips it, its bytes are copied to out + written on st and rebase() places its offsets.
-    int retire(Slot& s, const uint8_t* d_out, uint32_t total, uint32_t flag, bool put, cudaStream_t st, bool* wrote) {
-        if (flag) CUDA_TRY(cudaMemsetAsync(s.d_flag + k, 0, 4, st));
-        *wrote = put && !flag && written + total <= cap && written + total <= 0xFFFFFFFFull;
-        overflow |= flag || (put && !*wrote);
-        if (*wrote && total) CUDA_TRY(cudaMemcpyAsync(out + written, d_out, total, cudaMemcpyDeviceToHost, st));
-        if (*wrote) { at = written; written += total; }
-        return GOFR_OK;
-    }
-    void rebase(uint64_t first, uint32_t n) const { if (at) for (uint64_t i = first; i < first + n; i++) off[i] += (uint32_t)at; }
-    // Hands chunk ci's n records to the caller after the kernels on st_compute that left them in d_out / d_off (at
-    // *chain(e) & 15 when pinned, at 0 otherwise) and d_col, with the caller's copies.  The chunk's first and end offsets
-    // come back to h_ends, so that a batch short of cap still reports what it needed.  Pinned: deliver, the copies on
-    // st_egress behind the egress, then s.ev_egress.  Pageable: the overflow word and the chunk's size first, then exactly
-    // its bytes, its offsets and column and the copies on st_compute, then its offsets rebased.
-    int ship(gofr_engine* e, Slot& s, size_t ci, const uint8_t* d_out, const uint32_t* d_off, const uint32_t* d_col, uint32_t n,
-             std::initializer_list<ColCopy> copies) {
-        const uint64_t first = recs.base;
-        const bool put = recs.add(n) && n;
-        cudaStream_t st = e->st_compute;
-        uint32_t* ends = e->h_ends + 4 * shipped++ + 2 * k;
-        ends[0] = ends[1] = 0;
-        if (n) {
-            CUDA_TRY(cudaMemcpyAsync(&ends[0], d_off, 4, cudaMemcpyDeviceToHost, st));
-            CUDA_TRY(cudaMemcpyAsync(&ends[1], d_off + n, 4, cudaMemcpyDeviceToHost, st));
-        }
-        bool wrote = put;
-        if (pinned) {
-            int rc = deliver(e, s, ci, d_out, d_off, d_col, n, first, put);
-            if (rc) return rc;
-            st = e->st_egress;
-        } else {
-            CUDA_TRY(cudaMemcpyAsync(h_flag(s), s.d_flag + k, 4, cudaMemcpyDeviceToHost, st));
-            CUDA_TRY(cudaStreamSynchronize(st));
-            int rc = retire(s, d_out, ends[1], *h_flag(s), put, st, &wrote);
-            if (rc) return rc;
-            if (wrote) {
-                CUDA_TRY(cudaMemcpyAsync(off + first, d_off, (size_t)n * 4, cudaMemcpyDeviceToHost, st));
-                CUDA_TRY(cudaMemcpyAsync(col + first, d_col, (size_t)n * 4, cudaMemcpyDeviceToHost, st));
-            }
-        }
-        for (const ColCopy& c : copies)
-            if (c.dst && (wrote || !c.per_record)) CUDA_TRY(cudaMemcpyAsync(c.dst, c.src, c.bytes, cudaMemcpyDeviceToHost, st));
-        if (pinned) {
-            CUDA_TRY(cudaEventRecord(s.ev_egress, st));
-            s.egress_pending = true;
-        } else {
-            CUDA_TRY(cudaStreamSynchronize(st));
-            if (wrote) rebase(first, n);
-        }
-        return GOFR_OK;
-    }
-    // The end of a shipped batch, after finish: *bytes receives the bytes its chunks needed.  The closing offset
-    // off[recs.base] is stored when every chunk was written; otherwise the error is fmt with the records, the bytes, the
-    // record capacity and cap (all unsigned long long), and the result GOFR_ERR_CAPACITY.
-    int report(gofr_engine* e, uint64_t* bytes, const char* fmt) const {
-        uint64_t b = 0;
-        for (size_t j = 0; j < shipped; j++) b += e->h_ends[4 * j + 2 * k + 1] - e->h_ends[4 * j + 2 * k];
-        *bytes = b;
-        if (recs.short_ || overflow) {
-            set_last_error(fmt, (unsigned long long)recs.base, (unsigned long long)b, (unsigned long long)recs.cap, (unsigned long long)cap);
-            return GOFR_ERR_CAPACITY;
-        }
-        off[recs.base] = (uint32_t)written;
-        return GOFR_OK;
-    }
-    // Reads the pinned outputs' chain words back behind their egress and waits for it once.
-    static int finish(gofr_engine* e, uint32_t n, std::initializer_list<PackedOut*> outs) {
-        bool wait = false;
-        for (PackedOut* o : outs) {
-            if (o->pinned) CUDA_TRY(cudaMemcpyAsync(&e->h_status[2 * o->k], e->d_chain + o->k, 8, cudaMemcpyDeviceToHost, e->st_egress));
-            wait |= o->pinned;
-        }
-        if (!wait) return GOFR_OK;
-        CUDA_TRY(wait_batch(e, n));
-        for (auto& s : e->slots) s.egress_pending = false;
-        for (PackedOut* o : outs)
-            if (o->pinned) { o->written = e->h_status[2 * o->k]; o->overflow = e->h_status[2 * o->k + 1] != 0; }
-        return GOFR_OK;
-    }
 };
 
-// PackedOut::ship's read-backs for a batch of up to max_chunks chunks
+// PackedOut's first and end offsets for a batch of up to max_chunks chunks
 static int reserve_ends(gofr_engine* e, uint64_t max_chunks) {
     if (4 * max_chunks <= e->ends_cap) return GOFR_OK;
     if (e->h_ends) cudaFreeHost(e->h_ends);
@@ -1074,160 +1116,101 @@ static int reserve_ends(gofr_engine* e, uint64_t max_chunks) {
     return GOFR_OK;
 }
 
-// The chunk pipeline of the host-batch calls with a packed output (gofr_batch_submit, gofr_proto_batch_decode / _encode).
-// What differs between them:
-//   plan     the chunk that starts at record lo: its end, its input byte range and a bound on its device output; the
-//            records' input is validated here, chunk by chunk (see host_batch);
+// What the calls on a request or proto batch do per chunk, where they differ:
+//   plan     the chunk that starts at record lo: its end, its input byte range, a bound on its device output and, with a
+//            log, its log-arena range and a bound on its lines; the records' input is validated here, chunk by chunk
+//            (see host_batch);
 //   upload   the H2D copies of the chunk's input into the slot (and any buffers of the caller's own it needs);
-//   compute  the kernels that leave the chunk's packed output in the slot's d_out / d_off / d_meta, placed at
-//            *chain_pos & 15 when chain_pos is given (the serve kernel's convention), at 0 otherwise.
-// The pipeline reserves the slot, then runs upload and compute and hands the chunk to its PackedOut.
+//   compute  the kernels that leave the chunk's responses in the slot's d_out / d_off / d_meta, a packed output placed at
+//            *chain_pos & 15 when chain_pos is given (the serve kernel's convention), at 0 otherwise;
+//   lines    with a log, after the responses have shipped: the kernels that leave the chunk's packed lines in the slot's
+//            d_lout / d_loff, placed as compute places its output.
 struct ChunkSteps {
     std::function<int(uint32_t lo, ChunkPlan* c)> plan;
     std::function<int(Slot& s, const ChunkPlan& c, cudaStream_t st)> upload;
-    std::function<int(Slot& s, const ChunkPlan& c, cudaStream_t st, const unsigned long long* chain_pos)> compute;
+    std::function<int(Slot& s, const ChunkPlan& c, cudaStream_t st, const unsigned long long* chain_pos)> compute, lines;
 };
 
-static int run_chunks(gofr_engine* e, uint32_t n, const ChunkSteps& steps, gofr_resp_batch* out, gofr_ticket* ticket) {
-    out->out_bytes = 0;
+// The slot-layout responses of a chunk of n requests from lo: their size is known on the host (requests × slot bytes), so
+// they leave with three plain copies on the egress stream behind the serve kernel.
+static int ship_slots(gofr_engine* e, Slot& s, const gofr_slot_batch* out, uint32_t lo, uint32_t n) {
+    CUDA_TRY(cudaEventRecord(s.ev_served, e->st_compute));
+    CUDA_TRY(cudaStreamWaitEvent(e->st_egress, s.ev_served, 0));
+    CUDA_TRY(cudaMemcpyAsync(out->out + (size_t)lo * out->slot_bytes, s.d_out, (size_t)n * out->slot_bytes, cudaMemcpyDeviceToHost, e->st_egress));
+    CUDA_TRY(cudaMemcpyAsync(out->out_len + lo, s.d_off, (size_t)n * 4, cudaMemcpyDeviceToHost, e->st_egress));
+    CUDA_TRY(cudaMemcpyAsync(out->meta + lo, s.d_meta, (size_t)n * 4, cudaMemcpyDeviceToHost, e->st_egress));
+    return fence_egress(e, s);
+}
+
+// The chunk loop of the calls on a request or proto batch.  A call has one response output, packed (out) or in slots
+// (slots), and with a log the request-log lines (output 1, their per-record column meta).  Per chunk: plan, the slot's
+// buffers, upload on st_h2d, compute on st_compute, the responses shipped, then with a log the lines' kernels and the
+// lines.  A pageable chunk is retired when its slot comes round again, so kSlots of them are in flight, and the rest at
+// the end, oldest first.  The lines' kernel counts its lines into d_chain[2], read once at the end.
+static int req_chunks(gofr_engine* e, uint32_t n, const ChunkSteps& steps, gofr_resp_batch* out, const gofr_slot_batch* slots,
+                      gofr_batch_log* log, gofr_ticket* ticket) {
+    if (out) out->out_bytes = 0;
+    if (log) { log->lines = 0; log->out_bytes = 0; }
     if (n == 0) {  // nothing to do; the caller may have passed no buffers at all
-        if (out->out_off) out->out_off[0] = 0;
+        if (out && out->out_off) out->out_off[0] = 0;
+        if (log && log->log_off) log->log_off[0] = 0;
         complete(e, ticket, GOFR_OK);
         return GOFR_OK;
     }
-    PackedOut o(out->out, out->out_cap, out->out_off, out->meta, n, 0);
-    { int rc = o.start(e); if (rc) return rc; }
-    if (o.pinned) {  // ---- streaming path: egress is device driven, the host never blocks mid-batch ----
-        size_t ci = 0;
-        for (uint32_t lo = 0; lo < n; ci++) {
-            Slot& s = e->slots[ci % kSlots];
-            ChunkPlan c;
-            { int prc = steps.plan(lo, &c); if (prc) return prc; }
-            lo = c.hi;
-            uint32_t cn = c.hi - c.lo;
-            int rc = s.reserve(e, cn, (size_t)c.arena_hi - c.arena_lo, c.out_bound);
-            if (!rc) rc = steps.upload(s, c, e->st_h2d);
-            if (rc) return rc;
-            CUDA_TRY(cudaEventRecord(s.ev_h2d, e->st_h2d));
-            CUDA_TRY(cudaStreamWaitEvent(e->st_compute, s.ev_h2d, 0));
-            rc = steps.compute(s, c, e->st_compute, o.chain(e));
-            if (!rc) rc = o.deliver(e, s, ci, s.d_out, s.d_off, s.d_meta, cn, c.lo, true);
-            if (rc) return rc;
-            CUDA_TRY(cudaEventRecord(s.ev_egress, e->st_egress));
-            s.egress_pending = true;
-        }
-    } else {  // ---- pageable: 3-slot software pipeline, each chunk's exact size copied back once it is known ----
-        size_t issued = 0, finished = 0;
-        uint32_t next_lo = 0;
-        ChunkPlan inflight[kSlots];
-        // issue order == completion order == chunk order; out offsets are rebased on the host as chunks complete
-        while (next_lo < n || finished < issued) {
-            // keep up to kSlots chunks in flight
-            while (next_lo < n && issued - finished < (size_t)kSlots) {
-                int si = (int)(issued % kSlots);
-                Slot& s = e->slots[si];
-                ChunkPlan& c = inflight[si];
-                { int prc = steps.plan(next_lo, &c); if (prc) return prc; }
-                next_lo = c.hi;
-                uint32_t cn = c.hi - c.lo;
-                int rc = s.reserve(e, cn, (size_t)c.arena_hi - c.arena_lo, c.out_bound);
-                if (!rc) rc = steps.upload(s, c, s.stream);
-                if (!rc) rc = steps.compute(s, c, s.stream, nullptr);
-                if (rc) return rc;
-                CUDA_TRY(cudaMemcpyAsync(out->out_off + c.lo, s.d_off, (size_t)cn * 4, cudaMemcpyDeviceToHost, s.stream));
-                CUDA_TRY(cudaMemcpyAsync(out->meta + c.lo, s.d_meta, (size_t)cn * 4, cudaMemcpyDeviceToHost, s.stream));
-                CUDA_TRY(cudaMemcpyAsync(&s.h_tail[0], s.d_off + cn, 4, cudaMemcpyDeviceToHost, s.stream));
-                CUDA_TRY(cudaMemcpyAsync(o.h_flag(s), s.d_flag, 4, cudaMemcpyDeviceToHost, s.stream));
-                CUDA_TRY(cudaEventRecord(s.done, s.stream));
-                issued++;
-            }
-            // retire the oldest chunk: learn its size, then pull exactly that many bytes
-            Slot& s = e->slots[finished % kSlots];
-            const ChunkPlan& c = inflight[finished % kSlots];
-            CUDA_TRY(cudaEventSynchronize(s.done));
-            bool wrote = false;
-            { int rc = o.retire(s, s.d_out, s.h_tail[0], *o.h_flag(s), true, s.stream, &wrote); if (rc) return rc; }
-            if (wrote) o.rebase(c.lo, c.hi - c.lo);  // while the copy runs
-            CUDA_TRY(cudaStreamSynchronize(s.stream));
-            finished++;
-        }
+    // the calls with a log report what the batch needed, as the connection calls do; the others what was written
+    PackedOut ro, lo;
+    if (out) ro = PackedOut(out->out, out->out_cap, out->out_off, out->meta, n, 0, log != nullptr);
+    if (log) {
+        lo = PackedOut(log->out, log->out_cap, log->log_off, out ? out->meta : slots->meta, n, 1, true);
+        int rc = reserve_ends(e, (n + (uint64_t)e->chunk - 1) / e->chunk);  // a log's chunks are e->chunk requests
+        if (rc) return rc;
     }
-    { int rc = PackedOut::finish(e, n, {&o}); if (rc) return rc; }
-    if (o.overflow) set_last_error("output capacity too small (device chunk buffer or caller buffer)");
-    out->out_off[n] = (uint32_t)o.written;
-    out->out_bytes = o.written;
-    complete(e, ticket, o.overflow ? GOFR_ERR_CAPACITY : GOFR_OK);
-    return GOFR_OK;
-}
-
-static int batch_submit_locked(gofr_engine* e, const gofr_req_batch* in, gofr_resp_batch* out, gofr_ticket* ticket) {
-    ChunkSteps steps;
-    // Chunks are contiguous request ranges of e->chunk requests; a chunk's arena range is the min/max over its descriptors.
-    steps.plan = [&](uint32_t lo, ChunkPlan* c) -> int {
-        const uint32_t hi = std::min<uint32_t>(in->n, lo + e->chunk);
-        uint32_t alo = 0, ahi = 0;
-        uint64_t sizes[2];
-        int prc = chunk_arena_range(in, lo, hi, false, &alo, &ahi, sizes);
-        if (prc) return prc;
-        *c = {lo, hi, alo, ahi, chunk_out_bound(e, hi - lo, sizes)};
-        return GOFR_OK;
-    };
-    steps.upload = [&](Slot& s, const ChunkPlan& c, cudaStream_t st) -> int {
-        return upload_chunk(in, c.lo, c.hi - c.lo, c.arena_lo, c.arena_hi, s.d_desc, s.d_ids, s.d_arena, st);
-    };
-    // descriptors keep absolute arena offsets: pass a rebased arena pointer
-    steps.compute = [&](Slot& s, const ChunkPlan& c, cudaStream_t st, const unsigned long long* chain_pos) -> int {
-        return launch_serve(e, s.d_desc, s.d_ids, s.d_arena - c.arena_lo, c.hi - c.lo, in->date, s.d_out, s.cap_out, s.d_off,
-                            s.d_meta, &s.state, s.d_flag, s.d_bind, st, chain_pos);
-    };
-    return run_chunks(e, in->n, steps, out, ticket);
-}
-
-int gofr_batch_submit(gofr_engine* e, const gofr_req_batch* in, gofr_resp_batch* out, gofr_ticket* ticket) {
-    if (!e || !in || !out || !ticket) return GOFR_ERR_INVALID;
-    if (in->n && (!in->desc || !in->trace_ids || !out->out || !out->out_off || !out->meta)) return GOFR_ERR_INVALID;
-    return host_batch(e, [&] { return batch_submit_locked(e, in, out, ticket); });
-}
-
-static int batch_submit_slots_locked(gofr_engine* e, const gofr_req_batch* in, gofr_slot_batch* out, gofr_ticket* ticket) {
-    const uint32_t n = in->n, slot = out->slot_bytes;
-    const size_t nchunks = n ? (n + e->chunk - 1) / e->chunk : 0;
-    for (size_t ci = 0; ci < nchunks; ci++) {
+    { int rc = ro.start(e); if (!rc) rc = lo.start(e); if (rc) return rc; }
+    if (log) CUDA_TRY(cudaMemsetAsync(e->d_chain + 2, 0, 8, e->st_compute));
+    size_t ci = 0;
+    for (uint32_t next = 0; next < n; ci++) {
         Slot& s = e->slots[ci % kSlots];
-        // the chunk's request range and the arena bytes it covers (scanned right before the chunk is enqueued)
-        const uint32_t lo = (uint32_t)(ci * e->chunk), hi = std::min<uint32_t>(n, lo + e->chunk), cn = hi - lo;
-        uint32_t alo = 0, ahi = 0;
-        int rc = chunk_arena_range(in, lo, hi, false, &alo, &ahi);
-        const size_t obytes = (size_t)cn * slot;
-        if (!rc) rc = s.reserve(e, cn, (size_t)ahi - alo, obytes);
-        if (!rc) rc = upload_chunk(in, lo, cn, alo, ahi, s.d_desc, s.d_ids, s.d_arena, e->st_h2d);
+        ChunkPlan c;
+        int rc = ro.retire(e, ci);
+        if (!rc) rc = lo.retire(e, ci);
+        if (!rc) rc = steps.plan(next, &c);
+        if (rc) return rc;
+        next = c.hi;
+        const uint32_t cn = c.hi - c.lo;
+        rc = s.reserve(e, cn, (size_t)c.arena_hi - c.arena_lo, c.out_bound);
+        if (!rc && log) rc = s.reserve_lines(cn);
+        if (!rc && log) rc = s.reserve_line_bytes((size_t)c.log_hi - c.log_lo, c.log_bound);
+        if (!rc) rc = steps.upload(s, c, e->st_h2d);
         if (rc) return rc;
         CUDA_TRY(cudaEventRecord(s.ev_h2d, e->st_h2d));
         CUDA_TRY(cudaStreamWaitEvent(e->st_compute, s.ev_h2d, 0));
-        rc = launch_serve(e, s.d_desc, s.d_ids, s.d_arena - alo, cn, in->date, s.d_out, obytes, s.d_off, s.d_meta, nullptr, s.d_flag,
-                          s.d_bind, e->st_compute, nullptr, slot);
+        rc = steps.compute(s, c, e->st_compute, ro.chain(e));
+        if (!rc) rc = slots ? ship_slots(e, s, slots, c.lo, cn) : ro.post(e, s, ci, s.d_out, s.d_off, s.d_meta, cn);
+        if (!rc && log) rc = steps.lines(s, c, e->st_compute, lo.chain(e));
+        if (!rc && log) rc = lo.post(e, s, ci, s.d_lout, s.d_loff, s.d_meta, cn);
         if (rc) return rc;
-        CUDA_TRY(cudaEventRecord(s.ev_served, e->st_compute));
-        CUDA_TRY(cudaStreamWaitEvent(e->st_egress, s.ev_served, 0));
-        CUDA_TRY(cudaMemcpyAsync(out->out + (size_t)lo * slot, s.d_out, obytes, cudaMemcpyDeviceToHost, e->st_egress));
-        CUDA_TRY(cudaMemcpyAsync(out->out_len + lo, s.d_off, (size_t)cn * 4, cudaMemcpyDeviceToHost, e->st_egress));
-        CUDA_TRY(cudaMemcpyAsync(out->meta + lo, s.d_meta, (size_t)cn * 4, cudaMemcpyDeviceToHost, e->st_egress));
-        CUDA_TRY(cudaEventRecord(s.ev_egress, e->st_egress));
-        s.egress_pending = true;
     }
-    if (nchunks) {
-        CUDA_TRY(wait_batch(e, n));
-        for (auto& s : e->slots) s.egress_pending = false;
+    for (size_t j = ci; j < ci + kSlots; j++) {
+        int rc = ro.retire(e, j);
+        if (!rc) rc = lo.retire(e, j);
+        if (rc) return rc;
     }
-    complete(e, ticket, GOFR_OK);
+    { int rc = PackedOut::finish(e, n, {&ro, &lo}, slots != nullptr); if (rc) return rc; }
+    if (log) {
+        CUDA_TRY(cudaMemcpyAsync(&e->h_status[4], e->d_chain + 2, 8, cudaMemcpyDeviceToHost, e->st_compute));
+        CUDA_TRY(cudaStreamSynchronize(e->st_compute));
+        log->lines = (uint32_t)e->h_status[4];
+    }
+    int rc = GOFR_OK;
+    if (out)
+        rc = ro.report(e, &out->out_bytes, log ? "the batch needs %llu requests and %llu response bytes: n %llu, out_cap %llu"
+                                               : "output capacity too small (device chunk buffer or caller buffer)");
+    if (log) {
+        const int lrc = lo.report(e, &log->out_bytes, "the batch needs %llu log records and %llu log bytes: n %llu, out_cap %llu");
+        if (lrc) rc = lrc;
+    }
+    complete(e, ticket, rc);
     return GOFR_OK;
-}
-
-int gofr_batch_submit_slots(gofr_engine* e, const gofr_req_batch* in, gofr_slot_batch* out, gofr_ticket* ticket) {
-    if (!e || !in || !out || !ticket) return GOFR_ERR_INVALID;
-    if (in->n && (!in->desc || !in->trace_ids || !out->out || !out->out_len || !out->meta)) return GOFR_ERR_INVALID;
-    if (out->slot_bytes == 0 || (out->slot_bytes & 15u)) { set_last_error("slot_bytes must be a positive multiple of 16"); return GOFR_ERR_INVALID; }
-    return host_batch(e, [&] { return batch_submit_slots_locked(e, in, out, ticket); });
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -1527,10 +1510,10 @@ static int conn_batch_locked(gofr_engine* e, const gofr_conn_batch* in, const ui
     // chunks end at e->chunk connections or at the byte budget, where two neighbours together pass it
     const uint64_t max_chunks = (n + (uint64_t)e->chunk - 1) / e->chunk + 2 * (std::min<uint64_t>(in->buf_bytes, 1ull << 32) / kConnChunkBudget) + 2;
     { int rc = reserve_ends(e, max_chunks); if (rc) return rc; }
-    PackedOut ro(out->out, out->out_cap, out->out_off, out->meta, out->req_cap, 0), lo;
+    PackedOut ro(out->out, out->out_cap, out->out_off, out->meta, out->req_cap, 0, true), lo;
     { int rc = ro.start(e); if (rc) return rc; }
     if (log) {
-        lo = PackedOut(log->out, log->out_cap, log->log_off, log->log_req, log->line_cap, 1);
+        lo = PackedOut(log->out, log->out_cap, log->log_off, log->log_req, log->line_cap, 1, true);
         int rc = lo.start(e);
         if (rc) return rc;
     }
@@ -1663,7 +1646,7 @@ int gofr_conn_log_bound(const uint32_t* buf_off, const uint32_t* remote_off, uin
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// host batches with request-log lines (gofr_batch_submit_log, gofr_batch_submit_slots_log)
+// the serve calls on host batches: gofr_batch_submit / _slots, and with request-log lines _log
 // ---------------------------------------------------------------------------------------------------------------
 
 // The log records of requests [lo, hi): each is checked (its kind, its strings inside the arena), and *alo / *ahi receive
@@ -1693,95 +1676,70 @@ static int batch_log_plan(const gofr_batch_log* log, uint32_t lo, uint32_t hi, u
     return GOFR_OK;
 }
 
-// One call for both layouts: packed responses into `out`, or slots into `slots`.  Per chunk: the requests and their log
-// records and strings go up, the serve kernel answers, the serve-fed request-log kernel (batch_log_kernel.cu) writes each
-// request's line (empty for a request without one) in its own overflow word d_flag[1], chunk_pack_kernel places the lines
-// on the batch's chained position, and the lines leave as output 1 (PackedOut).  Line offsets are per request, so no count
-// comes back mid-batch; the kernel counts the lines into d_chain[2], read once at the end.  The lines carry meta as their
-// per-record column: the slot layout's meta leaves with them (and once more as a plain copy, so that it is complete when
-// only the log's capacity is short).
-static int batch_log_locked(gofr_engine* e, const gofr_req_batch* in, gofr_resp_batch* out, gofr_slot_batch* slots,
-                            gofr_batch_log* log, gofr_ticket* ticket) {
-    const uint32_t n = in->n;
-    log->lines = 0;
-    log->out_bytes = 0;
-    if (out) out->out_bytes = 0;
-    if (n == 0) {  // nothing to do; the caller may have passed no buffers at all
-        if (log->log_off) log->log_off[0] = 0;
-        if (out && out->out_off) out->out_off[0] = 0;
-        complete(e, ticket, GOFR_OK);
-        return GOFR_OK;
-    }
-    { int rc = reserve_ends(e, (n + (uint64_t)e->chunk - 1) / e->chunk); if (rc) return rc; }
-    uint32_t* meta = out ? out->meta : slots->meta;
-    PackedOut ro, lo(log->out, log->out_cap, log->log_off, meta, n, 1);
-    if (out) {
-        ro = PackedOut(out->out, out->out_cap, out->out_off, out->meta, n, 0);
-        int rc = ro.start(e);
+// The steps of the four serve calls: chunks of e->chunk requests, served into the packed layout (chained) or into slots
+// of slot_bytes.  With a log, each chunk's log records and the arena range of those that may get a line go up with its
+// requests; the serve-fed request-log kernel (batch_log_kernel.cu) reads each status from the chunk's meta and writes
+// every request's line (empty for a request without one) in its own overflow word d_flag[1], and chunk_pack_kernel
+// places the lines.  Line offsets are per request, so no count comes back mid-batch.
+static ChunkSteps serve_steps(gofr_engine* e, const gofr_req_batch* in, uint32_t slot_bytes, const gofr_batch_log* log) {
+    ChunkSteps steps;
+    steps.plan = [=](uint32_t lo, ChunkPlan* c) -> int {
+        const uint32_t hi = std::min<uint32_t>(in->n, lo + e->chunk);
+        uint64_t sizes[2];
+        *c = {lo, hi};
+        int rc = chunk_arena_range(in, lo, hi, false, &c->arena_lo, &c->arena_hi, sizes);
+        if (!rc && log) rc = batch_log_plan(log, lo, hi, &c->log_lo, &c->log_hi, &c->log_bound);
         if (rc) return rc;
-    }
-    { int rc = lo.start(e); if (rc) return rc; }
-    cudaStream_t st = e->st_compute;
-    unsigned long long* d_lines = e->d_chain + 2;
-    CUDA_TRY(cudaMemsetAsync(d_lines, 0, 8, st));
-    const int64_t log_ns = log->log_unix_ns;
-    for (size_t ci = 0; ci * e->chunk < n; ci++) {
-        Slot& s = e->slots[ci % kSlots];
-        const uint32_t c0 = (uint32_t)(ci * e->chunk), c1 = std::min<uint32_t>(n, c0 + e->chunk), cn = c1 - c0;
-        uint32_t alo = 0, ahi = 0, llo = 0, lhi = 0;
-        uint64_t sizes[2], lbytes = 0;
-        int rc = chunk_arena_range(in, c0, c1, false, &alo, &ahi, sizes);
-        if (!rc) rc = batch_log_plan(log, c0, c1, &llo, &lhi, &lbytes);
-        if (rc) return rc;
-        if (lbytes > 0xFFFFFFF0ull) {
-            set_last_error("the log lines of requests %u..%u could pass 4 GiB", c0, c1);
+        if (c->log_bound > 0xFFFFFFF0ull) {
+            set_last_error("the log lines of requests %u..%u could pass 4 GiB", lo, hi);
             return GOFR_ERR_UNSUPPORTED;
         }
-        const uint64_t obytes = out ? chunk_out_bound(e, cn, sizes) : (uint64_t)cn * slots->slot_bytes;
-        rc = s.reserve(e, cn, (size_t)ahi - alo, obytes);
-        if (!rc) rc = s.reserve_lines(cn);
-        if (!rc) rc = s.reserve_line_bytes((size_t)lhi - llo, lbytes);
-        if (!rc) rc = upload_chunk(in, c0, cn, alo, ahi, s.d_desc, s.d_ids, s.d_arena, e->st_h2d);
-        if (rc) return rc;
-        CUDA_TRY(cudaMemcpyAsync(s.d_ldesc, log->desc + c0, (size_t)cn * sizeof(gofr_log_desc), cudaMemcpyHostToDevice, e->st_h2d));
-        if (lhi > llo)
-            CUDA_TRY(cudaMemcpyAsync(s.d_larena, log->arena + llo, std::min<uint64_t>(lhi, log->arena_bytes) - llo, cudaMemcpyHostToDevice, e->st_h2d));
-        CUDA_TRY(cudaEventRecord(s.ev_h2d, e->st_h2d));
-        CUDA_TRY(cudaStreamWaitEvent(st, s.ev_h2d, 0));
-        rc = out ? launch_serve(e, s.d_desc, s.d_ids, s.d_arena - alo, cn, in->date, s.d_out, s.cap_out, s.d_off, s.d_meta, &s.state,
-                                s.d_flag, s.d_bind, st, ro.chain(e))
-                 : launch_serve(e, s.d_desc, s.d_ids, s.d_arena - alo, cn, in->date, s.d_out, obytes, s.d_off, s.d_meta, nullptr,
-                                s.d_flag, s.d_bind, st, nullptr, slots->slot_bytes);
-        if (!rc && out) rc = ro.ship(e, s, ci, s.d_out, s.d_off, s.d_meta, cn, {});
-        if (rc) return rc;
-        uint32_t* flag = s.d_flag + 1;
-        const uint32_t* d_meta = s.d_meta;
+        c->out_bound = slot_bytes ? (uint64_t)(hi - lo) * slot_bytes : chunk_out_bound(e, hi - lo, sizes);
+        return GOFR_OK;
+    };
+    steps.upload = [=](Slot& s, const ChunkPlan& c, cudaStream_t st) -> int {
+        const uint32_t cn = c.hi - c.lo;
+        int rc = upload_chunk(in, c.lo, cn, c.arena_lo, c.arena_hi, s.d_desc, s.d_ids, s.d_arena, st);
+        if (rc || !log) return rc;
+        CUDA_TRY(cudaMemcpyAsync(s.d_ldesc, log->desc + c.lo, (size_t)cn * sizeof(gofr_log_desc), cudaMemcpyHostToDevice, st));
+        if (c.log_hi > c.log_lo)
+            CUDA_TRY(cudaMemcpyAsync(s.d_larena, log->arena + c.log_lo, std::min<uint64_t>(c.log_hi, log->arena_bytes) - c.log_lo,
+                                     cudaMemcpyHostToDevice, st));
+        return GOFR_OK;
+    };
+    // descriptors keep absolute arena offsets: pass a rebased arena pointer
+    steps.compute = [=](Slot& s, const ChunkPlan& c, cudaStream_t st, const unsigned long long* chain_pos) -> int {
+        return launch_serve(e, s.d_desc, s.d_ids, s.d_arena - c.arena_lo, c.hi - c.lo, in->date, s.d_out,
+                            slot_bytes ? c.out_bound : s.cap_out, s.d_off, s.d_meta, &s.state, s.d_flag, s.d_bind, st, chain_pos,
+                            slot_bytes);
+    };
+    if (log) steps.lines = [=](Slot& s, const ChunkPlan& c, cudaStream_t st, const unsigned long long* chain_pos) -> int {
+        const uint32_t cn = c.hi - c.lo;
         LogParams lp;
         memset(&lp, 0, sizeof lp);
-        lp.desc = s.d_ldesc; lp.ids = s.d_ids; lp.arena = s.d_larena - llo;
-        rc = launch_frames_locked(e, K_BATCH_LOG, 0, lp, cn, s.d_lraw, s.cap_lraw - 16, s.d_lraw_off, s.state, flag, st, d_meta, log_ns, d_lines);
+        lp.desc = s.d_ldesc; lp.ids = s.d_ids; lp.arena = s.d_larena - c.log_lo;
+        int rc = launch_frames_locked(e, K_BATCH_LOG, 0, lp, cn, s.d_lraw, s.cap_lraw - 16, s.d_lraw_off, s.state, s.d_flag + 1, st,
+                                      (const uint32_t*)s.d_meta, log->log_unix_ns, e->d_chain + 2);
         if (rc) return rc;
         PackParams q;
         memset(&q, 0, sizeof q);
-        q.a = s.d_lraw; q.a_off = s.d_lraw_off; q.a_cap = s.cap_lraw - 16; q.chain_pos = lo.chain(e);
-        rc = launch_frames_locked(e, K_PACK, 0, q, cn, s.d_lout, s.cap_lout, s.d_loff, s.state, flag, st);
-        if (!rc && out) rc = lo.ship(e, s, ci, s.d_lout, s.d_loff, s.d_meta, cn, {});
-        if (!rc && !out)
-            rc = lo.ship(e, s, ci, s.d_lout, s.d_loff, s.d_meta, cn,
-                         {{slots->out + (size_t)c0 * slots->slot_bytes, s.d_out, (size_t)obytes, false},
-                          {slots->out_len + c0, s.d_off, (size_t)cn * 4, false},
-                          {slots->meta + c0, s.d_meta, (size_t)cn * 4, false}});
-        if (rc) return rc;
-    }
-    { int rc = out ? PackedOut::finish(e, n, {&ro, &lo}) : PackedOut::finish(e, n, {&lo}); if (rc) return rc; }
-    CUDA_TRY(cudaMemcpyAsync(&e->h_status[4], d_lines, 8, cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaStreamSynchronize(st));
-    log->lines = (uint32_t)e->h_status[4];
-    int final_rc = GOFR_OK;
-    if (out) final_rc = ro.report(e, &out->out_bytes, "the batch needs %llu requests and %llu response bytes: n %llu, out_cap %llu");
-    const int lrc = lo.report(e, &log->out_bytes, "the batch needs %llu log records and %llu log bytes: n %llu, out_cap %llu");
-    complete(e, ticket, lrc ? lrc : final_rc);
-    return GOFR_OK;
+        q.a = s.d_lraw; q.a_off = s.d_lraw_off; q.a_cap = s.cap_lraw - 16; q.chain_pos = chain_pos;
+        return launch_frames_locked(e, K_PACK, 0, q, cn, s.d_lout, s.cap_lout, s.d_loff, s.state, s.d_flag + 1, st);
+    };
+    return steps;
+}
+
+int gofr_batch_submit(gofr_engine* e, const gofr_req_batch* in, gofr_resp_batch* out, gofr_ticket* ticket) {
+    if (!e || !in || !out || !ticket) return GOFR_ERR_INVALID;
+    if (in->n && (!in->desc || !in->trace_ids || !out->out || !out->out_off || !out->meta)) return GOFR_ERR_INVALID;
+    return host_batch(e, [&] { return req_chunks(e, in->n, serve_steps(e, in, 0, nullptr), out, nullptr, nullptr, ticket); });
+}
+
+int gofr_batch_submit_slots(gofr_engine* e, const gofr_req_batch* in, gofr_slot_batch* out, gofr_ticket* ticket) {
+    if (!e || !in || !out || !ticket) return GOFR_ERR_INVALID;
+    if (in->n && (!in->desc || !in->trace_ids || !out->out || !out->out_len || !out->meta)) return GOFR_ERR_INVALID;
+    if (out->slot_bytes == 0 || (out->slot_bytes & 15u)) { set_last_error("slot_bytes must be a positive multiple of 16"); return GOFR_ERR_INVALID; }
+    return host_batch(e, [&] { return req_chunks(e, in->n, serve_steps(e, in, out->slot_bytes, nullptr), nullptr, out, nullptr, ticket); });
 }
 
 static bool batch_log_valid(const gofr_req_batch* in, const gofr_batch_log* log) {
@@ -1791,14 +1749,14 @@ static bool batch_log_valid(const gofr_req_batch* in, const gofr_batch_log* log)
 int gofr_batch_submit_log(gofr_engine* e, const gofr_req_batch* in, gofr_resp_batch* out, gofr_batch_log* log, gofr_ticket* ticket) {
     if (!e || !in || !out || !ticket || !batch_log_valid(in, log)) return GOFR_ERR_INVALID;
     if (in->n && (!in->desc || !in->trace_ids || !out->out || !out->out_off || !out->meta)) return GOFR_ERR_INVALID;
-    return host_batch(e, [&] { return batch_log_locked(e, in, out, nullptr, log, ticket); });
+    return host_batch(e, [&] { return req_chunks(e, in->n, serve_steps(e, in, 0, log), out, nullptr, log, ticket); });
 }
 
 int gofr_batch_submit_slots_log(gofr_engine* e, const gofr_req_batch* in, gofr_slot_batch* out, gofr_batch_log* log, gofr_ticket* ticket) {
     if (!e || !in || !out || !ticket || !batch_log_valid(in, log)) return GOFR_ERR_INVALID;
     if (in->n && (!in->desc || !in->trace_ids || !out->out || !out->out_len || !out->meta)) return GOFR_ERR_INVALID;
     if (out->slot_bytes == 0 || (out->slot_bytes & 15u)) { set_last_error("slot_bytes must be a positive multiple of 16"); return GOFR_ERR_INVALID; }
-    return host_batch(e, [&] { return batch_log_locked(e, in, nullptr, out, log, ticket); });
+    return host_batch(e, [&] { return req_chunks(e, in->n, serve_steps(e, in, out->slot_bytes, log), nullptr, out, log, ticket); });
 }
 
 int gofr_batch_log_bound(const gofr_log_desc* desc, uint32_t n, uint64_t* out_cap) {
@@ -2192,7 +2150,8 @@ int gofr_proto_nested_bound(const gofr_proto_nmsg* msgs, uint32_t n_msgs, const 
 // decoding (the two passes' rows and the packed chunk).
 static constexpr uint64_t kProtoChunkBudget = 256ull << 20;
 
-// The host-buffer calls of the nested codec: the chunk pipeline (run_chunks) with the codec kernels, then the pack kernel.
+// The host-buffer calls of the nested codec: the chunk loop of the request batches (req_chunks) with the codec kernels,
+// then the pack kernel.
 static int proto_batch_locked(gofr_engine* e, const PbnDesc& D, bool decode, const gofr_proto_batch* in, gofr_resp_batch* out,
                               gofr_ticket* ticket) {
     uint32_t per_byte = 0, per_record = 0;
@@ -2256,7 +2215,7 @@ static int proto_batch_locked(gofr_engine* e, const PbnDesc& D, bool decode, con
         if (!rc) rc = launch_frames_locked(e, K_PACK, 0, q, cn, s.d_out, s.cap_out, s.d_off, s.state, s.d_flag, st);
         return rc;
     };
-    return run_chunks(e, in->n, steps, out, ticket);
+    return req_chunks(e, in->n, steps, out, nullptr, nullptr, ticket);
 }
 
 static int proto_batch(gofr_engine* e, const gofr_proto_nmsg* msgs, uint32_t n_msgs, const gofr_proto_nfield* fields, uint32_t n_fields,
