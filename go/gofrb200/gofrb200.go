@@ -187,6 +187,23 @@ func (b *LogBatch) Append(start time.Time, elapsed time.Duration, now time.Time,
 	b.Arena = append(append(append(append(append(b.Arena, method...), userAgent...), xff...), remoteAddr...), requestURI...)
 }
 
+// AppendRPC packs what GoFr's gRPC LoggingInterceptor reads for one call (pkg/gofr/grpc/log.go:27-50): its start, the
+// handler's time.Since(start), the span's trace id and info.FullMethod.  The record asks for an RPCLog line
+// (GOFR_LOG_RPC); ProtoEncodeBatchLog fills its log time.
+func (b *LogBatch) AppendRPC(start time.Time, elapsed time.Duration, traceID [16]byte, method string) {
+	_, off := start.Zone()
+	var d C.gofr_log_desc
+	d.start_unix_ns = C.int64_t(start.UnixNano())
+	d.elapsed_ns = C.int64_t(elapsed.Nanoseconds())
+	d.arena_off = C.uint32_t(len(b.Arena))
+	d.method_len = C.uint16_t(len(method))
+	d.tz_offset_s = C.int32_t(off)
+	d.kind = C.GOFR_LOG_RPC
+	b.Desc = append(b.Desc, d)
+	b.TraceIDs = append(b.TraceIDs, traceID[:]...)
+	b.Arena = append(b.Arena, method...)
+}
+
 // SubmitLog serves one batch like Serve and writes middleware.Logging's line for each request in the same call
 // (gofr_batch_submit_log): log holds one record per request of b, appended with Append, whose status and clocks the call
 // fills from the response and from now; request i's line is lines[logOff[i]:logOff[i+1]], empty when mux answered it
@@ -798,6 +815,59 @@ func (e *Engine) ProtoEncodeBatch(msgs []ProtoNMsg, fields []ProtoNField, root u
 	return e.protoBatch(false, msgs, fields, root, presence, rows, off, out, outOff, meta)
 }
 
+// ProtoEncodeBatchLog marshals a batch of response rows like ProtoEncodeBatch and writes the gRPC LoggingInterceptor's
+// RPCLog line for each call in the same call (gofr_proto_batch_encode_log): log holds one record per row, appended with
+// AppendRPC; its log time is now.  A call whose handler failed passes an empty row: its frame is to be ignored, its line is
+// still written.  Call i's line is lines[logOff[i]:logOff[i+1]]; logOff needs len(off) entries; a short lines buffer is
+// gofr_batch_wait's GOFR_ERR_CAPACITY (gofr_batch_log_bound sizes it).  Returns the frame and line bytes the batch needed.
+func (e *Engine) ProtoEncodeBatchLog(msgs []ProtoNMsg, fields []ProtoNField, root uint32, presence []uint8, rows []byte, off []uint32,
+	log *LogBatch, now time.Time, out []byte, outOff, meta []uint32, lines []byte, logOff []uint32) (int, int, error) {
+	n := len(off) - 1
+	if n <= 0 {
+		return 0, 0, nil
+	}
+	if len(out) == 0 || len(outOff) < n+1 || len(meta) < n || len(log.Desc) != n || len(log.TraceIDs) < 16*n ||
+		len(logOff) < n+1 || len(lines) == 0 {
+		return 0, 0, errors.New("gofrb200: ProtoEncodeBatchLog columns too small")
+	}
+	pp, err := presenceArg(presence, fields)
+	if err != nil {
+		return 0, 0, err
+	}
+	var in C.gofr_proto_batch
+	if len(rows) > 0 {
+		in.data = (*C.uint8_t)(unsafe.Pointer(&rows[0]))
+	}
+	in.data_bytes = C.uint64_t(len(rows))
+	in.off = (*C.uint32_t)(unsafe.Pointer(&off[0]))
+	in.n = C.uint32_t(n)
+	var o C.gofr_resp_batch
+	o.out = (*C.uint8_t)(unsafe.Pointer(&out[0]))
+	o.out_cap = C.uint64_t(len(out))
+	o.out_off = (*C.uint32_t)(unsafe.Pointer(&outOff[0]))
+	o.meta = (*C.uint32_t)(unsafe.Pointer(&meta[0]))
+	var l C.gofr_batch_log
+	l.desc = &log.Desc[0]
+	if len(log.Arena) > 0 {
+		l.arena = (*C.uint8_t)(unsafe.Pointer(&log.Arena[0]))
+	}
+	l.arena_bytes = C.uint64_t(len(log.Arena))
+	l.log_unix_ns = C.int64_t(now.UnixNano())
+	l.out = (*C.uint8_t)(unsafe.Pointer(&lines[0]))
+	l.out_cap = C.uint64_t(len(lines))
+	l.log_off = (*C.uint32_t)(unsafe.Pointer(&logOff[0]))
+	var ticket C.gofr_ticket
+	cm, cf := (*C.gofr_proto_nmsg)(unsafe.Pointer(&msgs[0])), (*C.gofr_proto_nfield)(unsafe.Pointer(&fields[0]))
+	if err := check(C.gofr_proto_batch_encode_log(e.e, cm, C.uint32_t(len(msgs)), cf, C.uint32_t(len(fields)), C.uint32_t(root), pp, &in,
+		(*C.uint8_t)(unsafe.Pointer(&log.TraceIDs[0])), &o, &l, &ticket), "gofr_proto_batch_encode_log"); err != nil {
+		return 0, 0, err
+	}
+	if err := check(C.gofr_batch_wait(e.e, ticket), "gofr_batch_wait"); err != nil {
+		return 0, 0, err
+	}
+	return int(o.out_bytes), int(l.out_bytes), nil
+}
+
 // ProtoFrontend batches single messages from many goroutines through the nested codec (gofr_proto_frontend_*): the
 // per-message call grpc-go makes on its codec (encoding.Codec.Unmarshal for a request, Marshal for a response, on the
 // RPC's goroutine).  One message type, one direction.  Several ProtoFrontends and a Frontend may share one Engine.
@@ -805,6 +875,7 @@ type ProtoFrontend struct {
 	f         *C.gofr_proto_frontend
 	perByte   uint32
 	perRecord uint32
+	log       bool
 }
 
 // ErrProtoRecordTooLarge is what ProtoFrontend.Call returns, before anything is queued, for a record longer than the
@@ -834,7 +905,28 @@ func NewProtoFrontend(e *Engine, msgs []ProtoNMsg, fields []ProtoNField, root ui
 		C.uint32_t(maxWaitMicros), C.uint32_t(maxRecordBytes)), "gofr_proto_frontend_create"); err != nil {
 		return nil, err
 	}
-	return &ProtoFrontend{f, perByte, perRecord}, nil
+	return &ProtoFrontend{f, perByte, perRecord, false}, nil
+}
+
+// NewProtoFrontendLog creates the encode front-end of message type msgs[root] whose callers may also ask for their call's
+// RPCLog line (CallLog), for methods of at most maxLogBytes bytes (gofr_proto_frontend_create_log).
+func NewProtoFrontendLog(e *Engine, msgs []ProtoNMsg, fields []ProtoNField, root uint32, presence []uint8,
+	maxBatch, maxWaitMicros, maxRecordBytes, maxLogBytes int) (*ProtoFrontend, error) {
+	perByte, perRecord, err := ProtoNestedBound(msgs, fields, root, presence, false)
+	if err != nil {
+		return nil, err
+	}
+	pp, err := presenceArg(presence, fields)
+	if err != nil {
+		return nil, err
+	}
+	var f *C.gofr_proto_frontend
+	if err := check(C.gofr_proto_frontend_create_log(&f, e.e, (*C.gofr_proto_nmsg)(unsafe.Pointer(&msgs[0])), C.uint32_t(len(msgs)),
+		(*C.gofr_proto_nfield)(unsafe.Pointer(&fields[0])), C.uint32_t(len(fields)), C.uint32_t(root), pp, 0, C.uint32_t(maxBatch),
+		C.uint32_t(maxWaitMicros), C.uint32_t(maxRecordBytes), C.uint32_t(maxLogBytes)), "gofr_proto_frontend_create_log"); err != nil {
+		return nil, err
+	}
+	return &ProtoFrontend{f, perByte, perRecord, true}, nil
 }
 
 // Close must not run while a Call is in progress.
@@ -862,6 +954,32 @@ func (p *ProtoFrontend) Call(in []byte) (out []byte, status uint32, err error) {
 		return nil, 0, err
 	}
 	return buf[:n], uint32(st), nil
+}
+
+// CallLog is Call for an encode front-end made by NewProtoFrontendLog, plus the RPCLog line LoggingInterceptor writes once
+// the handler has returned: row is the handler's response (empty when it failed: the message is then to be ignored, the
+// line is still written), traceID the span's, start and elapsed the interceptor's clock around the handler, method
+// info.FullMethod.  The line is the batch's (gofr_proto_frontend_call_log); its buffer has room for the line's bound.  A row
+// longer than maxRecordBytes or a method longer than maxLogBytes is ErrProtoRecordTooLarge, before anything is queued.
+func (p *ProtoFrontend) CallLog(row []byte, traceID [16]byte, start time.Time, elapsed time.Duration, method string) (out []byte,
+	status uint32, line []byte, err error) {
+	if !p.log || len(method) > 0xFFFF {
+		return nil, 0, nil, errors.New("gofrb200: CallLog needs a front-end made by NewProtoFrontendLog and a method of at most 65535 bytes")
+	}
+	var lb LogBatch
+	lb.AppendRPC(start, elapsed, traceID, method)
+	buf := make([]byte, uint64(p.perByte)*uint64(len(row)+5)+uint64(p.perRecord))
+	lbuf := make([]byte, 320+7*len(method))
+	var n, st, ln C.uint32_t
+	rc := C.gofr_proto_frontend_call_log(p.f, bytesPtr(row), C.uint32_t(len(row)), (*C.uint8_t)(unsafe.Pointer(&traceID[0])), &lb.Desc[0],
+		bytesPtr(lb.Arena), bytesPtr(buf), C.uint32_t(len(buf)), &n, &st, bytesPtr(lbuf), C.uint32_t(len(lbuf)), &ln)
+	if rc == C.GOFR_ERR_CAPACITY {
+		return nil, 0, nil, ErrProtoRecordTooLarge
+	}
+	if err = check(rc, "gofr_proto_frontend_call_log"); err != nil {
+		return nil, 0, nil, err
+	}
+	return buf[:n], uint32(st), lbuf[:ln], nil
 }
 
 // ConnFrontend batches single reads from many connection goroutines through the connection pipeline

@@ -190,6 +190,10 @@ def lib():
     L.gofr_proto_frontend_destroy.restype = None
     L.gofr_proto_frontend_stats.argtypes = [vp, C.POINTER(u64), C.POINTER(u64)]
     L.gofr_proto_frontend_call.argtypes = [vp, C.c_char_p, u32, vp, u32, C.POINTER(u32), C.POINTER(u32)]
+    L.gofr_proto_frontend_create_log.argtypes = [C.POINTER(vp), vp, vp, u32, vp, u32, u32, vp, i32, u32, u32, u32, u32]
+    L.gofr_proto_frontend_set_log_clock.argtypes = [vp, C.c_int64]
+    L.gofr_proto_frontend_call_log.argtypes = [vp, C.c_char_p, u32, C.c_char_p, vp, C.c_char_p, vp, u32, C.POINTER(u32),
+                                               C.POINTER(u32), vp, u32, C.POINTER(u32)]
     L.gofr_conn_frontend_create.argtypes = [C.POINTER(vp), vp, u32, u32, u32, i32, C.c_int32, u64]
     L.gofr_conn_frontend_destroy.argtypes = [vp]
     L.gofr_conn_frontend_destroy.restype = None
@@ -220,6 +224,8 @@ def lib():
     L.gofr_batch_submit_log.argtypes = [vp, C.POINTER(ReqBatch), C.POINTER(RespBatch), C.POINTER(BatchLog), C.POINTER(u64)]
     L.gofr_batch_submit_slots_log.argtypes = [vp, C.POINTER(ReqBatch), C.POINTER(SlotBatch), C.POINTER(BatchLog), C.POINTER(u64)]
     L.gofr_batch_log_bound.argtypes = [vp, u32, C.POINTER(u64)]
+    L.gofr_proto_batch_encode_log.argtypes = [vp, vp, u32, vp, u32, u32, vp, C.POINTER(ProtoBatch), vp, C.POINTER(RespBatch),
+                                              C.POINTER(BatchLog), C.POINTER(u64)]
     L.gofr_frontend_create_log.argtypes = [C.POINTER(vp), vp, u32, u32, u32, u32, u32]
     L.gofr_frontend_set_log_clock.argtypes = [vp, C.c_int64]
     L.gofr_frontend_serve_log.argtypes = [vp, C.c_uint8, C.c_char_p, C.c_uint16, C.c_char_p, C.c_uint16, C.c_uint8, C.c_char_p,
@@ -243,9 +249,10 @@ DECLARED_SYMBOLS = [
     "gofr_table_route_count", "gofr_table_max_response_bytes", "gofr_engine_create", "gofr_engine_destroy",
     "gofr_serve_device", "gofr_serve_device_slots", "gofr_batch_submit", "gofr_batch_wait", "gofr_batch_submit_slots", "gofr_engine_set_chunk", "gofr_engine_set_tile",
     "gofr_engine_set_timing", "gofr_engine_overflowed", "gofr_engine_geometry", "gofr_engine_slot_ctas", "gofr_table_slot_ctas", "gofr_alloc_pinned", "gofr_free_pinned", "gofr_bind_host_thread", "gofr_bind_device", "gofr_batch_bind",
-    "gofr_grpc_hello_device", "gofr_requestlog_device", "gofr_batch_submit_log", "gofr_batch_submit_slots_log", "gofr_batch_log_bound", "gofr_http_parse_device", "gofr_http_frame_device", "gofr_conn_batch_submit", "gofr_conn_batch_bound", "gofr_conn_batch_submit_log", "gofr_conn_log_bound", "gofr_conn_batch_route", "gofr_conn_batch_respond", "gofr_conn_respond_bound", "gofr_conn_batch_respond_ex", "gofr_batch_route", "gofr_proto_encode_device", "gofr_proto_decode_device", "gofr_proto_encode_nested_device", "gofr_proto_decode_nested_device", "gofr_proto_nested_describe", "gofr_proto_encode_nested_ex_device", "gofr_proto_decode_nested_ex_device", "gofr_proto_nested_describe_ex", "gofr_proto_decode_nested_deferred_device", "gofr_proto_batch_decode", "gofr_proto_batch_encode", "gofr_proto_nested_bound", "gofr_table_response_bound", "gofr_frontend_create", "gofr_frontend_destroy", "gofr_frontend_set_clock",
+    "gofr_grpc_hello_device", "gofr_requestlog_device", "gofr_batch_submit_log", "gofr_batch_submit_slots_log", "gofr_batch_log_bound", "gofr_http_parse_device", "gofr_http_frame_device", "gofr_conn_batch_submit", "gofr_conn_batch_bound", "gofr_conn_batch_submit_log", "gofr_conn_log_bound", "gofr_conn_batch_route", "gofr_conn_batch_respond", "gofr_conn_respond_bound", "gofr_conn_batch_respond_ex", "gofr_batch_route", "gofr_proto_encode_device", "gofr_proto_decode_device", "gofr_proto_encode_nested_device", "gofr_proto_decode_nested_device", "gofr_proto_nested_describe", "gofr_proto_encode_nested_ex_device", "gofr_proto_decode_nested_ex_device", "gofr_proto_nested_describe_ex", "gofr_proto_decode_nested_deferred_device", "gofr_proto_batch_decode", "gofr_proto_batch_encode", "gofr_proto_batch_encode_log", "gofr_proto_nested_bound", "gofr_table_response_bound", "gofr_frontend_create", "gofr_frontend_destroy", "gofr_frontend_set_clock",
     "gofr_frontend_stats", "gofr_frontend_serve", "gofr_frontend_create_log", "gofr_frontend_set_log_clock", "gofr_frontend_serve_log", "gofr_proto_frontend_create", "gofr_proto_frontend_destroy",
-    "gofr_proto_frontend_stats", "gofr_proto_frontend_call", "gofr_conn_frontend_create", "gofr_conn_frontend_destroy",
+    "gofr_proto_frontend_stats", "gofr_proto_frontend_call", "gofr_proto_frontend_create_log", "gofr_proto_frontend_set_log_clock",
+    "gofr_proto_frontend_call_log", "gofr_conn_frontend_create", "gofr_conn_frontend_destroy",
     "gofr_conn_frontend_set_clock", "gofr_conn_frontend_stats", "gofr_conn_frontend_serve",
     "gofr_conn_app_frontend_create", "gofr_conn_app_frontend_destroy", "gofr_conn_app_frontend_set_clock",
     "gofr_conn_app_frontend_stats", "gofr_conn_app_frontend_route", "gofr_conn_app_frontend_respond",

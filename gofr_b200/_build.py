@@ -8,7 +8,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libgofr_b200.so")
-SOURCES = ["serve_kernel.cu", "serve_values_kernel.cu", "serve_slots_kernel.cu", "serve_slots_wide_kernel.cu", "serve_slots_values_kernel.cu", "grpc_kernel.cu", "proto_nested_kernel.cu", "proto_nested_decode_kernel.cu", "proto_nested_maps_kernel.cu", "proto_nested_presence_kernel.cu", "proto_nested_deferred_kernel.cu", "reqlog_kernel.cu", "batch_log_kernel.cu", "route_kernel.cu", "bind_kernel.cu", "http_kernel.cu", "http_frame_kernel.cu", "conn_kernel.cu", "conn_log_kernel.cu", "conn_result_kernel.cu", "egress_kernel.cu", "pack_kernel.cu", "engine.cu", "table_build.cpp", "frontend.cpp", "proto_frontend.cpp", "conn_frontend.cpp", "conn_app_frontend.cpp"]
+SOURCES = ["serve_kernel.cu", "serve_values_kernel.cu", "serve_slots_kernel.cu", "serve_slots_wide_kernel.cu", "serve_slots_values_kernel.cu", "grpc_kernel.cu", "proto_nested_kernel.cu", "proto_nested_decode_kernel.cu", "proto_nested_maps_kernel.cu", "proto_nested_presence_kernel.cu", "proto_nested_deferred_kernel.cu", "reqlog_kernel.cu", "batch_log_kernel.cu", "proto_log_kernel.cu", "route_kernel.cu", "bind_kernel.cu", "http_kernel.cu", "http_frame_kernel.cu", "conn_kernel.cu", "conn_log_kernel.cu", "conn_result_kernel.cu", "egress_kernel.cu", "pack_kernel.cu", "engine.cu", "table_build.cpp", "frontend.cpp", "proto_frontend.cpp", "conn_frontend.cpp", "conn_app_frontend.cpp"]
 HEADERS = ["frontend_ring.h", "conn_staging.h","frame_tiles.cuh", "pack_device.cuh", "proto_nested_codecs.cuh", "proto_nested_device.cuh", "proto_nested_decode_device.cuh", "proto_nested_deferred_device.cuh", "serve_body.cuh", "serve_device.cuh", "value_device.cuh", "float_device.cuh", "ryu_tables.inc", "el_tables.inc", "bind_device.cuh", "grpc_device.cuh", "reqlog_device.cuh", "reqlog_tiles.cuh", "batch_log_device.cuh", "http_device.cuh", "http_frame_device.cuh", "conn_device.cuh", "conn_log_device.cuh", "conn_result_device.cuh","tile_common.cuh", "table_format.h", "engine_internal.h",
            "../../include/gofr_b200.h"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC",

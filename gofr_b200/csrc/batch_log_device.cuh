@@ -1,6 +1,7 @@
-// batch_log_device.cuh — which request of a host batch gets middleware.Logging's line from gofr_batch_submit_log, and the
-// fields of its record the call fills.  Compiled for the device (batch_log_kernel.cu) and, through
-// tests/emu/emu_batch_log.cpp, for the host.
+// batch_log_device.cuh — which record of a host batch gets a log line from the calls that write one (gofr_batch_submit_log:
+// middleware.Logging's line; gofr_proto_batch_encode_log: the gRPC LoggingInterceptor's), and the fields of its record the
+// call fills.  Compiled for the device (batch_log_kernel.cu, proto_log_kernel.cu) and, through tests/emu/emu_batch_log.cpp
+// and tests/emu/emu_proto_log.cpp, for the host.
 #pragma once
 #include <stdint.h>
 
@@ -23,6 +24,16 @@ GOFR_INTERNAL_HD bool batch_log_fill(gofr_log_desc& d, uint32_t meta, int64_t lo
     d.status = (uint16_t)(meta & 0xFFFFu);
     d.log_unix_ns = log_ns;
     d.elapsed_ns = log_ns - d.start_unix_ns;
+    return true;
+}
+
+// Call i of an encode batch has a line exactly when the caller asked for one: LoggingInterceptor logs in its deferred
+// function (grpc/log.go:27-50), after the handler, whether or not the handler failed and before grpc-go marshals anything,
+// so neither the response row nor its encoding decides.  Its log time is the batch's; elapsed_ns is the caller's, who
+// measured time.Since(start) on the handler's own thread.
+GOFR_INTERNAL_HD bool proto_log_fill(gofr_log_desc& d, int64_t log_ns) {
+    if (d.kind != GOFR_LOG_RPC) return false;
+    d.log_unix_ns = log_ns;
     return true;
 }
 

@@ -18,9 +18,7 @@ struct ServeFed {
         memcpy(&g, &d, sizeof g);
         const bool line = batch_log_fill(g, __ldg(meta + i), log_ns);
         memcpy(&d, &g, sizeof g);
-        const uint32_t m = __activemask(), b = __ballot_sync(m, line);
-        if (line && (threadIdx.x & 31u) == (uint32_t)(__ffs(b) - 1)) atomicAdd(lines, (unsigned long long)__popc(b));
-        return line;
+        return count_line(line, lines);
     }
 };
 

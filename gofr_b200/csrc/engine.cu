@@ -67,6 +67,7 @@ __global__ void proto_decode_nested_presence_kernel(const GrpcParams p, const Pb
 __global__ void proto_decode_nested_deferred_kernel(const GrpcParams p, const uint32_t* meta_in, const PbnDesc D);  // proto_nested_deferred_kernel.cu
 __global__ void reqlog_kernel(const LogParams p);                // reqlog_kernel.cu
 __global__ void batch_log_kernel(const LogParams p, const uint32_t* meta, int64_t log_ns, unsigned long long* lines);  // batch_log_kernel.cu
+__global__ void proto_log_kernel(const LogParams p, int64_t log_ns, unsigned long long* lines);  // proto_log_kernel.cu
 __global__ void http_parse_kernel(const HttpParams p);           // http_kernel.cu
 __global__ void http_frame_kernel(const HttpFrameParams p);      // http_frame_kernel.cu
 __global__ void conn_compact_kernel(const ConnParams p);         // conn_kernel.cu
@@ -82,7 +83,7 @@ namespace {
 enum Kern {
     K_SERVE, K_SERVE_VALUES, K_SLOTS, K_SLOTS_WIDE, K_SLOTS_VALUES, K_HELLO, K_PROTO_ENC, K_PROTO_DEC, K_PBN_ENC, K_PBN_DEC,
     K_PBN_ENC_MAPS, K_PBN_DEC_MAPS, K_PBN_ENC_PRES, K_PBN_DEC_PRES, K_PBN_DEC_DEFERRED, K_REQLOG, K_HTTP, K_HTTP_FRAME, K_ROUTE, K_BIND, K_PACK,
-    K_CONN, K_CONN_LOG, K_CONN_RESULT, K_BATCH_LOG,
+    K_CONN, K_CONN_LOG, K_CONN_RESULT, K_BATCH_LOG, K_PROTO_LOG,
     K_COUNT
 };
 struct KernelRec {
@@ -116,6 +117,7 @@ const KernelRec kKernels[K_COUNT] = {
     {(const void*)conn_log_kernel, "connection log", kServeThreads},
     {(const void*)conn_result_kernel, "connection result", kServeThreads},
     {(const void*)batch_log_kernel, "batch log", kServeThreads},
+    {(const void*)proto_log_kernel, "proto log", kServeThreads},
 };
 
 constexpr int kSlots = 3;  // pipeline depth of the host-batch path
@@ -1125,10 +1127,13 @@ static int reserve_ends(gofr_engine* e, uint64_t max_chunks) {
 //            *chain_pos & 15 when chain_pos is given (the serve kernel's convention), at 0 otherwise;
 //   lines    with a log, after the responses have shipped: the kernels that leave the chunk's packed lines in the slot's
 //            d_lout / d_loff, placed as compute places its output.
+// max_chunks bounds the chunks plan cuts a batch into (0: chunks of e->chunk records); with a log, each chunk reads its
+// offsets back to h_ends.
 struct ChunkSteps {
     std::function<int(uint32_t lo, ChunkPlan* c)> plan;
     std::function<int(Slot& s, const ChunkPlan& c, cudaStream_t st)> upload;
     std::function<int(Slot& s, const ChunkPlan& c, cudaStream_t st, const unsigned long long* chain_pos)> compute, lines;
+    uint64_t max_chunks = 0;
 };
 
 // The slot-layout responses of a chunk of n requests from lo: their size is known on the host (requests × slot bytes), so
@@ -1162,7 +1167,7 @@ static int req_chunks(gofr_engine* e, uint32_t n, const ChunkSteps& steps, gofr_
     if (out) ro = PackedOut(out->out, out->out_cap, out->out_off, out->meta, n, 0, log != nullptr);
     if (log) {
         lo = PackedOut(log->out, log->out_cap, log->log_off, out ? out->meta : slots->meta, n, 1, true);
-        int rc = reserve_ends(e, (n + (uint64_t)e->chunk - 1) / e->chunk);  // a log's chunks are e->chunk requests
+        int rc = reserve_ends(e, steps.max_chunks ? steps.max_chunks : (n + (uint64_t)e->chunk - 1) / e->chunk);
         if (rc) return rc;
     }
     { int rc = ro.start(e); if (!rc) rc = lo.start(e); if (rc) return rc; }
@@ -1649,14 +1654,26 @@ int gofr_conn_log_bound(const uint32_t* buf_off, const uint32_t* remote_off, uin
 // the serve calls on host batches: gofr_batch_submit / _slots, and with request-log lines _log
 // ---------------------------------------------------------------------------------------------------------------
 
-// The log records of requests [lo, hi): each is checked (its kind, its strings inside the arena), and *alo / *ahi receive
-// the arena range of the records that may get a line (16-byte granular below), *bytes the bound of their lines.
-static int batch_log_plan(const gofr_batch_log* log, uint32_t lo, uint32_t hi, uint32_t* alo_out, uint32_t* ahi_out, uint64_t* bytes) {
+// The bytes a record's line may take (0 for GOFR_LOG_NONE): kConnLogFrame plus 6 per string byte, the most
+// encoding/json's escaping makes of one byte (\u00XX); an RPCLog method byte is escaped twice and may take 7 (\\u00XX,
+// rpc_method_slow in reqlog_device.cuh).
+static uint64_t log_line_bound(const gofr_log_desc& d) {
+    if (d.kind == GOFR_LOG_NONE) return 0;
+    const uint64_t len = (uint64_t)d.method_len + d.ua_len + d.xff_len + d.remote_len + d.uri_len;
+    return kConnLogFrame + 6 * len + (d.kind == GOFR_LOG_RPC ? d.method_len : 0);
+}
+
+// The log records of records [lo, hi): each is checked (its kind: `kind` or GOFR_LOG_NONE, its strings inside the arena),
+// and *alo / *ahi receive the arena range of the records that may get a line (16-byte granular below), *bytes the bound of
+// their lines.
+static int batch_log_plan(const gofr_batch_log* log, uint32_t kind, uint32_t lo, uint32_t hi, uint32_t* alo_out, uint32_t* ahi_out,
+                          uint64_t* bytes) {
     uint64_t alo = ~0ull, ahi = 0, b = 0;
     for (uint32_t i = lo; i < hi; i++) {
         const gofr_log_desc& d = log->desc[i];
-        if (d.kind != GOFR_LOG_REQUEST && d.kind != GOFR_LOG_NONE) {
-            set_last_error("log record %u: kind %u (GOFR_LOG_REQUEST or GOFR_LOG_NONE)", i, d.kind);
+        if (d.kind != kind && d.kind != GOFR_LOG_NONE) {
+            set_last_error("log record %u: kind %u (%s or GOFR_LOG_NONE)", i, d.kind,
+                           kind == GOFR_LOG_RPC ? "GOFR_LOG_RPC" : "GOFR_LOG_REQUEST");
             return GOFR_ERR_INVALID;
         }
         const uint64_t len = (uint64_t)d.method_len + d.ua_len + d.xff_len + d.remote_len + d.uri_len, end = d.arena_off + len;
@@ -1667,14 +1684,50 @@ static int batch_log_plan(const gofr_batch_log* log, uint32_t lo, uint32_t hi, u
         if (d.kind == GOFR_LOG_NONE) continue;
         alo = std::min<uint64_t>(alo, d.arena_off);
         ahi = std::max(ahi, end);
-        b += kConnLogFrame + 6 * len;
+        b += log_line_bound(d);
     }
     if (ahi == 0) alo = 0;
     *alo_out = (uint32_t)(alo & ~15ull);
     *ahi_out = (uint32_t)ahi;
     *bytes = b;
+    if (b > 0xFFFFFFF0ull) {
+        set_last_error("the log lines of records %u..%u could pass 4 GiB", lo, hi);
+        return GOFR_ERR_UNSUPPORTED;
+    }
     return GOFR_OK;
 }
+
+// The upload of a chunk's log records and the arena range of those that may get a line, on st; with ids, the chunk's
+// trace ids too (to d_lids: the proto calls have no request ids of their own).
+static int upload_log(Slot& s, const ChunkPlan& c, const gofr_batch_log* log, const uint8_t* ids, cudaStream_t st) {
+    const uint32_t cn = c.hi - c.lo;
+    CUDA_TRY(cudaMemcpyAsync(s.d_ldesc, log->desc + c.lo, (size_t)cn * sizeof(gofr_log_desc), cudaMemcpyHostToDevice, st));
+    if (ids) CUDA_TRY(cudaMemcpyAsync(s.d_lids, ids + (size_t)c.lo * 16, (size_t)cn * 16, cudaMemcpyHostToDevice, st));
+    if (c.log_hi > c.log_lo)
+        CUDA_TRY(cudaMemcpyAsync(s.d_larena, log->arena + c.log_lo, std::min<uint64_t>(c.log_hi, log->arena_bytes) - c.log_lo,
+                                 cudaMemcpyHostToDevice, st));
+    return GOFR_OK;
+}
+
+// The lines step: request-log kernel k over the chunk's records (ids: their trace ids on the device; `extra` the
+// instance's parameters after LogParams) writes every record's line in the lines' overflow word d_flag[1], then
+// chunk_pack_kernel places them at *chain_pos & 15.
+extern "C++" {
+template <class... Extra>
+static int chunk_lines(gofr_engine* e, Kern k, Slot& s, const ChunkPlan& c, const void* ids, cudaStream_t st,
+                       const unsigned long long* chain_pos, const Extra&... extra) {
+    const uint32_t cn = c.hi - c.lo;
+    LogParams lp;
+    memset(&lp, 0, sizeof lp);
+    lp.desc = s.d_ldesc; lp.ids = ids; lp.arena = s.d_larena - c.log_lo;
+    int rc = launch_frames_locked(e, k, 0, lp, cn, s.d_lraw, s.cap_lraw - 16, s.d_lraw_off, s.state, s.d_flag + 1, st, extra...);
+    if (rc) return rc;
+    PackParams q;
+    memset(&q, 0, sizeof q);
+    q.a = s.d_lraw; q.a_off = s.d_lraw_off; q.a_cap = s.cap_lraw - 16; q.chain_pos = chain_pos;
+    return launch_frames_locked(e, K_PACK, 0, q, cn, s.d_lout, s.cap_lout, s.d_loff, s.state, s.d_flag + 1, st);
+}
+}  // extern "C++"
 
 // The steps of the four serve calls: chunks of e->chunk requests, served into the packed layout (chained) or into slots
 // of slot_bytes.  With a log, each chunk's log records and the arena range of those that may get a line go up with its
@@ -1688,24 +1741,15 @@ static ChunkSteps serve_steps(gofr_engine* e, const gofr_req_batch* in, uint32_t
         uint64_t sizes[2];
         *c = {lo, hi};
         int rc = chunk_arena_range(in, lo, hi, false, &c->arena_lo, &c->arena_hi, sizes);
-        if (!rc && log) rc = batch_log_plan(log, lo, hi, &c->log_lo, &c->log_hi, &c->log_bound);
+        if (!rc && log) rc = batch_log_plan(log, GOFR_LOG_REQUEST, lo, hi, &c->log_lo, &c->log_hi, &c->log_bound);
         if (rc) return rc;
-        if (c->log_bound > 0xFFFFFFF0ull) {
-            set_last_error("the log lines of requests %u..%u could pass 4 GiB", lo, hi);
-            return GOFR_ERR_UNSUPPORTED;
-        }
         c->out_bound = slot_bytes ? (uint64_t)(hi - lo) * slot_bytes : chunk_out_bound(e, hi - lo, sizes);
         return GOFR_OK;
     };
     steps.upload = [=](Slot& s, const ChunkPlan& c, cudaStream_t st) -> int {
         const uint32_t cn = c.hi - c.lo;
         int rc = upload_chunk(in, c.lo, cn, c.arena_lo, c.arena_hi, s.d_desc, s.d_ids, s.d_arena, st);
-        if (rc || !log) return rc;
-        CUDA_TRY(cudaMemcpyAsync(s.d_ldesc, log->desc + c.lo, (size_t)cn * sizeof(gofr_log_desc), cudaMemcpyHostToDevice, st));
-        if (c.log_hi > c.log_lo)
-            CUDA_TRY(cudaMemcpyAsync(s.d_larena, log->arena + c.log_lo, std::min<uint64_t>(c.log_hi, log->arena_bytes) - c.log_lo,
-                                     cudaMemcpyHostToDevice, st));
-        return GOFR_OK;
+        return rc || !log ? rc : upload_log(s, c, log, nullptr, st);
     };
     // descriptors keep absolute arena offsets: pass a rebased arena pointer
     steps.compute = [=](Slot& s, const ChunkPlan& c, cudaStream_t st, const unsigned long long* chain_pos) -> int {
@@ -1714,17 +1758,7 @@ static ChunkSteps serve_steps(gofr_engine* e, const gofr_req_batch* in, uint32_t
                             slot_bytes);
     };
     if (log) steps.lines = [=](Slot& s, const ChunkPlan& c, cudaStream_t st, const unsigned long long* chain_pos) -> int {
-        const uint32_t cn = c.hi - c.lo;
-        LogParams lp;
-        memset(&lp, 0, sizeof lp);
-        lp.desc = s.d_ldesc; lp.ids = s.d_ids; lp.arena = s.d_larena - c.log_lo;
-        int rc = launch_frames_locked(e, K_BATCH_LOG, 0, lp, cn, s.d_lraw, s.cap_lraw - 16, s.d_lraw_off, s.state, s.d_flag + 1, st,
-                                      (const uint32_t*)s.d_meta, log->log_unix_ns, e->d_chain + 2);
-        if (rc) return rc;
-        PackParams q;
-        memset(&q, 0, sizeof q);
-        q.a = s.d_lraw; q.a_off = s.d_lraw_off; q.a_cap = s.cap_lraw - 16; q.chain_pos = chain_pos;
-        return launch_frames_locked(e, K_PACK, 0, q, cn, s.d_lout, s.cap_lout, s.d_loff, s.state, s.d_flag + 1, st);
+        return chunk_lines(e, K_BATCH_LOG, s, c, s.d_ids, st, chain_pos, (const uint32_t*)s.d_meta, log->log_unix_ns, e->d_chain + 2);
     };
     return steps;
 }
@@ -1762,9 +1796,7 @@ int gofr_batch_submit_slots_log(gofr_engine* e, const gofr_req_batch* in, gofr_s
 int gofr_batch_log_bound(const gofr_log_desc* desc, uint32_t n, uint64_t* out_cap) {
     if (!out_cap || (n && !desc)) return GOFR_ERR_INVALID;
     uint64_t b = 0;
-    for (uint32_t i = 0; i < n; i++)
-        if (desc[i].kind != GOFR_LOG_NONE)
-            b += kConnLogFrame + 6ull * ((uint64_t)desc[i].method_len + desc[i].ua_len + desc[i].xff_len + desc[i].remote_len + desc[i].uri_len);
+    for (uint32_t i = 0; i < n; i++) b += log_line_bound(desc[i]);
     *out_cap = b;
     return GOFR_OK;
 }
@@ -2151,9 +2183,11 @@ int gofr_proto_nested_bound(const gofr_proto_nmsg* msgs, uint32_t n_msgs, const 
 static constexpr uint64_t kProtoChunkBudget = 256ull << 20;
 
 // The host-buffer calls of the nested codec: the chunk loop of the request batches (req_chunks) with the codec kernels,
-// then the pack kernel.
+// then the pack kernel.  With a log (encode only): each chunk's log records, their arena range and trace_ids go up with its
+// rows, and after the frames have shipped the proto-fed request-log kernel (proto_log_kernel.cu) writes every record's
+// line, which is empty unless its kind is GOFR_LOG_RPC; chunk_pack_kernel places the lines.
 static int proto_batch_locked(gofr_engine* e, const PbnDesc& D, bool decode, const gofr_proto_batch* in, gofr_resp_batch* out,
-                              gofr_ticket* ticket) {
+                              gofr_batch_log* log, const uint8_t* trace_ids, gofr_ticket* ticket) {
     uint32_t per_byte = 0, per_record = 0;
     pbn_bound(D, decode, &per_byte, &per_record);
     const uint32_t levels = pbn_map_levels(D, D.root);
@@ -2185,14 +2219,18 @@ static int proto_batch_locked(gofr_engine* e, const PbnDesc& D, bool decode, con
         // a single record with a larger bound gets a chunk of its own; no output offset passes 32 bits, so neither does a
         // buffer (a record that would is reported as a capacity error by the kernels)
         *c = {lo, hi, (uint32_t)(start & ~15ull), off[hi], std::min<uint64_t>(bound, 1ull << 32) + 16};
-        return GOFR_OK;
+        return log ? batch_log_plan(log, GOFR_LOG_RPC, lo, hi, &c->log_lo, &c->log_hi, &c->log_bound) : GOFR_OK;
     };
+    // A chunk ends at e->chunk records, or where it and the next chunk's first record together pass the budget: two
+    // neighbours' bounds, which sum to at most per_byte * data_bytes + per_record * n over the batch, take more than it.
+    const uint64_t n = in->n, all = (uint64_t)per_byte * in->data_bytes + (uint64_t)per_record * n;
+    steps.max_chunks = (n + e->chunk - 1) / e->chunk + 2 * (all / kProtoChunkBudget) + 2;
     steps.upload = [&](Slot& s, const ChunkPlan& c, cudaStream_t st) -> int {
         const uint32_t cn = c.hi - c.lo;
         { int rc = s.reserve_codec(cn, c.out_bound, decode ? c.out_bound : 0); if (rc) return rc; }
         CUDA_TRY(cudaMemcpyAsync(s.d_in_off, off + c.lo, (size_t)(cn + 1) * 4, cudaMemcpyHostToDevice, st));
         if (c.arena_hi > c.arena_lo) CUDA_TRY(cudaMemcpyAsync(s.d_arena, in->data + c.arena_lo, c.arena_hi - c.arena_lo, cudaMemcpyHostToDevice, st));
-        return GOFR_OK;
+        return log ? upload_log(s, c, log, trace_ids, st) : GOFR_OK;
     };
     // records keep their absolute offsets: pass a rebased input pointer.  The codec kernels write from byte 0 of their own
     // buffers (16 bytes short of their end: the pack kernel's copy reads a word past a record's last byte).
@@ -2215,18 +2253,21 @@ static int proto_batch_locked(gofr_engine* e, const PbnDesc& D, bool decode, con
         if (!rc) rc = launch_frames_locked(e, K_PACK, 0, q, cn, s.d_out, s.cap_out, s.d_off, s.state, s.d_flag, st);
         return rc;
     };
-    return req_chunks(e, in->n, steps, out, nullptr, nullptr, ticket);
+    if (log) steps.lines = [&](Slot& s, const ChunkPlan& c, cudaStream_t st, const unsigned long long* chain_pos) -> int {
+        return chunk_lines(e, K_PROTO_LOG, s, c, s.d_lids, st, chain_pos, log->log_unix_ns, e->d_chain + 2);
+    };
+    return req_chunks(e, in->n, steps, out, nullptr, log, ticket);
 }
 
 static int proto_batch(gofr_engine* e, const gofr_proto_nmsg* msgs, uint32_t n_msgs, const gofr_proto_nfield* fields, uint32_t n_fields,
                        uint32_t root, const uint8_t* presence, const gofr_proto_batch* in, gofr_resp_batch* out, gofr_ticket* ticket,
-                       bool decode) {
+                       bool decode, gofr_batch_log* log = nullptr, const uint8_t* trace_ids = nullptr) {
     if (!e || !in || !out || !ticket) return GOFR_ERR_INVALID;
     if (in->n && (!in->off || !out->out || !out->out_off || !out->meta)) return GOFR_ERR_INVALID;
     if (in->data_bytes && !in->data) return GOFR_ERR_INVALID;
     PbnDesc D;
     { int rc = pbn_build(msgs, n_msgs, fields, n_fields, root, presence, &D); if (rc) return rc; }
-    return host_batch(e, [&] { return proto_batch_locked(e, D, decode, in, out, ticket); });
+    return host_batch(e, [&] { return proto_batch_locked(e, D, decode, in, out, log, trace_ids, ticket); });
 }
 
 int gofr_proto_batch_decode(gofr_engine* e, const gofr_proto_nmsg* msgs, uint32_t n_msgs, const gofr_proto_nfield* fields, uint32_t n_fields,
@@ -2237,6 +2278,13 @@ int gofr_proto_batch_decode(gofr_engine* e, const gofr_proto_nmsg* msgs, uint32_
 int gofr_proto_batch_encode(gofr_engine* e, const gofr_proto_nmsg* msgs, uint32_t n_msgs, const gofr_proto_nfield* fields, uint32_t n_fields,
                             uint32_t root, const uint8_t* presence, const gofr_proto_batch* in, gofr_resp_batch* out, gofr_ticket* ticket) {
     return proto_batch(e, msgs, n_msgs, fields, n_fields, root, presence, in, out, ticket, false);
+}
+
+int gofr_proto_batch_encode_log(gofr_engine* e, const gofr_proto_nmsg* msgs, uint32_t n_msgs, const gofr_proto_nfield* fields,
+                                uint32_t n_fields, uint32_t root, const uint8_t* presence, const gofr_proto_batch* in,
+                                const uint8_t* trace_ids, gofr_resp_batch* out, gofr_batch_log* log, gofr_ticket* ticket) {
+    if (!log || (in && in->n && (!log->desc || !log->out || !log->log_off || !trace_ids))) return GOFR_ERR_INVALID;
+    return proto_batch(e, msgs, n_msgs, fields, n_fields, root, presence, in, out, ticket, false, log, trace_ids);
 }
 
 // the descriptor gofr_proto_encode_nested_device would hand to its kernel (tests/emu drives the device code with it)

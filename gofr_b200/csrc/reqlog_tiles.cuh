@@ -1,9 +1,10 @@
 // reqlog_tiles.cuh — the tile loop of the request-log kernels (sm_90a), one thread per record on the tile skeleton of
 // tile_common.cuh; lines are packed in record order through the staging Writer.  Per-record logic: reqlog_device.cuh.
 //
-// Two instances: reqlog_kernel.cu (gofr_requestlog_device, the connection path's lines) takes every record as it is;
+// Three instances: reqlog_kernel.cu (gofr_requestlog_device, the connection path's lines) takes every record as it is;
 // batch_log_kernel.cu (gofr_batch_submit_log) first lets the serve kernel's status decide, per record, whether it has a
-// line at all (batch_log_device.cuh).  The Feed does that: feed(i, d) may rewrite record i and returns whether it has a
+// line at all, and proto_log_kernel.cu (gofr_proto_batch_encode_log) lets the record's kind decide (batch_log_device.cuh).
+// The Feed does that: feed(i, d) may rewrite record i and returns whether it has a
 // line; a record without one takes no staged bytes and gets an empty line.  Feed::kEvery says every record has one (the
 // first instance: its code stays what it was before the loop was shared).
 #pragma once
@@ -29,6 +30,14 @@ struct LogShared {
     uint32_t stage[GOFR_STAGE_WORDS * LT];
     __align__(16) uint8_t in[kLogStage + 32];
 };
+
+// A Feed's line count: each warp adds the lines of its records to *lines, the batch's count, so that it never has to come
+// back mid-batch.  Returns `line`.
+__device__ __forceinline__ bool count_line(bool line, unsigned long long* lines) {
+    const uint32_t m = __activemask(), b = __ballot_sync(m, line);
+    if (line && (threadIdx.x & 31u) == (uint32_t)(__ffs(b) - 1)) atomicAdd(lines, (unsigned long long)__popc(b));
+    return line;
+}
 
 template <class Feed>
 __device__ __forceinline__ void reqlog_tiles(const LogParams p, const Feed feed) {

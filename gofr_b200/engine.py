@@ -741,6 +741,48 @@ def _serve_host_log(self, batch: S.RequestBatch, date: bytes, log: S.LogBatch, l
 Engine.serve_host_log = _serve_host_log
 
 
+def _proto_encode_batch_log(self, msgs, root: int, rows: np.ndarray, row_off: np.ndarray, log: S.LogBatch, log_unix_ns: int,
+                            pinned: bool = True, log_pinned: Optional[bool] = None, out_cap: Optional[int] = None,
+                            log_out_cap: Optional[int] = None, raise_on_capacity: bool = True) -> BatchLogResult:
+    """gofr_proto_batch_encode_log + wait: rows in host memory → the frames gofr_proto_batch_encode gives, and for every
+    LogBatch record of kind LOG_RPC the gRPC LoggingInterceptor's RPCLog line (LOG_NONE: an empty line).  The log batch's
+    trace ids are the lines' ids; its start, elapsed time, zone and method are the caller's, log_unix_ns the batch's.  The
+    frames and lines go to pinned (device-driven egress) or pageable buffers, each its own (log_pinned defaults to pinned)."""
+    L = _abi.lib()
+    n = len(row_off) - 1
+    assert log.n == n
+    rows = np.ascontiguousarray(rows, dtype=np.uint8)
+    row_off = np.ascontiguousarray(row_off, dtype=np.uint32)
+    if out_cap is None:
+        per_byte, per_record = nested_bound(msgs, root, False)
+        out_cap = per_byte * int(row_off[-1] - row_off[0]) + per_record * n if n else 0
+    if log_out_cap is None:
+        log_out_cap = batch_log_bound(log)
+    alloc, lalloc = _alloc(pinned), _alloc(pinned if log_pinned is None else log_pinned)
+    out, out_off, meta = alloc(out_cap + 16, np.uint8), alloc(n + 1, np.uint32), alloc(n, np.uint32)
+    out[out_cap:] = 0xAB        # 16 bytes past each capacity that the call must leave alone
+    lout, log_off = lalloc(log_out_cap + 16, np.uint8), lalloc(n + 1, np.uint32)
+    lout[log_out_cap:] = 0xAB
+    nm, nf, k = S.proto_nested_tables(msgs)
+    pr = S.proto_nested_presence(msgs)
+    pb = _abi.ProtoBatch(data=rows.ctypes.data, data_bytes=rows.size, off=row_off.ctypes.data, n=n)
+    ob = _abi.RespBatch(out=out.ctypes.data, out_cap=out_cap, out_off=out_off.ctypes.data, meta=meta.ctypes.data, out_bytes=0)
+    lb = _abi.BatchLog(desc=log.desc.ctypes.data, arena=log.arena.ctypes.data if log.arena.size else None,
+                       arena_bytes=log.arena.size, log_unix_ns=log_unix_ns, out=lout.ctypes.data, out_cap=log_out_cap,
+                       log_off=log_off.ctypes.data, lines=0, reserved=0, out_bytes=0)
+    t = C.c_uint64()
+    _abi.check(L.gofr_proto_batch_encode_log(self._e, nm.ctypes.data, len(msgs), nf.ctypes.data, k, root,
+                                             None if pr is None else pr.ctypes.data, C.byref(pb), log.trace_ids.ctypes.data,
+                                             C.byref(ob), C.byref(lb), C.byref(t)), "gofr_proto_batch_encode_log")
+    rc = int(L.gofr_batch_wait(self._e, t.value))
+    if rc and (raise_on_capacity or rc != 7):
+        _abi.check(rc, "gofr_batch_wait")
+    return BatchLogResult(out, out_off, None, meta[:n], lout, log_off, int(lb.lines), int(lb.out_bytes), int(ob.out_bytes), rc)
+
+
+Engine.proto_encode_batch_log = _proto_encode_batch_log
+
+
 def pinned_array(nbytes: int, dtype=np.uint8) -> np.ndarray:
     """numpy view over cudaMallocHost memory (gofr_alloc_pinned).  The memory lives until process exit."""
     L = _abi.lib()

@@ -89,21 +89,29 @@ class Frontend:
 
 class ProtoFrontend:
     """One message type (spec.ProtoNField lists, as for Engine.proto_decode_batch) in one direction.  decode: call(message
-    without the 5-byte prefix) → (row, status); encode: call(row) → (marshalled message without the prefix, status)."""
+    without the 5-byte prefix) → (row, status); encode: call(row) → (marshalled message without the prefix, status).
+    max_log_bytes (encode only): log staging of that many method bytes per call (gofr_proto_frontend_create_log), so that
+    call takes log=; None: none."""
 
     def __init__(self, engine: Engine, msgs, root: int, decode: bool, max_batch: int = 1024, max_wait_us: int = 200,
-                 max_record_bytes: int = 4096):
+                 max_record_bytes: int = 4096, max_log_bytes: Optional[int] = None):
         self._f = C.c_void_p()
         self.engine = engine
         self.decode = bool(decode)
         self._nm, self._nf, k = S.proto_nested_tables(msgs)
         self._pr = S.proto_nested_presence(msgs)
         self.per_byte, self.per_record = nested_bound(msgs, root, self.decode)
-        _abi.check(_abi.lib().gofr_proto_frontend_create(C.byref(self._f), engine._e, self._nm.ctypes.data, len(msgs),
-                                                         self._nf.ctypes.data, k, root,
-                                                         None if self._pr is None else self._pr.ctypes.data, int(self.decode),
-                                                         max_batch, max_wait_us, max_record_bytes),
-                   "gofr_proto_frontend_create")
+        pr = None if self._pr is None else self._pr.ctypes.data
+        if max_log_bytes is None:
+            _abi.check(_abi.lib().gofr_proto_frontend_create(C.byref(self._f), engine._e, self._nm.ctypes.data, len(msgs),
+                                                             self._nf.ctypes.data, k, root, pr, int(self.decode), max_batch,
+                                                             max_wait_us, max_record_bytes),
+                       "gofr_proto_frontend_create")
+        else:
+            _abi.check(_abi.lib().gofr_proto_frontend_create_log(C.byref(self._f), engine._e, self._nm.ctypes.data, len(msgs),
+                                                                 self._nf.ctypes.data, k, root, pr, int(self.decode), max_batch,
+                                                                 max_wait_us, max_record_bytes, max_log_bytes),
+                       "gofr_proto_frontend_create_log")
 
     def close(self):
         if self._f:
@@ -121,13 +129,33 @@ class ProtoFrontend:
         _abi.check(_abi.lib().gofr_proto_frontend_stats(self._f, C.byref(b), C.byref(r)), "gofr_proto_frontend_stats")
         return int(b.value), int(r.value)
 
-    def call(self, data: bytes, out_cap: Optional[int] = None) -> Tuple[bytes, int]:
+    def set_log_clock(self, unix_ns: int) -> None:
+        """pin the log time of every line (tests); 0 = wall clock"""
+        _abi.check(_abi.lib().gofr_proto_frontend_set_log_clock(self._f, unix_ns), "gofr_proto_frontend_set_log_clock")
+
+    def call(self, data: bytes, out_cap: Optional[int] = None, log: Optional[S.LogRec] = None, trace_id: bytes = b"\0" * 16,
+             line_cap: int = 0):
         """One record → (result bytes, GOFR_GRPC_* status).  Blocks until the batch it joined has come back.  out_cap: size
-        of the caller's buffer, by default the bound of the record (never too small)."""
+        of the caller's buffer, by default the bound of the record (never too small).  With log (a LogRec: its start time,
+        elapsed time, zone, method and kind LOG_RPC / LOG_NONE; the rest is ignored) and the span's trace_id → (message,
+        status, RPCLog line) through gofr_proto_frontend_call_log; data may be empty (the handler failed); line_cap
+        defaults to the bound of the record."""
         if out_cap is None:
             out_cap = self.per_byte * (len(data) + 5) + self.per_record
         buf = C.create_string_buffer(max(out_cap, 1))
         n, status = C.c_uint32(), C.c_uint32()
+        if log is not None:
+            assert len(trace_id) == 16
+            lb = S.LogBatch.pack([log])
+            method = lb.arena.tobytes()[:int(lb.desc["method_len"][0])]
+            lcap = line_cap or 320 + 7 * len(method)
+            line = C.create_string_buffer(max(lcap, 1))
+            ln = C.c_uint32()
+            _abi.check(_abi.lib().gofr_proto_frontend_call_log(self._f, data, len(data), trace_id, lb.desc.ctypes.data, method,
+                                                               buf, out_cap, C.byref(n), C.byref(status), line, lcap,
+                                                               C.byref(ln)),
+                       "gofr_proto_frontend_call_log")
+            return buf.raw[:n.value], int(status.value), line.raw[:ln.value]
         _abi.check(_abi.lib().gofr_proto_frontend_call(self._f, data, len(data), buf, out_cap, C.byref(n), C.byref(status)),
                    "gofr_proto_frontend_call")
         return buf.raw[:n.value], int(status.value)

@@ -668,9 +668,33 @@ typedef struct gofr_batch_log {
 int gofr_batch_submit_log(gofr_engine*, const gofr_req_batch* in, gofr_resp_batch* out, gofr_batch_log* log, gofr_ticket* ticket);
 int gofr_batch_submit_slots_log(gofr_engine*, const gofr_req_batch* in, gofr_slot_batch* out, gofr_batch_log* log,
                                 gofr_ticket* ticket);
-/* No GPU needed: an out_cap that always suffices for gofr_batch_submit_log's lines of these n records — 320 bytes plus 6
- * per string byte for each record whose kind is not GOFR_LOG_NONE. */
+/* No GPU needed: an out_cap that always suffices for the lines of these n records (gofr_batch_submit_log,
+ * gofr_proto_batch_encode_log) — for each record whose kind is not GOFR_LOG_NONE, 320 bytes plus 6 per string byte, and
+ * for a GOFR_LOG_RPC record one more per method byte (RPCLog's method is escaped twice: one byte may leave as 7). */
 int gofr_batch_log_bound(const gofr_log_desc* desc, uint32_t n, uint64_t* out_cap);
+
+/* gofr_proto_batch_encode plus the gRPC LoggingInterceptor's RPCLog line (gofr_requestlog_device's GOFR_LOG_RPC format)
+ * for every call of the batch that asks for one, in the same call: the lines are a second output of the encode batch's
+ * chunk pipeline, written on the device.  LoggingInterceptor (pkg/gofr/grpc/log.go:27-50) logs once the handler has
+ * returned, which is when the call's response is handed to this call, and before grpc-go marshals it.  out, out_off, meta
+ * and the frames are byte for byte and status for status what gofr_proto_batch_encode gives for the same batch; out_bytes
+ * reports what the batch needed, as in the other _log calls.
+ *   trace_ids  16 bytes per record: the trace id of the span the interceptor started, the line's id.
+ *   log        one record per call (n = the gofr_proto_batch's n), in a gofr_batch_log as gofr_batch_submit_log takes it.
+ *              Read: start_unix_ns, elapsed_ns (the interceptor's time.Since(start): the handler ran on the caller's
+ *              thread), tz_offset_s, arena_off, method_len (info.FullMethod, at arena_off) and kind, which is GOFR_LOG_RPC
+ *              or GOFR_LOG_NONE (no line from this call).  The other four lengths are checked against the arena and
+ *              otherwise ignored.  Filled by the call: log_unix_ns (the batch's log->log_unix_ns).
+ * Record i has a line exactly when its kind is GOFR_LOG_RPC, whatever meta[i] says; every other record has an empty line.
+ * A call whose handler returned an error has no response for grpc-go to marshal: pass an empty row (off[i] == off[i + 1]).
+ * It still gets its line, and its frame and status are to be ignored.
+ * Lines, capacity, pinned and pageable buffers, the 4 GiB limit and n == 0 are as for gofr_batch_submit_log;
+ * gofr_batch_log_bound sizes log->out_cap.
+ * GOFR_ERR_INVALID: gofr_proto_batch_encode's cases, a null log column (arena may be NULL when every string is empty), a
+ * null trace_ids when n > 0, a record whose strings pass arena_bytes, a kind other than GOFR_LOG_RPC / GOFR_LOG_NONE. */
+int gofr_proto_batch_encode_log(gofr_engine*, const gofr_proto_nmsg* msgs, uint32_t n_msgs, const gofr_proto_nfield* fields,
+                                uint32_t n_fields, uint32_t root, const uint8_t* presence, const gofr_proto_batch* in,
+                                const uint8_t* trace_ids, gofr_resp_batch* out, gofr_batch_log* log, gofr_ticket* ticket);
 
 /* Batching front-end (SURVEY.md §8f rank 3): the reference serves one request per goroutine (net/http conn.serve →
  * router.ServeHTTP, pkg/gofr/httpServer.go:29-33); the GPU wants batches.  Any number of threads call
@@ -737,6 +761,25 @@ void gofr_proto_frontend_destroy(gofr_proto_frontend*);
 int gofr_proto_frontend_stats(gofr_proto_frontend*, uint64_t* batches, uint64_t* records);
 int gofr_proto_frontend_call(gofr_proto_frontend*, const uint8_t* in, uint32_t in_len, uint8_t* out, uint32_t out_cap,
                              uint32_t* out_len, uint32_t* status);
+/* An encode front-end whose callers may also ask for their call's RPCLog line: gofr_proto_frontend_create plus log
+ * staging of max_log_bytes method bytes per call.  Its batches run through gofr_proto_batch_encode_log when some caller of
+ * the batch logs (callers of gofr_proto_frontend_call ride along as GOFR_LOG_NONE), else through gofr_proto_batch_encode.
+ * The line belongs to the encode direction: decode != 0 is GOFR_ERR_INVALID. */
+int gofr_proto_frontend_create_log(gofr_proto_frontend** out, gofr_engine*, const gofr_proto_nmsg* msgs, uint32_t n_msgs,
+                                   const gofr_proto_nfield* fields, uint32_t n_fields, uint32_t root, const uint8_t* presence,
+                                   int decode, uint32_t max_batch, uint32_t max_wait_us, uint32_t max_record_bytes,
+                                   uint32_t max_log_bytes);
+/* The log time of every line (unix ns; 0 = the wall clock at dispatch). */
+int gofr_proto_frontend_set_log_clock(gofr_proto_frontend*, int64_t unix_ns);
+/* gofr_proto_frontend_call plus the call's line by gofr_proto_batch_encode_log's rule.  in: the row, empty for a call
+ * whose handler failed (its message and status are then to be ignored; the line is still written).  log: start_unix_ns,
+ * elapsed_ns, tz_offset_s, method_len and kind (GOFR_LOG_RPC or GOFR_LOG_NONE) are read, the rest is ignored; method:
+ * info.FullMethod, method_len bytes (at most max_log_bytes).  The line goes to line[0 .. *line_len) (empty for
+ * GOFR_LOG_NONE); a line longer than line_cap returns GOFR_ERR_CAPACITY with *line_len set, the message still delivered.
+ * GOFR_ERR_INVALID on a front-end made by gofr_proto_frontend_create. */
+int gofr_proto_frontend_call_log(gofr_proto_frontend*, const uint8_t* in, uint32_t in_len, const uint8_t trace_id[16],
+                                 const gofr_log_desc* log, const uint8_t* method, uint8_t* out, uint32_t out_cap, uint32_t* out_len,
+                                 uint32_t* status, uint8_t* line, uint32_t line_cap, uint32_t* line_len);
 
 /* HTTP/1.1 request heads (SURVEY.md §8f rank 2): what net/http's readRequest + url.ParseRequestURI hand to
  * Router.ServeHTTP, for a batch of raw request messages resident in HBM, in the layout the serve calls consume.

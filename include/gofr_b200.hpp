@@ -1068,7 +1068,9 @@ private:
 // back, so each RPC's thread calls it the way grpc-go calls encoding.Codec.Unmarshal / Marshal.  Decode: the message
 // without its 5-byte prefix → the row; encode: a row (padded with zero bytes to a multiple of 4) → the marshalled message
 // without the prefix.  One message type, one direction; any number of threads may call one ProtoFrontend.  Built from the
-// same Field lists as ProtoCodec; the app must be running (App::Run).
+// same Field lists as ProtoCodec; the app must be running (App::Run).  An encode front-end made with log also writes the
+// gRPC LoggingInterceptor's RPCLog line of each CallLog (gofr_proto_frontend_call_log), for methods of at most
+// max_log_bytes bytes.
 class ProtoFrontend {
 public:
     using Field = ProtoCodec::Field;
@@ -1076,17 +1078,24 @@ public:
         int rc = GOFR_OK;      // GOFR_ERR_CAPACITY: the record exceeds max_record_bytes, nothing was queued (use the host codec)
         uint32_t status = 0;   // GOFR_GRPC_*: GOFR_GRPC_DEFER is for the host's own decoder
         std::string record;    // the row (decode) or the message (encode); empty where status is not GOFR_GRPC_OK
+        std::string line;      // CallLog: the call's RPCLog line (empty for GOFR_LOG_NONE)
     };
 
     ProtoFrontend(const App& app, const std::vector<std::vector<Field>>& msgs, uint32_t root, bool decode, uint32_t max_batch = 1024,
-                  uint32_t max_wait_us = 200, uint32_t max_record_bytes = 4096)
+                  uint32_t max_wait_us = 200, uint32_t max_record_bytes = 4096, bool log = false, uint32_t max_log_bytes = 256)
         : d_(msgs, root) {
         if (!app.engine()) throw std::logic_error("gofr::ProtoFrontend: call App::Run first");
         std::tie(per_byte_, per_record_) = d_.bound(decode);
-        ProtoCodec::check(gofr_proto_frontend_create(&f_, app.engine(), d_.msgs.data(), (uint32_t)d_.msgs.size(), d_.fields.data(),
-                                                     (uint32_t)d_.fields.size(), root, d_.presence(), decode ? 1 : 0, max_batch,
-                                                     max_wait_us, max_record_bytes),
-                          "gofr_proto_frontend_create");
+        if (log)
+            ProtoCodec::check(gofr_proto_frontend_create_log(&f_, app.engine(), d_.msgs.data(), (uint32_t)d_.msgs.size(), d_.fields.data(),
+                                                             (uint32_t)d_.fields.size(), root, d_.presence(), decode ? 1 : 0,
+                                                             max_batch, max_wait_us, max_record_bytes, max_log_bytes),
+                              "gofr_proto_frontend_create_log");
+        else
+            ProtoCodec::check(gofr_proto_frontend_create(&f_, app.engine(), d_.msgs.data(), (uint32_t)d_.msgs.size(), d_.fields.data(),
+                                                         (uint32_t)d_.fields.size(), root, d_.presence(), decode ? 1 : 0, max_batch,
+                                                         max_wait_us, max_record_bytes),
+                              "gofr_proto_frontend_create");
     }
     ~ProtoFrontend() { gofr_proto_frontend_destroy(f_); }
     ProtoFrontend(const ProtoFrontend&) = delete;
@@ -1104,6 +1113,31 @@ public:
         ProtoCodec::check(r.rc, "gofr_proto_frontend_call");
         r.record.assign(reinterpret_cast<const char*>(out.data()), len);
         return r;
+    }
+    // Call plus the RPCLog line LoggingInterceptor writes once the handler has returned: `row` is the handler's response
+    // (empty when it failed: the record is then to be ignored, the line is still written), `trace_id` the span's, `log` its
+    // start_unix_ns, elapsed_ns, tz_offset_s and kind (GOFR_LOG_RPC, or GOFR_LOG_NONE for no line) and `method`
+    // info.FullMethod.
+    Result CallLog(const std::string& row, const std::array<uint8_t, 16>& trace_id, gofr_log_desc log, const std::string& method) const {
+        Result r;
+        std::vector<uint8_t> out((size_t)per_byte_ * (row.size() + 5) + per_record_);
+        std::string line(320 + 7 * method.size(), '\0');  // gofr_batch_log_bound of the record: never too small
+        uint32_t len = 0, line_len = 0;
+        log.method_len = (uint16_t)method.size();
+        r.rc = row.size() > UINT32_MAX || method.size() > UINT16_MAX
+                   ? GOFR_ERR_CAPACITY
+                   : gofr_proto_frontend_call_log(f_, reinterpret_cast<const uint8_t*>(row.data()), (uint32_t)row.size(), trace_id.data(),
+                                                  &log, reinterpret_cast<const uint8_t*>(method.data()), out.data(), (uint32_t)out.size(),
+                                                  &len, &r.status, reinterpret_cast<uint8_t*>(&line[0]), (uint32_t)line.size(), &line_len);
+        if (r.rc == GOFR_ERR_CAPACITY) return r;
+        ProtoCodec::check(r.rc, "gofr_proto_frontend_call_log");
+        r.record.assign(reinterpret_cast<const char*>(out.data()), len);
+        r.line.assign(line.data(), line_len);
+        return r;
+    }
+    // pin the log time of every line (tests); 0 = wall clock
+    void SetLogClock(int64_t unix_ns) const {
+        ProtoCodec::check(gofr_proto_frontend_set_log_clock(f_, unix_ns), "gofr_proto_frontend_set_log_clock");
     }
     std::pair<uint64_t, uint64_t> Stats() const {
         uint64_t b = 0, n = 0;
