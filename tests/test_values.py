@@ -16,6 +16,7 @@ import pytest
 
 from gofr_b200 import spec as S
 from gofr_b200.table import Table
+from tests import go_net_url as G
 from tests import oracle as O
 from tests.emu import emu as E
 
@@ -103,26 +104,13 @@ def go_json_time(v) -> str:
 
 
 def go_json_string(v) -> str:
-    """encoding/json string with escapeHTML (only for valid UTF-8 input, which is all these tests generate)"""
-    s = v if isinstance(v, str) else bytes(v).decode("utf-8")
-    out = ['"']
-    for ch in s:
-        if ch in HTML:
-            out.append(HTML[ch])
-        elif ch == '"' or ch == "\\":
-            out.append("\\" + ch)
-        elif ch == "\n":
-            out.append("\\n")
-        elif ch == "\r":
-            out.append("\\r")
-        elif ch == "\t":
-            out.append("\\t")
-        elif ord(ch) < 0x20:
-            out.append("\\u%04x" % ord(ch))
-        else:
-            out.append(ch)
-    out.append('"')
-    return "".join(out)
+    """encoding/json string with escapeHTML, over any bytes (tests/go_net_url.py: one \\ufffd per invalid byte)"""
+    return G.json_string(v.encode("utf-8") if isinstance(v, str) else bytes(v)).decode("utf-8")
+
+
+# RESULT_STRING payloads: invalid UTF-8 (truncated, overlong, surrogate, beyond U+10FFFF, lone continuation), U+2028/9
+STRING_PAYLOADS = [b"ok", b"\xe2\x82", b"\xe2\x82\xac", b"\xc0\xaf", b"\xed\xa0\x80", b"\xf4\x90\x80\x80", b"\x80\xbf", b"\xff<\xfe>",
+                   b"\xe2\x80\xa8\xe2\x80\xa9", b"\x08\x0c\x00", b"\xf0\x9f\x98", b"\xef\xbf\xbd", b""]
 
 
 class Unencodable(Exception):
@@ -426,16 +414,19 @@ def _batch(spec, n, seed, nan_rate=0.0, result=False, routed=None):
         except Unencodable:
             body = None
         if result:
-            which = rnd.randrange(3)
+            which = rnd.randrange(4)
             if which == 0:
                 data, body = S.result_record(S.RESULT_DATA, row), None if body is None else '{"data":%s}\n' % body
             elif which == 1:
                 es = rnd.randrange(3)
                 data, body = S.result_record(S.RESULT_RAW_DATA, row, es), None if body is None else body + "\n"
-            else:
+            elif which == 2:
                 msg = rnd.choice(["boom", "bad <thing>", ""])
                 data = S.result_both(sc, vals, msg.encode(), spec.schema)
                 body = None if body is None else '{"error":{"message":%s},"data":%s}\n' % (go_json_string(msg), body)
+            else:                                      # a string result of arbitrary bytes: invalid UTF-8 included
+                text = rnd.choice(STRING_PAYLOADS) + bytes(rnd.getrandbits(8) for _ in range(rnd.randrange(6)))
+                data, body = S.result_record(S.RESULT_STRING, text), '{"data":%s}\n' % go_json_string(text)
         else:
             data, body = row, None if body is None else '{"data":%s}\n' % body
         reqs.append(S.Req(S.M_GET, b"/v/%d" % sc.id, b"", data))
